@@ -173,7 +173,8 @@ typedef struct pm_cfg {
   int32_t  device;             /* CUDA ordinal */
   uint32_t flags;              /* pm_cfg_flag */
   uint32_t reserved0;
-  uint64_t cost_tile_bytes;    /* HBM budget for one materialised cost tile; 0 = 8 GiB */
+  uint64_t cost_tile_bytes;    /* HBM budget for one materialised cost tile; 0 = 8 GiB.  Tile rows are sized at
+                                  8 B per element; the 32-bit tile covers the same rows in half of it */
   /* Worker sharding across GPUs (SURVEY 8e): this engine evaluates the        */
   /* contiguous canonical-order range [shard_first, shard_first+shard_count)   */
   /* of the global worker table; shard_count == 0 means "all".                 */
@@ -247,7 +248,8 @@ enum pm_mode {
                            /* per ask (pm_auction.cuh); no reference counterpart, self-oracle */
 };
 enum pm_path {
-  PM_PATH_MATERIALIZED = 0,      /* build int64 cost tile in HBM, then argmin over it */
+  PM_PATH_MATERIALIZED = 0,      /* build a cost tile in HBM (the 32-bit cost word when every price is
+                                    below 0x7FFFFFFF, else the int64 packed cost), then argmin over it */
   PM_PATH_FUSED        = 1u << 8,/* evaluate + reduce on chip, matrix never written   */
   PM_NO_ASK_STATS      = 1u << 9 /* with PM_PATH_FUSED: skip ask_best / ask_count (the reference modes only
                                     need the per-worker first feasible ask); they read INF / 0 then      */

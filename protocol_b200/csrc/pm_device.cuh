@@ -19,6 +19,7 @@ namespace pm {
 
 constexpr uint32_t kNone = 0xFFFFFFFFu;
 constexpr long long kInf = 0x7FFFFFFFFFFFFFFFll;
+constexpr uint32_t kNarrowInfeasible = 0x7FFFFFFFu;   // the 32-bit cost tile's "infeasible": kInf's high word
 
 // Synthetic presence bits added on the device side (never part of the ABI):
 constexpr uint32_t kCandBit = 1u << 31;        // Healthy && p2p_id.is_some() && !assigned (mod.rs:492-497)

@@ -167,6 +167,7 @@ struct pm_engine {
   DevBuf<uint32_t> ask_counts, ask_newoff;
   bool asks_small = true;      // every ask operand fits the fast predicate (pm_device.cuh DevOptF)
   bool workers_small = false;  // ... and every worker operand (checked on the device)
+  bool prices_narrow = false;  // every worker price < 0x7FFFFFFF: the first-fit tile can hold the 32-bit cost word alone
   bool workers_checked = false;
   DevBuf<uint32_t> amin, amax, bits;
   DevBuf<uint32_t> scratch_idx, scratch_flags;
@@ -385,7 +386,7 @@ int pm_create(const pm_cfg* cfg, pm_engine** out) try {
   e->sms = (unsigned)std::max(1, prop.multiProcessorCount);
   if (const char* t = std::getenv("PM_TUNE_ARGMIN")) e->tune_argmin = std::atoi(t);
   if (const char* t = std::getenv("PM_TUNE_GENERIC")) e->tune_generic = std::atoi(t);
-  if (const char* t = std::getenv("PM_TUNE_BUILD")) e->tune_build = std::atoi(t);
+  if (const char* t = std::getenv("PM_TUNE_BUILD")) e->tune_build = std::atoi(t);   // 8: int64 tile on the FastRow path
   if (const char* t = std::getenv("PM_TUNE_AUCTION")) e->tune_auction = std::atoi(t);
   if (const char* t = std::getenv("PM_TUNE_AUCTION_POOL")) std::sscanf(t, "%d,%d", &e->tune_auc_good, &e->tune_auc_extra);   // pool fill of a class walk
   if (const char* t = std::getenv("PM_TUNE_PROX")) e->tune_prox = std::atoi(t);   // 0: all-SM cooperative sweep; 2: single-CTA sweep; 1: latitude-banded single-CTA sweep (experimental)
@@ -729,15 +730,16 @@ static int decide_fast(pm_engine* e, bool* fast) {
   *fast = false;
   if (e->tune_generic || !e->asks_small) return PM_OK;
   if (!e->workers_checked) {
-    uint32_t one = 1;
-    PM_CUDA(cudaMemcpyAsync(e->counters.p + 2, &one, 4, cudaMemcpyHostToDevice, e->stream));
+    const uint32_t one[2] = {1, 1};
+    PM_CUDA(cudaMemcpyAsync(e->counters.p + 2, one, 8, cudaMemcpyHostToDevice, e->stream));
     if (e->n_workers) {
       pm::pm_check_worker_ranges<<<blocks_for(e->n_workers, 256), 256, 0, e->stream>>>(e->wa.p, e->wb.p, e->n_workers, e->counters.p + 2);
       PM_LAUNCH_CHECK("pm_check_worker_ranges");
     }
-    PM_CUDA(cudaMemcpyAsync(e->h_scalars.p + 4, e->counters.p + 2, 4, cudaMemcpyDeviceToHost, e->stream));
+    PM_CUDA(cudaMemcpyAsync(e->h_scalars.p + 4, e->counters.p + 2, 8, cudaMemcpyDeviceToHost, e->stream));
     PM_CUDA(cudaStreamSynchronize(e->stream));
     e->workers_small = e->h_scalars.p[4] != 0;
+    e->prices_narrow = e->h_scalars.p[5] != 0;
     e->workers_checked = true;
   }
   *fast = e->workers_small;
@@ -782,9 +784,23 @@ static int worker_major(pm_engine* e, pm::EvalParams* p, int* bits_mode) {
   return PM_OK;
 }
 
-static void launch_build(pm_engine* e, const pm::EvalParams& p, int bits_mode, bool fast, dim3 grid,
+// The 32-bit cost tile (pm_build_cost_fast<.., true> + pm_argmin<.., true>): on the default FastRow path, for tables
+// whose every price is below 0x7FFFFFFF (decide_fast).  The staged kernels (PM_TUNE_BUILD = 1, 3, 4), the generic
+// predicate and other prices keep the int64 tile; PM_TUNE_BUILD=8 keeps it on the FastRow path too, for A/B runs.
+static bool narrow_tile(const pm_engine* e, bool fast) {
+  const int tb = e->tune_build;
+  return fast && e->prices_narrow && tb != 1 && tb != 3 && tb != 4 && tb != 8;
+}
+
+static void launch_build(pm_engine* e, const pm::EvalParams& p, int bits_mode, bool fast, bool narrow, dim3 grid,
                          uint32_t t0, uint32_t nt, uint32_t w0, uint32_t nw, size_t ld) {
 #define PM_BUILD_CASE(B, F) pm::pm_build_cost<B, F><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, t0, nt, w0, nw, e->cost.p, ld)
+#define PM_FAST_CASE(B, R)                                                                                              \
+  {                                                                                                                     \
+    grid.y = blocks_for(nt, R);                                                                                         \
+    if (narrow) pm::pm_build_cost_fast<B, R, true><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, t0, nt, w0, nw, e->cost.p, ld);   \
+    else pm::pm_build_cost_fast<B, R, false><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, t0, nt, w0, nw, e->cost.p, ld);         \
+  }
   if (fast && bits_mode == 2 && e->tune_build == 3) {
     pm::pm_build_cost<2, true, 3><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, t0, nt, w0, nw, e->cost.p, ld);
   } else if (fast && bits_mode == 2 && e->tune_build == 4) {
@@ -792,23 +808,17 @@ static void launch_build(pm_engine* e, const pm::EvalParams& p, int bits_mode, b
   } else if (fast && e->tune_build != 1) {   // the FastRow kernel; PM_TUNE_BUILD=1 keeps the staged-CSR form for A/B runs
     // one-word acceptance rows are bound into the FastRows (pm_bind_rows) however many rows there are
     if (p.words == 1) bits_mode = 2;
-    if (bits_mode == 2 && e->tune_build == 5) {          // rows-per-CTA experiments (tools/tune.py)
-      grid.y = blocks_for(nt, 128);
-      pm::pm_build_cost_fast<2, 128><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, t0, nt, w0, nw, e->cost.p, ld);
-    } else if (bits_mode == 2 && e->tune_build == 6) {
-      grid.y = blocks_for(nt, 256);
-      pm::pm_build_cost_fast<2, 256><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, t0, nt, w0, nw, e->cost.p, ld);
-    } else {
-      grid.y = blocks_for(nt, pm::kFastRows);
-      if (bits_mode == 2) pm::pm_build_cost_fast<2><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, t0, nt, w0, nw, e->cost.p, ld);
-      else if (bits_mode == 1) pm::pm_build_cost_fast<1><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, t0, nt, w0, nw, e->cost.p, ld);
-      else pm::pm_build_cost_fast<0><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, t0, nt, w0, nw, e->cost.p, ld);
-    }
+    if (bits_mode == 2 && e->tune_build == 5) PM_FAST_CASE(2, 128)          // rows-per-CTA experiments (tools/tune.py)
+    else if (bits_mode == 2 && e->tune_build == 6) PM_FAST_CASE(2, 256)
+    else if (bits_mode == 2) PM_FAST_CASE(2, pm::kFastRows)
+    else if (bits_mode == 1) PM_FAST_CASE(1, pm::kFastRows)
+    else PM_FAST_CASE(0, pm::kFastRows)
   } else if (fast) {
     if (bits_mode == 2) PM_BUILD_CASE(2, true); else if (bits_mode == 1) PM_BUILD_CASE(1, true); else PM_BUILD_CASE(0, true);
   } else {
     if (bits_mode == 2) PM_BUILD_CASE(2, false); else if (bits_mode == 1) PM_BUILD_CASE(1, false); else PM_BUILD_CASE(0, false);
   }
+#undef PM_FAST_CASE
 #undef PM_BUILD_CASE
 }
 
@@ -824,7 +834,13 @@ static void launch_fused(pm_engine* e, const pm::EvalParams& p, int bits_mode, b
 #undef PM_FUSED_CASE
 }
 
-static void launch_argmin(pm_engine* e, size_t ld, uint32_t nt, uint32_t t0, uint32_t w0, uint32_t nw) {
+static void launch_argmin(pm_engine* e, bool narrow, size_t ld, uint32_t nt, uint32_t t0, uint32_t w0, uint32_t nw) {
+  if (narrow) {   // 16 x 16 B in flight per lane, as the wide <8, 2>; PM_TUNE_ARGMIN shapes the int64 tile's kernel only
+    dim3 grid(blocks_for(ld, 8 * 128 * pm::kArgWarps), blocks_for(nt, pm::kArgRows));
+    pm::pm_argmin<8, 2, true><<<grid, pm::kArgThreads, 0, e->stream>>>(e->cost.p, ld, nt, t0, w0, nw, e->first_ask.p,
+                                                                      e->ask_best.p, e->ask_count.p);
+    return;
+  }
 #define PM_ARGMIN_CASE(S, RPW)                                                                      \
   {                                                                                                  \
     dim3 grid(blocks_for(ld, (S) * 64 * pm::kArgWarps), blocks_for(nt, pm::kArgRows));                               \
@@ -919,12 +935,16 @@ static int match_local_locked(pm_engine* e, uint32_t mode) {
         const int rc = bind_rows(e, wm);
         if (rc != PM_OK) return rc;
       }
+      // rows are sized by 8 B per element for both widths: the 32-bit tile covers the same asks in half the bytes, so
+      // tiles and launches are the same whichever width runs
+      const bool narrow = narrow_tile(e, fast);
+      const uint32_t elem_bytes = narrow ? 4u : 8u;
       uint64_t rows = e->cfg.cost_tile_bytes / (ld * 8);
       if (rows == 0) rows = 1;
       rows = std::min<uint64_t>(rows, T);
       rows = std::min<uint64_t>(rows, 65535ull * pm::kArgRows);
       if (rows >= 1024) rows &= ~(uint64_t)511;   // whole row bands of the build kernel (no ragged last band in every tile)
-      cudaError_t ce = e->cost.ensure((size_t)rows * ld);
+      cudaError_t ce = e->cost.ensure((size_t)rows * ld * elem_bytes / 8);   // ld is a multiple of 1024
       if (ce != cudaSuccess) {
         cudaGetLastError();
         return e->fail(PM_E_NOMEM, "pm_match: cannot allocate the cost tile; lower pm_cfg.cost_tile_bytes");
@@ -934,21 +954,22 @@ static int match_local_locked(pm_engine* e, uint32_t mode) {
         {
           Timer tm(e, &e->stats.ms_build);
           dim3 grid(blocks_for(ld, pm::kEvalCols), blocks_for(nt, pm::kEvalRows));
-          launch_build(e, p, bits_mode, fast, grid, t0, nt, w0, nw, ld);
+          launch_build(e, p, bits_mode, fast, narrow, grid, t0, nt, w0, nw, ld);
           PM_LAUNCH_CHECK("pm_build_cost");
           tm.stop();
           ++e->stats.n_build_launches;
         }
         {
           Timer tm(e, &e->stats.ms_argmin);
-          launch_argmin(e, ld, nt, t0, w0, nw);
+          launch_argmin(e, narrow, ld, nt, t0, w0, nw);
           PM_LAUNCH_CHECK("pm_argmin");
           tm.stop();
           ++e->stats.n_argmin_launches;
         }
         ++e->stats.n_tiles;
-        e->stats.cost_bytes_written += (uint64_t)nt * nw * 8;   // algorithmic: 8 B per evaluation (padding columns not counted)
-        e->stats.cost_bytes_read += (uint64_t)nt * nw * 8;
+        // algorithmic: 4 or 8 B per evaluation, the tile's element (padding columns not counted)
+        e->stats.cost_bytes_written += (uint64_t)nt * nw * elem_bytes;
+        e->stats.cost_bytes_read += (uint64_t)nt * nw * elem_bytes;
       }
     }
     e->stats.evals = (uint64_t)T * nw;
@@ -1652,7 +1673,7 @@ int pm_build_cost_tile(pm_engine* e, uint32_t t0, uint32_t nt, int64_t* host_out
     rc = bind_rows(e, wm);
     if (rc != PM_OK) return rc;
   }
-  launch_build(e, p, bits_mode, fast, grid, t0, nt, w0, nw, ld);
+  launch_build(e, p, bits_mode, fast, false, grid, t0, nt, w0, nw, ld);   // exports the int64 tile
   PM_LAUNCH_CHECK("pm_build_cost");
   PM_CUDA(cudaMemcpy2DAsync(host_out, (size_t)nw * 8, e->cost.p, ld * 8, (size_t)nw * 8, nt,
                             cudaMemcpyDeviceToHost, e->stream));

@@ -1,8 +1,9 @@
 // pm_kernels.cuh — sm_90a kernels of the matching pass.
 //
 //   pm_build_cost   cost-matrix build: int64 cost[t][w] for a tile of asks x a
-//                   stripe of workers, HBM-write-bound (8 B per evaluation)
-//   pm_argmin       one read of the tile (8 B per evaluation): per-ask packed
+//                   stripe of workers, HBM-write-bound (8 B per evaluation; the
+//                   FastRow form's narrow tile: the 32-bit cost word, 4 B)
+//   pm_argmin       one read of the tile (8 or 4 B per evaluation): per-ask packed
 //                   (min_cost, argmin) + feasible count, per-worker first ask
 //   pm_fused_eval   the same outputs without materialising the matrix
 //   pm_hist / pm_check_tails / pm_sweep / pm_emit_* : resolution sweep that turns
@@ -11,6 +12,7 @@
 // Reference semantics being reproduced: NodeGroupsPlugin::try_form_new_groups,
 // crates/orchestrator/src/plugins/node_groups/mod.rs:478-628.
 #pragma once
+#include <type_traits>
 #include "pm_device.cuh"
 
 namespace pm {
@@ -348,9 +350,15 @@ struct __align__(128) FastStage {
 constexpr int kFastRows = 512;   // asks per CTA: the prologue (worker rows from L2, the TMA of the FastRows) is paid once per CTA
                                  // (PM_TUNE_BUILD=5 / 6 select 128 / 256 rows for comparison)
 
-template <int BITS, int ROWS = kFastRows>
+// NARROW: the tile holds only the 32-bit cost word — the worker's price when feasible, kNarrowInfeasible when not — and
+// `tile` is uint32_t[rows][ld].  The worker index the wide element carries in its low word is the column (+ w0), which
+// pm_argmin<.., true> knows anyway: 4 B per evaluation instead of 8.  A lane then owns the 4 consecutive columns
+// 4l .. 4l+3 of its warp's 128, so each row is one 16-byte store per thread, 512 B per warp and 4 KB per CTA,
+// contiguous.  Only for tables whose every price is below kNarrowInfeasible (pm_check_worker_ranges): at that price a
+// feasible worker could not be told from the sentinel, and at >= 2^31 the wide tile's signed order differs.
+template <int BITS, int ROWS = kFastRows, bool NARROW = false>
 __global__ void __launch_bounds__(kEvalThreads, 2)
-pm_build_cost_fast(EvalParams p, uint32_t t0, uint32_t nt, uint32_t w0, uint32_t nw, long long* __restrict__ cost, size_t ld) {
+pm_build_cost_fast(EvalParams p, uint32_t t0, uint32_t nt, uint32_t w0, uint32_t nw, void* __restrict__ tile, size_t ld) {
   __shared__ FastStage<ROWS> s;
   const uint32_t r0 = blockIdx.y * ROWS;
   const uint32_t nrows = min(nt - r0, (uint32_t)ROWS);
@@ -364,22 +372,23 @@ pm_build_cost_fast(EvalParams p, uint32_t t0, uint32_t nt, uint32_t w0, uint32_t
     for (uint32_t i = threadIdx.x; i < total_words; i += blockDim.x) s.bits[i] = __ldg(p.bits + i);
   }
   const uint32_t lane = threadIdx.x & 31u;
-  const uint32_t cbase = blockIdx.x * kEvalCols + (threadIdx.x >> 5) * 128u + lane * 2u;
+  const uint32_t cbase = blockIdx.x * kEvalCols + (threadIdx.x >> 5) * 128u + lane * (NARROW ? 4u : 2u);
   WorkerReg w[kEvalWPT];
   uint32_t gw[kEvalWPT], dx[kEvalWPT], dy[kEvalWPT];
 #pragma unroll
   for (int k = 0; k < kEvalWPT; ++k) {
-    const uint32_t col = cbase + (k >> 1) * 64u + (k & 1);
+    const uint32_t col = NARROW ? cbase + k : cbase + (k >> 1) * 64u + (k & 1);
     gw[k] = w0 + col;
     if (col < nw) {
       w[k] = make_worker(__ldg(p.wa + w0 + col), __ldg(p.wb + w0 + col));
       if (p.nacc) w[k].mmask = __ldg(p.nacc + w0 + col);
     } else w[k] = null_worker();
     dx[k] = 0xFFFFFFFFu - gw[k];          // infeasible: 0x7FFFFFFF_FFFFFFFF = feasible word + (0/1) * difference
-    dy[k] = 0x7FFFFFFFu - w[k].price;
+    dy[k] = 0x7FFFFFFFu - w[k].price;     // (the narrow form keeps only this high word)
   }
-  uint4* out = reinterpret_cast<uint4*>(cost + (size_t)r0 * ld + cbase);
-  const size_t row_stride = ld / 2;
+  uint4* out = NARROW ? reinterpret_cast<uint4*>(static_cast<uint32_t*>(tile) + (size_t)r0 * ld + cbase)
+                      : reinterpret_cast<uint4*>(static_cast<long long*>(tile) + (size_t)r0 * ld + cbase);
+  const size_t row_stride = NARROW ? ld / 4 : ld / 2;   // in 16-byte units
   const uint32_t sh = p.sign_shift;
   __syncthreads();            // mbarrier initialised, acceptance words staged
   mbar_wait(&s.bar, 0);
@@ -391,21 +400,24 @@ pm_build_cost_fast(EvalParams p, uint32_t t0, uint32_t nt, uint32_t w0, uint32_t
     eval_fast_first<kEvalWPT, BITS>(cur, s.bits, w, p.bits, p.words, um);
     if (cur.n_opts > 1u)                      // OR-options (node.rs:420-438): the ask fails only if every option does
       eval_fast_more<kEvalWPT, BITS>(p.opts_fast + cur.opt_off + 1, cur.n_opts - 1u, s.bits, w, p.bits, p.words, um);
-    uint4 v0, v1;
-    {
-      uint32_t o[2 * kEvalWPT];
+    uint32_t o[2 * kEvalWPT];
 #pragma unroll
-      for (int k = 0; k < kEvalWPT; ++k) {
-        const uint32_t fail = um[k] | (w[k].cores - cur.cpu_cores) | (w[k].ram - cur.ram_mb) | (w[k].storage - cur.storage_gb);
-        const uint32_t b = fail >> sh;                                    // 1 when infeasible (sh == 31)
-        o[2 * k] = b * dx[k] + gw[k];                                     // feasible: (price << 32) | worker
-        o[2 * k + 1] = b * dy[k] + w[k].price;                            // infeasible: 0x7FFFFFFF_FFFFFFFF
+    for (int k = 0; k < kEvalWPT; ++k) {
+      const uint32_t fail = um[k] | (w[k].cores - cur.cpu_cores) | (w[k].ram - cur.ram_mb) | (w[k].storage - cur.storage_gb);
+      const uint32_t b = fail >> sh;                                    // 1 when infeasible (sh == 31)
+      if (NARROW) {
+        o[k] = b * dy[k] + w[k].price;                                  // feasible: price ; infeasible: kNarrowInfeasible
+      } else {
+        o[2 * k] = b * dx[k] + gw[k];                                   // feasible: (price << 32) | worker
+        o[2 * k + 1] = b * dy[k] + w[k].price;                          // infeasible: 0x7FFFFFFF_FFFFFFFF
       }
-      v0 = make_uint4(o[0], o[1], o[2], o[3]);
-      v1 = make_uint4(o[4], o[5], o[6], o[7]);
     }
-    __stcs(out, v0);
-    __stcs(out + 32, v1);     // + 64 columns
+    if (NARROW) {
+      __stcs(out, make_uint4(o[0], o[1], o[2], o[3]));
+    } else {
+      __stcs(out, make_uint4(o[0], o[1], o[2], o[3]));
+      __stcs(out + 32, make_uint4(o[4], o[5], o[6], o[7]));     // + 64 columns
+    }
     out += row_stride;
     cur = nxt;
   }
@@ -446,39 +458,50 @@ constexpr int kArgRows = 64;                     // rows per CTA
 // flight at S=8, RPW=2), folds them lane-locally, then one shuffle reduction per
 // row.  Per-column "first feasible ask" never leaves the lane's registers; per-row
 // (min, count) partials are merged in shared memory and flushed once per CTA.
-template <int S, int RPW>
+//
+// NARROW: the tile is pm_build_cost_fast<.., true>'s uint32_t words (price, or kNarrowInfeasible).  A 128-bit load then
+// holds 4 columns, so a warp's slice is S*128 columns and a lane keeps the same S*RPW loads in flight.  A lane folds its
+// words into (least word, its first column) — its columns are visited in increasing order, so a strict "<" keeps the
+// first — and forms the packed (word << 32) | (w0 + column) once per row for the shuffle: the int64 the wide tile
+// holds, so ask_best, ask_count and first_ask are bit-identical to the wide form's.
+template <int S, int RPW, bool NARROW = false>
 __global__ void __launch_bounds__(kArgThreads)
-pm_argmin(const long long* __restrict__ cost, size_t ld, uint32_t nt, uint32_t t0, uint32_t w0,
+pm_argmin(const void* __restrict__ tile, size_t ld, uint32_t nt, uint32_t t0, uint32_t w0,
           uint32_t nw, uint32_t* __restrict__ first_ask, long long* __restrict__ ask_best,
           uint32_t* __restrict__ ask_count) {
-  constexpr int kWarpCols = S * 64;
-  __shared__ unsigned long long s_best[kArgRows];
+  constexpr int kWarpCols = S * (NARROW ? 128 : 64);
+  __shared__ long long s_best[kArgRows];   // signed, as the packed cost: a price >= 2^31 makes it negative
   __shared__ uint32_t s_cnt[kArgRows];
   const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
   const uint32_t c0 = (blockIdx.x * kArgWarps + warp) * kWarpCols;   // this warp's first column
   const uint32_t r0 = blockIdx.y * kArgRows;
   const uint32_t rows = min((uint32_t)kArgRows, nt - r0);
   for (uint32_t i = threadIdx.x; i < (uint32_t)kArgRows; i += kArgThreads) {
-    s_best[i] = (unsigned long long)kInf;
+    s_best[i] = kInf;
     s_cnt[i] = 0;
   }
   __syncthreads();
 
-  uint32_t cm[S][2];
+  constexpr int CPL = NARROW ? 4 : 2;                  // columns per 128-bit load
+  using Vec = std::conditional_t<NARROW, uint4, longlong2>;
+  uint32_t cm[S][CPL];
 #pragma unroll
-  for (int s = 0; s < S; ++s) cm[s][0] = cm[s][1] = kNone;
+  for (int s = 0; s < S; ++s)
+#pragma unroll
+    for (int j = 0; j < CPL; ++j) cm[s][j] = kNone;
 
   if (c0 < ld) {
     for (uint32_t rr = 0; rr < rows; rr += RPW) {
-      longlong2 v[RPW][S];
+      Vec v[RPW][S];
 #pragma unroll
       for (int q = 0; q < RPW; ++q) {
         const uint32_t r = r0 + rr + q;
-        const longlong2* rowp = reinterpret_cast<const longlong2*>(cost + (size_t)r * ld);
+        const Vec* rowp = static_cast<const Vec*>(tile) + (size_t)r * (ld / CPL);
 #pragma unroll
         for (int s = 0; s < S; ++s) {
-          const uint32_t col = c0 + s * 64 + lane * 2;
-          if (rr + q < rows && col < ld) v[q][s] = __ldcs(rowp + (col >> 1));
+          const uint32_t col = c0 + s * 32 * CPL + lane * CPL;
+          if (rr + q < rows && col < ld) v[q][s] = __ldcs(rowp + col / CPL);
+          else if constexpr (NARROW) v[q][s] = make_uint4(kNarrowInfeasible, kNarrowInfeasible, kNarrowInfeasible, kNarrowInfeasible);
           else v[q][s] = make_longlong2(kInf, kInf);
         }
       }
@@ -487,13 +510,29 @@ pm_argmin(const long long* __restrict__ cost, size_t ld, uint32_t nt, uint32_t t
         const uint32_t t = t0 + r0 + rr + q;
         long long best = kInf;
         uint32_t cnt = 0;
+        if constexpr (NARROW) {
+          uint32_t bw = kNarrowInfeasible, bc = 0;   // least word of the lane and its column offset
 #pragma unroll
-        for (int s = 0; s < S; ++s) {
-          best = min(best, min(v[q][s].x, v[q][s].y));
-          const bool fx = v[q][s].x != kInf, fy = v[q][s].y != kInf;
-          cnt += (uint32_t)fx + (uint32_t)fy;
-          cm[s][0] = fx ? min(cm[s][0], t) : cm[s][0];
-          cm[s][1] = fy ? min(cm[s][1], t) : cm[s][1];
+          for (int s = 0; s < S; ++s) {
+            const uint32_t x[4] = {v[q][s].x, v[q][s].y, v[q][s].z, v[q][s].w};
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+              const bool f = x[j] != kNarrowInfeasible;
+              cnt += (uint32_t)f;
+              cm[s][j] = f ? min(cm[s][j], t) : cm[s][j];
+              if (x[j] < bw) { bw = x[j]; bc = s * 128 + j; }
+            }
+          }
+          if (bw != kNarrowInfeasible) best = (long long)(((unsigned long long)bw << 32) | (w0 + c0 + lane * 4 + bc));
+        } else {
+#pragma unroll
+          for (int s = 0; s < S; ++s) {
+            best = min(best, min(v[q][s].x, v[q][s].y));
+            const bool fx = v[q][s].x != kInf, fy = v[q][s].y != kInf;
+            cnt += (uint32_t)fx + (uint32_t)fy;
+            cm[s][0] = fx ? min(cm[s][0], t) : cm[s][0];
+            cm[s][1] = fy ? min(cm[s][1], t) : cm[s][1];
+          }
         }
 #pragma unroll
         for (int off = 16; off > 0; off >>= 1) {
@@ -501,22 +540,24 @@ pm_argmin(const long long* __restrict__ cost, size_t ld, uint32_t nt, uint32_t t
           cnt += __shfl_xor_sync(0xffffffffu, cnt, off);
         }
         if (lane == 0 && cnt) {
-          atomicMin(&s_best[rr + q], (unsigned long long)best);
+          atomicMin(&s_best[rr + q], best);
           atomicAdd(&s_cnt[rr + q], cnt);
         }
       }
     }
 #pragma unroll
     for (int s = 0; s < S; ++s) {
-      const uint32_t col = c0 + s * 64 + lane * 2;
-      if (cm[s][0] != kNone && col < nw) atomicMin(first_ask + w0 + col, cm[s][0]);
-      if (cm[s][1] != kNone && col + 1 < nw) atomicMin(first_ask + w0 + col + 1, cm[s][1]);
+#pragma unroll
+      for (int j = 0; j < CPL; ++j) {
+        const uint32_t col = c0 + s * 32 * CPL + lane * CPL + j;
+        if (cm[s][j] != kNone && col < nw) atomicMin(first_ask + w0 + col, cm[s][j]);
+      }
     }
   }
   __syncthreads();
   for (uint32_t i = threadIdx.x; i < rows; i += kArgThreads) {
     if (s_cnt[i]) {
-      atomicMin(ask_best + t0 + r0 + i, (long long)s_best[i]);
+      atomicMin(ask_best + t0 + r0 + i, s_best[i]);
       atomicAdd(ask_count + t0 + r0 + i, s_cnt[i]);
     }
   }
@@ -747,7 +788,8 @@ __global__ void pm_scatter_rows(uint4* wa, uint4* wb, double* lat, double* lon, 
 }
 
 // Do all workers satisfy the fast-path operand limits (values < 2^31, gpu count < 2^16,
-// count * memory_mb < 2^31 without wrapping)?  Clears *ok otherwise.
+// count * memory_mb < 2^31 without wrapping)?  Clears ok[0] otherwise.  Is every price below
+// kNarrowInfeasible, so that the 32-bit cost tile can hold it?  Clears ok[1] otherwise.
 __global__ void pm_check_worker_ranges(const uint4* __restrict__ wa, const uint4* __restrict__ wb,
                                        uint32_t n, uint32_t* __restrict__ ok) {
   uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -758,7 +800,8 @@ __global__ void pm_check_worker_ranges(const uint4* __restrict__ wa, const uint4
   if (a.w & PM_W_HAS_GPU_MEM) small &= a.y < kSign;
   if ((a.w & PM_W_HAS_GPU_COUNT) && (a.w & PM_W_HAS_GPU_MEM))
     small &= (unsigned long long)a.x * (unsigned long long)a.y < (unsigned long long)kSign;
-  if (!small) *ok = 0u;
+  if (!small) ok[0] = 0u;
+  if (b.w >= kNarrowInfeasible) ok[1] = 0u;
 }
 
 // ------------------------------------------------------------------ resolution

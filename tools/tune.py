@@ -35,11 +35,12 @@ def run(env, steps=4, mode=abi.PM_MODE_FIRST_FIT):
         st = eng.stats()
         for k in ("ms_build", "ms_argmin", "ms_fused", "ms_resolve", "ms_total"):
             acc[k] = acc.get(k, 0.0) + st[k] / steps
-    gb = T * (((W + 15) // 16) * 16) * 8 / 1e9
     out = dict(env=env, **{k: round(v, 3) for k, v in acc.items()})
     if acc["ms_build"]:
-        out["build_GBs"] = round(gb / acc["ms_build"] * 1e3, 0)
-        out["argmin_GBs"] = round(gb / acc["ms_argmin"] * 1e3, 0)
+        # the bytes the engine counts per pass: 4 or 8 per evaluation, whichever tile ran (padding columns excluded)
+        out["bytes_per_eval"] = st["cost_bytes_written"] / st["evals"]
+        out["build_GBs"] = round(st["cost_bytes_written"] / 1e9 / acc["ms_build"] * 1e3, 0)
+        out["argmin_GBs"] = round(st["cost_bytes_read"] / 1e9 / acc["ms_argmin"] * 1e3, 0)
         if PEAK:
             out["build_frac"] = round(out["build_GBs"] / PEAK, 3)
             out["argmin_frac"] = round(out["argmin_GBs"] / PEAK, 3)
@@ -73,7 +74,7 @@ if __name__ == "__main__":
     for v in os.environ.get("TUNE_ARGMIN", "1,2,3,4,5").split(","):
         if v:
             variants.append({"PM_TUNE_ARGMIN": v})
-    for v in os.environ.get("TUNE_BUILD", "").split(","):
+    for v in os.environ.get("TUNE_BUILD", "8").split(","):   # 8: the int64 tile on the FastRow path
         if v:
             variants.append({"PM_TUNE_BUILD": v})
     for env in variants:
