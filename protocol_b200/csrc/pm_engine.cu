@@ -11,6 +11,7 @@
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 
+#include <cuda.h>   // driver types and prototypes only: the entry points are resolved at run time (TileBuf)
 #include <dlfcn.h>
 #include <nccl.h>   // types and prototypes only: the library is resolved at run time (nccl_api below), never linked
 
@@ -24,6 +25,7 @@
 #include <new>
 #include <string>
 #include <thread>
+#include <type_traits>
 #include <vector>
 
 #include "pm_guard.hpp"
@@ -95,6 +97,128 @@ template <class T> struct PinBuf {
   }
 };
 
+// The cost tile, in compressible device memory where the device offers it (generic compute-data compression): the L2
+// stores runs of equal words — the "infeasible" sentinel of the 32-bit tile, 0x7FFFFFFF_FFFFFFFF of the int64 one — to
+// HBM in compressed form and reads them back the same way, so the HBM traffic of a sparse tile shrinks while its layout,
+// contents and the kernels stay what they are.  Elsewhere (or when the driver refuses), plain cudaMalloc.  The driver's
+// virtual-memory calls are looked up at run time: the library keeps no link-time dependency on libcuda.
+struct TileBuf {
+  long long* p = nullptr;
+  size_t n = 0;
+  CUmemGenericAllocationHandle h = 0;   // non-zero: compressible mapping of `bytes` bytes at p
+  size_t bytes = 0;
+
+  struct Api {
+    decltype(&cuMemGetAllocationGranularity) granularity = nullptr;
+    decltype(&cuMemCreate) create = nullptr;
+    decltype(&cuMemRelease) release = nullptr;
+    decltype(&cuMemAddressReserve) reserve = nullptr;
+    decltype(&cuMemAddressFree) address_free = nullptr;
+    decltype(&cuMemMap) map = nullptr;
+    decltype(&cuMemUnmap) unmap = nullptr;
+    decltype(&cuMemSetAccess) set_access = nullptr;
+    decltype(&cuMemGetAllocationPropertiesFromHandle) props = nullptr;
+    bool ok = false;
+  };
+  static const Api& api() {
+    static const Api a = [] {
+      Api x;
+      auto get = [](const char* name, auto** fn) {
+        cudaDriverEntryPointQueryResult q{};
+        void* f = nullptr;
+        if (cudaGetDriverEntryPoint(name, &f, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess) {
+          cudaGetLastError();
+          return false;
+        }
+        *fn = reinterpret_cast<std::remove_pointer_t<decltype(fn)>>(f);
+        return f != nullptr;
+      };
+      x.ok = get("cuMemGetAllocationGranularity", &x.granularity) && get("cuMemCreate", &x.create) &&
+             get("cuMemRelease", &x.release) && get("cuMemAddressReserve", &x.reserve) &&
+             get("cuMemAddressFree", &x.address_free) && get("cuMemMap", &x.map) && get("cuMemUnmap", &x.unmap) &&
+             get("cuMemSetAccess", &x.set_access) && get("cuMemGetAllocationPropertiesFromHandle", &x.props);
+      return x;
+    }();
+    return a;
+  }
+
+  // one compressible mapping of at least `want_bytes`, or false (nothing held)
+  bool map_compressible(int device, size_t want_bytes) {
+    const Api& a = api();   // a device without compression fails cuMemCreate or grants an uncompressed handle
+    if (!a.ok) return false;
+    CUmemAllocationProp prop{};
+    prop.type = CU_MEM_ALLOCATION_TYPE_PINNED;
+    prop.location.type = CU_MEM_LOCATION_TYPE_DEVICE;
+    prop.location.id = device;
+    prop.allocFlags.compressionType = CU_MEM_ALLOCATION_COMP_GENERIC;
+    size_t gran = 0;
+    if (a.granularity(&gran, &prop, CU_MEM_ALLOC_GRANULARITY_RECOMMENDED) != CUDA_SUCCESS || gran == 0) return false;
+    const size_t size = (want_bytes + gran - 1) / gran * gran;
+    CUmemGenericAllocationHandle hh = 0;
+    if (a.create(&hh, size, &prop, 0) != CUDA_SUCCESS) return false;
+    CUmemAllocationProp got{};
+    CUdeviceptr ptr = 0;
+    bool ok = a.props(&got, hh) == CUDA_SUCCESS && got.allocFlags.compressionType == CU_MEM_ALLOCATION_COMP_GENERIC &&
+              a.reserve(&ptr, size, 0, 0, 0) == CUDA_SUCCESS;
+    if (ok && a.map(ptr, size, 0, hh, 0) != CUDA_SUCCESS) {
+      a.address_free(ptr, size);
+      ok = false;
+    }
+    if (ok) {
+      CUmemAccessDesc acc{};
+      acc.location = prop.location;
+      acc.flags = CU_MEM_ACCESS_FLAGS_PROT_READWRITE;
+      if (a.set_access(ptr, size, &acc, 1) != CUDA_SUCCESS) {
+        a.unmap(ptr, size);
+        a.address_free(ptr, size);
+        ok = false;
+      }
+    }
+    if (!ok) {
+      a.release(hh);
+      return false;
+    }
+    p = reinterpret_cast<long long*>(ptr);
+    h = hh;
+    bytes = size;
+    return true;
+  }
+
+  // capacity >= want elements; the old contents are not kept.  The caller has ordered every use of the old tile before
+  // this call (a pass's kernels are joined into the engine stream, which is synchronised here).
+  cudaError_t ensure(size_t want, int device, bool compress, cudaStream_t st) {
+    if (want <= n && p) return cudaSuccess;
+    if (p) {
+      cudaError_t e = cudaStreamSynchronize(st);
+      if (e != cudaSuccess) return e;
+    }
+    release();
+    if (want == 0) want = 1;
+    if (compress && map_compressible(device, want * sizeof(long long))) {
+      n = want;
+      return cudaSuccess;
+    }
+    cudaError_t e = cudaMalloc(&p, want * sizeof(long long));
+    if (e == cudaSuccess) n = want;
+    else p = nullptr;
+    return e;
+  }
+  void release() {
+    if (h) {
+      const Api& a = api();
+      a.unmap(reinterpret_cast<CUdeviceptr>(p), bytes);
+      a.address_free(reinterpret_cast<CUdeviceptr>(p), bytes);
+      a.release(h);
+    } else if (p) {
+      cudaFree(p);
+    }
+    p = nullptr;
+    n = 0;
+    h = 0;
+    bytes = 0;
+  }
+};
+
 inline unsigned blocks_for(size_t n, unsigned threads) { return (unsigned)((n + threads - 1) / threads); }
 
 // NCCL is plumbing for the one exchange of a sharded pass.  It is looked up at run time so that the library loads
@@ -141,6 +265,10 @@ struct pm_engine {
   int device = 0;
   unsigned sms = 132;     // streaming multiprocessors of the device (an H100 SXM has 132): caps of the grid-stride launches
   cudaStream_t stream = nullptr;
+  // The double-buffered 32-bit tile's argmin runs here, beside the next tile's build on `stream`; forked from and
+  // joined back into `stream` by events inside every pass, so nothing is left running on it between calls.
+  cudaStream_t side = nullptr;
+  cudaEvent_t ev_fork = nullptr, ev_built = nullptr, ev_read[2] = {nullptr, nullptr};
   std::string err;
   std::mutex mu;
 
@@ -151,6 +279,8 @@ struct pm_engine {
   bool have_workers = false, have_asks = false, have_bits = false, have_loc = false, have_rank = false;
   bool all_solo = true;  // every ask has min == max == 1
   int tune_argmin = 0, tune_generic = 0, tune_build = 0, tune_auction = 0, tune_prox = 0, tune_auc_good = 0, tune_auc_extra = 0;   // PM_TUNE_*: kernel-shape experiments
+  int tune_overlap = 0;   // PM_TUNE_OVERLAP=1: the 32-bit tile's argmin(k) beside build(k + 1) (slower with compressible tile memory)
+  int tune_compress = 1;  // PM_TUNE_COMPRESS=0: the cost tile in plain cudaMalloc memory (A/B runs)
   DevBuf<uint4> wa, wb;
   DevBuf<double> lat, lon;
   DevBuf<uint32_t> addr_rank;
@@ -176,7 +306,7 @@ struct pm_engine {
   uint64_t table_version = 0;          // bumped by every call that changes a table (pm_table_version)
 
   // evaluation
-  DevBuf<long long> cost;
+  TileBuf cost;
   DevBuf<uint32_t> first_ask, ask_count;
   DevBuf<long long> ask_best;
 
@@ -290,28 +420,31 @@ struct pm_engine {
 namespace {
 
 // Per-launch CUDA-event timing without host synchronisation: start/stop events
-// are recorded on the engine stream around a region and resolved in one go at
-// the end of the match (which synchronises anyway to read the group count).
+// are recorded around a region on the stream its kernels run on and resolved in
+// one go at the end of the match (which synchronises anyway to read the group
+// count; every side-stream region is joined into the engine stream before that).
 struct Timer {
   pm_engine* e;
   float* acc;
+  cudaStream_t st;
   bool on;
   size_t slot = 0;
-  Timer(pm_engine* e_, float* acc_);
+  Timer(pm_engine* e_, float* acc_, cudaStream_t st_);
   void stop();
 };
 
-Timer::Timer(pm_engine* e_, float* acc_) : e(e_), acc(acc_), on((e_->cfg.flags & PM_CFG_TIMING) != 0) {
+Timer::Timer(pm_engine* e_, float* acc_, cudaStream_t st_)
+    : e(e_), acc(acc_), st(st_), on((e_->cfg.flags & PM_CFG_TIMING) != 0) {
   if (!on) return;
   cudaEvent_t a = e->take_event(), b = e->take_event();
   if (!a || !b) { on = false; return; }
   slot = e->ev_pending.size();
   e->ev_pending.push_back({a, b, acc});
-  cudaEventRecord(a, e->stream);
+  cudaEventRecord(a, st);
 }
 void Timer::stop() {
   if (!on) return;
-  cudaEventRecord(e->ev_pending[slot].b, e->stream);
+  cudaEventRecord(e->ev_pending[slot].b, st);
   on = false;
 }
 
@@ -390,6 +523,8 @@ int pm_create(const pm_cfg* cfg, pm_engine** out) try {
   if (const char* t = std::getenv("PM_TUNE_AUCTION")) e->tune_auction = std::atoi(t);
   if (const char* t = std::getenv("PM_TUNE_AUCTION_POOL")) std::sscanf(t, "%d,%d", &e->tune_auc_good, &e->tune_auc_extra);   // pool fill of a class walk
   if (const char* t = std::getenv("PM_TUNE_PROX")) e->tune_prox = std::atoi(t);   // 0: all-SM cooperative sweep; 2: single-CTA sweep; 1: latitude-banded single-CTA sweep (experimental)
+  if (const char* t = std::getenv("PM_TUNE_OVERLAP")) e->tune_overlap = std::atoi(t);
+  if (const char* t = std::getenv("PM_TUNE_COMPRESS")) e->tune_compress = std::atoi(t);
   bool ok = cudaSetDevice(e->device) == cudaSuccess;
   if (ok && cfg->stream) {
     e->stream = (cudaStream_t)cfg->stream;  // caller's stream (e.g. torch's current stream)
@@ -397,12 +532,19 @@ int pm_create(const pm_cfg* cfg, pm_engine** out) try {
   } else if (ok) {
     ok = cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking) == cudaSuccess;
   }
+  int prio = 0;
+  ok = ok && cudaStreamGetPriority(e->stream, &prio) == cudaSuccess &&
+       cudaStreamCreateWithPriority(&e->side, cudaStreamNonBlocking, prio) == cudaSuccess &&
+       cudaEventCreateWithFlags(&e->ev_fork, cudaEventDisableTiming) == cudaSuccess &&
+       cudaEventCreateWithFlags(&e->ev_built, cudaEventDisableTiming) == cudaSuccess &&
+       cudaEventCreateWithFlags(&e->ev_read[0], cudaEventDisableTiming) == cudaSuccess &&
+       cudaEventCreateWithFlags(&e->ev_read[1], cudaEventDisableTiming) == cudaSuccess;
   ok = ok &&
             cudaEventCreate(&e->ev0) == cudaSuccess && cudaEventCreate(&e->ev1) == cudaSuccess &&
             e->h_scalars.ensure(64) == cudaSuccess && e->counters.ensure(32) == cudaSuccess;
   if (!ok) {
     g_create_error = std::string("pm_create: ") + cudaGetErrorString(cudaGetLastError());
-    delete e;
+    pm_destroy(e);
     return PM_E_CUDA;
   }
   *out = e;
@@ -448,6 +590,9 @@ void pm_destroy(pm_engine* e) {
   if (e->ev0) cudaEventDestroy(e->ev0);
   if (e->ev1) cudaEventDestroy(e->ev1);
   for (cudaEvent_t ev : e->ev_pool) cudaEventDestroy(ev);
+  for (cudaEvent_t ev : {e->ev_fork, e->ev_built, e->ev_read[0], e->ev_read[1]})
+    if (ev) cudaEventDestroy(ev);
+  if (e->side) cudaStreamDestroy(e->side);
   if (e->stream && e->own_stream) cudaStreamDestroy(e->stream);
   delete e;
 }
@@ -793,18 +938,18 @@ static bool narrow_tile(const pm_engine* e, bool fast) {
 }
 
 static void launch_build(pm_engine* e, const pm::EvalParams& p, int bits_mode, bool fast, bool narrow, dim3 grid,
-                         uint32_t t0, uint32_t nt, uint32_t w0, uint32_t nw, size_t ld) {
-#define PM_BUILD_CASE(B, F) pm::pm_build_cost<B, F><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, t0, nt, w0, nw, e->cost.p, ld)
+                         uint32_t t0, uint32_t nt, uint32_t w0, uint32_t nw, long long* tile, size_t ld) {
+#define PM_BUILD_CASE(B, F) pm::pm_build_cost<B, F><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, t0, nt, w0, nw, tile, ld)
 #define PM_FAST_CASE(B, R)                                                                                              \
   {                                                                                                                     \
     grid.y = blocks_for(nt, R);                                                                                         \
-    if (narrow) pm::pm_build_cost_fast<B, R, true><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, t0, nt, w0, nw, e->cost.p, ld);   \
-    else pm::pm_build_cost_fast<B, R, false><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, t0, nt, w0, nw, e->cost.p, ld);         \
+    if (narrow) pm::pm_build_cost_fast<B, R, true><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, t0, nt, w0, nw, tile, ld);   \
+    else pm::pm_build_cost_fast<B, R, false><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, t0, nt, w0, nw, tile, ld);         \
   }
   if (fast && bits_mode == 2 && e->tune_build == 3) {
-    pm::pm_build_cost<2, true, 3><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, t0, nt, w0, nw, e->cost.p, ld);
+    pm::pm_build_cost<2, true, 3><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, t0, nt, w0, nw, tile, ld);
   } else if (fast && bits_mode == 2 && e->tune_build == 4) {
-    pm::pm_build_cost<2, true, 4><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, t0, nt, w0, nw, e->cost.p, ld);
+    pm::pm_build_cost<2, true, 4><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, t0, nt, w0, nw, tile, ld);
   } else if (fast && e->tune_build != 1) {   // the FastRow kernel; PM_TUNE_BUILD=1 keeps the staged-CSR form for A/B runs
     // one-word acceptance rows are bound into the FastRows (pm_bind_rows) however many rows there are
     if (p.words == 1) bits_mode = 2;
@@ -834,17 +979,18 @@ static void launch_fused(pm_engine* e, const pm::EvalParams& p, int bits_mode, b
 #undef PM_FUSED_CASE
 }
 
-static void launch_argmin(pm_engine* e, bool narrow, size_t ld, uint32_t nt, uint32_t t0, uint32_t w0, uint32_t nw) {
+static void launch_argmin(pm_engine* e, cudaStream_t st, bool narrow, const long long* tile, size_t ld, uint32_t nt,
+                          uint32_t t0, uint32_t w0, uint32_t nw) {
   if (narrow) {   // 16 x 16 B in flight per lane, as the wide <8, 2>; PM_TUNE_ARGMIN shapes the int64 tile's kernel only
     dim3 grid(blocks_for(ld, 8 * 128 * pm::kArgWarps), blocks_for(nt, pm::kArgRows));
-    pm::pm_argmin<8, 2, true><<<grid, pm::kArgThreads, 0, e->stream>>>(e->cost.p, ld, nt, t0, w0, nw, e->first_ask.p,
-                                                                      e->ask_best.p, e->ask_count.p);
+    pm::pm_argmin<8, 2, true><<<grid, pm::kArgThreads, 0, st>>>(tile, ld, nt, t0, w0, nw, e->first_ask.p,
+                                                               e->ask_best.p, e->ask_count.p);
     return;
   }
 #define PM_ARGMIN_CASE(S, RPW)                                                                      \
   {                                                                                                  \
     dim3 grid(blocks_for(ld, (S) * 64 * pm::kArgWarps), blocks_for(nt, pm::kArgRows));                               \
-    pm::pm_argmin<S, RPW><<<grid, pm::kArgThreads, 0, e->stream>>>(e->cost.p, ld, nt, t0, w0, nw,    \
+    pm::pm_argmin<S, RPW><<<grid, pm::kArgThreads, 0, st>>>(tile, ld, nt, t0, w0, nw,                \
                                                                    e->first_ask.p, e->ask_best.p,   \
                                                                    e->ask_count.p);                 \
   }
@@ -916,7 +1062,7 @@ static int match_local_locked(pm_engine* e, uint32_t mode) {
       if (rc != PM_OK) return rc;
     }
     if (mode & PM_PATH_FUSED) {
-      Timer tm(e, &e->stats.ms_fused);
+      Timer tm(e, &e->stats.ms_fused, e->stream);
       const uint32_t rows_per_launch = 65535u * pm::kEvalRows;
       for (uint32_t t0 = 0; t0 < T; t0 += rows_per_launch) {
         const uint32_t nt = std::min(rows_per_launch, T - t0);
@@ -944,33 +1090,58 @@ static int match_local_locked(pm_engine* e, uint32_t mode) {
       rows = std::min<uint64_t>(rows, T);
       rows = std::min<uint64_t>(rows, 65535ull * pm::kArgRows);
       if (rows >= 1024) rows &= ~(uint64_t)511;   // whole row bands of the build kernel (no ragged last band in every tile)
-      cudaError_t ce = e->cost.ensure((size_t)rows * ld * elem_bytes / 8);   // ld is a multiple of 1024
-      if (ce != cudaSuccess) {
+      // Two 32-bit tiles take the bytes of one int64 tile: with both, argmin(k) runs on the side stream beside
+      // build(k + 1) into the other buffer.  The build is limited by instruction issue and the argmin by HBM, so the
+      // pair overlaps instead of leaving each kernel's tail wave and the other's unused bandwidth idle.  When the
+      // second buffer does not fit, the tiles run one after the other as with the int64 tile.
+      const size_t tile_elems = (size_t)rows * ld * elem_bytes / 8;   // TileBuf elements; ld is a multiple of 1024
+      bool overlap = narrow && e->tune_overlap != 0 && T > rows;
+      if (overlap && e->cost.ensure(2 * tile_elems, e->device, e->tune_compress != 0, e->stream) != cudaSuccess) {
+        cudaGetLastError();
+        overlap = false;
+      }
+      if (!overlap && e->cost.ensure(tile_elems, e->device, e->tune_compress != 0, e->stream) != cudaSuccess) {
         cudaGetLastError();
         return e->fail(PM_E_NOMEM, "pm_match: cannot allocate the cost tile; lower pm_cfg.cost_tile_bytes");
       }
-      for (uint32_t t0 = 0; t0 < T; t0 += (uint32_t)rows) {
+      cudaStream_t arg_stream = e->stream;
+      if (overlap) {   // the side stream starts after the results are initialised and the tables are bound
+        PM_CUDA(cudaEventRecord(e->ev_fork, e->stream));
+        PM_CUDA(cudaStreamWaitEvent(e->side, e->ev_fork, 0));
+        arg_stream = e->side;
+      }
+      uint32_t k = 0;
+      for (uint32_t t0 = 0; t0 < T; t0 += (uint32_t)rows, ++k) {
         const uint32_t nt = (uint32_t)std::min<uint64_t>(rows, T - t0);
+        long long* tile = e->cost.p + (overlap ? (k & 1u) * tile_elems : 0);
+        if (overlap && k >= 2) PM_CUDA(cudaStreamWaitEvent(e->stream, e->ev_read[k & 1u], 0));   // argmin(k - 2) is done with it
         {
-          Timer tm(e, &e->stats.ms_build);
+          Timer tm(e, &e->stats.ms_build, e->stream);
           dim3 grid(blocks_for(ld, pm::kEvalCols), blocks_for(nt, pm::kEvalRows));
-          launch_build(e, p, bits_mode, fast, narrow, grid, t0, nt, w0, nw, ld);
+          launch_build(e, p, bits_mode, fast, narrow, grid, t0, nt, w0, nw, tile, ld);
           PM_LAUNCH_CHECK("pm_build_cost");
           tm.stop();
           ++e->stats.n_build_launches;
         }
+        if (overlap) {
+          PM_CUDA(cudaEventRecord(e->ev_built, e->stream));
+          PM_CUDA(cudaStreamWaitEvent(e->side, e->ev_built, 0));
+        }
         {
-          Timer tm(e, &e->stats.ms_argmin);
-          launch_argmin(e, narrow, ld, nt, t0, w0, nw);
+          Timer tm(e, &e->stats.ms_argmin, arg_stream);
+          launch_argmin(e, arg_stream, narrow, tile, ld, nt, t0, w0, nw);
           PM_LAUNCH_CHECK("pm_argmin");
           tm.stop();
           ++e->stats.n_argmin_launches;
         }
+        if (overlap) PM_CUDA(cudaEventRecord(e->ev_read[k & 1u], e->side));
         ++e->stats.n_tiles;
         // algorithmic: 4 or 8 B per evaluation, the tile's element (padding columns not counted)
         e->stats.cost_bytes_written += (uint64_t)nt * nw * elem_bytes;
         e->stats.cost_bytes_read += (uint64_t)nt * nw * elem_bytes;
       }
+      // join: the resolution, the exchange and the caller's own work on the engine stream come after the last argmin
+      if (overlap) PM_CUDA(cudaStreamWaitEvent(e->stream, e->ev_read[(k - 1) & 1u], 0));
     }
     e->stats.evals = (uint64_t)T * nw;
   }
@@ -1009,7 +1180,7 @@ static int match_finish_locked(pm_engine* e, uint32_t mode) {
   const bool prox_general = (base_mode == PM_MODE_PROXIMITY && !e->all_solo) || merge_mode;
   const uint32_t shift = (base_mode == PM_MODE_PROXIMITY && !prox_general) ? 1u : 0u;
   const uint32_t n_bins = T << shift;
-  Timer tm(e, &e->stats.ms_resolve);
+  Timer tm(e, &e->stats.ms_resolve, e->stream);
 
   PM_CUDA(e->keys.ensure(W)); PM_CUDA(e->keys_sorted.ensure(W)); PM_CUDA(e->iota.ensure(W));
   PM_CUDA(e->order.ensure(W)); PM_CUDA(e->hist.ensure((size_t)n_bins + 1));
@@ -1219,7 +1390,7 @@ static int match_auction_locked(pm_engine* e) {
   e->ev_pending.clear();
   e->ev_used = 0;
   if (e->cfg.flags & PM_CFG_TIMING) PM_CUDA(cudaEventRecord(e->ev0, e->stream));
-  Timer tm(e, &e->stats.ms_fused);
+  Timer tm(e, &e->stats.ms_fused, e->stream);
   if (!e->auc_classes_valid) {
     const int rc = auction_build_classes(e);
     if (rc != PM_OK) return rc;
@@ -1400,7 +1571,7 @@ static int match_auction_locked(pm_engine* e) {
   e->stats.n_launches = e->h_ctl.p->rounds * (packed_claim ? 6u : 7u);
   e->stats.n_build_launches = (uint32_t)std::min<unsigned long long>(e->h_ctl.p->n_refills, 0xFFFFFFFFull);
   tm.stop();
-  Timer tr(e, &e->stats.ms_resolve);
+  Timer tr(e, &e->stats.ms_resolve, e->stream);
   // result: one solo group per assigned ask, ask order
   pm::pm_auction_flags<<<blocks_for((size_t)T + 1, 256), 256, 0, e->stream>>>(e->auc_assigned.p, T, e->auc_flag.p);
   PM_LAUNCH_CHECK("pm_auction_flags");
@@ -1506,7 +1677,7 @@ static int exchange_locked(pm_engine* e) {
   const size_t stride = (((size_t)T * 12 + (size_t)per * 4) + 15) & ~(size_t)15;
   PM_CUDA(e->xchg_send.ensure(stride));
   PM_CUDA(e->xchg_recv.ensure(stride * n));
-  Timer tm(e, &e->stats.ms_exchange);
+  Timer tm(e, &e->stats.ms_exchange, e->stream);
   const size_t work = std::max<size_t>(std::max<size_t>(T, W), 1);
   pm::pm_xchg_pack<<<std::min(blocks_for(work, 256), 8u * e->sms), 256, 0, e->stream>>>(e->first_ask.p + w0, nw, per, e->ask_best.p, e->ask_count.p, T,
                                                                                   e->xchg_send.p);
@@ -1654,7 +1825,7 @@ int pm_build_cost_tile(pm_engine* e, uint32_t t0, uint32_t nt, int64_t* host_out
   }
   const size_t ld = (((size_t)nw + pm::kEvalCols - 1) / pm::kEvalCols) * pm::kEvalCols;
   if (nt > 65535u * pm::kEvalRows) return e->fail(PM_E_INVALID, "pm_build_cost_tile: too many rows");
-  if (e->cost.ensure((size_t)nt * ld) != cudaSuccess) {
+  if (e->cost.ensure((size_t)nt * ld, e->device, e->tune_compress != 0, e->stream) != cudaSuccess) {
     cudaGetLastError();
     return e->fail(PM_E_NOMEM, "pm_build_cost_tile: cannot allocate the tile");
   }
@@ -1673,7 +1844,7 @@ int pm_build_cost_tile(pm_engine* e, uint32_t t0, uint32_t nt, int64_t* host_out
     rc = bind_rows(e, wm);
     if (rc != PM_OK) return rc;
   }
-  launch_build(e, p, bits_mode, fast, false, grid, t0, nt, w0, nw, ld);   // exports the int64 tile
+  launch_build(e, p, bits_mode, fast, false, grid, t0, nt, w0, nw, e->cost.p, ld);   // exports the int64 tile
   PM_LAUNCH_CHECK("pm_build_cost");
   PM_CUDA(cudaMemcpy2DAsync(host_out, (size_t)nw * 8, e->cost.p, ld * 8, (size_t)nw * 8, nt,
                             cudaMemcpyDeviceToHost, e->stream));

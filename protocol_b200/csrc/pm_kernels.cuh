@@ -343,7 +343,7 @@ __device__ __forceinline__ void eval_fast_more(const DevOptF* __restrict__ gopts
 
 template <int ROWS>
 struct __align__(128) FastStage {
-  FastRow row[ROWS];
+  FastRow row[ROWS + 2];   // + 2: the look-ahead loads of the band's last pair of rows may read past it (never used)
   uint32_t bits[kBitsCap];
   uint64_t bar;
 };
@@ -385,26 +385,35 @@ pm_build_cost_fast(EvalParams p, uint32_t t0, uint32_t nt, uint32_t w0, uint32_t
     } else w[k] = null_worker();
     dx[k] = 0xFFFFFFFFu - gw[k];          // infeasible: 0x7FFFFFFF_FFFFFFFF = feasible word + (0/1) * difference
     dy[k] = 0x7FFFFFFFu - w[k].price;     // (the narrow form keeps only this high word)
+    asm("" : "+r"(dy[k]));                // kept in a register: ptxas would otherwise recompute it from the price every row
   }
   uint4* out = NARROW ? reinterpret_cast<uint4*>(static_cast<uint32_t*>(tile) + (size_t)r0 * ld + cbase)
                       : reinterpret_cast<uint4*>(static_cast<long long*>(tile) + (size_t)r0 * ld + cbase);
-  const size_t row_stride = NARROW ? ld / 4 : ld / 2;   // in 16-byte units
+  size_t row_stride = NARROW ? ld / 4 : ld / 2;   // in 16-byte units
+  asm("" : "+l"(row_stride));           // held in registers: ptxas would otherwise re-derive it from `ld` every row
   const uint32_t sh = p.sign_shift;
-  __syncthreads();            // mbarrier initialised, acceptance words staged
-  mbar_wait(&s.bar, 0);
-  FastRow cur = s.row[0];
-  for (uint32_t r = 0; r < nrows; ++r) {
-    FastRow nxt = cur;
-    if (r + 1 < nrows) nxt = s.row[r + 1];    // in flight while this row is evaluated
-    uint32_t um[kEvalWPT];
-    eval_fast_first<kEvalWPT, BITS>(cur, s.bits, w, p.bits, p.words, um);
-    if (cur.n_opts > 1u)                      // OR-options (node.rs:420-438): the ask fails only if every option does
-      eval_fast_more<kEvalWPT, BITS>(p.opts_fast + cur.opt_off + 1, cur.n_opts - 1u, s.bits, w, p.bits, p.words, um);
+  // One row.  The ask's scalar thresholds are OR-ed into the first option's clauses before the further OR-options are
+  // AND-ed in — fail = AND_o(u_o | s) = (AND_o u_o) | s — so a single-option row is one 7-term OR per worker.
+  auto emit = [&](const FastRow& q, uint4* dst) {
+    uint32_t f[kEvalWPT], sc[kEvalWPT];
+    eval_fast_first<kEvalWPT, BITS>(q, s.bits, w, p.bits, p.words, f);
+#pragma unroll
+    for (int k = 0; k < kEvalWPT; ++k) {
+      sc[k] = (w[k].cores - q.cpu_cores) | (w[k].ram - q.ram_mb) | (w[k].storage - q.storage_gb);
+      f[k] |= sc[k];
+    }
+    if (q.n_opts > 1u) {   // OR-options (node.rs:420-438), one ask in ten: the ask fails only if every option does
+      uint32_t um[kEvalWPT];
+#pragma unroll
+      for (int k = 0; k < kEvalWPT; ++k) um[k] = 0xFFFFFFFFu;
+      eval_fast_more<kEvalWPT, BITS>(p.opts_fast + q.opt_off + 1, q.n_opts - 1u, s.bits, w, p.bits, p.words, um);
+#pragma unroll
+      for (int k = 0; k < kEvalWPT; ++k) f[k] &= um[k] | sc[k];
+    }
     uint32_t o[2 * kEvalWPT];
 #pragma unroll
     for (int k = 0; k < kEvalWPT; ++k) {
-      const uint32_t fail = um[k] | (w[k].cores - cur.cpu_cores) | (w[k].ram - cur.ram_mb) | (w[k].storage - cur.storage_gb);
-      const uint32_t b = fail >> sh;                                    // 1 when infeasible (sh == 31)
+      const uint32_t b = f[k] >> sh;                                    // 1 when infeasible (sh == 31)
       if (NARROW) {
         o[k] = b * dy[k] + w[k].price;                                  // feasible: price ; infeasible: kNarrowInfeasible
       } else {
@@ -413,13 +422,24 @@ pm_build_cost_fast(EvalParams p, uint32_t t0, uint32_t nt, uint32_t w0, uint32_t
       }
     }
     if (NARROW) {
-      __stcs(out, make_uint4(o[0], o[1], o[2], o[3]));
+      __stcs(dst, make_uint4(o[0], o[1], o[2], o[3]));
     } else {
-      __stcs(out, make_uint4(o[0], o[1], o[2], o[3]));
-      __stcs(out + 32, make_uint4(o[4], o[5], o[6], o[7]));     // + 64 columns
+      __stcs(dst, make_uint4(o[0], o[1], o[2], o[3]));
+      __stcs(dst + 32, make_uint4(o[4], o[5], o[6], o[7]));     // + 64 columns
     }
-    out += row_stride;
-    cur = nxt;
+  };
+  __syncthreads();            // mbarrier initialised, acceptance words staged
+  mbar_wait(&s.bar, 0);
+  // Two rows per iteration share the loop test and the output-pointer bump.  Each row's FastRow is loaded one row
+  // ahead, into registers the previous row has finished with, so no row is copied from one buffer to another.
+  const FastRow* q = s.row;
+  FastRow a = q[0];
+  for (uint32_t r = 0; r < nrows; r += 2, q += 2) {
+    const FastRow b = q[1];                   // in flight while row r is evaluated
+    emit(a, out);
+    a = q[2];                                 // in flight while row r + 1 is evaluated
+    if (r + 1 < nrows) emit(b, out + row_stride);
+    out += 2 * row_stride;
   }
 }
 
