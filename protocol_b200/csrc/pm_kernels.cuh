@@ -585,11 +585,14 @@ pm_argmin(const void* __restrict__ tile, size_t ld, uint32_t nt, uint32_t t0, ui
 
 // ------------------------------------------------------------------ fused
 // Same stripe/row decomposition as pm_build_cost, but the int64 cost never
-// leaves the SM: per-row results go through ballots (first-fit cost is the
-// worker index, so the row minimum is the lowest set bit), per-worker results
-// stay in registers.  Integer-issue-bound, not HBM-bound.
+// leaves the SM: per-worker results stay in registers, and each row's minimum is
+// the one pm_argmin finds, the signed int64 least (price << 32) | worker over the
+// feasible workers.  A warp takes it in two steps: the least price read as int32
+// (signed redux; that order is the packed cost's for prices >= 2^31 too), then
+// the lowest worker at that price from one ballot per k.  Integer-issue-bound,
+// not HBM-bound.
 // STATS = false skips the per-ask (min, count) outputs — the reference modes only need the
-// per-worker first feasible ask — which removes the ballots from the inner loop.
+// per-worker first feasible ask — which removes the reductions from the inner loop.
 template <int BITS, bool FAST, bool STATS>
 __global__ void __launch_bounds__(kEvalThreads, 2)
 pm_fused_eval(EvalParams p, uint32_t t0, uint32_t nt, uint32_t w0, uint32_t nw,
@@ -597,12 +600,15 @@ pm_fused_eval(EvalParams p, uint32_t t0, uint32_t nt, uint32_t w0, uint32_t nw,
               uint32_t* __restrict__ ask_count) {
   __shared__ EvalStage s;
   __shared__ uint32_t s_cnt[kEvalRows];
-  __shared__ uint32_t s_best[kEvalRows];
+  // signed, as the packed cost: a price >= 2^31 makes it negative.  Unused without STATS, where it keeps the 32-bit
+  // form the lean kernel has always been compiled with.
+  using Best = std::conditional_t<STATS, long long, uint32_t>;
+  __shared__ Best s_best[kEvalRows];
   const uint32_t r0 = blockIdx.y * kEvalRows;
   const uint32_t r1 = min(nt, r0 + (uint32_t)kEvalRows);
   for (uint32_t i = threadIdx.x; i < (uint32_t)kEvalRows; i += kEvalThreads) {
     s_cnt[i] = 0;
-    s_best[i] = kNone;
+    s_best[i] = STATS ? (Best)kInf : (Best)kNone;
   }
   const uint32_t lane = threadIdx.x & 31u;
   const uint32_t c = blockIdx.x * kEvalCols + threadIdx.x * kEvalWPT;
@@ -628,16 +634,24 @@ pm_fused_eval(EvalParams p, uint32_t t0, uint32_t nt, uint32_t w0, uint32_t nw,
 #pragma unroll
     for (int k = 0; k < kEvalWPT; ++k) first[k] = min(first[k], t | ~f[k]);
     if (STATS) {
-      uint32_t cnt = 0, best = kNone;
+      uint32_t n = 0;
+      int lp = INT32_MAX;   // the lane's least feasible price, or INT32_MAX: the ballots below only see feasible workers
 #pragma unroll
       for (int k = 0; k < kEvalWPT; ++k) {
-        const uint32_t b = __ballot_sync(0xffffffffu, f[k] != 0u);
-        cnt += (uint32_t)__popc(b);
+        n += f[k] & 1u;
+        if (f[k]) lp = min(lp, (int)w[k].price);
+      }
+      const uint32_t cnt = __reduce_add_sync(0xffffffffu, n);
+      const int price = __reduce_min_sync(0xffffffffu, lp);
+      uint32_t best = kNone;   // the warp's lowest worker offset at that price
+#pragma unroll
+      for (int k = 0; k < kEvalWPT; ++k) {
+        const uint32_t b = __ballot_sync(0xffffffffu, f[k] != 0u && (int)w[k].price == price);
         if (b) best = min(best, ((uint32_t)__ffs(b) - 1u) * kEvalWPT + k);
       }
       if (cnt && lane == 0) {
         atomicAdd(&s_cnt[r], cnt);
-        atomicMin(&s_best[r], warp_gw0 + best);
+        atomicMin(&s_best[r], (long long)(((unsigned long long)(uint32_t)price << 32) | (warp_gw0 + best)));
       }
     }
   });
@@ -649,7 +663,7 @@ pm_fused_eval(EvalParams p, uint32_t t0, uint32_t nt, uint32_t w0, uint32_t nw,
   for (uint32_t i = threadIdx.x; i < r1 - r0; i += kEvalThreads) {
     if (s_cnt[i]) {
       atomicAdd(ask_count + t0 + r0 + i, s_cnt[i]);
-      atomicMin(ask_best + t0 + r0 + i, (long long)s_best[i]);
+      atomicMin(ask_best + t0 + r0 + i, s_best[i]);
     }
   }
 }

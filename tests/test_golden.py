@@ -32,6 +32,15 @@ def test_oracle_reproduces_golden(name):
     g = orc.soa_form_groups(w.a, w.b, a.asks, a.opts, bits, words, addr_rank=w.addr_rank, lat=w.lat, lon=w.lon, proximity=prox)
     assert np.array_equal(g.cfg, z["group_ask"]) and np.array_equal(g.off, z["group_off"])
     assert np.array_equal(g.members, z["group_members"])
+    ev = orc.soa_eval_matrix(w.a, w.b, a.asks, a.opts, bits, words, 0, len(a), 0, len(w), threads=8)
+    assert np.array_equal(ev["row_best"], z["ask_best"]) and np.array_equal(ev["row_count"], z["ask_count"])
+
+
+def test_priced_golden_has_ties_and_negative_costs():
+    """first_fit_priced freezes row minima at Zipf prices and at prices of 2^31 and above (negative packed costs)."""
+    z = load("first_fit_priced")
+    hi = z["ask_best"][z["ask_count"] > 0] >> 32
+    assert (hi == -(1 << 31)).any() and (hi == -1).any() and (hi > 0).any() and (hi != 0).all()
 
 
 @pytest.mark.gpu

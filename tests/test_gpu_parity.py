@@ -16,8 +16,8 @@ pytestmark = pytest.mark.gpu
 MAT, FUSED = abi.PM_PATH_MATERIALIZED, abi.PM_PATH_FUSED
 
 
-def synth_tables(n_asks, n_workers, kind="mixed", group_sizes=None, seed_shift=0, with_addresses=False):
-    w = synth.make_workers(n_workers, seed=synth.SEED_WORKERS + seed_shift, with_addresses=with_addresses)
+def synth_tables(n_asks, n_workers, kind="mixed", group_sizes=None, seed_shift=0, with_addresses=False, price=None):
+    w = synth.make_workers(n_workers, seed=synth.SEED_WORKERS + seed_shift, with_addresses=with_addresses, price=price)
     a = synth.make_asks(n_asks, kind, seed=synth.SEED_ASKS + seed_shift, group_sizes=group_sizes)
     bits, npat, nmod, words = synth.intern_tables(w, a)
     return w, a, dict(asks=a.asks, opts=a.opts, wa=w.a, wb=w.b, bits=bits, n_patterns=npat, n_models=nmod,
@@ -179,12 +179,15 @@ def test_proximity_solo_groups_order():
 
 
 def test_materialized_and_fused_agree_multi_tile():
-    w, a, t = synth_tables(5000, 20000, "skewed")
+    """Zipf prices (many ties in the cost's high word): the fused pass's row minimum is the argmin's, lowest worker
+    among the cheapest."""
+    w, a, t = synth_tables(5000, 20000, "skewed", price="zipf")
     eng = Engine(cost_tile_bytes=32 << 20)
     load_engine(eng, t)
     eng.match(abi.PM_MODE_FIRST_FIT | MAT)
     r1 = eng.fetch()
     assert r1.stats["n_tiles"] > 1
+    assert (r1.ask_best[r1.ask_count > 0] >> 32 >= 1).all()   # every row minimum carries a price
     eng.match(abi.PM_MODE_FIRST_FIT | FUSED)
     r2 = eng.fetch()
     for f in ("worker_group", "worker_ask", "group_ask", "group_off", "group_members", "ask_best", "ask_count"):
@@ -742,7 +745,7 @@ def test_cfg4_shape_one_million_asks_x_250k_workers():
     # the other paths agree bit for bit
     eng.match(abi.PM_MODE_FIRST_FIT | FUSED)
     r2 = eng.fetch()
-    for f in ("worker_group", "worker_ask", "group_ask", "group_off", "group_members", "ask_count"):
+    for f in ("worker_group", "worker_ask", "group_ask", "group_off", "group_members", "ask_best", "ask_count"):
         assert np.array_equal(getattr(r1, f), getattr(r2, f)), f
     eng.close()
 

@@ -139,9 +139,12 @@ def many_option_requirement(n_opts, feasible_every, pats):
     return ";".join(parts)
 
 
-@pytest.mark.parametrize("n_models", [16, 200], ids=["uniform_word", "per_worker_word"])
-def test_asks_with_more_options_than_the_stage_holds(n_models):
-    """One ask with 500 OR-options (eval_row_global), neighbours with exactly 384 and 385, between ordinary asks."""
+BIG_ASKS = {40: 500, 41: 384, 42: 385, 170: 1200, 299: 400}   # ask -> OR-options; the stage holds 384
+
+
+def many_option_tables(n_models):
+    """300 ordinary asks over 5000 workers, with the asks of BIG_ASKS replaced by ones with that many OR-options:
+    (workers, asks, oracle table, product table, n_patterns, n_models, words)."""
     cat = synth.wide_model_catalogue(n_models)
     w = synth.make_workers(5000, seed=synth.SEED_WORKERS + 9, catalogue=cat)
     base = synth.make_asks(300, "mixed", seed=synth.SEED_ASKS + 9)
@@ -152,11 +155,10 @@ def test_asks_with_more_options_than_the_stage_holds(n_models):
     for i, p in enumerate(pats):
         assert it.pattern(p) == i
     rows, opts = [], []
-    big = {40: 500, 41: 384, 42: 385, 170: 1200, 299: 400}
     for t in range(300):
-        if t in big:
-            row, o = it.parse(many_option_requirement(big[t], 97 if t != 41 else 50, pats), max_opts=2048)
-            assert len(o) == big[t]
+        if t in BIG_ASKS:
+            row, o = it.parse(many_option_requirement(BIG_ASKS[t], 97 if t != 41 else 50, pats), max_opts=2048)
+            assert len(o) == BIG_ASKS[t]
         else:
             row, o = base.asks[t].copy(), base.opts[int(base.asks["opt_off"][t]):int(base.asks["opt_off"][t]) + int(base.asks["n_opts"][t])]
         row = row.copy()
@@ -169,8 +171,15 @@ def test_asks_with_more_options_than_the_stage_holds(n_models):
     it.close()
     obits, o_npat, o_nmod, o_words = orc.model_table(w.model_strings, pats)
     assert (npat, nmod, words) == (o_npat, o_nmod, o_words) and np.array_equal(obits, pbits)
+    return w, a, obits, pbits, npat, nmod, words
+
+
+@pytest.mark.parametrize("n_models", [16, 200], ids=["uniform_word", "per_worker_word"])
+def test_asks_with_more_options_than_the_stage_holds(n_models):
+    """One ask with 500 OR-options (eval_row_global), neighbours with exactly 384 and 385, between ordinary asks."""
+    w, a, obits, pbits, npat, nmod, words = many_option_tables(n_models)
     # the big asks must not be trivially empty or trivially full
     ev = orc.soa_eval_matrix(w.a, w.b, a.asks, a.opts, obits, words, 0, 300, 0, 5000, threads=8)
-    for t in big:
+    for t in BIG_ASKS:
         assert 0 < ev["row_count"][t] < 4500
     run_all_paths(w, a, obits, pbits, npat, nmod, words, expect_bits=2 if n_models <= 31 else 1, check_cost_rows=300)
