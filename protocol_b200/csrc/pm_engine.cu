@@ -265,10 +265,6 @@ struct pm_engine {
   int device = 0;
   unsigned sms = 132;     // streaming multiprocessors of the device (an H100 SXM has 132): caps of the grid-stride launches
   cudaStream_t stream = nullptr;
-  // The double-buffered 32-bit tile's argmin runs here, beside the next tile's build on `stream`; forked from and
-  // joined back into `stream` by events inside every pass, so nothing is left running on it between calls.
-  cudaStream_t side = nullptr;
-  cudaEvent_t ev_fork = nullptr, ev_built = nullptr, ev_read[2] = {nullptr, nullptr};
   std::string err;
   std::mutex mu;
 
@@ -279,8 +275,8 @@ struct pm_engine {
   bool have_workers = false, have_asks = false, have_bits = false, have_loc = false, have_rank = false;
   bool all_solo = true;  // every ask has min == max == 1
   int tune_argmin = 0, tune_generic = 0, tune_build = 0, tune_auction = 0, tune_prox = 0, tune_auc_good = 0, tune_auc_extra = 0;   // PM_TUNE_*: kernel-shape experiments
-  int tune_overlap = 0;   // PM_TUNE_OVERLAP=1: the 32-bit tile's argmin(k) beside build(k + 1) (slower with compressible tile memory)
   int tune_compress = 1;  // PM_TUNE_COMPRESS=0: the cost tile in plain cudaMalloc memory (A/B runs)
+  int tune_pipe = 16;     // PM_TUNE_PIPE: rows per band of pm_build_argmin (8 / 16 / 32 / 64); 0: build + argmin launches
   DevBuf<uint4> wa, wb;
   DevBuf<double> lat, lon;
   DevBuf<uint32_t> addr_rank;
@@ -422,7 +418,7 @@ namespace {
 // Per-launch CUDA-event timing without host synchronisation: start/stop events
 // are recorded around a region on the stream its kernels run on and resolved in
 // one go at the end of the match (which synchronises anyway to read the group
-// count; every side-stream region is joined into the engine stream before that).
+// count).
 struct Timer {
   pm_engine* e;
   float* acc;
@@ -523,8 +519,11 @@ int pm_create(const pm_cfg* cfg, pm_engine** out) try {
   if (const char* t = std::getenv("PM_TUNE_AUCTION")) e->tune_auction = std::atoi(t);
   if (const char* t = std::getenv("PM_TUNE_AUCTION_POOL")) std::sscanf(t, "%d,%d", &e->tune_auc_good, &e->tune_auc_extra);   // pool fill of a class walk
   if (const char* t = std::getenv("PM_TUNE_PROX")) e->tune_prox = std::atoi(t);   // 0: all-SM cooperative sweep; 2: single-CTA sweep; 1: latitude-banded single-CTA sweep (experimental)
-  if (const char* t = std::getenv("PM_TUNE_OVERLAP")) e->tune_overlap = std::atoi(t);
   if (const char* t = std::getenv("PM_TUNE_COMPRESS")) e->tune_compress = std::atoi(t);
+  if (const char* t = std::getenv("PM_TUNE_PIPE")) {   // other values keep the default band
+    const int v = std::atoi(t);
+    if (v == 0 || v == 8 || v == 16 || v == 32 || v == 64) e->tune_pipe = v;
+  }
   bool ok = cudaSetDevice(e->device) == cudaSuccess;
   if (ok && cfg->stream) {
     e->stream = (cudaStream_t)cfg->stream;  // caller's stream (e.g. torch's current stream)
@@ -532,13 +531,6 @@ int pm_create(const pm_cfg* cfg, pm_engine** out) try {
   } else if (ok) {
     ok = cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking) == cudaSuccess;
   }
-  int prio = 0;
-  ok = ok && cudaStreamGetPriority(e->stream, &prio) == cudaSuccess &&
-       cudaStreamCreateWithPriority(&e->side, cudaStreamNonBlocking, prio) == cudaSuccess &&
-       cudaEventCreateWithFlags(&e->ev_fork, cudaEventDisableTiming) == cudaSuccess &&
-       cudaEventCreateWithFlags(&e->ev_built, cudaEventDisableTiming) == cudaSuccess &&
-       cudaEventCreateWithFlags(&e->ev_read[0], cudaEventDisableTiming) == cudaSuccess &&
-       cudaEventCreateWithFlags(&e->ev_read[1], cudaEventDisableTiming) == cudaSuccess;
   ok = ok &&
             cudaEventCreate(&e->ev0) == cudaSuccess && cudaEventCreate(&e->ev1) == cudaSuccess &&
             e->h_scalars.ensure(64) == cudaSuccess && e->counters.ensure(32) == cudaSuccess;
@@ -590,9 +582,6 @@ void pm_destroy(pm_engine* e) {
   if (e->ev0) cudaEventDestroy(e->ev0);
   if (e->ev1) cudaEventDestroy(e->ev1);
   for (cudaEvent_t ev : e->ev_pool) cudaEventDestroy(ev);
-  for (cudaEvent_t ev : {e->ev_fork, e->ev_built, e->ev_read[0], e->ev_read[1]})
-    if (ev) cudaEventDestroy(ev);
-  if (e->side) cudaStreamDestroy(e->side);
   if (e->stream && e->own_stream) cudaStreamDestroy(e->stream);
   delete e;
 }
@@ -929,7 +918,8 @@ static int worker_major(pm_engine* e, pm::EvalParams* p, int* bits_mode) {
   return PM_OK;
 }
 
-// The 32-bit cost tile (pm_build_cost_fast<.., true> + pm_argmin<.., true>): on the default FastRow path, for tables
+// The 32-bit cost tile (pm_build_argmin, or pm_build_cost_fast<.., true> + pm_argmin<.., true> under PM_TUNE_PIPE=0 and
+// PM_TUNE_BUILD=5 / 6): on the default FastRow path, for tables
 // whose every price is below 0x7FFFFFFF (decide_fast).  The staged kernels (PM_TUNE_BUILD = 1, 3, 4), the generic
 // predicate and other prices keep the int64 tile; PM_TUNE_BUILD=8 keeps it on the FastRow path too, for A/B runs.
 static bool narrow_tile(const pm_engine* e, bool fast) {
@@ -977,6 +967,18 @@ static void launch_fused(pm_engine* e, const pm::EvalParams& p, int bits_mode, b
     if (bits_mode == 2) PM_FUSED_CASE(2, false, true); else if (bits_mode == 1) PM_FUSED_CASE(1, false, true); else PM_FUSED_CASE(0, false, true);
   }
 #undef PM_FUSED_CASE
+}
+
+// pm_build_argmin: the 32-bit tile's build and argmin in one launch (PM_TUNE_PIPE rows per band)
+static void launch_build_argmin(pm_engine* e, const pm::EvalParams& p, int bits_mode, uint32_t t0, uint32_t nt, uint32_t w0,
+                                uint32_t nw, long long* tile, size_t ld) {
+  const dim3 grid(blocks_for(ld, pm::kEvalCols), blocks_for(nt, pm::kFastRows));
+  const pm::BandOut bo{(uint32_t)e->tune_pipe, e->first_ask.p, e->ask_best.p, e->ask_count.p};
+  uint32_t* t32 = reinterpret_cast<uint32_t*>(tile);
+  if (p.words == 1) bits_mode = 2;   // one-word acceptance rows are bound into the FastRows, as in launch_build
+  if (bits_mode == 2) pm::pm_build_argmin<2><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, t0, nt, w0, nw, t32, ld, bo);
+  else if (bits_mode == 1) pm::pm_build_argmin<1><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, t0, nt, w0, nw, t32, ld, bo);
+  else pm::pm_build_argmin<0><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, t0, nt, w0, nw, t32, ld, bo);
 }
 
 static void launch_argmin(pm_engine* e, cudaStream_t st, bool narrow, const long long* tile, size_t ld, uint32_t nt,
@@ -1090,58 +1092,49 @@ static int match_local_locked(pm_engine* e, uint32_t mode) {
       rows = std::min<uint64_t>(rows, T);
       rows = std::min<uint64_t>(rows, 65535ull * pm::kArgRows);
       if (rows >= 1024) rows &= ~(uint64_t)511;   // whole row bands of the build kernel (no ragged last band in every tile)
-      // Two 32-bit tiles take the bytes of one int64 tile: with both, argmin(k) runs on the side stream beside
-      // build(k + 1) into the other buffer.  The build is limited by instruction issue and the argmin by HBM, so the
-      // pair overlaps instead of leaving each kernel's tail wave and the other's unused bandwidth idle.  When the
-      // second buffer does not fit, the tiles run one after the other as with the int64 tile.
       const size_t tile_elems = (size_t)rows * ld * elem_bytes / 8;   // TileBuf elements; ld is a multiple of 1024
-      bool overlap = narrow && e->tune_overlap != 0 && T > rows;
-      if (overlap && e->cost.ensure(2 * tile_elems, e->device, e->tune_compress != 0, e->stream) != cudaSuccess) {
-        cudaGetLastError();
-        overlap = false;
-      }
-      if (!overlap && e->cost.ensure(tile_elems, e->device, e->tune_compress != 0, e->stream) != cudaSuccess) {
+      if (e->cost.ensure(tile_elems, e->device, e->tune_compress != 0, e->stream) != cudaSuccess) {
         cudaGetLastError();
         return e->fail(PM_E_NOMEM, "pm_match: cannot allocate the cost tile; lower pm_cfg.cost_tile_bytes");
       }
-      cudaStream_t arg_stream = e->stream;
-      if (overlap) {   // the side stream starts after the results are initialised and the tables are bound
-        PM_CUDA(cudaEventRecord(e->ev_fork, e->stream));
-        PM_CUDA(cudaStreamWaitEvent(e->side, e->ev_fork, 0));
-        arg_stream = e->side;
-      }
-      uint32_t k = 0;
-      for (uint32_t t0 = 0; t0 < T; t0 += (uint32_t)rows, ++k) {
+      // One launch per tile (pm_build_argmin) wherever the 32-bit tile runs, unless PM_TUNE_PIPE=0 or a rows-per-CTA
+      // experiment (PM_TUNE_BUILD=5 / 6) asks for the separate build and argmin
+      const bool pipe = narrow && e->tune_pipe != 0 && e->tune_build != 5 && e->tune_build != 6;
+      long long* tile = e->cost.p;
+      for (uint32_t t0 = 0; t0 < T; t0 += (uint32_t)rows) {
         const uint32_t nt = (uint32_t)std::min<uint64_t>(rows, T - t0);
-        long long* tile = e->cost.p + (overlap ? (k & 1u) * tile_elems : 0);
-        if (overlap && k >= 2) PM_CUDA(cudaStreamWaitEvent(e->stream, e->ev_read[k & 1u], 0));   // argmin(k - 2) is done with it
-        {
-          Timer tm(e, &e->stats.ms_build, e->stream);
-          dim3 grid(blocks_for(ld, pm::kEvalCols), blocks_for(nt, pm::kEvalRows));
-          launch_build(e, p, bits_mode, fast, narrow, grid, t0, nt, w0, nw, tile, ld);
-          PM_LAUNCH_CHECK("pm_build_cost");
-          tm.stop();
+        if (pipe) {
+          // one launch that is both: its time counts in ms_build and in ms_argmin
+          Timer tb(e, &e->stats.ms_build, e->stream);
+          Timer ta(e, &e->stats.ms_argmin, e->stream);
+          launch_build_argmin(e, p, bits_mode, t0, nt, w0, nw, tile, ld);
+          PM_LAUNCH_CHECK("pm_build_argmin");
+          ta.stop();
+          tb.stop();
           ++e->stats.n_build_launches;
-        }
-        if (overlap) {
-          PM_CUDA(cudaEventRecord(e->ev_built, e->stream));
-          PM_CUDA(cudaStreamWaitEvent(e->side, e->ev_built, 0));
-        }
-        {
-          Timer tm(e, &e->stats.ms_argmin, arg_stream);
-          launch_argmin(e, arg_stream, narrow, tile, ld, nt, t0, w0, nw);
-          PM_LAUNCH_CHECK("pm_argmin");
-          tm.stop();
           ++e->stats.n_argmin_launches;
+        } else {
+          {
+            Timer tm(e, &e->stats.ms_build, e->stream);
+            dim3 grid(blocks_for(ld, pm::kEvalCols), blocks_for(nt, pm::kEvalRows));
+            launch_build(e, p, bits_mode, fast, narrow, grid, t0, nt, w0, nw, tile, ld);
+            PM_LAUNCH_CHECK("pm_build_cost");
+            tm.stop();
+            ++e->stats.n_build_launches;
+          }
+          {
+            Timer tm(e, &e->stats.ms_argmin, e->stream);
+            launch_argmin(e, e->stream, narrow, tile, ld, nt, t0, w0, nw);
+            PM_LAUNCH_CHECK("pm_argmin");
+            tm.stop();
+            ++e->stats.n_argmin_launches;
+          }
         }
-        if (overlap) PM_CUDA(cudaEventRecord(e->ev_read[k & 1u], e->side));
         ++e->stats.n_tiles;
         // algorithmic: 4 or 8 B per evaluation, the tile's element (padding columns not counted)
         e->stats.cost_bytes_written += (uint64_t)nt * nw * elem_bytes;
         e->stats.cost_bytes_read += (uint64_t)nt * nw * elem_bytes;
       }
-      // join: the resolution, the exchange and the caller's own work on the engine stream come after the last argmin
-      if (overlap) PM_CUDA(cudaStreamWaitEvent(e->stream, e->ev_read[(k - 1) & 1u], 0));
     }
     e->stats.evals = (uint64_t)T * nw;
   }

@@ -356,9 +356,20 @@ constexpr int kFastRows = 512;   // asks per CTA: the prologue (worker rows from
 // 4l .. 4l+3 of its warp's 128, so each row is one 16-byte store per thread, 512 B per warp and 4 KB per CTA,
 // contiguous.  Only for tables whose every price is below kNarrowInfeasible (pm_check_worker_ranges): at that price a
 // feasible worker could not be told from the sentinel, and at >= 2^31 the wide tile's signed order differs.
-template <int BITS, int ROWS = kFastRows, bool NARROW = false>
-__global__ void __launch_bounds__(kEvalThreads, 2)
-pm_build_cost_fast(EvalParams p, uint32_t t0, uint32_t nt, uint32_t w0, uint32_t nw, void* __restrict__ tile, size_t ld) {
+//
+// PIPE (pm_build_argmin, narrow only): the CTA also reduces what it wrote, band by band — see there.  `bo` is unused
+// otherwise.
+struct BandOut {
+  uint32_t band;                 // rows per band, even
+  uint32_t* first_ask;
+  long long* ask_best;
+  uint32_t* ask_count;
+};
+
+template <int BITS, int ROWS, bool NARROW, bool PIPE>
+__device__ __forceinline__ void build_fast(const EvalParams& p, uint32_t t0, uint32_t nt, uint32_t w0, uint32_t nw,
+                                           void* __restrict__ tile, size_t ld, const BandOut& bo) {
+  static_assert(!PIPE || NARROW, "the banded read-back folds the 32-bit tile");
   __shared__ FastStage<ROWS> s;
   const uint32_t r0 = blockIdx.y * ROWS;
   const uint32_t nrows = min(nt - r0, (uint32_t)ROWS);
@@ -392,9 +403,12 @@ pm_build_cost_fast(EvalParams p, uint32_t t0, uint32_t nt, uint32_t w0, uint32_t
   size_t row_stride = NARROW ? ld / 4 : ld / 2;   // in 16-byte units
   asm("" : "+l"(row_stride));           // held in registers: ptxas would otherwise re-derive it from `ld` every row
   const uint32_t sh = p.sign_shift;
+  uint32_t cm[kEvalWPT];                // PIPE: per column, the first feasible ask so far (kNone: none yet)
+#pragma unroll
+  for (int k = 0; k < kEvalWPT; ++k) cm[k] = kNone;
   // One row.  The ask's scalar thresholds are OR-ed into the first option's clauses before the further OR-options are
   // AND-ed in — fail = AND_o(u_o | s) = (AND_o u_o) | s — so a single-option row is one 7-term OR per worker.
-  auto emit = [&](const FastRow& q, uint4* dst) {
+  auto emit = [&](const FastRow& q, uint4* dst, uint32_t t) {
     uint32_t f[kEvalWPT], sc[kEvalWPT];
     eval_fast_first<kEvalWPT, BITS>(q, s.bits, w, p.bits, p.words, f);
 #pragma unroll
@@ -420,8 +434,11 @@ pm_build_cost_fast(EvalParams p, uint32_t t0, uint32_t nt, uint32_t w0, uint32_t
         o[2 * k] = b * dx[k] + gw[k];                                   // feasible: (price << 32) | worker
         o[2 * k + 1] = b * dy[k] + w[k].price;                          // infeasible: 0x7FFFFFFF_FFFFFFFF
       }
+      if (PIPE) cm[k] = min(cm[k], t | (uint32_t)((int32_t)f[k] >> sh));   // t when feasible, else kNone
     }
-    if (NARROW) {
+    if (PIPE) {
+      *dst = make_uint4(o[0], o[1], o[2], o[3]);                        // default policy: stays in L2 for the read-back
+    } else if (NARROW) {
       __stcs(dst, make_uint4(o[0], o[1], o[2], o[3]));
     } else {
       __stcs(dst, make_uint4(o[0], o[1], o[2], o[3]));
@@ -434,13 +451,83 @@ pm_build_cost_fast(EvalParams p, uint32_t t0, uint32_t nt, uint32_t w0, uint32_t
   // ahead, into registers the previous row has finished with, so no row is copied from one buffer to another.
   const FastRow* q = s.row;
   FastRow a = q[0];
-  for (uint32_t r = 0; r < nrows; r += 2, q += 2) {
-    const FastRow b = q[1];                   // in flight while row r is evaluated
-    emit(a, out);
-    a = q[2];                                 // in flight while row r + 1 is evaluated
-    if (r + 1 < nrows) emit(b, out + row_stride);
-    out += 2 * row_stride;
+  if constexpr (!PIPE) {
+    for (uint32_t r = 0; r < nrows; r += 2, q += 2) {
+      const FastRow b = q[1];                 // in flight while row r is evaluated
+      emit(a, out, 0u);
+      a = q[2];                               // in flight while row r + 1 is evaluated
+      if (r + 1 < nrows) emit(b, out + row_stride, 0u);
+      out += 2 * row_stride;
+    }
+  } else {
+    const uint32_t warp = threadIdx.x >> 5;
+    const uint32_t c0 = blockIdx.x * kEvalCols;                  // the CTA's first column
+    const uint4* band_in = reinterpret_cast<const uint4*>(static_cast<const uint32_t*>(tile) + (size_t)r0 * ld + c0) + lane;
+    for (uint32_t b0 = 0; b0 < nrows; b0 += bo.band) {
+      const uint32_t b1 = min(nrows, b0 + bo.band);
+      for (uint32_t r = b0; r < b1; r += 2, q += 2) {           // the band is even: pairs never straddle two bands
+        const FastRow b = q[1];
+        emit(a, out, t0 + r0 + r);
+        a = q[2];
+        if (r + 1 < b1) emit(b, out + row_stride, t0 + r0 + r + 1);
+        out += 2 * row_stride;
+      }
+      __syncthreads();                        // the band's stores are visible to every thread of the CTA
+      // A warp takes whole rows of the CTA's 1024 columns: load j holds columns j * 128 + 4 * lane .. + 3 (warp j's
+      // slice of the build), so a lane's columns arrive in increasing order and a strict "<" keeps the first of its
+      // least words, as pm_argmin<.., true> does.
+      for (uint32_t r = b0 + warp; r < b1; r += kEvalThreads / 32) {
+        const uint4* rowp = band_in + (size_t)r * row_stride;
+        uint4 v[kEvalCols / 128];
+#pragma unroll
+        for (int j = 0; j < kEvalCols / 128; ++j) v[j] = __ldcs(rowp + j * 32);   // read once: evict first
+        uint32_t bw = kNarrowInfeasible, bc = 0, cnt = 0;
+#pragma unroll
+        for (int j = 0; j < kEvalCols / 128; ++j) {
+          const uint32_t x[4] = {v[j].x, v[j].y, v[j].z, v[j].w};
+#pragma unroll
+          for (int c = 0; c < 4; ++c) {
+            cnt += (uint32_t)(x[c] != kNarrowInfeasible);
+            if (x[c] < bw) { bw = x[c]; bc = j * 128 + c; }
+          }
+        }
+        // the row's least word, then the least column holding it: the least packed (word << 32) | column
+        cnt = __reduce_add_sync(0xffffffffu, cnt);
+        const uint32_t wmin = __reduce_min_sync(0xffffffffu, bw);
+        const uint32_t cmin = __reduce_min_sync(0xffffffffu, bw == wmin ? bc + lane * 4u : kNone);
+        if (lane == 0 && cnt) {
+          const uint32_t t = t0 + r0 + r;
+          atomicMin(bo.ask_best + t, (long long)(((unsigned long long)wmin << 32) | (w0 + c0 + cmin)));
+          atomicAdd(bo.ask_count + t, cnt);
+        }
+      }
+    }
+#pragma unroll
+    for (int k = 0; k < kEvalWPT; ++k)
+      if (cm[k] != kNone && cbase + k < nw) atomicMin(bo.first_ask + w0 + cbase + k, cm[k]);
   }
+}
+
+template <int BITS, int ROWS = kFastRows, bool NARROW = false>
+__global__ void __launch_bounds__(kEvalThreads, 2)
+pm_build_cost_fast(EvalParams p, uint32_t t0, uint32_t nt, uint32_t w0, uint32_t nw, void* __restrict__ tile, size_t ld) {
+  build_fast<BITS, ROWS, NARROW, false>(p, t0, nt, w0, nw, tile, ld, BandOut{});
+}
+
+// ------------------------------------------------------------------ build + argmin, one kernel
+// pm_build_cost_fast<BITS, kFastRows, true> followed by pm_argmin<.., true>, without the second pass over HBM.  The CTA
+// walks its 512 rows in bands of bo.band rows: it evaluates and stores a band exactly as the build does (but with the
+// default store policy, so the lines stay in L2), waits at a barrier, and reads the band straight back with
+// evict-first loads while the lines are still in L2.  The tile bytes written and not yet read are at most
+// (resident CTAs) x band x 4 KB — 17 MB at 264 CTAs and 16 rows — well inside the 50 MB L2; the tile itself still
+// streams through HBM as the stores write back.  The outputs are pm_argmin's, bit for bit: per row and CTA one
+// (least word, least column) from three warp reductions, merged with atomicMin / atomicAdd; per column the first
+// feasible ask from the sign bit the build already holds, flushed once per CTA.
+template <int BITS>
+__global__ void __launch_bounds__(kEvalThreads, 2)
+pm_build_argmin(EvalParams p, uint32_t t0, uint32_t nt, uint32_t w0, uint32_t nw, uint32_t* __restrict__ tile, size_t ld,
+                BandOut bo) {
+  build_fast<BITS, kFastRows, true, true>(p, t0, nt, w0, nw, tile, ld, bo);
 }
 
 // Worker-major acceptance: bit r of nacc[w] is set when pattern row r rejects worker w's model (row 0 never does).
