@@ -251,9 +251,26 @@ enum pm_path {
   PM_PATH_MATERIALIZED = 0,      /* build a cost tile in HBM (the 32-bit cost word when every price is
                                     below 0x7FFFFFFF, else the int64 packed cost), then argmin over it */
   PM_PATH_FUSED        = 1u << 8,/* evaluate + reduce on chip, matrix never written   */
-  PM_NO_ASK_STATS      = 1u << 9 /* with PM_PATH_FUSED: skip ask_best / ask_count (the reference modes only
+  PM_NO_ASK_STATS      = 1u << 9,/* with PM_PATH_FUSED: skip ask_best / ask_count (the reference modes only
                                     need the per-worker first feasible ask); they read INF / 0 then      */
+  PM_INCREMENTAL       = 1u << 10 /* reuse the engine's stored per-worker first feasible ask: re-evaluate only the worker
+                                    rows written since the last evaluation on this engine, or everything when there is no
+                                    valid stored evaluation or more rows changed than the cutoff (PM_TUNE_INCR at
+                                    pm_create).  Every array pm_fetch_result returns equals the same call's without the
+                                    flag (ask_best = PM_COST_INF, ask_count = 0).  Valid with PM_PATH_FUSED |
+                                    PM_NO_ASK_STATS and a reference mode only (else PM_E_INVALID); PM_E_UNSUPPORTED on a
+                                    sharded engine or one with a communicator attached.  See "Incremental passes" below */
 };
+
+/* Incremental passes (PM_INCREMENTAL).  Every full evaluation of an unsharded engine, with the flag or without, keeps
+ * a copy of its per-worker result.  A row becomes "written" through pm_upsert_workers (the range), pm_update_workers
+ * and pm_set_flags (the in-range indices, each once) and pm_resize_workers (the rows past the old end).
+ * pm_set_worker_locations, pm_set_worker_addr_rank and pm_set_worker_reputation write nothing the predicate reads.
+ * pm_set_asks, pm_set_model_table, pm_set_worker_count, pm_set_shard, pm_attach_comm and a pass that fails discard the
+ * stored evaluation.  Without the flag pm_match evaluates every pair as before.  pm_stats under the flag:
+ *   evals    pair evaluations executed: T x W on a full evaluation, the kernel's own count on an incremental one,
+ *            0 when no row changed;
+ *   n_tiles  worker rows re-evaluated (W on a full evaluation).                                                      */
 
 typedef struct pm_stats {
   uint64_t evals;            /* predicate evaluations executed on the device        */

@@ -48,6 +48,7 @@ PM_CFG_TIMING = 1 << 0
 
 PM_MODE_FIRST_FIT, PM_MODE_PROXIMITY, PM_MODE_AUCTION, PM_MODE_PROXIMITY_MERGE = 0, 1, 2, 3
 PM_PATH_MATERIALIZED, PM_PATH_FUSED, PM_NO_ASK_STATS = 0, 1 << 8, 1 << 9
+PM_INCREMENTAL = 1 << 10   # re-evaluate only the worker rows written since the stored evaluation (prime_match.h)
 
 PM_BUF_WORKER_FIRST_ASK, PM_BUF_ASK_BEST, PM_BUF_ASK_COUNT = 0, 1, 2
 

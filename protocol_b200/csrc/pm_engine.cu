@@ -306,6 +306,50 @@ struct pm_engine {
   DevBuf<uint32_t> first_ask, ask_count;
   DevBuf<long long> ask_best;
 
+  // The stored evaluation of PM_INCREMENTAL: the per-worker first feasible ask of the last evaluation, in its own
+  // buffer (first_ask is the resolution's working copy: the sweeps and the auction overwrite it), and the worker rows
+  // written since then.  Rows are tracked on the host, where their indices arrive: a mark per row, the list of marked
+  // rows, and `dirty_over` once more rows changed than an incremental pass would take (tune_incr).
+  DevBuf<uint32_t> eval_first;
+  bool eval_valid = false;
+  std::vector<uint8_t> dirty_mark;      // [rows of the stored evaluation, grown with the table]; set <=> in dirty_rows
+  std::vector<uint32_t> dirty_rows;
+  bool dirty_over = false;
+  bool workers_base = false;            // workers_small / prices_narrow hold for every row outside dirty_rows
+  bool nacc_base = false;               // nacc holds every row outside dirty_rows (model table unchanged)
+  uint32_t tune_incr = 1u << 18;        // PM_TUNE_INCR: most dirty rows an incremental pass re-evaluates (DESIGN §5)
+  PinBuf<uint32_t> h_dirty;
+  DevBuf<uint32_t> dirty_dev;
+  DevBuf<unsigned long long> incr_evals;
+  bool incr_evals_pending = false;      // stats.evals of the incremental pass arrives with the pass's one sync
+
+  void clear_dirty() {
+    for (uint32_t i : dirty_rows) dirty_mark[i] = 0;
+    dirty_rows.clear();
+    dirty_over = false;
+  }
+  void invalidate_eval() {
+    clear_dirty();
+    eval_valid = false;
+    workers_base = nacc_base = false;
+  }
+  void mark_dirty(uint32_t i) {
+    if (!eval_valid || dirty_over || i >= dirty_mark.size() || dirty_mark[i]) return;
+    dirty_mark[i] = 1;
+    dirty_rows.push_back(i);
+    if (dirty_rows.size() > tune_incr) mark_all_dirty();
+  }
+  void mark_range_dirty(uint32_t first, uint32_t n) {
+    if (!eval_valid || dirty_over) return;
+    if (n > tune_incr) { mark_all_dirty(); return; }
+    for (uint32_t i = 0; i < n; ++i) mark_dirty(first + i);
+  }
+  void mark_all_dirty() {   // the next pass evaluates everything
+    if (!eval_valid) return;
+    clear_dirty();
+    dirty_over = true;
+  }
+
   // resolution
   DevBuf<uint32_t> keys, keys_sorted, iota, order, hist, seg_start, ngroups, group_base;
   DevBuf<uint32_t> base_len, xhead, xnext, xcount, popped, counters;  // counters: [0]=any_bad [1]=n_bumped
@@ -520,6 +564,7 @@ int pm_create(const pm_cfg* cfg, pm_engine** out) try {
   if (const char* t = std::getenv("PM_TUNE_AUCTION_POOL")) std::sscanf(t, "%d,%d", &e->tune_auc_good, &e->tune_auc_extra);   // pool fill of a class walk
   if (const char* t = std::getenv("PM_TUNE_PROX")) e->tune_prox = std::atoi(t);   // 0: all-SM cooperative sweep; 2: single-CTA sweep; 1: latitude-banded single-CTA sweep (experimental)
   if (const char* t = std::getenv("PM_TUNE_COMPRESS")) e->tune_compress = std::atoi(t);
+  if (const char* t = std::getenv("PM_TUNE_INCR")) e->tune_incr = (uint32_t)std::strtoul(t, nullptr, 10);   // 0: always full
   if (const char* t = std::getenv("PM_TUNE_PIPE")) {   // other values keep the default band
     const int v = std::atoi(t);
     if (v == 0 || v == 8 || v == 16 || v == 32 || v == 64) e->tune_pipe = v;
@@ -553,6 +598,7 @@ void pm_destroy(pm_engine* e) {
   e->scratch_idx.release(); e->scratch_flags.release();
   e->upd_a.release(); e->upd_b.release(); e->upd_lat.release(); e->upd_lon.release();
   e->cost.release(); e->first_ask.release(); e->ask_count.release(); e->ask_best.release();
+  e->eval_first.release(); e->h_dirty.release(); e->dirty_dev.release(); e->incr_evals.release();
   e->keys.release(); e->keys_sorted.release(); e->iota.release(); e->order.release();
   e->hist.release(); e->seg_start.release(); e->ngroups.release(); e->group_base.release();
   e->base_len.release(); e->xhead.release(); e->xnext.release(); e->xcount.release();
@@ -593,6 +639,7 @@ int pm_set_asks(pm_engine* e, const pm_ask* asks, uint32_t n_asks, const pm_gpu_
   if (!e) return PM_E_INVALID;
   std::lock_guard<std::mutex> lk(e->mu);
   ++e->table_version;
+  e->invalidate_eval();
   if ((n_asks && !asks) || (n_opts && !opts)) return e->fail(PM_E_INVALID, "pm_set_asks: null table");
   if (n_asks >= (1u << 30)) return e->fail(PM_E_INVALID, "pm_set_asks: too many asks");
   PM_CUDA(cudaSetDevice(e->device));
@@ -653,6 +700,7 @@ int pm_set_model_table(pm_engine* e, const uint32_t* bits, uint32_t n_patterns, 
   if (!e) return PM_E_INVALID;
   std::lock_guard<std::mutex> lk(e->mu);
   ++e->table_version;
+  e->invalidate_eval();
   if (words == 0) words = 1;
   if (n_patterns && !bits) return e->fail(PM_E_INVALID, "pm_set_model_table: null table");
   if ((uint64_t)words * 32 < n_models) return e->fail(PM_E_INVALID, "pm_set_model_table: words too small");
@@ -692,6 +740,7 @@ int pm_set_worker_count(pm_engine* e, uint32_t n_workers) try {
   if (!e) return PM_E_INVALID;
   std::lock_guard<std::mutex> lk(e->mu);
   ++e->table_version;
+  e->invalidate_eval();
   PM_CUDA(cudaSetDevice(e->device));
   if (n_workers > e->wa.n || !e->wa.p) {
     // grow, preserving nothing: callers upsert after (re)sizing
@@ -718,6 +767,7 @@ int pm_upsert_workers(pm_engine* e, const pm_worker_a* a, const pm_worker_b* b, 
   if (!e->have_workers) return e->fail(PM_E_STATE, "pm_upsert_workers: call pm_set_worker_count first");
   if ((uint64_t)first + n > e->n_workers) return e->fail(PM_E_INVALID, "pm_upsert_workers: range out of bounds");
   if (n && (!a || !b)) return e->fail(PM_E_INVALID, "pm_upsert_workers: null plane");
+  e->mark_range_dirty(first, n);
   PM_CUDA(cudaSetDevice(e->device));
   if (n) {
     PM_CUDA(cudaMemcpyAsync(e->wa.p + first, a, (size_t)n * 16, cudaMemcpyHostToDevice, e->stream));
@@ -767,6 +817,7 @@ int pm_set_flags(pm_engine* e, const uint32_t* idx, const uint32_t* flags, uint3
   if (!e->have_workers) return e->fail(PM_E_STATE, "pm_set_flags: no worker table");
   if (n == 0) return PM_OK;
   if (!idx || !flags) return e->fail(PM_E_INVALID, "pm_set_flags: null");
+  for (uint32_t i = 0; i < n; ++i) e->mark_dirty(idx[i]);   // out-of-range indices are skipped, as the scatter does
   PM_CUDA(cudaSetDevice(e->device));
   PM_CUDA(e->scratch_idx.ensure(n));
   PM_CUDA(e->scratch_flags.ensure(n));
@@ -787,6 +838,20 @@ int pm_resize_workers(pm_engine* e, uint32_t n_workers) try {
   ++e->table_version;
   PM_CUDA(cudaSetDevice(e->device));
   const size_t keep = e->have_workers ? e->n_workers : 0;
+  if (e->eval_valid) {
+    // the stored evaluation follows the table: kept rows keep their entries, rows past the old end are dirty
+    PM_CUDA(e->eval_first.grow_keep(std::max<uint32_t>(n_workers, 1), keep, e->stream));
+    if (n_workers < keep) {
+      size_t j = 0;
+      for (uint32_t i : e->dirty_rows) {
+        if (i < n_workers) e->dirty_rows[j++] = i;
+        else e->dirty_mark[i] = 0;
+      }
+      e->dirty_rows.resize(j);
+    }
+    e->dirty_mark.resize(n_workers, 0);
+    if (n_workers > keep) e->mark_range_dirty((uint32_t)keep, n_workers - (uint32_t)keep);
+  }
   PM_CUDA(e->wa.grow_keep(std::max<uint32_t>(n_workers, 1), keep, e->stream));
   PM_CUDA(e->wb.grow_keep(std::max<uint32_t>(n_workers, 1), keep, e->stream));
   if (e->have_loc) {
@@ -821,6 +886,7 @@ int pm_update_workers(pm_engine* e, const uint32_t* idx, const pm_worker_a* a, c
   if (n == 0) return PM_OK;
   if (!idx || !a || !b || ((lat == nullptr) != (lon == nullptr))) return e->fail(PM_E_INVALID, "pm_update_workers: null");
   ++e->table_version;
+  for (uint32_t i = 0; i < n; ++i) e->mark_dirty(idx[i]);   // out-of-range indices are skipped, as the scatter does
   PM_CUDA(cudaSetDevice(e->device));
   PM_CUDA(e->scratch_idx.ensure(n)); PM_CUDA(e->upd_a.ensure(n)); PM_CUDA(e->upd_b.ensure(n));
   PM_CUDA(cudaMemcpyAsync(e->scratch_idx.p, idx, (size_t)n * 4, cudaMemcpyHostToDevice, e->stream));
@@ -859,14 +925,22 @@ int pm_create_sibling(const pm_engine* e, pm_engine** out) try {
 } catch (...) { return pm_guard_rc(); }
 
 // ------------------------------------------------------------------ evaluation
-// Fast predicate only when both tables fit its operand limits; decided per match.
-static int decide_fast(pm_engine* e, bool* fast) {
+// Fast predicate only when both tables fit its operand limits; decided per match.  `rows` (an incremental pass, the
+// device list of the n_rows rows written since the last evaluation): when every other row passed the last check, only
+// these are checked, starting from that check's flags.
+static int decide_fast(pm_engine* e, bool* fast, const uint32_t* rows = nullptr, uint32_t n_rows = 0) {
   *fast = false;
   if (e->tune_generic || !e->asks_small) return PM_OK;
   if (!e->workers_checked) {
-    const uint32_t one[2] = {1, 1};
+    const bool partial = rows && e->workers_base;
+    const uint32_t one[2] = {partial ? (uint32_t)e->workers_small : 1u, partial ? (uint32_t)e->prices_narrow : 1u};
     PM_CUDA(cudaMemcpyAsync(e->counters.p + 2, one, 8, cudaMemcpyHostToDevice, e->stream));
-    if (e->n_workers) {
+    if (partial) {
+      if (n_rows) {
+        pm::pm_check_worker_rows<<<blocks_for(n_rows, 256), 256, 0, e->stream>>>(e->wa.p, e->wb.p, rows, n_rows, e->counters.p + 2);
+        PM_LAUNCH_CHECK("pm_check_worker_rows");
+      }
+    } else if (e->n_workers) {
       pm::pm_check_worker_ranges<<<blocks_for(e->n_workers, 256), 256, 0, e->stream>>>(e->wa.p, e->wb.p, e->n_workers, e->counters.p + 2);
       PM_LAUNCH_CHECK("pm_check_worker_ranges");
     }
@@ -897,7 +971,16 @@ static int bind_rows(pm_engine* e, bool wm) {
 // (row, worker) pair, build kernel at 0.64 of the copy peak with 100k strings): turn the table around.  With at most 30
 // patterns a worker's acceptance over ALL of them is one word, computed once per table change; the kernels then run
 // their one-word form (BITS == 2) with the roles of row and worker swapped (EvalParams::nacc).  Fast predicate only.
-static int worker_major(pm_engine* e, pm::EvalParams* p, int* bits_mode) {
+// `rows` as in decide_fast: an incremental pass recomputes only the listed rows' words when the others still hold.
+static int worker_major(pm_engine* e, pm::EvalParams* p, int* bits_mode, const uint32_t* rows = nullptr, uint32_t n_rows = 0) {
+  if (!e->nacc_valid && rows && e->nacc_base) {
+    PM_CUDA(e->nacc.grow_keep(std::max<uint32_t>(e->n_workers, 1), e->nacc.n, e->stream));   // new rows are listed
+    if (n_rows) {
+      pm::pm_worker_nacc_rows<<<blocks_for(n_rows, 256), 256, 0, e->stream>>>(e->wa.p, e->bits.p, e->words, p->n_bits_rows, rows, n_rows, e->nacc.p);
+      PM_LAUNCH_CHECK("pm_worker_nacc_rows");
+    }
+    e->nacc_valid = true;
+  }
   if (!e->nacc_valid) {
     PM_CUDA(e->nacc.ensure(std::max<uint32_t>(e->n_workers, 1)));
     PM_CUDA(e->bits_wm.ensure(32));
@@ -960,12 +1043,13 @@ static void launch_build(pm_engine* e, const pm::EvalParams& p, int bits_mode, b
 static void launch_fused(pm_engine* e, const pm::EvalParams& p, int bits_mode, bool fast, bool stats, dim3 grid,
                          uint32_t t0, uint32_t nt, uint32_t w0, uint32_t nw) {
 #define PM_FUSED_CASE(B, F, S) pm::pm_fused_eval<B, F, S><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, t0, nt, w0, nw, e->first_ask.p, e->ask_best.p, e->ask_count.p)
-  if (fast && !stats && bits_mode == 2) { PM_FUSED_CASE(2, true, false); return; }   // the lean common case
-  if (fast) {
-    if (bits_mode == 2) PM_FUSED_CASE(2, true, true); else if (bits_mode == 1) PM_FUSED_CASE(1, true, true); else PM_FUSED_CASE(0, true, true);
-  } else {
-    if (bits_mode == 2) PM_FUSED_CASE(2, false, true); else if (bits_mode == 1) PM_FUSED_CASE(1, false, true); else PM_FUSED_CASE(0, false, true);
-  }
+  // !stats (PM_NO_ASK_STATS) skips the per-ask outputs in every variant: they read INF / 0, as an incremental pass's do
+#define PM_FUSED_BITS(F, S) { if (bits_mode == 2) PM_FUSED_CASE(2, F, S); else if (bits_mode == 1) PM_FUSED_CASE(1, F, S); else PM_FUSED_CASE(0, F, S); }
+  if (fast && stats) PM_FUSED_BITS(true, true)
+  else if (fast) PM_FUSED_BITS(true, false)
+  else if (stats) PM_FUSED_BITS(false, true)
+  else PM_FUSED_BITS(false, false)
+#undef PM_FUSED_BITS
 #undef PM_FUSED_CASE
 }
 
@@ -1010,6 +1094,59 @@ static void launch_argmin(pm_engine* e, cudaStream_t st, bool narrow, const long
 #undef PM_ARGMIN_CASE
 }
 
+// The incremental evaluation: the stored per-worker first feasible ask is rewritten for the rows written since it was
+// taken (pm_first_ask_rows), then copied to first_ask, the resolution's working copy.  Same predicate variant as the
+// full pass would pick; the O(W) preludes (operand-range check, worker-major acceptance words) cover the listed rows.
+static int eval_incremental(pm_engine* e) {
+  const uint32_t W = e->n_workers, T = e->n_asks;
+  const uint32_t k = (uint32_t)e->dirty_rows.size();
+  e->stats.n_tiles = k;
+  if (k) {
+    PM_CUDA(e->h_dirty.ensure(k));
+    std::memcpy(e->h_dirty.p, e->dirty_rows.data(), (size_t)k * 4);
+    PM_CUDA(e->dirty_dev.ensure(k));
+    PM_CUDA(cudaMemcpyAsync(e->dirty_dev.p, e->h_dirty.p, (size_t)k * 4, cudaMemcpyHostToDevice, e->stream));
+    PM_CUDA(e->incr_evals.ensure(1));
+    PM_CUDA(cudaMemsetAsync(e->incr_evals.p, 0, 8, e->stream));
+    pm::EvalParams p = eval_params(e);
+    int bits_mode = ((uint64_t)p.n_bits_rows * p.words <= (uint64_t)pm::kBitsCap) ? (p.words == 1 ? 2 : 1) : 0;
+    bool fast = false;
+    {
+      const int rc = decide_fast(e, &fast, e->dirty_dev.p, k);
+      if (rc != PM_OK) return rc;
+    }
+    const bool wm = fast && bits_mode == 0 && p.n_bits_rows <= 31u && e->tune_build != 7;   // as the full pass
+    if (wm) {
+      const int rc = worker_major(e, &p, &bits_mode, e->dirty_dev.p, k);
+      if (rc != PM_OK) return rc;
+    }
+    Timer tm(e, &e->stats.ms_fused, e->stream);
+    pm::pm_scatter_value<<<blocks_for(k, 256), 256, 0, e->stream>>>(e->eval_first.p, e->dirty_dev.p, k, pm::kNone);
+    PM_LAUNCH_CHECK("pm_scatter_value");
+    // about four CTAs per SM in all: few listed workers split the asks into more chunks
+    const uint32_t gx = blocks_for(k, pm::kEvalCols);
+    const uint32_t steps = blocks_for(T, pm::kEvalRows);
+    const uint32_t want_y = std::max(1u, std::min(steps, blocks_for(4u * e->sms, gx)));
+    const uint32_t chunk = blocks_for(steps, want_y) * pm::kEvalRows;
+    const dim3 grid(gx, blocks_for(T, chunk));
+#define PM_ROWS_CASE(B, F) pm::pm_first_ask_rows<B, F><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, e->dirty_dev.p, k, chunk, e->eval_first.p, e->incr_evals.p)
+    if (fast) {
+      if (bits_mode == 2) PM_ROWS_CASE(2, true); else if (bits_mode == 1) PM_ROWS_CASE(1, true); else PM_ROWS_CASE(0, true);
+    } else {
+      if (bits_mode == 2) PM_ROWS_CASE(2, false); else if (bits_mode == 1) PM_ROWS_CASE(1, false); else PM_ROWS_CASE(0, false);
+    }
+#undef PM_ROWS_CASE
+    PM_LAUNCH_CHECK("pm_first_ask_rows");
+    tm.stop();
+    // read back with the pass's one host synchronisation (match_finish_locked)
+    PM_CUDA(cudaMemcpyAsync(e->h_scalars.p + 30, e->incr_evals.p, 8, cudaMemcpyDeviceToHost, e->stream));
+    e->incr_evals_pending = true;
+  }
+  PM_CUDA(cudaMemcpyAsync(e->first_ask.p, e->eval_first.p, (size_t)W * 4, cudaMemcpyDeviceToDevice, e->stream));
+  e->clear_dirty();
+  return PM_OK;
+}
+
 static int match_local_locked(pm_engine* e, uint32_t mode) {
   if (!e->have_workers || !e->have_asks) return e->fail(PM_E_STATE, "pm_match: worker and ask tables must be set first");
   if (e->max_pattern_row > e->n_patterns || (e->max_pattern_row && !e->have_bits))
@@ -1035,22 +1172,33 @@ static int match_local_locked(pm_engine* e, uint32_t mode) {
   }
 
   e->stats = pm_stats{};
+  e->incr_evals_pending = false;
   e->ev_pending.clear();
   e->ev_used = 0;
   const bool timing = (e->cfg.flags & PM_CFG_TIMING) != 0;
   if (timing) PM_CUDA(cudaEventRecord(e->ev0, e->stream));
 
+  // PM_INCREMENTAL: re-evaluate the rows written since the stored evaluation when there is one and few rows changed.
+  // Only an engine that evaluates the whole table keeps a stored evaluation (a shard's first_ask holds its range only).
+  const bool keep_eval = !e->comm && w0 == 0 && nw == W;
+  const bool incr = (mode & PM_INCREMENTAL) != 0;
+  const bool use_incr = incr && keep_eval && e->eval_valid && !e->dirty_over && e->tune_incr != 0 &&
+                        e->dirty_rows.size() <= e->tune_incr && T && W;
+
   PM_CUDA(e->first_ask.ensure(W));
   PM_CUDA(e->ask_best.ensure(T));
   PM_CUDA(e->ask_count.ensure(T));
-  PM_CUDA(cudaMemsetAsync(e->first_ask.p, 0xFF, (size_t)std::max<uint32_t>(W, 1) * 4, e->stream));
+  if (!use_incr) PM_CUDA(cudaMemsetAsync(e->first_ask.p, 0xFF, (size_t)std::max<uint32_t>(W, 1) * 4, e->stream));
   PM_CUDA(cudaMemsetAsync(e->ask_count.p, 0, (size_t)std::max<uint32_t>(T, 1) * 4, e->stream));
   if (T) {
     pm::pm_fill_i64<<<std::min(blocks_for(T, 256), 8u * e->sms), 256, 0, e->stream>>>(e->ask_best.p, pm::kInf, T);
     PM_LAUNCH_CHECK("pm_fill_i64");
   }
 
-  if (T && nw) {
+  if (use_incr) {
+    const int rc = eval_incremental(e);
+    if (rc != PM_OK) return rc;
+  } else if (T && nw) {
     pm::EvalParams p = eval_params(e);
     int bits_mode = ((uint64_t)p.n_bits_rows * p.words <= (uint64_t)pm::kBitsCap) ? (p.words == 1 ? 2 : 1) : 0;
     bool fast = false;
@@ -1138,6 +1286,20 @@ static int match_local_locked(pm_engine* e, uint32_t mode) {
     }
     e->stats.evals = (uint64_t)T * nw;
   }
+  if (!use_incr) {
+    if (keep_eval) {   // every full evaluation refreshes the stored one: one 4 B-per-worker copy
+      PM_CUDA(e->eval_first.ensure(std::max<uint32_t>(W, 1)));
+      PM_CUDA(cudaMemcpyAsync(e->eval_first.p, e->first_ask.p, (size_t)W * 4, cudaMemcpyDeviceToDevice, e->stream));
+      e->clear_dirty();
+      e->dirty_mark.resize(W, 0);   // every mark is clear after clear_dirty
+      e->eval_valid = true;
+    } else {
+      e->invalidate_eval();
+    }
+    if (incr) e->stats.n_tiles = W;   // rows re-evaluated
+  }
+  e->workers_base = e->eval_valid && e->workers_checked;
+  e->nacc_base = e->eval_valid && e->nacc_valid;
   e->local_done = true;
   e->matched = false;
   return PM_OK;
@@ -1323,7 +1485,11 @@ static int match_finish_locked(pm_engine* e, uint32_t mode) {
   e->n_groups = e->h_scalars.p[8];
   e->n_assigned = e->h_scalars.p[9];
   e->stats.n_bumped = e->h_scalars.p[10];
-  if (prox_grid_ran) {   // cooperative proximity sweep: seed-parallel batches, groups formed in them, groups formed one at a time
+  if (e->incr_evals_pending) {
+    std::memcpy(&e->stats.evals, e->h_scalars.p + 30, 8);
+    e->incr_evals_pending = false;
+  }
+  if (prox_grid_ran && !(mode & PM_INCREMENTAL)) {   // with PM_INCREMENTAL n_tiles keeps the rows re-evaluated   // cooperative proximity sweep: seed-parallel batches, groups formed in them, groups formed one at a time
     e->stats.n_tiles = e->h_scalars.p[24];
     e->stats.n_rounds = e->h_scalars.p[25];
     e->stats.n_build_launches = e->h_scalars.p[26];
@@ -1685,28 +1851,49 @@ static int exchange_locked(pm_engine* e) {
   return PM_OK;
 }
 
+// PM_INCREMENTAL: a reference mode on the fused lean path, on an engine that evaluates the whole table
+static int check_incremental(pm_engine* e, uint32_t mode) {
+  if (!(mode & PM_INCREMENTAL)) return PM_OK;
+  if ((mode & 0xFFu) == PM_MODE_AUCTION) return e->fail(PM_E_INVALID, "pm_match: PM_INCREMENTAL is for the reference modes, not the auction");
+  if ((mode & (PM_PATH_FUSED | PM_NO_ASK_STATS)) != (PM_PATH_FUSED | PM_NO_ASK_STATS))
+    return e->fail(PM_E_INVALID, "pm_match: PM_INCREMENTAL needs PM_PATH_FUSED | PM_NO_ASK_STATS");
+  if (e->cfg.shard_first || e->cfg.shard_count || e->comm)
+    return e->fail(PM_E_UNSUPPORTED, "pm_match: PM_INCREMENTAL is single-GPU (no shard, no communicator)");
+  return PM_OK;
+}
+
+// A pass that fails may have consumed the rows written since the stored evaluation: nothing of it is trusted again.
+static int invalidate_on_failure(pm_engine* e, int rc) {
+  if (rc != PM_OK) e->invalidate_eval();
+  return rc;
+}
+
 int pm_match_local(pm_engine* e, uint32_t mode) try {
   if (!e) return PM_E_INVALID;
   std::lock_guard<std::mutex> lk(e->mu);
   if ((mode & 0xFFu) == PM_MODE_AUCTION) return e->fail(PM_E_UNSUPPORTED, "pm_match_local: auction mode is single-GPU (use pm_match)");
-  return match_local_locked(e, mode);
+  const int rc = check_incremental(e, mode);
+  if (rc != PM_OK) return rc;
+  return invalidate_on_failure(e, match_local_locked(e, mode));
 } catch (...) { return pm_guard_rc(); }
 int pm_match_finish(pm_engine* e, uint32_t mode) try {
   if (!e) return PM_E_INVALID;
   std::lock_guard<std::mutex> lk(e->mu);
-  return match_finish_locked(e, mode);
+  return invalidate_on_failure(e, match_finish_locked(e, mode));
 } catch (...) { return pm_guard_rc(); }
 int pm_match(pm_engine* e, uint32_t mode) try {
   if (!e) return PM_E_INVALID;
   std::lock_guard<std::mutex> lk(e->mu);
-  if ((mode & 0xFFu) == PM_MODE_AUCTION) return match_auction_locked(e);
-  int rc = match_local_locked(e, mode);
+  int rc = check_incremental(e, mode);
   if (rc != PM_OK) return rc;
+  if ((mode & 0xFFu) == PM_MODE_AUCTION) return match_auction_locked(e);
+  rc = match_local_locked(e, mode);
+  if (rc != PM_OK) return invalidate_on_failure(e, rc);
   if (e->comm && e->comm->n_ranks > 1) {
     rc = exchange_locked(e);
-    if (rc != PM_OK) return rc;
+    if (rc != PM_OK) return invalidate_on_failure(e, rc);
   }
-  return match_finish_locked(e, mode);
+  return invalidate_on_failure(e, match_finish_locked(e, mode));
 } catch (...) { return pm_guard_rc(); }
 
 int pm_set_shard(pm_engine* e, uint32_t first, uint32_t count) try {
@@ -1714,6 +1901,7 @@ int pm_set_shard(pm_engine* e, uint32_t first, uint32_t count) try {
   std::lock_guard<std::mutex> lk(e->mu);
   e->cfg.shard_first = first;
   e->cfg.shard_count = count;
+  e->invalidate_eval();
   e->matched = e->local_done = false;
   return PM_OK;
 } catch (...) { return pm_guard_rc(); }
@@ -1765,6 +1953,7 @@ int pm_attach_comm(pm_engine* e, pm_comm* c) try {
   std::lock_guard<std::mutex> lk(e->mu);
   if (c && c->device != e->device) return e->fail(PM_E_INVALID, "pm_attach_comm: communicator and engine are on different devices");
   e->comm = c;
+  e->invalidate_eval();
   e->matched = e->local_done = false;
   return PM_OK;
 } catch (...) { return pm_guard_rc(); }

@@ -531,17 +531,29 @@ pm_build_argmin(EvalParams p, uint32_t t0, uint32_t nt, uint32_t w0, uint32_t nw
 }
 
 // Worker-major acceptance: bit r of nacc[w] is set when pattern row r rejects worker w's model (row 0 never does).
-__global__ void pm_worker_nacc(const uint4* __restrict__ wa, const uint32_t* __restrict__ bits, uint32_t words, uint32_t n_rows,
-                               uint32_t n, uint32_t* __restrict__ nacc) {
-  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const uint4 a = wa[i];
+__device__ __forceinline__ uint32_t worker_nacc(const uint4& a, const uint32_t* __restrict__ bits, uint32_t words,
+                                                uint32_t n_rows) {
   const uint32_t mid = (a.w & PM_W_HAS_GPU_MODEL) ? a.z : 0u;
   const uint32_t mword = mid / kModelsPerWord, mmask = 1u << (mid % kModelsPerWord);
   uint32_t rej = 0;
   for (uint32_t r = 1; r < n_rows; ++r)
     if (!(__ldg(bits + (size_t)r * words + mword) & mmask)) rej |= 1u << r;
-  nacc[i] = rej;
+  return rej;
+}
+__global__ void pm_worker_nacc(const uint4* __restrict__ wa, const uint32_t* __restrict__ bits, uint32_t words, uint32_t n_rows,
+                               uint32_t n, uint32_t* __restrict__ nacc) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  nacc[i] = worker_nacc(wa[i], bits, words, n_rows);
+}
+// ... for the listed rows only (an incremental pass: the other rows' words are still those of the table in force)
+__global__ void pm_worker_nacc_rows(const uint4* __restrict__ wa, const uint32_t* __restrict__ bits, uint32_t words,
+                                    uint32_t n_rows, const uint32_t* __restrict__ rows, uint32_t n,
+                                    uint32_t* __restrict__ nacc) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const uint32_t w = rows[i];
+  nacc[w] = worker_nacc(wa[w], bits, words, n_rows);
 }
 
 // `wp` of every FastRow: the first option's acceptance WORD when rows are one word wide, else its pattern row.
@@ -755,6 +767,94 @@ pm_fused_eval(EvalParams p, uint32_t t0, uint32_t nt, uint32_t w0, uint32_t nw,
   }
 }
 
+// ------------------------------------------------------------------ incremental: first feasible ask of listed rows
+// pm_fused_eval's per-worker output (the lowest ask t with feasible(t, w)) for the workers named in `rows` only: an
+// incremental pass re-evaluates the rows written since the stored evaluation and keeps the others.  Same predicate
+// code as pm_fused_eval (for_each_staged_row, eval_row_fast / eval_row / eval_row_global, every BITS form, the
+// worker-major `nacc` word), so the values are the fused pass's by construction.
+//
+// grid = (ceil(n / 1024), chunks): a CTA gathers 1024 listed workers into registers (4 per thread, as the fused
+// kernel holds its stripe) and walks its chunk of `chunk` asks in steps of kEvalRows staged rows.  Asks are in
+// priority order, so a hit is final for the chunk; before each step the CTA stops once every one of its workers has a
+// hit of its own, or a hit below the step's first row in `first_ask` (published by the CTAs of earlier chunks with
+// atomicMin), or is not a candidate at all (no ask can accept it).  `first_ask[rows[i]]` must hold kNone on entry.
+// `evals` gains the pairs evaluated: rows walked x listed workers of the CTA.
+__device__ __forceinline__ void gather_workers(const EvalParams& p, const uint32_t* __restrict__ rows, uint32_t n,
+                                               uint32_t c, WorkerReg (&w)[kEvalWPT], uint32_t (&gw)[kEvalWPT]) {
+#pragma unroll
+  for (int k = 0; k < kEvalWPT; ++k) {
+    const uint32_t col = c + k;
+    if (col < n) {
+      gw[k] = __ldg(rows + col);
+      w[k] = make_worker(__ldg(p.wa + gw[k]), __ldg(p.wb + gw[k]));
+      if (p.nacc) w[k].mmask = __ldg(p.nacc + gw[k]);
+    } else {
+      gw[k] = kNone;
+      w[k] = null_worker();
+    }
+  }
+}
+
+template <int BITS, bool FAST>
+__global__ void __launch_bounds__(kEvalThreads, 2)
+pm_first_ask_rows(EvalParams p, const uint32_t* __restrict__ rows, uint32_t n, uint32_t chunk,
+                  uint32_t* __restrict__ first_ask, unsigned long long* __restrict__ evals) {
+  __shared__ EvalStage s;
+  const uint32_t cta0 = blockIdx.x * kEvalCols;
+  const uint32_t c = cta0 + threadIdx.x * kEvalWPT;
+  WorkerReg w[kEvalWPT];
+  uint32_t gw[kEvalWPT];
+  gather_workers(p, rows, n, c, w, gw);
+  const uint32_t n_cta = min(n - cta0, (uint32_t)kEvalCols);   // listed workers of this CTA
+  uint32_t first[kEvalWPT];
+  bool open[kEvalWPT];   // a listed candidate without a hit published yet
+#pragma unroll
+  for (int k = 0; k < kEvalWPT; ++k) {
+    first[k] = kNone;
+    open[k] = gw[k] != kNone && (w[k].flags & kCandBit) != 0u;
+  }
+  const uint32_t c0 = blockIdx.y * chunk, c1 = min(p.n_asks, c0 + chunk);
+  unsigned long long pairs = 0;
+  for (uint32_t r0 = c0; r0 < c1; r0 += kEvalRows) {
+    // publish this CTA's hits (each is final: later rows are higher), then stop when no worker can still improve
+    bool done = true;
+#pragma unroll
+    for (int k = 0; k < kEvalWPT; ++k) {
+      if (!open[k]) continue;
+      if (first[k] != kNone) {
+        atomicMin(first_ask + gw[k], first[k]);
+        open[k] = false;
+      } else {
+        done &= *reinterpret_cast<volatile const uint32_t*>(first_ask + gw[k]) < r0;
+      }
+    }
+    // also the barrier that lets for_each_staged_row re-initialise its mbarrier and overwrite the stage
+    if (__syncthreads_and(done)) break;
+    const uint32_t r1 = min(c1, r0 + (uint32_t)kEvalRows);
+    for_each_staged_row(s, p, FAST, r0, 0u, r1 - r0, [&](uint32_t r, const DevAsk& a, uint32_t obegin, bool staged) {
+      uint32_t f[kEvalWPT];
+      if (FAST && staged) {
+        uint32_t fail[kEvalWPT];
+        eval_row_fast<kEvalWPT, BITS>(s, a, obegin, w, p.bits, p.words, fail);
+#pragma unroll
+        for (int k = 0; k < kEvalWPT; ++k) f[k] = ~(uint32_t)((int32_t)fail[k] >> 31);   // all-ones <=> feasible
+      } else if (staged) {
+        eval_row<kEvalWPT, BITS>(s, a, obegin, w, p.bits, p.words, f);
+      } else {
+        eval_row_global<kEvalWPT>(p, a, w, f);
+      }
+      const uint32_t t = r0 + r;
+#pragma unroll
+      for (int k = 0; k < kEvalWPT; ++k) first[k] = min(first[k], t | ~f[k]);
+    });
+    pairs += (unsigned long long)(r1 - r0) * n_cta;
+  }
+#pragma unroll
+  for (int k = 0; k < kEvalWPT; ++k)
+    if (open[k] && first[k] != kNone) atomicMin(first_ask + gw[k], first[k]);
+  if (threadIdx.x == 0 && pairs) atomicAdd(evals, pairs);
+}
+
 // ------------------------------------------------------------------ ask-table conversion
 // pm_ask / pm_gpu_opt (ABI form, field-for-field NodeGroupConfiguration + GpuRequirements) ->
 // DevAsk / DevOpt / DevOptF, on the device: the upload is a plain memcpy of the caller's tables
@@ -911,11 +1011,7 @@ __global__ void pm_scatter_rows(uint4* wa, uint4* wb, double* lat, double* lon, 
 // Do all workers satisfy the fast-path operand limits (values < 2^31, gpu count < 2^16,
 // count * memory_mb < 2^31 without wrapping)?  Clears ok[0] otherwise.  Is every price below
 // kNarrowInfeasible, so that the 32-bit cost tile can hold it?  Clears ok[1] otherwise.
-__global__ void pm_check_worker_ranges(const uint4* __restrict__ wa, const uint4* __restrict__ wb,
-                                       uint32_t n, uint32_t* __restrict__ ok) {
-  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const uint4 a = wa[i], b = wb[i];
+__device__ __forceinline__ void check_worker_range(const uint4& a, const uint4& b, uint32_t* __restrict__ ok) {
   bool small = (b.x | b.y | b.z) < kSign;
   if (a.w & PM_W_HAS_GPU_COUNT) small &= a.x < 65536u;
   if (a.w & PM_W_HAS_GPU_MEM) small &= a.y < kSign;
@@ -923,6 +1019,26 @@ __global__ void pm_check_worker_ranges(const uint4* __restrict__ wa, const uint4
     small &= (unsigned long long)a.x * (unsigned long long)a.y < (unsigned long long)kSign;
   if (!small) ok[0] = 0u;
   if (b.w >= kNarrowInfeasible) ok[1] = 0u;
+}
+__global__ void pm_check_worker_ranges(const uint4* __restrict__ wa, const uint4* __restrict__ wb,
+                                       uint32_t n, uint32_t* __restrict__ ok) {
+  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  check_worker_range(wa[i], wb[i], ok);
+}
+// ... over the listed rows only: an incremental pass starts from the flags of the last full check, so a flag cleared
+// once stays cleared until a full check (both predicates give the same answers; only the speed differs)
+__global__ void pm_check_worker_rows(const uint4* __restrict__ wa, const uint4* __restrict__ wb,
+                                     const uint32_t* __restrict__ rows, uint32_t n, uint32_t* __restrict__ ok) {
+  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const uint32_t w = rows[i];
+  check_worker_range(wa[w], wb[w], ok);
+}
+
+__global__ void pm_scatter_value(uint32_t* __restrict__ dst, const uint32_t* __restrict__ rows, uint32_t n, uint32_t v) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) dst[rows[i]] = v;
 }
 
 // ------------------------------------------------------------------ resolution

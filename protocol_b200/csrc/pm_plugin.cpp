@@ -1108,7 +1108,9 @@ int pm_plugin_try_form_new_groups(pm_plugin* p, uint32_t* n_formed) try {
     // the pass needs the per-worker first feasible configuration only: evaluate and reduce on chip, skip the per-ask
     // statistics (same groups as the materialised pass, ~20 MB of DRAM traffic instead of 16 B per pair)
     mode = (p->policy.proximity_enabled ? PM_MODE_PROXIMITY : PM_MODE_FIRST_FIT) | PM_PATH_FUSED | PM_NO_ASK_STATS;
-    p->resident_version = ~0ull;   // not valid again until this pass has put its rows on the device
+    // resident tables: the engine re-evaluates only the rows this pass sends (a full upload re-evaluates everything)
+    if (!full) mode |= PM_INCREMENTAL;
+    p->resident_version = ~0ull;  // not valid again until this pass has put its rows on the device
   }
   // ---- phase 2 (tables unlocked: heartbeats keep being served): the pass on the GPU
   auto chk = [&](int r, const char* what) {
