@@ -197,6 +197,17 @@ void  pm_free_pinned(void*);
 /* [opt_off, opt_off + n_opts) ranges may overlap or be shared between asks.  */
 int pm_set_asks(pm_engine*, const pm_ask* asks, uint32_t n_asks,
                 const pm_gpu_opt* opts, uint32_t n_opts);
+/* Enabled configurations (get_available_configurations, mod.rs:399-418; enable_configuration, mod.rs:1328-1346).
+ * After pm_set_asks every ask is enabled.  A disabled ask behaves as if it were absent from the table: no worker's
+ * first feasible ask is a disabled one, no under-filled tail is handed down to one, it forms no group (not the empty
+ * group of min_group_size == 0 either), its ask_best reads PM_COST_INF and its ask_count 0, its pm_build_cost_tile
+ * rows are all infeasible, and per-table facts are taken over the enabled asks (a disabled max_group_size == 0 ask does
+ * not make PM_MODE_PROXIMITY refuse).  Result indices (worker_ask, group_ask, ask_best / ask_count positions) stay
+ * indices of the full table.  enabled[i] != 0 enables ask idx[i]; the last entry for an ask decides.  An index
+ * >= n_asks is PM_E_INVALID and changes nothing; PM_E_STATE without an ask table.  PM_MODE_AUCTION returns
+ * PM_E_UNSUPPORTED while any ask is disabled.  The stored evaluation of PM_INCREMENTAL is kept: see "Incremental
+ * passes".                                                                                                          */
+int pm_set_ask_enabled(pm_engine*, const uint32_t* idx, const uint8_t* enabled, uint32_t n);
 int pm_set_model_table(pm_engine*, const uint32_t* bits, uint32_t n_patterns,
                        uint32_t n_models, uint32_t words_per_pattern);
 /* replaces NodeStore::get_nodes per pass (store/domains/node_store.rs:163-209);
@@ -267,10 +278,15 @@ enum pm_path {
  * and pm_set_flags (the in-range indices, each once) and pm_resize_workers (the rows past the old end).
  * pm_set_worker_locations, pm_set_worker_addr_rank and pm_set_worker_reputation write nothing the predicate reads.
  * pm_set_asks, pm_set_model_table, pm_set_worker_count, pm_set_shard, pm_attach_comm and a pass that fails discard the
- * stored evaluation.  Without the flag pm_match evaluates every pair as before.  pm_stats under the flag:
- *   evals    pair evaluations executed: T x W on a full evaluation, the kernel's own count on an incremental one,
- *            0 when no row changed;
- *   n_tiles  worker rows re-evaluated (W on a full evaluation).                                                      */
+ * stored evaluation.  Without the flag pm_match evaluates every pair as before.
+ * pm_set_ask_enabled keeps the stored evaluation: the next incremental pass also walks the workers whose stored first
+ * ask was disabled since ("orphans", from the ask after it) and evaluates every worker against the asks enabled since
+ * (only those whose stored first ask lies beyond the first of them; an ask switched off and on again counts as
+ * neither).  With many asks enabled the pass evaluates everything instead: the pairs of that walk, |E| x W, count as
+ * |E| x W / T written rows against the PM_TUNE_INCR cutoff.  pm_stats under the flag:
+ *   evals    pair evaluations executed: T x W on a full evaluation; on an incremental one the kernels' own count over
+ *            the three walks (written rows, orphans, newly enabled asks); 0 when no row and no mask changed;
+ *   n_tiles  worker rows walked in full: W on a full evaluation, else written rows + orphans.                      */
 
 typedef struct pm_stats {
   uint64_t evals;            /* predicate evaluations executed on the device        */
@@ -362,6 +378,7 @@ uint32_t    pm_multi_size(const pm_multi*);
 pm_engine*  pm_multi_engine(pm_multi*, uint32_t i);   /* per-device access (stats, auction params, ...) */
 const char* pm_multi_last_error(const pm_multi*);
 int pm_multi_set_asks(pm_multi*, const pm_ask* asks, uint32_t n_asks, const pm_gpu_opt* opts, uint32_t n_opts);
+int pm_multi_set_ask_enabled(pm_multi*, const uint32_t* idx, const uint8_t* enabled, uint32_t n);
 int pm_multi_set_model_table(pm_multi*, const uint32_t* bits, uint32_t n_patterns, uint32_t n_models,
                              uint32_t words_per_pattern);
 int pm_multi_set_worker_count(pm_multi*, uint32_t n_workers);

@@ -273,7 +273,19 @@ struct pm_engine {
   uint32_t n_patterns = 0, n_models = 0, words = 1;
   uint32_t max_pattern_row = 0;
   bool have_workers = false, have_asks = false, have_bits = false, have_loc = false, have_rank = false;
-  bool all_solo = true;  // every ask has min == max == 1
+  bool all_solo = true;  // every enabled ask has min == max == 1
+  // The enabled-configuration mask (pm_set_ask_enabled): the host copy is the mask; the converted rows carry it
+  // (pm_ask_convert).  Per ask its kind (kAskKindNotSolo / kAskKindMaxZero), and how many enabled asks have each kind:
+  // the per-table facts all_solo and any_max_zero are taken over the enabled asks.
+  std::vector<uint8_t> ask_on, ask_kind;
+  uint32_t n_off = 0, n_on_not_solo = 0, n_on_max_zero = 0;
+  static constexpr uint8_t kAskKindNotSolo = 1, kAskKindMaxZero = 2;
+  void count_kind(uint32_t t, int d) {
+    if (ask_kind[t] & kAskKindNotSolo) n_on_not_solo += d;
+    if (ask_kind[t] & kAskKindMaxZero) n_on_max_zero += d;
+    all_solo = n_on_not_solo == 0;
+    any_max_zero = n_on_max_zero != 0;
+  }
   int tune_argmin = 0, tune_generic = 0, tune_build = 0, tune_auction = 0, tune_prox = 0, tune_auc_good = 0, tune_auc_extra = 0;   // PM_TUNE_*: kernel-shape experiments
   int tune_compress = 1;  // PM_TUNE_COMPRESS=0: the cost tile in plain cudaMalloc memory (A/B runs)
   int tune_pipe = 16;     // PM_TUNE_PIPE: rows per band of pm_build_argmin (8 / 16 / 32 / 64); 0: build + argmin launches
@@ -322,7 +334,25 @@ struct pm_engine {
   DevBuf<uint32_t> dirty_dev;
   DevBuf<unsigned long long> incr_evals;
   bool incr_evals_pending = false;      // stats.evals of the incremental pass arrives with the pass's one sync
+  // The mask the stored evaluation was taken under (eval_on) and the asks toggled since (toggled, each once; an ask
+  // switched off and on again is listed but has eval_on == ask_on).  walk_start: the orphan walk's start bounds.
+  std::vector<uint8_t> eval_on, toggle_mark;
+  std::vector<uint32_t> toggled;
+  DevBuf<uint32_t> walk_start, toggle_dev;
 
+  // E (enabled since the stored evaluation) and D (disabled since), increasing
+  void split_toggles(std::vector<uint32_t>* en, std::vector<uint32_t>* dis) const {
+    en->clear();
+    dis->clear();
+    for (uint32_t t : toggled)
+      if (ask_on[t] != eval_on[t]) (ask_on[t] ? en : dis)->push_back(t);
+    std::sort(en->begin(), en->end());
+    std::sort(dis->begin(), dis->end());
+  }
+  void clear_toggled() {
+    for (uint32_t t : toggled) { toggle_mark[t] = 0; eval_on[t] = ask_on[t]; }
+    toggled.clear();
+  }
   void clear_dirty() {
     for (uint32_t i : dirty_rows) dirty_mark[i] = 0;
     dirty_rows.clear();
@@ -330,6 +360,7 @@ struct pm_engine {
   }
   void invalidate_eval() {
     clear_dirty();
+    clear_toggled();
     eval_valid = false;
     workers_base = nacc_base = false;
   }
@@ -507,6 +538,10 @@ pm::EvalParams eval_params(pm_engine* e) {
   return p;
 }
 
+pm::AskTables ask_tables(pm_engine* e) {
+  return pm::AskTables{e->asks.p, e->opts.p, e->opts_fast.p, e->frows.p, e->amin.p, e->amax.p};
+}
+
 }  // namespace
 
 extern "C" {
@@ -599,6 +634,7 @@ void pm_destroy(pm_engine* e) {
   e->upd_a.release(); e->upd_b.release(); e->upd_lat.release(); e->upd_lon.release();
   e->cost.release(); e->first_ask.release(); e->ask_count.release(); e->ask_best.release();
   e->eval_first.release(); e->h_dirty.release(); e->dirty_dev.release(); e->incr_evals.release();
+  e->walk_start.release(); e->toggle_dev.release();
   e->keys.release(); e->keys_sorted.release(); e->iota.release(); e->order.release();
   e->hist.release(); e->seg_start.release(); e->ngroups.release(); e->group_base.release();
   e->base_len.release(); e->xhead.release(); e->xnext.release(); e->xcount.release();
@@ -667,11 +703,14 @@ int pm_set_asks(pm_engine* e, const pm_ask* asks, uint32_t n_asks, const pm_gpu_
     PM_CUDA(cub::DeviceScan::ExclusiveSum(e->cub_tmp.p, tmp, e->ask_counts.p, e->ask_newoff.p, (int)(n_asks + 1), e->stream));
   }
   if (n_asks) {
-    pm::pm_ask_convert<<<blocks_for(n_asks, 256), 256, 0, e->stream>>>(e->raw_asks.p, e->raw_opts.p, n_asks, e->ask_newoff.p, e->asks.p,
-                                                                        e->opts.p, e->opts_fast.p, e->amin.p, e->amax.p,
-                                                                        e->counters.p + 12, e->counters.p + 13, e->frows.p);
+    pm::pm_ask_convert<<<blocks_for(n_asks, 256), 256, 0, e->stream>>>(e->raw_asks.p, e->raw_opts.p, n_asks, e->ask_newoff.p,
+                                                                        ask_tables(e), e->counters.p + 12, e->counters.p + 13);
     PM_LAUNCH_CHECK("pm_ask_convert");
   }
+  std::vector<uint8_t> kind(n_asks);
+  for (uint32_t i = 0; i < n_asks; ++i)
+    kind[i] = (uint8_t)((asks[i].min_group_size == 1 && asks[i].max_group_size == 1 ? 0 : pm_engine::kAskKindNotSolo) |
+                        (asks[i].max_group_size == 0 ? pm_engine::kAskKindMaxZero : 0));
   PM_CUDA(cudaMemcpyAsync(e->h_scalars.p + 20, e->counters.p + 12, 8, cudaMemcpyDeviceToHost, e->stream));
   PM_CUDA(cudaMemcpyAsync(e->h_scalars.p + 22, e->ask_newoff.p + n_asks, 4, cudaMemcpyDeviceToHost, e->stream));
   PM_CUDA(cudaStreamSynchronize(e->stream));  // also: the caller's tables are no longer read after return
@@ -684,13 +723,67 @@ int pm_set_asks(pm_engine* e, const pm_ask* asks, uint32_t n_asks, const pm_gpu_
   e->n_asks = n_asks;
   e->n_opts = e->h_scalars.p[22];
   e->max_pattern_row = e->h_scalars.p[21];
-  e->all_solo = (st & pm::kAskNotSolo) == 0;
   e->asks_small = (st & pm::kAskNotSmall) == 0;
-  e->any_max_zero = (st & pm::kAskMaxZero) != 0;
+  // every ask enabled
+  e->ask_kind = std::move(kind);
+  e->ask_on.assign(n_asks, 1);
+  e->eval_on.assign(n_asks, 1);
+  e->toggle_mark.assign(n_asks, 0);
+  e->n_off = e->n_on_not_solo = e->n_on_max_zero = 0;
+  for (uint32_t i = 0; i < n_asks; ++i) e->count_kind(i, +1);
+  e->all_solo = e->n_on_not_solo == 0;
+  e->any_max_zero = e->n_on_max_zero != 0;
   e->have_caps = false;
   e->have_min_rep = false;
   e->auc_classes_valid = false;
   e->have_asks = true;
+  e->matched = e->local_done = false;
+  return PM_OK;
+} catch (...) { return pm_guard_rc(); }
+
+// Enabled configurations.  Only the asks whose state changes are converted again (pm_ask_toggle); the stored
+// evaluation is kept, and the asks toggled since it are listed for the next incremental pass.
+int pm_set_ask_enabled(pm_engine* e, const uint32_t* idx, const uint8_t* enabled, uint32_t n) try {
+  if (!e) return PM_E_INVALID;
+  std::lock_guard<std::mutex> lk(e->mu);
+  if (!e->have_asks) return e->fail(PM_E_STATE, "pm_set_ask_enabled: no ask table");
+  if (n == 0) return PM_OK;
+  if (!idx || !enabled) return e->fail(PM_E_INVALID, "pm_set_ask_enabled: null");
+  for (uint32_t i = 0; i < n; ++i)
+    if (idx[i] >= e->n_asks) return e->fail(PM_E_INVALID, "pm_set_ask_enabled: ask index out of range");
+  // the last entry for an ask decides its state
+  std::vector<uint32_t> ord(n);
+  for (uint32_t i = 0; i < n; ++i) ord[i] = i;
+  std::stable_sort(ord.begin(), ord.end(), [&](uint32_t x, uint32_t y) { return idx[x] < idx[y]; });
+  std::vector<uint32_t> changes;   // ask << 1 | enabled
+  for (uint32_t j = 0; j < n; ++j) {
+    if (j + 1 < n && idx[ord[j + 1]] == idx[ord[j]]) continue;
+    const uint32_t t = idx[ord[j]];
+    const uint8_t on = enabled[ord[j]] ? 1 : 0;
+    if (on != e->ask_on[t]) changes.push_back(t << 1 | on);
+  }
+  if (changes.empty()) return PM_OK;
+  ++e->table_version;
+  PM_CUDA(cudaSetDevice(e->device));
+  PM_CUDA(e->toggle_dev.ensure(changes.size()));
+  PM_CUDA(cudaMemcpyAsync(e->toggle_dev.p, changes.data(), changes.size() * 4, cudaMemcpyHostToDevice, e->stream));
+  pm::pm_ask_toggle<<<blocks_for(changes.size(), 256), 256, 0, e->stream>>>(e->raw_asks.p, e->raw_opts.p, e->ask_newoff.p,
+                                                                            e->toggle_dev.p, (uint32_t)changes.size(), ask_tables(e));
+  PM_LAUNCH_CHECK("pm_ask_toggle");
+  PM_CUDA(cudaStreamSynchronize(e->stream));   // `changes` is a local
+  for (uint32_t v : changes) {
+    const uint32_t t = v >> 1;
+    const bool on = (v & 1u) != 0;
+    e->ask_on[t] = on ? 1 : 0;
+    e->n_off += on ? (uint32_t)-1 : 1u;
+    e->count_kind(t, on ? +1 : -1);
+    if (e->eval_valid && !e->toggle_mark[t]) {
+      e->toggle_mark[t] = 1;
+      e->toggled.push_back(t);
+    }
+  }
+  e->rows_bound = false;           // the FastRows were converted again: pm_bind_rows binds them anew
+  e->auc_classes_valid = false;
   e->matched = e->local_done = false;
   return PM_OK;
 } catch (...) { return pm_guard_rc(); }
@@ -1094,18 +1187,33 @@ static void launch_argmin(pm_engine* e, cudaStream_t st, bool narrow, const long
 #undef PM_ARGMIN_CASE
 }
 
-// The incremental evaluation: the stored per-worker first feasible ask is rewritten for the rows written since it was
-// taken (pm_first_ask_rows), then copied to first_ask, the resolution's working copy.  Same predicate variant as the
-// full pass would pick; the O(W) preludes (operand-range check, worker-major acceptance words) cover the listed rows.
-static int eval_incremental(pm_engine* e) {
+// The incremental evaluation.  Three walks (pm_first_ask_rows) rewrite the stored per-worker first feasible ask; each
+// merges with atomicMin after the resets, so their order does not matter:
+//   * the rows written since it was taken: reset, and walked over every ask;
+//   * after asks were disabled (`dis`, D): the orphans, workers whose stored first ask f is in D.  Only the device
+//     holds the stored evaluation, so pm_collect_orphans finds them, resets them and lists them after the written rows,
+//     each to be walked from f + 1; reading their count back is the pass's one extra host synchronisation, and only
+//     D makes it;
+//   * after asks were enabled (`en`, E): the E-pass, every worker against E only.  A worker whose f lies below every
+//     ask of E is settled; the others gain min(f, first feasible ask of E).
+// Then the stored copy goes to first_ask, the resolution's working copy.  Same predicate variant as the full pass
+// would pick; the O(W) preludes (operand-range check, worker-major acceptance words) cover the written rows.
+static int eval_incremental(pm_engine* e, const std::vector<uint32_t>& en, const std::vector<uint32_t>& dis) {
   const uint32_t W = e->n_workers, T = e->n_asks;
   const uint32_t k = (uint32_t)e->dirty_rows.size();
+  const uint32_t ne = (uint32_t)en.size(), nd = (uint32_t)dis.size();
   e->stats.n_tiles = k;
-  if (k) {
-    PM_CUDA(e->h_dirty.ensure(k));
+  if (k || ne || nd) {
+    // host staging [written rows | E | D]; device: written rows (then the orphans) in dirty_dev, E and D in toggle_dev
+    PM_CUDA(e->h_dirty.ensure((size_t)k + ne + nd));
     std::memcpy(e->h_dirty.p, e->dirty_rows.data(), (size_t)k * 4);
-    PM_CUDA(e->dirty_dev.ensure(k));
-    PM_CUDA(cudaMemcpyAsync(e->dirty_dev.p, e->h_dirty.p, (size_t)k * 4, cudaMemcpyHostToDevice, e->stream));
+    std::memcpy(e->h_dirty.p + k, en.data(), (size_t)ne * 4);
+    std::memcpy(e->h_dirty.p + k + ne, dis.data(), (size_t)nd * 4);
+    PM_CUDA(e->dirty_dev.ensure(nd ? (size_t)k + W : std::max<size_t>(k, 1)));
+    PM_CUDA(e->toggle_dev.ensure((size_t)ne + nd));
+    if (k) PM_CUDA(cudaMemcpyAsync(e->dirty_dev.p, e->h_dirty.p, (size_t)k * 4, cudaMemcpyHostToDevice, e->stream));
+    if (ne + nd)
+      PM_CUDA(cudaMemcpyAsync(e->toggle_dev.p, e->h_dirty.p + k, ((size_t)ne + nd) * 4, cudaMemcpyHostToDevice, e->stream));
     PM_CUDA(e->incr_evals.ensure(1));
     PM_CUDA(cudaMemsetAsync(e->incr_evals.p, 0, 8, e->stream));
     pm::EvalParams p = eval_params(e);
@@ -1120,23 +1228,50 @@ static int eval_incremental(pm_engine* e) {
       const int rc = worker_major(e, &p, &bits_mode, e->dirty_dev.p, k);
       if (rc != PM_OK) return rc;
     }
-    Timer tm(e, &e->stats.ms_fused, e->stream);
-    pm::pm_scatter_value<<<blocks_for(k, 256), 256, 0, e->stream>>>(e->eval_first.p, e->dirty_dev.p, k, pm::kNone);
-    PM_LAUNCH_CHECK("pm_scatter_value");
-    // about four CTAs per SM in all: few listed workers split the asks into more chunks
-    const uint32_t gx = blocks_for(k, pm::kEvalCols);
-    const uint32_t steps = blocks_for(T, pm::kEvalRows);
-    const uint32_t want_y = std::max(1u, std::min(steps, blocks_for(4u * e->sms, gx)));
-    const uint32_t chunk = blocks_for(steps, want_y) * pm::kEvalRows;
-    const dim3 grid(gx, blocks_for(T, chunk));
-#define PM_ROWS_CASE(B, F) pm::pm_first_ask_rows<B, F><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, e->dirty_dev.p, k, chunk, e->eval_first.p, e->incr_evals.p)
-    if (fast) {
-      if (bits_mode == 2) PM_ROWS_CASE(2, true); else if (bits_mode == 1) PM_ROWS_CASE(1, true); else PM_ROWS_CASE(0, true);
-    } else {
-      if (bits_mode == 2) PM_ROWS_CASE(2, false); else if (bits_mode == 1) PM_ROWS_CASE(1, false); else PM_ROWS_CASE(0, false);
-    }
+    auto walk = [&](const pm::AskWalk& a, dim3 grid) -> int {
+#define PM_ROWS_CASE(B, F) pm::pm_first_ask_rows<B, F><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, a, e->eval_first.p, e->incr_evals.p)
+      if (fast) {
+        if (bits_mode == 2) PM_ROWS_CASE(2, true); else if (bits_mode == 1) PM_ROWS_CASE(1, true); else PM_ROWS_CASE(0, true);
+      } else {
+        if (bits_mode == 2) PM_ROWS_CASE(2, false); else if (bits_mode == 1) PM_ROWS_CASE(1, false); else PM_ROWS_CASE(0, false);
+      }
 #undef PM_ROWS_CASE
-    PM_LAUNCH_CHECK("pm_first_ask_rows");
+      PM_LAUNCH_CHECK("pm_first_ask_rows");
+      return PM_OK;
+    };
+    Timer tm(e, &e->stats.ms_fused, e->stream);
+    if (k) {
+      pm::pm_scatter_value<<<blocks_for(k, 256), 256, 0, e->stream>>>(e->eval_first.p, e->dirty_dev.p, k, pm::kNone);
+      PM_LAUNCH_CHECK("pm_scatter_value");
+    }
+    uint32_t n_walk = k;
+    const uint32_t* starts = nullptr;
+    if (nd) {
+      PM_CUDA(e->walk_start.ensure((size_t)k + W));
+      if (k) PM_CUDA(cudaMemsetAsync(e->walk_start.p, 0, (size_t)k * 4, e->stream));   // written rows: every ask
+      PM_CUDA(cudaMemsetAsync(e->counters.p + 16, 0, 4, e->stream));
+      pm::pm_collect_orphans<<<blocks_for(W, 256), 256, 0, e->stream>>>(e->eval_first.p, W, e->toggle_dev.p + ne, nd,
+                                                                        e->dirty_dev.p + k, e->walk_start.p + k, e->counters.p + 16);
+      PM_LAUNCH_CHECK("pm_collect_orphans");
+      PM_CUDA(cudaMemcpyAsync(e->h_scalars.p + 16, e->counters.p + 16, 4, cudaMemcpyDeviceToHost, e->stream));
+      PM_CUDA(cudaStreamSynchronize(e->stream));   // the orphan count sizes the walk's grid
+      n_walk = k + e->h_scalars.p[16];
+      starts = e->walk_start.p;
+      e->stats.n_tiles = n_walk;
+    }
+    if (n_walk) {
+      // about four CTAs per SM in all: few listed workers split the asks into more chunks
+      const uint32_t gx = blocks_for(n_walk, pm::kEvalCols);
+      const uint32_t steps = blocks_for(T, pm::kEvalRows);
+      const uint32_t want_y = std::max(1u, std::min(steps, blocks_for(4u * e->sms, gx)));
+      const uint32_t chunk = blocks_for(steps, want_y) * pm::kEvalRows;
+      const int rc = walk(pm::AskWalk{e->dirty_dev.p, starts, nullptr, n_walk, T, chunk}, dim3(gx, blocks_for(T, chunk)));
+      if (rc != PM_OK) return rc;
+    }
+    if (ne) {   // every worker against all of E: E is short, and W / 1024 CTAs spread over the SMs
+      const int rc = walk(pm::AskWalk{nullptr, nullptr, e->toggle_dev.p, W, ne, ne}, dim3(blocks_for(W, pm::kEvalCols), 1));
+      if (rc != PM_OK) return rc;
+    }
     tm.stop();
     // read back with the pass's one host synchronisation (match_finish_locked)
     PM_CUDA(cudaMemcpyAsync(e->h_scalars.p + 30, e->incr_evals.p, 8, cudaMemcpyDeviceToHost, e->stream));
@@ -1144,6 +1279,7 @@ static int eval_incremental(pm_engine* e) {
   }
   PM_CUDA(cudaMemcpyAsync(e->first_ask.p, e->eval_first.p, (size_t)W * 4, cudaMemcpyDeviceToDevice, e->stream));
   e->clear_dirty();
+  e->clear_toggled();
   return PM_OK;
 }
 
@@ -1182,8 +1318,13 @@ static int match_local_locked(pm_engine* e, uint32_t mode) {
   // Only an engine that evaluates the whole table keeps a stored evaluation (a shard's first_ask holds its range only).
   const bool keep_eval = !e->comm && w0 == 0 && nw == W;
   const bool incr = (mode & PM_INCREMENTAL) != 0;
+  std::vector<uint32_t> en, dis;   // asks enabled / disabled since the stored evaluation
+  if (incr && keep_eval && e->eval_valid) e->split_toggles(&en, &dis);
+  // The E-pass evaluates up to |E| x W pairs, as many as |E| W / T written rows walked in full: they count against the
+  // same cutoff (DESIGN §5)
+  const uint64_t e_rows = T ? ((uint64_t)en.size() * W + T - 1) / T : 0;
   const bool use_incr = incr && keep_eval && e->eval_valid && !e->dirty_over && e->tune_incr != 0 &&
-                        e->dirty_rows.size() <= e->tune_incr && T && W;
+                        e->dirty_rows.size() + e_rows <= e->tune_incr && T && W;
 
   PM_CUDA(e->first_ask.ensure(W));
   PM_CUDA(e->ask_best.ensure(T));
@@ -1196,7 +1337,7 @@ static int match_local_locked(pm_engine* e, uint32_t mode) {
   }
 
   if (use_incr) {
-    const int rc = eval_incremental(e);
+    const int rc = eval_incremental(e, en, dis);
     if (rc != PM_OK) return rc;
   } else if (T && nw) {
     pm::EvalParams p = eval_params(e);
@@ -1292,6 +1433,8 @@ static int match_local_locked(pm_engine* e, uint32_t mode) {
       PM_CUDA(cudaMemcpyAsync(e->eval_first.p, e->first_ask.p, (size_t)W * 4, cudaMemcpyDeviceToDevice, e->stream));
       e->clear_dirty();
       e->dirty_mark.resize(W, 0);   // every mark is clear after clear_dirty
+      e->clear_toggled();
+      e->eval_on = e->ask_on;       // the mask this evaluation was taken under
       e->eval_valid = true;
     } else {
       e->invalidate_eval();
@@ -1538,6 +1681,8 @@ static int match_auction_locked(pm_engine* e) {
   if (e->max_pattern_row > e->n_patterns || (e->max_pattern_row && !e->have_bits))
     return e->fail(PM_E_STATE, "pm_match: an ask references a model pattern missing from the model table");
   if (e->cfg.shard_count || e->comm) return e->fail(PM_E_UNSUPPORTED, "pm_match: auction mode is single-GPU");
+  // the class cache is keyed on requirement rows, which a disabled ask's no longer are
+  if (e->n_off) return e->fail(PM_E_UNSUPPORTED, "pm_match: auction mode with disabled asks");
   PM_CUDA(cudaSetDevice(e->device));
   const uint32_t W = e->n_workers, T = e->n_asks;
   if (!e->have_bits) {
@@ -2130,6 +2275,14 @@ const char* pm_multi_last_error(const pm_multi* m) { return m ? m->err.c_str() :
 
 int pm_multi_set_asks(pm_multi* m, const pm_ask* asks, uint32_t n_asks, const pm_gpu_opt* opts, uint32_t n_opts) try {
   PM_MULTI_EACH(pm_set_asks(e, asks, n_asks, opts, n_opts));
+} catch (...) { return pm_guard_rc(); }
+int pm_multi_set_ask_enabled(pm_multi* m, const uint32_t* idx, const uint8_t* enabled, uint32_t n) try {
+  if (m && !m->engines.empty()) {   // an index out of range changes nothing on any device
+    pm_engine* e0 = m->engines[0];
+    for (uint32_t i = 0; idx && i < n; ++i)
+      if (idx[i] >= e0->n_asks) { m->err = "pm_set_ask_enabled: ask index out of range"; return PM_E_INVALID; }
+  }
+  PM_MULTI_EACH(pm_set_ask_enabled(e, idx, enabled, n));
 } catch (...) { return pm_guard_rc(); }
 int pm_multi_set_model_table(pm_multi* m, const uint32_t* bits, uint32_t n_patterns, uint32_t n_models, uint32_t words) try {
   PM_MULTI_EACH(pm_set_model_table(e, bits, n_patterns, n_models, words));

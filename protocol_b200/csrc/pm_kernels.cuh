@@ -194,24 +194,31 @@ __device__ __forceinline__ void load_workers(const EvalParams& p, uint32_t w0, u
 
 // Drives `body(row_in_tile, ask, obegin, staged)` over rows [r0, r1) of the tile:
 // ask headers, then as many option rows as fit, arrive in shared memory through
-// 1-D TMA bulk copies signalled on one mbarrier.
+// 1-D TMA bulk copies signalled on one mbarrier.  With `list` the tile's rows are the asks list[t0 + r] (increasing):
+// their headers are gathered by the CTA's threads, and each staged option range is the one that spans the listed
+// asks (the rows between them come along unused, or the step holds fewer asks).
 template <class Body>
 __device__ __forceinline__ void for_each_staged_row(EvalStage& s, const EvalParams& p, bool fast,
-                                                    uint32_t t0, uint32_t r0, uint32_t r1, Body&& body) {
+                                                    uint32_t t0, uint32_t r0, uint32_t r1, Body&& body,
+                                                    const uint32_t* __restrict__ list = nullptr) {
   const DevOpt* opt_src = fast ? reinterpret_cast<const DevOpt*>(p.opts_fast) : p.opts;
   if (threadIdx.x == 0) mbar_init(&s.bar, 1);
   const uint32_t total_words = (p.n_bits_rows)*p.words;
   if (total_words <= (uint32_t)kBitsCap)
     for (uint32_t i = threadIdx.x; i < total_words; i += blockDim.x) s.bits[i] = __ldg(p.bits + i);
+  const uint32_t nrows = r1 - r0;
+  if (list)
+    for (uint32_t i = threadIdx.x; i < nrows; i += blockDim.x) s.ask[i] = p.asks[__ldg(list + t0 + r0 + i)];
   __syncthreads();
   uint32_t phase = 0;
-  const uint32_t nrows = r1 - r0;
-  if (threadIdx.x == 0) {
-    mbar_expect_tx(&s.bar, nrows * (uint32_t)sizeof(DevAsk));
-    bulk_g2s(s.ask, p.asks + t0 + r0, nrows * (uint32_t)sizeof(DevAsk), &s.bar);
+  if (!list) {
+    if (threadIdx.x == 0) {
+      mbar_expect_tx(&s.bar, nrows * (uint32_t)sizeof(DevAsk));
+      bulk_g2s(s.ask, p.asks + t0 + r0, nrows * (uint32_t)sizeof(DevAsk), &s.bar);
+    }
+    mbar_wait(&s.bar, phase);
+    phase ^= 1u;
   }
-  mbar_wait(&s.bar, phase);
-  phase ^= 1u;
   uint32_t row = 0;
   while (row < nrows) {
     const uint32_t obegin = s.ask[row].opt_off;
@@ -777,15 +784,34 @@ pm_fused_eval(EvalParams p, uint32_t t0, uint32_t nt, uint32_t w0, uint32_t nw,
 // kernel holds its stripe) and walks its chunk of `chunk` asks in steps of kEvalRows staged rows.  Asks are in
 // priority order, so a hit is final for the chunk; before each step the CTA stops once every one of its workers has a
 // hit of its own, or a hit below the step's first row in `first_ask` (published by the CTAs of earlier chunks with
-// atomicMin), or is not a candidate at all (no ask can accept it).  `first_ask[rows[i]]` must hold kNone on entry.
-// `evals` gains the pairs evaluated: rows walked x listed workers of the CTA.
+// atomicMin), or is not a candidate at all (no ask can accept it).  The result is min(first_ask[w] on entry, the
+// first hit): a written row enters with kNone.  `evals` gains the pairs evaluated: rows walked x listed workers of the
+// CTA.
+//
+// The same kernel makes the two other walks of an incremental pass after configurations were enabled or disabled
+// (AskWalk):
+//   * the E-pass: every worker (rows == null) against the newly enabled asks only (asks = their increasing list).  A
+//     worker enters with its stored first ask f, so the first step's test already drops it when f lies below every
+//     listed ask, and a CTA whose workers all do exits before its first row;
+//   * the orphans: workers whose stored first ask was disabled, each with a start bound (the ask after it).  Asks
+//     below the start that were enabled then still reject the worker; those enabled since are the E-pass's.  The CTA
+//     starts at the least bound of its workers.
+struct AskWalk {
+  const uint32_t* rows;     // listed workers, or null: workers [0, n)
+  const uint32_t* starts;   // per listed worker, the first ask it can still need; null: 0
+  const uint32_t* asks;     // the asks walked, increasing; null: the whole table
+  uint32_t n;               // listed workers
+  uint32_t n_seq;           // asks walked: entries of `asks`, or the table's n_asks
+  uint32_t chunk;           // asks per grid row (blockIdx.y)
+};
+
 __device__ __forceinline__ void gather_workers(const EvalParams& p, const uint32_t* __restrict__ rows, uint32_t n,
                                                uint32_t c, WorkerReg (&w)[kEvalWPT], uint32_t (&gw)[kEvalWPT]) {
 #pragma unroll
   for (int k = 0; k < kEvalWPT; ++k) {
     const uint32_t col = c + k;
     if (col < n) {
-      gw[k] = __ldg(rows + col);
+      gw[k] = rows ? __ldg(rows + col) : col;
       w[k] = make_worker(__ldg(p.wa + gw[k]), __ldg(p.wb + gw[k]));
       if (p.nacc) w[k].mmask = __ldg(p.nacc + gw[k]);
     } else {
@@ -797,15 +823,15 @@ __device__ __forceinline__ void gather_workers(const EvalParams& p, const uint32
 
 template <int BITS, bool FAST>
 __global__ void __launch_bounds__(kEvalThreads, 2)
-pm_first_ask_rows(EvalParams p, const uint32_t* __restrict__ rows, uint32_t n, uint32_t chunk,
-                  uint32_t* __restrict__ first_ask, unsigned long long* __restrict__ evals) {
+pm_first_ask_rows(EvalParams p, AskWalk a, uint32_t* __restrict__ first_ask, unsigned long long* __restrict__ evals) {
   __shared__ EvalStage s;
+  __shared__ uint32_t s_lo;
   const uint32_t cta0 = blockIdx.x * kEvalCols;
   const uint32_t c = cta0 + threadIdx.x * kEvalWPT;
   WorkerReg w[kEvalWPT];
   uint32_t gw[kEvalWPT];
-  gather_workers(p, rows, n, c, w, gw);
-  const uint32_t n_cta = min(n - cta0, (uint32_t)kEvalCols);   // listed workers of this CTA
+  gather_workers(p, a.rows, a.n, c, w, gw);
+  const uint32_t n_cta = min(a.n - cta0, (uint32_t)kEvalCols);   // listed workers of this CTA
   uint32_t first[kEvalWPT];
   bool open[kEvalWPT];   // a listed candidate without a hit published yet
 #pragma unroll
@@ -813,9 +839,23 @@ pm_first_ask_rows(EvalParams p, const uint32_t* __restrict__ rows, uint32_t n, u
     first[k] = kNone;
     open[k] = gw[k] != kNone && (w[k].flags & kCandBit) != 0u;
   }
-  const uint32_t c0 = blockIdx.y * chunk, c1 = min(p.n_asks, c0 + chunk);
+  uint32_t c0 = blockIdx.y * a.chunk;
+  const uint32_t c1 = min(a.n_seq, c0 + a.chunk);
+  if (a.starts) {   // the CTA's least start bound
+    if (threadIdx.x == 0) s_lo = kNone;
+    __syncthreads();
+    uint32_t lo = kNone;
+#pragma unroll
+    for (int k = 0; k < kEvalWPT; ++k)
+      if (c + k < a.n) lo = min(lo, __ldg(a.starts + c + k));
+    lo = __reduce_min_sync(0xffffffffu, lo);
+    if ((threadIdx.x & 31u) == 0u) atomicMin(&s_lo, lo);
+    __syncthreads();
+    c0 = max(c0, s_lo);
+  }
   unsigned long long pairs = 0;
   for (uint32_t r0 = c0; r0 < c1; r0 += kEvalRows) {
+    const uint32_t t_first = a.asks ? __ldg(a.asks + r0) : r0;   // the step's first ask
     // publish this CTA's hits (each is final: later rows are higher), then stop when no worker can still improve
     bool done = true;
 #pragma unroll
@@ -825,28 +865,28 @@ pm_first_ask_rows(EvalParams p, const uint32_t* __restrict__ rows, uint32_t n, u
         atomicMin(first_ask + gw[k], first[k]);
         open[k] = false;
       } else {
-        done &= *reinterpret_cast<volatile const uint32_t*>(first_ask + gw[k]) < r0;
+        done &= *reinterpret_cast<volatile const uint32_t*>(first_ask + gw[k]) < t_first;
       }
     }
     // also the barrier that lets for_each_staged_row re-initialise its mbarrier and overwrite the stage
     if (__syncthreads_and(done)) break;
     const uint32_t r1 = min(c1, r0 + (uint32_t)kEvalRows);
-    for_each_staged_row(s, p, FAST, r0, 0u, r1 - r0, [&](uint32_t r, const DevAsk& a, uint32_t obegin, bool staged) {
+    for_each_staged_row(s, p, FAST, r0, 0u, r1 - r0, [&](uint32_t r, const DevAsk& q, uint32_t obegin, bool staged) {
       uint32_t f[kEvalWPT];
       if (FAST && staged) {
         uint32_t fail[kEvalWPT];
-        eval_row_fast<kEvalWPT, BITS>(s, a, obegin, w, p.bits, p.words, fail);
+        eval_row_fast<kEvalWPT, BITS>(s, q, obegin, w, p.bits, p.words, fail);
 #pragma unroll
         for (int k = 0; k < kEvalWPT; ++k) f[k] = ~(uint32_t)((int32_t)fail[k] >> 31);   // all-ones <=> feasible
       } else if (staged) {
-        eval_row<kEvalWPT, BITS>(s, a, obegin, w, p.bits, p.words, f);
+        eval_row<kEvalWPT, BITS>(s, q, obegin, w, p.bits, p.words, f);
       } else {
-        eval_row_global<kEvalWPT>(p, a, w, f);
+        eval_row_global<kEvalWPT>(p, q, w, f);
       }
-      const uint32_t t = r0 + r;
+      const uint32_t t = a.asks ? __ldg(a.asks + r0 + r) : r0 + r;
 #pragma unroll
       for (int k = 0; k < kEvalWPT; ++k) first[k] = min(first[k], t | ~f[k]);
-    });
+    }, a.asks);
     pairs += (unsigned long long)(r1 - r0) * n_cta;
   }
 #pragma unroll
@@ -862,9 +902,7 @@ pm_first_ask_rows(EvalParams p, const uint32_t* __restrict__ rows, uint32_t n, u
 enum AskStatusBit : uint32_t {
   kAskBadSizes = 1u << 0,   // max_group_size < min_group_size (is_valid, mod.rs:55-60)
   kAskBadRange = 1u << 1,   // opt_off + n_opts out of bounds
-  kAskNotSmall = 1u << 2,   // an operand does not fit the fast predicate
-  kAskNotSolo = 1u << 3,    // some ask is not min == max == 1
-  kAskMaxZero = 1u << 4     // some ask has max_group_size == 0
+  kAskNotSmall = 1u << 2    // an operand does not fit the fast predicate
 };
 
 __global__ void pm_ask_counts(const pm_ask* __restrict__ asks, uint32_t n_asks, uint32_t n_opts,
@@ -876,29 +914,37 @@ __global__ void pm_ask_counts(const pm_ask* __restrict__ asks, uint32_t n_asks, 
   uint32_t st = 0;
   if (a.max_group_size < a.min_group_size) st |= kAskBadSizes;
   if ((unsigned long long)a.opt_off + a.n_opts > n_opts) st |= kAskBadRange;
-  if (!(a.min_group_size == 1 && a.max_group_size == 1)) st |= kAskNotSolo;
-  if (a.max_group_size == 0) st |= kAskMaxZero;
   if (st) atomicOr(status, st);
   // every converted ask owns at least one option row: an ask without GPU options gets a neutral one (pm_ask_convert)
   counts[t] = max(((a.flags & PM_A_HAS_REQ) && !(st & kAskBadRange)) ? a.n_opts : 0u, 1u);
 }
 
-__global__ void pm_ask_convert(const pm_ask* __restrict__ asks, const pm_gpu_opt* __restrict__ opts,
-                               uint32_t n_asks, const uint32_t* __restrict__ new_off,
-                               DevAsk* __restrict__ dasks, DevOpt* __restrict__ dopts,
-                               DevOptF* __restrict__ doptsf, uint32_t* __restrict__ amin,
-                               uint32_t* __restrict__ amax, uint32_t* __restrict__ status,
-                               uint32_t* __restrict__ max_row, FastRow* __restrict__ frows) {
-  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= n_asks) return;
+struct AskTables {   // the converted forms of the ask table the kernels read
+  DevAsk* dasks;
+  DevOpt* dopts;
+  DevOptF* doptsf;
+  FastRow* frows;
+  uint32_t* amin;
+  uint32_t* amax;
+};
+
+// Ask t in every converted form.  A disabled ask (`off`) carries kNeverBit in its presence mask — DevAsk.need and the
+// m / v of each of its DevOptF rows and its FastRow — so every predicate variant rejects every worker, and its amin is
+// at least 1, so it forms no empty group either: it behaves as if it were absent from the table.  Converting it again
+// with off == false restores the rows exactly.  `status` / `max_row` may be null (a toggle: the table was checked).
+__device__ __forceinline__ void convert_ask(uint32_t t, bool off, bool bad_range, const pm_ask* __restrict__ asks,
+                                            const pm_gpu_opt* __restrict__ opts, const uint32_t* __restrict__ new_off,
+                                            const AskTables& o, uint32_t* __restrict__ status,
+                                            uint32_t* __restrict__ max_row) {
+  DevAsk* __restrict__ dasks = o.dasks;
+  DevOpt* __restrict__ dopts = o.dopts;
+  DevOptF* __restrict__ doptsf = o.doptsf;
   const pm_ask a = asks[t];
   DevAsk d;
   d.n_opts = 0; d.cpu_cores = 0; d.ram_mb = 0; d.storage_gb = 0; d.pad0 = 0; d.pad1 = 0;
   const bool has_req = (a.flags & PM_A_HAS_REQ) != 0;
   uint32_t need = kCandBit;
   const uint32_t n_rows = new_off[t + 1] - new_off[t];                  // >= 1
-  // option rows that come from the caller (none are read when pm_ask_counts found a range out of bounds: the call fails)
-  const bool bad_range = (*reinterpret_cast<volatile uint32_t*>(status) & kAskBadRange) != 0u;
   const uint32_t n_eff = (has_req && !bad_range) ? min(a.n_opts, n_rows) : 0u;
   if (has_req) {
     need |= PM_W_HAS_SPECS;
@@ -909,7 +955,7 @@ __global__ void pm_ask_convert(const pm_ask* __restrict__ asks, const pm_gpu_opt
     if (a.n_opts) need |= PM_W_HAS_GPU;
   }
   d.n_opts = n_rows;
-  if (a.max_group_size == 0) need |= kNeverBit;   // first-fit with max_group_size == 0 takes nobody (mod.rs:555-556)
+  if (a.max_group_size == 0 || off) need |= kNeverBit;   // first-fit with max_group_size == 0 takes nobody (mod.rs:555-556)
   d.need = need;
   d.opt_off = new_off[t];
   uint32_t st = 0, mrow = 0;
@@ -972,12 +1018,64 @@ __global__ void pm_ask_convert(const pm_ask* __restrict__ asks, const pm_gpu_opt
     fr.m = f.m; fr.v = f.v; fr.mem_lo = f.mem_lo; fr.mem_hi = f.mem_hi;
     fr.tot_lo = f.tot_lo; fr.tot_hi = f.tot_hi; fr.wp = f.pattern_row; fr.n_opts = n_rows;
     fr.cpu_cores = d.cpu_cores; fr.ram_mb = d.ram_mb; fr.storage_gb = d.storage_gb; fr.opt_off = d.opt_off;
-    frows[t] = fr;
+    o.frows[t] = fr;
   }
-  amin[t] = a.min_group_size;
-  amax[t] = a.max_group_size;
-  if (st) atomicOr(status, st);
-  if (mrow) atomicMax(max_row, mrow);
+  o.amin[t] = off ? max(a.min_group_size, 1u) : a.min_group_size;
+  o.amax[t] = a.max_group_size;
+  if (st && status) atomicOr(status, st);
+  if (mrow && max_row) atomicMax(max_row, mrow);
+}
+
+__global__ void pm_ask_convert(const pm_ask* __restrict__ asks, const pm_gpu_opt* __restrict__ opts,
+                               uint32_t n_asks, const uint32_t* __restrict__ new_off, AskTables o,
+                               uint32_t* __restrict__ status, uint32_t* __restrict__ max_row) {
+  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= n_asks) return;
+  // option rows that come from the caller (none are read when pm_ask_counts found a range out of bounds: the call fails)
+  const bool bad_range = (*reinterpret_cast<volatile uint32_t*>(status) & kAskBadRange) != 0u;
+  convert_ask(t, false, bad_range, asks, opts, new_off, o, status, max_row);
+}
+
+// pm_set_ask_enabled: the listed asks converted again, enabled or disabled; entry i = ask << 1 | enabled, one entry
+// per ask.
+__global__ void pm_ask_toggle(const pm_ask* __restrict__ asks, const pm_gpu_opt* __restrict__ opts,
+                              const uint32_t* __restrict__ new_off, const uint32_t* __restrict__ list, uint32_t n,
+                              AskTables o) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const uint32_t v = list[i];
+  convert_ask(v >> 1, (v & 1u) == 0u, false, asks, opts, new_off, o, nullptr, nullptr);
+}
+
+// An incremental pass after configurations were disabled: the workers whose stored first ask is one of them (`dis`,
+// increasing, nd entries).  Each is appended to out[] with the ask after its stored one as its walk's start bound, and
+// its stored entry is reset.  One thread per worker, one atomic per warp.
+__global__ void pm_collect_orphans(uint32_t* __restrict__ eval_first, uint32_t n_workers, const uint32_t* __restrict__ dis,
+                                   uint32_t nd, uint32_t* __restrict__ out, uint32_t* __restrict__ starts,
+                                   uint32_t* __restrict__ count) {
+  const uint32_t w = blockIdx.x * blockDim.x + threadIdx.x;
+  const uint32_t f = w < n_workers ? eval_first[w] : kNone;
+  bool hit = false;
+  if (f != kNone) {
+    uint32_t lo = 0, hi = nd;
+    while (lo < hi) {
+      const uint32_t mid = (lo + hi) >> 1;
+      if (__ldg(dis + mid) < f) lo = mid + 1; else hi = mid;
+    }
+    hit = lo < nd && __ldg(dis + lo) == f;
+  }
+  const uint32_t lane = threadIdx.x & 31u;
+  const uint32_t b = __ballot_sync(0xffffffffu, hit);
+  if (!b) return;
+  uint32_t base = 0;
+  if (lane == 0) base = atomicAdd(count, (uint32_t)__popc(b));
+  base = __shfl_sync(0xffffffffu, base, 0);
+  if (hit) {
+    const uint32_t pos = base + (uint32_t)__popc(b & ((1u << lane) - 1u));
+    out[pos] = w;
+    starts[pos] = f + 1;
+    eval_first[w] = kNone;
+  }
 }
 
 // ------------------------------------------------------------------ small utilities

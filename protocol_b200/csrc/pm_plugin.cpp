@@ -186,7 +186,13 @@ struct pm_plugin {
   std::vector<uint32_t> dirty_list;
   uint32_t resident_rows = 0;
   uint64_t resident_version = ~0ull;
-  std::string resident_asks_sig;
+  // The configurations on the engine: every sealed one, in the order available_configurations() puts them when all are
+  // enabled (the sealed order stably re-sorted by min_group_size desc), uploaded with the worker table; a pass then
+  // sends only the enable flags that changed (pm_set_ask_enabled), which keeps the engine's stored evaluation.  A
+  // stable sort of a subset is the same subset of the stable sort of the whole, so the enabled ones keep the priority
+  // order available_configurations() gives them.
+  std::vector<uint32_t> resident_cfgs;   // indices into templates
+  std::vector<uint8_t> resident_on;      // the flags the engine holds, per resident_cfgs entry
   uint32_t resident_npat = ~0u, resident_nmod = ~0u;
   pm_engine* merge_engine = nullptr;   // solo-group merging works on its own small table: a sibling engine, created on demand
   void touch(size_t i) {
@@ -1027,8 +1033,9 @@ int pm_plugin_export_tables(pm_plugin* p, pm_worker_a* a, pm_worker_b* b, double
 // The worker table stays RESIDENT on the engine between passes, rows in table (insertion) order — every candidate is
 // Healthy, so the candidates' relative order is the canonical order of the status-sorted node list
 // (node_store.rs:195-206) and the groups are the same — and a pass sends only the rows touched since the previous one
-// (status changes, new group members, new nodes): the reference re-reads and re-parses every node per pass.  Asks and
-// the model table travel only when the configurations or the interner changed.  Members of a group are put in
+// (status changes, new group members, new nodes): the reference re-reads and re-parses every node per pass.  Every
+// sealed configuration travels once, with a full upload; after that a pass sends only the enable flags that changed
+// (task events toggle configurations), and the model table only when the interner changed.  Members of a group are put in
 // BTreeSet<String> order here at publication (the address strings are at hand), so no address ranks travel at all.
 int pm_plugin_try_form_new_groups(pm_plugin* p, uint32_t* n_formed) try {
   if (!p) return PM_E_INVALID;
@@ -1041,7 +1048,9 @@ int pm_plugin_try_form_new_groups(pm_plugin* p, uint32_t* n_formed) try {
   std::vector<pm_worker_a> ua;
   std::vector<pm_worker_b> ub;
   std::vector<double> ulat, ulon;
-  std::vector<std::string> cfg_names;
+  std::vector<std::string> cfg_names;   // per engine ask (every sealed configuration)
+  std::vector<uint32_t> toggle_idx;
+  std::vector<uint8_t> toggle_on;
   std::vector<pm_ask> asks;
   std::vector<pm_gpu_opt> opts;
   std::vector<uint32_t> bits_copy;
@@ -1083,21 +1092,35 @@ int pm_plugin_try_form_new_groups(pm_plugin* p, uint32_t* n_formed) try {
       }
     }
     p->dirty_list.clear();
-    const auto configs = p->available_configurations();
-    std::string sig;
-    for (const Config* c : configs) {
-      pm_ask a = c->ask;
-      a.opt_off = (uint32_t)opts.size();
-      a.min_group_size = c->min_group_size;
-      a.max_group_size = c->max_group_size;
-      opts.insert(opts.end(), c->opts.begin(), c->opts.end());
-      asks.push_back(a);
-      cfg_names.push_back(c->name);
-      sig += c->name;
-      sig += '\x1f';
+    send_asks = full;
+    if (send_asks) {
+      const uint32_t C = (uint32_t)p->templates.size();
+      p->resident_cfgs.resize(C);
+      for (uint32_t i = 0; i < C; ++i) p->resident_cfgs[i] = i;
+      std::stable_sort(p->resident_cfgs.begin(), p->resident_cfgs.end(), [&](uint32_t x, uint32_t y) {
+        return p->templates[x].min_group_size > p->templates[y].min_group_size;
+      });
+      p->resident_on.assign(C, 1);   // pm_set_asks enables every ask
+      for (uint32_t i : p->resident_cfgs) {
+        const Config& c = p->templates[i];
+        pm_ask a = c.ask;
+        a.opt_off = (uint32_t)opts.size();
+        a.min_group_size = c.min_group_size;
+        a.max_group_size = c.max_group_size;
+        opts.insert(opts.end(), c.opts.begin(), c.opts.end());
+        asks.push_back(a);
+      }
     }
-    send_asks = full || sig != p->resident_asks_sig;
-    p->resident_asks_sig = sig;
+    for (uint32_t j = 0; j < (uint32_t)p->resident_cfgs.size(); ++j) {
+      const Config& c = p->templates[p->resident_cfgs[j]];
+      cfg_names.push_back(c.name);
+      const uint8_t on = p->available.count(c.name) ? 1 : 0;   // get_available_configurations, mod.rs:399-418
+      if (on != p->resident_on[j]) {
+        toggle_idx.push_back(j);
+        toggle_on.push_back(on);
+        p->resident_on[j] = on;
+      }
+    }
     const uint32_t* bits = nullptr;
     int rc = pm_interner_table(p->interner, &bits, &npat, &nmod, &words);
     if (rc != PM_OK) return p->fail(rc, "pm_interner_table");
@@ -1123,6 +1146,9 @@ int pm_plugin_try_form_new_groups(pm_plugin* p, uint32_t* n_formed) try {
   };
   int rc;
   if (send_asks && (rc = chk(pm_set_asks(p->engine, asks.data(), (uint32_t)asks.size(), opts.data(), (uint32_t)opts.size()), "pm_set_asks"))) return rc;
+  if (!toggle_idx.empty() &&
+      (rc = chk(pm_set_ask_enabled(p->engine, toggle_idx.data(), toggle_on.data(), (uint32_t)toggle_idx.size()), "pm_set_ask_enabled")))
+    return rc;
   if (send_bits && (rc = chk(pm_set_model_table(p->engine, bits_copy.data(), npat, nmod, words), "pm_set_model_table"))) return rc;
   if (full) {
     if ((rc = chk(pm_set_worker_count(p->engine, W), "pm_set_worker_count"))) return rc;

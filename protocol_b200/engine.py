@@ -147,6 +147,12 @@ class Engine:
         self._check(self._lib.pm_set_asks(self._h, _ptr(asks), len(asks), _ptr(opts), len(opts)))
         self.n_asks = len(asks)
 
+    def set_ask_enabled(self, idx, enabled):
+        """Enable (True) or disable (False) the asks idx (pm_set_ask_enabled): a disabled ask behaves as if it were
+        absent from the table; result indices stay those of the full table."""
+        idx, en = _ask_enabled_args(idx, enabled)
+        self._check(self._lib.pm_set_ask_enabled(self._h, _ptr(idx), _ptr(en), len(idx)))
+
     def set_model_table(self, bits: np.ndarray, n_patterns: int, n_models: int, words: int):
         bits = np.ascontiguousarray(bits, dtype=np.uint32)
         self._check(self._lib.pm_set_model_table(self._h, _ptr(bits), n_patterns, n_models, words))
@@ -264,6 +270,13 @@ class Engine:
         self._comm = comm   # keep it alive
 
 
+def _ask_enabled_args(idx, enabled):
+    """(idx, enabled) as the C call takes them; a scalar `enabled` applies to every index."""
+    idx = np.ascontiguousarray(np.atleast_1d(idx), dtype=np.uint32)
+    en = np.broadcast_to(np.asarray(enabled, dtype=bool), idx.shape)
+    return idx, np.ascontiguousarray(en, dtype=np.uint8)
+
+
 def _result_views(r: "abi.PmResult", copy: bool) -> MatchResult:
     def view(ptr, n, dt):
         if n == 0:
@@ -345,6 +358,10 @@ class MultiEngine:
         asks = np.ascontiguousarray(asks, dtype=abi.ASK)
         opts = np.ascontiguousarray(opts, dtype=abi.GPU_OPT)
         self._check(self._lib.pm_multi_set_asks(self._h, _ptr(asks), len(asks), _ptr(opts), len(opts)))
+
+    def set_ask_enabled(self, idx, enabled):
+        idx, en = _ask_enabled_args(idx, enabled)
+        self._check(self._lib.pm_multi_set_ask_enabled(self._h, _ptr(idx), _ptr(en), len(idx)))
 
     def set_model_table(self, bits, n_patterns, n_models, words):
         bits = np.ascontiguousarray(bits, dtype=np.uint32)

@@ -10,7 +10,14 @@ update_workers).  The incremental engine is created with PM_TUNE_INCR above ever
 evaluation and the crossover shows.  For every k, a sibling engine that received the same calls runs the full pass
 and every pm_fetch_result array is compared.  Device time is pm_stats.ms_total (CUDA events on the engine stream);
 host time is the wall time around match() ending in a stream sync.  The card, its power limit and SM clock come from
-the same run."""
+the same run.
+
+    python tools/incremental_bench.py --toggle [...]
+
+The toggle series: configurations enabled and disabled between passes (pm_set_ask_enabled), no worker row written.
+25 000 random asks start disabled, so there are asks to enable.  Per round and for every j in J, alternated with the
+full fused lean pass: ceil(j/2) asks are disabled — half of them the asks that own the most workers, half asks that
+own none — and j//2 disabled ones are enabled, then one incremental pass runs.  Same sibling check as above."""
 from __future__ import annotations
 
 import argparse
@@ -54,15 +61,80 @@ def timed(eng, mode):
     return {"ms_device": st["ms_total"], "ms_host": wall, "evals": st["evals"], "n_tiles": st["n_tiles"]}
 
 
+J = (1, 10, 100, 1_000, 10_000, 50_000)
+
+
+def same_as_full(inc, ref):
+    r = inc.fetch()
+    ref.match(LEAN)
+    q = ref.fetch()
+    return r, all(np.array_equal(getattr(r, f), getattr(q, f)) for f in FIELDS)
+
+
+def toggle_series(args, w, a, bits, npat, nmod, words, env):
+    os.environ["PM_TUNE_INCR"] = str(1 << 31)   # never fall back, so the crossover shows
+    inc = Engine(timing=True)
+    del os.environ["PM_TUNE_INCR"]
+    ref = Engine(timing=True)
+    engines = (inc, ref)
+    W, T = len(w), len(a)
+    rng = np.random.default_rng(2025)
+    on = np.ones(T, bool)
+    on[rng.choice(T, 25_000, replace=False)] = False
+    for e in engines:
+        e.set_asks(a.asks, a.opts)
+        e.set_model_table(bits, npat, nmod, words)
+        e.set_workers(w.a, w.b)
+        e.set_ask_enabled(np.nonzero(~on)[0], False)
+        e.match(LEAN)   # warm-up: allocations, first launches
+    rows = {"full": []}
+    rows.update({j: [] for j in J})
+    checked = set()
+    for rnd in range(args.rounds):
+        for j in J:
+            rows["full"].append(timed(inc, LEAN))   # refreshes the stored evaluation
+            wk = inc.fetch().worker_ask
+            owners = np.bincount(wk[wk != abi.PM_NONE], minlength=T)
+            n_off, n_on = (j + 1) // 2, j // 2
+            enabled = np.nonzero(on)[0]
+            top = enabled[np.argsort(owners[enabled])[::-1][:(n_off + 1) // 2]]
+            idle = enabled[owners[enabled] == 0]
+            off = np.concatenate([top, rng.choice(idle, min(len(idle), n_off - len(top)), replace=False)])
+            disabled = np.nonzero(~on)[0]
+            en = rng.choice(disabled, min(n_on, len(disabled)), replace=False)
+            for e in engines:
+                e.set_ask_enabled(off, False)
+                e.set_ask_enabled(en, True)
+            on[off], on[en] = False, True
+            rows[j].append(dict(timed(inc, INCR), n_off=len(off), n_on=len(en)))
+            if j not in checked:
+                _, same = same_as_full(inc, ref)
+                if not same:
+                    raise SystemExit(f"j={j}: the incremental result differs from the full pass")
+                checked.add(j)
+    for e in engines:
+        e.close()
+    return rows, checked, f"{T} asks x {W} workers (synth mixed, 25 000 asks disabled at the start), first fit, fused lean"
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--workers", type=int, default=1_000_000)
     ap.add_argument("--asks", type=int, default=100_000)
     ap.add_argument("--rounds", type=int, default=3)
+    ap.add_argument("--toggle", action="store_true", help="configurations toggled between passes instead of rows written")
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
 
     w = synth.make_workers(args.workers)
+    if args.toggle:
+        a = synth.make_asks(args.asks, "mixed")
+        bits, npat, nmod, words = synth.intern_tables(w, a)
+        env = card()
+        rows, checked, workload = toggle_series(args, w, a, bits, npat, nmod, words, env)
+        report(rows, checked, workload, env, "j", args.out, "incremental_toggle_bench.json")
+        return
+
     pool = synth.make_workers(200_000, seed=synth.SEED_WORKERS + 101)
     a = synth.make_asks(args.asks, "mixed")
     bits, npat, nmod, words = synth.intern_tables(w, a)
@@ -102,31 +174,33 @@ def main():
                     e.update_workers(up, na, nb)
             rows[k].append(timed(inc, INCR))
             if k not in checked:   # the sibling's full pass on the same tables: every array equal
-                r = inc.fetch()
-                ref.match(LEAN)
-                q = ref.fetch()
-                same = all(np.array_equal(getattr(r, f), getattr(q, f)) for f in FIELDS)
+                _, same = same_as_full(inc, ref)
                 if not same:
                     raise SystemExit(f"k={k}: the incremental result differs from the full pass")
                 checked.add(k)
-    summary = []
-    for key, rs in rows.items():
-        summary.append({"k": key, "ms_device_median": float(np.median([r["ms_device"] for r in rs])),
-                        "ms_host_median": float(np.median([r["ms_host"] for r in rs])),
-                        "evals": int(rs[-1]["evals"]), "n_tiles": int(rs[-1]["n_tiles"]), "runs": len(rs)})
-    out = {"workload": f"{T} asks x {W} workers (synth mixed), first fit, fused lean", "card": env,
-           "checked_equal_to_full_pass": sorted(checked), "rows": summary}
-    print(f"{env.get('name')}  power limit {env.get('power_limit_w')} W  SM {env.get('sm_mhz')}/{env.get('sm_max_mhz')} MHz")
-    print(f"{'k':>8} {'device ms':>10} {'host ms':>9} {'evals':>16} {'n_tiles':>9}")
-    for s in summary:
-        print(f"{s['k']:>8} {s['ms_device_median']:>10.3f} {s['ms_host_median']:>9.3f} {s['evals']:>16} {s['n_tiles']:>9}")
-    print(json.dumps(out))
-    if args.out:
-        os.makedirs(args.out, exist_ok=True)
-        with open(os.path.join(args.out, "incremental_bench.json"), "w") as f:
-            json.dump(out, f, indent=1)
     for e in engines:
         e.close()
+    report(rows, checked, f"{T} asks x {W} workers (synth mixed), first fit, fused lean", env, "k", args.out,
+           "incremental_bench.json")
+
+
+def report(rows, checked, workload, env, key_name, out_dir, file_name):
+    summary = []
+    for key, rs in rows.items():
+        summary.append({key_name: key, "ms_device_median": float(np.median([r["ms_device"] for r in rs])),
+                        "ms_host_median": float(np.median([r["ms_host"] for r in rs])),
+                        "evals": int(rs[-1]["evals"]), "n_tiles": int(rs[-1]["n_tiles"]), "runs": len(rs),
+                        **{k: rs[-1][k] for k in ("n_off", "n_on") if k in rs[-1]}})
+    out = {"workload": workload, "card": env, "checked_equal_to_full_pass": sorted(checked), "rows": summary}
+    print(f"{env.get('name')}  power limit {env.get('power_limit_w')} W  SM {env.get('sm_mhz')}/{env.get('sm_max_mhz')} MHz")
+    print(f"{key_name:>8} {'device ms':>10} {'host ms':>9} {'evals':>16} {'n_tiles':>9}")
+    for s in summary:
+        print(f"{s[key_name]:>8} {s['ms_device_median']:>10.3f} {s['ms_host_median']:>9.3f} {s['evals']:>16} {s['n_tiles']:>9}")
+    print(json.dumps(out))
+    if out_dir:
+        os.makedirs(out_dir, exist_ok=True)
+        with open(os.path.join(out_dir, file_name), "w") as f:
+            json.dump(out, f, indent=1)
 
 
 if __name__ == "__main__":
