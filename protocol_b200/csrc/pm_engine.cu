@@ -288,7 +288,7 @@ struct pm_engine {
   }
   int tune_argmin = 0, tune_generic = 0, tune_build = 0, tune_auction = 0, tune_prox = 0, tune_auc_good = 0, tune_auc_extra = 0;   // PM_TUNE_*: kernel-shape experiments
   int tune_compress = 1;  // PM_TUNE_COMPRESS=0: the cost tile in plain cudaMalloc memory (A/B runs)
-  int tune_pipe = 16;     // PM_TUNE_PIPE: rows per band of pm_build_argmin (8 / 16 / 32 / 64); 0: build + argmin launches
+  bool tune_pipe = true;  // PM_TUNE_PIPE=0: the separate build + argmin launches instead of pm_build_argmin
   DevBuf<uint4> wa, wb;
   DevBuf<double> lat, lon;
   DevBuf<uint32_t> addr_rank;
@@ -317,6 +317,8 @@ struct pm_engine {
   TileBuf cost;
   DevBuf<uint32_t> first_ask, ask_count;
   DevBuf<long long> ask_best;
+  DevBuf<uint32_t> stripe_rank;        // pm_stripe_rank, once per pass of pm_build_argmin: [ld] column -> rank in its stripe
+  DevBuf<long long> rank_best;         // ... [ld] stripe * 1024 + rank -> (price << 32) | worker
 
   // The stored evaluation of PM_INCREMENTAL: the per-worker first feasible ask of the last evaluation, in its own
   // buffer (first_ask is the resolution's working copy: the sweeps and the auction overwrite it), and the worker rows
@@ -600,10 +602,8 @@ int pm_create(const pm_cfg* cfg, pm_engine** out) try {
   if (const char* t = std::getenv("PM_TUNE_PROX")) e->tune_prox = std::atoi(t);   // 0: all-SM cooperative sweep; 2: single-CTA sweep; 1: latitude-banded single-CTA sweep (experimental)
   if (const char* t = std::getenv("PM_TUNE_COMPRESS")) e->tune_compress = std::atoi(t);
   if (const char* t = std::getenv("PM_TUNE_INCR")) e->tune_incr = (uint32_t)std::strtoul(t, nullptr, 10);   // 0: always full
-  if (const char* t = std::getenv("PM_TUNE_PIPE")) {   // other values keep the default band
-    const int v = std::atoi(t);
-    if (v == 0 || v == 8 || v == 16 || v == 32 || v == 64) e->tune_pipe = v;
-  }
+  // any other value (8 / 16 / 32 / 64 set the rows per band of an earlier read-back) keeps the one launch
+  if (const char* t = std::getenv("PM_TUNE_PIPE")) e->tune_pipe = std::atoi(t) != 0;
   bool ok = cudaSetDevice(e->device) == cudaSuccess;
   if (ok && cfg->stream) {
     e->stream = (cudaStream_t)cfg->stream;  // caller's stream (e.g. torch's current stream)
@@ -633,6 +633,7 @@ void pm_destroy(pm_engine* e) {
   e->scratch_idx.release(); e->scratch_flags.release();
   e->upd_a.release(); e->upd_b.release(); e->upd_lat.release(); e->upd_lon.release();
   e->cost.release(); e->first_ask.release(); e->ask_count.release(); e->ask_best.release();
+  e->stripe_rank.release(); e->rank_best.release();
   e->eval_first.release(); e->h_dirty.release(); e->dirty_dev.release(); e->incr_evals.release();
   e->walk_start.release(); e->toggle_dev.release();
   e->keys.release(); e->keys_sorted.release(); e->iota.release(); e->order.release();
@@ -1146,16 +1147,16 @@ static void launch_fused(pm_engine* e, const pm::EvalParams& p, int bits_mode, b
 #undef PM_FUSED_CASE
 }
 
-// pm_build_argmin: the 32-bit tile's build and argmin in one launch (PM_TUNE_PIPE rows per band)
+// pm_build_argmin: the 32-bit tile's build and argmin in one launch (the stripe ranks of pm_stripe_rank in place)
 static void launch_build_argmin(pm_engine* e, const pm::EvalParams& p, int bits_mode, uint32_t t0, uint32_t nt, uint32_t w0,
                                 uint32_t nw, long long* tile, size_t ld) {
   const dim3 grid(blocks_for(ld, pm::kEvalCols), blocks_for(nt, pm::kFastRows));
-  const pm::BandOut bo{(uint32_t)e->tune_pipe, e->first_ask.p, e->ask_best.p, e->ask_count.p};
+  const pm::FoldOut fo{e->stripe_rank.p, e->rank_best.p, e->first_ask.p, e->ask_best.p, e->ask_count.p};
   uint32_t* t32 = reinterpret_cast<uint32_t*>(tile);
   if (p.words == 1) bits_mode = 2;   // one-word acceptance rows are bound into the FastRows, as in launch_build
-  if (bits_mode == 2) pm::pm_build_argmin<2><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, t0, nt, w0, nw, t32, ld, bo);
-  else if (bits_mode == 1) pm::pm_build_argmin<1><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, t0, nt, w0, nw, t32, ld, bo);
-  else pm::pm_build_argmin<0><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, t0, nt, w0, nw, t32, ld, bo);
+  if (bits_mode == 2) pm::pm_build_argmin<2><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, t0, nt, w0, nw, t32, ld, fo);
+  else if (bits_mode == 1) pm::pm_build_argmin<1><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, t0, nt, w0, nw, t32, ld, fo);
+  else pm::pm_build_argmin<0><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, t0, nt, w0, nw, t32, ld, fo);
 }
 
 static void launch_argmin(pm_engine* e, cudaStream_t st, bool narrow, const long long* tile, size_t ld, uint32_t nt,
@@ -1388,7 +1389,14 @@ static int match_local_locked(pm_engine* e, uint32_t mode) {
       }
       // One launch per tile (pm_build_argmin) wherever the 32-bit tile runs, unless PM_TUNE_PIPE=0 or a rows-per-CTA
       // experiment (PM_TUNE_BUILD=5 / 6) asks for the separate build and argmin
-      const bool pipe = narrow && e->tune_pipe != 0 && e->tune_build != 5 && e->tune_build != 6;
+      const bool pipe = narrow && e->tune_pipe && e->tune_build != 5 && e->tune_build != 6;
+      if (pipe) {   // each column's rank within its stripe, from this pass's prices (ordered after any table update)
+        PM_CUDA(e->stripe_rank.ensure(ld));
+        PM_CUDA(e->rank_best.ensure(ld));
+        pm::pm_stripe_rank<<<(unsigned)(ld / pm::kEvalCols), pm::kEvalThreads, 0, e->stream>>>(e->wb.p, w0, nw, e->stripe_rank.p,
+                                                                                               e->rank_best.p);
+        PM_LAUNCH_CHECK("pm_stripe_rank");
+      }
       long long* tile = e->cost.p;
       for (uint32_t t0 = 0; t0 < T; t0 += (uint32_t)rows) {
         const uint32_t nt = (uint32_t)std::min<uint64_t>(rows, T - t0);

@@ -13,6 +13,7 @@
 // crates/orchestrator/src/plugins/node_groups/mod.rs:478-628.
 #pragma once
 #include <type_traits>
+#include <cub/block/block_radix_sort.cuh>
 #include "pm_device.cuh"
 
 namespace pm {
@@ -350,7 +351,7 @@ __device__ __forceinline__ void eval_fast_more(const DevOptF* __restrict__ gopts
 
 template <int ROWS>
 struct __align__(128) FastStage {
-  FastRow row[ROWS + 2];   // + 2: the look-ahead loads of the band's last pair of rows may read past it (never used)
+  FastRow row[ROWS + 2];   // + 2: the look-ahead loads of the last pair of rows may read past it (never used)
   uint32_t bits[kBitsCap];
   uint64_t bar;
 };
@@ -364,10 +365,11 @@ constexpr int kFastRows = 512;   // asks per CTA: the prologue (worker rows from
 // contiguous.  Only for tables whose every price is below kNarrowInfeasible (pm_check_worker_ranges): at that price a
 // feasible worker could not be told from the sentinel, and at >= 2^31 the wide tile's signed order differs.
 //
-// PIPE (pm_build_argmin, narrow only): the CTA also reduces what it wrote, band by band — see there.  `bo` is unused
-// otherwise.
-struct BandOut {
-  uint32_t band;                 // rows per band, even
+// PIPE (pm_build_argmin, narrow only): the CTA also folds each row's minimum and feasible count from the registers it
+// stores — see there.  `fo` is unused otherwise.
+struct FoldOut {
+  const uint32_t* rank;            // [ld] each column's rank within its 1024-column stripe (pm_stripe_rank)
+  const long long* best_of_rank;   // [ld] stripe s, rank ρ at s * 1024 + ρ: that column's (price << 32) | (w0 + column)
   uint32_t* first_ask;
   long long* ask_best;
   uint32_t* ask_count;
@@ -375,9 +377,15 @@ struct BandOut {
 
 template <int BITS, int ROWS, bool NARROW, bool PIPE>
 __device__ __forceinline__ void build_fast(const EvalParams& p, uint32_t t0, uint32_t nt, uint32_t w0, uint32_t nw,
-                                           void* __restrict__ tile, size_t ld, const BandOut& bo) {
-  static_assert(!PIPE || NARROW, "the banded read-back folds the 32-bit tile");
+                                           void* __restrict__ tile, size_t ld, const FoldOut& fo) {
+  static_assert(!PIPE || NARROW, "the row fold ranks the 32-bit tile's columns");
   __shared__ FastStage<ROWS> s;
+  // PIPE: per warp and row of the CTA, the warp's least key (the least stripe rank of its feasible columns, or
+  // kNoRank and more when it has none) and its infeasible columns — plain stores, no atomics; 12 KB at 512 rows
+  constexpr int kWarps = kEvalThreads / 32;
+  constexpr uint32_t kNoRank = 0x8000u;   // added to an infeasible column's rank (< 1024): the key still fits 16 bits
+  __shared__ uint16_t s_key[PIPE ? kWarps : 1][PIPE ? ROWS : 1];
+  __shared__ uint8_t s_nb[PIPE ? kWarps : 1][PIPE ? ROWS : 1];
   const uint32_t r0 = blockIdx.y * ROWS;
   const uint32_t nrows = min(nt - r0, (uint32_t)ROWS);
   if (threadIdx.x == 0) {
@@ -410,12 +418,24 @@ __device__ __forceinline__ void build_fast(const EvalParams& p, uint32_t t0, uin
   size_t row_stride = NARROW ? ld / 4 : ld / 2;   // in 16-byte units
   asm("" : "+l"(row_stride));           // held in registers: ptxas would otherwise re-derive it from `ld` every row
   const uint32_t sh = p.sign_shift;
-  uint32_t cm[kEvalWPT];                // PIPE: per column, the first feasible ask so far (kNone: none yet)
+  // PIPE: per column, the first feasible ask so far — the least of ask | fail's sign bit (asks are below 2^31): >= 2^31
+  // while there is none
+  uint32_t cm[kEvalWPT];
 #pragma unroll
   for (int k = 0; k < kEvalWPT; ++k) cm[k] = kNone;
-  // One row.  The ask's scalar thresholds are OR-ed into the first option's clauses before the further OR-options are
-  // AND-ed in — fail = AND_o(u_o | s) = (AND_o u_o) | s — so a single-option row is one 7-term OR per worker.
-  auto emit = [&](const FastRow& q, uint4* dst, uint32_t t) {
+  const uint32_t t_cta = t0 + r0;       // PIPE: the ask of the CTA's first row
+  uint32_t rk[kEvalWPT];                // PIPE: per column, its rank within the stripe
+  uint32_t key_slot = 0, nb_slot = 0;   // PIPE: the warp's row 0 in s_key / s_nb (shared-window addresses)
+  if constexpr (PIPE) {
+    const uint4 v = __ldg(reinterpret_cast<const uint4*>(fo.rank + cbase));
+    rk[0] = v.x; rk[1] = v.y; rk[2] = v.z; rk[3] = v.w;
+    key_slot = (uint32_t)__cvta_generic_to_shared(&s_key[threadIdx.x >> 5][0]);
+    nb_slot = (uint32_t)__cvta_generic_to_shared(&s_nb[threadIdx.x >> 5][0]);
+    asm("" : "+r"(key_slot), "+r"(nb_slot));   // held in registers: ptxas would otherwise re-derive them every row
+  }
+  // One row (`r` of the CTA).  The ask's scalar thresholds are OR-ed into the first option's clauses before the further
+  // OR-options are AND-ed in — fail = AND_o(u_o | s) = (AND_o u_o) | s — so a single-option row is one 7-term OR per worker.
+  auto emit = [&](const FastRow& q, uint4* dst, uint32_t r) {
     uint32_t f[kEvalWPT], sc[kEvalWPT];
     eval_fast_first<kEvalWPT, BITS>(q, s.bits, w, p.bits, p.words, f);
 #pragma unroll
@@ -432,6 +452,7 @@ __device__ __forceinline__ void build_fast(const EvalParams& p, uint32_t t0, uin
       for (int k = 0; k < kEvalWPT; ++k) f[k] &= um[k] | sc[k];
     }
     uint32_t o[2 * kEvalWPT];
+    uint32_t key = kNone, nb = 0;       // PIPE: the lane's least key and its infeasible columns
 #pragma unroll
     for (int k = 0; k < kEvalWPT; ++k) {
       const uint32_t b = f[k] >> sh;                                    // 1 when infeasible (sh == 31)
@@ -441,15 +462,24 @@ __device__ __forceinline__ void build_fast(const EvalParams& p, uint32_t t0, uin
         o[2 * k] = b * dx[k] + gw[k];                                   // feasible: (price << 32) | worker
         o[2 * k + 1] = b * dy[k] + w[k].price;                          // infeasible: 0x7FFFFFFF_FFFFFFFF
       }
-      if (PIPE) cm[k] = min(cm[k], t | (uint32_t)((int32_t)f[k] >> sh));   // t when feasible, else kNone
+      if (PIPE) {
+        cm[k] = min(cm[k], (t_cta + r) | (f[k] & 0x80000000u));        // the ask, + 2^31 when infeasible
+        key = min(key, b * kNoRank + rk[k]);                            // the rank, + kNoRank when infeasible
+        nb += b;
+      }
     }
-    if (PIPE) {
-      *dst = make_uint4(o[0], o[1], o[2], o[3]);                        // default policy: stays in L2 for the read-back
-    } else if (NARROW) {
+    if (NARROW) {
       __stcs(dst, make_uint4(o[0], o[1], o[2], o[3]));
     } else {
       __stcs(dst, make_uint4(o[0], o[1], o[2], o[3]));
       __stcs(dst + 32, make_uint4(o[4], o[5], o[6], o[7]));     // + 64 columns
+    }
+    if (PIPE) {   // the warp's 128 columns: one reduction each, kept in the warp's slot of the row
+      key = __reduce_min_sync(0xffffffffu, key);
+      nb = __reduce_add_sync(0xffffffffu, nb);
+      // every lane stores the same value to the same address: one store each, without a branch around lane 0
+      asm volatile("st.shared.u16 [%0], %1;" ::"r"(key_slot + 2u * r), "r"(key) : "memory");
+      asm volatile("st.shared.u8 [%0], %1;" ::"r"(nb_slot + r), "r"(nb) : "memory");
     }
   };
   __syncthreads();            // mbarrier initialised, acceptance words staged
@@ -458,83 +488,81 @@ __device__ __forceinline__ void build_fast(const EvalParams& p, uint32_t t0, uin
   // ahead, into registers the previous row has finished with, so no row is copied from one buffer to another.
   const FastRow* q = s.row;
   FastRow a = q[0];
-  if constexpr (!PIPE) {
-    for (uint32_t r = 0; r < nrows; r += 2, q += 2) {
-      const FastRow b = q[1];                 // in flight while row r is evaluated
-      emit(a, out, 0u);
-      a = q[2];                               // in flight while row r + 1 is evaluated
-      if (r + 1 < nrows) emit(b, out + row_stride, 0u);
-      out += 2 * row_stride;
-    }
-  } else {
-    const uint32_t warp = threadIdx.x >> 5;
-    const uint32_t c0 = blockIdx.x * kEvalCols;                  // the CTA's first column
-    const uint4* band_in = reinterpret_cast<const uint4*>(static_cast<const uint32_t*>(tile) + (size_t)r0 * ld + c0) + lane;
-    for (uint32_t b0 = 0; b0 < nrows; b0 += bo.band) {
-      const uint32_t b1 = min(nrows, b0 + bo.band);
-      for (uint32_t r = b0; r < b1; r += 2, q += 2) {           // the band is even: pairs never straddle two bands
-        const FastRow b = q[1];
-        emit(a, out, t0 + r0 + r);
-        a = q[2];
-        if (r + 1 < b1) emit(b, out + row_stride, t0 + r0 + r + 1);
-        out += 2 * row_stride;
+  for (uint32_t r = 0; r < nrows; r += 2, q += 2) {
+    const FastRow b = q[1];                   // in flight while row r is evaluated
+    emit(a, out, r);
+    a = q[2];                                 // in flight while row r + 1 is evaluated
+    if (r + 1 < nrows) emit(b, out + row_stride, r + 1);
+    out += 2 * row_stride;
+  }
+  if constexpr (PIPE) {
+    __syncthreads();                          // every warp has written its slot of every row
+    const long long* best = fo.best_of_rank + blockIdx.x * kEvalCols;
+    for (uint32_t i = threadIdx.x; i < nrows; i += kEvalThreads) {
+      uint32_t key = kNone, nb = 0;
+#pragma unroll
+      for (int j = 0; j < kWarps; ++j) {
+        key = min(key, (uint32_t)s_key[j][i]);
+        nb += s_nb[j][i];
       }
-      __syncthreads();                        // the band's stores are visible to every thread of the CTA
-      // A warp takes whole rows of the CTA's 1024 columns: load j holds columns j * 128 + 4 * lane .. + 3 (warp j's
-      // slice of the build), so a lane's columns arrive in increasing order and a strict "<" keeps the first of its
-      // least words, as pm_argmin<.., true> does.
-      for (uint32_t r = b0 + warp; r < b1; r += kEvalThreads / 32) {
-        const uint4* rowp = band_in + (size_t)r * row_stride;
-        uint4 v[kEvalCols / 128];
-#pragma unroll
-        for (int j = 0; j < kEvalCols / 128; ++j) v[j] = __ldcs(rowp + j * 32);   // read once: evict first
-        uint32_t bw = kNarrowInfeasible, bc = 0, cnt = 0;
-#pragma unroll
-        for (int j = 0; j < kEvalCols / 128; ++j) {
-          const uint32_t x[4] = {v[j].x, v[j].y, v[j].z, v[j].w};
-#pragma unroll
-          for (int c = 0; c < 4; ++c) {
-            cnt += (uint32_t)(x[c] != kNarrowInfeasible);
-            if (x[c] < bw) { bw = x[c]; bc = j * 128 + c; }
-          }
-        }
-        // the row's least word, then the least column holding it: the least packed (word << 32) | column
-        cnt = __reduce_add_sync(0xffffffffu, cnt);
-        const uint32_t wmin = __reduce_min_sync(0xffffffffu, bw);
-        const uint32_t cmin = __reduce_min_sync(0xffffffffu, bw == wmin ? bc + lane * 4u : kNone);
-        if (lane == 0 && cnt) {
-          const uint32_t t = t0 + r0 + r;
-          atomicMin(bo.ask_best + t, (long long)(((unsigned long long)wmin << 32) | (w0 + c0 + cmin)));
-          atomicAdd(bo.ask_count + t, cnt);
-        }
+      if (nb < (uint32_t)kEvalCols) {         // a feasible column: key is its least rank
+        atomicMin(fo.ask_best + t_cta + i, __ldg(best + key));
+        atomicAdd(fo.ask_count + t_cta + i, kEvalCols - nb);
       }
     }
 #pragma unroll
     for (int k = 0; k < kEvalWPT; ++k)
-      if (cm[k] != kNone && cbase + k < nw) atomicMin(bo.first_ask + w0 + cbase + k, cm[k]);
+      if (cm[k] < 0x80000000u && cbase + k < nw) atomicMin(fo.first_ask + w0 + cbase + k, cm[k]);
   }
 }
 
 template <int BITS, int ROWS = kFastRows, bool NARROW = false>
 __global__ void __launch_bounds__(kEvalThreads, 2)
 pm_build_cost_fast(EvalParams p, uint32_t t0, uint32_t nt, uint32_t w0, uint32_t nw, void* __restrict__ tile, size_t ld) {
-  build_fast<BITS, ROWS, NARROW, false>(p, t0, nt, w0, nw, tile, ld, BandOut{});
+  build_fast<BITS, ROWS, NARROW, false>(p, t0, nt, w0, nw, tile, ld, FoldOut{});
 }
 
 // ------------------------------------------------------------------ build + argmin, one kernel
-// pm_build_cost_fast<BITS, kFastRows, true> followed by pm_argmin<.., true>, without the second pass over HBM.  The CTA
-// walks its 512 rows in bands of bo.band rows: it evaluates and stores a band exactly as the build does (but with the
-// default store policy, so the lines stay in L2), waits at a barrier, and reads the band straight back with
-// evict-first loads while the lines are still in L2.  The tile bytes written and not yet read are at most
-// (resident CTAs) x band x 4 KB — 17 MB at 264 CTAs and 16 rows — well inside the 50 MB L2; the tile itself still
-// streams through HBM as the stores write back.  The outputs are pm_argmin's, bit for bit: per row and CTA one
-// (least word, least column) from three warp reductions, merged with atomicMin / atomicAdd; per column the first
-// feasible ask from the sign bit the build already holds, flushed once per CTA.
+// pm_build_cost_fast<BITS, kFastRows, true> and pm_argmin<.., true>'s outputs in one pass: the tile is written with
+// streaming stores, as the build writes it, and never read back.  Within a 1024-column stripe the packed minimum
+// (word << 32) | (w0 + column) over the feasible columns orders them by (price, column) whatever the ask, so a
+// column's rank in that order (pm_stripe_rank, once per pass) stands for its packed cost.  Per row and lane the
+// fold is one multiply-add per column on the fail bit the store already formed — key = b * kNoRank + rank — the
+// least of the 4 keys and the sum of the bits; per warp one min and one add reduction, stored in the warp's slot of
+// the row (no atomics, no barrier in the row loop).  At the end of the CTA each row with a feasible column merges
+// best_of_rank[its least rank] into ask_best (atomicMin) and its count into ask_count; per column the first feasible
+// ask, kept from the same sign bit, is flushed once.  The outputs are pm_argmin's bit for bit.
 template <int BITS>
 __global__ void __launch_bounds__(kEvalThreads, 2)
 pm_build_argmin(EvalParams p, uint32_t t0, uint32_t nt, uint32_t w0, uint32_t nw, uint32_t* __restrict__ tile, size_t ld,
-                BandOut bo) {
-  build_fast<BITS, kFastRows, true, true>(p, t0, nt, w0, nw, tile, ld, bo);
+                FoldOut fo) {
+  build_fast<BITS, kFastRows, true, true>(p, t0, nt, w0, nw, tile, ld, fo);
+}
+
+// One CTA per 1024-column stripe of a tile with leading dimension ld: sorts the stripe's (price, column) pairs —
+// the order of the packed cost (price << 32) | (w0 + column) — and writes rank[c], each column's place in that order
+// (padding columns at or past nw last), and best_of_rank[stripe * 1024 + ρ], the packed cost of the column at place
+// ρ (kInf for padding, which is never feasible).  Prices are below 2^31 wherever the 32-bit tile runs, so a key is
+// (price << 10) | column in 41 bits.
+__global__ void __launch_bounds__(kEvalThreads)
+pm_stripe_rank(const uint4* __restrict__ wb, uint32_t w0, uint32_t nw, uint32_t* __restrict__ rank,
+               long long* __restrict__ best_of_rank) {
+  using Sort = cub::BlockRadixSort<unsigned long long, kEvalThreads, kEvalWPT>;
+  __shared__ typename Sort::TempStorage tmp;
+  const uint32_t c0 = blockIdx.x * kEvalCols;
+  unsigned long long key[kEvalWPT];
+#pragma unroll
+  for (int k = 0; k < kEvalWPT; ++k) {
+    const uint32_t c = threadIdx.x * kEvalWPT + k;
+    key[k] = c0 + c < nw ? ((unsigned long long)__ldg(&wb[w0 + c0 + c].w) << 10) | c : (1ull << 41) | c;
+  }
+  Sort(tmp).Sort(key, 0, 42);   // blocked: thread i holds places 4i .. 4i + 3
+#pragma unroll
+  for (int k = 0; k < kEvalWPT; ++k) {
+    const uint32_t rho = threadIdx.x * kEvalWPT + k, c = (uint32_t)key[k] & (kEvalCols - 1);
+    rank[c0 + c] = rho;
+    best_of_rank[c0 + rho] = key[k] >> 41 ? kInf : (long long)(((key[k] >> 10) << 32) | (w0 + c0 + c));
+  }
 }
 
 // Worker-major acceptance: bit r of nacc[w] is set when pattern row r rejects worker w's model (row 0 never does).

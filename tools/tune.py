@@ -77,9 +77,8 @@ if __name__ == "__main__":
     for v in os.environ.get("TUNE_BUILD", "8").split(","):   # 8: the int64 tile on the FastRow path
         if v:
             variants.append({"PM_TUNE_BUILD": v})
-    # rows per band of the one-launch build + argmin; 0: the two launches.  The band's tile bytes in flight are
-    # (resident CTAs) x rows x 4 KB, so the time should jump once that passes L2
-    for v in os.environ.get("TUNE_PIPE", "0,8,16,32,64").split(","):
+    # 0: the separate build and argmin launches, against the one-launch build + argmin of the default run above
+    for v in os.environ.get("TUNE_PIPE", "0").split(","):
         if v:
             variants.append({"PM_TUNE_PIPE": v})
     for env in variants:
