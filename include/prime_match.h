@@ -269,24 +269,37 @@ enum pm_path {
                                     valid stored evaluation or more rows changed than the cutoff (PM_TUNE_INCR at
                                     pm_create).  Every array pm_fetch_result returns equals the same call's without the
                                     flag (ask_best = PM_COST_INF, ask_count = 0).  Valid with PM_PATH_FUSED |
-                                    PM_NO_ASK_STATS and a reference mode only (else PM_E_INVALID); PM_E_UNSUPPORTED on a
-                                    sharded engine or one with a communicator attached.  See "Incremental passes" below */
+                                    PM_NO_ASK_STATS and a reference mode only (else PM_E_INVALID).  Works on a sharded
+                                    engine through pm_match_local and with a communicator attached (pm_comm, pm_multi);
+                                    PM_E_UNSUPPORTED from pm_match on a shard engine without a communicator.  See
+                                    "Incremental passes" below */
 };
 
-/* Incremental passes (PM_INCREMENTAL).  Every full evaluation of an unsharded engine, with the flag or without, keeps
- * a copy of its per-worker result.  A row becomes "written" through pm_upsert_workers (the range), pm_update_workers
- * and pm_set_flags (the in-range indices, each once) and pm_resize_workers (the rows past the old end).
+/* Incremental passes (PM_INCREMENTAL).  Every full evaluation, with the flag or without, keeps a copy of its
+ * per-worker result over the engine's range: the whole table, the pm_cfg / pm_set_shard range, or with a communicator
+ * the rank's equal share; PM_NONE outside it (a communicator engine takes the copy before the exchange).  A row becomes
+ * "written" through pm_upsert_workers (the range), pm_update_workers and pm_set_flags (the in-range indices, each once)
+ * and pm_resize_workers (the rows past the old end).  An incremental pass re-evaluates the written rows inside the
+ * engine's range only; the others still count for the O(W) checks of the replicated table.  A communicator's share
+ * (ceil(W / N) per rank) moves when pm_resize_workers changes W: rows that enter a rank's range count as written there,
+ * rows that leave it return to PM_NONE.  A fixed pm_set_shard range does not move; a shrink that cuts into it fails at
+ * the next pass (PM_E_INVALID), as without the flag.
  * pm_set_worker_locations, pm_set_worker_addr_rank and pm_set_worker_reputation write nothing the predicate reads.
  * pm_set_asks, pm_set_model_table, pm_set_worker_count, pm_set_shard, pm_attach_comm and a pass that fails discard the
  * stored evaluation.  Without the flag pm_match evaluates every pair as before.
+ * pm_match on a shard engine without a communicator refuses the flag (PM_E_UNSUPPORTED): that call resolves one range
+ * as if it were the table, so it has no whole-table result to keep incremental.  pm_match_local takes it on any engine.
  * pm_set_ask_enabled keeps the stored evaluation: the next incremental pass also walks the workers whose stored first
  * ask was disabled since ("orphans", from the ask after it) and evaluates every worker against the asks enabled since
  * (only those whose stored first ask lies beyond the first of them; an ask switched off and on again counts as
- * neither).  With many asks enabled the pass evaluates everything instead: the pairs of that walk, |E| x W, count as
- * |E| x W / T written rows against the PM_TUNE_INCR cutoff.  pm_stats under the flag:
- *   evals    pair evaluations executed: T x W on a full evaluation; on an incremental one the kernels' own count over
- *            the three walks (written rows, orphans, newly enabled asks); 0 when no row and no mask changed;
- *   n_tiles  worker rows walked in full: W on a full evaluation, else written rows + orphans.                      */
+ * neither).  With many asks enabled the pass evaluates everything instead: the pairs of that walk, |E| x nw, count as
+ * |E| x nw / T written rows against the PM_TUNE_INCR cutoff, next to the range's written rows.  Each engine decides
+ * against the cutoff by its own range's counts, so in one sharded pass some ranks may evaluate their range in full
+ * while others run incrementally; every rank still makes the one exchange.  pm_stats under the flag (nw = the range's
+ * workers, W on an unsharded engine):
+ *   evals    pair evaluations executed: T x nw on a full evaluation; on an incremental one the kernels' own count over
+ *            the three walks (written rows, orphans, newly enabled asks) in the range; 0 when no row and no mask changed;
+ *   n_tiles  worker rows walked in full: nw on a full evaluation, else the range's written rows + orphans.         */
 
 typedef struct pm_stats {
   uint64_t evals;            /* predicate evaluations executed on the device        */
@@ -386,6 +399,11 @@ int pm_multi_upsert_workers(pm_multi*, const pm_worker_a* a, const pm_worker_b* 
 int pm_multi_set_worker_locations(pm_multi*, const double* lat, const double* lon, uint32_t first, uint32_t n);
 int pm_multi_set_worker_addr_rank(pm_multi*, const uint32_t* rank, uint32_t first, uint32_t n);
 int pm_multi_set_flags(pm_multi*, const uint32_t* idx, const uint32_t* flags, uint32_t n);
+/* the resident-table deltas (pm_resize_workers, pm_update_workers) on every device: with them the management loop
+ * runs PM_INCREMENTAL through pm_multi_match, each device re-evaluating only its share's written rows */
+int pm_multi_resize_workers(pm_multi*, uint32_t n_workers);
+int pm_multi_update_workers(pm_multi*, const uint32_t* idx, const pm_worker_a* a, const pm_worker_b* b, const double* lat,
+                            const double* lon, uint32_t n);
 int pm_multi_sync(pm_multi*);
 int pm_multi_match(pm_multi*, uint32_t mode);
 int pm_multi_fetch_result(pm_multi*, pm_result* out);

@@ -91,6 +91,8 @@ def load() -> C.CDLL:
         "pm_multi_set_worker_locations": (i32, [vp, vp, vp, u32, u32]),
         "pm_multi_set_worker_addr_rank": (i32, [vp, vp, u32, u32]),
         "pm_multi_set_flags": (i32, [vp, vp, vp, u32]),
+        "pm_multi_resize_workers": (i32, [vp, u32]),
+        "pm_multi_update_workers": (i32, [vp, vp, vp, vp, vp, vp, u32]),
         "pm_multi_sync": (i32, [vp]),
         "pm_multi_match": (i32, [vp, u32]),
         "pm_multi_fetch_result": (i32, [vp, P(abi.PmResult)]),

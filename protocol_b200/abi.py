@@ -119,7 +119,8 @@ EXPORTS = [
     "pm_comm_unique_id", "pm_comm_create", "pm_comm_destroy", "pm_attach_comm",
     "pm_multi_create", "pm_multi_destroy", "pm_multi_size", "pm_multi_engine", "pm_multi_last_error",
     "pm_multi_set_asks", "pm_multi_set_ask_enabled", "pm_multi_set_model_table", "pm_multi_set_worker_count", "pm_multi_upsert_workers",
-    "pm_multi_set_worker_locations", "pm_multi_set_worker_addr_rank", "pm_multi_set_flags", "pm_multi_sync",
+    "pm_multi_set_worker_locations", "pm_multi_set_worker_addr_rank", "pm_multi_set_flags",
+    "pm_multi_resize_workers", "pm_multi_update_workers", "pm_multi_sync",
     "pm_multi_match", "pm_multi_fetch_result",
     "pm_plugin_create", "pm_plugin_destroy", "pm_plugin_last_error", "pm_plugin_add_config", "pm_plugin_seal_configs",
     "pm_plugin_enable_configuration", "pm_plugin_upsert_node", "pm_plugin_set_node_status", "pm_plugin_sync_discovery", "pm_plugin_sync_discovery_json", "pm_plugin_get_node", "pm_plugin_add_task",

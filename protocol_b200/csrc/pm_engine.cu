@@ -320,15 +320,20 @@ struct pm_engine {
   DevBuf<uint32_t> stripe_rank;        // pm_stripe_rank, once per pass of pm_build_argmin: [ld] column -> rank in its stripe
   DevBuf<long long> rank_best;         // ... [ld] stripe * 1024 + rank -> (price << 32) | worker
 
-  // The stored evaluation of PM_INCREMENTAL: the per-worker first feasible ask of the last evaluation, in its own
-  // buffer (first_ask is the resolution's working copy: the sweeps and the auction overwrite it), and the worker rows
-  // written since then.  Rows are tracked on the host, where their indices arrive: a mark per row, the list of marked
-  // rows, and `dirty_over` once more rows changed than an incremental pass would take (tune_incr).
+  // The stored evaluation of PM_INCREMENTAL: the per-worker first feasible ask of the last evaluation of this engine's
+  // range (shard()), PM_NONE outside it, in its own buffer (first_ask is the resolution's working copy: the sweeps, the
+  // exchange and the auction overwrite it), and the worker rows written since then.  Rows are tracked on the host,
+  // where their indices arrive: a mark per row and the list of marked rows.  The list holds every written row of the
+  // range, which the walks re-evaluate, and the written rows outside it, which only the O(W) preludes read (decide_fast,
+  // worker_major: they describe the whole replicated table).  `dirty_over` once more rows of the range changed than
+  // an incremental pass would take (tune_incr); `rows_over` once more rows outside it did: the list then stops taking
+  // them and the preludes check every row.
   DevBuf<uint32_t> eval_first;
   bool eval_valid = false;
   std::vector<uint8_t> dirty_mark;      // [rows of the stored evaluation, grown with the table]; set <=> in dirty_rows
   std::vector<uint32_t> dirty_rows;
-  bool dirty_over = false;
+  uint32_t dirty_in = 0;                // entries of dirty_rows inside the range
+  bool dirty_over = false, rows_over = false;
   bool workers_base = false;            // workers_small / prices_narrow hold for every row outside dirty_rows
   bool nacc_base = false;               // nacc holds every row outside dirty_rows (model table unchanged)
   uint32_t tune_incr = 1u << 18;        // PM_TUNE_INCR: most dirty rows an incremental pass re-evaluates (DESIGN §5)
@@ -358,7 +363,8 @@ struct pm_engine {
   void clear_dirty() {
     for (uint32_t i : dirty_rows) dirty_mark[i] = 0;
     dirty_rows.clear();
-    dirty_over = false;
+    dirty_in = 0;
+    dirty_over = rows_over = false;
   }
   void invalidate_eval() {
     clear_dirty();
@@ -366,16 +372,34 @@ struct pm_engine {
     eval_valid = false;
     workers_base = nacc_base = false;
   }
+  bool in_range(uint32_t i) const {
+    uint32_t w0 = 0, nw = 0;
+    shard(&w0, &nw);
+    return i - w0 < nw;
+  }
   void mark_dirty(uint32_t i) {
     if (!eval_valid || dirty_over || i >= dirty_mark.size() || dirty_mark[i]) return;
+    const bool in = in_range(i);
+    if (!in && rows_over) return;
     dirty_mark[i] = 1;
     dirty_rows.push_back(i);
-    if (dirty_rows.size() > tune_incr) mark_all_dirty();
+    dirty_in += in;
+    if (dirty_in > tune_incr) mark_all_dirty();
+    else if (dirty_rows.size() - dirty_in > tune_incr) rows_over = true;
   }
   void mark_range_dirty(uint32_t first, uint32_t n) {
     if (!eval_valid || dirty_over) return;
-    if (n > tune_incr) { mark_all_dirty(); return; }
-    for (uint32_t i = 0; i < n; ++i) mark_dirty(first + i);
+    uint32_t w0 = 0, nw = 0;
+    shard(&w0, &nw);
+    const uint64_t lo = std::max<uint64_t>(first, w0), hi = std::min<uint64_t>((uint64_t)first + n, (uint64_t)w0 + nw);
+    const uint64_t inside = hi > lo ? hi - lo : 0;
+    if (inside > tune_incr) { mark_all_dirty(); return; }
+    if (n - inside > tune_incr) rows_over = true;   // the rows outside the range are not listed
+    if (rows_over) {
+      for (uint64_t i = lo; i < hi; ++i) mark_dirty((uint32_t)i);
+    } else {
+      for (uint32_t i = 0; i < n; ++i) mark_dirty(first + i);
+    }
   }
   void mark_all_dirty() {   // the next pass evaluates everything
     if (!eval_valid) return;
@@ -932,9 +956,13 @@ int pm_resize_workers(pm_engine* e, uint32_t n_workers) try {
   ++e->table_version;
   PM_CUDA(cudaSetDevice(e->device));
   const size_t keep = e->have_workers ? e->n_workers : 0;
+  uint32_t a0 = 0, na = 0;   // the range before the resize
+  e->shard(&a0, &na);
   if (e->eval_valid) {
-    // the stored evaluation follows the table: kept rows keep their entries, rows past the old end are dirty
+    // the stored evaluation follows the table: kept rows keep their entries, rows past the old end are NONE and dirty
     PM_CUDA(e->eval_first.grow_keep(std::max<uint32_t>(n_workers, 1), keep, e->stream));
+    if (n_workers > keep)
+      PM_CUDA(cudaMemsetAsync(e->eval_first.p + keep, 0xFF, (size_t)(n_workers - keep) * 4, e->stream));
     if (n_workers < keep) {
       size_t j = 0;
       for (uint32_t i : e->dirty_rows) {
@@ -944,7 +972,6 @@ int pm_resize_workers(pm_engine* e, uint32_t n_workers) try {
       e->dirty_rows.resize(j);
     }
     e->dirty_mark.resize(n_workers, 0);
-    if (n_workers > keep) e->mark_range_dirty((uint32_t)keep, n_workers - (uint32_t)keep);
   }
   PM_CUDA(e->wa.grow_keep(std::max<uint32_t>(n_workers, 1), keep, e->stream));
   PM_CUDA(e->wb.grow_keep(std::max<uint32_t>(n_workers, 1), keep, e->stream));
@@ -965,6 +992,28 @@ int pm_resize_workers(pm_engine* e, uint32_t n_workers) try {
     if (e->have_rep) PM_CUDA(cudaMemsetAsync(e->reputation.p + keep, 0, (size_t)(n_workers - keep) * 4, e->stream));
   }
   e->n_workers = n_workers;
+  if (e->eval_valid) {
+    // A communicator's equal share, or an open-ended pm_set_shard range, moves with W.  Rows that leave the range
+    // return to NONE; rows that enter it were evaluated by another rank, or never: they are written.  Each is at most
+    // two intervals.  The rows past the old end are written for the preludes wherever they lie.
+    uint32_t b0 = 0, nb = 0;
+    e->shard(&b0, &nb);
+    const uint64_t a1 = std::min<uint64_t>((uint64_t)a0 + na, n_workers), b1 = (uint64_t)b0 + nb;
+    auto none = [&](uint64_t lo, uint64_t hi) -> cudaError_t {
+      return hi > lo ? cudaMemsetAsync(e->eval_first.p + lo, 0xFF, (size_t)(hi - lo) * 4, e->stream) : cudaSuccess;
+    };
+    PM_CUDA(none(a0, std::min<uint64_t>(a1, b0)));
+    PM_CUDA(none(std::max<uint64_t>(a0, b1), a1));
+    e->dirty_in = 0;
+    for (uint32_t i : e->dirty_rows) e->dirty_in += e->in_range(i);
+    if (e->dirty_in > e->tune_incr) e->mark_all_dirty();
+    auto enter = [&](uint64_t lo, uint64_t hi) {
+      if (hi > lo) e->mark_range_dirty((uint32_t)lo, (uint32_t)(hi - lo));
+    };
+    enter(b0, std::min<uint64_t>(b1, a0));
+    enter(std::max<uint64_t>(b0, (uint64_t)a0 + na), b1);
+    if (n_workers > keep) e->mark_range_dirty((uint32_t)keep, n_workers - (uint32_t)keep);
+  }
   e->have_workers = true;
   e->workers_checked = false;
   e->nacc_valid = false;
@@ -1198,35 +1247,54 @@ static void launch_argmin(pm_engine* e, cudaStream_t st, bool narrow, const long
 //   * after asks were enabled (`en`, E): the E-pass, every worker against E only.  A worker whose f lies below every
 //     ask of E is settled; the others gain min(f, first feasible ask of E).
 // Then the stored copy goes to first_ask, the resolution's working copy.  Same predicate variant as the full pass
-// would pick; the O(W) preludes (operand-range check, worker-major acceptance words) cover the written rows.
+// would pick; the O(W) preludes (operand-range check, worker-major acceptance words) cover every written row, the walks
+// the engine's range [w0, w0 + nw) only: written rows outside it are dropped, orphans are collected inside it and the
+// E-pass walks its workers.
 static int eval_incremental(pm_engine* e, const std::vector<uint32_t>& en, const std::vector<uint32_t>& dis) {
   const uint32_t W = e->n_workers, T = e->n_asks;
-  const uint32_t k = (uint32_t)e->dirty_rows.size();
+  uint32_t w0 = 0, nw = 0;
+  e->shard(&w0, &nw);
+  const uint32_t k = (uint32_t)e->dirty_rows.size(), kr = e->dirty_in;
   const uint32_t ne = (uint32_t)en.size(), nd = (uint32_t)dis.size();
-  e->stats.n_tiles = k;
+  e->stats.n_tiles = kr;
   if (k || ne || nd) {
-    // host staging [written rows | E | D]; device: written rows (then the orphans) in dirty_dev, E and D in toggle_dev
-    PM_CUDA(e->h_dirty.ensure((size_t)k + ne + nd));
-    std::memcpy(e->h_dirty.p, e->dirty_rows.data(), (size_t)k * 4);
-    std::memcpy(e->h_dirty.p + k, en.data(), (size_t)ne * 4);
-    std::memcpy(e->h_dirty.p + k + ne, dis.data(), (size_t)nd * 4);
-    PM_CUDA(e->dirty_dev.ensure(nd ? (size_t)k + W : std::max<size_t>(k, 1)));
+    // host staging [written rows (the preludes' list) | the range's written rows (the walk's list) | E | D]; the two
+    // row lists are one when every written row lies in the range, and the preludes have none after rows_over.
+    // Device: the row lists (then the orphans) in dirty_dev, E and D in toggle_dev
+    const uint32_t kp = e->rows_over ? 0 : k;
+    const bool one_list = kp == kr;
+    const uint32_t kh = kp + (one_list ? 0 : kr);
+    PM_CUDA(e->h_dirty.ensure((size_t)kh + ne + nd));
+    uint32_t* h = e->h_dirty.p;
+    if (one_list && kp) {
+      std::memcpy(h, e->dirty_rows.data(), (size_t)k * 4);
+    } else {
+      std::memcpy(h, e->dirty_rows.data(), (size_t)kp * 4);
+      uint32_t j = kp;
+      for (uint32_t i : e->dirty_rows)
+        if (i - w0 < nw) h[j++] = i;
+    }
+    std::memcpy(h + kh, en.data(), (size_t)ne * 4);
+    std::memcpy(h + kh + ne, dis.data(), (size_t)nd * 4);
+    PM_CUDA(e->dirty_dev.ensure(nd ? (size_t)kh + nw : std::max<size_t>(kh, 1)));
     PM_CUDA(e->toggle_dev.ensure((size_t)ne + nd));
-    if (k) PM_CUDA(cudaMemcpyAsync(e->dirty_dev.p, e->h_dirty.p, (size_t)k * 4, cudaMemcpyHostToDevice, e->stream));
+    if (kh) PM_CUDA(cudaMemcpyAsync(e->dirty_dev.p, h, (size_t)kh * 4, cudaMemcpyHostToDevice, e->stream));
     if (ne + nd)
-      PM_CUDA(cudaMemcpyAsync(e->toggle_dev.p, e->h_dirty.p + k, ((size_t)ne + nd) * 4, cudaMemcpyHostToDevice, e->stream));
+      PM_CUDA(cudaMemcpyAsync(e->toggle_dev.p, h + kh, ((size_t)ne + nd) * 4, cudaMemcpyHostToDevice, e->stream));
+    const uint32_t* pre = e->rows_over ? nullptr : e->dirty_dev.p;   // null: the preludes check every row
+    uint32_t* rows = e->dirty_dev.p + (one_list ? 0 : kp);
     PM_CUDA(e->incr_evals.ensure(1));
     PM_CUDA(cudaMemsetAsync(e->incr_evals.p, 0, 8, e->stream));
     pm::EvalParams p = eval_params(e);
     int bits_mode = ((uint64_t)p.n_bits_rows * p.words <= (uint64_t)pm::kBitsCap) ? (p.words == 1 ? 2 : 1) : 0;
     bool fast = false;
     {
-      const int rc = decide_fast(e, &fast, e->dirty_dev.p, k);
+      const int rc = decide_fast(e, &fast, pre, kp);
       if (rc != PM_OK) return rc;
     }
     const bool wm = fast && bits_mode == 0 && p.n_bits_rows <= 31u && e->tune_build != 7;   // as the full pass
     if (wm) {
-      const int rc = worker_major(e, &p, &bits_mode, e->dirty_dev.p, k);
+      const int rc = worker_major(e, &p, &bits_mode, pre, kp);
       if (rc != PM_OK) return rc;
     }
     auto walk = [&](const pm::AskWalk& a, dim3 grid) -> int {
@@ -1241,22 +1309,22 @@ static int eval_incremental(pm_engine* e, const std::vector<uint32_t>& en, const
       return PM_OK;
     };
     Timer tm(e, &e->stats.ms_fused, e->stream);
-    if (k) {
-      pm::pm_scatter_value<<<blocks_for(k, 256), 256, 0, e->stream>>>(e->eval_first.p, e->dirty_dev.p, k, pm::kNone);
+    if (kr) {
+      pm::pm_scatter_value<<<blocks_for(kr, 256), 256, 0, e->stream>>>(e->eval_first.p, rows, kr, pm::kNone);
       PM_LAUNCH_CHECK("pm_scatter_value");
     }
-    uint32_t n_walk = k;
+    uint32_t n_walk = kr;
     const uint32_t* starts = nullptr;
-    if (nd) {
-      PM_CUDA(e->walk_start.ensure((size_t)k + W));
-      if (k) PM_CUDA(cudaMemsetAsync(e->walk_start.p, 0, (size_t)k * 4, e->stream));   // written rows: every ask
+    if (nd && nw) {
+      PM_CUDA(e->walk_start.ensure((size_t)kr + nw));
+      if (kr) PM_CUDA(cudaMemsetAsync(e->walk_start.p, 0, (size_t)kr * 4, e->stream));   // written rows: every ask
       PM_CUDA(cudaMemsetAsync(e->counters.p + 16, 0, 4, e->stream));
-      pm::pm_collect_orphans<<<blocks_for(W, 256), 256, 0, e->stream>>>(e->eval_first.p, W, e->toggle_dev.p + ne, nd,
-                                                                        e->dirty_dev.p + k, e->walk_start.p + k, e->counters.p + 16);
+      pm::pm_collect_orphans<<<blocks_for(nw, 256), 256, 0, e->stream>>>(e->eval_first.p, w0, nw, e->toggle_dev.p + ne, nd,
+                                                                         rows + kr, e->walk_start.p + kr, e->counters.p + 16);
       PM_LAUNCH_CHECK("pm_collect_orphans");
       PM_CUDA(cudaMemcpyAsync(e->h_scalars.p + 16, e->counters.p + 16, 4, cudaMemcpyDeviceToHost, e->stream));
       PM_CUDA(cudaStreamSynchronize(e->stream));   // the orphan count sizes the walk's grid
-      n_walk = k + e->h_scalars.p[16];
+      n_walk = kr + e->h_scalars.p[16];
       starts = e->walk_start.p;
       e->stats.n_tiles = n_walk;
     }
@@ -1266,11 +1334,11 @@ static int eval_incremental(pm_engine* e, const std::vector<uint32_t>& en, const
       const uint32_t steps = blocks_for(T, pm::kEvalRows);
       const uint32_t want_y = std::max(1u, std::min(steps, blocks_for(4u * e->sms, gx)));
       const uint32_t chunk = blocks_for(steps, want_y) * pm::kEvalRows;
-      const int rc = walk(pm::AskWalk{e->dirty_dev.p, starts, nullptr, n_walk, T, chunk}, dim3(gx, blocks_for(T, chunk)));
+      const int rc = walk(pm::AskWalk{rows, starts, nullptr, n_walk, T, chunk, 0}, dim3(gx, blocks_for(T, chunk)));
       if (rc != PM_OK) return rc;
     }
-    if (ne) {   // every worker against all of E: E is short, and W / 1024 CTAs spread over the SMs
-      const int rc = walk(pm::AskWalk{nullptr, nullptr, e->toggle_dev.p, W, ne, ne}, dim3(blocks_for(W, pm::kEvalCols), 1));
+    if (ne && nw) {   // every worker of the range against all of E: E is short, and nw / 1024 CTAs spread over the SMs
+      const int rc = walk(pm::AskWalk{nullptr, nullptr, e->toggle_dev.p, nw, ne, ne, w0}, dim3(blocks_for(nw, pm::kEvalCols), 1));
       if (rc != PM_OK) return rc;
     }
     tm.stop();
@@ -1315,17 +1383,16 @@ static int match_local_locked(pm_engine* e, uint32_t mode) {
   const bool timing = (e->cfg.flags & PM_CFG_TIMING) != 0;
   if (timing) PM_CUDA(cudaEventRecord(e->ev0, e->stream));
 
-  // PM_INCREMENTAL: re-evaluate the rows written since the stored evaluation when there is one and few rows changed.
-  // Only an engine that evaluates the whole table keeps a stored evaluation (a shard's first_ask holds its range only).
-  const bool keep_eval = !e->comm && w0 == 0 && nw == W;
+  // PM_INCREMENTAL: re-evaluate the rows of this engine's range written since the stored evaluation when there is one
+  // and few of them changed.  Each engine decides for itself: sharded ranks may differ (exchange_locked).
   const bool incr = (mode & PM_INCREMENTAL) != 0;
   std::vector<uint32_t> en, dis;   // asks enabled / disabled since the stored evaluation
-  if (incr && keep_eval && e->eval_valid) e->split_toggles(&en, &dis);
-  // The E-pass evaluates up to |E| x W pairs, as many as |E| W / T written rows walked in full: they count against the
-  // same cutoff (DESIGN §5)
-  const uint64_t e_rows = T ? ((uint64_t)en.size() * W + T - 1) / T : 0;
-  const bool use_incr = incr && keep_eval && e->eval_valid && !e->dirty_over && e->tune_incr != 0 &&
-                        e->dirty_rows.size() + e_rows <= e->tune_incr && T && W;
+  if (incr && e->eval_valid) e->split_toggles(&en, &dis);
+  // The E-pass evaluates up to |E| x nw pairs, as many as |E| nw / T written rows walked in full: they count against
+  // the same cutoff (DESIGN §5)
+  const uint64_t e_rows = T ? ((uint64_t)en.size() * nw + T - 1) / T : 0;
+  const bool use_incr = incr && e->eval_valid && !e->dirty_over && e->tune_incr != 0 &&
+                        e->dirty_in + e_rows <= e->tune_incr && T && nw;
 
   PM_CUDA(e->first_ask.ensure(W));
   PM_CUDA(e->ask_best.ensure(T));
@@ -1436,18 +1503,16 @@ static int match_local_locked(pm_engine* e, uint32_t mode) {
     e->stats.evals = (uint64_t)T * nw;
   }
   if (!use_incr) {
-    if (keep_eval) {   // every full evaluation refreshes the stored one: one 4 B-per-worker copy
-      PM_CUDA(e->eval_first.ensure(std::max<uint32_t>(W, 1)));
-      PM_CUDA(cudaMemcpyAsync(e->eval_first.p, e->first_ask.p, (size_t)W * 4, cudaMemcpyDeviceToDevice, e->stream));
-      e->clear_dirty();
-      e->dirty_mark.resize(W, 0);   // every mark is clear after clear_dirty
-      e->clear_toggled();
-      e->eval_on = e->ask_on;       // the mask this evaluation was taken under
-      e->eval_valid = true;
-    } else {
-      e->invalidate_eval();
-    }
-    if (incr) e->stats.n_tiles = W;   // rows re-evaluated
+    // every full evaluation refreshes the stored one: one 4 B-per-worker copy of the range's entries and NONE outside
+    // it, taken before a communicator's exchange fills the rest of first_ask
+    PM_CUDA(e->eval_first.ensure(std::max<uint32_t>(W, 1)));
+    PM_CUDA(cudaMemcpyAsync(e->eval_first.p, e->first_ask.p, (size_t)W * 4, cudaMemcpyDeviceToDevice, e->stream));
+    e->clear_dirty();
+    e->dirty_mark.resize(W, 0);   // every mark is clear after clear_dirty
+    e->clear_toggled();
+    e->eval_on = e->ask_on;       // the mask this evaluation was taken under
+    e->eval_valid = true;
+    if (incr) e->stats.n_tiles = nw;   // rows re-evaluated
   }
   e->workers_base = e->eval_valid && e->workers_checked;
   e->nacc_base = e->eval_valid && e->nacc_valid;
@@ -1979,6 +2044,11 @@ int pm_set_auction_params(pm_engine* e, uint64_t cost_scale, uint64_t eps_start,
 // count over its workers, first feasible ask of its own workers} into one buffer, ONE all-gather over NVLink moves
 // them, and every rank folds the contributions into the same global arrays.  Enqueued on the engine's stream: no host
 // synchronisation, nothing but NCCL's kernel between the evaluation and the resolution sweep.
+// Under PM_INCREMENTAL every rank decides full or incremental for its own range (match_local_locked: its own written
+// rows against the cutoff), so in one pass some ranks may evaluate their range in full while others walk a few rows.
+// Either way each rank's range of first_ask is exact, and every rank makes this same single all-gather, so the
+// collective sequence of the ranks never diverges.  Under PM_NO_ASK_STATS ask_best / ask_count are INF / 0 on every
+// rank and the fold keeps them so.
 static int exchange_locked(pm_engine* e) {
   const NcclApi& nccl = nccl_api();
   if (!nccl.ok) return e->fail(PM_E_UNSUPPORTED, nccl.err);
@@ -2004,14 +2074,16 @@ static int exchange_locked(pm_engine* e) {
   return PM_OK;
 }
 
-// PM_INCREMENTAL: a reference mode on the fused lean path, on an engine that evaluates the whole table
-static int check_incremental(pm_engine* e, uint32_t mode) {
+// PM_INCREMENTAL: a reference mode on the fused lean path.  pm_match_local takes it on any engine (the host moves the
+// three arrays); pm_match on a shard engine without a communicator refuses it: that call resolves one range as if it
+// were the table, so there is no whole-table result to keep incremental.
+static int check_incremental(pm_engine* e, uint32_t mode, bool local) {
   if (!(mode & PM_INCREMENTAL)) return PM_OK;
   if ((mode & 0xFFu) == PM_MODE_AUCTION) return e->fail(PM_E_INVALID, "pm_match: PM_INCREMENTAL is for the reference modes, not the auction");
   if ((mode & (PM_PATH_FUSED | PM_NO_ASK_STATS)) != (PM_PATH_FUSED | PM_NO_ASK_STATS))
     return e->fail(PM_E_INVALID, "pm_match: PM_INCREMENTAL needs PM_PATH_FUSED | PM_NO_ASK_STATS");
-  if (e->cfg.shard_first || e->cfg.shard_count || e->comm)
-    return e->fail(PM_E_UNSUPPORTED, "pm_match: PM_INCREMENTAL is single-GPU (no shard, no communicator)");
+  if (!local && !e->comm && (e->cfg.shard_first || e->cfg.shard_count))
+    return e->fail(PM_E_UNSUPPORTED, "pm_match: PM_INCREMENTAL on a shard engine needs a communicator or pm_match_local");
   return PM_OK;
 }
 
@@ -2025,7 +2097,7 @@ int pm_match_local(pm_engine* e, uint32_t mode) try {
   if (!e) return PM_E_INVALID;
   std::lock_guard<std::mutex> lk(e->mu);
   if ((mode & 0xFFu) == PM_MODE_AUCTION) return e->fail(PM_E_UNSUPPORTED, "pm_match_local: auction mode is single-GPU (use pm_match)");
-  const int rc = check_incremental(e, mode);
+  const int rc = check_incremental(e, mode, true);
   if (rc != PM_OK) return rc;
   return invalidate_on_failure(e, match_local_locked(e, mode));
 } catch (...) { return pm_guard_rc(); }
@@ -2037,7 +2109,7 @@ int pm_match_finish(pm_engine* e, uint32_t mode) try {
 int pm_match(pm_engine* e, uint32_t mode) try {
   if (!e) return PM_E_INVALID;
   std::lock_guard<std::mutex> lk(e->mu);
-  int rc = check_incremental(e, mode);
+  int rc = check_incremental(e, mode, false);
   if (rc != PM_OK) return rc;
   if ((mode & 0xFFu) == PM_MODE_AUCTION) return match_auction_locked(e);
   rc = match_local_locked(e, mode);
@@ -2309,6 +2381,13 @@ int pm_multi_set_worker_addr_rank(pm_multi* m, const uint32_t* rank, uint32_t fi
 } catch (...) { return pm_guard_rc(); }
 int pm_multi_set_flags(pm_multi* m, const uint32_t* idx, const uint32_t* flags, uint32_t n) try {
   PM_MULTI_EACH(pm_set_flags(e, idx, flags, n));
+} catch (...) { return pm_guard_rc(); }
+int pm_multi_resize_workers(pm_multi* m, uint32_t n_workers) try {
+  PM_MULTI_EACH(pm_resize_workers(e, n_workers));
+} catch (...) { return pm_guard_rc(); }
+int pm_multi_update_workers(pm_multi* m, const uint32_t* idx, const pm_worker_a* a, const pm_worker_b* b, const double* lat,
+                            const double* lon, uint32_t n) try {
+  PM_MULTI_EACH(pm_update_workers(e, idx, a, b, lat, lon, n));
 } catch (...) { return pm_guard_rc(); }
 int pm_multi_sync(pm_multi* m) try {
   PM_MULTI_EACH(pm_stream_sync(e));

@@ -818,28 +818,30 @@ pm_fused_eval(EvalParams p, uint32_t t0, uint32_t nt, uint32_t w0, uint32_t nw,
 //
 // The same kernel makes the two other walks of an incremental pass after configurations were enabled or disabled
 // (AskWalk):
-//   * the E-pass: every worker (rows == null) against the newly enabled asks only (asks = their increasing list).  A
-//     worker enters with its stored first ask f, so the first step's test already drops it when f lies below every
-//     listed ask, and a CTA whose workers all do exits before its first row;
+//   * the E-pass: every worker of the engine's range (rows == null: workers row0 + [0, n)) against the newly enabled
+//     asks only (asks = their increasing list).  A worker enters with its stored first ask f, so the first step's test
+//     already drops it when f lies below every listed ask, and a CTA whose workers all do exits before its first row;
 //   * the orphans: workers whose stored first ask was disabled, each with a start bound (the ask after it).  Asks
 //     below the start that were enabled then still reject the worker; those enabled since are the E-pass's.  The CTA
 //     starts at the least bound of its workers.
 struct AskWalk {
-  const uint32_t* rows;     // listed workers, or null: workers [0, n)
+  const uint32_t* rows;     // listed workers, or null: workers [row0, row0 + n)
   const uint32_t* starts;   // per listed worker, the first ask it can still need; null: 0
   const uint32_t* asks;     // the asks walked, increasing; null: the whole table
   uint32_t n;               // listed workers
   uint32_t n_seq;           // asks walked: entries of `asks`, or the table's n_asks
   uint32_t chunk;           // asks per grid row (blockIdx.y)
+  uint32_t row0;            // rows == null: the first worker
 };
 
-__device__ __forceinline__ void gather_workers(const EvalParams& p, const uint32_t* __restrict__ rows, uint32_t n,
-                                               uint32_t c, WorkerReg (&w)[kEvalWPT], uint32_t (&gw)[kEvalWPT]) {
+__device__ __forceinline__ void gather_workers(const EvalParams& p, const uint32_t* __restrict__ rows, uint32_t row0,
+                                               uint32_t n, uint32_t c, WorkerReg (&w)[kEvalWPT],
+                                               uint32_t (&gw)[kEvalWPT]) {
 #pragma unroll
   for (int k = 0; k < kEvalWPT; ++k) {
     const uint32_t col = c + k;
     if (col < n) {
-      gw[k] = rows ? __ldg(rows + col) : col;
+      gw[k] = rows ? __ldg(rows + col) : row0 + col;
       w[k] = make_worker(__ldg(p.wa + gw[k]), __ldg(p.wb + gw[k]));
       if (p.nacc) w[k].mmask = __ldg(p.nacc + gw[k]);
     } else {
@@ -858,7 +860,7 @@ pm_first_ask_rows(EvalParams p, AskWalk a, uint32_t* __restrict__ first_ask, uns
   const uint32_t c = cta0 + threadIdx.x * kEvalWPT;
   WorkerReg w[kEvalWPT];
   uint32_t gw[kEvalWPT];
-  gather_workers(p, a.rows, a.n, c, w, gw);
+  gather_workers(p, a.rows, a.row0, a.n, c, w, gw);
   const uint32_t n_cta = min(a.n - cta0, (uint32_t)kEvalCols);   // listed workers of this CTA
   uint32_t first[kEvalWPT];
   bool open[kEvalWPT];   // a listed candidate without a hit published yet
@@ -1075,14 +1077,15 @@ __global__ void pm_ask_toggle(const pm_ask* __restrict__ asks, const pm_gpu_opt*
   convert_ask(v >> 1, (v & 1u) == 0u, false, asks, opts, new_off, o, nullptr, nullptr);
 }
 
-// An incremental pass after configurations were disabled: the workers whose stored first ask is one of them (`dis`,
-// increasing, nd entries).  Each is appended to out[] with the ask after its stored one as its walk's start bound, and
-// its stored entry is reset.  One thread per worker, one atomic per warp.
-__global__ void pm_collect_orphans(uint32_t* __restrict__ eval_first, uint32_t n_workers, const uint32_t* __restrict__ dis,
+// An incremental pass after configurations were disabled: the workers of the range [w0, w0 + nw) whose stored first
+// ask is one of them (`dis`, increasing, nd entries).  Each is appended to out[] with the ask after its stored one as
+// its walk's start bound, and its stored entry is reset.  One thread per worker, one atomic per warp.
+__global__ void pm_collect_orphans(uint32_t* __restrict__ eval_first, uint32_t w0, uint32_t nw, const uint32_t* __restrict__ dis,
                                    uint32_t nd, uint32_t* __restrict__ out, uint32_t* __restrict__ starts,
                                    uint32_t* __restrict__ count) {
-  const uint32_t w = blockIdx.x * blockDim.x + threadIdx.x;
-  const uint32_t f = w < n_workers ? eval_first[w] : kNone;
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  const uint32_t w = w0 + i;
+  const uint32_t f = i < nw ? eval_first[w] : kNone;
   bool hit = false;
   if (f != kNone) {
     uint32_t lo = 0, hi = nd;

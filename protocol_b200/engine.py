@@ -385,6 +385,33 @@ class MultiEngine:
         self._check(self._lib.pm_multi_set_worker_addr_rank(self._h, _ptr(rank), 0, len(rank)))
         self._check(self._lib.pm_multi_sync(self._h))
 
+    def upsert_workers(self, a, b, first: int = 0):
+        a = np.ascontiguousarray(a, dtype=abi.WORKER_A)
+        b = np.ascontiguousarray(b, dtype=abi.WORKER_B)
+        self._check(self._lib.pm_multi_upsert_workers(self._h, _ptr(a), _ptr(b), first, len(a)))
+        self._check(self._lib.pm_multi_sync(self._h))
+
+    def set_flags(self, idx, flags):
+        idx = np.ascontiguousarray(idx, dtype=np.uint32)
+        flags = np.ascontiguousarray(flags, dtype=np.uint32)
+        self._check(self._lib.pm_multi_set_flags(self._h, _ptr(idx), _ptr(flags), len(idx)))
+        self._check(self._lib.pm_multi_sync(self._h))
+
+    def resize_workers(self, n: int):
+        self._check(self._lib.pm_multi_resize_workers(self._h, n))
+
+    def update_workers(self, idx, a, b, lat=None, lon=None):
+        """Scatter changed rows into every device's resident table (pm_multi_update_workers)."""
+        idx = np.ascontiguousarray(idx, dtype=np.uint32)
+        a = np.ascontiguousarray(a, dtype=abi.WORKER_A)
+        b = np.ascontiguousarray(b, dtype=abi.WORKER_B)
+        la = np.ascontiguousarray(lat, dtype=np.float64) if lat is not None else None
+        lo = np.ascontiguousarray(lon, dtype=np.float64) if lon is not None else None
+        self._check(self._lib.pm_multi_update_workers(self._h, _ptr(idx), _ptr(a), _ptr(b),
+                                                      _ptr(la) if la is not None else None,
+                                                      _ptr(lo) if lo is not None else None, len(idx)))
+        self._check(self._lib.pm_multi_sync(self._h))
+
     def match(self, mode: int = abi.PM_MODE_FIRST_FIT):
         self._check(self._lib.pm_multi_match(self._h, mode))
 

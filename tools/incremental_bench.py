@@ -17,7 +17,18 @@ the same run.
 The toggle series: configurations enabled and disabled between passes (pm_set_ask_enabled), no worker row written.
 25 000 random asks start disabled, so there are asks to enable.  Per round and for every j in J, alternated with the
 full fused lean pass: ceil(j/2) asks are disabled — half of them the asks that own the most workers, half asks that
-own none — and j//2 disabled ones are enabled, then one incremental pass runs.  Same sibling check as above."""
+own none — and j//2 disabled ones are enabled, then one incremental pass runs.  Same sibling check as above.
+
+    python tools/incremental_bench.py --shards N [--toggle] [...]
+    python tools/incremental_bench.py --multi [--toggle] [...]
+
+The same two series on sharded engines, reported per rank.  --shards N: N shard engines on device 0 (pm_set_shard,
+equal shares of the table), each pass pm_match_local on every shard, the merge of the three arrays (concatenate / min /
+sum, as the collective does) and pm_match_finish.  Per rank: `ms_local_host` (wall time of pm_match_local ending in a
+stream sync), `ms_fused` (device time of its evaluation kernels), `ms_total` (device, pm_match_local to the end of
+pm_match_finish, so it includes the wait for the host merge).  --multi: pm_multi over every visible GPU,
+pm_multi_match; per rank `ms_total`, `ms_exchange` and `exchange_bytes` as well.  Every step is checked against an
+unsharded engine's full pass (pm_fetch_result of rank 0)."""
 from __future__ import annotations
 
 import argparse
@@ -33,7 +44,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 from protocol_b200 import abi, synth  # noqa: E402
-from protocol_b200.engine import Engine  # noqa: E402
+from protocol_b200.engine import Engine, MultiEngine  # noqa: E402
+from protocol_b200.sharded import shard_range, wrap_device_buffers  # noqa: E402
 
 LEAN = abi.PM_MODE_FIRST_FIT | abi.PM_PATH_FUSED | abi.PM_NO_ASK_STATS
 INCR = LEAN | abi.PM_INCREMENTAL
@@ -117,16 +129,201 @@ def toggle_series(args, w, a, bits, npat, nmod, words, env):
     return rows, checked, f"{T} asks x {W} workers (synth mixed, 25 000 asks disabled at the start), first fit, fused lean"
 
 
+class Ranks:
+    """Sharded engines with the interface the series need: `apply` a table call to every rank and to the unsharded
+    sibling, `timed` one PM_INCREMENTAL (or full) pass returning per-rank rows, `same_as_full` against the sibling."""
+
+    def __init__(self, n_shards, multi, n_workers):
+        import torch
+
+        os.environ["PM_TUNE_INCR"] = str(1 << 31)   # read at pm_create: never fall back, so the crossover shows
+        if multi:
+            self.devices = list(range(torch.cuda.device_count()))
+            self.m = MultiEngine(self.devices, timing=True)
+            self.engines = []
+        else:
+            self.m = None
+            self.engines = [Engine(timing=True) for _ in range(n_shards)]
+        del os.environ["PM_TUNE_INCR"]
+        self.ref = Engine(timing=True)
+        self.n_shards = len(self.devices) if multi else n_shards
+
+    def apply(self, name, *args):
+        for e in ([self.m] if self.m else self.engines) + [self.ref]:
+            getattr(e, name)(*args)
+
+    def set_ranges(self, W):
+        for r, e in enumerate(self.engines):
+            lo, hi = shard_range(W, self.n_shards, r)
+            e.set_shard(lo, hi - lo)
+
+    def timed(self, mode):
+        import torch
+
+        if self.m:
+            t = time.perf_counter()
+            self.m.match(mode)
+            self.m._check(self.m._lib.pm_multi_sync(self.m._h))
+            wall = (time.perf_counter() - t) * 1e3
+            sts = [self.m.stats(i) for i in range(self.n_shards)]
+            return {"ms_host": wall, "ranks": [{k: s[k] for k in ("ms_total", "ms_exchange", "exchange_bytes", "evals",
+                                                                  "n_tiles")} for s in sts]}
+        W, T = self.ref.n_workers, self.ref.n_asks
+        local = []
+        t = time.perf_counter()
+        for e in self.engines:
+            t0 = time.perf_counter()
+            e.match_local(mode)
+            e.sync()
+            local.append((time.perf_counter() - t0) * 1e3)
+        bufs = [wrap_device_buffers(e, W, T) for e in self.engines]
+        first = torch.cat([bufs[r][0][slice(*shard_range(W, self.n_shards, r))] for r in range(self.n_shards)])
+        best = torch.stack([b[1] for b in bufs]).min(dim=0).values
+        cnt = torch.stack([b[2] for b in bufs]).sum(dim=0).to(torch.int32)
+        for b in bufs:
+            b[0].copy_(first)
+            b[1].copy_(best)
+            b[2].copy_(cnt)
+        torch.cuda.synchronize()
+        for e in self.engines:
+            e.match_finish(mode)
+            e.sync()
+        wall = (time.perf_counter() - t) * 1e3
+        sts = [e.stats() for e in self.engines]
+        return {"ms_host": wall, "ranks": [dict(ms_local_host=lh, **{k: s[k] for k in ("ms_fused", "ms_total", "evals", "n_tiles")})
+                                           for lh, s in zip(local, sts)]}
+
+    def fetch(self):
+        return self.m.fetch() if self.m else self.engines[0].fetch()
+
+    def same_as_full(self):
+        r = self.fetch()
+        self.ref.match(LEAN)
+        q = self.ref.fetch()
+        return r, all(np.array_equal(getattr(r, f), getattr(q, f)) for f in FIELDS)
+
+    def close(self):
+        for e in ([self.m] if self.m else self.engines) + [self.ref]:
+            e.close()
+
+
+def sharded_series(args, w, a, bits, npat, nmod, words, pool):
+    """The k series (pool given) or the toggle series (pool None) on Ranks; per-rank rows."""
+    rk = Ranks(args.shards, args.multi, len(w))
+    W, T = len(w), len(a)
+    rk.apply("set_asks", a.asks, a.opts)
+    rk.apply("set_model_table", bits, npat, nmod, words)
+    rk.apply("set_workers", w.a, w.b)
+    rk.set_ranges(W)
+    rng = np.random.default_rng(2024 if pool is not None else 2025)
+    on = np.ones(T, bool)
+    if pool is None:
+        on[rng.choice(T, 25_000, replace=False)] = False
+        rk.apply("set_ask_enabled", np.nonzero(~on)[0], False)
+    rk.timed(LEAN)   # warm-up: allocations, first launches
+    wa = w.a.copy()
+    keys = K if pool is not None else J
+    rows = {"full": []}
+    rows.update({k: [] for k in keys})
+    checked = set()
+    for rnd in range(args.rounds):
+        for k in keys:
+            if pool is None or k == keys[0]:
+                rows["full"].append(rk.timed(LEAN))   # refreshes every rank's stored evaluation
+            extra = {}
+            if pool is not None and k:
+                idx = rng.choice(W, k, replace=False).astype(np.uint32)
+                fl, up = idx[:k // 2], idx[k // 2:]
+                if len(fl):
+                    f = wa["flags"][fl] ^ np.where(rng.random(len(fl)) < 0.7, abi.PM_W_ASSIGNED, abi.PM_W_HEALTHY).astype(np.uint32)
+                    wa["flags"][fl] = f
+                    rk.apply("set_flags", fl, f)
+                src = rng.integers(0, len(pool), len(up))
+                rk.apply("update_workers", up, pool.a[src].copy(), pool.b[src].copy())
+            elif pool is None:
+                wk = rk.fetch().worker_ask
+                owners = np.bincount(wk[wk != abi.PM_NONE], minlength=T)
+                n_off, n_on = (k + 1) // 2, k // 2
+                enabled = np.nonzero(on)[0]
+                top = enabled[np.argsort(owners[enabled])[::-1][:(n_off + 1) // 2]]
+                idle = enabled[owners[enabled] == 0]
+                off = np.concatenate([top, rng.choice(idle, min(len(idle), n_off - len(top)), replace=False)])
+                en = rng.choice(np.nonzero(~on)[0], min(n_on, int((~on).sum())), replace=False)
+                rk.apply("set_ask_enabled", off, False)
+                rk.apply("set_ask_enabled", en, True)
+                on[off], on[en] = False, True
+                extra = {"n_off": len(off), "n_on": len(en)}
+            rows[k].append(dict(rk.timed(INCR), **extra))
+            _, same = rk.same_as_full()   # every step, against the sibling's full pass
+            if not same:
+                raise SystemExit(f"{k}: the incremental result differs from the full pass")
+            checked.add(k)
+    n = rk.n_shards
+    rk.close()
+    what = f"{n} shard engines on device 0" if not args.multi else f"pm_multi over {n} GPU(s)"
+    return rows, checked, f"{T} asks x {W} workers (synth mixed), first fit, fused lean, {what}"
+
+
+def report_ranks(rows, checked, workload, env, key_name, out_dir, file_name, multi):
+    summary = []
+    for key, rs in rows.items():
+        n = len(rs[0]["ranks"])
+        per = []
+        for r in range(n):
+            rr = [x["ranks"][r] for x in rs]
+            d = {"rank": r, "evals": int(rr[-1]["evals"]), "n_tiles": int(rr[-1]["n_tiles"]),
+                 "ms_total_median": float(np.median([x["ms_total"] for x in rr]))}
+            if multi:
+                d["ms_exchange_median"] = float(np.median([x["ms_exchange"] for x in rr]))
+                d["exchange_bytes"] = int(rr[-1]["exchange_bytes"])
+            else:
+                d["ms_local_host_median"] = float(np.median([x["ms_local_host"] for x in rr]))
+                d["ms_fused_median"] = float(np.median([x["ms_fused"] for x in rr]))
+            per.append(d)
+        summary.append({key_name: key, "ms_host_median": float(np.median([x["ms_host"] for x in rs])), "runs": len(rs),
+                        "ranks": per, **{k: rs[-1][k] for k in ("n_off", "n_on") if k in rs[-1]}})
+    out = {"workload": workload, "card": env, "checked_equal_to_full_pass": [str(c) for c in sorted(checked)],
+           "rows": summary}
+    if multi and len(summary[0]["ranks"]) < 2:
+        out["note"] = "one GPU: multi-GPU numbers not measured"
+    print(f"{env.get('name')}  power limit {env.get('power_limit_w')} W  SM {env.get('sm_mhz')}/{env.get('sm_max_mhz')} MHz")
+    print(workload)
+    cols = "ms_total ms_exchange   xchg_bytes" if multi else "ms_local_host ms_fused ms_total"
+    print(f"{key_name:>8} {'rank':>4} {cols} {'evals':>16} {'n_tiles':>9}")
+    for s in summary:
+        for d in s["ranks"]:
+            vals = (f"{d['ms_total_median']:>8.3f} {d['ms_exchange_median']:>11.3f} {d['exchange_bytes']:>12}" if multi else
+                    f"{d['ms_local_host_median']:>13.3f} {d['ms_fused_median']:>8.3f} {d['ms_total_median']:>8.3f}")
+            print(f"{s[key_name]:>8} {d['rank']:>4} {vals} {d['evals']:>16} {d['n_tiles']:>9}")
+    print(json.dumps(out))
+    if out_dir:
+        os.makedirs(out_dir, exist_ok=True)
+        with open(os.path.join(out_dir, file_name), "w") as f:
+            json.dump(out, f, indent=1)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--workers", type=int, default=1_000_000)
     ap.add_argument("--asks", type=int, default=100_000)
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--toggle", action="store_true", help="configurations toggled between passes instead of rows written")
+    ap.add_argument("--shards", type=int, default=0, help="N shard engines on device 0 (pm_match_local + host merge)")
+    ap.add_argument("--multi", action="store_true", help="pm_multi over every visible GPU")
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
 
     w = synth.make_workers(args.workers)
+    if args.shards or args.multi:
+        a = synth.make_asks(args.asks, "mixed")
+        bits, npat, nmod, words = synth.intern_tables(w, a)
+        env = card()
+        pool = None if args.toggle else synth.make_workers(200_000, seed=synth.SEED_WORKERS + 101)
+        rows, checked, workload = sharded_series(args, w, a, bits, npat, nmod, words, pool)
+        name = ("multi" if args.multi else f"shards{args.shards}") + ("_toggle" if args.toggle else "")
+        report_ranks(rows, checked, workload, env, "j" if args.toggle else "k", args.out,
+                     f"incremental_bench_{name}.json", args.multi)
+        return
     if args.toggle:
         a = synth.make_asks(args.asks, "mixed")
         bits, npat, nmod, words = synth.intern_tables(w, a)
