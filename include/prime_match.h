@@ -405,6 +405,14 @@ int pm_multi_resize_workers(pm_multi*, uint32_t n_workers);
 int pm_multi_update_workers(pm_multi*, const uint32_t* idx, const pm_worker_a* a, const pm_worker_b* b, const double* lat,
                             const double* lon, uint32_t n);
 int pm_multi_sync(pm_multi*);
+/* changes whenever any table call changed a table on any device, including calls made directly on
+ * pm_multi_engine(m, i) (the sum of the engines' pm_table_version); 0 for NULL                                      */
+uint64_t pm_multi_table_version(const pm_multi*);
+/* With more than one device, a pass that fails on any device aborts every communicator, so that no device is left
+ * waiting in the exchange.  The next pm_multi_match re-creates them over the same devices (ncclCommInitAll), attaches
+ * them again and discards every device's stored evaluation (as pm_attach_comm does): that pass runs in full on every
+ * device.  A refused pass (PM_E_UNSUPPORTED in proximity mode with an enabled max_group_size == 0 ask, say) is
+ * therefore retried like any other once its cause is gone.                                                            */
 int pm_multi_match(pm_multi*, uint32_t mode);
 int pm_multi_fetch_result(pm_multi*, pm_result* out);
 
@@ -471,6 +479,11 @@ typedef struct pm_discovery_node {    /* shared/src/models/node.rs:552-570 (fiel
 /* NodeGroupsPlugin::new_with_policy (mod.rs:129-175).  engine may be NULL (then
  * pm_plugin_try_form_new_groups fails with PM_E_NO_DEVICE); policy NULL = defaults. */
 int  pm_plugin_create(pm_engine* engine, const pm_plugin_policy* policy, pm_plugin** out);
+/* Same, with the formation pass on several GPUs: every table call of pm_plugin_try_form_new_groups goes through
+ * pm_multi_* and the pass is pm_multi_match (each device evaluates its share of the workers, incrementally on resident
+ * tables).  Solo-group merging runs on a sibling engine of pm_multi_engine(multi, 0), on device 0 only.  multi NULL is
+ * PM_E_INVALID.  The plugin does not own the pm_multi (nor an engine): destroy the plugin first.                      */
+int  pm_plugin_create_multi(pm_multi* multi, const pm_plugin_policy* policy, pm_plugin** out);
 void pm_plugin_destroy(pm_plugin*);
 const char* pm_plugin_last_error(const pm_plugin*);
 /* duplicate name / max < min are PM_E_INVALID (the reference panics, mod.rs:141-147);

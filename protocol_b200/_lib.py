@@ -94,9 +94,11 @@ def load() -> C.CDLL:
         "pm_multi_resize_workers": (i32, [vp, u32]),
         "pm_multi_update_workers": (i32, [vp, vp, vp, vp, vp, vp, u32]),
         "pm_multi_sync": (i32, [vp]),
+        "pm_multi_table_version": (C.c_uint64, [vp]),
         "pm_multi_match": (i32, [vp, u32]),
         "pm_multi_fetch_result": (i32, [vp, P(abi.PmResult)]),
         "pm_plugin_create": (i32, [vp, P(abi.PmPluginPolicy), P(vp)]),
+        "pm_plugin_create_multi": (i32, [vp, P(abi.PmPluginPolicy), P(vp)]),
         "pm_plugin_destroy": (None, [vp]),
         "pm_plugin_last_error": (cp, [vp]),
         "pm_plugin_add_config": (i32, [vp, cp, u32, u32, cp]),

@@ -120,9 +120,9 @@ EXPORTS = [
     "pm_multi_create", "pm_multi_destroy", "pm_multi_size", "pm_multi_engine", "pm_multi_last_error",
     "pm_multi_set_asks", "pm_multi_set_ask_enabled", "pm_multi_set_model_table", "pm_multi_set_worker_count", "pm_multi_upsert_workers",
     "pm_multi_set_worker_locations", "pm_multi_set_worker_addr_rank", "pm_multi_set_flags",
-    "pm_multi_resize_workers", "pm_multi_update_workers", "pm_multi_sync",
+    "pm_multi_resize_workers", "pm_multi_update_workers", "pm_multi_sync", "pm_multi_table_version",
     "pm_multi_match", "pm_multi_fetch_result",
-    "pm_plugin_create", "pm_plugin_destroy", "pm_plugin_last_error", "pm_plugin_add_config", "pm_plugin_seal_configs",
+    "pm_plugin_create", "pm_plugin_create_multi", "pm_plugin_destroy", "pm_plugin_last_error", "pm_plugin_add_config", "pm_plugin_seal_configs",
     "pm_plugin_enable_configuration", "pm_plugin_upsert_node", "pm_plugin_set_node_status", "pm_plugin_sync_discovery", "pm_plugin_sync_discovery_json", "pm_plugin_get_node", "pm_plugin_add_task",
     "pm_plugin_delete_task", "pm_plugin_record_upload", "pm_plugin_try_form_new_groups", "pm_plugin_try_merge_solo_groups", "pm_plugin_get_node_group", "pm_plugin_get_all_groups", "pm_plugin_get_group_by_id", "pm_plugin_handle_group_not_found", "pm_plugin_restore_group", "pm_plugin_export_tables", "pm_plugin_redis_writeback",
     "pm_scheduler_get_task_for_node",

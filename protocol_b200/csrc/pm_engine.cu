@@ -2293,6 +2293,7 @@ int pm_stream_sync(pm_engine* e) try {
 struct pm_multi {
   std::vector<pm_engine*> engines;
   std::vector<pm_comm*> comms;
+  std::vector<int> devices;   // kept to re-create the communicators after a failed pass aborted them
   std::string err;
 };
 
@@ -2307,6 +2308,7 @@ int pm_multi_create(const pm_cfg* cfg, const int32_t* devices, uint32_t n, pm_mu
   if (!cfg || !devices || !out || n == 0) return PM_E_INVALID;
   *out = nullptr;
   pm_multi* m = new pm_multi;
+  m->devices.assign(devices, devices + n);
   for (uint32_t i = 0; i < n; ++i) {
     pm_cfg c = *cfg;
     c.device = devices[i];
@@ -2321,8 +2323,7 @@ int pm_multi_create(const pm_cfg* cfg, const int32_t* devices, uint32_t n, pm_mu
     const NcclApi& nccl = nccl_api();
     if (!nccl.ok) { g_create_error = nccl.err; pm_multi_destroy(m); return PM_E_UNSUPPORTED; }
     std::vector<ncclComm_t> raw(n, nullptr);
-    std::vector<int> devs(devices, devices + n);
-    const ncclResult_t nr = nccl.CommInitAll(raw.data(), (int)n, devs.data());
+    const ncclResult_t nr = nccl.CommInitAll(raw.data(), (int)n, m->devices.data());
     if (nr != ncclSuccess) {
       g_create_error = std::string("ncclCommInitAll: ") + nccl.GetErrorString(nr);
       pm_multi_destroy(m);
@@ -2394,6 +2395,33 @@ int pm_multi_sync(pm_multi* m) try {
 } catch (...) { return pm_guard_rc(); }
 #undef PM_MULTI_EACH
 
+// every engine's version only grows, so the sum changes whenever any of them does
+uint64_t pm_multi_table_version(const pm_multi* m) {
+  if (!m) return 0;
+  uint64_t v = 0;
+  for (const pm_engine* e : m->engines) v += pm_table_version(e);
+  return v;
+}
+
+// After a failed pass aborted the communicators: new ones over the same devices, attached again.  pm_attach_comm
+// discards each engine's stored evaluation, so the pass that follows evaluates every device's share in full.
+static int multi_reconnect(pm_multi* m) {
+  const NcclApi& nccl = nccl_api();
+  const uint32_t n = (uint32_t)m->engines.size();
+  std::vector<ncclComm_t> raw(n, nullptr);
+  const ncclResult_t nr = nccl.CommInitAll(raw.data(), (int)n, m->devices.data());
+  if (nr != ncclSuccess) {
+    m->err = std::string("pm_multi_match: ncclCommInitAll: ") + nccl.GetErrorString(nr);
+    return PM_E_CUDA;
+  }
+  for (uint32_t i = 0; i < n; ++i) m->comms[i]->nccl = raw[i];
+  for (uint32_t i = 0; i < n; ++i) {
+    const int rc = pm_attach_comm(m->engines[i], m->comms[i]);
+    if (rc != PM_OK) { m->err = pm_last_error(m->engines[i]); return rc; }
+  }
+  return PM_OK;
+}
+
 int pm_multi_match(pm_multi* m, uint32_t mode) try {
   if (!m) return PM_E_INVALID;
   const size_t n = m->engines.size();
@@ -2403,13 +2431,17 @@ int pm_multi_match(pm_multi* m, uint32_t mode) try {
     return rc;
   }
   // a rank that fails before the collective would leave the others waiting in it: check what can be checked first,
-  // and abort every communicator if a rank still fails on the way
+  // and abort every communicator if a rank still fails on the way (the next pass makes new ones)
   for (pm_engine* e : m->engines) {
     if (!e->have_workers || !e->have_asks) { m->err = "pm_multi_match: worker and ask tables must be set first"; return PM_E_STATE; }
     if (e->n_workers != m->engines[0]->n_workers || e->n_asks != m->engines[0]->n_asks) {
       m->err = "pm_multi_match: engines hold different tables";
       return PM_E_STATE;
     }
+  }
+  if (!m->comms[0]->nccl) {   // the abort below clears every communicator at once
+    const int rc = multi_reconnect(m);
+    if (rc != PM_OK) return rc;
   }
   std::vector<int> rcs(n, PM_OK);
   std::atomic<bool> aborted{false};

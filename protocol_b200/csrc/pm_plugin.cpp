@@ -131,10 +131,42 @@ bool task_applicable(const TaskRec& t, const std::string& configuration_name) {
   return std::find(t.topologies.begin(), t.topologies.end(), configuration_name) != t.topologies.end();
 }
 
+// Where the formation pass runs: one engine, or a pm_multi (table calls reach every device, the pass is sharded).
+struct Device {
+  pm_engine* engine = nullptr;
+  pm_multi* multi = nullptr;
+
+  explicit operator bool() const { return engine || multi; }
+  pm_engine* first() const { return multi ? pm_multi_engine(multi, 0) : engine; }   // home of the merge pass's sibling
+  const char* last_error() const { return multi ? pm_multi_last_error(multi) : pm_last_error(engine); }
+  uint64_t table_version() const { return multi ? pm_multi_table_version(multi) : pm_table_version(engine); }
+  int set_asks(const pm_ask* a, uint32_t n, const pm_gpu_opt* o, uint32_t no) const {
+    return multi ? pm_multi_set_asks(multi, a, n, o, no) : pm_set_asks(engine, a, n, o, no);
+  }
+  int set_ask_enabled(const uint32_t* idx, const uint8_t* on, uint32_t n) const {
+    return multi ? pm_multi_set_ask_enabled(multi, idx, on, n) : pm_set_ask_enabled(engine, idx, on, n);
+  }
+  int set_model_table(const uint32_t* bits, uint32_t npat, uint32_t nmod, uint32_t words) const {
+    return multi ? pm_multi_set_model_table(multi, bits, npat, nmod, words) : pm_set_model_table(engine, bits, npat, nmod, words);
+  }
+  int set_worker_count(uint32_t n) const { return multi ? pm_multi_set_worker_count(multi, n) : pm_set_worker_count(engine, n); }
+  int resize_workers(uint32_t n) const { return multi ? pm_multi_resize_workers(multi, n) : pm_resize_workers(engine, n); }
+  int update_workers(const uint32_t* idx, const pm_worker_a* a, const pm_worker_b* b, const double* lat, const double* lon,
+                     uint32_t n) const {
+    return multi ? pm_multi_update_workers(multi, idx, a, b, lat, lon, n) : pm_update_workers(engine, idx, a, b, lat, lon, n);
+  }
+  int set_worker_locations(const double* lat, const double* lon, uint32_t first_row, uint32_t n) const {
+    return multi ? pm_multi_set_worker_locations(multi, lat, lon, first_row, n) : pm_set_worker_locations(engine, lat, lon, first_row, n);
+  }
+  int sync() const { return multi ? pm_multi_sync(multi) : pm_stream_sync(engine); }
+  int match(uint32_t mode) const { return multi ? pm_multi_match(multi, mode) : pm_match(engine, mode); }
+  int fetch_result(pm_result* r) const { return multi ? pm_multi_fetch_result(multi, r) : pm_fetch_result(engine, r); }
+};
+
 }  // namespace
 
 struct pm_plugin {
-  pm_engine* engine = nullptr;
+  Device dev;   // not owned
   pm_plugin_policy policy{};
   pm_interner* interner = nullptr;
   std::string err;
@@ -301,11 +333,10 @@ static const char* canon_address(const pm_plugin* p, const char* address, char (
   var = canon_address(p, var, var##_canon);                                                \
   if (!var) return p->fail(PM_E_INVALID, "not an address (policy.canonical_addresses)")
 
-int pm_plugin_create(pm_engine* engine, const pm_plugin_policy* policy, pm_plugin** out) try {
-  if (!out) return PM_E_INVALID;
+static int plugin_create(Device dev, const pm_plugin_policy* policy, pm_plugin** out) {
   pm_plugin* p = new (std::nothrow) pm_plugin;
   if (!p) return PM_E_NOMEM;
-  p->engine = engine;
+  p->dev = dev;
   if (policy) p->policy = *policy;
   else {  // TaskSwitchingPolicy::default / ProximityOptimizationPolicy::default, mod.rs:85-98
     p->policy.task_switching_enabled = 1;
@@ -315,6 +346,20 @@ int pm_plugin_create(pm_engine* engine, const pm_plugin_policy* policy, pm_plugi
   p->interner = pm_interner_create();
   *out = p;
   return PM_OK;
+}
+
+int pm_plugin_create(pm_engine* engine, const pm_plugin_policy* policy, pm_plugin** out) try {
+  if (!out) return PM_E_INVALID;
+  Device dev;
+  dev.engine = engine;
+  return plugin_create(dev, policy, out);
+} catch (...) { return pm_guard_rc(); }
+
+int pm_plugin_create_multi(pm_multi* multi, const pm_plugin_policy* policy, pm_plugin** out) try {
+  if (!out || !multi) return PM_E_INVALID;
+  Device dev;
+  dev.multi = multi;
+  return plugin_create(dev, policy, out);
 } catch (...) { return pm_guard_rc(); }
 
 void pm_plugin_destroy(pm_plugin* p) {
@@ -1057,10 +1102,10 @@ int pm_plugin_try_form_new_groups(pm_plugin* p, uint32_t* n_formed) try {
   uint32_t npat = 0, nmod = 0, words = 1;
   {
     std::lock_guard<std::shared_mutex> lk(p->mu);
-    if (!p->engine) return p->fail(PM_E_NO_DEVICE, "no engine attached: group formation has no CPU path");
+    if (!p->dev) return p->fail(PM_E_NO_DEVICE, "no engine attached: group formation has no CPU path");
     if (!p->sealed) return p->fail(PM_E_STATE, "configurations not sealed");
     W = (uint32_t)p->nodes.size();
-    full = pm_table_version(p->engine) != p->resident_version || p->resident_rows > W;
+    full = p->dev.table_version() != p->resident_version || p->resident_rows > W;
     auto row_of = [&](uint32_t i, pm_worker_a* a, pm_worker_b* b, double* la, double* lo) {
       const NodeRec& n = p->nodes[i];
       *a = n.a;
@@ -1136,36 +1181,37 @@ int pm_plugin_try_form_new_groups(pm_plugin* p, uint32_t* n_formed) try {
     p->resident_version = ~0ull;  // not valid again until this pass has put its rows on the device
   }
   // ---- phase 2 (tables unlocked: heartbeats keep being served): the pass on the GPU
+  const Device& dev = p->dev;
   auto chk = [&](int r, const char* what) {
     if (r != PM_OK) {
-      const char* m = pm_last_error(p->engine);
+      const char* m = dev.last_error();
       std::lock_guard<std::shared_mutex> lk(p->mu);
       p->err = std::string(what) + ": " + (m ? m : "");
     }
     return r;
   };
   int rc;
-  if (send_asks && (rc = chk(pm_set_asks(p->engine, asks.data(), (uint32_t)asks.size(), opts.data(), (uint32_t)opts.size()), "pm_set_asks"))) return rc;
+  if (send_asks && (rc = chk(dev.set_asks(asks.data(), (uint32_t)asks.size(), opts.data(), (uint32_t)opts.size()), "pm_set_asks"))) return rc;
   if (!toggle_idx.empty() &&
-      (rc = chk(pm_set_ask_enabled(p->engine, toggle_idx.data(), toggle_on.data(), (uint32_t)toggle_idx.size()), "pm_set_ask_enabled")))
+      (rc = chk(dev.set_ask_enabled(toggle_idx.data(), toggle_on.data(), (uint32_t)toggle_idx.size()), "pm_set_ask_enabled")))
     return rc;
-  if (send_bits && (rc = chk(pm_set_model_table(p->engine, bits_copy.data(), npat, nmod, words), "pm_set_model_table"))) return rc;
+  if (send_bits && (rc = chk(dev.set_model_table(bits_copy.data(), npat, nmod, words), "pm_set_model_table"))) return rc;
   if (full) {
-    if ((rc = chk(pm_set_worker_count(p->engine, W), "pm_set_worker_count"))) return rc;
+    if ((rc = chk(dev.set_worker_count(W), "pm_set_worker_count"))) return rc;
   } else if (W != p->resident_rows) {
-    if ((rc = chk(pm_resize_workers(p->engine, W), "pm_resize_workers"))) return rc;
+    if ((rc = chk(dev.resize_workers(W), "pm_resize_workers"))) return rc;
   }
   if (!idx.empty()) {
-    if ((rc = chk(pm_update_workers(p->engine, idx.data(), ua.data(), ub.data(), ulat.data(), ulon.data(), (uint32_t)idx.size()), "pm_update_workers"))) return rc;
-    if ((rc = chk(pm_stream_sync(p->engine), "pm_stream_sync"))) return rc;   // staging vectors are read asynchronously
+    if ((rc = chk(dev.update_workers(idx.data(), ua.data(), ub.data(), ulat.data(), ulon.data(), (uint32_t)idx.size()), "pm_update_workers"))) return rc;
+    if ((rc = chk(dev.sync(), "pm_stream_sync"))) return rc;   // staging vectors are read asynchronously
   } else if (full) {   // an empty table still needs its location columns for the proximity mode
-    if ((rc = chk(pm_set_worker_locations(p->engine, nullptr, nullptr, 0, 0), "pm_set_worker_locations"))) return rc;
+    if ((rc = chk(dev.set_worker_locations(nullptr, nullptr, 0, 0), "pm_set_worker_locations"))) return rc;
   }
   p->resident_rows = W;
-  const uint64_t version_after_upload = pm_table_version(p->engine);
-  if ((rc = chk(pm_match(p->engine, mode), "pm_match"))) return rc;
+  const uint64_t version_after_upload = dev.table_version();
+  if ((rc = chk(dev.match(mode), "pm_match"))) return rc;
   pm_result res{};
-  if ((rc = chk(pm_fetch_result(p->engine, &res), "pm_fetch_result"))) return rc;
+  if ((rc = chk(dev.fetch_result(&res), "pm_fetch_result"))) return rc;
 
   // ---- phase 3 (tables locked): publish the groups (create_group_atomically, mod.rs:299-322, 568-581)
   std::lock_guard<std::shared_mutex> lk(p->mu);
@@ -1250,9 +1296,9 @@ static int merge_pass(pm_plugin* p, const std::vector<const Config*>& configs, c
   int rc = pm_interner_table(p->interner, &bits, &npat, &nmod, &words);
   if (rc != PM_OK) return p->fail(rc, "pm_interner_table");
   // merging works on its own small table (the nodes of solo groups only): a sibling engine, so that the formation
-  // pass's resident worker table stays where it is
+  // pass's resident worker table stays where it is.  Over a pm_multi it is device 0's: the table is small.
   if (!p->merge_engine) {
-    rc = pm_create_sibling(p->engine, &p->merge_engine);
+    rc = pm_create_sibling(p->dev.first(), &p->merge_engine);
     if (rc != PM_OK) return p->fail(rc, "pm_create_sibling");
   }
   pm_engine* const eng = p->merge_engine;
@@ -1285,7 +1331,7 @@ int pm_plugin_try_merge_solo_groups(pm_plugin* p, uint32_t* n_merged) try {
   std::lock_guard<std::mutex> loop_lk(p->loop_mu);
   std::lock_guard<std::shared_mutex> lk(p->mu);   // solo groups are few: the whole merge pass stays under the table lock
   if (n_merged) *n_merged = 0;
-  if (!p->engine) return p->fail(PM_E_NO_DEVICE, "no engine attached: merging has no CPU path");
+  if (!p->dev) return p->fail(PM_E_NO_DEVICE, "no engine attached: merging has no CPU path");
   auto solo_list = [&]() {
     std::vector<std::string> ids;  // std::map iterates in id order == get_all_groups() order
     for (const auto& kv : p->groups)

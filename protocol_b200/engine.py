@@ -412,6 +412,10 @@ class MultiEngine:
                                                       _ptr(lo) if lo is not None else None, len(idx)))
         self._check(self._lib.pm_multi_sync(self._h))
 
+    def table_version(self) -> int:
+        """Changes whenever a table call changed a table on any device (pm_multi_table_version)."""
+        return int(self._lib.pm_multi_table_version(self._h))
+
     def match(self, mode: int = abi.PM_MODE_FIRST_FIT):
         self._check(self._lib.pm_multi_match(self._h, mode))
 

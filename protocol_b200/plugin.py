@@ -10,6 +10,7 @@ from dataclasses import dataclass, field
 
 from . import abi
 from ._lib import PrimeMatchError, load
+from .engine import MultiEngine
 
 
 class NodeStatus:  # crates/orchestrator/src/models/node.rs:74-85
@@ -85,7 +86,8 @@ def _b(s):
 
 
 class NodeGroupsPlugin:
-    """NodeGroupsPlugin::new_with_policy (mod.rs:129-175)."""
+    """NodeGroupsPlugin::new_with_policy (mod.rs:129-175).  `engine` is an Engine, a MultiEngine (the formation pass
+    then runs on all of its GPUs) or None (no group formation).  Close the plugin before its engine."""
 
     def __init__(self, configuration_templates, engine=None, task_switching_enabled=True,
                  prefer_larger_groups=True, proximity_enabled=True, canonical_addresses=False):
@@ -93,9 +95,13 @@ class NodeGroupsPlugin:
         pol = abi.PmPluginPolicy(int(task_switching_enabled), int(prefer_larger_groups), int(proximity_enabled), int(canonical_addresses))
         h = C.c_void_p()
         self._engine = engine
-        rc = self._lib.pm_plugin_create(engine._h if engine is not None else None, C.byref(pol), C.byref(h))
+        if isinstance(engine, MultiEngine):
+            create, name = self._lib.pm_plugin_create_multi, "pm_plugin_create_multi"
+        else:
+            create, name = self._lib.pm_plugin_create, "pm_plugin_create"
+        rc = create(engine._h if engine is not None else None, C.byref(pol), C.byref(h))
         if rc != abi.PM_OK:
-            raise PrimeMatchError(rc, "pm_plugin_create")
+            raise PrimeMatchError(rc, name)
         self._h = h
         for c in configuration_templates:
             self._check(self._lib.pm_plugin_add_config(self._h, c.name.encode(), c.min_group_size, c.max_group_size,
