@@ -264,7 +264,7 @@ enum pm_path {
   PM_PATH_FUSED        = 1u << 8,/* evaluate + reduce on chip, matrix never written   */
   PM_NO_ASK_STATS      = 1u << 9,/* with PM_PATH_FUSED: skip ask_best / ask_count (the reference modes only
                                     need the per-worker first feasible ask); they read INF / 0 then      */
-  PM_INCREMENTAL       = 1u << 10 /* reuse the engine's stored per-worker first feasible ask: re-evaluate only the worker
+  PM_INCREMENTAL       = 1u << 10,/* reuse the engine's stored per-worker first feasible ask: re-evaluate only the worker
                                     rows written since the last evaluation on this engine, or everything when there is no
                                     valid stored evaluation or more rows changed than the cutoff (PM_TUNE_INCR at
                                     pm_create).  Every array pm_fetch_result returns equals the same call's without the
@@ -273,6 +273,9 @@ enum pm_path {
                                     engine through pm_match_local and with a communicator attached (pm_comm, pm_multi);
                                     PM_E_UNSUPPORTED from pm_match on a shard engine without a communicator.  See
                                     "Incremental passes" below */
+  PM_AUCTION_WARM      = 1u << 11 /* PM_MODE_AUCTION only (else PM_E_INVALID): start from the last auction pass's prices and
+                                    assignment, releasing only the asks the changes since disturb; a cold pass when there is
+                                    no stored state or the changes exceed the cutoff.  See "Auction warm start" below */
 };
 
 /* Incremental passes (PM_INCREMENTAL).  Every full evaluation, with the flag or without, keeps a copy of its
@@ -300,6 +303,27 @@ enum pm_path {
  *   evals    pair evaluations executed: T x nw on a full evaluation; on an incremental one the kernels' own count over
  *            the three walks (written rows, orphans, newly enabled asks) in the range; 0 when no row and no mask changed;
  *   n_tiles  worker rows walked in full: nw on a full evaluation, else the range's written rows + orphans.         */
+
+/* Auction warm start (PM_AUCTION_WARM).  Every successful auction pass, cold or warm, keeps its state on the device:
+ * the worker prices, the assignment, and the caps and reputation floors it ran with.  A warm pass (DESIGN 4):
+ *   1. changed rows R0: rows written through pm_upsert_workers, pm_update_workers, pm_set_flags or
+ *      pm_set_worker_reputation, and rows added by pm_resize_workers; changed asks A0: asks whose cap or floor differs
+ *      from the stored one, and asks toggled by pm_set_ask_enabled since;
+ *   2. releases every ask of A0, every owner of a row of R0 and every owner of a row a shrink removed: a released ask
+ *      gives up its worker, whose price becomes 0; every other unowned worker with a positive price (only an eps-scaled
+ *      pass leaves one) goes to 0 too.  Every changed row and every reset worker joins R;
+ *   3. releases, until nothing changes, every ask still holding w_t for which some w in R is feasible with
+ *      value(w) - 1 > value(w_t); its worker goes to price 0 and joins R;
+ *   4. runs the rounds at eps = 1 (whatever eps_start is) from that state, every unassigned ask active.
+ * The result is within T of the optimum of the current instance (the optimum with cost_scale = T + 1), as a cold
+ * pass's is; it need not equal the cold pass's result.  The warm pass runs when a stored state exists and
+ * |R0| + |A0| <= the PM_TUNE_INCR cutoff, else the pass is cold.  pm_set_asks, pm_set_model_table,
+ * pm_set_worker_count, pm_set_auction_params, pm_set_shard, pm_attach_comm and a failed auction pass discard the
+ * stored state; reference-mode passes leave it alone.  pm_stats of a warm pass: evals = the release's pair evaluations
+ * (classes x raised workers per iteration) + the rounds'; n_rounds = the warm rounds.
+ * pm_auction_state reports on the last auction pass: price [its n_workers] (or NULL), warm = 1 if it started warm,
+ * n_released = the asks its warm start released; PM_E_STATE when no auction pass ran since the state was discarded. */
+int pm_auction_state(pm_engine*, int64_t* price, uint32_t* warm, uint32_t* n_released);
 
 typedef struct pm_stats {
   uint64_t evals;            /* predicate evaluations executed on the device        */

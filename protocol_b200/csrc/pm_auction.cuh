@@ -100,6 +100,8 @@ struct AuctionCtl {
   uint32_t packed_claim;           // ... and fewer than 2^23 asks: bid_max[] holds (bid, bidder), pm_auction_claim has nothing to do
   unsigned long long evals;
   unsigned long long n_class_scans, n_ask_scans, n_refills;
+  uint32_t n_released;             // warm start: asks released from the stored assignment
+  uint32_t n_raised;               // ... workers whose price was reset (the list R of the release closure)
 };
 
 struct AuctionParams {
@@ -899,6 +901,100 @@ __global__ void pm_auction_gather_sorted(const uint4* __restrict__ wa, const uin
   pos_of[w] = i;
   price_s[i] = price[w];
   if (rep_s) rep_s[i] = rep[w];
+}
+
+// ---- warm start (PM_AUCTION_WARM) --------------------------------------------------------------
+// The stored state of the last pass (price, owner, assigned) is released where the changes since disturb it, then the
+// rounds run from what is left.  Every reset worker, and every changed row, joins the list R (`raised`) once; all of
+// them have price 0, so value(w) = -(ask_price[w] * S) on the whole list.
+__device__ __forceinline__ void auc_release(const AuctionParams& p, uint32_t t) {
+  const uint32_t w = atomicExch(p.assigned + t, kNone);   // an ask may be named twice (changed, and owner of a changed row)
+  if (w == kNone) return;
+  if (w < p.ev.n_workers) p.owner[w] = kNone;   // its price goes to 0 in pm_auction_warm_reset
+  atomicAdd(&p.ctl->n_released, 1u);
+}
+// the initial release: every ask holding a worker at or past n_kept (a row a shrink cut off since the stored state),
+// every owner of a changed row, every changed ask
+__global__ void pm_auction_warm_seed(AuctionParams p, const uint32_t* __restrict__ rows, uint32_t n_rows,
+                                     const uint32_t* __restrict__ changed_asks, uint32_t n_changed, uint32_t n_kept) {
+  const uint32_t T = p.n_asks, n = T + n_rows + n_changed;
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    if (i < T) {
+      const uint32_t w = p.assigned[i];
+      if (w != kNone && w >= n_kept) auc_release(p, i);
+    } else if (i < T + n_rows) {
+      const uint32_t t = p.owner[rows[i - T]];
+      if (t != kNone) auc_release(p, t);
+    } else {
+      auc_release(p, changed_asks[i - T - n_rows]);
+    }
+  }
+}
+// every unowned worker with a positive price (the released ones, and what an eps-scaled pass left inflated) goes to 0
+// and joins R; mark[w] says whether it did
+__global__ void pm_auction_warm_reset(AuctionParams p, uint32_t* __restrict__ raised, uint32_t* __restrict__ mark) {
+  const uint32_t W = p.ev.n_workers;
+  for (uint32_t w = blockIdx.x * blockDim.x + threadIdx.x; w < W; w += gridDim.x * blockDim.x) {
+    uint32_t m = 0u;
+    if (p.owner[w] == kNone && p.price[w] != 0) {
+      p.price[w] = 0;
+      raised[atomicAdd(&p.ctl->n_raised, 1u)] = w;
+      m = 1u;
+    }
+    mark[w] = m;
+  }
+}
+// ... and every changed row (the listed ones below n_kept, every row from n_kept on) that is not on R yet
+__global__ void pm_auction_warm_rows(AuctionParams p, const uint32_t* __restrict__ rows, uint32_t n_rows, uint32_t n_kept,
+                                     uint32_t* __restrict__ raised, uint32_t* __restrict__ mark) {
+  const uint32_t W = p.ev.n_workers, n = n_rows + (W > n_kept ? W - n_kept : 0u);
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const uint32_t w = i < n_rows ? rows[i] : n_kept + (i - n_rows);   // distinct rows: no two threads share a mark
+    if (!mark[w]) {
+      mark[w] = 1u;
+      raised[atomicAdd(&p.ctl->n_raised, 1u)] = w;
+    }
+  }
+}
+// Closure, step 1: C x |R_new| predicate evaluations.  cmin[c] = the lowest ask_price among the newly raised workers
+// class c accepts (reputation floor included): with every raised price at 0 that worker is, for each ask of the class
+// whose cap reaches it, its best raised worker.  One CTA per (class, 256 raised workers).
+__global__ void __launch_bounds__(256) pm_auction_release_classes(AuctionParams p, const uint32_t* __restrict__ raised, uint32_t lo,
+                                                                  uint32_t hi, const uint32_t* __restrict__ rep,
+                                                                  uint32_t* __restrict__ cmin) {
+  const uint32_t c = blockIdx.x;
+  const uint32_t i = lo + blockIdx.y * 256u + threadIdx.x;
+  const uint32_t t = p.class_rep[c];
+  const DevAsk ask = p.ev.asks[t];
+  const DevOpt opt0 = p.ev.opts[ask.n_opts ? ask.opt_off : 0u];
+  const uint32_t floor_rep = rep ? p.min_rep[t] : 0u;
+  uint32_t ap = 0xFFFFFFFFu;
+  if (i < hi) {
+    const uint32_t w = raised[i];
+    const WorkerReg wr = make_worker(p.ev.wa[w], p.ev.wb[w]);
+    if ((!rep || rep[w] >= floor_rep) && auc_meets(ask, opt0, p.ev.opts, wr, p.ev.bits, p.ev.words)) ap = wr.price;
+  }
+  ap = __reduce_min_sync(0xffffffffu, ap);
+  if ((threadIdx.x & 31u) == 0u && ap != 0xFFFFFFFFu) atomicMin(cmin + c, ap);
+}
+// Closure, step 2: an ask still holding w_t is released when its best affordable raised worker beats w_t by more than
+// eps (its eps-complementary slackness no longer holds); w_t goes to price 0 and joins R for the next iteration.
+__global__ void pm_auction_release_asks(AuctionParams p, const uint32_t* __restrict__ cmin, uint32_t* __restrict__ raised) {
+  for (uint32_t t = blockIdx.x * blockDim.x + threadIdx.x; t < p.n_asks; t += gridDim.x * blockDim.x) {
+    const uint32_t w = p.assigned[t];
+    if (w == kNone) continue;
+    const uint32_t m = cmin[p.class_of[t]];
+    if (m == 0xFFFFFFFFu || m > p.price_cap[t]) continue;
+    const long long v_raised = -((long long)m * p.scale);
+    const long long v_held = -((long long)p.ev.wb[w].w * p.scale) - p.price[w];
+    if (v_raised - p.eps > v_held) {
+      p.assigned[t] = kNone;
+      p.owner[w] = kNone;
+      p.price[w] = 0;
+      raised[atomicAdd(&p.ctl->n_raised, 1u)] = w;
+      atomicAdd(&p.ctl->n_released, 1u);
+    }
+  }
 }
 
 // result in the engine's group form: one solo group per assigned ask, in ask order

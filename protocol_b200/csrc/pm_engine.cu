@@ -441,6 +441,39 @@ struct pm_engine {
   bool have_rep = false, have_min_rep = false;
   uint64_t auc_scale = 1, auc_eps_start = 1;
   uint32_t auc_eps_div = 4;
+  // Auction warm start (PM_AUCTION_WARM).  The stored state is auc_price / auc_owner / auc_assigned as the last auction
+  // pass left them, over auc_state_w rows, with the caps and floors it ran with.  Rows and asks changed since are tracked
+  // here, apart from the reference modes' dirty_rows / toggled (a reference-mode pass clears those): rows below auc_kept
+  // one by one (auc_rows, each once; auc_rows_over past the cutoff), every row from auc_kept on as a range (rows a
+  // shrink cut off, or a resize added), and the asks toggled since.  Changed caps and floors are found by a diff.
+  bool auc_state = false;
+  uint32_t auc_state_w = 0, auc_kept = 0;
+  std::vector<uint8_t> auc_row_mark, auc_ask_mark;
+  std::vector<uint32_t> auc_rows, auc_toggled;
+  bool auc_rows_over = false;
+  std::vector<uint32_t> cap_host, floor_host, auc_cap_stored, auc_floor_stored;
+  bool auc_last_warm = false;   // pm_auction_state: the last pass
+  uint32_t auc_last_released = 0;
+  DevBuf<uint32_t> auc_raised, auc_mark, auc_cmin, auc_chg;
+  void auc_discard() {
+    auc_state = false;
+    auc_rows.clear();
+    auc_toggled.clear();
+    auc_row_mark.clear();
+    auc_ask_mark.clear();
+    auc_rows_over = false;
+  }
+  void auc_mark_row(uint32_t i) {
+    if (!auc_state || auc_rows_over || i >= auc_kept || auc_row_mark[i]) return;
+    auc_row_mark[i] = 1;
+    auc_rows.push_back(i);
+    if (auc_rows.size() > tune_incr) auc_rows_over = true;
+  }
+  void auc_mark_rows(uint32_t first, uint32_t n) {
+    if (!auc_state) return;
+    const uint32_t hi = (uint32_t)std::min<uint64_t>((uint64_t)first + n, auc_kept);
+    for (uint32_t i = first; i < hi && !auc_rows_over; ++i) auc_mark_row(i);
+  }
   DevBuf<uint32_t> worker_group, worker_ask, group_ask, group_off, members;
   PinBuf<uint32_t> h_scalars;  // small D2H mailbox
 
@@ -681,6 +714,7 @@ void pm_destroy(pm_engine* e) {
   e->auc_idx.release(); e->auc_sorted.release(); e->auc_incl.release(); e->auc_hash.release();
   e->auc_hash_out.release(); e->auc_wa_s.release(); e->auc_wb_s.release(); e->auc_price_s.release(); e->auc_ctl.release();
   e->h_ctl.release();
+  e->auc_raised.release(); e->auc_mark.release(); e->auc_cmin.release(); e->auc_chg.release();
   e->worker_group.release(); e->worker_ask.release(); e->group_ask.release();
   e->group_off.release(); e->members.release(); e->h_scalars.release();
   e->xchg_send.release(); e->xchg_recv.release();
@@ -701,6 +735,7 @@ int pm_set_asks(pm_engine* e, const pm_ask* asks, uint32_t n_asks, const pm_gpu_
   std::lock_guard<std::mutex> lk(e->mu);
   ++e->table_version;
   e->invalidate_eval();
+  e->auc_discard();
   if ((n_asks && !asks) || (n_opts && !opts)) return e->fail(PM_E_INVALID, "pm_set_asks: null table");
   if (n_asks >= (1u << 30)) return e->fail(PM_E_INVALID, "pm_set_asks: too many asks");
   PM_CUDA(cudaSetDevice(e->device));
@@ -806,6 +841,10 @@ int pm_set_ask_enabled(pm_engine* e, const uint32_t* idx, const uint8_t* enabled
       e->toggle_mark[t] = 1;
       e->toggled.push_back(t);
     }
+    if (e->auc_state && !e->auc_ask_mark[t]) {
+      e->auc_ask_mark[t] = 1;
+      e->auc_toggled.push_back(t);
+    }
   }
   e->rows_bound = false;           // the FastRows were converted again: pm_bind_rows binds them anew
   e->auc_classes_valid = false;
@@ -819,6 +858,7 @@ int pm_set_model_table(pm_engine* e, const uint32_t* bits, uint32_t n_patterns, 
   std::lock_guard<std::mutex> lk(e->mu);
   ++e->table_version;
   e->invalidate_eval();
+  e->auc_discard();
   if (words == 0) words = 1;
   if (n_patterns && !bits) return e->fail(PM_E_INVALID, "pm_set_model_table: null table");
   if ((uint64_t)words * 32 < n_models) return e->fail(PM_E_INVALID, "pm_set_model_table: words too small");
@@ -859,6 +899,7 @@ int pm_set_worker_count(pm_engine* e, uint32_t n_workers) try {
   std::lock_guard<std::mutex> lk(e->mu);
   ++e->table_version;
   e->invalidate_eval();
+  e->auc_discard();
   PM_CUDA(cudaSetDevice(e->device));
   if (n_workers > e->wa.n || !e->wa.p) {
     // grow, preserving nothing: callers upsert after (re)sizing
@@ -886,6 +927,7 @@ int pm_upsert_workers(pm_engine* e, const pm_worker_a* a, const pm_worker_b* b, 
   if ((uint64_t)first + n > e->n_workers) return e->fail(PM_E_INVALID, "pm_upsert_workers: range out of bounds");
   if (n && (!a || !b)) return e->fail(PM_E_INVALID, "pm_upsert_workers: null plane");
   e->mark_range_dirty(first, n);
+  e->auc_mark_rows(first, n);
   PM_CUDA(cudaSetDevice(e->device));
   if (n) {
     PM_CUDA(cudaMemcpyAsync(e->wa.p + first, a, (size_t)n * 16, cudaMemcpyHostToDevice, e->stream));
@@ -935,7 +977,10 @@ int pm_set_flags(pm_engine* e, const uint32_t* idx, const uint32_t* flags, uint3
   if (!e->have_workers) return e->fail(PM_E_STATE, "pm_set_flags: no worker table");
   if (n == 0) return PM_OK;
   if (!idx || !flags) return e->fail(PM_E_INVALID, "pm_set_flags: null");
-  for (uint32_t i = 0; i < n; ++i) e->mark_dirty(idx[i]);   // out-of-range indices are skipped, as the scatter does
+  for (uint32_t i = 0; i < n; ++i) {   // out-of-range indices are skipped, as the scatter does
+    e->mark_dirty(idx[i]);
+    e->auc_mark_row(idx[i]);
+  }
   PM_CUDA(cudaSetDevice(e->device));
   PM_CUDA(e->scratch_idx.ensure(n));
   PM_CUDA(e->scratch_flags.ensure(n));
@@ -992,6 +1037,15 @@ int pm_resize_workers(pm_engine* e, uint32_t n_workers) try {
     if (e->have_rep) PM_CUDA(cudaMemsetAsync(e->reputation.p + keep, 0, (size_t)(n_workers - keep) * 4, e->stream));
   }
   e->n_workers = n_workers;
+  if (e->auc_state && n_workers < e->auc_kept) {   // rows from the new end on count as changed from here on, as a range
+    e->auc_kept = n_workers;
+    size_t j = 0;
+    for (uint32_t i : e->auc_rows) {
+      if (i < n_workers) e->auc_rows[j++] = i;
+      else e->auc_row_mark[i] = 0;
+    }
+    e->auc_rows.resize(j);
+  }
   if (e->eval_valid) {
     // A communicator's equal share, or an open-ended pm_set_shard range, moves with W.  Rows that leave the range
     // return to NONE; rows that enter it were evaluated by another rank, or never: they are written.  Each is at most
@@ -1029,7 +1083,10 @@ int pm_update_workers(pm_engine* e, const uint32_t* idx, const pm_worker_a* a, c
   if (n == 0) return PM_OK;
   if (!idx || !a || !b || ((lat == nullptr) != (lon == nullptr))) return e->fail(PM_E_INVALID, "pm_update_workers: null");
   ++e->table_version;
-  for (uint32_t i = 0; i < n; ++i) e->mark_dirty(idx[i]);   // out-of-range indices are skipped, as the scatter does
+  for (uint32_t i = 0; i < n; ++i) {   // out-of-range indices are skipped, as the scatter does
+    e->mark_dirty(idx[i]);
+    e->auc_mark_row(idx[i]);
+  }
   PM_CUDA(cudaSetDevice(e->device));
   PM_CUDA(e->scratch_idx.ensure(n)); PM_CUDA(e->upd_a.ensure(n)); PM_CUDA(e->upd_b.ensure(n));
   PM_CUDA(cudaMemcpyAsync(e->scratch_idx.p, idx, (size_t)n * 4, cudaMemcpyHostToDevice, e->stream));
@@ -1748,7 +1805,8 @@ static int auction_build_classes(pm_engine* e) {
   return PM_OK;
 }
 
-static int match_auction_locked(pm_engine* e) {
+static int auction_pass(pm_engine* e, bool want_warm);
+static int match_auction_locked(pm_engine* e, uint32_t mode) {
   if (!e->have_workers || !e->have_asks) return e->fail(PM_E_STATE, "pm_match: worker and ask tables must be set first");
   if (!e->have_caps) return e->fail(PM_E_STATE, "pm_match: auction mode needs pm_set_ask_price_caps");
   if (e->max_pattern_row > e->n_patterns || (e->max_pattern_row && !e->have_bits))
@@ -1756,6 +1814,12 @@ static int match_auction_locked(pm_engine* e) {
   if (e->cfg.shard_count || e->comm) return e->fail(PM_E_UNSUPPORTED, "pm_match: auction mode is single-GPU");
   // the class cache is keyed on requirement rows, which a disabled ask's no longer are
   if (e->n_off) return e->fail(PM_E_UNSUPPORTED, "pm_match: auction mode with disabled asks");
+  const int rc = auction_pass(e, (mode & PM_AUCTION_WARM) != 0);
+  if (rc != PM_OK) e->auc_discard();   // the stored state may be half released or half bid: it is not trusted again
+  return rc;
+}
+
+static int auction_pass(pm_engine* e, bool want_warm) {
   PM_CUDA(cudaSetDevice(e->device));
   const uint32_t W = e->n_workers, T = e->n_asks;
   if (!e->have_bits) {
@@ -1774,8 +1838,25 @@ static int match_auction_locked(pm_engine* e) {
   }
   const uint32_t C = e->auc_n_classes;
   const unsigned kScanGrid = 2u * e->sms;   // two scanning CTAs per SM (shared memory)
-  PM_CUDA(e->auc_price.ensure((size_t)W + 2)); PM_CUDA(e->auc_owner.ensure(W)); PM_CUDA(e->auc_bid_max.ensure(W));
-  PM_CUDA(e->auc_winner.ensure(W)); PM_CUDA(e->auc_assigned.ensure(T)); PM_CUDA(e->auc_withdrawn.ensure(T));
+  // Warm start from the stored state when there is one and the changed rows R0 plus the changed asks A0 stay within the
+  // cutoff.  A0: caps or floors that differ from the stored ones (a diff of the host copies), and asks toggled since.
+  std::vector<uint32_t> changed;   // the listed rows of R0, then A0
+  bool warm = false;
+  uint32_t n_kept = 0;
+  if (want_warm && e->auc_state && !e->auc_rows_over) {
+    changed = e->auc_rows;
+    for (uint32_t t = 0; t < T; ++t) {
+      const uint32_t fl = e->have_min_rep ? e->floor_host[t] : 0u;
+      if (e->cap_host[t] != e->auc_cap_stored[t] || fl != e->auc_floor_stored[t] || e->auc_ask_mark[t]) changed.push_back(t);
+    }
+    n_kept = std::min(e->auc_kept, W);
+    warm = (uint64_t)changed.size() + (W - n_kept) <= e->tune_incr;
+  }
+  const uint32_t n_rows = warm ? (uint32_t)e->auc_rows.size() : 0u, n_chg = warm ? (uint32_t)changed.size() - n_rows : 0u;
+  // the stored state survives the buffers' growth (a resize since the last pass); a cold pass overwrites it below
+  PM_CUDA(e->auc_price.grow_keep((size_t)W + 2, e->auc_price.n, e->stream)); PM_CUDA(e->auc_owner.grow_keep(W, e->auc_owner.n, e->stream));
+  PM_CUDA(e->auc_assigned.grow_keep(T, e->auc_assigned.n, e->stream));
+  PM_CUDA(e->auc_bid_max.ensure(W)); PM_CUDA(e->auc_winner.ensure(W)); PM_CUDA(e->auc_withdrawn.ensure(T));
   PM_CUDA(e->auc_active.ensure((size_t)2 * std::max<uint32_t>(T, 1))); PM_CUDA(e->auc_bid_w.ensure(T)); PM_CUDA(e->auc_bid_p.ensure(T));
   PM_CUDA(e->auc_flag.ensure((size_t)T + 1)); PM_CUDA(e->auc_gidx.ensure((size_t)T + 1));
   PM_CUDA(e->auc_theta.ensure(C)); PM_CUDA(e->auc_theta_w.ensure(C)); PM_CUDA(e->auc_cand.ensure((size_t)C * pm::kAucCache));
@@ -1793,7 +1874,12 @@ static int match_auction_locked(pm_engine* e) {
   PM_CUDA(e->worker_group.ensure(W)); PM_CUDA(e->worker_ask.ensure(W)); PM_CUDA(e->members.ensure(std::max(W, T)));
   PM_CUDA(e->group_ask.ensure((size_t)T + 1)); PM_CUDA(e->group_off.ensure((size_t)T + 2));
   PM_CUDA(e->ask_best.ensure(T)); PM_CUDA(e->ask_count.ensure(T)); PM_CUDA(e->first_ask.ensure(W));
-  PM_CUDA(cudaMemsetAsync(e->auc_price.p, 0, ((size_t)W + 2) * 8, e->stream));
+  if (warm) {   // rows from n_kept on were cut off or added since the stored state: unowned, price 0
+    if (W > n_kept) PM_CUDA(cudaMemsetAsync(e->auc_owner.p + n_kept, 0xFF, (size_t)(W - n_kept) * 4, e->stream));
+    PM_CUDA(cudaMemsetAsync(e->auc_price.p + n_kept, 0, ((size_t)W + 2 - n_kept) * 8, e->stream));
+  } else {
+    PM_CUDA(cudaMemsetAsync(e->auc_price.p, 0, ((size_t)W + 2) * 8, e->stream));
+  }
   PM_CUDA(cudaMemsetAsync(e->auc_price_s.p, 0, ((size_t)W + 2) * 8, e->stream));
   PM_CUDA(cudaMemsetAsync(e->auc_ctl.p, 0, sizeof(pm::AuctionCtl), e->stream));
   PM_CUDA(cudaMemsetAsync(e->auc_class_req.p, 0, (size_t)std::max<uint32_t>(C, 1) * 4, e->stream));
@@ -1809,9 +1895,68 @@ static int match_auction_locked(pm_engine* e) {
     PM_CUDA(e->auc_rep_s.ensure((size_t)W + 4));
     PM_CUDA(cudaMemsetAsync(e->auc_rep_s.p, 0, ((size_t)W + 4) * 4, e->stream));
   }
+  pm::AuctionParams ap;
+  ap.ev = eval_params(e);
+  ap.wa_s = e->auc_wa_s.p; ap.wb_s = e->auc_wb_s.p; ap.perm = e->auc_perm.p; ap.pos_of = e->auc_pos_of.p; ap.price_s = e->auc_price_s.p;
+  ap.csort_s = reinterpret_cast<const unsigned long long*>(e->auc_ckey_s.p);
+  ap.rep_s = use_rep ? e->auc_rep_s.p : nullptr; ap.min_rep = use_rep ? e->ask_min_rep.p : nullptr;
+  ap.price_cap = e->price_cap.p; ap.price = e->auc_price.p; ap.owner = e->auc_owner.p; ap.assigned = e->auc_assigned.p;
+  ap.withdrawn = e->auc_withdrawn.p; ap.active = e->auc_active.p; ap.n_asks = T; ap.bid_w = e->auc_bid_w.p; ap.bid_p = e->auc_bid_p.p;
+  ap.bid_max = e->auc_bid_max.p; ap.winner = e->auc_winner.p; ap.scale = (long long)e->auc_scale;
+  ap.class_of = e->auc_class_of.p; ap.class_rep = e->auc_class_rep.p; ap.class_req = e->auc_class_req.p;
+  ap.cand = e->auc_cand.p; ap.theta = e->auc_theta.p; ap.theta_w = e->auc_theta_w.p;
+  ap.pool = e->auc_pool.p; ap.pool_bound_v = e->auc_pool_bound_v.p; ap.pool_bound_w = e->auc_pool_bound_w.p;
+  ap.walk_list = e->auc_walk_list.p; ap.split_bound_v = e->auc_split_v.p; ap.split_bound_w = e->auc_split_w.p; ap.split_ticket = e->auc_split_ticket.p; ap.split_first = e->auc_split_first.p;
+  ap.skip_key = reinterpret_cast<unsigned long long*>(e->auc_skip_key.p);
+  ap.class_list = e->auc_class_list.p; ap.retry = e->auc_retry.p; ap.fallback = e->auc_fallback.p; ap.ctl = e->auc_ctl.p;
+  ap.dbg = (uint32_t)e->tune_auction;
+  ap.pool_good = e->tune_auc_good > 0 ? (uint32_t)e->tune_auc_good : (uint32_t)pm::kAucPoolGood;
+  ap.pool_extra = e->tune_auc_extra > 0 ? (uint32_t)e->tune_auc_extra : (uint32_t)pm::kAucPoolExtra;
   if (W) {
     pm::pm_fill_i64<<<std::min(blocks_for(W, 256), 8u * e->sms), 256, 0, e->stream>>>(e->auc_bid_max.p, pm::kAucNeg, W);
     PM_LAUNCH_CHECK("pm_fill_i64");
+  }
+  // Release (warm start, steps 2 and 3 of DESIGN 4): the initial release and price reset, then the closure — per
+  // iteration C x |R_new| predicate evaluations and one compare per still-assigned ask, one poll of the control block.
+  // Every reset happens here, before the first sort of the worker copy: within the rounds sort keys still only rise.
+  uint64_t closure_evals = 0;
+  uint32_t n_released = 0;
+  if (warm) {
+    PM_CUDA(e->auc_raised.ensure(std::max<uint32_t>(W, 1))); PM_CUDA(e->auc_mark.ensure(std::max<uint32_t>(W, 1)));
+    PM_CUDA(e->auc_cmin.ensure(std::max<uint32_t>(C, 1))); PM_CUDA(e->auc_chg.ensure(std::max<size_t>(changed.size(), 1)));
+    if (!changed.empty()) PM_CUDA(cudaMemcpyAsync(e->auc_chg.p, changed.data(), changed.size() * 4, cudaMemcpyHostToDevice, e->stream));
+    ap.eps = 1;
+    const unsigned g_seed = std::max(1u, std::min(blocks_for((size_t)T + changed.size(), 256), 8u * e->sms));
+    pm::pm_auction_warm_seed<<<g_seed, 256, 0, e->stream>>>(ap, e->auc_chg.p, n_rows, e->auc_chg.p + n_rows, n_chg, n_kept);
+    PM_LAUNCH_CHECK("pm_auction_warm_seed");
+    if (W) {
+      const unsigned g_w = std::max(1u, std::min(blocks_for(W, 256), 8u * e->sms));
+      pm::pm_auction_warm_reset<<<g_w, 256, 0, e->stream>>>(ap, e->auc_raised.p, e->auc_mark.p);
+      PM_LAUNCH_CHECK("pm_auction_warm_reset");
+      pm::pm_auction_warm_rows<<<g_w, 256, 0, e->stream>>>(ap, e->auc_chg.p, n_rows, n_kept, e->auc_raised.p, e->auc_mark.p);
+      PM_LAUNCH_CHECK("pm_auction_warm_rows");
+    }
+    const unsigned g_t = std::max(1u, std::min(blocks_for(T, 256), 8u * e->sms));
+    const uint32_t kYChunk = 65535u * 256u;   // raised workers per launch of pm_auction_release_classes (grid.y limit)
+    uint32_t lo = 0;
+    for (;;) {
+      PM_CUDA(cudaMemcpyAsync(e->h_ctl.p, e->auc_ctl.p, sizeof(pm::AuctionCtl), cudaMemcpyDeviceToHost, e->stream));
+      PM_CUDA(cudaStreamSynchronize(e->stream));
+      const uint32_t hi = e->h_ctl.p->n_raised;
+      if (hi == lo || C == 0) break;
+      PM_CUDA(cudaMemsetAsync(e->auc_cmin.p, 0xFF, (size_t)C * 4, e->stream));
+      for (uint32_t s0 = lo; s0 < hi; s0 += kYChunk) {
+        const uint32_t s1 = std::min(hi, s0 + kYChunk);
+        pm::pm_auction_release_classes<<<dim3(C, (s1 - s0 + 255) / 256), 256, 0, e->stream>>>(
+            ap, e->auc_raised.p, s0, s1, use_rep ? e->reputation.p : nullptr, e->auc_cmin.p);
+        PM_LAUNCH_CHECK("pm_auction_release_classes");
+      }
+      pm::pm_auction_release_asks<<<g_t, 256, 0, e->stream>>>(ap, e->auc_cmin.p, e->auc_raised.p);
+      PM_LAUNCH_CHECK("pm_auction_release_asks");
+      closure_evals += (uint64_t)C * (hi - lo);
+      lo = hi;
+    }
+    n_released = e->h_ctl.p->n_released;
   }
   // worker planes sorted by (ask_price * S + price, index): stable radix sort; redone as prices move (below)
   auto sort_workers = [&]() -> int {
@@ -1835,29 +1980,15 @@ static int match_auction_locked(pm_engine* e) {
   PM_CUDA(cudaMemsetAsync(e->auc_winner.p, 0xFF, (size_t)std::max<uint32_t>(W, 1) * 4, e->stream));
   // one packed 64-bit sort key per candidate when every reachable cost fits (decided on the device, read by the kernels)
   pm::pm_auction_limits<<<std::max(1u, std::min(blocks_for(std::max(W, T), 256), 4u * e->sms)), 256, 0, e->stream>>>(e->wb.p, W, e->price_cap.p, T, e->auc_ctl.p);
-  pm::pm_auction_decide_packed<<<1, 1, 0, e->stream>>>(e->auc_ctl.p, W, T, e->auc_scale, e->auc_eps_start ? e->auc_eps_start : 1, (uint32_t)e->tune_auction);
+  // (a warm pass: every price an ask kept was bid under its unchanged cap at eps = 1, every other price is 0, so the
+  // bound on reachable costs is the cold one at eps = 1)
+  pm::pm_auction_decide_packed<<<1, 1, 0, e->stream>>>(e->auc_ctl.p, W, T, e->auc_scale, warm ? 1 : (e->auc_eps_start ? e->auc_eps_start : 1),
+                                                       (uint32_t)e->tune_auction);
   PM_LAUNCH_CHECK("pm_auction_decide_packed");
   PM_CUDA(cudaMemcpyAsync(e->h_ctl.p, e->auc_ctl.p, sizeof(pm::AuctionCtl), cudaMemcpyDeviceToHost, e->stream));
   PM_CUDA(cudaStreamSynchronize(e->stream));
   const bool packed_claim = e->h_ctl.p->packed_claim != 0;   // then no round launches pm_auction_claim at all
 
-  pm::AuctionParams ap;
-  ap.ev = eval_params(e);
-  ap.wa_s = e->auc_wa_s.p; ap.wb_s = e->auc_wb_s.p; ap.perm = e->auc_perm.p; ap.pos_of = e->auc_pos_of.p; ap.price_s = e->auc_price_s.p;
-  ap.csort_s = reinterpret_cast<const unsigned long long*>(e->auc_ckey_s.p);
-  ap.rep_s = use_rep ? e->auc_rep_s.p : nullptr; ap.min_rep = use_rep ? e->ask_min_rep.p : nullptr;
-  ap.price_cap = e->price_cap.p; ap.price = e->auc_price.p; ap.owner = e->auc_owner.p; ap.assigned = e->auc_assigned.p;
-  ap.withdrawn = e->auc_withdrawn.p; ap.active = e->auc_active.p; ap.n_asks = T; ap.bid_w = e->auc_bid_w.p; ap.bid_p = e->auc_bid_p.p;
-  ap.bid_max = e->auc_bid_max.p; ap.winner = e->auc_winner.p; ap.scale = (long long)e->auc_scale;
-  ap.class_of = e->auc_class_of.p; ap.class_rep = e->auc_class_rep.p; ap.class_req = e->auc_class_req.p;
-  ap.cand = e->auc_cand.p; ap.theta = e->auc_theta.p; ap.theta_w = e->auc_theta_w.p;
-  ap.pool = e->auc_pool.p; ap.pool_bound_v = e->auc_pool_bound_v.p; ap.pool_bound_w = e->auc_pool_bound_w.p;
-  ap.walk_list = e->auc_walk_list.p; ap.split_bound_v = e->auc_split_v.p; ap.split_bound_w = e->auc_split_w.p; ap.split_ticket = e->auc_split_ticket.p; ap.split_first = e->auc_split_first.p;
-  ap.skip_key = reinterpret_cast<unsigned long long*>(e->auc_skip_key.p);
-  ap.class_list = e->auc_class_list.p; ap.retry = e->auc_retry.p; ap.fallback = e->auc_fallback.p; ap.ctl = e->auc_ctl.p;
-  ap.dbg = (uint32_t)e->tune_auction;
-  ap.pool_good = e->tune_auc_good > 0 ? (uint32_t)e->tune_auc_good : (uint32_t)pm::kAucPoolGood;
-  ap.pool_extra = e->tune_auc_extra > 0 ? (uint32_t)e->tune_auc_extra : (uint32_t)pm::kAucPoolExtra;
   const size_t smem = pm::kAucStages * sizeof(pm::AuctionStage) + sizeof(pm::AuctionMerge);
   PM_CUDA(cudaFuncSetAttribute(pm::pm_auction_scan, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   // fixed grids: every kernel strides over a list whose length it reads from the control block
@@ -1868,17 +1999,21 @@ static int match_auction_locked(pm_engine* e) {
   const unsigned g_thr = std::max(1u, std::min(blocks_for(T, 256), 4u * e->sms));
   const uint32_t kBatch = 32;  // rounds launched between polls of the control block
   const uint32_t kResort = (e->tune_auction >> 8) ? (uint32_t)(e->tune_auction >> 8) : 4u;   // batches between re-sorts of the worker copy
-  uint64_t eps = e->auc_eps_start ? e->auc_eps_start : 1;
+  uint64_t eps = warm ? 1 : (e->auc_eps_start ? e->auc_eps_start : 1);   // a warm pass is one phase at eps = 1
   const uint32_t div = e->auc_eps_div < 2 ? 2 : e->auc_eps_div;
+  bool first_phase = true;
   for (;;) {  // eps phases: assignment cleared, prices (and so the class caches' bounds) kept
-    PM_CUDA(cudaMemsetAsync(e->auc_owner.p, 0xFF, (size_t)std::max<uint32_t>(W, 1) * 4, e->stream));
-    PM_CUDA(cudaMemsetAsync(e->auc_assigned.p, 0xFF, (size_t)std::max<uint32_t>(T, 1) * 4, e->stream));
+    if (!warm) {   // a warm pass starts from the released state: every unassigned ask is active (withdrawn ones too)
+      PM_CUDA(cudaMemsetAsync(e->auc_owner.p, 0xFF, (size_t)std::max<uint32_t>(W, 1) * 4, e->stream));
+      PM_CUDA(cudaMemsetAsync(e->auc_assigned.p, 0xFF, (size_t)std::max<uint32_t>(T, 1) * 4, e->stream));
+    }
     PM_CUDA(cudaMemsetAsync(e->auc_withdrawn.p, 0, (size_t)std::max<uint32_t>(T, 1) * 4, e->stream));
-    if (C && eps == (e->auc_eps_start ? e->auc_eps_start : 1)) {  // no cache yet: "invalid" sends every class to a scan
+    if (C && first_phase) {  // no cache yet (on every pass, warm or cold): "invalid" sends every class to a scan
       pm::pm_fill_i64<<<std::min(blocks_for(C, 256), 8u * e->sms), 256, 0, e->stream>>>(e->auc_theta.p, pm::kThetaInvalid, C);
       pm::pm_fill_i64<<<std::min(blocks_for(C, 256), 8u * e->sms), 256, 0, e->stream>>>(e->auc_pool_bound_v.p, pm::kThetaInvalid, C);
       PM_LAUNCH_CHECK("pm_fill_i64");
     }
+    first_phase = false;
     ap.eps = (long long)eps;
     if (T) {
       pm::pm_auction_compact<<<blocks_for(T, 256), 256, 0, e->stream>>>(ap, T);
@@ -1942,7 +2077,7 @@ static int match_auction_locked(pm_engine* e) {
     eps = std::max<uint64_t>(1, eps / div);
   }
   e->stats.n_rounds = e->h_ctl.p->rounds;
-  e->stats.evals = e->h_ctl.p->evals;
+  e->stats.evals = e->h_ctl.p->evals + closure_evals;
   e->stats.n_tiles = (uint32_t)std::min<unsigned long long>(e->h_ctl.p->n_class_scans, 0xFFFFFFFFull);
   e->stats.n_fused_launches = (uint32_t)std::min<unsigned long long>(e->h_ctl.p->n_ask_scans, 0xFFFFFFFFull);
   e->stats.n_launches = e->h_ctl.p->rounds * (packed_claim ? 6u : 7u);
@@ -1979,10 +2114,36 @@ static int match_auction_locked(pm_engine* e) {
     PM_CUDA(cudaEventElapsedTime(&e->stats.ms_total, e->ev0, e->ev1));
     e->resolve_timers();
   }
+  // the stored state for the next warm start: prices, owners and assignment stay in their buffers
+  e->auc_discard();
+  e->auc_state = true;
+  e->auc_state_w = e->auc_kept = W;
+  e->auc_row_mark.assign(W, 0);
+  e->auc_ask_mark.assign(T, 0);
+  e->auc_cap_stored = e->cap_host;
+  if (e->have_min_rep) e->auc_floor_stored = e->floor_host;
+  else e->auc_floor_stored.assign(T, 0u);
+  e->auc_last_warm = warm;
+  e->auc_last_released = n_released;
   e->matched = true;
   e->local_done = false;
   return PM_OK;
 }
+
+// The last auction pass: its prices, whether it started warm, how many asks its warm start released.
+int pm_auction_state(pm_engine* e, int64_t* price, uint32_t* warm, uint32_t* n_released) try {
+  if (!e) return PM_E_INVALID;
+  std::lock_guard<std::mutex> lk(e->mu);
+  if (!e->auc_state) return e->fail(PM_E_STATE, "pm_auction_state: no auction pass since the engine's tables were last replaced");
+  PM_CUDA(cudaSetDevice(e->device));
+  if (price && e->auc_state_w) {
+    PM_CUDA(cudaMemcpyAsync(price, e->auc_price.p, (size_t)e->auc_state_w * 8, cudaMemcpyDeviceToHost, e->stream));
+    PM_CUDA(cudaStreamSynchronize(e->stream));
+  }
+  if (warm) *warm = e->auc_last_warm ? 1u : 0u;
+  if (n_released) *n_released = e->auc_last_released;
+  return PM_OK;
+} catch (...) { return pm_guard_rc(); }
 
 int pm_set_ask_price_caps(pm_engine* e, const uint32_t* price_cap, uint32_t n_asks) try {
   if (!e) return PM_E_INVALID;
@@ -1992,6 +2153,7 @@ int pm_set_ask_price_caps(pm_engine* e, const uint32_t* price_cap, uint32_t n_as
   PM_CUDA(e->price_cap.ensure(n_asks));
   if (n_asks) PM_CUDA(cudaMemcpyAsync(e->price_cap.p, price_cap, (size_t)n_asks * 4, cudaMemcpyHostToDevice, e->stream));
   PM_CUDA(cudaStreamSynchronize(e->stream));
+  e->cap_host.assign(price_cap, price_cap + n_asks);   // a warm start finds the changed caps by a diff
   e->have_caps = true;
   return PM_OK;
 } catch (...) { return pm_guard_rc(); }
@@ -2009,6 +2171,7 @@ int pm_set_worker_reputation(pm_engine* e, const uint32_t* reputation, uint32_t 
     PM_CUDA(e->reputation.ensure(std::max<size_t>(e->wa.n, 1)));
     PM_CUDA(cudaMemsetAsync(e->reputation.p, 0, std::max<size_t>(e->wa.n, 1) * 4, e->stream));
   }
+  e->auc_mark_rows(first, n);   // the auction reads reputation: for its warm start these rows changed
   if (n) PM_CUDA(cudaMemcpyAsync(e->reputation.p + first, reputation, (size_t)n * 4, cudaMemcpyHostToDevice, e->stream));
   PM_CUDA(cudaStreamSynchronize(e->stream));
   e->have_rep = true;
@@ -2025,6 +2188,7 @@ int pm_set_ask_min_reputation(pm_engine* e, const uint32_t* min_reputation, uint
   PM_CUDA(e->ask_min_rep.ensure(std::max<uint32_t>(n_asks, 1)));
   if (n_asks) PM_CUDA(cudaMemcpyAsync(e->ask_min_rep.p, min_reputation, (size_t)n_asks * 4, cudaMemcpyHostToDevice, e->stream));
   PM_CUDA(cudaStreamSynchronize(e->stream));
+  e->floor_host.assign(min_reputation, min_reputation + n_asks);
   e->have_min_rep = true;
   e->auc_classes_valid = false;   // the floor is part of an ask's class
   e->matched = e->local_done = false;
@@ -2034,6 +2198,7 @@ int pm_set_ask_min_reputation(pm_engine* e, const uint32_t* min_reputation, uint
 int pm_set_auction_params(pm_engine* e, uint64_t cost_scale, uint64_t eps_start, uint32_t eps_div) try {
   if (!e) return PM_E_INVALID;
   std::lock_guard<std::mutex> lk(e->mu);
+  e->auc_discard();
   e->auc_scale = cost_scale ? cost_scale : 1;
   e->auc_eps_start = eps_start ? eps_start : 1;
   e->auc_eps_div = eps_div < 2 ? 2 : eps_div;
@@ -2078,6 +2243,8 @@ static int exchange_locked(pm_engine* e) {
 // three arrays); pm_match on a shard engine without a communicator refuses it: that call resolves one range as if it
 // were the table, so there is no whole-table result to keep incremental.
 static int check_incremental(pm_engine* e, uint32_t mode, bool local) {
+  if ((mode & PM_AUCTION_WARM) && (mode & 0xFFu) != PM_MODE_AUCTION)
+    return e->fail(PM_E_INVALID, "pm_match: PM_AUCTION_WARM is for the auction only");
   if (!(mode & PM_INCREMENTAL)) return PM_OK;
   if ((mode & 0xFFu) == PM_MODE_AUCTION) return e->fail(PM_E_INVALID, "pm_match: PM_INCREMENTAL is for the reference modes, not the auction");
   if ((mode & (PM_PATH_FUSED | PM_NO_ASK_STATS)) != (PM_PATH_FUSED | PM_NO_ASK_STATS))
@@ -2104,6 +2271,7 @@ int pm_match_local(pm_engine* e, uint32_t mode) try {
 int pm_match_finish(pm_engine* e, uint32_t mode) try {
   if (!e) return PM_E_INVALID;
   std::lock_guard<std::mutex> lk(e->mu);
+  if (mode & PM_AUCTION_WARM) return e->fail(PM_E_INVALID, "pm_match_finish: PM_AUCTION_WARM is for the auction only");
   return invalidate_on_failure(e, match_finish_locked(e, mode));
 } catch (...) { return pm_guard_rc(); }
 int pm_match(pm_engine* e, uint32_t mode) try {
@@ -2111,7 +2279,7 @@ int pm_match(pm_engine* e, uint32_t mode) try {
   std::lock_guard<std::mutex> lk(e->mu);
   int rc = check_incremental(e, mode, false);
   if (rc != PM_OK) return rc;
-  if ((mode & 0xFFu) == PM_MODE_AUCTION) return match_auction_locked(e);
+  if ((mode & 0xFFu) == PM_MODE_AUCTION) return match_auction_locked(e, mode);
   rc = match_local_locked(e, mode);
   if (rc != PM_OK) return invalidate_on_failure(e, rc);
   if (e->comm && e->comm->n_ranks > 1) {
@@ -2127,6 +2295,7 @@ int pm_set_shard(pm_engine* e, uint32_t first, uint32_t count) try {
   e->cfg.shard_first = first;
   e->cfg.shard_count = count;
   e->invalidate_eval();
+  e->auc_discard();
   e->matched = e->local_done = false;
   return PM_OK;
 } catch (...) { return pm_guard_rc(); }
@@ -2179,6 +2348,7 @@ int pm_attach_comm(pm_engine* e, pm_comm* c) try {
   if (c && c->device != e->device) return e->fail(PM_E_INVALID, "pm_attach_comm: communicator and engine are on different devices");
   e->comm = c;
   e->invalidate_eval();
+  e->auc_discard();
   e->matched = e->local_done = false;
   return PM_OK;
 } catch (...) { return pm_guard_rc(); }

@@ -123,6 +123,7 @@ class Engine:
             raise PrimeMatchError(rc, (self._lib.pm_last_error(None) or b"").decode())
         self._h = h
         self.n_workers = 0
+        self._auction_workers = 0   # workers of the last auction pass (auction_state)
         self.n_asks = 0
 
     def close(self):
@@ -224,9 +225,19 @@ class Engine:
     def set_auction_params(self, cost_scale: int = 1, eps_start: int = 1, eps_div: int = 4):
         self._check(self._lib.pm_set_auction_params(self._h, cost_scale, eps_start, eps_div))
 
+    def auction_state(self, prices: bool = True):
+        """The last auction pass (pm_auction_state): (prices i64[n_workers of that pass] or None, started warm, asks
+        released by its warm start)."""
+        price = np.zeros(self._auction_workers, dtype=np.int64) if prices else None
+        warm, released = C.c_uint32(), C.c_uint32()
+        self._check(self._lib.pm_auction_state(self._h, _ptr(price) if prices else None, C.byref(warm), C.byref(released)))
+        return price, bool(warm.value), int(released.value)
+
     # ---- the pass ---------------------------------------------------------
     def match(self, mode: int = abi.PM_MODE_FIRST_FIT):
         self._check(self._lib.pm_match(self._h, mode))
+        if mode & 0xFF == abi.PM_MODE_AUCTION:
+            self._auction_workers = self.n_workers   # the length of the prices auction_state() returns
 
     def match_local(self, mode: int = abi.PM_MODE_FIRST_FIT):
         self._check(self._lib.pm_match_local(self._h, mode))

@@ -1,0 +1,127 @@
+"""Warm-started auction passes (PM_AUCTION_WARM) at 100k asks x 1M workers, BASELINE configs[2]'s instance (the one
+tools/auction_scale.py and tests/test_gpu_parity.py build).
+
+One cold pass, then warm passes after 0, 10, 1 000 and 100 000 rewritten worker rows, with the rows drawn from unowned
+workers (nothing to release but the raised rows' own competition) and from owned workers (every owner released, and
+the release cascades through its class), and after 100 changed caps.  Each warm pass is followed by a cold pass of
+the same tables in the same run, so cold and warm times sit side by side.  Per pass: wall ms (host clock around
+pm_match, which ends in a device synchronise), ms_fused (CUDA events around the pass), rounds, released asks, evals.
+The card's name and power limit are read in the same run.  One JSON line per pass; a summary table on stderr.
+
+    python tools/auction_warm_bench.py [--out results/auction_warm.json]
+"""
+from __future__ import annotations
+
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+
+import numpy as np
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from protocol_b200 import abi, synth  # noqa: E402
+from protocol_b200.engine import Engine  # noqa: E402
+
+NONE = 0xFFFFFFFF
+
+
+def card():
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
+                             text=True, timeout=30).stdout.strip().splitlines()
+        return out[0] if out else "unknown"
+    except Exception as ex:   # noqa: BLE001
+        return f"unknown ({ex})"
+
+
+def instance():
+    T, W = 100_000, 1_000_000
+    w = synth.make_workers(W, seed=synth.SEED_WORKERS)
+    a = synth.make_asks(T, "mixed", seed=synth.SEED_ASKS)
+    bits, npat, nmod, words = synth.intern_tables(w, a)
+    wb = w.b.copy()
+    wb["ext_ask_price"] = np.exp(np.log(10) + synth._unit(synth.SEED_EXT, W, 1) * np.log(200)).astype(np.uint32)
+    cap = np.exp(np.log(20) + synth._unit(synth.SEED_EXT, T, 2) * np.log(150)).astype(np.uint32)
+    return a, w.a.copy(), wb, bits, npat, nmod, words, cap
+
+
+def timed(eng, mode):
+    t0 = time.perf_counter()
+    eng.match(mode)
+    ms = (time.perf_counter() - t0) * 1e3
+    st = eng.stats()
+    _, warm, released = eng.auction_state(prices=False)
+    return dict(wall_ms=round(ms, 2), ms_fused=round(st["ms_fused"], 2), rounds=st["n_rounds"], warm=warm,
+                released=released, evals=st["evals"])
+
+
+def assigned_of(eng, T):
+    res = eng.fetch()
+    got = np.full(T, NONE, dtype=np.uint32)
+    got[res.group_ask] = res.group_members
+    return got
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--out", default=None)
+    ap.add_argument("--counts", default="0,10,1000,100000")
+    args = ap.parse_args()
+    gpu = card()
+    print(f"card: {gpu}", file=sys.stderr)
+    a, wa, wb, bits, npat, nmod, words, cap = instance()
+    T, W = len(cap), len(wa)
+    eng = Engine(timing=True)
+    eng.set_asks(a.asks, a.opts)
+    eng.set_model_table(bits, npat, nmod, words)
+    eng.set_workers(wa, wb)
+    eng.set_price_caps(cap)
+    rows = []
+
+    def record(case, n, r):
+        r = dict(case=case, n=n, **r, card=gpu)
+        rows.append(r)
+        print(json.dumps(r), flush=True)
+
+    warm_mode = abi.PM_MODE_AUCTION | abi.PM_AUCTION_WARM
+    record("cold", 0, timed(eng, abi.PM_MODE_AUCTION))
+    rng = np.random.default_rng(1)
+    for variant in ("unowned", "owned"):
+        for n in [int(x) for x in args.counts.split(",")]:
+            eng.match(abi.PM_MODE_AUCTION)                 # the stored state: a cold pass of the current tables
+            got = assigned_of(eng, T)
+            owned = np.zeros(W, dtype=bool)
+            owned[got[got != NONE]] = True
+            pool = np.flatnonzero(owned if variant == "owned" else ~owned)
+            idx = np.sort(rng.choice(pool, size=min(n, len(pool)), replace=False)).astype(np.uint32)
+            if len(idx):
+                b = wb[idx].copy()
+                b["ext_ask_price"] = np.maximum(1, (b["ext_ask_price"] * rng.uniform(0.5, 1.5, len(idx))).astype(np.uint32))
+                wb[idx] = b
+                eng.update_workers(idx, wa[idx], b)
+            record(f"warm_rows_{variant}", int(len(idx)), timed(eng, warm_mode))
+            record("cold", 0, timed(eng, abi.PM_MODE_AUCTION))
+    eng.match(abi.PM_MODE_AUCTION)
+    cap2 = cap.copy()
+    idx = rng.choice(T, 100, replace=False)
+    cap2[idx] = np.maximum(1, (cap2[idx] * rng.uniform(0.5, 1.5, 100)).astype(np.uint32))
+    eng.set_price_caps(cap2)
+    record("warm_caps", 100, timed(eng, warm_mode))
+    record("cold", 0, timed(eng, abi.PM_MODE_AUCTION))
+    eng.close()
+    print(f"{'case':>20} {'n':>7} {'wall ms':>9} {'ms_fused':>9} {'rounds':>7} {'warm':>5} {'released':>9} {'evals':>14}",
+          file=sys.stderr)
+    for r in rows:
+        print(f"{r['case']:>20} {r['n']:>7} {r['wall_ms']:>9} {r['ms_fused']:>9} {r['rounds']:>7} {int(r['warm']):>5} "
+              f"{r['released']:>9} {r['evals']:>14}", file=sys.stderr)
+    if args.out:
+        os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
+        with open(args.out, "w") as f:
+            json.dump(dict(card=gpu, rows=rows), f, indent=1)
+
+
+if __name__ == "__main__":
+    main()
