@@ -273,9 +273,12 @@ enum pm_path {
                                     engine through pm_match_local and with a communicator attached (pm_comm, pm_multi);
                                     PM_E_UNSUPPORTED from pm_match on a shard engine without a communicator.  See
                                     "Incremental passes" below */
-  PM_AUCTION_WARM      = 1u << 11 /* PM_MODE_AUCTION only (else PM_E_INVALID): start from the last auction pass's prices and
+  PM_AUCTION_WARM      = 1u << 11,/* PM_MODE_AUCTION only (else PM_E_INVALID): start from the last auction pass's prices and
                                     assignment, releasing only the asks the changes since disturb; a cold pass when there is
                                     no stored state or the changes exceed the cutoff.  See "Auction warm start" below */
+  PM_AUCTION_REVERSE   = 1u << 12 /* PM_MODE_AUCTION only, not with PM_AUCTION_WARM (else PM_E_INVALID): every eps phase
+                                    ends with reverse rounds that return every unowned worker to price 0, which makes
+                                    eps_start > 1 keep the eps = 1 bound.  See "Auction reverse rounds" below */
 };
 
 /* Incremental passes (PM_INCREMENTAL).  Every full evaluation, with the flag or without, keeps a copy of its
@@ -324,6 +327,28 @@ enum pm_path {
  * pm_auction_state reports on the last auction pass: price [its n_workers] (or NULL), warm = 1 if it started warm,
  * n_released = the asks its warm start released; PM_E_STATE when no auction pass ran since the state was discarded. */
 int pm_auction_state(pm_engine*, int64_t* price, uint32_t* warm, uint32_t* n_released);
+
+/* Auction reverse rounds (PM_AUCTION_REVERSE).  Each eps phase (eps_start, eps_start / eps_div, ..., 1) runs the
+ * forward rounds as without the bit (assignment cleared, prices kept, until every ask holds a worker or withdrew), then
+ * reverse rounds until no unowned worker has a positive price.  With S = cost_scale, a(w) = -(ask_price[w] * S), an
+ * ask's profit pi(t) = a(w_t) - price[w_t] when it holds w_t, else -(cap[t] + 1) * S.  One reverse round, every bid
+ * reading the state at the round's start:
+ *   - the bidders are the unowned workers with price > 0;
+ *   - a bidder w takes g(t) = a(w) - pi(t) over the asks it is feasible for (candidate, compatible, ask_price <= cap,
+ *     reputation >= floor): beta the largest, t* the lowest ask reaching it, omega the second value of the multiset;
+ *   - no feasible ask, or beta <= eps: price[w] = 0 and w stays unowned;
+ *   - else w offers itself to t* at p' = max(0, omega - eps);
+ *   - each ask takes the offer with the highest a(w) - p' (ties: the lowest worker): the worker's price becomes p', the
+ *     ask holds it (withdrawn or not before), and the ask's previous worker becomes unowned at its price.
+ * The reverse rounds keep eps-complementary slackness and end with every unowned worker at price 0, so the final
+ * eps = 1 phase gives a total cost within T of the optimum (the optimum with cost_scale = T + 1), whatever eps_start
+ * is (DESIGN 4).  With eps_start = 1 there is nothing to do: the pass equals the pass without the bit.  The pass
+ * stores its state like any auction pass; a later PM_AUCTION_WARM pass may start from it.  pm_stats: n_rounds counts
+ * the forward rounds; evals adds the reverse rounds' predicate evaluations (classes x bids); with PM_CFG_TIMING,
+ * ms_build is the time of the reverse rounds (part of ms_fused).
+ * pm_auction_reverse_stats reports on the last auction pass: its eps phases, reverse rounds and bids (each NULL-able),
+ * all 0 for a pass without the bit; PM_E_STATE where pm_auction_state returns it. */
+int pm_auction_reverse_stats(pm_engine*, uint32_t* n_phases, uint32_t* n_reverse_rounds, uint64_t* n_reverse_bids);
 
 typedef struct pm_stats {
   uint64_t evals;            /* predicate evaluations executed on the device        */

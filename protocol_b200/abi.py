@@ -50,6 +50,7 @@ PM_MODE_FIRST_FIT, PM_MODE_PROXIMITY, PM_MODE_AUCTION, PM_MODE_PROXIMITY_MERGE =
 PM_PATH_MATERIALIZED, PM_PATH_FUSED, PM_NO_ASK_STATS = 0, 1 << 8, 1 << 9
 PM_INCREMENTAL = 1 << 10   # re-evaluate only the worker rows written since the stored evaluation (prime_match.h)
 PM_AUCTION_WARM = 1 << 11  # PM_MODE_AUCTION: start from the last auction pass's prices and assignment (prime_match.h)
+PM_AUCTION_REVERSE = 1 << 12  # PM_MODE_AUCTION: end every eps phase with reverse rounds (prime_match.h)
 
 PM_BUF_WORKER_FIRST_ASK, PM_BUF_ASK_BEST, PM_BUF_ASK_COUNT = 0, 1, 2
 
@@ -114,7 +115,7 @@ EXPORTS = [
     "pm_set_asks", "pm_set_ask_enabled", "pm_set_model_table", "pm_set_worker_count", "pm_upsert_workers",
     "pm_set_worker_locations", "pm_set_worker_addr_rank", "pm_set_flags",
     "pm_set_ask_price_caps", "pm_set_auction_params", "pm_set_worker_reputation", "pm_set_ask_min_reputation",
-    "pm_auction_state",
+    "pm_auction_state", "pm_auction_reverse_stats",
     "pm_match", "pm_fetch_result", "pm_get_stats", "pm_build_cost_tile",
     "pm_match_local", "pm_match_finish", "pm_device_buffer", "pm_stream_sync", "pm_set_shard",
     "pm_resize_workers", "pm_update_workers", "pm_table_version", "pm_create_sibling",

@@ -64,6 +64,9 @@
 // each stripe), items drawn from a counter because their lengths differ by two orders of magnitude.
 // Collisions are resolved by atomicMax on (bid, bidder) packed in one word — or, when they do not fit, by atomicMax on
 // the bid and atomicMin on the bidder (pm_auction_claim) — applied by the single winner of each worker.
+//
+// PM_AUCTION_REVERSE ends every eps phase with reverse rounds (the section at the end): they only lower prices, so the
+// engine rebuilds the class caches and the worker order after a stage that lowered one.
 #pragma once
 #include "pm_kernels.cuh"
 
@@ -102,6 +105,11 @@ struct AuctionCtl {
   unsigned long long n_class_scans, n_ask_scans, n_refills;
   uint32_t n_released;             // warm start: asks released from the stored assignment
   uint32_t n_raised;               // ... workers whose price was reset (the list R of the release closure)
+  uint32_t n_bid;                  // reverse stage: bidders of the current round (unowned, positive price)
+  uint32_t rev_last;               // ... of the last round run (0: the stage is over)
+  uint32_t rev_rounds;             // ... rounds with at least one bidder, over the pass
+  uint32_t rev_lowered;            // ... some price went down since the host last cleared this
+  unsigned long long rev_bids;     // ... bids over the pass
 };
 
 struct AuctionParams {
@@ -956,6 +964,15 @@ __global__ void pm_auction_warm_rows(AuctionParams p, const uint32_t* __restrict
     }
   }
 }
+// Does class c accept worker w (compatibility and the reputation floor, both part of the class; the cap is per ask)?
+// rep: the `reputation` column in worker order, or null when no floor was given.
+__device__ __forceinline__ bool auc_class_accepts(const AuctionParams& p, uint32_t c, const WorkerReg& wr, uint32_t w,
+                                                  const uint32_t* __restrict__ rep) {
+  const uint32_t t = p.class_rep[c];
+  const DevAsk ask = p.ev.asks[t];
+  const DevOpt opt0 = p.ev.opts[ask.n_opts ? ask.opt_off : 0u];
+  return (!rep || rep[w] >= p.min_rep[t]) && auc_meets(ask, opt0, p.ev.opts, wr, p.ev.bits, p.ev.words);
+}
 // Closure, step 1: C x |R_new| predicate evaluations.  cmin[c] = the lowest ask_price among the newly raised workers
 // class c accepts (reputation floor included): with every raised price at 0 that worker is, for each ask of the class
 // whose cap reaches it, its best raised worker.  One CTA per (class, 256 raised workers).
@@ -964,15 +981,11 @@ __global__ void __launch_bounds__(256) pm_auction_release_classes(AuctionParams 
                                                                   uint32_t* __restrict__ cmin) {
   const uint32_t c = blockIdx.x;
   const uint32_t i = lo + blockIdx.y * 256u + threadIdx.x;
-  const uint32_t t = p.class_rep[c];
-  const DevAsk ask = p.ev.asks[t];
-  const DevOpt opt0 = p.ev.opts[ask.n_opts ? ask.opt_off : 0u];
-  const uint32_t floor_rep = rep ? p.min_rep[t] : 0u;
   uint32_t ap = 0xFFFFFFFFu;
   if (i < hi) {
     const uint32_t w = raised[i];
     const WorkerReg wr = make_worker(p.ev.wa[w], p.ev.wb[w]);
-    if ((!rep || rep[w] >= floor_rep) && auc_meets(ask, opt0, p.ev.opts, wr, p.ev.bits, p.ev.words)) ap = wr.price;
+    if (auc_class_accepts(p, c, wr, w, rep)) ap = wr.price;
   }
   ap = __reduce_min_sync(0xffffffffu, ap);
   if ((threadIdx.x & 31u) == 0u && ap != 0xFFFFFFFFu) atomicMin(cmin + c, ap);
@@ -995,6 +1008,185 @@ __global__ void pm_auction_release_asks(AuctionParams p, const uint32_t* __restr
       atomicAdd(&p.ctl->n_released, 1u);
     }
   }
+}
+
+// ---- reverse rounds (PM_AUCTION_REVERSE) -----------------------------------------------------------
+// Every eps phase ends with them: the unowned workers whose price is still positive (what a coarser phase left
+// stranded) bid for asks, synchronously, until none is left.  With a(w) = -(ask_price[w] * S) and the ask's profit
+// pi(t) = a(w_t) - price[w_t] when it holds w_t, else outside(t): a bidder w takes the gains g(t) = a(w) - pi(t) over
+// its feasible asks, best beta on t* (lowest ask among equals), second value omega of the multiset; beta <= eps (or no
+// feasible ask) sends its price to 0, else it offers itself to t* at p' = max(0, omega - eps).  Each ask takes the
+// offer of highest profit a(w) - p' (ties: lowest worker); its previous worker becomes unowned at its price.
+// All of a round reads the state of its start: the collect step writes the asks' profits before anyone bids.
+constexpr uint32_t kRevChunk = 8192;   // classes per chunk of the bid's class mask (1 KB of shared memory)
+constexpr unsigned long long kRevPackLim = 1ull << 40;   // packed offer: (2^40 - 1 - cost) << 24 | (2^24 - 1 - worker)
+
+struct AuctionRev {
+  uint32_t* bidders;           // [W] this round's bidders (ctl->n_bid of them)
+  uint32_t* offer_t;           // [W] per bidder: the ask it offers itself to, or kNone (its price went to 0)
+  long long* offer_p;          // [W] ... the price it offers at
+  long long* best;             // [T] per ask: the best packed offer key (0: none), or unpacked the best profit
+  uint32_t* win;               // [T] unpacked: the lowest worker among the ask's best offers
+  long long* pi_s;             // [T] profit of the ask at sorted position i, at the start of the round
+  const uint32_t* cap_s;       // [T] cap of the ask at sorted position i
+  const uint32_t* sorted;      // [T] asks in class order (the class build's sort): each class is one run
+  const uint32_t* cls_s;       // [T] class of sorted position i, plus one (the class build's inclusive scan)
+  const uint32_t* cstart;      // [C + 1] first sorted position of each class
+  const uint32_t* rep;         // [W] `reputation` in worker order, or null (no floor given)
+  uint32_t n_classes;
+};
+
+__device__ __forceinline__ bool auc_rev_packed(const AuctionParams& p) { return p.ctl->packed != 0u && !(p.dbg & 128u); }
+
+// once per pass: the run of each class in sorted order, and the caps in that order
+__global__ void pm_auction_rev_classes(const uint32_t* __restrict__ sorted, const uint32_t* __restrict__ incl,
+                                       const uint32_t* __restrict__ cap, uint32_t n_asks, uint32_t n_classes,
+                                       uint32_t* __restrict__ cstart, uint32_t* __restrict__ cap_s) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_asks) return;
+  cap_s[i] = cap[sorted[i]];
+  if (i == 0 || incl[i] != incl[i - 1]) cstart[incl[i] - 1u] = i;
+  if (i == n_asks - 1u) cstart[n_classes] = n_asks;
+}
+
+// Start of a round: the bidder list, every ask's profit (in sorted order), no offers yet.
+__global__ void pm_auction_rev_collect(AuctionParams p, AuctionRev r) {
+  const uint32_t W = p.ev.n_workers, T = p.n_asks, n = max(W, T);
+  const bool pk = auc_rev_packed(p);
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    if (i < W && p.owner[i] == kNone && p.price[i] > 0) r.bidders[atomicAdd(&p.ctl->n_bid, 1u)] = i;
+    if (i < T) {
+      const uint32_t wt = p.assigned[r.sorted[i]];
+      r.pi_s[i] = wt != kNone ? -((long long)p.ev.wb[wt].w * p.scale) - p.price[wt] : -(((long long)r.cap_s[i] + 1) * p.scale);
+      r.best[i] = pk ? 0ll : kAucNeg;   // (indexed by ask: i runs over all of them)
+      r.win[i] = kNone;
+    }
+  }
+}
+
+// (best gain, its ask, second value) of two parts of the multiset
+__device__ __forceinline__ void auc_rev_merge(long long& g1, uint32_t& t1, long long& g2, long long o1, uint32_t ot1, long long o2) {
+  if (o1 > g1 || (o1 == g1 && ot1 < t1)) { g2 = max(g1, o2); g1 = o1; t1 = ot1; }
+  else g2 = max(g2, o1);
+}
+
+// One CTA per bidder: C predicate evaluations against the class representatives give a class mask in shared memory
+// (kRevChunk classes at a time), then a walk over the asks of those classes in sorted order — class bit, cap, gain —
+// keeps the best two; thread 0 drops the price to 0 or posts the offer.
+__global__ void __launch_bounds__(kAucThreads, 4) pm_auction_rev_bid(AuctionParams p, AuctionRev r) {
+  __shared__ uint32_t mask[kRevChunk / 32];
+  __shared__ long long red_g1[kAucWarps], red_g2[kAucWarps];
+  __shared__ uint32_t red_t1[kAucWarps];
+  const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+  const uint32_t n = p.ctl->n_bid, C = r.n_classes;
+  const bool pk = auc_rev_packed(p);
+  for (uint32_t slot = blockIdx.x; slot < n; slot += gridDim.x) {
+    const uint32_t w = r.bidders[slot];
+    const WorkerReg wr = make_worker(p.ev.wa[w], p.ev.wb[w]);
+    const long long a = -((long long)wr.price * p.scale);
+    long long g1 = kAucNeg, g2 = kAucNeg;
+    uint32_t t1 = kNone;
+    for (uint32_t c0 = 0; c0 < C; c0 += kRevChunk) {
+      const uint32_t nc = min(C - c0, kRevChunk);
+      const uint32_t kmax = (nc + kAucThreads - 1u) / kAucThreads * kAucThreads;   // the same trip count on every thread
+      for (uint32_t k = threadIdx.x; k < kmax; k += kAucThreads) {
+        const bool ok = k < nc && auc_class_accepts(p, c0 + k, wr, w, r.rep);
+        const uint32_t m = __ballot_sync(0xffffffffu, ok);   // warp-aligned k: one mask word per warp
+        if (lane == 0) mask[k >> 5] = m;
+      }
+      __syncthreads();
+      // four positions per thread and step, their class loads issued together (the walk is latency-bound)
+      const uint32_t i1 = r.cstart[c0 + nc];
+      for (uint32_t i = r.cstart[c0] + threadIdx.x; i < i1; i += 4u * kAucThreads) {
+        uint32_t cs[4];
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+          const uint32_t j = i + (uint32_t)u * kAucThreads;
+          cs[u] = j < i1 ? r.cls_s[j] - 1u - c0 : kNone;
+        }
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+          const uint32_t j = i + (uint32_t)u * kAucThreads, c = cs[u];
+          if (c != kNone && ((mask[c >> 5] >> (c & 31u)) & 1u) && r.cap_s[j] >= wr.price) {
+            const long long g = a - r.pi_s[j];
+            const uint32_t t = r.sorted[j];
+            if (g > g1 || (g == g1 && t < t1)) { g2 = g1; g1 = g; t1 = t; }
+            else g2 = max(g2, g);
+          }
+        }
+      }
+      __syncthreads();   // the mask is rewritten by the next chunk
+    }
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) {
+      const long long o1 = __shfl_xor_sync(0xffffffffu, g1, off), o2 = __shfl_xor_sync(0xffffffffu, g2, off);
+      const uint32_t ot = __shfl_xor_sync(0xffffffffu, t1, off);
+      auc_rev_merge(g1, t1, g2, o1, ot, o2);
+    }
+    if (lane == 0) { red_g1[warp] = g1; red_g2[warp] = g2; red_t1[warp] = t1; }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      for (uint32_t k = 1; k < (uint32_t)kAucWarps; ++k) auc_rev_merge(g1, t1, g2, red_g1[k], red_t1[k], red_g2[k]);
+      if (t1 == kNone || g1 <= p.eps) {   // nothing worth offering: the price goes to 0, the worker stays unowned
+        p.price[w] = 0;
+        p.price_s[p.pos_of[w]] = 0;
+        r.offer_t[slot] = kNone;
+        p.ctl->rev_lowered = 1u;
+      } else {
+        const long long pn = max(0ll, g2 - p.eps);   // no second value: kAucNeg, so 0
+        const long long profit = a - pn;
+        r.offer_t[slot] = t1;
+        r.offer_p[slot] = pn;
+        // packed: the highest profit, among equal ones the lowest worker, is the largest key (every cost < 2^40, W < 2^24)
+        if (pk) atomicMax(reinterpret_cast<unsigned long long*>(r.best) + t1,
+                          ((kRevPackLim - 1ull - (unsigned long long)(-profit)) << kAucPackShift) | (unsigned long long)(((1u << kAucPackShift) - 1u) - w));
+        else atomicMax(r.best + t1, profit);
+      }
+    }
+    __syncthreads();   // red_* are reused by the CTA's next bidder
+  }
+}
+
+// unpacked offers: among the best offers on an ask the lowest worker wins
+__global__ void pm_auction_rev_claim(AuctionParams p, AuctionRev r) {
+  if (auc_rev_packed(p)) return;
+  const uint32_t n = p.ctl->n_bid;
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const uint32_t t = r.offer_t[i];
+    if (t == kNone) continue;
+    const uint32_t w = r.bidders[i];
+    if (-((long long)p.ev.wb[w].w * p.scale) - r.offer_p[i] == r.best[t]) atomicMin(r.win + t, w);
+  }
+}
+
+// The winners take their asks; an ask's previous worker becomes unowned at its price (it bids next round if that is
+// positive).  Asks only gain or trade up here: nobody is pushed back into the forward rounds.
+__global__ void pm_auction_rev_apply(AuctionParams p, AuctionRev r) {
+  const uint32_t n = p.ctl->n_bid;
+  const bool pk = auc_rev_packed(p);
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const uint32_t t = r.offer_t[i];
+    if (t == kNone) continue;
+    const uint32_t w = r.bidders[i];
+    const bool won = pk ? (uint32_t)((1u << kAucPackShift) - 1u) - (uint32_t)((unsigned long long)r.best[t] & ((1ull << kAucPackShift) - 1ull)) == w
+                        : r.win[t] == w;
+    if (!won) continue;
+    const uint32_t prev = p.assigned[t];
+    if (prev != kNone) p.owner[prev] = kNone;
+    p.owner[w] = t;
+    p.assigned[t] = w;
+    p.withdrawn[t] = 0u;
+    const long long pn = r.offer_p[i];
+    if (pn < p.price[w]) p.ctl->rev_lowered = 1u;
+    p.price[w] = pn;
+    p.price_s[p.pos_of[w]] = pn;
+  }
+}
+__global__ void pm_auction_rev_advance(AuctionCtl* ctl) {
+  const uint32_t n = ctl->n_bid;
+  if (n) { ++ctl->rev_rounds; ctl->rev_bids += n; }
+  ctl->rev_last = n;
+  ctl->n_bid = 0;
 }
 
 // result in the engine's group form: one solo group per assigned ask, in ask order

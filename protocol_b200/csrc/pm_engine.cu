@@ -454,7 +454,12 @@ struct pm_engine {
   std::vector<uint32_t> cap_host, floor_host, auc_cap_stored, auc_floor_stored;
   bool auc_last_warm = false;   // pm_auction_state: the last pass
   uint32_t auc_last_released = 0;
+  uint32_t auc_last_phases = 0, auc_last_rev_rounds = 0;   // pm_auction_reverse_stats: the last pass (0 without the bit)
+  uint64_t auc_last_rev_bids = 0;
   DevBuf<uint32_t> auc_raised, auc_mark, auc_cmin, auc_chg;
+  // reverse rounds (PM_AUCTION_REVERSE): bidder list and offers, per-ask profits and caps in class order, class runs
+  DevBuf<uint32_t> auc_rev_bidders, auc_rev_offer_t, auc_rev_win, auc_rev_cap_s, auc_rev_cstart;
+  DevBuf<long long> auc_rev_offer_p, auc_rev_best, auc_rev_pi_s;
   void auc_discard() {
     auc_state = false;
     auc_rows.clear();
@@ -715,6 +720,8 @@ void pm_destroy(pm_engine* e) {
   e->auc_hash_out.release(); e->auc_wa_s.release(); e->auc_wb_s.release(); e->auc_price_s.release(); e->auc_ctl.release();
   e->h_ctl.release();
   e->auc_raised.release(); e->auc_mark.release(); e->auc_cmin.release(); e->auc_chg.release();
+  e->auc_rev_bidders.release(); e->auc_rev_offer_t.release(); e->auc_rev_win.release(); e->auc_rev_cap_s.release();
+  e->auc_rev_cstart.release(); e->auc_rev_offer_p.release(); e->auc_rev_best.release(); e->auc_rev_pi_s.release();
   e->worker_group.release(); e->worker_ask.release(); e->group_ask.release();
   e->group_off.release(); e->members.release(); e->h_scalars.release();
   e->xchg_send.release(); e->xchg_recv.release();
@@ -1805,7 +1812,7 @@ static int auction_build_classes(pm_engine* e) {
   return PM_OK;
 }
 
-static int auction_pass(pm_engine* e, bool want_warm);
+static int auction_pass(pm_engine* e, bool want_warm, bool reverse);
 static int match_auction_locked(pm_engine* e, uint32_t mode) {
   if (!e->have_workers || !e->have_asks) return e->fail(PM_E_STATE, "pm_match: worker and ask tables must be set first");
   if (!e->have_caps) return e->fail(PM_E_STATE, "pm_match: auction mode needs pm_set_ask_price_caps");
@@ -1814,12 +1821,12 @@ static int match_auction_locked(pm_engine* e, uint32_t mode) {
   if (e->cfg.shard_count || e->comm) return e->fail(PM_E_UNSUPPORTED, "pm_match: auction mode is single-GPU");
   // the class cache is keyed on requirement rows, which a disabled ask's no longer are
   if (e->n_off) return e->fail(PM_E_UNSUPPORTED, "pm_match: auction mode with disabled asks");
-  const int rc = auction_pass(e, (mode & PM_AUCTION_WARM) != 0);
+  const int rc = auction_pass(e, (mode & PM_AUCTION_WARM) != 0, (mode & PM_AUCTION_REVERSE) != 0);
   if (rc != PM_OK) e->auc_discard();   // the stored state may be half released or half bid: it is not trusted again
   return rc;
 }
 
-static int auction_pass(pm_engine* e, bool want_warm) {
+static int auction_pass(pm_engine* e, bool want_warm, bool reverse) {
   PM_CUDA(cudaSetDevice(e->device));
   const uint32_t W = e->n_workers, T = e->n_asks;
   if (!e->have_bits) {
@@ -2001,6 +2008,63 @@ static int auction_pass(pm_engine* e, bool want_warm) {
   const uint32_t kResort = (e->tune_auction >> 8) ? (uint32_t)(e->tune_auction >> 8) : 4u;   // batches between re-sorts of the worker copy
   uint64_t eps = warm ? 1 : (e->auc_eps_start ? e->auc_eps_start : 1);   // a warm pass is one phase at eps = 1
   const uint32_t div = e->auc_eps_div < 2 ? 2 : e->auc_eps_div;
+  // Reverse rounds (PM_AUCTION_REVERSE): per round collect the bidders and the asks' profits, one CTA per bid, (claim),
+  // apply, advance; batched into one CUDA graph per phase like the forward rounds, one poll of the control block per batch.
+  const bool rev_on = reverse && T && W;
+  pm::AuctionRev rv{};
+  if (rev_on) {
+    PM_CUDA(e->auc_rev_bidders.ensure(W)); PM_CUDA(e->auc_rev_offer_t.ensure(W)); PM_CUDA(e->auc_rev_offer_p.ensure(W));
+    PM_CUDA(e->auc_rev_best.ensure(T)); PM_CUDA(e->auc_rev_win.ensure(T)); PM_CUDA(e->auc_rev_pi_s.ensure(T));
+    PM_CUDA(e->auc_rev_cap_s.ensure(T)); PM_CUDA(e->auc_rev_cstart.ensure((size_t)C + 1));
+    rv.bidders = e->auc_rev_bidders.p; rv.offer_t = e->auc_rev_offer_t.p; rv.offer_p = e->auc_rev_offer_p.p;
+    rv.best = e->auc_rev_best.p; rv.win = e->auc_rev_win.p; rv.pi_s = e->auc_rev_pi_s.p; rv.cap_s = e->auc_rev_cap_s.p;
+    rv.sorted = e->auc_sorted.p; rv.cls_s = e->auc_incl.p; rv.cstart = e->auc_rev_cstart.p;
+    rv.rep = use_rep ? e->reputation.p : nullptr; rv.n_classes = C;
+    pm::pm_auction_rev_classes<<<blocks_for(T, 256), 256, 0, e->stream>>>(e->auc_sorted.p, e->auc_incl.p, e->price_cap.p, T, C,
+                                                                          e->auc_rev_cstart.p, e->auc_rev_cap_s.p);
+    PM_LAUNCH_CHECK("pm_auction_rev_classes");
+  }
+  const bool rev_packed = e->h_ctl.p->packed != 0 && !(e->tune_auction & 128);   // then no round launches pm_auction_rev_claim
+  const unsigned g_rev = std::max(1u, std::min(blocks_for(std::max(W, T), 256), 8u * e->sms));
+  const unsigned g_rev_bid = 4u * e->sms;   // 64 registers per thread (no spills): four resident CTAs per SM
+  const uint32_t kRevBatch = 16;   // reverse rounds launched between polls of the control block
+  uint32_t n_phases = 0;
+  auto reverse_stage = [&]() -> int {
+    auto launch_rev = [&]() {
+      for (uint32_t r = 0; r < kRevBatch; ++r) {
+        pm::pm_auction_rev_collect<<<g_rev, 256, 0, e->stream>>>(ap, rv);
+        pm::pm_auction_rev_bid<<<g_rev_bid, pm::kAucThreads, 0, e->stream>>>(ap, rv);
+        if (!rev_packed) pm::pm_auction_rev_claim<<<g_rev, 256, 0, e->stream>>>(ap, rv);
+        pm::pm_auction_rev_apply<<<g_rev, 256, 0, e->stream>>>(ap, rv);
+        pm::pm_auction_rev_advance<<<1, 1, 0, e->stream>>>(e->auc_ctl.p);
+      }
+    };
+    cudaGraph_t graph = nullptr;
+    cudaGraphExec_t graph_exec = nullptr;
+    if (cudaStreamBeginCapture(e->stream, cudaStreamCaptureModeThreadLocal) == cudaSuccess) {
+      launch_rev();
+      if (cudaStreamEndCapture(e->stream, &graph) != cudaSuccess || cudaGraphInstantiate(&graph_exec, graph, 0) != cudaSuccess) {
+        if (graph) cudaGraphDestroy(graph);
+        graph = nullptr;
+        graph_exec = nullptr;
+      }
+    }
+    (void)cudaGetLastError();
+    int rc = PM_OK;
+    for (;;) {
+      cudaError_t ce;
+      if (graph_exec) ce = cudaGraphLaunch(graph_exec, e->stream);
+      else { launch_rev(); ce = cudaGetLastError(); }
+      if (ce == cudaSuccess) ce = cudaMemcpyAsync(e->h_ctl.p, e->auc_ctl.p, sizeof(pm::AuctionCtl), cudaMemcpyDeviceToHost, e->stream);
+      if (ce == cudaSuccess) ce = cudaStreamSynchronize(e->stream);
+      if (ce != cudaSuccess) { rc = e->fail(PM_E_CUDA, std::string("pm_match: auction reverse rounds: ") + cudaGetErrorString(ce)); break; }
+      if (e->h_ctl.p->rev_last == 0) break;
+      if (e->h_ctl.p->rev_rounds > 50u * 1000u * 1000u) { rc = e->fail(PM_E_CUDA, "pm_match: auction reverse rounds did not terminate"); break; }
+    }
+    if (graph_exec) cudaGraphExecDestroy(graph_exec);
+    if (graph) cudaGraphDestroy(graph);
+    return rc;
+  };
   bool first_phase = true;
   for (;;) {  // eps phases: assignment cleared, prices (and so the class caches' bounds) kept
     if (!warm) {   // a warm pass starts from the released state: every unassigned ask is active (withdrawn ones too)
@@ -2073,11 +2137,32 @@ static int auction_pass(pm_engine* e, bool want_warm) {
     if (graph_exec) cudaGraphExecDestroy(graph_exec);
     if (graph) cudaGraphDestroy(graph);
     if (rc_rounds != PM_OK) return rc_rounds;
+    ++n_phases;
+    if (rev_on) {
+      Timer trv(e, &e->stats.ms_build, e->stream);   // (auction mode builds no cost tile: ms_build is the reverse rounds)
+      const int rc = reverse_stage();
+      trv.stop();
+      if (rc != PM_OK) return rc;
+      // The class caches, pool bounds, skip keys and the worker copy's order rest on "prices only rise": a stage that
+      // lowered a price leaves them to be rebuilt before the next phase's forward rounds (after the last phase nothing
+      // reads them, and the next pass starts them afresh).
+      if (e->h_ctl.p->rev_lowered && eps != 1) {
+        if (C) {
+          pm::pm_fill_i64<<<std::min(blocks_for(C, 256), 8u * e->sms), 256, 0, e->stream>>>(e->auc_theta.p, pm::kThetaInvalid, C);
+          pm::pm_fill_i64<<<std::min(blocks_for(C, 256), 8u * e->sms), 256, 0, e->stream>>>(e->auc_pool_bound_v.p, pm::kThetaInvalid, C);
+          PM_LAUNCH_CHECK("pm_fill_i64");
+          PM_CUDA(cudaMemsetAsync(e->auc_skip_key.p, 0, (size_t)C * 8, e->stream));
+        }
+        PM_CUDA(cudaMemsetAsync(&e->auc_ctl.p->rev_lowered, 0, sizeof(uint32_t), e->stream));
+        const int rs = sort_workers();
+        if (rs != PM_OK) return rs;
+      }
+    }
     if (eps == 1) break;
     eps = std::max<uint64_t>(1, eps / div);
   }
   e->stats.n_rounds = e->h_ctl.p->rounds;
-  e->stats.evals = e->h_ctl.p->evals + closure_evals;
+  e->stats.evals = e->h_ctl.p->evals + closure_evals + (uint64_t)C * e->h_ctl.p->rev_bids;
   e->stats.n_tiles = (uint32_t)std::min<unsigned long long>(e->h_ctl.p->n_class_scans, 0xFFFFFFFFull);
   e->stats.n_fused_launches = (uint32_t)std::min<unsigned long long>(e->h_ctl.p->n_ask_scans, 0xFFFFFFFFull);
   e->stats.n_launches = e->h_ctl.p->rounds * (packed_claim ? 6u : 7u);
@@ -2125,6 +2210,9 @@ static int auction_pass(pm_engine* e, bool want_warm) {
   else e->auc_floor_stored.assign(T, 0u);
   e->auc_last_warm = warm;
   e->auc_last_released = n_released;
+  e->auc_last_phases = reverse ? n_phases : 0u;
+  e->auc_last_rev_rounds = reverse ? e->h_ctl.p->rev_rounds : 0u;
+  e->auc_last_rev_bids = reverse ? e->h_ctl.p->rev_bids : 0u;
   e->matched = true;
   e->local_done = false;
   return PM_OK;
@@ -2142,6 +2230,17 @@ int pm_auction_state(pm_engine* e, int64_t* price, uint32_t* warm, uint32_t* n_r
   }
   if (warm) *warm = e->auc_last_warm ? 1u : 0u;
   if (n_released) *n_released = e->auc_last_released;
+  return PM_OK;
+} catch (...) { return pm_guard_rc(); }
+
+// The last auction pass's eps phases, reverse rounds and reverse bids (all 0 for a pass without PM_AUCTION_REVERSE).
+int pm_auction_reverse_stats(pm_engine* e, uint32_t* n_phases, uint32_t* n_reverse_rounds, uint64_t* n_reverse_bids) try {
+  if (!e) return PM_E_INVALID;
+  std::lock_guard<std::mutex> lk(e->mu);
+  if (!e->auc_state) return e->fail(PM_E_STATE, "pm_auction_reverse_stats: no auction pass since the engine's tables were last replaced");
+  if (n_phases) *n_phases = e->auc_last_phases;
+  if (n_reverse_rounds) *n_reverse_rounds = e->auc_last_rev_rounds;
+  if (n_reverse_bids) *n_reverse_bids = e->auc_last_rev_bids;
   return PM_OK;
 } catch (...) { return pm_guard_rc(); }
 
@@ -2245,6 +2344,11 @@ static int exchange_locked(pm_engine* e) {
 static int check_incremental(pm_engine* e, uint32_t mode, bool local) {
   if ((mode & PM_AUCTION_WARM) && (mode & 0xFFu) != PM_MODE_AUCTION)
     return e->fail(PM_E_INVALID, "pm_match: PM_AUCTION_WARM is for the auction only");
+  if ((mode & PM_AUCTION_REVERSE) && (mode & 0xFFu) != PM_MODE_AUCTION)
+    return e->fail(PM_E_INVALID, "pm_match: PM_AUCTION_REVERSE is for the auction only");
+  // a warm pass is one eps = 1 phase whose release already leaves every unowned worker at price 0
+  if ((mode & PM_AUCTION_REVERSE) && (mode & PM_AUCTION_WARM))
+    return e->fail(PM_E_INVALID, "pm_match: PM_AUCTION_REVERSE does not go with PM_AUCTION_WARM");
   if (!(mode & PM_INCREMENTAL)) return PM_OK;
   if ((mode & 0xFFu) == PM_MODE_AUCTION) return e->fail(PM_E_INVALID, "pm_match: PM_INCREMENTAL is for the reference modes, not the auction");
   if ((mode & (PM_PATH_FUSED | PM_NO_ASK_STATS)) != (PM_PATH_FUSED | PM_NO_ASK_STATS))
@@ -2272,6 +2376,7 @@ int pm_match_finish(pm_engine* e, uint32_t mode) try {
   if (!e) return PM_E_INVALID;
   std::lock_guard<std::mutex> lk(e->mu);
   if (mode & PM_AUCTION_WARM) return e->fail(PM_E_INVALID, "pm_match_finish: PM_AUCTION_WARM is for the auction only");
+  if (mode & PM_AUCTION_REVERSE) return e->fail(PM_E_INVALID, "pm_match_finish: PM_AUCTION_REVERSE is for the auction only");
   return invalidate_on_failure(e, match_finish_locked(e, mode));
 } catch (...) { return pm_guard_rc(); }
 int pm_match(pm_engine* e, uint32_t mode) try {

@@ -233,6 +233,13 @@ class Engine:
         self._check(self._lib.pm_auction_state(self._h, _ptr(price) if prices else None, C.byref(warm), C.byref(released)))
         return price, bool(warm.value), int(released.value)
 
+    def auction_reverse_stats(self):
+        """The last auction pass (pm_auction_reverse_stats): (eps phases, reverse rounds, reverse bids); all 0 for a pass
+        without PM_AUCTION_REVERSE."""
+        phases, rounds, bids = C.c_uint32(), C.c_uint32(), C.c_uint64()
+        self._check(self._lib.pm_auction_reverse_stats(self._h, C.byref(phases), C.byref(rounds), C.byref(bids)))
+        return int(phases.value), int(rounds.value), int(bids.value)
+
     # ---- the pass ---------------------------------------------------------
     def match(self, mode: int = abi.PM_MODE_FIRST_FIT):
         self._check(self._lib.pm_match(self._h, mode))
