@@ -240,7 +240,16 @@ int      pm_create_sibling(const pm_engine*, pm_engine** out);
 
 /* NORTH-STAR EXTENSION columns (no reference counterpart; only PM_MODE_AUCTION reads them):
  * per-ask price cap against pm_worker_b.ext_ask_price, and the auction's parameters
- * (value = -(ask_price * cost_scale) - price; eps runs eps_start, /eps_div, ..., 1).       */
+ * (value = -(ask_price * cost_scale) - price; eps runs eps_start, /eps_div, ..., 1).
+ * Integer domain of PM_MODE_AUCTION: with P = the largest ext_ask_price over every row of the worker table (feasible or
+ * not), K = the largest price cap, S = cost_scale and E = eps_start (0 counts as 1 for both),
+ *     (P + K + 2) * S + E < 2^61          (evaluated without overflow).
+ * Inside it every value, outside option, bid, price, profit and sort key the auction computes in int64 lies strictly
+ * between -2^61 and 2^61 (DESIGN 4).  pm_set_auction_params refuses cost_scale or eps_start >= 2^61 (PM_E_INVALID,
+ * nothing changes: the stored auction state is kept).  pm_match(PM_MODE_AUCTION ...) refuses a pass whose tables and
+ * parameters are outside the domain with PM_E_INVALID before it changes anything: the stored warm state,
+ * pm_auction_state and pm_auction_reverse_stats stay as they were.  Round counts grow with S (an eps = 1 price war
+ * between equal workers takes O(S) rounds): large scales want eps-scaling with PM_AUCTION_REVERSE.                   */
 int pm_set_ask_price_caps(pm_engine*, const uint32_t* price_cap, uint32_t n_asks);
 int pm_set_auction_params(pm_engine*, uint64_t cost_scale, uint64_t eps_start, uint32_t eps_div);
 /* `reputation` (north_star worker column; SURVEY 8 A21 side column ext_reputation:u32) and the per-ask floor on it:

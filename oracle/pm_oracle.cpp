@@ -1137,7 +1137,15 @@ uint32_t orc_soa_auction_rep(const pm_worker_a* a, const pm_worker_b* b, uint32_
                              const uint32_t* reputation, const uint32_t* min_reputation,
                              uint64_t cost_scale, uint64_t eps_start, uint32_t eps_div,
                              uint32_t* ask_worker_out, int64_t* worker_price_out) {
-  const int64_t S = cost_scale ? int64_t(cost_scale) : 1;
+  if (cost_scale == 0) cost_scale = 1;
+  if (eps_start == 0) eps_start = 1;
+  {  // the engine's integer domain: (max ask_price + max cap + 2) * S + eps_start < 2^61, in 128 bits
+    uint32_t P = 0, K = 0;
+    for (u32 w = 0; w < n_workers; ++w) P = std::max(P, b[w].ext_ask_price);
+    for (u32 t = 0; t < n_asks; ++t) K = std::max(K, price_cap[t]);
+    if (((unsigned __int128)P + K + 2u) * cost_scale + eps_start >= ((unsigned __int128)1 << 61)) return ORC_AUCTION_REFUSED;
+  }
+  const int64_t S = int64_t(cost_scale);
   const int64_t NEG = INT64_MIN / 4;
   std::vector<int64_t> price(n_workers, 0);
   std::vector<u32> owner(n_workers, PM_NONE), assigned(n_asks, PM_NONE);
@@ -1151,7 +1159,6 @@ uint32_t orc_soa_auction_rep(const pm_worker_a* a, const pm_worker_b* b, uint32_
           orc_soa_compatible(&a[w], &b[w], &asks[t], opts, model_bits, words))
         feas[t].push_back(w);
   u32 rounds = 0;
-  if (eps_start == 0) eps_start = 1;
   if (eps_div < 2) eps_div = 2;
   for (uint64_t eps = eps_start;; eps = std::max<uint64_t>(1, eps / eps_div)) {
     std::fill(owner.begin(), owner.end(), PM_NONE);

@@ -187,7 +187,11 @@ void orc_soa_first_feasible(const pm_worker_a* a, const pm_worker_b* b, uint32_t
  *   (ties: lowest worker index); a worker takes the highest bid (ties: lowest task index) and
  *   releases its previous owner; a task whose best value drops below its outside option withdraws.
  * eps runs eps_start, eps_start/eps_div, ..., 1 (assignment cleared between phases, prices kept).
- * ask_worker_out[T]: assigned worker or PM_NONE.  Returns the number of bidding rounds.     */
+ * ask_worker_out[T]: assigned worker or PM_NONE.  Returns the number of bidding rounds, or
+ * ORC_AUCTION_REFUSED (nothing written) outside the engine's integer domain (prime_match.h,
+ * pm_set_auction_params): (max ext_ask_price + max price_cap + 2) * cost_scale + eps_start >= 2^61. */
+#define ORC_AUCTION_REFUSED 0xFFFFFFFFu
+
 uint32_t orc_soa_auction(const pm_worker_a* a, const pm_worker_b* b, uint32_t n_workers,
                          const pm_ask* asks, uint32_t n_asks, const pm_gpu_opt* opts,
                          const uint32_t* model_bits, uint32_t words, const uint32_t* price_cap,

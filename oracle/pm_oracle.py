@@ -20,6 +20,7 @@ ORC_HAS_CPU, ORC_HAS_CPU_CORES, ORC_HAS_RAM, ORC_HAS_STORAGE = 32, 64, 128, 256
 ORC_HAS_P2P, ORC_HAS_LOC, ORC_ASSIGNED = 512, 1024, 2048
 DISCOVERED, WAITING, HEALTHY, UNHEALTHY, DEAD, EJECTED, BANNED, LOWBALANCE = range(8)
 PM_NONE = 0xFFFFFFFF
+AUCTION_REFUSED = 0xFFFFFFFF   # orc_soa_auction(_rep) outside the engine's integer domain
 
 
 class OrcNode(C.Structure):
@@ -367,7 +368,8 @@ def soa_first_feasible(a, b, asks, opts, bits, words, threads=8):
 def soa_auction(a, b, asks, opts, bits, words, price_cap, cost_scale=1, eps_start=1, eps_div=4, reputation=None,
                 min_reputation=None):
     """EXTENSION self-oracle (no reference counterpart): returns (ask_worker u32[T], worker_price i64[W], rounds).
-    reputation u32[W] / min_reputation u32[T] (north-star column, optional): feasible only if reputation >= floor."""
+    reputation u32[W] / min_reputation u32[T] (north-star column, optional): feasible only if reputation >= floor.
+    ValueError outside the engine's integer domain, (max ask_price + max cap + 2) * cost_scale + eps_start >= 2^61."""
     a = np.ascontiguousarray(a); b = np.ascontiguousarray(b)
     asks = np.ascontiguousarray(asks); opts = np.ascontiguousarray(opts)
     bits = np.ascontiguousarray(bits, dtype=np.uint32)
@@ -382,6 +384,8 @@ def soa_auction(a, b, asks, opts, bits, words, price_cap, cost_scale=1, eps_star
                                         bits.ctypes.data, words, cap.ctypes.data, None if rep is None else rep.ctypes.data,
                                         None if floor is None else floor.ctypes.data, cost_scale, eps_start, eps_div,
                                         out.ctypes.data, price.ctypes.data)
+    if rounds == AUCTION_REFUSED:
+        raise ValueError("soa_auction: (max ask_price + max cap + 2) * cost_scale + eps_start must stay below 2^61")
     return out, price, rounds
 
 

@@ -1812,7 +1812,14 @@ static int auction_build_classes(pm_engine* e) {
   return PM_OK;
 }
 
-static int auction_pass(pm_engine* e, bool want_warm, bool reverse);
+// The auction's integer domain (prime_match.h, DESIGN 4): with P the largest ask price of the worker table, K the largest
+// cap, S = cost_scale and E = eps_start, (P + K + 2) * S + E < 2^61 keeps every value, outside option, bid, profit and
+// sort key strictly between -2^61 (kAucNeg, "no worker") and 2^61.  Evaluated in 128 bits: no product can wrap.
+static bool auction_in_domain(uint32_t P, uint32_t K, uint64_t S, uint64_t E) {
+  return ((unsigned __int128)P + K + 2u) * S + E < ((unsigned __int128)1 << 61);
+}
+
+static int auction_pass(pm_engine* e, bool want_warm, bool reverse, bool* refused);
 static int match_auction_locked(pm_engine* e, uint32_t mode) {
   if (!e->have_workers || !e->have_asks) return e->fail(PM_E_STATE, "pm_match: worker and ask tables must be set first");
   if (!e->have_caps) return e->fail(PM_E_STATE, "pm_match: auction mode needs pm_set_ask_price_caps");
@@ -1821,12 +1828,14 @@ static int match_auction_locked(pm_engine* e, uint32_t mode) {
   if (e->cfg.shard_count || e->comm) return e->fail(PM_E_UNSUPPORTED, "pm_match: auction mode is single-GPU");
   // the class cache is keyed on requirement rows, which a disabled ask's no longer are
   if (e->n_off) return e->fail(PM_E_UNSUPPORTED, "pm_match: auction mode with disabled asks");
-  const int rc = auction_pass(e, (mode & PM_AUCTION_WARM) != 0, (mode & PM_AUCTION_REVERSE) != 0);
-  if (rc != PM_OK) e->auc_discard();   // the stored state may be half released or half bid: it is not trusted again
+  bool refused = false;
+  const int rc = auction_pass(e, (mode & PM_AUCTION_WARM) != 0, (mode & PM_AUCTION_REVERSE) != 0, &refused);
+  // the stored state may be half released or half bid: it is not trusted again (a refused pass touched none of it)
+  if (rc != PM_OK && !refused) e->auc_discard();
   return rc;
 }
 
-static int auction_pass(pm_engine* e, bool want_warm, bool reverse) {
+static int auction_pass(pm_engine* e, bool want_warm, bool reverse, bool* refused) {
   PM_CUDA(cudaSetDevice(e->device));
   const uint32_t W = e->n_workers, T = e->n_asks;
   if (!e->have_bits) {
@@ -1881,6 +1890,25 @@ static int auction_pass(pm_engine* e, bool want_warm, bool reverse) {
   PM_CUDA(e->worker_group.ensure(W)); PM_CUDA(e->worker_ask.ensure(W)); PM_CUDA(e->members.ensure(std::max(W, T)));
   PM_CUDA(e->group_ask.ensure((size_t)T + 1)); PM_CUDA(e->group_off.ensure((size_t)T + 2));
   PM_CUDA(e->ask_best.ensure(T)); PM_CUDA(e->ask_count.ensure(T)); PM_CUDA(e->first_ask.ensure(W));
+  PM_CUDA(cudaMemsetAsync(e->auc_ctl.p, 0, sizeof(pm::AuctionCtl), e->stream));
+  // The table limits, read back before anything of the stored state is touched: a pass outside the integer domain is
+  // refused and leaves the stored state as it was.  The same read-back tells whether (value, worker) sorts as one packed
+  // 64-bit key (decided on the device, read by the kernels).
+  pm::pm_auction_limits<<<std::max(1u, std::min(blocks_for(std::max(W, T), 256), 4u * e->sms)), 256, 0, e->stream>>>(e->wb.p, W, e->price_cap.p, T, e->auc_ctl.p);
+  PM_LAUNCH_CHECK("pm_auction_limits");
+  // (a warm pass: every price an ask kept was bid under its unchanged cap at eps = 1, every other price is 0, so the
+  // bound on reachable costs is the cold one at eps = 1)
+  pm::pm_auction_decide_packed<<<1, 1, 0, e->stream>>>(e->auc_ctl.p, W, T, e->auc_scale, warm ? 1 : e->auc_eps_start,
+                                                       (uint32_t)e->tune_auction);
+  PM_LAUNCH_CHECK("pm_auction_decide_packed");
+  PM_CUDA(cudaMemcpyAsync(e->h_ctl.p, e->auc_ctl.p, sizeof(pm::AuctionCtl), cudaMemcpyDeviceToHost, e->stream));
+  PM_CUDA(cudaStreamSynchronize(e->stream));
+  if (!auction_in_domain(e->h_ctl.p->max_ask_price, e->h_ctl.p->max_cap, e->auc_scale, e->auc_eps_start)) {
+    *refused = true;
+    return e->fail(PM_E_INVALID, "pm_match: (max ask_price + max cap + 2) * cost_scale + eps_start must stay below 2^61");
+  }
+  const bool packed_claim = e->h_ctl.p->packed_claim != 0;   // then no round launches pm_auction_claim at all
+  const bool cost_packed = e->h_ctl.p->packed != 0;
   if (warm) {   // rows from n_kept on were cut off or added since the stored state: unowned, price 0
     if (W > n_kept) PM_CUDA(cudaMemsetAsync(e->auc_owner.p + n_kept, 0xFF, (size_t)(W - n_kept) * 4, e->stream));
     PM_CUDA(cudaMemsetAsync(e->auc_price.p + n_kept, 0, ((size_t)W + 2 - n_kept) * 8, e->stream));
@@ -1888,7 +1916,6 @@ static int auction_pass(pm_engine* e, bool want_warm, bool reverse) {
     PM_CUDA(cudaMemsetAsync(e->auc_price.p, 0, ((size_t)W + 2) * 8, e->stream));
   }
   PM_CUDA(cudaMemsetAsync(e->auc_price_s.p, 0, ((size_t)W + 2) * 8, e->stream));
-  PM_CUDA(cudaMemsetAsync(e->auc_ctl.p, 0, sizeof(pm::AuctionCtl), e->stream));
   PM_CUDA(cudaMemsetAsync(e->auc_class_req.p, 0, (size_t)std::max<uint32_t>(C, 1) * 4, e->stream));
   PM_CUDA(e->auc_ckey.ensure(W)); PM_CUDA(e->auc_ckey_s.ensure(W));
   // `reputation` clause: only when a floor was given; a missing worker column is a column of zeros
@@ -1985,16 +2012,6 @@ static int auction_pass(pm_engine* e, bool want_warm, bool reverse) {
     if (rc != PM_OK) return rc;
   }
   PM_CUDA(cudaMemsetAsync(e->auc_winner.p, 0xFF, (size_t)std::max<uint32_t>(W, 1) * 4, e->stream));
-  // one packed 64-bit sort key per candidate when every reachable cost fits (decided on the device, read by the kernels)
-  pm::pm_auction_limits<<<std::max(1u, std::min(blocks_for(std::max(W, T), 256), 4u * e->sms)), 256, 0, e->stream>>>(e->wb.p, W, e->price_cap.p, T, e->auc_ctl.p);
-  // (a warm pass: every price an ask kept was bid under its unchanged cap at eps = 1, every other price is 0, so the
-  // bound on reachable costs is the cold one at eps = 1)
-  pm::pm_auction_decide_packed<<<1, 1, 0, e->stream>>>(e->auc_ctl.p, W, T, e->auc_scale, warm ? 1 : (e->auc_eps_start ? e->auc_eps_start : 1),
-                                                       (uint32_t)e->tune_auction);
-  PM_LAUNCH_CHECK("pm_auction_decide_packed");
-  PM_CUDA(cudaMemcpyAsync(e->h_ctl.p, e->auc_ctl.p, sizeof(pm::AuctionCtl), cudaMemcpyDeviceToHost, e->stream));
-  PM_CUDA(cudaStreamSynchronize(e->stream));
-  const bool packed_claim = e->h_ctl.p->packed_claim != 0;   // then no round launches pm_auction_claim at all
 
   const size_t smem = pm::kAucStages * sizeof(pm::AuctionStage) + sizeof(pm::AuctionMerge);
   PM_CUDA(cudaFuncSetAttribute(pm::pm_auction_scan, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -2024,7 +2041,7 @@ static int auction_pass(pm_engine* e, bool want_warm, bool reverse) {
                                                                           e->auc_rev_cstart.p, e->auc_rev_cap_s.p);
     PM_LAUNCH_CHECK("pm_auction_rev_classes");
   }
-  const bool rev_packed = e->h_ctl.p->packed != 0 && !(e->tune_auction & 128);   // then no round launches pm_auction_rev_claim
+  const bool rev_packed = cost_packed && !(e->tune_auction & 128);   // then no round launches pm_auction_rev_claim
   const unsigned g_rev = std::max(1u, std::min(blocks_for(std::max(W, T), 256), 8u * e->sms));
   const unsigned g_rev_bid = 4u * e->sms;   // 64 registers per thread (no spills): four resident CTAs per SM
   const uint32_t kRevBatch = 16;   // reverse rounds launched between polls of the control block
@@ -2297,6 +2314,8 @@ int pm_set_ask_min_reputation(pm_engine* e, const uint32_t* min_reputation, uint
 int pm_set_auction_params(pm_engine* e, uint64_t cost_scale, uint64_t eps_start, uint32_t eps_div) try {
   if (!e) return PM_E_INVALID;
   std::lock_guard<std::mutex> lk(e->mu);
+  if (cost_scale >= (1ull << 61) || eps_start >= (1ull << 61))   // outside the domain whatever the tables; changes nothing
+    return e->fail(PM_E_INVALID, "pm_set_auction_params: cost_scale and eps_start must stay below 2^61");
   e->auc_discard();
   e->auc_scale = cost_scale ? cost_scale : 1;
   e->auc_eps_start = eps_start ? eps_start : 1;
