@@ -285,9 +285,13 @@ enum pm_path {
   PM_AUCTION_WARM      = 1u << 11,/* PM_MODE_AUCTION only (else PM_E_INVALID): start from the last auction pass's prices and
                                     assignment, releasing only the asks the changes since disturb; a cold pass when there is
                                     no stored state or the changes exceed the cutoff.  See "Auction warm start" below */
-  PM_AUCTION_REVERSE   = 1u << 12 /* PM_MODE_AUCTION only, not with PM_AUCTION_WARM (else PM_E_INVALID): every eps phase
+  PM_AUCTION_REVERSE   = 1u << 12,/* PM_MODE_AUCTION only, not with PM_AUCTION_WARM (else PM_E_INVALID): every eps phase
                                     ends with reverse rounds that return every unowned worker to price 0, which makes
                                     eps_start > 1 keep the eps = 1 bound.  See "Auction reverse rounds" below */
+  PM_AUCTION_REPAIR    = 1u << 13 /* only as PM_MODE_AUCTION | PM_AUCTION_WARM | PM_AUCTION_REPAIR (else PM_E_INVALID; not
+                                    with PM_AUCTION_REVERSE): a warm pass that keeps every stored price, raises the changed
+                                    rows instead of releasing what they disturb, and ends with reverse rounds.  See
+                                    "Auction warm repair" below */
 };
 
 /* Incremental passes (PM_INCREMENTAL).  Every full evaluation, with the flag or without, keeps a copy of its
@@ -358,6 +362,27 @@ int pm_auction_state(pm_engine*, int64_t* price, uint32_t* warm, uint32_t* n_rel
  * pm_auction_reverse_stats reports on the last auction pass: its eps phases, reverse rounds and bids (each NULL-able),
  * all 0 for a pass without the bit; PM_E_STATE where pm_auction_state returns it. */
 int pm_auction_reverse_stats(pm_engine*, uint32_t* n_phases, uint32_t* n_reverse_rounds, uint64_t* n_reverse_bids);
+
+/* Auction warm repair (PM_MODE_AUCTION | PM_AUCTION_WARM | PM_AUCTION_REPAIR).  The same stored state, changed rows R0,
+ * changed asks A0 and PM_TUNE_INCR cutoff as a warm pass; without a stored state or above the cutoff it is the cold pass
+ * PM_AUCTION_WARM falls back to (warm = 0).  Otherwise, with eps = 1 and a(w), pi(t) as for the reverse rounds:
+ *   1. release: every ask of A0, every owner of a row of R0 and every holder of a row a shrink cut off gives up its
+ *      worker, which becomes unowned AT ITS STORED PRICE; every other price stays as stored (an eps-scaled pass's
+ *      positive prices on unowned workers too);
+ *   2. raise: every row of R0 and every row added since (rows >= the stored pass's row count after any shrink) gets
+ *      price[w] = max(0, beta(w) - eps), beta(w) = the largest a(w) - pi(t) over the asks t that still hold a worker
+ *      after step 1 and are feasible for w (candidate, compatible, ask_price <= cap, reputation >= floor), or 0 when
+ *      there is none.  Every beta is read from the state after step 1; a raised row holds no ask, so the order of the
+ *      rows does not matter.  Asks that hold no worker do not count: they bid in step 3;
+ *   3. the forward rounds at eps = 1 from that state, every unassigned ask active (withdrawn ones too);
+ *   4. one reverse stage at eps = 1 (the rounds of PM_AUCTION_REVERSE), until no unowned worker has a positive price.
+ * eps-complementary slackness holds after every step, so the result is within T of the optimum of the current instance
+ * (the optimum with cost_scale = T + 1), as a cold pass's is (DESIGN 4); it need not equal the cold or the warm pass's
+ * result.  Nothing is released beyond step 1.  pm_auction_state: warm = 1, n_released = the asks of step 1.
+ * pm_auction_reverse_stats: 1 phase, the reverse rounds and bids of step 4.  pm_stats: n_rounds = the forward rounds;
+ * evals = classes x raised rows + the rounds' evaluations + classes x reverse bids; with PM_CFG_TIMING, ms_build = the
+ * reverse rounds.  The pass stores its state like any auction pass.  Refusals are those of PM_AUCTION_WARM (disabled
+ * asks, shard engines: PM_E_UNSUPPORTED; outside the integer domain: PM_E_INVALID), and none changes the stored state. */
 
 typedef struct pm_stats {
   uint64_t evals;            /* predicate evaluations executed on the device        */

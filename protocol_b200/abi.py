@@ -51,6 +51,7 @@ PM_PATH_MATERIALIZED, PM_PATH_FUSED, PM_NO_ASK_STATS = 0, 1 << 8, 1 << 9
 PM_INCREMENTAL = 1 << 10   # re-evaluate only the worker rows written since the stored evaluation (prime_match.h)
 PM_AUCTION_WARM = 1 << 11  # PM_MODE_AUCTION: start from the last auction pass's prices and assignment (prime_match.h)
 PM_AUCTION_REVERSE = 1 << 12  # PM_MODE_AUCTION: end every eps phase with reverse rounds (prime_match.h)
+PM_AUCTION_REPAIR = 1 << 13  # with PM_AUCTION_WARM: keep the stored prices, raise the changed rows, end with reverse rounds
 
 PM_BUF_WORKER_FIRST_ASK, PM_BUF_ASK_BEST, PM_BUF_ASK_COUNT = 0, 1, 2
 

@@ -66,7 +66,8 @@
 // the bid and atomicMin on the bidder (pm_auction_claim) — applied by the single winner of each worker.
 //
 // PM_AUCTION_REVERSE ends every eps phase with reverse rounds (the section at the end): they only lower prices, so the
-// engine rebuilds the class caches and the worker order after a stage that lowered one.
+// engine rebuilds the class caches and the worker order after a stage that lowered one.  PM_AUCTION_REPAIR's raise
+// (pm_auction_repair_raise) reuses the reverse bid's gain walk before the forward rounds and ends with a reverse stage.
 #pragma once
 #include "pm_kernels.cuh"
 
@@ -1070,63 +1071,80 @@ __device__ __forceinline__ void auc_rev_merge(long long& g1, uint32_t& t1, long 
   else g2 = max(g2, o1);
 }
 
-// One CTA per bidder: C predicate evaluations against the class representatives give a class mask in shared memory
-// (kRevChunk classes at a time), then a walk over the asks of those classes in sorted order — class bit, cap, gain —
-// keeps the best two; thread 0 drops the price to 0 or posts the offer.
-__global__ void __launch_bounds__(kAucThreads, 4) pm_auction_rev_bid(AuctionParams p, AuctionRev r) {
-  __shared__ uint32_t mask[kRevChunk / 32];
-  __shared__ long long red_g1[kAucWarps], red_g2[kAucWarps];
-  __shared__ uint32_t red_t1[kAucWarps];
+struct AuctionRevSmem {   // shared memory of one bidder's gain walk
+  uint32_t mask[kRevChunk / 32];
+  long long red_g1[kAucWarps], red_g2[kAucWarps];
+  uint32_t red_t1[kAucWarps];
+};
+
+// The gains of worker w (all threads of the CTA): C predicate evaluations against the class representatives give a class
+// mask in shared memory (kRevChunk classes at a time), then a walk over the asks of those classes in sorted order —
+// class bit, cap, gain — keeps the best two.  HELD_ONLY (the warm repair's raise) also skips every ask that holds no
+// worker.  (g1, t1, g2) = (beta, t*, omega) is valid on thread 0 (t1 = kNone: no ask counted); the caller puts a barrier
+// between two calls (red_* are rewritten).
+template <bool HELD_ONLY>
+__device__ __forceinline__ void auc_rev_gains(const AuctionParams& p, const AuctionRev& r, AuctionRevSmem& sm, uint32_t w,
+                                              const WorkerReg& wr, long long a, long long& g1, uint32_t& t1, long long& g2) {
   const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
-  const uint32_t n = p.ctl->n_bid, C = r.n_classes;
+  const uint32_t C = r.n_classes;
+  g1 = kAucNeg; g2 = kAucNeg; t1 = kNone;
+  for (uint32_t c0 = 0; c0 < C; c0 += kRevChunk) {
+    const uint32_t nc = min(C - c0, kRevChunk);
+    const uint32_t kmax = (nc + kAucThreads - 1u) / kAucThreads * kAucThreads;   // the same trip count on every thread
+    for (uint32_t k = threadIdx.x; k < kmax; k += kAucThreads) {
+      const bool ok = k < nc && auc_class_accepts(p, c0 + k, wr, w, r.rep);
+      const uint32_t m = __ballot_sync(0xffffffffu, ok);   // warp-aligned k: one mask word per warp
+      if (lane == 0) sm.mask[k >> 5] = m;
+    }
+    __syncthreads();
+    // four positions per thread and step, their class loads issued together (the walk is latency-bound)
+    const uint32_t i1 = r.cstart[c0 + nc];
+    for (uint32_t i = r.cstart[c0] + threadIdx.x; i < i1; i += 4u * kAucThreads) {
+      uint32_t cs[4];
+#pragma unroll
+      for (int u = 0; u < 4; ++u) {
+        const uint32_t j = i + (uint32_t)u * kAucThreads;
+        cs[u] = j < i1 ? r.cls_s[j] - 1u - c0 : kNone;
+      }
+#pragma unroll
+      for (int u = 0; u < 4; ++u) {
+        const uint32_t j = i + (uint32_t)u * kAucThreads, c = cs[u];
+        if (c != kNone && ((sm.mask[c >> 5] >> (c & 31u)) & 1u) && r.cap_s[j] >= wr.price) {
+          const uint32_t t = r.sorted[j];
+          if (HELD_ONLY && p.assigned[t] == kNone) continue;   // an ask that holds no worker bids in the rounds instead
+          const long long g = a - r.pi_s[j];
+          if (g > g1 || (g == g1 && t < t1)) { g2 = g1; g1 = g; t1 = t; }
+          else g2 = max(g2, g);
+        }
+      }
+    }
+    __syncthreads();   // the mask is rewritten by the next chunk
+  }
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) {
+    const long long o1 = __shfl_xor_sync(0xffffffffu, g1, off), o2 = __shfl_xor_sync(0xffffffffu, g2, off);
+    const uint32_t ot = __shfl_xor_sync(0xffffffffu, t1, off);
+    auc_rev_merge(g1, t1, g2, o1, ot, o2);
+  }
+  if (lane == 0) { sm.red_g1[warp] = g1; sm.red_g2[warp] = g2; sm.red_t1[warp] = t1; }
+  __syncthreads();
+  if (threadIdx.x == 0)
+    for (uint32_t k = 1; k < (uint32_t)kAucWarps; ++k) auc_rev_merge(g1, t1, g2, sm.red_g1[k], sm.red_t1[k], sm.red_g2[k]);
+}
+
+// One CTA per bidder: its gains, then thread 0 drops the price to 0 or posts the offer.
+__global__ void __launch_bounds__(kAucThreads, 4) pm_auction_rev_bid(AuctionParams p, AuctionRev r) {
+  __shared__ AuctionRevSmem sm;
+  const uint32_t n = p.ctl->n_bid;
   const bool pk = auc_rev_packed(p);
   for (uint32_t slot = blockIdx.x; slot < n; slot += gridDim.x) {
     const uint32_t w = r.bidders[slot];
     const WorkerReg wr = make_worker(p.ev.wa[w], p.ev.wb[w]);
     const long long a = -((long long)wr.price * p.scale);
-    long long g1 = kAucNeg, g2 = kAucNeg;
-    uint32_t t1 = kNone;
-    for (uint32_t c0 = 0; c0 < C; c0 += kRevChunk) {
-      const uint32_t nc = min(C - c0, kRevChunk);
-      const uint32_t kmax = (nc + kAucThreads - 1u) / kAucThreads * kAucThreads;   // the same trip count on every thread
-      for (uint32_t k = threadIdx.x; k < kmax; k += kAucThreads) {
-        const bool ok = k < nc && auc_class_accepts(p, c0 + k, wr, w, r.rep);
-        const uint32_t m = __ballot_sync(0xffffffffu, ok);   // warp-aligned k: one mask word per warp
-        if (lane == 0) mask[k >> 5] = m;
-      }
-      __syncthreads();
-      // four positions per thread and step, their class loads issued together (the walk is latency-bound)
-      const uint32_t i1 = r.cstart[c0 + nc];
-      for (uint32_t i = r.cstart[c0] + threadIdx.x; i < i1; i += 4u * kAucThreads) {
-        uint32_t cs[4];
-#pragma unroll
-        for (int u = 0; u < 4; ++u) {
-          const uint32_t j = i + (uint32_t)u * kAucThreads;
-          cs[u] = j < i1 ? r.cls_s[j] - 1u - c0 : kNone;
-        }
-#pragma unroll
-        for (int u = 0; u < 4; ++u) {
-          const uint32_t j = i + (uint32_t)u * kAucThreads, c = cs[u];
-          if (c != kNone && ((mask[c >> 5] >> (c & 31u)) & 1u) && r.cap_s[j] >= wr.price) {
-            const long long g = a - r.pi_s[j];
-            const uint32_t t = r.sorted[j];
-            if (g > g1 || (g == g1 && t < t1)) { g2 = g1; g1 = g; t1 = t; }
-            else g2 = max(g2, g);
-          }
-        }
-      }
-      __syncthreads();   // the mask is rewritten by the next chunk
-    }
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) {
-      const long long o1 = __shfl_xor_sync(0xffffffffu, g1, off), o2 = __shfl_xor_sync(0xffffffffu, g2, off);
-      const uint32_t ot = __shfl_xor_sync(0xffffffffu, t1, off);
-      auc_rev_merge(g1, t1, g2, o1, ot, o2);
-    }
-    if (lane == 0) { red_g1[warp] = g1; red_g2[warp] = g2; red_t1[warp] = t1; }
-    __syncthreads();
+    long long g1, g2;
+    uint32_t t1;
+    auc_rev_gains<false>(p, r, sm, w, wr, a, g1, t1, g2);
     if (threadIdx.x == 0) {
-      for (uint32_t k = 1; k < (uint32_t)kAucWarps; ++k) auc_rev_merge(g1, t1, g2, red_g1[k], red_t1[k], red_g2[k]);
       if (t1 == kNone || g1 <= p.eps) {   // nothing worth offering: the price goes to 0, the worker stays unowned
         p.price[w] = 0;
         p.price_s[p.pos_of[w]] = 0;
@@ -1144,6 +1162,27 @@ __global__ void __launch_bounds__(kAucThreads, 4) pm_auction_rev_bid(AuctionPara
       }
     }
     __syncthreads();   // red_* are reused by the CTA's next bidder
+  }
+}
+
+// Warm repair (PM_AUCTION_WARM | PM_AUCTION_REPAIR), step 2: one CTA per raised row w (the changed rows, all unowned
+// after the release), the bid's gains over the asks that still hold a worker, read from pi_s as pm_auction_rev_collect
+// wrote it after the release; price[w] = max(0, beta - eps), or 0 when no held ask is feasible for w.  No offer: the
+// forward rounds and the reverse stage take it from here.  A raised row holds no ask, so it changes no profit any other
+// raised row reads: the result does not depend on the order.
+__global__ void __launch_bounds__(kAucThreads, 4) pm_auction_repair_raise(AuctionParams p, AuctionRev r,
+                                                                           const uint32_t* __restrict__ raised) {
+  __shared__ AuctionRevSmem sm;
+  const uint32_t n = p.ctl->n_raised;
+  for (uint32_t slot = blockIdx.x; slot < n; slot += gridDim.x) {
+    const uint32_t w = raised[slot];
+    const WorkerReg wr = make_worker(p.ev.wa[w], p.ev.wb[w]);
+    const long long a = -((long long)wr.price * p.scale);
+    long long g1, g2;
+    uint32_t t1;
+    auc_rev_gains<true>(p, r, sm, w, wr, a, g1, t1, g2);
+    if (threadIdx.x == 0) p.price[w] = t1 == kNone ? 0ll : max(0ll, g1 - p.eps);
+    __syncthreads();   // red_* are reused by the CTA's next row
   }
 }
 

@@ -1819,7 +1819,7 @@ static bool auction_in_domain(uint32_t P, uint32_t K, uint64_t S, uint64_t E) {
   return ((unsigned __int128)P + K + 2u) * S + E < ((unsigned __int128)1 << 61);
 }
 
-static int auction_pass(pm_engine* e, bool want_warm, bool reverse, bool* refused);
+static int auction_pass(pm_engine* e, bool want_warm, bool want_repair, bool reverse, bool* refused);
 static int match_auction_locked(pm_engine* e, uint32_t mode) {
   if (!e->have_workers || !e->have_asks) return e->fail(PM_E_STATE, "pm_match: worker and ask tables must be set first");
   if (!e->have_caps) return e->fail(PM_E_STATE, "pm_match: auction mode needs pm_set_ask_price_caps");
@@ -1829,13 +1829,14 @@ static int match_auction_locked(pm_engine* e, uint32_t mode) {
   // the class cache is keyed on requirement rows, which a disabled ask's no longer are
   if (e->n_off) return e->fail(PM_E_UNSUPPORTED, "pm_match: auction mode with disabled asks");
   bool refused = false;
-  const int rc = auction_pass(e, (mode & PM_AUCTION_WARM) != 0, (mode & PM_AUCTION_REVERSE) != 0, &refused);
+  const int rc = auction_pass(e, (mode & PM_AUCTION_WARM) != 0, (mode & PM_AUCTION_REPAIR) != 0, (mode & PM_AUCTION_REVERSE) != 0,
+                              &refused);
   // the stored state may be half released or half bid: it is not trusted again (a refused pass touched none of it)
   if (rc != PM_OK && !refused) e->auc_discard();
   return rc;
 }
 
-static int auction_pass(pm_engine* e, bool want_warm, bool reverse, bool* refused) {
+static int auction_pass(pm_engine* e, bool want_warm, bool want_repair, bool reverse, bool* refused) {
   PM_CUDA(cudaSetDevice(e->device));
   const uint32_t W = e->n_workers, T = e->n_asks;
   if (!e->have_bits) {
@@ -1869,6 +1870,7 @@ static int auction_pass(pm_engine* e, bool want_warm, bool reverse, bool* refuse
     warm = (uint64_t)changed.size() + (W - n_kept) <= e->tune_incr;
   }
   const uint32_t n_rows = warm ? (uint32_t)e->auc_rows.size() : 0u, n_chg = warm ? (uint32_t)changed.size() - n_rows : 0u;
+  const bool repair = want_repair && warm;   // PM_AUCTION_REPAIR: the same warm start, repaired by raising instead of releasing
   // the stored state survives the buffers' growth (a resize since the last pass); a cold pass overwrites it below
   PM_CUDA(e->auc_price.grow_keep((size_t)W + 2, e->auc_price.n, e->stream)); PM_CUDA(e->auc_owner.grow_keep(W, e->auc_owner.n, e->stream));
   PM_CUDA(e->auc_assigned.grow_keep(T, e->auc_assigned.n, e->stream));
@@ -1897,8 +1899,9 @@ static int auction_pass(pm_engine* e, bool want_warm, bool reverse, bool* refuse
   pm::pm_auction_limits<<<std::max(1u, std::min(blocks_for(std::max(W, T), 256), 4u * e->sms)), 256, 0, e->stream>>>(e->wb.p, W, e->price_cap.p, T, e->auc_ctl.p);
   PM_LAUNCH_CHECK("pm_auction_limits");
   // (a warm pass: every price an ask kept was bid under its unchanged cap at eps = 1, every other price is 0, so the
-  // bound on reachable costs is the cold one at eps = 1)
-  pm::pm_auction_decide_packed<<<1, 1, 0, e->stream>>>(e->auc_ctl.p, W, T, e->auc_scale, warm ? 1 : e->auc_eps_start,
+  // bound on reachable costs is the cold one at eps = 1.  A warm repair keeps the stored prices of unowned workers too,
+  // which an eps-scaled pass may have left at up to (K + 1) * S + eps_start: it is decided with eps_start.)
+  pm::pm_auction_decide_packed<<<1, 1, 0, e->stream>>>(e->auc_ctl.p, W, T, e->auc_scale, warm && !repair ? 1 : e->auc_eps_start,
                                                        (uint32_t)e->tune_auction);
   PM_LAUNCH_CHECK("pm_auction_decide_packed");
   PM_CUDA(cudaMemcpyAsync(e->h_ctl.p, e->auc_ctl.p, sizeof(pm::AuctionCtl), cudaMemcpyDeviceToHost, e->stream));
@@ -1950,12 +1953,60 @@ static int auction_pass(pm_engine* e, bool want_warm, bool reverse, bool* refuse
     pm::pm_fill_i64<<<std::min(blocks_for(W, 256), 8u * e->sms), 256, 0, e->stream>>>(e->auc_bid_max.p, pm::kAucNeg, W);
     PM_LAUNCH_CHECK("pm_fill_i64");
   }
+  // Reverse rounds (PM_AUCTION_REVERSE, and the last stage of a warm repair): per round collect the bidders and the asks'
+  // profits, one CTA per bid, (claim), apply, advance; batched into one CUDA graph per phase like the forward rounds, one
+  // poll of the control block per batch.  (Set up here: a warm repair's raise runs on the same buffers before the rounds.)
+  const bool rev_on = (reverse || repair) && T && W;
+  pm::AuctionRev rv{};
+  if (rev_on) {
+    PM_CUDA(e->auc_rev_bidders.ensure(W)); PM_CUDA(e->auc_rev_offer_t.ensure(W)); PM_CUDA(e->auc_rev_offer_p.ensure(W));
+    PM_CUDA(e->auc_rev_best.ensure(T)); PM_CUDA(e->auc_rev_win.ensure(T)); PM_CUDA(e->auc_rev_pi_s.ensure(T));
+    PM_CUDA(e->auc_rev_cap_s.ensure(T)); PM_CUDA(e->auc_rev_cstart.ensure((size_t)C + 1));
+    rv.bidders = e->auc_rev_bidders.p; rv.offer_t = e->auc_rev_offer_t.p; rv.offer_p = e->auc_rev_offer_p.p;
+    rv.best = e->auc_rev_best.p; rv.win = e->auc_rev_win.p; rv.pi_s = e->auc_rev_pi_s.p; rv.cap_s = e->auc_rev_cap_s.p;
+    rv.sorted = e->auc_sorted.p; rv.cls_s = e->auc_incl.p; rv.cstart = e->auc_rev_cstart.p;
+    rv.rep = use_rep ? e->reputation.p : nullptr; rv.n_classes = C;
+    pm::pm_auction_rev_classes<<<blocks_for(T, 256), 256, 0, e->stream>>>(e->auc_sorted.p, e->auc_incl.p, e->price_cap.p, T, C,
+                                                                          e->auc_rev_cstart.p, e->auc_rev_cap_s.p);
+    PM_LAUNCH_CHECK("pm_auction_rev_classes");
+  }
+  const bool rev_packed = cost_packed && !(e->tune_auction & 128);   // then no round launches pm_auction_rev_claim
+  const unsigned g_rev = std::max(1u, std::min(blocks_for(std::max(W, T), 256), 8u * e->sms));
+  const unsigned g_rev_bid = 4u * e->sms;   // 64 registers per thread (no spills): four resident CTAs per SM
   // Release (warm start, steps 2 and 3 of DESIGN 4): the initial release and price reset, then the closure — per
   // iteration C x |R_new| predicate evaluations and one compare per still-assigned ask, one poll of the control block.
+  // A warm repair instead keeps every stored price and raises the changed rows (below).
   // Every reset happens here, before the first sort of the worker copy: within the rounds sort keys still only rise.
   uint64_t closure_evals = 0;
   uint32_t n_released = 0;
-  if (warm) {
+  if (repair) {
+    // 1. the warm start's initial release, no price reset: a released worker is unowned at its stored price;
+    // 2. R = the changed rows (R0, and every row from n_kept on), each raised to max(0, beta - 1) against the asks that
+    //    still hold a worker, with their profits as the release left them (the collect writes them into pi_s; the
+    //    bidder list it also makes is dropped: the reverse stage collects its own).  A raised price may be lower than
+    //    the stored one, but it comes before the first sort of the worker copy, so sort keys still only rise within
+    //    the forward rounds.
+    PM_CUDA(e->auc_raised.ensure(std::max<uint32_t>(W, 1))); PM_CUDA(e->auc_mark.ensure(std::max<uint32_t>(W, 1)));
+    PM_CUDA(e->auc_chg.ensure(std::max<size_t>(changed.size(), 1)));
+    if (!changed.empty()) PM_CUDA(cudaMemcpyAsync(e->auc_chg.p, changed.data(), changed.size() * 4, cudaMemcpyHostToDevice, e->stream));
+    ap.eps = 1;
+    const unsigned g_seed = std::max(1u, std::min(blocks_for((size_t)T + changed.size(), 256), 8u * e->sms));
+    pm::pm_auction_warm_seed<<<g_seed, 256, 0, e->stream>>>(ap, e->auc_chg.p, n_rows, e->auc_chg.p + n_rows, n_chg, n_kept);
+    PM_LAUNCH_CHECK("pm_auction_warm_seed");
+    if (rev_on) {
+      const unsigned g_w = std::max(1u, std::min(blocks_for(W, 256), 8u * e->sms));
+      PM_CUDA(cudaMemsetAsync(e->auc_mark.p, 0, (size_t)W * 4, e->stream));
+      pm::pm_auction_warm_rows<<<g_w, 256, 0, e->stream>>>(ap, e->auc_chg.p, n_rows, n_kept, e->auc_raised.p, e->auc_mark.p);
+      PM_LAUNCH_CHECK("pm_auction_warm_rows");
+      pm::pm_auction_rev_collect<<<g_rev, 256, 0, e->stream>>>(ap, rv);
+      PM_LAUNCH_CHECK("pm_auction_rev_collect");
+      pm::pm_auction_repair_raise<<<g_rev_bid, pm::kAucThreads, 0, e->stream>>>(ap, rv, e->auc_raised.p);
+      PM_LAUNCH_CHECK("pm_auction_repair_raise");
+      PM_CUDA(cudaMemsetAsync(&e->auc_ctl.p->n_bid, 0, sizeof(uint32_t), e->stream));
+    } else if (W) {   // no asks: nobody holds a worker, so every price ends at 0
+      PM_CUDA(cudaMemsetAsync(e->auc_price.p, 0, (size_t)W * 8, e->stream));
+    }
+  } else if (warm) {
     PM_CUDA(e->auc_raised.ensure(std::max<uint32_t>(W, 1))); PM_CUDA(e->auc_mark.ensure(std::max<uint32_t>(W, 1)));
     PM_CUDA(e->auc_cmin.ensure(std::max<uint32_t>(C, 1))); PM_CUDA(e->auc_chg.ensure(std::max<size_t>(changed.size(), 1)));
     if (!changed.empty()) PM_CUDA(cudaMemcpyAsync(e->auc_chg.p, changed.data(), changed.size() * 4, cudaMemcpyHostToDevice, e->stream));
@@ -2025,25 +2076,6 @@ static int auction_pass(pm_engine* e, bool want_warm, bool reverse, bool* refuse
   const uint32_t kResort = (e->tune_auction >> 8) ? (uint32_t)(e->tune_auction >> 8) : 4u;   // batches between re-sorts of the worker copy
   uint64_t eps = warm ? 1 : (e->auc_eps_start ? e->auc_eps_start : 1);   // a warm pass is one phase at eps = 1
   const uint32_t div = e->auc_eps_div < 2 ? 2 : e->auc_eps_div;
-  // Reverse rounds (PM_AUCTION_REVERSE): per round collect the bidders and the asks' profits, one CTA per bid, (claim),
-  // apply, advance; batched into one CUDA graph per phase like the forward rounds, one poll of the control block per batch.
-  const bool rev_on = reverse && T && W;
-  pm::AuctionRev rv{};
-  if (rev_on) {
-    PM_CUDA(e->auc_rev_bidders.ensure(W)); PM_CUDA(e->auc_rev_offer_t.ensure(W)); PM_CUDA(e->auc_rev_offer_p.ensure(W));
-    PM_CUDA(e->auc_rev_best.ensure(T)); PM_CUDA(e->auc_rev_win.ensure(T)); PM_CUDA(e->auc_rev_pi_s.ensure(T));
-    PM_CUDA(e->auc_rev_cap_s.ensure(T)); PM_CUDA(e->auc_rev_cstart.ensure((size_t)C + 1));
-    rv.bidders = e->auc_rev_bidders.p; rv.offer_t = e->auc_rev_offer_t.p; rv.offer_p = e->auc_rev_offer_p.p;
-    rv.best = e->auc_rev_best.p; rv.win = e->auc_rev_win.p; rv.pi_s = e->auc_rev_pi_s.p; rv.cap_s = e->auc_rev_cap_s.p;
-    rv.sorted = e->auc_sorted.p; rv.cls_s = e->auc_incl.p; rv.cstart = e->auc_rev_cstart.p;
-    rv.rep = use_rep ? e->reputation.p : nullptr; rv.n_classes = C;
-    pm::pm_auction_rev_classes<<<blocks_for(T, 256), 256, 0, e->stream>>>(e->auc_sorted.p, e->auc_incl.p, e->price_cap.p, T, C,
-                                                                          e->auc_rev_cstart.p, e->auc_rev_cap_s.p);
-    PM_LAUNCH_CHECK("pm_auction_rev_classes");
-  }
-  const bool rev_packed = cost_packed && !(e->tune_auction & 128);   // then no round launches pm_auction_rev_claim
-  const unsigned g_rev = std::max(1u, std::min(blocks_for(std::max(W, T), 256), 8u * e->sms));
-  const unsigned g_rev_bid = 4u * e->sms;   // 64 registers per thread (no spills): four resident CTAs per SM
   const uint32_t kRevBatch = 16;   // reverse rounds launched between polls of the control block
   uint32_t n_phases = 0;
   auto reverse_stage = [&]() -> int {
@@ -2179,6 +2211,10 @@ static int auction_pass(pm_engine* e, bool want_warm, bool reverse, bool* refuse
     eps = std::max<uint64_t>(1, eps / div);
   }
   e->stats.n_rounds = e->h_ctl.p->rounds;
+  if (repair) {   // (nothing after the seed counts releases or raised rows: the last poll has them)
+    n_released = e->h_ctl.p->n_released;
+    closure_evals = (uint64_t)C * e->h_ctl.p->n_raised;   // the raise: one bid's class evaluations per raised row
+  }
   e->stats.evals = e->h_ctl.p->evals + closure_evals + (uint64_t)C * e->h_ctl.p->rev_bids;
   e->stats.n_tiles = (uint32_t)std::min<unsigned long long>(e->h_ctl.p->n_class_scans, 0xFFFFFFFFull);
   e->stats.n_fused_launches = (uint32_t)std::min<unsigned long long>(e->h_ctl.p->n_ask_scans, 0xFFFFFFFFull);
@@ -2227,9 +2263,9 @@ static int auction_pass(pm_engine* e, bool want_warm, bool reverse, bool* refuse
   else e->auc_floor_stored.assign(T, 0u);
   e->auc_last_warm = warm;
   e->auc_last_released = n_released;
-  e->auc_last_phases = reverse ? n_phases : 0u;
-  e->auc_last_rev_rounds = reverse ? e->h_ctl.p->rev_rounds : 0u;
-  e->auc_last_rev_bids = reverse ? e->h_ctl.p->rev_bids : 0u;
+  e->auc_last_phases = reverse || repair ? n_phases : 0u;
+  e->auc_last_rev_rounds = reverse || repair ? e->h_ctl.p->rev_rounds : 0u;
+  e->auc_last_rev_bids = reverse || repair ? e->h_ctl.p->rev_bids : 0u;
   e->matched = true;
   e->local_done = false;
   return PM_OK;
@@ -2368,6 +2404,10 @@ static int check_incremental(pm_engine* e, uint32_t mode, bool local) {
   // a warm pass is one eps = 1 phase whose release already leaves every unowned worker at price 0
   if ((mode & PM_AUCTION_REVERSE) && (mode & PM_AUCTION_WARM))
     return e->fail(PM_E_INVALID, "pm_match: PM_AUCTION_REVERSE does not go with PM_AUCTION_WARM");
+  // a warm repair is a kind of warm pass (and the check above keeps PM_AUCTION_REVERSE off it: it ends with its own
+  // reverse stage)
+  if ((mode & PM_AUCTION_REPAIR) && !(mode & PM_AUCTION_WARM))
+    return e->fail(PM_E_INVALID, "pm_match: PM_AUCTION_REPAIR needs PM_AUCTION_WARM");
   if (!(mode & PM_INCREMENTAL)) return PM_OK;
   if ((mode & 0xFFu) == PM_MODE_AUCTION) return e->fail(PM_E_INVALID, "pm_match: PM_INCREMENTAL is for the reference modes, not the auction");
   if ((mode & (PM_PATH_FUSED | PM_NO_ASK_STATS)) != (PM_PATH_FUSED | PM_NO_ASK_STATS))
@@ -2396,6 +2436,7 @@ int pm_match_finish(pm_engine* e, uint32_t mode) try {
   std::lock_guard<std::mutex> lk(e->mu);
   if (mode & PM_AUCTION_WARM) return e->fail(PM_E_INVALID, "pm_match_finish: PM_AUCTION_WARM is for the auction only");
   if (mode & PM_AUCTION_REVERSE) return e->fail(PM_E_INVALID, "pm_match_finish: PM_AUCTION_REVERSE is for the auction only");
+  if (mode & PM_AUCTION_REPAIR) return e->fail(PM_E_INVALID, "pm_match_finish: PM_AUCTION_REPAIR is for the auction only");
   return invalidate_on_failure(e, match_finish_locked(e, mode));
 } catch (...) { return pm_guard_rc(); }
 int pm_match(pm_engine* e, uint32_t mode) try {

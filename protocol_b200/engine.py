@@ -242,6 +242,11 @@ class Engine:
 
     # ---- the pass ---------------------------------------------------------
     def match(self, mode: int = abi.PM_MODE_FIRST_FIT):
+        """pm_match.  Auction passes (PM_MODE_AUCTION) take PM_AUCTION_WARM: start from the last auction pass's state,
+        releasing only the asks the changes since disturb (a cold pass without a stored state or past the cutoff); with
+        PM_AUCTION_WARM | PM_AUCTION_REPAIR the warm pass keeps every stored price, raises the changed rows instead, and
+        ends with reverse rounds (auction_reverse_stats: 1 phase).  PM_AUCTION_REVERSE: reverse rounds after every eps
+        phase.  See prime_match.h."""
         self._check(self._lib.pm_match(self._h, mode))
         if mode & 0xFF == abi.PM_MODE_AUCTION:
             self._auction_workers = self.n_workers   # the length of the prices auction_state() returns

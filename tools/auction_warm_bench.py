@@ -8,7 +8,11 @@ the same tables in the same run, so cold and warm times sit side by side.  Per p
 pm_match, which ends in a device synchronise), ms_fused (CUDA events around the pass), rounds, released asks, evals.
 The card's name and power limit are read in the same run.  One JSON line per pass; a summary table on stderr.
 
-    python tools/auction_warm_bench.py [--out results/auction_warm.json]
+--repair: every change set runs a warm pass, a warm repair (PM_AUCTION_WARM | PM_AUCTION_REPAIR: stored prices kept,
+changed rows raised, reverse rounds at the end) and a cold pass, alternately, each warm or repair pass after a cold pass
+of the current tables and a fresh draw of the same kind and number of changes.  Per pass also: reverse rounds and bids.
+
+    python tools/auction_warm_bench.py [--repair] [--out results/auction_warm.json]
 """
 from __future__ import annotations
 
@@ -54,8 +58,9 @@ def timed(eng, mode):
     ms = (time.perf_counter() - t0) * 1e3
     st = eng.stats()
     _, warm, released = eng.auction_state(prices=False)
+    _, rev_rounds, rev_bids = eng.auction_reverse_stats()
     return dict(wall_ms=round(ms, 2), ms_fused=round(st["ms_fused"], 2), rounds=st["n_rounds"], warm=warm,
-                released=released, evals=st["evals"])
+                released=released, evals=st["evals"], rev_rounds=rev_rounds, rev_bids=rev_bids)
 
 
 def assigned_of(eng, T):
@@ -69,6 +74,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", default=None)
     ap.add_argument("--counts", default="0,10,1000,100000")
+    ap.add_argument("--repair", action="store_true", help="also run PM_AUCTION_REPAIR on every change set")
     args = ap.parse_args()
     gpu = card()
     print(f"card: {gpu}", file=sys.stderr)
@@ -86,37 +92,42 @@ def main():
         rows.append(r)
         print(json.dumps(r), flush=True)
 
-    warm_mode = abi.PM_MODE_AUCTION | abi.PM_AUCTION_WARM
+    modes = [("warm", abi.PM_MODE_AUCTION | abi.PM_AUCTION_WARM)]
+    if args.repair:
+        modes.append(("repair", abi.PM_MODE_AUCTION | abi.PM_AUCTION_WARM | abi.PM_AUCTION_REPAIR))
     record("cold", 0, timed(eng, abi.PM_MODE_AUCTION))
     rng = np.random.default_rng(1)
     for variant in ("unowned", "owned"):
         for n in [int(x) for x in args.counts.split(",")]:
-            eng.match(abi.PM_MODE_AUCTION)                 # the stored state: a cold pass of the current tables
-            got = assigned_of(eng, T)
-            owned = np.zeros(W, dtype=bool)
-            owned[got[got != NONE]] = True
-            pool = np.flatnonzero(owned if variant == "owned" else ~owned)
-            idx = np.sort(rng.choice(pool, size=min(n, len(pool)), replace=False)).astype(np.uint32)
-            if len(idx):
-                b = wb[idx].copy()
-                b["ext_ask_price"] = np.maximum(1, (b["ext_ask_price"] * rng.uniform(0.5, 1.5, len(idx))).astype(np.uint32))
-                wb[idx] = b
-                eng.update_workers(idx, wa[idx], b)
-            record(f"warm_rows_{variant}", int(len(idx)), timed(eng, warm_mode))
+            for name, mode in modes:
+                eng.match(abi.PM_MODE_AUCTION)             # the stored state: a cold pass of the current tables
+                got = assigned_of(eng, T)
+                owned = np.zeros(W, dtype=bool)
+                owned[got[got != NONE]] = True
+                pool = np.flatnonzero(owned if variant == "owned" else ~owned)
+                idx = np.sort(rng.choice(pool, size=min(n, len(pool)), replace=False)).astype(np.uint32)
+                if len(idx):
+                    b = wb[idx].copy()
+                    b["ext_ask_price"] = np.maximum(1, (b["ext_ask_price"] * rng.uniform(0.5, 1.5, len(idx))).astype(np.uint32))
+                    wb[idx] = b
+                    eng.update_workers(idx, wa[idx], b)
+                record(f"{name}_rows_{variant}", int(len(idx)), timed(eng, mode))
             record("cold", 0, timed(eng, abi.PM_MODE_AUCTION))
-    eng.match(abi.PM_MODE_AUCTION)
-    cap2 = cap.copy()
-    idx = rng.choice(T, 100, replace=False)
-    cap2[idx] = np.maximum(1, (cap2[idx] * rng.uniform(0.5, 1.5, 100)).astype(np.uint32))
-    eng.set_price_caps(cap2)
-    record("warm_caps", 100, timed(eng, warm_mode))
+    for name, mode in modes:
+        eng.match(abi.PM_MODE_AUCTION)
+        cap2 = cap.copy()                              # 100 caps changed against the stored pass's
+        idx = rng.choice(T, 100, replace=False)
+        cap2[idx] = np.maximum(1, (cap2[idx] * rng.uniform(0.5, 1.5, 100)).astype(np.uint32))
+        eng.set_price_caps(cap2)
+        record(f"{name}_caps", int((cap2 != cap).sum()), timed(eng, mode))
+        cap = cap2
     record("cold", 0, timed(eng, abi.PM_MODE_AUCTION))
     eng.close()
-    print(f"{'case':>20} {'n':>7} {'wall ms':>9} {'ms_fused':>9} {'rounds':>7} {'warm':>5} {'released':>9} {'evals':>14}",
-          file=sys.stderr)
+    print(f"{'case':>22} {'n':>7} {'wall ms':>9} {'ms_fused':>9} {'rounds':>7} {'rev rnds':>8} {'rev bids':>10} {'warm':>5} "
+          f"{'released':>9} {'evals':>14}", file=sys.stderr)
     for r in rows:
-        print(f"{r['case']:>20} {r['n']:>7} {r['wall_ms']:>9} {r['ms_fused']:>9} {r['rounds']:>7} {int(r['warm']):>5} "
-              f"{r['released']:>9} {r['evals']:>14}", file=sys.stderr)
+        print(f"{r['case']:>22} {r['n']:>7} {r['wall_ms']:>9} {r['ms_fused']:>9} {r['rounds']:>7} {r['rev_rounds']:>8} "
+              f"{r['rev_bids']:>10} {int(r['warm']):>5} {r['released']:>9} {r['evals']:>14}", file=sys.stderr)
     if args.out:
         os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
         with open(args.out, "w") as f:
