@@ -384,6 +384,44 @@ int pm_auction_reverse_stats(pm_engine*, uint32_t* n_phases, uint32_t* n_reverse
  * reverse rounds.  The pass stores its state like any auction pass.  Refusals are those of PM_AUCTION_WARM (disabled
  * asks, shard engines: PM_E_UNSUPPORTED; outside the integer domain: PM_E_INVALID), and none changes the stored state. */
 
+/* Auction certificate.  pm_auction_certificate checks the stored prices and assignment of the last auction pass
+ * against the tables, caps, floors and cost_scale as they stand now (so it also audits a stored state after table
+ * changes, before the next warm pass), with one sweep over every (ask, worker) pair.  With S = cost_scale,
+ * feasible(t,w) as for the reverse rounds and key(w) = ask_price[w] * S + price[w]:
+ *   row(t)  = min((cap[t] + 1) * S, the least key(w) over the workers feasible for t)     (ask_bound[t])
+ *   bound   = sum_t row(t) - sum_w price[w]: for any prices >= 0 a lower bound on the optimal total cost (weak duality)
+ *   cost    = sum over held asks of ask_price[w_t] * S + sum over unheld asks of (cap[t] + 1) * S
+ *   gap     = cost - bound >= cost - optimum
+ *   slack(t) = key(w_t) - row(t) when t holds w_t, else (cap[t] + 1) * S - row(t)
+ * Without shared holds gap = sum_t slack(t) + the sum of the prices of unowned workers; so every slack <= eps with every
+ * unowned worker at price 0 gives gap <= T * eps, and with S = T + 1 (every cost a multiple of S) gap < S proves the
+ * assignment optimal (DESIGN 4).  After a cold pass at eps_start = 1, a PM_AUCTION_REVERSE pass, a warm pass or a warm
+ * repair, on unchanged tables: no bad, shared or priced unowned hold, n_slack_over = 0 and gap <= T; an eps-scaled pass
+ * without reverse rounds can leave priced unowned workers, and the gap shows it.  Ownership is recounted from the
+ * assignment.  cost, bound, gap and the
+ * priced-unowned sum are exact 128-bit integers (hi: the signed high 64 bits, lo: the low 64 bits).  evals = T x W.
+ * ask_bound (NULL-able): row(t) per ask.  Refusals, none of which changes anything: NULL engine or out: PM_E_INVALID;
+ * no stored state (where pm_auction_state returns PM_E_STATE), a worker count other than the stored pass's, or an ask
+ * referencing a model pattern missing from the model table: PM_E_STATE; disabled asks: PM_E_UNSUPPORTED; tables and
+ * parameters outside the auction's integer domain: PM_E_INVALID.  The call changes nothing pm_fetch_result,
+ * pm_get_stats, pm_table_version, pm_auction_state or pm_auction_reverse_stats report, nor what the next warm or repair
+ * pass starts from. */
+typedef struct pm_auction_cert {
+  int64_t  cost_hi;   uint64_t cost_lo;    /* the stored assignment's total cost                           */
+  int64_t  bound_hi;  uint64_t bound_lo;   /* a lower bound on the optimum of the current tables           */
+  int64_t  gap_hi;    uint64_t gap_lo;     /* cost - bound                                                 */
+  uint32_t n_held;                         /* asks holding a worker                                        */
+  uint32_t n_bad_holds;                    /* held pairs infeasible under the current tables               */
+  uint32_t n_shared;                       /* workers held by more than one ask                            */
+  uint32_t n_priced_unowned;               /* unowned workers with price > 0                               */
+  uint32_t n_slack_over;                   /* asks whose slack exceeds 1 (the eps of every pass's last phase) */
+  uint32_t reserved;
+  int64_t  max_slack;                      /* over the asks; 0 without asks                                */
+  uint64_t priced_unowned_lo, priced_unowned_hi;   /* the sum of their prices                              */
+  uint64_t evals;                          /* (ask, worker) pairs evaluated                                */
+} pm_auction_cert;
+int pm_auction_certificate(pm_engine*, pm_auction_cert* out, int64_t* ask_bound);
+
 typedef struct pm_stats {
   uint64_t evals;            /* predicate evaluations executed on the device        */
   uint64_t cost_bytes_written;

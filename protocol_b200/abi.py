@@ -97,6 +97,17 @@ class PmStats(C.Structure):
         return {n: getattr(self, n) for n, _ in self._fields_ if n != "reserved"}
 
 
+class PmAuctionCert(C.Structure):
+    """pm_auction_cert: 128-bit quantities as (signed high, low) 64-bit halves."""
+    _fields_ = [
+        ("cost_hi", C.c_int64), ("cost_lo", C.c_uint64), ("bound_hi", C.c_int64), ("bound_lo", C.c_uint64),
+        ("gap_hi", C.c_int64), ("gap_lo", C.c_uint64), ("n_held", C.c_uint32), ("n_bad_holds", C.c_uint32),
+        ("n_shared", C.c_uint32), ("n_priced_unowned", C.c_uint32), ("n_slack_over", C.c_uint32),
+        ("reserved", C.c_uint32), ("max_slack", C.c_int64), ("priced_unowned_lo", C.c_uint64),
+        ("priced_unowned_hi", C.c_uint64), ("evals", C.c_uint64),
+    ]
+
+
 class PmResult(C.Structure):
     _fields_ = [
         ("n_workers", C.c_uint32), ("n_asks", C.c_uint32), ("n_groups", C.c_uint32), ("n_members", C.c_uint32),
@@ -116,7 +127,7 @@ EXPORTS = [
     "pm_set_asks", "pm_set_ask_enabled", "pm_set_model_table", "pm_set_worker_count", "pm_upsert_workers",
     "pm_set_worker_locations", "pm_set_worker_addr_rank", "pm_set_flags",
     "pm_set_ask_price_caps", "pm_set_auction_params", "pm_set_worker_reputation", "pm_set_ask_min_reputation",
-    "pm_auction_state", "pm_auction_reverse_stats",
+    "pm_auction_state", "pm_auction_reverse_stats", "pm_auction_certificate",
     "pm_match", "pm_fetch_result", "pm_get_stats", "pm_build_cost_tile",
     "pm_match_local", "pm_match_finish", "pm_device_buffer", "pm_stream_sync", "pm_set_shard",
     "pm_resize_workers", "pm_update_workers", "pm_table_version", "pm_create_sibling",

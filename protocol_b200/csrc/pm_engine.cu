@@ -34,6 +34,7 @@
 #include "pm_proximity_band.cuh"
 #include "pm_proximity_grid.cuh"
 #include "pm_auction.cuh"
+#include "pm_auction_cert.cuh"
 
 struct pm_engine;
 
@@ -460,6 +461,12 @@ struct pm_engine {
   // reverse rounds (PM_AUCTION_REVERSE): bidder list and offers, per-ask profits and caps in class order, class runs
   DevBuf<uint32_t> auc_rev_bidders, auc_rev_offer_t, auc_rev_win, auc_rev_cap_s, auc_rev_cstart;
   DevBuf<long long> auc_rev_offer_p, auc_rev_best, auc_rev_pi_s;
+  // pm_auction_certificate's own scratch: row minima, held-pair feasibility, ownership counts, row terms, accumulators
+  DevBuf<uint64_t> cert_min, cert_acc;
+  DevBuf<uint32_t> cert_ok, cert_own;
+  DevBuf<long long> cert_bound;
+  PinBuf<uint64_t> h_cert_acc;
+  PinBuf<long long> h_cert_bound;
   void auc_discard() {
     auc_state = false;
     auc_rows.clear();
@@ -722,6 +729,8 @@ void pm_destroy(pm_engine* e) {
   e->auc_raised.release(); e->auc_mark.release(); e->auc_cmin.release(); e->auc_chg.release();
   e->auc_rev_bidders.release(); e->auc_rev_offer_t.release(); e->auc_rev_win.release(); e->auc_rev_cap_s.release();
   e->auc_rev_cstart.release(); e->auc_rev_offer_p.release(); e->auc_rev_best.release(); e->auc_rev_pi_s.release();
+  e->cert_min.release(); e->cert_acc.release(); e->cert_ok.release(); e->cert_own.release(); e->cert_bound.release();
+  e->h_cert_acc.release(); e->h_cert_bound.release();
   e->worker_group.release(); e->worker_ask.release(); e->group_ask.release();
   e->group_off.release(); e->members.release(); e->h_scalars.release();
   e->xchg_send.release(); e->xchg_recv.release();
@@ -2294,6 +2303,110 @@ int pm_auction_reverse_stats(pm_engine* e, uint32_t* n_phases, uint32_t* n_rever
   if (n_phases) *n_phases = e->auc_last_phases;
   if (n_reverse_rounds) *n_reverse_rounds = e->auc_last_rev_rounds;
   if (n_reverse_bids) *n_reverse_bids = e->auc_last_rev_bids;
+  return PM_OK;
+} catch (...) { return pm_guard_rc(); }
+
+// The certificate of the stored auction state (pm_auction_cert.cuh): one sweep over every pair, then one pass over the
+// asks and one over the workers, on private buffers; one synchronisation.  Reads the stored state and the tables only:
+// the result buffers, pm_stats, the table version and the warm-start bookkeeping stay as they are.
+int pm_auction_certificate(pm_engine* e, pm_auction_cert* out, int64_t* ask_bound) try {
+  if (!e || !out) return e ? e->fail(PM_E_INVALID, "pm_auction_certificate: null output") : PM_E_INVALID;
+  std::lock_guard<std::mutex> lk(e->mu);
+  if (!e->auc_state) return e->fail(PM_E_STATE, "pm_auction_certificate: no auction pass since the engine's tables were last replaced");
+  const uint32_t W = e->n_workers, T = e->n_asks;
+  if (W != e->auc_state_w) return e->fail(PM_E_STATE, "pm_auction_certificate: the worker table was resized since the last auction pass");
+  if (e->max_pattern_row > e->n_patterns || (e->max_pattern_row && !e->have_bits))
+    return e->fail(PM_E_STATE, "pm_auction_certificate: an ask references a model pattern missing from the model table");
+  if (e->n_off) return e->fail(PM_E_UNSUPPORTED, "pm_auction_certificate: disabled asks");
+  // pm_get_stats keeps reporting the last pass: the launch checks below count into e->stats, which is put back on return
+  struct KeepStats {
+    pm_engine* e;
+    pm_stats saved;
+    ~KeepStats() { e->stats = saved; }
+  } keep_stats{e, e->stats};
+  PM_CUDA(cudaSetDevice(e->device));
+  if (!e->have_bits) {   // as an auction pass: no model table is one all-ones word
+    PM_CUDA(e->bits.ensure(1));
+    PM_CUDA(cudaMemsetAsync(e->bits.p, 0xFF, 4, e->stream));
+    e->words = 1;
+  }
+  PM_CUDA(e->cert_min.ensure(std::max<uint32_t>(T, 1))); PM_CUDA(e->cert_ok.ensure(std::max<uint32_t>(T, 1)));
+  PM_CUDA(e->cert_bound.ensure(std::max<uint32_t>(T, 1))); PM_CUDA(e->cert_own.ensure(std::max<uint32_t>(W, 1)));
+  PM_CUDA(e->cert_acc.ensure(pm::kCertAccWords)); PM_CUDA(e->h_cert_acc.ensure(pm::kCertAccWords));
+  if (ask_bound) PM_CUDA(e->h_cert_bound.ensure(std::max<uint32_t>(T, 1)));
+  PM_CUDA(cudaMemsetAsync(e->cert_min.p, 0xFF, (size_t)std::max<uint32_t>(T, 1) * 8, e->stream));
+  PM_CUDA(cudaMemsetAsync(e->cert_own.p, 0, (size_t)std::max<uint32_t>(W, 1) * 4, e->stream));
+  PM_CUDA(cudaMemsetAsync(e->cert_acc.p, 0, pm::kCertAccWords * 8, e->stream));
+  pm::CertParams c;
+  c.price = e->auc_price.p;
+  c.rep = e->have_min_rep && e->have_rep ? e->reputation.p : nullptr;
+  c.cap = e->price_cap.p;
+  c.floor = e->have_min_rep ? e->ask_min_rep.p : nullptr;
+  c.assigned = e->auc_assigned.p;
+  c.row_min = reinterpret_cast<unsigned long long*>(e->cert_min.p);
+  c.held_ok = e->cert_ok.p;
+  c.own = e->cert_own.p;
+  c.ask_bound = e->cert_bound.p;
+  c.acc = reinterpret_cast<unsigned long long*>(e->cert_acc.p);
+  c.scale = e->auc_scale;
+  c.n_workers = W;
+  c.n_asks = T;
+  if (T && W) {   // the fused pass's predicate variant (pm_match, PM_PATH_FUSED)
+    pm::EvalParams p = eval_params(e);
+    int bits_mode = ((uint64_t)p.n_bits_rows * p.words <= (uint64_t)pm::kBitsCap) ? (p.words == 1 ? 2 : 1) : 0;
+    bool fast = false;
+    int rc = decide_fast(e, &fast);
+    if (rc != PM_OK) return rc;
+    if (fast && bits_mode == 0 && p.n_bits_rows <= 31u && e->tune_build != 7) {
+      rc = worker_major(e, &p, &bits_mode);
+      if (rc != PM_OK) return rc;
+    }
+    const uint32_t rows_per_launch = 65535u * pm::kEvalRows;
+    for (uint32_t t0 = 0; t0 < T; t0 += rows_per_launch) {
+      const uint32_t nt = std::min(rows_per_launch, T - t0);
+      const dim3 grid(blocks_for(W, pm::kEvalCols), blocks_for(nt, pm::kEvalRows));
+#define PM_CERT_CASE(B, F) pm::pm_auction_cert_sweep<B, F><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, c, t0, nt)
+      if (fast) { if (bits_mode == 2) PM_CERT_CASE(2, true); else if (bits_mode == 1) PM_CERT_CASE(1, true); else PM_CERT_CASE(0, true); }
+      else { if (bits_mode == 2) PM_CERT_CASE(2, false); else if (bits_mode == 1) PM_CERT_CASE(1, false); else PM_CERT_CASE(0, false); }
+#undef PM_CERT_CASE
+      PM_LAUNCH_CHECK("pm_auction_cert_sweep");
+    }
+  }
+  if (T) {
+    pm::pm_auction_cert_asks<<<std::min(blocks_for(T, 256), 4u * e->sms), 256, 0, e->stream>>>(c, e->wb.p);
+    PM_LAUNCH_CHECK("pm_auction_cert_asks");
+  }
+  if (W) {
+    pm::pm_auction_cert_workers<<<std::min(blocks_for(W, 256), 4u * e->sms), 256, 0, e->stream>>>(c, e->wb.p);
+    PM_LAUNCH_CHECK("pm_auction_cert_workers");
+  }
+  PM_CUDA(cudaMemcpyAsync(e->h_cert_acc.p, e->cert_acc.p, pm::kCertAccWords * 8, cudaMemcpyDeviceToHost, e->stream));
+  if (ask_bound && T) PM_CUDA(cudaMemcpyAsync(e->h_cert_bound.p, e->cert_bound.p, (size_t)T * 8, cudaMemcpyDeviceToHost, e->stream));
+  PM_CUDA(cudaStreamSynchronize(e->stream));
+  const uint64_t* h = e->h_cert_acc.p;
+  uint32_t K = 0;
+  for (uint32_t t = 0; t < T; ++t) K = std::max(K, e->cap_host[t]);
+  if (!auction_in_domain((uint32_t)h[pm::kCertMaxAskPrice], K, e->auc_scale, e->auc_eps_start))
+    return e->fail(PM_E_INVALID, "pm_auction_certificate: (max ask_price + max cap + 2) * cost_scale + eps_start must stay below 2^61");
+  using i128 = __int128;
+  auto join = [&](int i) { return (i128)h[i] + ((i128)h[i + 1] << 32); };
+  const i128 cost = join(pm::kCertCostLo), bound = join(pm::kCertRowLo) - join(pm::kCertPriceLo), gap = cost - bound;
+  const i128 free_sum = join(pm::kCertFreeLo);
+  pm_auction_cert r{};
+  r.cost_hi = (int64_t)(cost >> 64); r.cost_lo = (uint64_t)cost;
+  r.bound_hi = (int64_t)(bound >> 64); r.bound_lo = (uint64_t)bound;
+  r.gap_hi = (int64_t)(gap >> 64); r.gap_lo = (uint64_t)gap;
+  r.n_held = (uint32_t)h[pm::kCertHeld];
+  r.n_bad_holds = (uint32_t)h[pm::kCertBadHolds];
+  r.n_shared = (uint32_t)h[pm::kCertShared];
+  r.n_priced_unowned = (uint32_t)h[pm::kCertFree];
+  r.n_slack_over = (uint32_t)h[pm::kCertSlackOver];
+  r.max_slack = T ? (int64_t)(h[pm::kCertMaxSlack] ^ 0x8000000000000000ull) : 0;
+  r.priced_unowned_lo = (uint64_t)free_sum;
+  r.priced_unowned_hi = (uint64_t)(free_sum >> 64);
+  r.evals = (uint64_t)T * W;
+  *out = r;
+  if (ask_bound && T) std::memcpy(ask_bound, e->h_cert_bound.p, (size_t)T * 8);
   return PM_OK;
 } catch (...) { return pm_guard_rc(); }
 

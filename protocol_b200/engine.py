@@ -240,6 +240,23 @@ class Engine:
         self._check(self._lib.pm_auction_reverse_stats(self._h, C.byref(phases), C.byref(rounds), C.byref(bids)))
         return int(phases.value), int(rounds.value), int(bids.value)
 
+    def auction_certificate(self, ask_bound: bool = False) -> dict:
+        """The certificate of the last auction pass's stored prices and assignment against the current tables
+        (pm_auction_certificate): cost, bound (a lower bound on the optimum) and gap = cost - bound as Python ints, the
+        hold counts, n_slack_over, max_slack, the priced-unowned sum, evals; with ask_bound, the per-ask row terms
+        (int64[n_asks])."""
+        cert = abi.PmAuctionCert()
+        rows = np.zeros(self.n_asks, dtype=np.int64) if ask_bound else None
+        self._check(self._lib.pm_auction_certificate(self._h, C.byref(cert), _ptr(rows) if ask_bound else None))
+        out = {n: int(getattr(cert, n)) for n in ("n_held", "n_bad_holds", "n_shared", "n_priced_unowned", "n_slack_over",
+                                                  "max_slack", "evals")}
+        for n in ("cost", "bound", "gap"):
+            out[n] = (int(getattr(cert, n + "_hi")) << 64) | int(getattr(cert, n + "_lo"))
+        out["priced_unowned_sum"] = (int(cert.priced_unowned_hi) << 64) | int(cert.priced_unowned_lo)
+        if ask_bound:
+            out["ask_bound"] = rows
+        return out
+
     # ---- the pass ---------------------------------------------------------
     def match(self, mode: int = abi.PM_MODE_FIRST_FIT):
         """pm_match.  Auction passes (PM_MODE_AUCTION) take PM_AUCTION_WARM: start from the last auction pass's state,
