@@ -241,6 +241,8 @@ int      pm_create_sibling(const pm_engine*, pm_engine** out);
 /* NORTH-STAR EXTENSION columns (no reference counterpart; only PM_MODE_AUCTION reads them):
  * per-ask price cap against pm_worker_b.ext_ask_price, and the auction's parameters
  * (value = -(ask_price * cost_scale) - price; eps runs eps_start, /eps_div, ..., 1).
+ * PM_MODE_AUCTION has no group sizes: an ask with max_group_size == 0, which no reference mode fills, takes a worker
+ * like any other there (and in pm_auction_certificate).
  * Integer domain of PM_MODE_AUCTION: with P = the largest ext_ask_price over every row of the worker table (feasible or
  * not), K = the largest price cap, S = cost_scale and E = eps_start (0 counts as 1 for both),
  *     (P + K + 2) * S + E < 2^61          (evaluated without overflow).
@@ -305,7 +307,13 @@ enum pm_path {
  * the next pass (PM_E_INVALID), as without the flag.
  * pm_set_worker_locations, pm_set_worker_addr_rank and pm_set_worker_reputation write nothing the predicate reads.
  * pm_set_asks, pm_set_model_table, pm_set_worker_count, pm_set_shard, pm_attach_comm and a pass that fails discard the
- * stored evaluation.  Without the flag pm_match evaluates every pair as before.
+ * stored evaluation.  "A pass that fails" is a reference-mode pass that returns an error once its mode bits are
+ * accepted (PM_E_UNSUPPORTED in proximity mode with an enabled max_group_size == 0 ask, say).  Two refusals are not:
+ * a call that pm_match or pm_match_local refuses in its mode check, before any pass runs (PM_E_INVALID for a flag
+ * combination, PM_E_UNSUPPORTED for PM_INCREMENTAL from pm_match on a shard engine without a communicator), and an
+ * auction-mode pass, refused (disabled asks, shard engines, outside the integer domain) or not, neither of which reads
+ * or writes the stored evaluation: both keep it and the rows written since.  Without the flag pm_match evaluates every
+ * pair as before.
  * pm_match on a shard engine without a communicator refuses the flag (PM_E_UNSUPPORTED): that call resolves one range
  * as if it were the table, so it has no whole-table result to keep incremental.  pm_match_local takes it on any engine.
  * pm_set_ask_enabled keeps the stored evaluation: the next incremental pass also walks the workers whose stored first

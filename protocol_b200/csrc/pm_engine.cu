@@ -298,6 +298,7 @@ struct pm_engine {
   DevBuf<pm::DevOptF> opts_fast;
   DevBuf<pm::FastRow> frows;
   bool rows_bound = false;     // FastRow.wp matches the current model table (pm_bind_rows)
+  bool rows_auction = false;   // the enabled max_group_size == 0 asks are in the auction's form (use_ask_form)
   bool rows_bound_wm = false;  // ... bound to the worker-major one-word table
   DevBuf<uint32_t> nacc, bits_wm;   // worker-major acceptance (pm_worker_nacc) and its one-word table ~(1 << row)
   bool nacc_valid = false;
@@ -613,6 +614,32 @@ pm::AskTables ask_tables(pm_engine* e) {
   return pm::AskTables{e->asks.p, e->opts.p, e->opts_fast.p, e->frows.p, e->amin.p, e->amax.p};
 }
 
+// PM_MODE_AUCTION has no group sizes: its feasibility is candidate, compatible, cap and floor (prime_match.h), so an ask
+// with max_group_size == 0, which the reference modes never fill, bids like any other there.  The converted rows carry
+// the reference modes' clause; the auction and its certificate convert the enabled max_group_size == 0 asks again
+// without it (auction = true), and the next call that reads the rows for a reference mode or toggles an ask converts
+// them back.  Nothing else changes: a table without such asks is never converted again.
+static int use_ask_form(pm_engine* e, bool auction) {
+  if (e->rows_auction == auction) return PM_OK;
+  std::vector<uint32_t> list;   // ask << 1 | enabled, as pm_ask_toggle takes it
+  for (uint32_t t = 0; t < e->n_asks; ++t)
+    if ((e->ask_kind[t] & pm_engine::kAskKindMaxZero) && e->ask_on[t]) list.push_back(t << 1 | 1u);
+  if (!list.empty()) {
+    PM_CUDA(cudaSetDevice(e->device));
+    PM_CUDA(e->toggle_dev.ensure(list.size()));
+    PM_CUDA(cudaMemcpyAsync(e->toggle_dev.p, list.data(), list.size() * 4, cudaMemcpyHostToDevice, e->stream));
+    pm::pm_ask_toggle<<<blocks_for(list.size(), 256), 256, 0, e->stream>>>(e->raw_asks.p, e->raw_opts.p, e->ask_newoff.p,
+                                                                         e->toggle_dev.p, (uint32_t)list.size(),
+                                                                         ask_tables(e), !auction);
+    PM_LAUNCH_CHECK("pm_ask_toggle");
+    PM_CUDA(cudaStreamSynchronize(e->stream));   // `list` is a local
+    e->rows_bound = false;
+    e->auc_classes_valid = false;
+  }
+  e->rows_auction = auction;
+  return PM_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -812,6 +839,7 @@ int pm_set_asks(pm_engine* e, const pm_ask* asks, uint32_t n_asks, const pm_gpu_
   e->have_caps = false;
   e->have_min_rep = false;
   e->auc_classes_valid = false;
+  e->rows_auction = false;
   e->have_asks = true;
   e->matched = e->local_done = false;
   return PM_OK;
@@ -840,11 +868,16 @@ int pm_set_ask_enabled(pm_engine* e, const uint32_t* idx, const uint8_t* enabled
   }
   if (changes.empty()) return PM_OK;
   ++e->table_version;
+  {
+    const int rc = use_ask_form(e, false);   // every row in one form: the toggled asks are converted in the reference one
+    if (rc != PM_OK) return rc;
+  }
   PM_CUDA(cudaSetDevice(e->device));
   PM_CUDA(e->toggle_dev.ensure(changes.size()));
   PM_CUDA(cudaMemcpyAsync(e->toggle_dev.p, changes.data(), changes.size() * 4, cudaMemcpyHostToDevice, e->stream));
   pm::pm_ask_toggle<<<blocks_for(changes.size(), 256), 256, 0, e->stream>>>(e->raw_asks.p, e->raw_opts.p, e->ask_newoff.p,
-                                                                            e->toggle_dev.p, (uint32_t)changes.size(), ask_tables(e));
+                                                                            e->toggle_dev.p, (uint32_t)changes.size(), ask_tables(e),
+                                                                            true);
   PM_LAUNCH_CHECK("pm_ask_toggle");
   PM_CUDA(cudaStreamSynchronize(e->stream));   // `changes` is a local
   for (uint32_t v : changes) {
@@ -1438,6 +1471,10 @@ static int match_local_locked(pm_engine* e, uint32_t mode) {
     if (e->any_max_zero)
       return e->fail(PM_E_UNSUPPORTED, "pm_match: max_group_size == 0 is not supported in proximity mode");
   }
+  {
+    const int rc = use_ask_form(e, false);
+    if (rc != PM_OK) return rc;
+  }
   PM_CUDA(cudaSetDevice(e->device));
   const uint32_t W = e->n_workers, T = e->n_asks;
   uint32_t w0 = 0, nw = 0;
@@ -1837,6 +1874,10 @@ static int match_auction_locked(pm_engine* e, uint32_t mode) {
   if (e->cfg.shard_count || e->comm) return e->fail(PM_E_UNSUPPORTED, "pm_match: auction mode is single-GPU");
   // the class cache is keyed on requirement rows, which a disabled ask's no longer are
   if (e->n_off) return e->fail(PM_E_UNSUPPORTED, "pm_match: auction mode with disabled asks");
+  {
+    const int rc = use_ask_form(e, true);
+    if (rc != PM_OK) return rc;
+  }
   bool refused = false;
   const int rc = auction_pass(e, (mode & PM_AUCTION_WARM) != 0, (mode & PM_AUCTION_REPAIR) != 0, (mode & PM_AUCTION_REVERSE) != 0,
                               &refused);
@@ -2318,6 +2359,10 @@ int pm_auction_certificate(pm_engine* e, pm_auction_cert* out, int64_t* ask_boun
   if (e->max_pattern_row > e->n_patterns || (e->max_pattern_row && !e->have_bits))
     return e->fail(PM_E_STATE, "pm_auction_certificate: an ask references a model pattern missing from the model table");
   if (e->n_off) return e->fail(PM_E_UNSUPPORTED, "pm_auction_certificate: disabled asks");
+  {
+    const int rc = use_ask_form(e, true);
+    if (rc != PM_OK) return rc;
+  }
   // pm_get_stats keeps reporting the last pass: the launch checks below count into e->stats, which is put back on return
   struct KeepStats {
     pm_engine* e;
@@ -2668,6 +2713,10 @@ int pm_build_cost_tile(pm_engine* e, uint32_t t0, uint32_t nt, int64_t* host_out
   if (e->max_pattern_row > e->n_patterns || (e->max_pattern_row && !e->have_bits))
     return e->fail(PM_E_STATE, "pm_build_cost_tile: model table missing");
   if ((uint64_t)t0 + nt > e->n_asks || nt == 0) return e->fail(PM_E_INVALID, "pm_build_cost_tile: ask range");
+  {
+    const int rc = use_ask_form(e, false);
+    if (rc != PM_OK) return rc;
+  }
   PM_CUDA(cudaSetDevice(e->device));
   const uint32_t W = e->n_workers;
   uint32_t w0 = 0, nw = 0;

@@ -962,7 +962,9 @@ struct AskTables {   // the converted forms of the ask table the kernels read
 // m / v of each of its DevOptF rows and its FastRow — so every predicate variant rejects every worker, and its amin is
 // at least 1, so it forms no empty group either: it behaves as if it were absent from the table.  Converting it again
 // with off == false restores the rows exactly.  `status` / `max_row` may be null (a toggle: the table was checked).
-__device__ __forceinline__ void convert_ask(uint32_t t, bool off, bool bad_range, const pm_ask* __restrict__ asks,
+// `sizes`: the reference modes' group-size clause (max_group_size == 0 takes nobody) is part of the rows; the auction,
+// which has no group sizes, converts its max_group_size == 0 asks without it.
+__device__ __forceinline__ void convert_ask(uint32_t t, bool off, bool sizes, bool bad_range, const pm_ask* __restrict__ asks,
                                             const pm_gpu_opt* __restrict__ opts, const uint32_t* __restrict__ new_off,
                                             const AskTables& o, uint32_t* __restrict__ status,
                                             uint32_t* __restrict__ max_row) {
@@ -985,7 +987,7 @@ __device__ __forceinline__ void convert_ask(uint32_t t, bool off, bool bad_range
     if (a.n_opts) need |= PM_W_HAS_GPU;
   }
   d.n_opts = n_rows;
-  if (a.max_group_size == 0 || off) need |= kNeverBit;   // first-fit with max_group_size == 0 takes nobody (mod.rs:555-556)
+  if ((sizes && a.max_group_size == 0) || off) need |= kNeverBit;   // first-fit with max_group_size == 0 takes nobody (mod.rs:555-556)
   d.need = need;
   d.opt_off = new_off[t];
   uint32_t st = 0, mrow = 0;
@@ -1063,18 +1065,18 @@ __global__ void pm_ask_convert(const pm_ask* __restrict__ asks, const pm_gpu_opt
   if (t >= n_asks) return;
   // option rows that come from the caller (none are read when pm_ask_counts found a range out of bounds: the call fails)
   const bool bad_range = (*reinterpret_cast<volatile uint32_t*>(status) & kAskBadRange) != 0u;
-  convert_ask(t, false, bad_range, asks, opts, new_off, o, status, max_row);
+  convert_ask(t, false, true, bad_range, asks, opts, new_off, o, status, max_row);
 }
 
 // pm_set_ask_enabled: the listed asks converted again, enabled or disabled; entry i = ask << 1 | enabled, one entry
-// per ask.
+// per ask.  Also the switch of the max_group_size == 0 asks between the reference modes' form and the auction's (sizes).
 __global__ void pm_ask_toggle(const pm_ask* __restrict__ asks, const pm_gpu_opt* __restrict__ opts,
                               const uint32_t* __restrict__ new_off, const uint32_t* __restrict__ list, uint32_t n,
-                              AskTables o) {
+                              AskTables o, bool sizes) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const uint32_t v = list[i];
-  convert_ask(v >> 1, (v & 1u) == 0u, false, asks, opts, new_off, o, nullptr, nullptr);
+  convert_ask(v >> 1, (v & 1u) == 0u, sizes, false, asks, opts, new_off, o, nullptr, nullptr);
 }
 
 // An incremental pass after configurations were disabled: the workers of the range [w0, w0 + nw) whose stored first

@@ -1,0 +1,237 @@
+"""One engine through long random histories of every table call, every pass kind and the auction certificate
+(tests/engine_history.py), compared after every call with plain references computed from the host mirror: the CPU
+oracle for reference passes, the exact auction checkers for auction passes, the certificate restatement for the
+certificate, and the mirror's change sets for whether a pass stays incremental or warm.  Refused calls must return the
+status the header gives and leave behind what it says: the next pass of each kind shows it.  After every reference
+pass a fresh engine with the same settings, loaded from the mirror, must return the same arrays.
+
+PM_TEST_BIG=1 runs histories three times as long."""
+import os
+
+import numpy as np
+import pytest
+
+import auction_certificate as ac
+import engine_history as eh
+from protocol_b200 import abi
+from protocol_b200._lib import PrimeMatchError
+from protocol_b200.engine import Engine
+
+pytestmark = pytest.mark.gpu
+
+FIELDS = ("worker_group", "worker_ask", "group_ask", "group_off", "group_members", "ask_best", "ask_count")
+
+
+def new_engine(setting):
+    """An engine created with the setting's PM_TUNE_* knobs (they are read at pm_create)."""
+    env = {k: str(v) for k, v in eh.SETTINGS[setting].items()}
+    old = {k: os.environ.get(k) for k in env}
+    os.environ.update(env)
+    try:
+        return Engine(cost_tile_bytes=eh.TILE_BYTES.get(setting, 0))
+    finally:
+        for k, v in old.items():
+            if v is None:
+                os.environ.pop(k, None)
+            else:
+                os.environ[k] = v
+
+
+def refused(call, statuses):
+    """Run `call`; return its PrimeMatchError status, or None when it succeeded."""
+    try:
+        call()
+    except PrimeMatchError as ex:
+        assert statuses and ex.status in statuses, f"status {ex.status}, expected {statuses}: {ex}"
+        return ex.status
+    return None
+
+
+class Runner:
+    def __init__(self, shape, setting):
+        self.setting = setting
+        self.h = eh.History(shape, eh.cutoff_of(setting))
+        self.eng = new_engine(setting)
+        eh.load(self.eng, self.h)
+        self.counts = {}
+
+    def close(self):
+        self.eng.close()
+
+    def stored_state_kept(self):
+        h = self.h
+        if h.auc_state:
+            price, _, _ = self.eng.auction_state()
+            assert np.array_equal(price, h.price), "a refused call changed the stored auction state"
+
+    # ---- passes
+    def reference(self, kind):
+        h, eng = self.h, self.eng
+        why, statuses = h.refusal(kind)
+        plan = h.incremental_plan() if kind in eh.INCREMENTAL else None
+        if refused(lambda: eng.match(eh.MODES[kind]), statuses) is not None:
+            h.reference_done(False)
+            return
+        assert why is None, f"{kind}: ran, expected refusal {why}"
+        r = eng.fetch()
+        want = eh.expect_reference(h, kind)
+        for f in FIELDS:
+            assert np.array_equal(getattr(r, f), want[f]), f"{kind}: {f} differs from the oracle"
+        if "n_bumped" in want:
+            assert r.stats["n_bumped"] == want["n_bumped"], (kind, "n_bumped", r.stats["n_bumped"], want["n_bumped"])
+        if plan is not None:
+            full, n_tiles, en, dis, sure = plan
+            T, W = len(h.asks), h.n_workers
+            if sure:
+                assert r.stats["n_tiles"] == n_tiles, (kind, "n_tiles", r.stats["n_tiles"], n_tiles, full)
+            if not full:
+                assert r.stats["evals"] <= T * n_tiles + len(en) * W, (kind, r.stats)
+                if n_tiles == 0 and not en and not dis:
+                    assert r.stats["evals"] == 0, (kind, r.stats)
+        fresh = new_engine(self.setting)
+        eh.load(fresh, h)
+        fresh.match(eh.MODES[kind])
+        q = fresh.fetch()
+        fresh.close()
+        for f in FIELDS:
+            assert np.array_equal(getattr(r, f), getattr(q, f)), f"{kind}: {f} differs from a fresh engine's"
+        assert r.stats["n_bumped"] == q.stats["n_bumped"], (kind, "n_bumped")
+        h.reference_done(True)
+
+    def auction(self, kind):
+        h, eng = self.h, self.eng
+        why, statuses = h.refusal(kind)
+        want_warm, sure = h.warm_plan() if kind in ("warm", "repair") else (False, True)
+        if refused(lambda: eng.match(eh.MODES[kind]), statuses) is not None:
+            self.stored_state_kept()
+            return
+        assert why is None, f"{kind}: ran, expected refusal {why}"
+        res = eng.fetch()
+        got = np.full(len(h.asks), eh.NONE, dtype=np.uint32)
+        for ask, members in res.groups():
+            assert len(members) == 1
+            got[ask] = members[0]
+        price, warm, released = eng.auction_state()
+        rs = eng.auction_reverse_stats()
+        if not sure:
+            want_warm = warm
+        a, p, n, rel, wrs = eh.expect_auction(h, kind, want_warm)
+        assert warm == want_warm, (kind, "warm", warm)
+        assert np.array_equal(got, a), f"{kind}: assignment differs from the checker"
+        assert np.array_equal(price, p), f"{kind}: prices differ from the checker"
+        assert res.stats["n_rounds"] == n, (kind, "n_rounds", res.stats["n_rounds"], n)
+        assert released == rel, (kind, "n_released", released, rel)
+        assert rs == wrs, (kind, "reverse stats", rs, wrs)
+        h.auction_done(p, a)
+
+    def certificate(self):
+        h, eng = self.h, self.eng
+        why, statuses = h.refusal("certificate")
+        out = {}
+        if refused(lambda: out.update(eng.auction_certificate(ask_bound=True)), statuses) is not None:
+            self.stored_state_kept()
+            return
+        assert why is None, f"certificate: ran, expected refusal {why}"
+        want = eh.expect_certificate(h)
+        for k in ac.FIELDS:
+            assert out[k] == want[k], ("certificate", k, out[k], want[k])
+        assert np.array_equal(out["ask_bound"], want["ask_bound"])
+
+    def step(self, ev):
+        if ev[0] == "call":
+            eh.drive(self.eng, ev[1])
+            self.h.apply(ev[1])
+            return
+        kind = ev[1]
+        self.counts[kind] = self.counts.get(kind, 0) + 1
+        if kind in eh.REFERENCE:
+            self.reference(kind)
+        elif kind == "certificate":
+            self.certificate()
+        else:   # the auction kinds, and auction_incr (always refused)
+            self.auction(kind)
+
+
+def replay(shape, setting, events):
+    """Run `events` on one engine; an AssertionError names the failing event."""
+    r = Runner(shape, setting)
+    try:
+        for i, ev in enumerate(events):
+            try:
+                r.step(ev)
+            except AssertionError as ex:
+                what = ev[1] if ev[0] == "pass" else ev[1][0]
+                raise AssertionError(f"{shape}/{setting}: event {i} ({ev[0]} {what}): {ex}") from ex
+    finally:
+        r.close()
+    return r.counts
+
+
+@pytest.mark.parametrize("setting", list(eh.SETTINGS))
+@pytest.mark.parametrize("shape", eh.SHAPES)
+def test_history(shape, setting):
+    events, _ = eh.generate(shape, eh.seed_of(shape, setting), cutoff=eh.cutoff_of(setting),
+                            slot=eh.slot_of(shape, setting), n_slots=eh.N_SLOTS)
+    counts = replay(shape, setting, events)
+    assert all(counts.get(k, 0) for k in eh.PASSES), counts
+
+
+def shortened(shape, setting, events):
+    """The shortest prefix-and-subset of `events` that still fails (for turning a failing history into a regression
+    test): a history fails when replay raises AssertionError; any other exception counts as passing."""
+    def fails(evs):
+        try:
+            replay(shape, setting, evs)
+        except AssertionError:
+            return True
+        except Exception:
+            return False
+        return False
+
+    n = len(events)
+    while n > 1 and fails(events[:n - 1]):
+        n -= 1
+    return eh.shrink(events[:n], fails)
+
+
+def test_auction_fills_an_ask_of_max_group_size_zero():
+    """The first history finding, shortened to one load and one cold auction pass: PM_MODE_AUCTION's feasibility is
+    candidate, compatible, ask_price <= cap and reputation >= floor (prime_match.h); group sizes belong to the
+    reference modes.  An ask with max_group_size == 0 and feasible workers bids like any other, as in the oracle's
+    auction, while a first-fit pass between auction passes still never fills it, and the certificate and a warm pass
+    after that first-fit pass see the auction's rule again."""
+    from helpers import groups_equal, load_engine
+    from oracle import pm_oracle as orc
+    from test_gpu_auction_warm import tables
+
+    t, cap = tables(50, 700, 2)
+    F = eh.wc.feasible(t["wa"], t["wb"], t["asks"], t["opts"], t["bits"], t["words"], cap)
+    z = int(np.flatnonzero(F.any(axis=1))[0])
+    t["asks"] = t["asks"].copy()
+    t["asks"][z]["min_group_size"] = t["asks"][z]["max_group_size"] = 0
+    eng = Engine()
+    load_engine(eng, t)
+    eng.set_price_caps(cap)
+
+    def auction(mode):
+        eng.match(mode)
+        got = np.full(len(cap), eh.NONE, dtype=np.uint32)
+        for ask, members in eng.fetch().groups():
+            got[ask] = members[0]
+        return got, eng.auction_state()
+
+    want, wprice, _ = orc.soa_auction(t["wa"], t["wb"], t["asks"], t["opts"], t["bits"], t["words"], cap)
+    assert want[z] != eh.NONE
+    got, (price, _, _) = auction(abi.PM_MODE_AUCTION)
+    assert np.array_equal(got, want) and np.array_equal(price, wprice)
+    eng.match(abi.PM_MODE_FIRST_FIT | eh.LEAN)
+    r = eng.fetch()
+    og = orc.soa_form_groups(t["wa"], t["wb"], t["asks"], t["opts"], t["bits"], t["words"])
+    assert groups_equal(r, og) and not (r.worker_ask == z).any()
+    c = eng.auction_certificate(ask_bound=True)
+    wc_ = ac.certificate(F, t["wb"]["ext_ask_price"], cap, 1, wprice, want)
+    assert all(c[k] == wc_[k] for k in ac.FIELDS) and np.array_equal(c["ask_bound"], wc_["ask_bound"])
+    assert c["n_bad_holds"] == 0
+    got, (price, warm, released) = auction(eh.WARM)
+    assert warm and released == 0 and np.array_equal(got, want) and np.array_equal(price, wprice)
+    eng.close()
