@@ -6,6 +6,8 @@ clusters, one point), scattered coordinates, nobody located, groups larger than 
 groups (min 0), long hand-downs between configurations (ordered compaction), solo configurations after grouped ones.
 The edges of the coordinate space (EDGES: poles, antimeridian, antipodes, latitudes beyond ±90) run on these and on
 the experimental latitude-banded sweep (PM_TUNE_PROX=1), whose pruning must switch off where the latitude bound fails.
+Past the first stride (thousands of configurations, hand-downs across the shared-memory limit, seed-parallel batches on
+many CTAs, selections in several chunks of 16): tests/test_gpu_proximity_sweeps.py.
 """
 import math
 import os
