@@ -208,6 +208,31 @@ int pm_set_asks(pm_engine*, const pm_ask* asks, uint32_t n_asks,
  * PM_E_UNSUPPORTED while any ask is disabled.  The stored evaluation of PM_INCREMENTAL is kept: see "Incremental
  * passes".                                                                                                          */
 int pm_set_ask_enabled(pm_engine*, const uint32_t* idx, const uint8_t* enabled, uint32_t n);
+/* Ask-table deltas: a resident ask table changed in place (a new task with a price cap is an appended row, a finished
+ * one a removed row).  After any sequence of pm_set_asks, pm_update_asks, pm_resize_asks and pm_set_ask_enabled calls
+ * the engine is the engine pm_set_asks would give for the current rows with the same enabled mask: every array
+ * pm_fetch_result returns, pm_build_cost_tile and a cold auction pass are bit-identical to a fresh engine's, with or
+ * without PM_INCREMENTAL, on every path and in every mode.  Ask index stays priority.
+ *   pm_update_asks   replace rows idx[i] (each < n_asks) by asks[i]; asks[i].opt_off / n_opts index `opts`, as in
+ *                    pm_set_asks.  A replaced row keeps its enabled flag, its price cap and its reputation floor.  For
+ *                    repeated indices the last entry decides.
+ *   pm_resize_asks   shrink: drop asks [n_asks, old); grow: append `n_asks - old` rows from `added` (options in `opts`)
+ *                    at the lowest priorities, enabled, with cap 0 and floor 0 until pm_set_ask_price_caps /
+ *                    pm_set_ask_min_reputation set them (both still take exactly n_asks entries).  Inserting in the
+ *                    middle is pm_set_asks.
+ * Refusals, none of which changes anything (no table, no stored evaluation, no auction state, no pm_table_version):
+ * PM_E_INVALID for a null pointer with a count > 0, an index >= n_asks, max_group_size < min_group_size, an option
+ * range outside `opts`, growth without `added`, n_asks >= 2^30 or more than 2^31 converted option rows; PM_E_STATE
+ * without an ask table.  Every row is checked on the host before anything on the device is touched.  A row that
+ * references a pattern beyond the model table is accepted; the next pass returns PM_E_STATE, as after pm_set_asks.
+ * Unlike pm_set_asks, both keep the stored evaluation of PM_INCREMENTAL and the stored auction state: see "Incremental
+ * passes", "Auction warm start", "Auction warm repair" and "Auction certificate".  Each call converts the whole table
+ * again on the device (O(T + the option rows)).  Only the option ranges the new rows reference are copied from `opts`
+ * (a caller may pass its whole option table); the option rows replaced or removed rows leave behind are compacted
+ * away once they outnumber the live ones.                                                                                    */
+int pm_update_asks(pm_engine*, const uint32_t* idx, const pm_ask* asks, uint32_t n,
+                   const pm_gpu_opt* opts, uint32_t n_opts);
+int pm_resize_asks(pm_engine*, uint32_t n_asks, const pm_ask* added, const pm_gpu_opt* opts, uint32_t n_opts);
 int pm_set_model_table(pm_engine*, const uint32_t* bits, uint32_t n_patterns,
                        uint32_t n_models, uint32_t words_per_pattern);
 /* replaces NodeStore::get_nodes per pass (store/domains/node_store.rs:163-209);
@@ -320,7 +345,13 @@ enum pm_path {
  * ask was disabled since ("orphans", from the ask after it) and evaluates every worker against the asks enabled since
  * (only those whose stored first ask lies beyond the first of them; an ask switched off and on again counts as
  * neither).  With many asks enabled the pass evaluates everything instead: the pairs of that walk, |E| x nw, count as
- * |E| x nw / T written rows against the PM_TUNE_INCR cutoff, next to the range's written rows.  Each engine decides
+ * |E| x nw / T written rows against the PM_TUNE_INCR cutoff, next to the range's written rows.
+ * pm_update_asks and pm_resize_asks keep it too.  A replaced row counts as disabled and enabled again: it is in E when
+ * it is enabled now and in D when it was enabled at the stored evaluation, and its orphans are walked from the ask
+ * itself, not the one after it (the new row may still accept them); workers whose stored first ask lies beyond it
+ * meet it in the E-pass.  Appended rows are in E.  A shrink sets every stored first ask >= the new n_asks to PM_NONE
+ * (that worker had no feasible ask before it).  Replaced and appended asks count against the cutoff as E does.  Each
+ * engine decides
  * against the cutoff by its own range's counts, so in one sharded pass some ranks may evaluate their range in full
  * while others run incrementally; every rank still makes the one exchange.  pm_stats under the flag (nw = the range's
  * workers, W on an unsharded engine):
@@ -343,7 +374,12 @@ enum pm_path {
  * pass's is; it need not equal the cold pass's result.  The warm pass runs when a stored state exists and
  * |R0| + |A0| <= the PM_TUNE_INCR cutoff, else the pass is cold.  pm_set_asks, pm_set_model_table,
  * pm_set_worker_count, pm_set_auction_params, pm_set_shard, pm_attach_comm and a failed auction pass discard the
- * stored state; reference-mode passes leave it alone.  pm_stats of a warm pass: evals = the release's pair evaluations
+ * stored state; reference-mode passes leave it alone.  pm_update_asks and pm_resize_asks keep it: A0 also holds every
+ * replaced ask and every appended ask (which has no stored cap or floor), and step 1 also releases the holder of every
+ * removed ask (a shrink of pm_resize_asks): that worker becomes unowned at its stored price as the shrink runs, joins
+ * R at price 0 here when its price was positive, and is not counted in n_released (its ask no longer exists).  The
+ * cutoff test counts |R0| + |A0| + the rows past a worker shrink + the removed asks that held a worker.  pm_stats of a
+ * warm pass: evals = the release's pair evaluations
  * (classes x raised workers per iteration) + the rounds'; n_rounds = the warm rounds.
  * pm_auction_state reports on the last auction pass: price [its n_workers] (or NULL), warm = 1 if it started warm,
  * n_released = the asks its warm start released; PM_E_STATE when no auction pass ran since the state was discarded. */
@@ -386,7 +422,9 @@ int pm_auction_reverse_stats(pm_engine*, uint32_t* n_phases, uint32_t* n_reverse
  *   4. one reverse stage at eps = 1 (the rounds of PM_AUCTION_REVERSE), until no unowned worker has a positive price.
  * eps-complementary slackness holds after every step, so the result is within T of the optimum of the current instance
  * (the optimum with cost_scale = T + 1), as a cold pass's is (DESIGN 4); it need not equal the cold or the warm pass's
- * result.  Nothing is released beyond step 1.  pm_auction_state: warm = 1, n_released = the asks of step 1.
+ * result.  Nothing is released beyond step 1.  After pm_update_asks / pm_resize_asks, A0 and the release are those
+ * of the warm start: a removed ask's worker is unowned at its stored price.  pm_auction_state: warm = 1, n_released =
+ * the asks of step 1.
  * pm_auction_reverse_stats: 1 phase, the reverse rounds and bids of step 4.  pm_stats: n_rounds = the forward rounds;
  * evals = classes x raised rows + the rounds' evaluations + classes x reverse bids; with PM_CFG_TIMING, ms_build = the
  * reverse rounds.  The pass stores its state like any auction pass.  Refusals are those of PM_AUCTION_WARM (disabled
@@ -409,7 +447,9 @@ int pm_auction_reverse_stats(pm_engine*, uint32_t* n_phases, uint32_t* n_reverse
  * assignment.  cost, bound, gap and the
  * priced-unowned sum are exact 128-bit integers (hi: the signed high 64 bits, lo: the low 64 bits).  evals = T x W.
  * ask_bound (NULL-able): row(t) per ask.  Refusals, none of which changes anything: NULL engine or out: PM_E_INVALID;
- * no stored state (where pm_auction_state returns PM_E_STATE), a worker count other than the stored pass's, or an ask
+ * no stored state (where pm_auction_state returns PM_E_STATE), a worker count other than the stored pass's, an ask table
+ * resized by pm_resize_asks since the last auction pass (pm_update_asks is audited: n_bad_holds shows the holds the new
+ * rows reject), or an ask
  * referencing a model pattern missing from the model table: PM_E_STATE; disabled asks: PM_E_UNSUPPORTED; tables and
  * parameters outside the auction's integer domain: PM_E_INVALID.  The call changes nothing pm_fetch_result,
  * pm_get_stats, pm_table_version, pm_auction_state or pm_auction_reverse_stats report, nor what the next warm or repair
@@ -521,6 +561,10 @@ pm_engine*  pm_multi_engine(pm_multi*, uint32_t i);   /* per-device access (stat
 const char* pm_multi_last_error(const pm_multi*);
 int pm_multi_set_asks(pm_multi*, const pm_ask* asks, uint32_t n_asks, const pm_gpu_opt* opts, uint32_t n_opts);
 int pm_multi_set_ask_enabled(pm_multi*, const uint32_t* idx, const uint8_t* enabled, uint32_t n);
+/* pm_update_asks / pm_resize_asks on every device; a refused call changes no device */
+int pm_multi_update_asks(pm_multi*, const uint32_t* idx, const pm_ask* asks, uint32_t n,
+                         const pm_gpu_opt* opts, uint32_t n_opts);
+int pm_multi_resize_asks(pm_multi*, uint32_t n_asks, const pm_ask* added, const pm_gpu_opt* opts, uint32_t n_opts);
 int pm_multi_set_model_table(pm_multi*, const uint32_t* bits, uint32_t n_patterns, uint32_t n_models,
                              uint32_t words_per_pattern);
 int pm_multi_set_worker_count(pm_multi*, uint32_t n_workers);

@@ -939,6 +939,19 @@ __global__ void pm_auction_warm_seed(AuctionParams p, const uint32_t* __restrict
     }
   }
 }
+// pm_resize_asks shrank the ask table under a stored state: every kept row held by a removed ask (index >= n_asks)
+// becomes unowned at its stored price, as a released worker does; `count` gets how many there were
+__global__ void pm_auction_drop_asks(uint32_t* __restrict__ owner, uint32_t n_rows, uint32_t n_asks, uint32_t* __restrict__ count) {
+  uint32_t k = 0;
+  for (uint32_t w = blockIdx.x * blockDim.x + threadIdx.x; w < n_rows; w += gridDim.x * blockDim.x) {
+    const uint32_t t = owner[w];
+    if (t != kNone && t >= n_asks) {
+      owner[w] = kNone;
+      ++k;
+    }
+  }
+  if (k) atomicAdd(count, k);
+}
 // every unowned worker with a positive price (the released ones, and what an eps-scaled pass left inflated) goes to 0
 // and joins R; mark[w] says whether it did
 __global__ void pm_auction_warm_reset(AuctionParams p, uint32_t* __restrict__ raised, uint32_t* __restrict__ mark) {

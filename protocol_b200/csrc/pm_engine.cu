@@ -305,6 +305,14 @@ struct pm_engine {
   DevBuf<pm_ask> raw_asks;
   DevBuf<pm_gpu_opt> raw_opts;
   DevBuf<uint32_t> ask_counts, ask_newoff;
+  // The caller's rows as raw_asks holds them (opt_off into raw_opts), kept on the host so that pm_update_asks and
+  // pm_resize_asks can check a delta against the whole table before anything changes.  raw_n_opts: rows of raw_opts in
+  // use (replaced rows leave theirs behind until a compaction); opt_rows / live_opts: the sums over the asks of
+  // max(n_opts, 1) (the converted table's rows) and of n_opts.
+  std::vector<pm_ask> asks_h;
+  uint32_t raw_n_opts = 0;
+  uint64_t opt_rows = 0, live_opts = 0;
+  DevBuf<pm_ask> upd_asks;             // staging of pm_update_asks / pm_resize_asks
   bool asks_small = true;      // every ask operand fits the fast predicate (pm_device.cuh DevOptF)
   bool workers_small = false;  // ... and every worker operand (checked on the device)
   bool prices_narrow = false;  // every worker price < 0x7FFFFFFF: the first-fit tile can hold the 32-bit cost word alone
@@ -343,24 +351,40 @@ struct pm_engine {
   DevBuf<uint32_t> dirty_dev;
   DevBuf<unsigned long long> incr_evals;
   bool incr_evals_pending = false;      // stats.evals of the incremental pass arrives with the pass's one sync
-  // The mask the stored evaluation was taken under (eval_on) and the asks toggled since (toggled, each once; an ask
-  // switched off and on again is listed but has eval_on == ask_on).  walk_start: the orphan walk's start bounds.
-  std::vector<uint8_t> eval_on, toggle_mark;
+  // The mask the stored evaluation was taken under (eval_on) and the asks toggled, replaced or appended since (toggled,
+  // each once; an ask switched off and on again is listed but has eval_on == ask_on; replaced: repl_mark).  Appended
+  // asks have eval_on == 0.  walk_start: the orphan walk's start bounds.
+  std::vector<uint8_t> eval_on, toggle_mark, repl_mark;
   std::vector<uint32_t> toggled;
   DevBuf<uint32_t> walk_start, toggle_dev;
 
-  // E (enabled since the stored evaluation) and D (disabled since), increasing
+  // E (enabled since the stored evaluation) and D (disabled since), increasing; a D entry is ask << 1 | replaced.  A
+  // replaced row counts as disabled and enabled again: in E when it is enabled now, in D when it was at the stored
+  // evaluation, its orphans walked from the ask itself
   void split_toggles(std::vector<uint32_t>* en, std::vector<uint32_t>* dis) const {
     en->clear();
     dis->clear();
-    for (uint32_t t : toggled)
-      if (ask_on[t] != eval_on[t]) (ask_on[t] ? en : dis)->push_back(t);
+    for (uint32_t t : toggled) {
+      if (repl_mark[t]) {
+        if (ask_on[t]) en->push_back(t);
+        if (eval_on[t]) dis->push_back(t << 1 | 1u);
+      } else if (ask_on[t] != eval_on[t]) {
+        if (ask_on[t]) en->push_back(t);
+        else dis->push_back(t << 1);
+      }
+    }
     std::sort(en->begin(), en->end());
     std::sort(dis->begin(), dis->end());
   }
   void clear_toggled() {
-    for (uint32_t t : toggled) { toggle_mark[t] = 0; eval_on[t] = ask_on[t]; }
+    for (uint32_t t : toggled) { toggle_mark[t] = 0; repl_mark[t] = 0; eval_on[t] = ask_on[t]; }
     toggled.clear();
+  }
+  void mark_toggled(uint32_t t) {
+    if (eval_valid && !toggle_mark[t]) {
+      toggle_mark[t] = 1;
+      toggled.push_back(t);
+    }
   }
   void clear_dirty() {
     for (uint32_t i : dirty_rows) dirty_mark[i] = 0;
@@ -468,6 +492,11 @@ struct pm_engine {
   DevBuf<long long> cert_bound;
   PinBuf<uint64_t> h_cert_acc;
   PinBuf<long long> h_cert_bound;
+  // pm_resize_asks since the stored state: the removed asks that held a kept row (those rows are unowned now, at their
+  // stored prices; they count against the cutoff), and whether the ask table was resized at all (the certificate then
+  // waits for the next pass)
+  uint32_t auc_removed_held = 0;
+  bool auc_asks_resized = false;
   void auc_discard() {
     auc_state = false;
     auc_rows.clear();
@@ -475,6 +504,14 @@ struct pm_engine {
     auc_row_mark.clear();
     auc_ask_mark.clear();
     auc_rows_over = false;
+    auc_removed_held = 0;
+    auc_asks_resized = false;
+  }
+  void auc_mark_ask(uint32_t t) {   // A0: toggled, replaced or appended since the stored state
+    if (auc_state && !auc_ask_mark[t]) {
+      auc_ask_mark[t] = 1;
+      auc_toggled.push_back(t);
+    }
   }
   void auc_mark_row(uint32_t i) {
     if (!auc_state || auc_rows_over || i >= auc_kept || auc_row_mark[i]) return;
@@ -640,6 +677,183 @@ static int use_ask_form(pm_engine* e, bool auction) {
   return PM_OK;
 }
 
+// The whole ask table converted from the resident raw rows, O(T + sum K) on the device: pm_ask_counts -> scan ->
+// pm_ask_convert.  pm_set_asks and every delta of pm_update_asks / pm_resize_asks take this one path.  Every row comes
+// out enabled, in the reference modes' form; *st gets the status bits.  Sets n_opts, max_pattern_row and asks_small.
+static int convert_asks(pm_engine* e, uint32_t n_asks, uint32_t n_raw_opts, uint64_t opt_rows, uint32_t* st) {
+  PM_CUDA(e->ask_counts.ensure((size_t)n_asks + 1)); PM_CUDA(e->ask_newoff.ensure((size_t)n_asks + 1));
+  PM_CUDA(e->asks.ensure(n_asks)); PM_CUDA(e->amin.ensure(n_asks)); PM_CUDA(e->amax.ensure(n_asks));
+  const size_t opt_cap = std::max<size_t>(n_raw_opts, (size_t)opt_rows);
+  PM_CUDA(e->opts.ensure(opt_cap)); PM_CUDA(e->opts_fast.ensure(opt_cap)); PM_CUDA(e->frows.ensure(n_asks));
+  e->rows_bound = false;
+  e->rows_auction = false;
+  e->auc_classes_valid = false;
+  PM_CUDA(cudaMemsetAsync(e->counters.p + 12, 0, 8, e->stream));
+  pm::pm_ask_counts<<<blocks_for((size_t)n_asks + 1, 256), 256, 0, e->stream>>>(e->raw_asks.p, n_asks, n_raw_opts, e->ask_counts.p,
+                                                                                 e->counters.p + 12);
+  PM_LAUNCH_CHECK("pm_ask_counts");
+  {
+    size_t tmp = 0;
+    cub::DeviceScan::ExclusiveSum(nullptr, tmp, e->ask_counts.p, e->ask_newoff.p, (int)(n_asks + 1), e->stream);
+    PM_CUDA(e->cub_tmp.ensure(tmp));
+    PM_CUDA(cub::DeviceScan::ExclusiveSum(e->cub_tmp.p, tmp, e->ask_counts.p, e->ask_newoff.p, (int)(n_asks + 1), e->stream));
+  }
+  if (n_asks) {
+    pm::pm_ask_convert<<<blocks_for(n_asks, 256), 256, 0, e->stream>>>(e->raw_asks.p, e->raw_opts.p, n_asks, e->ask_newoff.p,
+                                                                        ask_tables(e), e->counters.p + 12, e->counters.p + 13);
+    PM_LAUNCH_CHECK("pm_ask_convert");
+  }
+  PM_CUDA(cudaMemcpyAsync(e->h_scalars.p + 20, e->counters.p + 12, 8, cudaMemcpyDeviceToHost, e->stream));
+  PM_CUDA(cudaMemcpyAsync(e->h_scalars.p + 22, e->ask_newoff.p + n_asks, 4, cudaMemcpyDeviceToHost, e->stream));
+  PM_CUDA(cudaStreamSynchronize(e->stream));
+  *st = e->h_scalars.p[20];
+  e->n_opts = e->h_scalars.p[22];
+  e->max_pattern_row = e->h_scalars.p[21];
+  e->asks_small = (*st & pm::kAskNotSmall) == 0;
+  return PM_OK;
+}
+
+// Per ask its kind, and the per-table facts over the enabled asks (asks_h and ask_on over n_asks)
+static void recount_kinds(pm_engine* e) {
+  const uint32_t T = e->n_asks;
+  e->ask_kind.resize(T);
+  e->n_off = e->n_on_not_solo = e->n_on_max_zero = 0;
+  for (uint32_t t = 0; t < T; ++t) {
+    const pm_ask& a = e->asks_h[t];
+    e->ask_kind[t] = (uint8_t)((a.min_group_size == 1 && a.max_group_size == 1 ? 0 : pm_engine::kAskKindNotSolo) |
+                               (a.max_group_size == 0 ? pm_engine::kAskKindMaxZero : 0));
+    if (e->ask_on[t]) e->count_kind(t, +1);
+    else ++e->n_off;
+  }
+  e->all_solo = e->n_on_not_solo == 0;
+  e->any_max_zero = e->n_on_max_zero != 0;
+}
+
+// The caller's rows of pm_update_asks (idx given) or pm_resize_asks, checked on the host before anything changes: the
+// indices, the group sizes and the option ranges within `opts` of every entry; then, over the distinct entries (the
+// last one of an index decides), the converted option rows of the table they make.  The distinct entries go to
+// uidx / urows (idx null: rows appended after the n_asks rows there are).
+static int check_ask_rows(const pm_engine* e, const char* fn, const uint32_t* idx, const pm_ask* rows, uint32_t n,
+                          uint32_t n_opts, std::vector<uint32_t>* uidx, std::vector<pm_ask>* urows, std::string* err) {
+  for (uint32_t i = 0; i < n; ++i) {
+    if (idx && idx[i] >= e->n_asks) { *err = std::string(fn) + ": ask index out of range"; return PM_E_INVALID; }
+    if (rows[i].max_group_size < rows[i].min_group_size) {
+      *err = std::string(fn) + ": max_group_size < min_group_size (Plugin configuration is invalid)";
+      return PM_E_INVALID;
+    }
+    if ((uint64_t)rows[i].opt_off + rows[i].n_opts > n_opts) { *err = std::string(fn) + ": option range out of bounds"; return PM_E_INVALID; }
+  }
+  uidx->clear();
+  urows->clear();
+  uint64_t opt_rows = e->opt_rows;
+  if (idx) {
+    std::vector<uint32_t> ord(n);
+    for (uint32_t i = 0; i < n; ++i) ord[i] = i;
+    std::stable_sort(ord.begin(), ord.end(), [&](uint32_t x, uint32_t y) { return idx[x] < idx[y]; });
+    for (uint32_t j = 0; j < n; ++j) {
+      if (j + 1 < n && idx[ord[j + 1]] == idx[ord[j]]) continue;
+      const uint32_t t = idx[ord[j]];
+      uidx->push_back(t);
+      urows->push_back(rows[ord[j]]);
+      opt_rows -= std::max<uint32_t>(e->asks_h[t].n_opts, 1u);
+    }
+  } else {
+    for (uint32_t i = 0; i < n; ++i) {
+      uidx->push_back(e->n_asks + i);
+      urows->push_back(rows[i]);
+    }
+  }
+  for (const pm_ask& a : *urows) opt_rows += std::max<uint32_t>(a.n_opts, 1u);
+  if (opt_rows >= (1ull << 31)) { *err = std::string(fn) + ": too many option rows"; return PM_E_INVALID; }
+  return PM_OK;
+}
+
+// pm_update_asks / pm_resize_asks after their checks (the masks already sized to n_asks): rows[i] goes to ask idx[i]
+// (distinct, < n_asks; a grow's rows are the indices past the kept ones), the option range it references in `opts`
+// appended to raw_opts and its opt_off rebased onto that copy; raw_opts is compacted when its dead rows outnumber the
+// live ones; then the whole table is converted again and the disabled asks are turned off (pm_ask_toggle).
+static int commit_asks(pm_engine* e, uint32_t n_asks, const uint32_t* idx, const pm_ask* rows, uint32_t n,
+                       const pm_gpu_opt* opts) {
+  const uint32_t base = e->raw_n_opts;
+  // only the option ranges the new rows reference go up, each row's range after the last, opt_off rebased onto it:
+  // a caller may pass its whole option table for one changed ask without leaving that table behind as dead rows
+  std::vector<pm_ask> moved(rows, rows + n);
+  std::vector<pm_gpu_opt> add;
+  for (pm_ask& a : moved) {
+    const uint32_t off = base + (uint32_t)add.size();
+    add.insert(add.end(), opts + a.opt_off, opts + a.opt_off + a.n_opts);
+    a.opt_off = off;
+  }
+  e->asks_h.resize(n_asks);
+  for (uint32_t i = 0; i < n; ++i) e->asks_h[idx[i]] = moved[i];
+  uint64_t opt_rows = 0, live = 0;
+  for (const pm_ask& a : e->asks_h) {
+    opt_rows += std::max<uint32_t>(a.n_opts, 1u);
+    live += a.n_opts;
+  }
+  const uint64_t raw = (uint64_t)base + add.size();
+  if (raw - std::min(raw, live) > live || raw >= (1ull << 31)) {
+    // compaction: every ask's options copied once, in ask order, from the rows as they stand (old ones read back)
+    std::vector<pm_gpu_opt> all(raw);
+    if (base) {
+      PM_CUDA(cudaMemcpyAsync(all.data(), e->raw_opts.p, (size_t)base * sizeof(pm_gpu_opt), cudaMemcpyDeviceToHost, e->stream));
+      PM_CUDA(cudaStreamSynchronize(e->stream));
+    }
+    if (!add.empty()) std::memcpy(all.data() + base, add.data(), add.size() * sizeof(pm_gpu_opt));
+    std::vector<pm_gpu_opt> packed;
+    packed.reserve(live);
+    for (pm_ask& a : e->asks_h) {
+      const uint32_t off = (uint32_t)packed.size();
+      packed.insert(packed.end(), all.begin() + a.opt_off, all.begin() + a.opt_off + a.n_opts);
+      a.opt_off = off;
+    }
+    PM_CUDA(e->raw_asks.ensure(n_asks)); PM_CUDA(e->raw_opts.ensure(packed.size()));
+    if (n_asks)
+      PM_CUDA(cudaMemcpyAsync(e->raw_asks.p, e->asks_h.data(), (size_t)n_asks * sizeof(pm_ask), cudaMemcpyHostToDevice, e->stream));
+    if (!packed.empty())
+      PM_CUDA(cudaMemcpyAsync(e->raw_opts.p, packed.data(), packed.size() * sizeof(pm_gpu_opt), cudaMemcpyHostToDevice, e->stream));
+    PM_CUDA(cudaStreamSynchronize(e->stream));   // `packed` is a local
+    e->raw_n_opts = (uint32_t)packed.size();
+  } else {
+    if (!add.empty()) {
+      PM_CUDA(e->raw_opts.grow_keep(raw, base, e->stream));
+      PM_CUDA(cudaMemcpyAsync(e->raw_opts.p + base, add.data(), add.size() * sizeof(pm_gpu_opt), cudaMemcpyHostToDevice, e->stream));
+    }
+    PM_CUDA(e->raw_asks.grow_keep(std::max<uint32_t>(n_asks, 1), std::min<size_t>(e->raw_asks.n, n_asks), e->stream));
+    if (n) {
+      PM_CUDA(e->scratch_idx.ensure(n)); PM_CUDA(e->upd_asks.ensure(n));
+      PM_CUDA(cudaMemcpyAsync(e->scratch_idx.p, idx, (size_t)n * 4, cudaMemcpyHostToDevice, e->stream));
+      PM_CUDA(cudaMemcpyAsync(e->upd_asks.p, moved.data(), (size_t)n * sizeof(pm_ask), cudaMemcpyHostToDevice, e->stream));
+      pm::pm_scatter_asks<<<blocks_for(n, 256), 256, 0, e->stream>>>(e->raw_asks.p, e->scratch_idx.p, e->upd_asks.p, n);
+      PM_LAUNCH_CHECK("pm_scatter_asks");
+    }
+    e->raw_n_opts = (uint32_t)raw;
+  }
+  e->opt_rows = opt_rows;
+  e->live_opts = live;
+  uint32_t st = 0;
+  {
+    const int rc = convert_asks(e, n_asks, e->raw_n_opts, opt_rows, &st);   // (synchronises: `moved` and `add` are no longer read)
+    if (rc != PM_OK) return rc;
+  }
+  if (st & (pm::kAskBadSizes | pm::kAskBadRange)) return e->fail(PM_E_INVALID, "ask table delta: rows out of bounds");
+  e->n_asks = n_asks;
+  std::vector<uint32_t> off;   // ask << 1 | 0, as pm_ask_toggle takes it
+  for (uint32_t t = 0; t < n_asks; ++t)
+    if (!e->ask_on[t]) off.push_back(t << 1);
+  if (!off.empty()) {
+    PM_CUDA(e->toggle_dev.ensure(off.size()));
+    PM_CUDA(cudaMemcpyAsync(e->toggle_dev.p, off.data(), off.size() * 4, cudaMemcpyHostToDevice, e->stream));
+    pm::pm_ask_toggle<<<blocks_for(off.size(), 256), 256, 0, e->stream>>>(e->raw_asks.p, e->raw_opts.p, e->ask_newoff.p,
+                                                                          e->toggle_dev.p, (uint32_t)off.size(), ask_tables(e), true);
+    PM_LAUNCH_CHECK("pm_ask_toggle");
+    PM_CUDA(cudaStreamSynchronize(e->stream));   // `off` is a local
+  }
+  recount_kinds(e);
+  e->matched = e->local_done = false;
+  return PM_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -725,7 +939,7 @@ void pm_destroy(pm_engine* e) {
   if (e->stream) cudaStreamSynchronize(e->stream);
   e->wa.release(); e->wb.release(); e->lat.release(); e->lon.release(); e->addr_rank.release();
   e->asks.release(); e->opts.release(); e->opts_fast.release(); e->frows.release();
-  e->raw_asks.release(); e->raw_opts.release(); e->ask_counts.release(); e->ask_newoff.release(); e->amin.release(); e->amax.release(); e->bits.release();
+  e->raw_asks.release(); e->raw_opts.release(); e->upd_asks.release(); e->ask_counts.release(); e->ask_newoff.release(); e->amin.release(); e->amax.release(); e->bits.release();
   e->scratch_idx.release(); e->scratch_flags.release();
   e->upd_a.release(); e->upd_b.release(); e->upd_lat.release(); e->upd_lon.release();
   e->cost.release(); e->first_ask.release(); e->ask_count.release(); e->ask_best.release();
@@ -784,58 +998,37 @@ int pm_set_asks(pm_engine* e, const pm_ask* asks, uint32_t n_asks, const pm_gpu_
   PM_CUDA(cudaSetDevice(e->device));
   // the caller's tables go up as they are; the device converts them (pm_ask_convert)
   PM_CUDA(e->raw_asks.ensure(n_asks)); PM_CUDA(e->raw_opts.ensure(n_opts));
-  PM_CUDA(e->ask_counts.ensure((size_t)n_asks + 1)); PM_CUDA(e->ask_newoff.ensure((size_t)n_asks + 1));
-  PM_CUDA(e->asks.ensure(n_asks)); PM_CUDA(e->amin.ensure(n_asks)); PM_CUDA(e->amax.ensure(n_asks));
   // asks may share or overlap option rows, so the converted table (one private range per ask) can be longer than
   // the caller's: size it by the sum of the per-ask counts
-  uint64_t opt_rows = 0;
-  for (uint32_t i = 0; i < n_asks; ++i) opt_rows += std::max<uint32_t>(asks[i].n_opts, 1u);   // an ask without options gets a neutral row
+  uint64_t opt_rows = 0, live = 0;
+  for (uint32_t i = 0; i < n_asks; ++i) {
+    opt_rows += std::max<uint32_t>(asks[i].n_opts, 1u);   // an ask without options gets a neutral row
+    live += asks[i].n_opts;
+  }
   if (opt_rows >= (1ull << 31)) return e->fail(PM_E_INVALID, "pm_set_asks: too many option rows");
-  const size_t opt_cap = std::max<size_t>(n_opts, (size_t)opt_rows);
-  PM_CUDA(e->opts.ensure(opt_cap)); PM_CUDA(e->opts_fast.ensure(opt_cap)); PM_CUDA(e->frows.ensure(n_asks));
-  e->rows_bound = false;
   if (n_asks) PM_CUDA(cudaMemcpyAsync(e->raw_asks.p, asks, (size_t)n_asks * sizeof(pm_ask), cudaMemcpyHostToDevice, e->stream));
   if (n_opts) PM_CUDA(cudaMemcpyAsync(e->raw_opts.p, opts, (size_t)n_opts * sizeof(pm_gpu_opt), cudaMemcpyHostToDevice, e->stream));
-  PM_CUDA(cudaMemsetAsync(e->counters.p + 12, 0, 8, e->stream));
-  pm::pm_ask_counts<<<blocks_for((size_t)n_asks + 1, 256), 256, 0, e->stream>>>(e->raw_asks.p, n_asks, n_opts, e->ask_counts.p, e->counters.p + 12);
-  PM_LAUNCH_CHECK("pm_ask_counts");
-  {
-    size_t tmp = 0;
-    cub::DeviceScan::ExclusiveSum(nullptr, tmp, e->ask_counts.p, e->ask_newoff.p, (int)(n_asks + 1), e->stream);
-    PM_CUDA(e->cub_tmp.ensure(tmp));
-    PM_CUDA(cub::DeviceScan::ExclusiveSum(e->cub_tmp.p, tmp, e->ask_counts.p, e->ask_newoff.p, (int)(n_asks + 1), e->stream));
-  }
-  if (n_asks) {
-    pm::pm_ask_convert<<<blocks_for(n_asks, 256), 256, 0, e->stream>>>(e->raw_asks.p, e->raw_opts.p, n_asks, e->ask_newoff.p,
-                                                                        ask_tables(e), e->counters.p + 12, e->counters.p + 13);
-    PM_LAUNCH_CHECK("pm_ask_convert");
-  }
-  std::vector<uint8_t> kind(n_asks);
-  for (uint32_t i = 0; i < n_asks; ++i)
-    kind[i] = (uint8_t)((asks[i].min_group_size == 1 && asks[i].max_group_size == 1 ? 0 : pm_engine::kAskKindNotSolo) |
-                        (asks[i].max_group_size == 0 ? pm_engine::kAskKindMaxZero : 0));
-  PM_CUDA(cudaMemcpyAsync(e->h_scalars.p + 20, e->counters.p + 12, 8, cudaMemcpyDeviceToHost, e->stream));
-  PM_CUDA(cudaMemcpyAsync(e->h_scalars.p + 22, e->ask_newoff.p + n_asks, 4, cudaMemcpyDeviceToHost, e->stream));
-  PM_CUDA(cudaStreamSynchronize(e->stream));  // also: the caller's tables are no longer read after return
-  const uint32_t st = e->h_scalars.p[20];
   e->have_asks = false;
+  uint32_t st = 0;
+  {
+    const int rc = convert_asks(e, n_asks, n_opts, opt_rows, &st);   // also: the caller's tables are no longer read after return
+    if (rc != PM_OK) return rc;
+  }
   // NodeGroupConfiguration::is_valid, mod.rs:55-60 (the reference panics at construction)
   if (st & pm::kAskBadSizes)
     return e->fail(PM_E_INVALID, "pm_set_asks: max_group_size < min_group_size (Plugin configuration is invalid)");
   if (st & pm::kAskBadRange) return e->fail(PM_E_INVALID, "pm_set_asks: option range out of bounds");
   e->n_asks = n_asks;
-  e->n_opts = e->h_scalars.p[22];
-  e->max_pattern_row = e->h_scalars.p[21];
-  e->asks_small = (st & pm::kAskNotSmall) == 0;
+  e->asks_h.assign(asks, asks + n_asks);
+  e->raw_n_opts = n_opts;
+  e->opt_rows = opt_rows;
+  e->live_opts = live;
   // every ask enabled
-  e->ask_kind = std::move(kind);
   e->ask_on.assign(n_asks, 1);
   e->eval_on.assign(n_asks, 1);
   e->toggle_mark.assign(n_asks, 0);
-  e->n_off = e->n_on_not_solo = e->n_on_max_zero = 0;
-  for (uint32_t i = 0; i < n_asks; ++i) e->count_kind(i, +1);
-  e->all_solo = e->n_on_not_solo == 0;
-  e->any_max_zero = e->n_on_max_zero != 0;
+  e->repl_mark.assign(n_asks, 0);
+  recount_kinds(e);
   e->have_caps = false;
   e->have_min_rep = false;
   e->auc_classes_valid = false;
@@ -899,6 +1092,142 @@ int pm_set_ask_enabled(pm_engine* e, const uint32_t* idx, const uint8_t* enabled
   e->auc_classes_valid = false;
   e->matched = e->local_done = false;
   return PM_OK;
+} catch (...) { return pm_guard_rc(); }
+
+// Ask-table deltas.  Both calls check everything on the host first (a refusal changes nothing), then edit the raw rows
+// and convert the whole table again (commit_asks).  The stored evaluation and the stored auction state are kept: the
+// changed asks are listed for the next incremental pass (E / D) and the next warm pass (A0).  A failure after the
+// checks (a CUDA error) leaves tables that are not trusted: the ask table is dropped, as a failed pm_set_asks does.
+static int ask_delta_failed(pm_engine* e, int rc) {
+  if (rc != PM_OK) {
+    e->have_asks = false;
+    e->invalidate_eval();
+    e->auc_discard();
+  }
+  return rc;
+}
+// The part of a delta after its checks: any failure in it, a CUDA error or a host exception (an allocation the table
+// size makes fail), leaves host bookkeeping and device tables that may disagree, so the ask table is dropped
+extern "C++" {   // a template: C++ linkage inside the C block
+template <class Body> static int ask_delta(pm_engine* e, Body&& body) {
+  int rc;
+  try {
+    rc = body();
+  } catch (...) {
+    rc = pm_guard_rc();
+    e->err = "ask table delta: host exception (the ask table was dropped)";
+  }
+  return ask_delta_failed(e, rc);
+}
+}
+
+int pm_update_asks(pm_engine* e, const uint32_t* idx, const pm_ask* asks, uint32_t n, const pm_gpu_opt* opts,
+                   uint32_t n_opts) try {
+  if (!e) return PM_E_INVALID;
+  std::lock_guard<std::mutex> lk(e->mu);
+  if (!e->have_asks) return e->fail(PM_E_STATE, "pm_update_asks: no ask table");
+  if ((n && (!idx || !asks)) || (n_opts && !opts)) return e->fail(PM_E_INVALID, "pm_update_asks: null");
+  std::vector<uint32_t> uidx;
+  std::vector<pm_ask> urows;
+  {
+    std::string err;
+    const int rc = check_ask_rows(e, "pm_update_asks", idx, asks, n, n_opts, &uidx, &urows, &err);
+    if (rc != PM_OK) return e->fail((pm_status)rc, err);
+  }
+  if (n == 0) return PM_OK;
+  ++e->table_version;
+  return ask_delta(e, [&]() -> int {
+    PM_CUDA(cudaSetDevice(e->device));
+    for (uint32_t t : uidx) {   // a replaced row counts as disabled and enabled again (split_toggles)
+      if (e->eval_valid) e->repl_mark[t] = 1;
+      e->mark_toggled(t);
+      e->auc_mark_ask(t);
+    }
+    return commit_asks(e, e->n_asks, uidx.data(), urows.data(), (uint32_t)uidx.size(), opts);
+  });
+} catch (...) { return pm_guard_rc(); }
+
+int pm_resize_asks(pm_engine* e, uint32_t n_asks, const pm_ask* added, const pm_gpu_opt* opts, uint32_t n_opts) try {
+  if (!e) return PM_E_INVALID;
+  std::lock_guard<std::mutex> lk(e->mu);
+  if (!e->have_asks) return e->fail(PM_E_STATE, "pm_resize_asks: no ask table");
+  if (n_asks >= (1u << 30)) return e->fail(PM_E_INVALID, "pm_resize_asks: too many asks");
+  const uint32_t old = e->n_asks;
+  const uint32_t n_add = n_asks > old ? n_asks - old : 0u;
+  if ((n_add && !added) || (n_opts && !opts)) return e->fail(PM_E_INVALID, "pm_resize_asks: null");
+  std::vector<uint32_t> uidx;
+  std::vector<pm_ask> urows;
+  {
+    std::string err;
+    const int rc = check_ask_rows(e, "pm_resize_asks", nullptr, added, n_add, n_opts, &uidx, &urows, &err);
+    if (rc != PM_OK) return e->fail((pm_status)rc, err);
+  }
+  if (n_asks == old) return PM_OK;
+  ++e->table_version;
+  return ask_delta(e, [&]() -> int {
+    PM_CUDA(cudaSetDevice(e->device));
+    auto drop_from = [&](std::vector<uint32_t>* list) {
+      list->erase(std::remove_if(list->begin(), list->end(), [&](uint32_t t) { return t >= n_asks; }), list->end());
+    };
+    auto cut = [&](auto* v) { if (v->size() > n_asks) v->resize(n_asks); };
+    if (n_asks < old) {
+      // a worker whose stored first ask was removed had no feasible ask before it: it has none now
+      if (e->eval_valid && e->n_workers) {
+        pm::pm_drop_first_asks<<<std::min(blocks_for(e->n_workers, 256), 8u * e->sms), 256, 0, e->stream>>>(e->eval_first.p, e->n_workers,
+                                                                                                            n_asks);
+        const cudaError_t ce = cudaGetLastError();
+        if (ce != cudaSuccess) return e->fail(PM_E_CUDA, std::string("launch pm_drop_first_asks: ") + cudaGetErrorString(ce));
+      }
+      drop_from(&e->toggled);
+      // the kept rows held by a removed ask become unowned at their stored prices; they count against the cutoff
+      if (e->auc_state && e->auc_kept) {
+        cudaError_t ce = cudaMemsetAsync(e->counters.p + 17, 0, 4, e->stream);
+        if (ce == cudaSuccess) {
+          pm::pm_auction_drop_asks<<<std::min(blocks_for(e->auc_kept, 256), 8u * e->sms), 256, 0, e->stream>>>(e->auc_owner.p, e->auc_kept,
+                                                                                                               n_asks, e->counters.p + 17);
+          ce = cudaGetLastError();
+        }
+        if (ce == cudaSuccess) ce = cudaMemcpyAsync(e->h_scalars.p + 17, e->counters.p + 17, 4, cudaMemcpyDeviceToHost, e->stream);
+        if (ce == cudaSuccess) ce = cudaStreamSynchronize(e->stream);
+        if (ce != cudaSuccess) return e->fail(PM_E_CUDA, std::string("pm_resize_asks: ") + cudaGetErrorString(ce));
+        e->auc_removed_held += e->h_scalars.p[17];
+      }
+      drop_from(&e->auc_toggled);
+      cut(&e->auc_ask_mark); cut(&e->auc_cap_stored); cut(&e->auc_floor_stored);
+      cut(&e->ask_on); cut(&e->eval_on); cut(&e->toggle_mark); cut(&e->repl_mark); cut(&e->cap_host); cut(&e->floor_host);
+    } else {
+      // appended rows: enabled, cap 0, floor 0, in E (eval_on 0) and in A0 (no stored cap or floor), holding nothing
+      e->ask_on.resize(n_asks, 1);
+      e->eval_on.resize(n_asks, 0);
+      e->toggle_mark.resize(n_asks, 0);
+      e->repl_mark.resize(n_asks, 0);
+      for (uint32_t t = old; t < n_asks; ++t) e->mark_toggled(t);
+      auto zero_tail = [&](auto& buf, int byte) -> cudaError_t {
+        cudaError_t ce = buf.grow_keep(n_asks, old, e->stream);
+        if (ce == cudaSuccess) ce = cudaMemsetAsync(buf.p + old, byte, (size_t)(n_asks - old) * sizeof(*buf.p), e->stream);
+        return ce;
+      };
+      cudaError_t ce = cudaSuccess;
+      if (e->have_caps) {
+        e->cap_host.resize(n_asks, 0u);
+        ce = zero_tail(e->price_cap, 0);
+      }
+      if (ce == cudaSuccess && e->have_min_rep) {
+        e->floor_host.resize(n_asks, 0u);
+        ce = zero_tail(e->ask_min_rep, 0);
+      }
+      if (ce == cudaSuccess && e->auc_state) {
+        ce = zero_tail(e->auc_assigned, 0xFF);
+        e->auc_ask_mark.resize(n_asks, 0);
+        e->auc_cap_stored.resize(n_asks, 0u);
+        e->auc_floor_stored.resize(n_asks, 0u);
+        for (uint32_t t = old; t < n_asks; ++t) e->auc_mark_ask(t);
+      }
+      if (ce != cudaSuccess) return e->fail(PM_E_CUDA, std::string("pm_resize_asks: ") + cudaGetErrorString(ce));
+    }
+    if (e->auc_state) e->auc_asks_resized = true;
+    return commit_asks(e, n_asks, uidx.data(), urows.data(), (uint32_t)uidx.size(), opts);
+  });
 } catch (...) { return pm_guard_rc(); }
 
 int pm_set_model_table(pm_engine* e, const uint32_t* bits, uint32_t n_patterns, uint32_t n_models,
@@ -1917,7 +2246,7 @@ static int auction_pass(pm_engine* e, bool want_warm, bool want_repair, bool rev
       if (e->cap_host[t] != e->auc_cap_stored[t] || fl != e->auc_floor_stored[t] || e->auc_ask_mark[t]) changed.push_back(t);
     }
     n_kept = std::min(e->auc_kept, W);
-    warm = (uint64_t)changed.size() + (W - n_kept) <= e->tune_incr;
+    warm = (uint64_t)changed.size() + (W - n_kept) + e->auc_removed_held <= e->tune_incr;
   }
   const uint32_t n_rows = warm ? (uint32_t)e->auc_rows.size() : 0u, n_chg = warm ? (uint32_t)changed.size() - n_rows : 0u;
   const bool repair = want_repair && warm;   // PM_AUCTION_REPAIR: the same warm start, repaired by raising instead of releasing
@@ -2356,6 +2685,7 @@ int pm_auction_certificate(pm_engine* e, pm_auction_cert* out, int64_t* ask_boun
   if (!e->auc_state) return e->fail(PM_E_STATE, "pm_auction_certificate: no auction pass since the engine's tables were last replaced");
   const uint32_t W = e->n_workers, T = e->n_asks;
   if (W != e->auc_state_w) return e->fail(PM_E_STATE, "pm_auction_certificate: the worker table was resized since the last auction pass");
+  if (e->auc_asks_resized) return e->fail(PM_E_STATE, "pm_auction_certificate: the ask table was resized since the last auction pass");
   if (e->max_pattern_row > e->n_patterns || (e->max_pattern_row && !e->have_bits))
     return e->fail(PM_E_STATE, "pm_auction_certificate: an ask references a model pattern missing from the model table");
   if (e->n_off) return e->fail(PM_E_UNSUPPORTED, "pm_auction_certificate: disabled asks");
@@ -2861,6 +3191,35 @@ int pm_multi_set_ask_enabled(pm_multi* m, const uint32_t* idx, const uint8_t* en
       if (idx[i] >= e0->n_asks) { m->err = "pm_set_ask_enabled: ask index out of range"; return PM_E_INVALID; }
   }
   PM_MULTI_EACH(pm_set_ask_enabled(e, idx, enabled, n));
+} catch (...) { return pm_guard_rc(); }
+// the ask-table deltas on every device; a call the checks refuse is refused before any device changes
+int pm_multi_update_asks(pm_multi* m, const uint32_t* idx, const pm_ask* asks, uint32_t n, const pm_gpu_opt* opts,
+                         uint32_t n_opts) try {
+  if (m && !m->engines.empty()) {
+    pm_engine* e0 = m->engines[0];
+    std::lock_guard<std::mutex> lk(e0->mu);
+    if (e0->have_asks && !((n && (!idx || !asks)) || (n_opts && !opts))) {
+      std::vector<uint32_t> uidx;
+      std::vector<pm_ask> urows;
+      const int rc = check_ask_rows(e0, "pm_update_asks", idx, asks, n, n_opts, &uidx, &urows, &m->err);
+      if (rc != PM_OK) return rc;
+    }
+  }
+  PM_MULTI_EACH(pm_update_asks(e, idx, asks, n, opts, n_opts));
+} catch (...) { return pm_guard_rc(); }
+int pm_multi_resize_asks(pm_multi* m, uint32_t n_asks, const pm_ask* added, const pm_gpu_opt* opts, uint32_t n_opts) try {
+  if (m && !m->engines.empty()) {
+    pm_engine* e0 = m->engines[0];
+    std::lock_guard<std::mutex> lk(e0->mu);
+    const uint32_t n_add = n_asks > e0->n_asks ? n_asks - e0->n_asks : 0u;
+    if (e0->have_asks && n_asks < (1u << 30) && !((n_add && !added) || (n_opts && !opts))) {
+      std::vector<uint32_t> uidx;
+      std::vector<pm_ask> urows;
+      const int rc = check_ask_rows(e0, "pm_resize_asks", nullptr, added, n_add, n_opts, &uidx, &urows, &m->err);
+      if (rc != PM_OK) return rc;
+    }
+  }
+  PM_MULTI_EACH(pm_resize_asks(e, n_asks, added, opts, n_opts));
 } catch (...) { return pm_guard_rc(); }
 int pm_multi_set_model_table(pm_multi* m, const uint32_t* bits, uint32_t n_patterns, uint32_t n_models, uint32_t words) try {
   PM_MULTI_EACH(pm_set_model_table(e, bits, n_patterns, n_models, words));

@@ -1079,9 +1079,27 @@ __global__ void pm_ask_toggle(const pm_ask* __restrict__ asks, const pm_gpu_opt*
   convert_ask(v >> 1, (v & 1u) == 0u, sizes, false, asks, opts, new_off, o, nullptr, nullptr);
 }
 
-// An incremental pass after configurations were disabled: the workers of the range [w0, w0 + nw) whose stored first
-// ask is one of them (`dis`, increasing, nd entries).  Each is appended to out[] with the ask after its stored one as
-// its walk's start bound, and its stored entry is reset.  One thread per worker, one atomic per warp.
+// pm_update_asks / pm_resize_asks: the caller's rows scattered into the resident raw table (idx distinct, each < n_asks)
+__global__ void pm_scatter_asks(pm_ask* __restrict__ asks, const uint32_t* __restrict__ idx, const pm_ask* __restrict__ rows,
+                                uint32_t n) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) asks[idx[i]] = rows[i];
+}
+
+// pm_resize_asks shrank the table under a stored evaluation: a worker whose stored first ask was removed had no feasible
+// ask before it, so it has none now (until the asks enabled since meet it in the E-pass)
+__global__ void pm_drop_first_asks(uint32_t* __restrict__ eval_first, uint32_t n, uint32_t n_asks) {
+  for (uint32_t w = blockIdx.x * blockDim.x + threadIdx.x; w < n; w += gridDim.x * blockDim.x) {
+    const uint32_t f = eval_first[w];
+    if (f != kNone && f >= n_asks) eval_first[w] = kNone;
+  }
+}
+
+// An incremental pass after configurations were disabled or replaced: the workers of the range [w0, w0 + nw) whose
+// stored first ask is one of them (`dis`, entries ask << 1 | replaced, increasing, nd entries).  Each is appended to
+// out[] with its walk's start bound — the ask after its stored one, or the stored one itself when that row was
+// replaced (the new row may still accept it) — and its stored entry is reset.  One thread per worker, one atomic per
+// warp.
 __global__ void pm_collect_orphans(uint32_t* __restrict__ eval_first, uint32_t w0, uint32_t nw, const uint32_t* __restrict__ dis,
                                    uint32_t nd, uint32_t* __restrict__ out, uint32_t* __restrict__ starts,
                                    uint32_t* __restrict__ count) {
@@ -1089,13 +1107,15 @@ __global__ void pm_collect_orphans(uint32_t* __restrict__ eval_first, uint32_t w
   const uint32_t w = w0 + i;
   const uint32_t f = i < nw ? eval_first[w] : kNone;
   bool hit = false;
+  uint32_t d = 0;
   if (f != kNone) {
     uint32_t lo = 0, hi = nd;
     while (lo < hi) {
       const uint32_t mid = (lo + hi) >> 1;
-      if (__ldg(dis + mid) < f) lo = mid + 1; else hi = mid;
+      if ((__ldg(dis + mid) >> 1) < f) lo = mid + 1; else hi = mid;
     }
-    hit = lo < nd && __ldg(dis + lo) == f;
+    if (lo < nd) d = __ldg(dis + lo);
+    hit = lo < nd && (d >> 1) == f;
   }
   const uint32_t lane = threadIdx.x & 31u;
   const uint32_t b = __ballot_sync(0xffffffffu, hit);
@@ -1106,7 +1126,7 @@ __global__ void pm_collect_orphans(uint32_t* __restrict__ eval_first, uint32_t w
   if (hit) {
     const uint32_t pos = base + (uint32_t)__popc(b & ((1u << lane) - 1u));
     out[pos] = w;
-    starts[pos] = f + 1;
+    starts[pos] = f + 1u - (d & 1u);
     eval_first[w] = kNone;
   }
 }

@@ -154,6 +154,20 @@ class Engine:
         idx, en = _ask_enabled_args(idx, enabled)
         self._check(self._lib.pm_set_ask_enabled(self._h, _ptr(idx), _ptr(en), len(idx)))
 
+    def update_asks(self, idx, asks: np.ndarray, opts: np.ndarray | None = None):
+        """Replace the ask rows idx (pm_update_asks); asks["opt_off"] / ["n_opts"] index `opts`.  A replaced row keeps
+        its enabled flag, price cap and reputation floor; the stored evaluation and auction state are kept."""
+        idx, asks, opts = _ask_delta_args(idx, asks, opts)
+        self._check(self._lib.pm_update_asks(self._h, _ptr(idx), _ptr(asks), len(idx), _ptr(opts), len(opts)))
+
+    def resize_asks(self, n: int, added: np.ndarray | None = None, opts: np.ndarray | None = None):
+        """Shrink the ask table to its first n rows, or append rows `added` (options in `opts`) at the lowest
+        priorities, enabled, with cap 0 and floor 0 (pm_resize_asks)."""
+        added = np.ascontiguousarray(np.zeros(0, dtype=abi.ASK) if added is None else added, dtype=abi.ASK)
+        opts = np.ascontiguousarray(np.zeros(0, dtype=abi.GPU_OPT) if opts is None else opts, dtype=abi.GPU_OPT)
+        self._check(self._lib.pm_resize_asks(self._h, n, _ptr(added) if len(added) else None, _ptr(opts), len(opts)))
+        self.n_asks = n
+
     def set_model_table(self, bits: np.ndarray, n_patterns: int, n_models: int, words: int):
         bits = np.ascontiguousarray(bits, dtype=np.uint32)
         self._check(self._lib.pm_set_model_table(self._h, _ptr(bits), n_patterns, n_models, words))
@@ -317,6 +331,14 @@ def _ask_enabled_args(idx, enabled):
     return idx, np.ascontiguousarray(en, dtype=np.uint8)
 
 
+def _ask_delta_args(idx, asks, opts):
+    """(idx, asks, opts) as pm_update_asks takes them; opts None = no option rows."""
+    idx = np.ascontiguousarray(np.atleast_1d(idx), dtype=np.uint32)
+    asks = np.ascontiguousarray(np.atleast_1d(asks), dtype=abi.ASK)
+    opts = np.ascontiguousarray(np.zeros(0, dtype=abi.GPU_OPT) if opts is None else opts, dtype=abi.GPU_OPT)
+    return idx, asks, opts
+
+
 def _result_views(r: "abi.PmResult", copy: bool) -> MatchResult:
     def view(ptr, n, dt):
         if n == 0:
@@ -402,6 +424,17 @@ class MultiEngine:
     def set_ask_enabled(self, idx, enabled):
         idx, en = _ask_enabled_args(idx, enabled)
         self._check(self._lib.pm_multi_set_ask_enabled(self._h, _ptr(idx), _ptr(en), len(idx)))
+
+    def update_asks(self, idx, asks, opts=None):
+        """pm_multi_update_asks: Engine.update_asks on every device."""
+        idx, asks, opts = _ask_delta_args(idx, asks, opts)
+        self._check(self._lib.pm_multi_update_asks(self._h, _ptr(idx), _ptr(asks), len(idx), _ptr(opts), len(opts)))
+
+    def resize_asks(self, n: int, added=None, opts=None):
+        """pm_multi_resize_asks: Engine.resize_asks on every device."""
+        added = np.ascontiguousarray(np.zeros(0, dtype=abi.ASK) if added is None else added, dtype=abi.ASK)
+        opts = np.ascontiguousarray(np.zeros(0, dtype=abi.GPU_OPT) if opts is None else opts, dtype=abi.GPU_OPT)
+        self._check(self._lib.pm_multi_resize_asks(self._h, n, _ptr(added) if len(added) else None, _ptr(opts), len(opts)))
 
     def set_model_table(self, bits, n_patterns, n_models, words):
         bits = np.ascontiguousarray(bits, dtype=np.uint32)

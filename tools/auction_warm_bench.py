@@ -12,7 +12,12 @@ The card's name and power limit are read in the same run.  One JSON line per pas
 changed rows raised, reverse rounds at the end) and a cold pass, alternately, each warm or repair pass after a cold pass
 of the current tables and a fresh draw of the same kind and number of changes.  Per pass also: reverse rounds and bids.
 
-    python tools/auction_warm_bench.py [--repair] [--out results/auction_warm.json]
+--asks: ask-table change sets instead (pm_update_asks / pm_resize_asks): append 1, 100 and 1 000 asks, replace 100,
+remove the last 100 asks (most of them hold a worker).  Each runs as a warm pass, a warm repair and a cold pass on the
+same tables, alternately, each warm or repair pass after a cold pass of the tables before the change; and as
+pm_set_asks + a cold pass, the one way to take such a change without the deltas.
+
+    python tools/auction_warm_bench.py [--repair | --asks] [--out results/auction_warm.json]
 """
 from __future__ import annotations
 
@@ -70,11 +75,60 @@ def assigned_of(eng, T):
     return got
 
 
+def ask_series(eng, a, cap, record):
+    """--asks: the change sets of the task-arrival loop, each as warm, repair, cold and pm_set_asks + cold."""
+    rng = np.random.default_rng(3)
+    asks, cap = a.asks.copy(), cap.copy()
+    opts = a.opts   # every table below indexes these option rows (pm_set_asks gets them whole)
+
+    def draw(n):
+        """n new rows, copies of the instance's rows (their patterns are in the model table), with only their own
+        option rows, as a caller sends a new task's."""
+        src = a.asks[rng.integers(0, len(a.asks), n)]
+        rows = src.copy()
+        rows["opt_off"] = np.concatenate([[0], np.cumsum(src["n_opts"])[:-1]]).astype(np.uint32)
+        own = np.concatenate([a.opts[o:o + k] for o, k in zip(src["opt_off"], src["n_opts"])] or [a.opts[:0]])
+        return src, rows, own
+
+    warm = abi.PM_MODE_AUCTION | abi.PM_AUCTION_WARM
+    modes = [("warm", warm), ("repair", warm | abi.PM_AUCTION_REPAIR)]
+    for case, n in (("append", 1), ("append", 100), ("append", 1000), ("replace", 100), ("remove", 100)):
+        for name, mode in modes:
+            eng.match(abi.PM_MODE_AUCTION)             # the stored state: a cold pass of the current tables
+            T = len(asks)
+            t0 = time.perf_counter()
+            if case == "append":
+                src, rows, own = draw(n)
+                eng.resize_asks(T + n, rows, own)
+                asks = np.concatenate([asks, src])
+                cap = np.concatenate([cap, rng.integers(20, 3000, n).astype(np.uint32)])
+                eng.set_price_caps(cap)
+            elif case == "replace":
+                idx = np.sort(rng.choice(T, n, replace=False)).astype(np.uint32)
+                src, rows, own = draw(n)
+                eng.update_asks(idx, rows, own)
+                asks[idx] = src
+            else:
+                eng.resize_asks(T - n)
+                asks, cap = asks[:T - n].copy(), cap[:T - n].copy()
+            eng.sync()
+            call_ms = round((time.perf_counter() - t0) * 1e3, 2)
+            record(f"{name}_{case}", n, dict(timed(eng, mode), call_ms=call_ms))
+            record(f"cold_{case}", n, timed(eng, abi.PM_MODE_AUCTION))
+        t0 = time.perf_counter()                       # today's only option: the whole table again, then a cold pass
+        eng.set_asks(asks, opts)
+        eng.set_price_caps(cap)
+        r = timed(eng, abi.PM_MODE_AUCTION)
+        r["wall_ms"] = round((time.perf_counter() - t0) * 1e3, 2)
+        record(f"set_asks_cold_{case}", n, r)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", default=None)
     ap.add_argument("--counts", default="0,10,1000,100000")
     ap.add_argument("--repair", action="store_true", help="also run PM_AUCTION_REPAIR on every change set")
+    ap.add_argument("--asks", action="store_true", help="ask-table change sets (pm_update_asks / pm_resize_asks)")
     args = ap.parse_args()
     gpu = card()
     print(f"card: {gpu}", file=sys.stderr)
@@ -91,6 +145,16 @@ def main():
         r = dict(case=case, n=n, **r, card=gpu)
         rows.append(r)
         print(json.dumps(r), flush=True)
+
+    if args.asks:
+        record("cold", 0, timed(eng, abi.PM_MODE_AUCTION))
+        ask_series(eng, a, cap, record)
+        eng.close()
+        if args.out:
+            os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
+            with open(args.out, "w") as f:
+                json.dump(dict(card=gpu, rows=rows), f, indent=1)
+        return
 
     modes = [("warm", abi.PM_MODE_AUCTION | abi.PM_AUCTION_WARM)]
     if args.repair:

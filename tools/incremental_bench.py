@@ -310,10 +310,19 @@ def main():
     ap.add_argument("--toggle", action="store_true", help="configurations toggled between passes instead of rows written")
     ap.add_argument("--shards", type=int, default=0, help="N shard engines on device 0 (pm_match_local + host merge)")
     ap.add_argument("--multi", action="store_true", help="pm_multi over every visible GPU")
+    ap.add_argument("--ask-updates", dest="ask_updates", action="store_true",
+                    help="asks replaced between passes (pm_update_asks) instead of rows written; also times the call")
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
 
     w = synth.make_workers(args.workers)
+    if args.ask_updates:
+        a = synth.make_asks(args.asks, "mixed")
+        bits, npat, nmod, words = synth.intern_tables(w, a)
+        env = card()
+        rows, checked, workload = ask_update_series(args, w, a, bits, npat, nmod, words)
+        report(rows, checked, workload, env, "u", args.out, "incremental_ask_update_bench.json")
+        return
     if args.shards or args.multi:
         a = synth.make_asks(args.asks, "mixed")
         bits, npat, nmod, words = synth.intern_tables(w, a)
@@ -381,7 +390,74 @@ def main():
            "incremental_bench.json")
 
 
+U = (1, 100, 1_000)
+
+
+def own_options(src, opts):
+    """Rows `src` (opt_off into `opts`) with only their own option rows, as a caller sends changed asks."""
+    rows = src.copy()
+    rows["opt_off"] = np.concatenate([[0], np.cumsum(src["n_opts"])[:-1]]).astype(np.uint32)
+    own = np.concatenate([opts[o:o + k] for o, k in zip(src["opt_off"], src["n_opts"])] or [opts[:0]])
+    return rows, own
+
+
+def ask_update_series(args, w, a, bits, npat, nmod, words):
+    """U asks replaced by other rows of the table (pm_update_asks) between passes: the incremental pass against the full
+    one, the result checked equal once per U; then pm_update_asks itself (U rows, host clock around the call and a
+    synchronise) at T = the table's asks and at T = 1M."""
+    os.environ["PM_TUNE_INCR"] = str(1 << 31)   # read at pm_create: never fall back, so the crossover shows
+    inc = Engine(timing=True)
+    del os.environ["PM_TUNE_INCR"]
+    ref = Engine(timing=True)
+    engines = (inc, ref)
+    for e in engines:
+        e.set_asks(a.asks, a.opts)
+        e.set_model_table(bits, npat, nmod, words)
+        e.set_workers(w.a, w.b)
+        e.match(LEAN)
+    W, T = len(w), len(a)
+    rng = np.random.default_rng(2026)
+    rows = {"full": []}
+    rows.update({u: [] for u in U})
+    checked = set()
+    for rnd in range(args.rounds):
+        for u in U:
+            rows["full"].append(timed(inc, LEAN))
+            idx = np.sort(rng.choice(T, u, replace=False)).astype(np.uint32)
+            new, own = own_options(a.asks[rng.integers(0, T, u)], a.opts)
+            for e in engines:
+                e.update_asks(idx, new, own)
+            rows[u].append(timed(inc, INCR))
+            if u not in checked:
+                _, same = same_as_full(inc, ref)
+                if not same:
+                    raise SystemExit(f"u={u}: the incremental result differs from the full pass")
+                checked.add(u)
+    for e in engines:
+        e.close()
+    calls = []
+    for n_asks in (T, 1_000_000):
+        big = a if n_asks == T else synth.make_asks(n_asks, "mixed")
+        e = Engine(timing=True)
+        e.set_asks(big.asks, big.opts)
+        for u in U:
+            ms = []
+            for _ in range(5):
+                idx = np.sort(rng.choice(n_asks, u, replace=False)).astype(np.uint32)
+                new, own = own_options(big.asks[rng.integers(0, n_asks, u)], big.opts)
+                t = time.perf_counter()
+                e.update_asks(idx, new, own)
+                e.sync()
+                ms.append((time.perf_counter() - t) * 1e3)
+            calls.append({"n_asks": n_asks, "u": u, "ms_update_asks_median": float(np.median(ms))})
+            print(json.dumps(calls[-1]))
+        e.close()
+    rows["update_asks_calls"] = calls
+    return rows, checked, f"{T} asks x {W} workers (synth mixed), first fit, fused lean; u asks replaced per pass"
+
+
 def report(rows, checked, workload, env, key_name, out_dir, file_name):
+    extra = rows.pop("update_asks_calls", None)
     summary = []
     for key, rs in rows.items():
         summary.append({key_name: key, "ms_device_median": float(np.median([r["ms_device"] for r in rs])),
@@ -389,6 +465,8 @@ def report(rows, checked, workload, env, key_name, out_dir, file_name):
                         "evals": int(rs[-1]["evals"]), "n_tiles": int(rs[-1]["n_tiles"]), "runs": len(rs),
                         **{k: rs[-1][k] for k in ("n_off", "n_on") if k in rs[-1]}})
     out = {"workload": workload, "card": env, "checked_equal_to_full_pass": sorted(checked), "rows": summary}
+    if extra is not None:
+        out["update_asks_calls"] = extra
     print(f"{env.get('name')}  power limit {env.get('power_limit_w')} W  SM {env.get('sm_mhz')}/{env.get('sm_max_mhz')} MHz")
     print(f"{key_name:>8} {'device ms':>10} {'host ms':>9} {'evals':>16} {'n_tiles':>9}")
     for s in summary:
