@@ -374,7 +374,10 @@ enum pm_path {
  * pass's is; it need not equal the cold pass's result.  The warm pass runs when a stored state exists and
  * |R0| + |A0| <= the PM_TUNE_INCR cutoff, else the pass is cold.  pm_set_asks, pm_set_model_table,
  * pm_set_worker_count, pm_set_auction_params, pm_set_shard, pm_attach_comm and a failed auction pass discard the
- * stored state; reference-mode passes leave it alone.  pm_update_asks and pm_resize_asks keep it: A0 also holds every
+ * stored state; reference-mode passes leave it alone.  An auction pass refused before it runs keeps it: disabled asks
+ * (PM_E_UNSUPPORTED), tables outside the integer domain (PM_E_INVALID), and an ask, enabled or not, referencing a
+ * model pattern missing from the model table (PM_E_STATE; any pattern_id >= n_patterns, 0xFFFFFFFF included); so does
+ * a certificate refused for any reason.  pm_update_asks and pm_resize_asks keep it: A0 also holds every
  * replaced ask and every appended ask (which has no stored cap or floor), and step 1 also releases the holder of every
  * removed ask (a shrink of pm_resize_asks): that worker becomes unowned at its stored price as the shrink runs, joins
  * R at price 0 here when its price was positive, and is not counted in n_released (its ask no longer exists).  The

@@ -1013,7 +1013,9 @@ __device__ __forceinline__ void convert_ask(uint32_t t, bool off, bool sizes, bo
     if (q.present & PM_O_MODEL) {
       x.need |= PM_W_HAS_GPU_MODEL;
       x.pattern_row = q.pattern_id + 1;
-      mrow = max(mrow, x.pattern_row);
+      // pattern_id 0xFFFFFFFF wraps to row 0 ("no model clause"): count it as the largest row, so that the table is
+      // refused (PM_E_STATE) as for any pattern past the model table
+      mrow = max(mrow, q.pattern_id == 0xFFFFFFFFu ? 0xFFFFFFFFu : x.pattern_row);
     }
     dopts[d.opt_off + o] = x;
     DevOptF f;

@@ -1,20 +1,28 @@
 """Long random histories of one engine: every table call, every pass kind and the auction certificate, and a host
 mirror that says what each call must do.
 
-`History` extends the warm checker's `Market` (worker rows, caps, floors, reputation, resizes and the auction's change
-set) with what the reference modes read (locations, address ranks, the ask table with its group sizes, the model table,
-the enabled mask) and with the two change trackers of prime_match.h, restated from the header and DESIGN §4-§6b:
+`History` extends the delta tests' `AskMarket` (worker rows, caps, floors, reputation, resizes, the ask rows as
+pm_update_asks / pm_resize_asks change them and the auction's change set) with what the reference modes read
+(locations, address ranks, the model table, the enabled mask) and with the two change trackers of prime_match.h,
+restated from the header and DESIGN §4-§6b:
 
   reference tracker (PM_INCREMENTAL): a stored evaluation exists after every successful reference-mode pass; rows
       written since through pm_update_workers / pm_set_flags / pm_upsert_workers (each once) and rows a grow adds are
       dirty; a shrink drops the dirty rows it cuts off; asks enabled / disabled since count against the stored mask
-      (off and on again counts as neither); the next incremental pass walks the dirty rows and the orphans of the asks
-      disabled since, or everything when there is no stored evaluation or the count passes the PM_TUNE_INCR cutoff.
-      pm_set_asks, pm_set_model_table, pm_set_worker_count and a reference-mode pass that fails discard it; a call
-      refused on its mode bits and every auction-mode pass, refused or not, leave it as it is.
-  auction tracker (PM_AUCTION_WARM): a stored state exists after every successful auction pass; Market tracks R0 and
-      A0; pm_set_asks, pm_set_model_table, pm_set_worker_count and pm_set_auction_params discard it; a refused auction
-      pass keeps it; reference-mode passes and certificates leave it alone.
+      (off and on again counts as neither); a replaced ask is in E when enabled now and in D when enabled at the stored
+      evaluation; appended asks were not enabled at it; an ask shrink cuts the mask and sets every stored first ask past
+      the new end to NONE (those workers are no orphans).  The next incremental pass walks the dirty rows and the
+      orphans of D, or everything when there is no stored evaluation or the dirty rows plus ceil(|E| W / T) pass the
+      PM_TUNE_INCR cutoff.  pm_set_asks, pm_set_model_table, pm_set_worker_count and a reference-mode pass that fails
+      discard it; a call refused on its mode bits and every auction-mode pass, refused or not, leave it as it is.
+  auction tracker (PM_AUCTION_WARM): a stored state exists after every successful auction pass; AskMarket tracks R0,
+      A0 (toggled, replaced and appended asks) and the removed asks that held a worker; any ask resize since marks it
+      resized (the certificate waits for the next pass); pm_set_asks, pm_set_model_table, pm_set_worker_count and
+      pm_set_auction_params discard it; a refused auction pass keeps it; reference-mode passes and certificates leave
+      it alone.
+
+Ask rows referencing a model pattern the model table lacks make every pass, auction pass, certificate and cost tile
+return PM_E_STATE while they are in the table, enabled or not.
 
 `generate` draws the seeded histories the GPU suite runs (tests/test_gpu_engine_history.py) and the CPU suite audits
 (tests/test_engine_history_inputs.py).  Events are plain data, so a failing history can be replayed and shortened
@@ -30,6 +38,7 @@ import numpy as np
 import auction_warm_checker as wc
 from oracle import pm_oracle as orc
 from protocol_b200 import abi, synth
+from test_ask_deltas_formulation import AskMarket, own_options
 
 NONE = abi.PM_NONE
 INF = abi.PM_COST_INF
@@ -48,10 +57,16 @@ INCREMENTAL = ("lean_incr", "proximity_incr")
 AUCTION = ("auction", "reverse", "warm", "repair")
 PASSES = REFERENCE + AUCTION + ("certificate",)
 CALLS = ("update", "set_flags", "upsert", "grow", "shrink", "reputation", "caps", "floors", "ask_off", "ask_on",
-         "locations", "addr_rank", "set_asks", "model_table", "auction_params", "set_workers")
-RARE = ("set_asks", "model_table", "auction_params", "set_workers")
+         "locations", "addr_rank", "set_asks", "model_table", "auction_params", "set_workers", "update_asks",
+         "append_asks", "shrink_asks", "ask_delta_refused")
+RARE = ("set_asks", "model_table", "auction_params", "set_workers", "ask_delta_refused")
+ASK_DELTAS = ("update_asks", "append_asks", "shrink_asks")
 REFUSALS = ("auction_disabled", "auction_domain", "auction_incremental", "proximity_max0", "certificate_no_state",
-            "certificate_resized", "certificate_disabled")
+            "certificate_resized", "certificate_disabled", "certificate_asks_resized", "pattern_missing",
+            "ask_delta_refused")
+# the PM_E_INVALID cases of pm_update_asks / pm_resize_asks (each changes nothing, pm_table_version included)
+DELTA_REFUSALS = ("index", "sizes", "range", "grow_without_rows", "grow_bad_range", "too_many")
+EDGE_ASKS = ("max0", "min0", "no_opts", "big_cpu", "none", "missing")
 GROUPS = [(1, 1), (2, 3), (3, 5), (4, 4), (2, 8)]
 PARAMS = [(1, 1, 4), (1, 64, 4), (3, 1, 4)]
 # (P + K + 2) * 2 + E < 2^61 holds for every ordinary price and for 0x7FFFFFFF / 0x80000000, not for 0xFFFFFFFE up
@@ -105,6 +120,65 @@ def in_domain(wb, cap, params):
     return (P + K + 2) * max(S, 1) + max(E, 1) < (1 << 61)
 
 
+def option_rows(asks):
+    """Per ask the option rows pm_ask_convert reads ([opt_off, opt_off + n_opts) when the ask has requirements)."""
+    has = (asks["flags"] & abi.PM_A_HAS_REQ) != 0
+    return [range(int(o), int(o) + int(k)) if h else range(0) for o, k, h in zip(asks["opt_off"], asks["n_opts"], has)]
+
+
+def asks_small(asks, opts):
+    """The fast predicate's operand limits over every ask row, enabled or not (pm_ask_convert's kAskNotSmall)."""
+    f = asks["flags"]
+    has = (f & abi.PM_A_HAS_REQ) != 0
+    cpu = np.where(has & ((f & abi.PM_A_REQ_CPU) != 0) & ((f & abi.PM_A_REQ_CPU_CORES) != 0), asks["cpu_cores"], 0)
+    ram = np.where(has & ((f & abi.PM_A_REQ_RAM) != 0), asks["ram_mb"], 0)
+    sto = np.where(has & ((f & abi.PM_A_REQ_STORAGE) != 0), asks["storage_gb"], 0)
+    if ((cpu | ram | sto) >= SIGN).any():
+        return False
+    rows = np.array(sorted({o for r in option_rows(asks) for o in r}), dtype=np.int64)
+    if len(rows) == 0:
+        return True
+    q = opts[rows]
+    p = q["present"]
+    count = ((p & abi.PM_O_COUNT) != 0) & (q["count"] >= 65536)
+    mem_lo = np.maximum(np.where((p & abi.PM_O_MEM) != 0, q["memory_mb"], 0),
+                        np.where((p & abi.PM_O_MEM_MIN) != 0, q["memory_mb_min"], 0))
+    mem_hi = np.where((p & abi.PM_O_MEM_MAX) != 0, q["memory_mb_max"], 0xFFFFFFFF)
+    mem_lo = np.where(mem_lo > mem_hi, 0, mem_lo)
+    tot_lo = np.where((p & abi.PM_O_TOT_MIN) != 0, q["total_memory_min"], 0)
+    tot_hi = np.where((p & abi.PM_O_TOT_MAX) != 0, q["total_memory_max"], 0xFFFFFFFF)
+    tot_lo = np.where(tot_lo > tot_hi, 0, tot_lo)
+    return not (count | (mem_lo >= SIGN) | (tot_lo >= SIGN)).any()
+
+
+def missing_pattern(asks, opts, n_patterns):
+    """bool[T]: the ask has an option row whose model pattern the model table lacks.  pm_ask_convert stores
+    pattern_id + 1 as a 32-bit pattern row and the engine refuses when the largest row exceeds n_patterns, so a
+    pattern_id >= n_patterns is missing (0xFFFFFFFF included: its row would wrap to 0, "no model clause")."""
+    q = opts["pattern_id"].astype(np.int64)
+    miss = ((opts["present"] & abi.PM_O_MODEL) != 0) & (q >= n_patterns)
+    return np.array([bool(miss[list(r)].any()) if len(r) else False for r in option_rows(asks)], dtype=bool)
+
+
+def split_toggles(mask, eval_mask, replaced):
+    """E and D of the next incremental pass: E = enabled now and (replaced or not enabled at the stored evaluation),
+    D = enabled at the stored evaluation and (replaced or disabled now); a replaced ask's orphans are walked from the
+    ask itself."""
+    rep = np.zeros(len(mask), dtype=bool)
+    rep[sorted(replaced)] = True
+    en = mask & (rep | ~eval_mask)
+    dis = eval_mask & (rep | ~mask)
+    return set(np.flatnonzero(en).tolist()), set(np.flatnonzero(dis).tolist())
+
+
+def walked_rows(stored, dirty, dis):
+    """n_tiles of an incremental pass: the written rows and the orphans (workers whose stored first ask is in D) that
+    are not among them."""
+    orphans = np.isin(stored, sorted(dis)) if dis else np.zeros(len(stored), dtype=bool)
+    orphans[sorted(dirty)] = False
+    return len(dirty) + int(orphans.sum())
+
+
 # ------------------------------------------------------------------------------------------------ the fixed tables
 @functools.lru_cache(maxsize=4)
 def setup(shape):
@@ -142,14 +216,32 @@ def setup(shape):
     wb = w.b.copy()
     wb["ext_ask_price"] = rng.integers(10, 1000, W).astype(np.uint32)
     lat, lon = synth.CITIES[rng.integers(0, len(synth.CITIES), W)].T.copy()
+    # the option table both ask tables index, with two option rows past it whose model patterns the model tables lack:
+    # the first pattern past the table, and 0xFFFFFFFF (whose 32-bit pattern row pattern_id + 1 wraps to 0)
+    miss = np.zeros(2, dtype=abi.GPU_OPT)
+    miss["present"] = abi.PM_O_MODEL
+    miss["pattern_id"] = [npat, 0xFFFFFFFF]
+    opts = np.concatenate([np.ascontiguousarray(opts), miss])
+    # rows a delta sends besides the two tables' rows: a max_group_size 0 ask and a min_group_size 0 ask (copies of z,
+    # which many workers meet), a row without option rows, a cpu_cores threshold >= 2^31 (the generic predicate), a
+    # row no worker meets, and the two rows with a missing pattern
+    edge = np.repeat(asks[z:z + 1], len(EDGE_ASKS) + 1).copy()
+    edge[0]["min_group_size"], edge[0]["max_group_size"] = 0, 0
+    edge[1]["min_group_size"], edge[1]["max_group_size"] = 0, 3
+    edge[2]["n_opts"], edge[2]["min_group_size"], edge[2]["max_group_size"] = 0, 1, 2
+    edge[3] = (abi.PM_A_HAS_REQ | abi.PM_A_REQ_CPU | abi.PM_A_REQ_CPU_CORES, 0, 0, (1 << 31) + 5, 0, 0, 1, 1)
+    edge[4] = (abi.PM_A_HAS_REQ | abi.PM_A_REQ_RAM, 0, 0, 0, 0xFFFFFFFF, 0, 1, 1)
+    edge[5] = (abi.PM_A_HAS_REQ, 1, len(opts) - 2, 0, 0, 0, 1, 1)
+    edge[6] = (abi.PM_A_HAS_REQ, 1, len(opts) - 1, 0, 0, 0, 1, 1)
     return dict(T=T, W=W, z=z, asks=[asks, asks2], opts=opts, bits=[np.asarray(bits, dtype=np.uint32), bits2],
                 npat=npat, nmod=nmod, words=words, wa=w.a.copy(), wb=wb, lat=lat, lon=lon,
                 rank=rng.permutation(W).astype(np.uint32), cap=rng.integers(50, 1500, T).astype(np.uint32),
-                rep=rng.integers(0, 4, W).astype(np.uint32), floors=rng.integers(0, 3, T).astype(np.uint32))
+                rep=rng.integers(0, 4, W).astype(np.uint32), floors=rng.integers(0, 3, T).astype(np.uint32),
+                pool=np.concatenate([asks, asks2]), edge=edge)
 
 
 # ------------------------------------------------------------------------------------------------ the mirror
-class History(wc.Market):
+class History(AskMarket):
     def __init__(self, shape, cutoff=DEFAULT_CUTOFF):
         s = setup(shape)
         self.s, self.cutoff, self.z = s, cutoff, s["z"]
@@ -163,22 +255,32 @@ class History(wc.Market):
         self.eval = False
         self.dirty, self.over = set(), False
         self.eval_mask, self.eval_ff = self.mask.copy(), None
-        self.eval_facts = None              # (workers_small, prices_narrow) at the stored evaluation
-        self.flipped = set()                # which of the two facts changed since the stored evaluation
-        # auction tracker
+        self.replaced = set()               # asks replaced since the stored evaluation
+        self.appended = set()               # asks appended since it
+        self.dropped = 0                    # stored first asks an ask shrink set to NONE since it
+        self.eval_facts = None              # (workers_small, prices_narrow, asks_small) at the stored evaluation
+        self.flipped = set()                # which of the facts changed since the stored evaluation
+        # auction tracker (A0 is AskMarket's `toggled`)
         self.auc_state, self.auc_w, self.auc_over = False, 0, False
-        self.auc_toggled = set()
+        self.resized = False                # an ask resize since the stored state
 
     # ---- facts
     def facts(self):
-        return workers_small(self.wa, self.wb), prices_narrow(self.wb)
+        return workers_small(self.wa, self.wb), prices_narrow(self.wb), asks_small(self.asks, self.opts)
 
     def _note_facts(self):
         if self.eval_facts is not None:
             now = self.facts()
-            for name, a, b in zip(("fast", "narrow"), self.eval_facts, now):
+            for name, a, b in zip(("fast", "narrow", "ask_fast"), self.eval_facts, now):
                 if a != b:
                     self.flipped.add(name)
+
+    def max0_on(self):
+        """The enabled asks with max_group_size == 0 (PM_MODE_PROXIMITY refuses while there is one)."""
+        return np.flatnonzero(self.mask & (self.asks["max_group_size"] == 0))
+
+    def pattern_missing(self):
+        return bool(missing_pattern(self.asks, self.opts, self.s["npat"]).any())
 
     def first_feasible(self):
         up = np.flatnonzero(self.mask).astype(np.uint32)
@@ -197,29 +299,30 @@ class History(wc.Market):
 
     def discard_eval(self):
         self.eval, self.dirty, self.over = False, set(), False
+        self.replaced, self.appended, self.dropped = set(), set(), 0
         self.eval_facts, self.flipped = None, set()
 
     def discard_auction(self):
-        self.auc_state, self.auc_over, self.auc_toggled = False, False, set()
+        self.auc_state, self.auc_over, self.resized = False, False, False
         self.store(None, None)
+
+    def e_rows(self, en):
+        """|E| x W / T rounded up: what the E-pass counts against the cutoff (the current T)."""
+        T = len(self.asks)
+        return -(-len(en) * self.n_workers // T) if T else 0
 
     def incremental_plan(self):
         """(full, n_tiles, enabled since, disabled since, count certain) of the next incremental pass."""
         W, T = self.n_workers, len(self.asks)
         if not self.eval or self.cutoff == 0 or T == 0 or W == 0:
             return True, W, set(), set(), True
-        en = set(np.flatnonzero(self.mask & ~self.eval_mask).tolist())
-        dis = set(np.flatnonzero(~self.mask & self.eval_mask).tolist())
-        e_rows = -(-len(en) * W // T)
-        full_now = len(self.dirty) + e_rows > self.cutoff
+        en, dis = split_toggles(self.mask, self.eval_mask, self.replaced)
+        full_now = len(self.dirty) + self.e_rows(en) > self.cutoff
         full = self.over or full_now
         sure = self.over == (len(self.dirty) > self.cutoff)   # a shrink since the count passed the cutoff: unspecified
         if full:
             return True, W, en, dis, sure
-        ff = self.eval_ff
-        orphans = np.isin(ff, list(dis)) if dis else np.zeros(W, dtype=bool)
-        orphans[list(self.dirty)] = False
-        return False, len(self.dirty) + int(orphans.sum()), en, dis, sure
+        return False, walked_rows(self.eval_ff, self.dirty, dis), en, dis, sure
 
     def warm_plan(self):
         """(warm, certain) of the next PM_AUCTION_WARM pass."""
@@ -228,20 +331,49 @@ class History(wc.Market):
         fits = self.n_changes() <= self.cutoff
         return (fits and not self.auc_over), self.auc_over == (len(self.rows) > self.cutoff)
 
-    def changed_asks(self):
-        d = (self.cap != self.cap0) | (self.floors_or_zero() != self.floors0)
-        return sorted(set(np.flatnonzero(d).tolist()) | self.auc_toggled)
+    # ---- the ask table in place (AskMarket keeps the rows, caps, floors and A0; these keep the rest)
+    def update_asks(self, idx, rows):
+        self.replace(idx, rows)
+        if self.eval:
+            self.replaced |= {int(t) for t in idx}
+        self._note_facts()
+
+    def append_asks(self, rows):
+        k, T = len(rows), len(self.asks)
+        if self.eval:
+            self.appended |= set(range(T, T + k))
+        self.append(rows)
+        self.mask = np.concatenate([self.mask, np.ones(k, dtype=bool)])
+        self.eval_mask = np.concatenate([self.eval_mask, np.zeros(k, dtype=bool)])
+        self.resized |= self.auc_state
+        self._note_facts()
+
+    def shrink_asks(self, n):
+        self.shrink(n)
+        self.mask, self.eval_mask = self.mask[:n].copy(), self.eval_mask[:n].copy()
+        self.replaced = {t for t in self.replaced if t < n}
+        self.appended = {t for t in self.appended if t < n}
+        if self.eval_ff is not None:   # a worker whose stored first ask was removed had no feasible ask before it
+            cut = (self.eval_ff != NONE) & (self.eval_ff >= n)
+            self.dropped += int(cut.sum()) if self.eval else 0
+            self.eval_ff = np.where(cut, NONE, self.eval_ff).astype(np.uint32)
+        self.resized |= self.auc_state
+        self._note_facts()
 
     # ---- predictions of refusals (the set of statuses the header allows)
     def refusal(self, kind):
         """(refusal name, statuses) or (None, None) for a pass or certificate that must run."""
         if kind == "auction_incr":
             return "auction_incremental", {abi.PM_E_INVALID}
+        if kind in REFERENCE and self.pattern_missing():
+            return "pattern_missing", {abi.PM_E_STATE}
         if kind == "proximity" or kind == "proximity_incr":
-            if self.mask[self.z] and self.asks[self.z]["max_group_size"] == 0:
+            if len(self.max0_on()):
                 return "proximity_max0", {abi.PM_E_UNSUPPORTED}
             return None, None
         if kind in AUCTION:
+            if self.pattern_missing():   # refused before the pass: the stored state stays
+                return "pattern_missing", {abi.PM_E_STATE}
             st, why = set(), None
             if not self.mask.all():
                 st.add(abi.PM_E_UNSUPPORTED)
@@ -258,6 +390,12 @@ class History(wc.Market):
             elif self.n_workers != self.auc_w:
                 st.add(abi.PM_E_STATE)
                 why = "certificate_resized"
+            elif self.resized:
+                st.add(abi.PM_E_STATE)
+                why = "certificate_asks_resized"
+            elif self.pattern_missing():
+                st.add(abi.PM_E_STATE)
+                why = "pattern_missing"
             if not self.mask.all():
                 st.add(abi.PM_E_UNSUPPORTED)
                 why = why or "certificate_disabled"
@@ -273,13 +411,14 @@ class History(wc.Market):
             self.discard_eval()
             return
         self.eval, self.dirty, self.over = True, set(), False
+        self.replaced, self.appended, self.dropped = set(), set(), 0
         self.eval_mask = self.mask.copy()
         self.eval_ff = self.first_feasible()
         self.eval_facts, self.flipped = self.facts(), set()
 
     def auction_done(self, price, assigned):
         self.store(price, assigned)
-        self.auc_state, self.auc_w, self.auc_over, self.auc_toggled = True, self.n_workers, False, set()
+        self.auc_state, self.auc_w, self.auc_over, self.resized = True, self.n_workers, False, False
 
     # ---- table calls (the mirror's side)
     def apply(self, ev):
@@ -330,15 +469,28 @@ class History(wc.Market):
             changed = [int(t) for t in x["idx"] if self.mask[t] != on]
             self.mask[x["idx"]] = on
             if self.auc_state:
-                self.auc_toggled |= set(changed)
+                self.toggled |= set(changed)
         elif name == "locations":
             self.lat, self.lon = x["lat"].copy(), x["lon"].copy()
         elif name == "addr_rank":
             self.rank = x["rank"].copy()
+        elif name == "update_asks":
+            self.update_asks(x["idx"], x["rows"])
+        elif name == "append_asks":
+            self.append_asks(x["rows"])
+            if x["cap"] is not None:
+                self.set_caps(x["cap"])
+        elif name == "shrink_asks":
+            if x["n"] != len(self.asks):    # pm_resize_asks to the current size changes nothing
+                self.shrink_asks(x["n"])
+        elif name == "ask_delta_refused":   # PM_E_INVALID: nothing changes
+            pass
         elif name == "set_asks":
             self.ask_table = x["table"]
-            self.asks = self.s["asks"][x["table"]]
+            self.asks = self.s["asks"][x["table"]].copy()
             self.mask = np.ones(len(self.asks), dtype=bool)
+            self.cap, self.floors = x["cap"].copy(), x["floors"].copy()
+            self.eval_mask = self.mask.copy()
             self.discard_eval()
             self.discard_auction()
         elif name == "model_table":
@@ -390,6 +542,16 @@ def drive(eng, ev):
         eng.set_locations(x["lat"], x["lon"])
     elif name == "addr_rank":
         eng.set_addr_rank(x["rank"])
+    elif name == "update_asks":
+        eng.update_asks(x["idx"], *delta_rows(x))
+    elif name == "append_asks":
+        eng.resize_asks(x["n"], *delta_rows(x))
+        if x["cap"] is not None:
+            eng.set_price_caps(x["cap"])
+    elif name == "shrink_asks":
+        eng.resize_asks(x["n"])
+    elif name == "ask_delta_refused":
+        refuse_delta(eng, x)
     elif name == "set_asks":
         s = x["setup"]
         eng.set_asks(s["asks"][x["table"]], s["opts"])
@@ -410,10 +572,43 @@ def drive(eng, ev):
         raise ValueError(name)
 
 
+def delta_rows(x):
+    """(rows, opts) as a delta sends them: each row with only its own option rows, or with the whole option table."""
+    return own_options(x["rows"], x["opts"]) if x["own"] else (x["rows"], x["opts"])
+
+
+def refuse_delta(eng, x):
+    """One PM_E_INVALID case of pm_update_asks / pm_resize_asks: the call is refused and pm_table_version stays."""
+    from protocol_b200._lib import PrimeMatchError
+
+    T, rows, opts = x["T"], x["rows"], x["opts"]
+    assert getattr(eng, "n_asks", T) == T
+    bad_sizes = rows.copy()
+    bad_sizes["min_group_size"][-1], bad_sizes["max_group_size"][-1] = 5, 2
+    bad_range = rows.copy()
+    bad_range["opt_off"][0], bad_range["n_opts"][0] = len(opts), 1
+    bad_range["flags"][0] |= abi.PM_A_HAS_REQ
+    calls = {"index": lambda: eng.update_asks(np.array([1, T], dtype=np.uint32), rows, opts),
+             "sizes": lambda: eng.update_asks(np.array([1, 2], dtype=np.uint32), bad_sizes, opts),
+             "range": lambda: eng.update_asks(np.array([1, 2], dtype=np.uint32), bad_range, opts),
+             "grow_without_rows": lambda: eng.resize_asks(T + 2),
+             "grow_bad_range": lambda: eng.resize_asks(T + 2, bad_range, opts),
+             "too_many": lambda: eng.resize_asks(1 << 30, rows, opts)}
+    v = eng.table_version()
+    try:
+        calls[x["case"]]()
+    except PrimeMatchError as ex:
+        assert ex.status == abi.PM_E_INVALID, (x["case"], ex.status)
+    else:
+        raise AssertionError(f"ask delta {x['case']}: accepted")
+    assert eng.table_version() == v, (x["case"], "pm_table_version changed")
+    assert getattr(eng, "n_asks", T) == T, (x["case"], "n_asks changed")
+
+
 def load(eng, h: History):
     """Load an engine with the mirror's current tables (a fresh engine's start, or the start of a history)."""
     s = h.s
-    eng.set_asks(s["asks"][h.ask_table], s["opts"])
+    eng.set_asks(h.asks, h.opts)
     eng.set_model_table(s["bits"][h.bits_table], s["npat"], s["nmod"], s["words"])
     eng.set_workers(h.wa, h.wb)
     eng.set_locations(h.lat, h.lon)
@@ -493,6 +688,44 @@ class Gen:
     def points(self, n):
         return synth.CITIES[self.rng.integers(0, len(synth.CITIES), n)].T.copy()
 
+    def ask_rows(self, k, edge=0.15, missing=True):
+        """k ask rows from both tables, sometimes an edge row (EDGE_ASKS; the missing-pattern rows only if `missing`)."""
+        rng, s = self.rng, self.h.s
+        rows = s["pool"][rng.integers(0, len(s["pool"]), k)].copy()
+        n_edge = len(s["edge"]) if missing else len(s["edge"]) - 2
+        for i in np.flatnonzero(rng.random(k) < edge):
+            j = int(rng.integers(0, n_edge))
+            if j >= len(s["edge"]) - 2 and rng.random() < 0.7:   # rarer than the other edge rows
+                j = int(rng.integers(0, len(s["edge"]) - 2))
+            rows[i] = s["edge"][j]
+        return rows
+
+    def delta(self, name, rows, **x):
+        return (name, dict(x, rows=rows, opts=self.h.opts, own=bool(self.rng.random() < 0.7)))
+
+    def update_asks(self, idx, rows=None):
+        """Replace asks idx; the rows of asks with a missing pattern are replaced too (by ordinary rows)."""
+        h = self.h
+        miss = np.flatnonzero(missing_pattern(h.asks, h.opts, h.s["npat"]))
+        rows = self.ask_rows(len(idx)) if rows is None else rows
+        if len(miss):
+            idx = np.concatenate([np.asarray(idx, dtype=np.uint32), miss.astype(np.uint32)])
+            rows = np.concatenate([rows, self.ask_rows(len(miss), edge=0)])
+        return self.delta("update_asks", rows, idx=np.asarray(idx, dtype=np.uint32))
+
+    def held_asks(self):
+        """Asks holding a worker in the stored auction state, and asks that are many workers' stored first ask."""
+        h = self.h
+        held = np.flatnonzero(h.assigned != NONE) if h.auc_state and h.assigned is not None else np.zeros(0, np.int64)
+        first = np.zeros(0, dtype=np.int64)
+        if h.eval and h.eval_ff is not None:
+            ff = h.eval_ff[h.eval_ff != NONE].astype(np.int64)
+            if len(ff):
+                c = np.bincount(ff, minlength=len(h.asks))
+                first = np.argsort(-c, kind="stable")[:8]
+                first = first[c[first] > 0]
+        return held, first
+
     def call(self, name):
         rng, h = self.rng, self.h
         W, T = h.n_workers, len(h.asks)
@@ -545,9 +778,37 @@ class Gen:
         if name == "ask_off":
             on = np.flatnonzero(h.mask)
             i = rng.choice(on, min(len(on), int(rng.integers(1, 8))), replace=False)
-            if rng.random() < 0.3 and h.mask[h.z]:
-                i = np.union1d(i, [h.z])
+            if rng.random() < 0.3:
+                i = np.union1d(i, h.max0_on())
             return ("ask_off", dict(idx=np.unique(i).astype(np.uint32)))
+        if name == "update_asks":
+            held, first = self.held_asks()
+            k = int(rng.integers(1, 4))
+            r = rng.random()
+            if r < 0.3 and len(held):
+                idx = rng.choice(held, min(k, len(held)), replace=False)
+            elif r < 0.55 and len(first):
+                idx = rng.choice(first, min(k, len(first)), replace=False)
+            elif r < 0.7 and not h.mask.all():
+                idx = rng.choice(np.flatnonzero(~h.mask), 1)
+            else:
+                idx = rng.integers(0, T, k)
+            idx = np.asarray(idx, dtype=np.uint32)
+            if rng.random() < 0.2:                      # a repeated index: the last entry decides
+                idx = np.concatenate([idx, idx[:1]])
+            return self.update_asks(idx)
+        if name == "append_asks":
+            k = int(rng.integers(1, 4 if T < 280 else 2))
+            cap = None
+            if rng.random() < 0.6:
+                cap = np.concatenate([h.cap, rng.integers(50, 1500, k)]).astype(np.uint32)
+            return self.delta("append_asks", self.ask_rows(k), n=T + k, cap=cap)
+        if name == "shrink_asks":
+            n = T - int(rng.integers(1, 6 if T > 210 else 2)) if rng.random() < 0.95 else T   # T: changes nothing
+            return ("shrink_asks", dict(n=n))
+        if name == "ask_delta_refused":
+            return self.delta("ask_delta_refused", self.ask_rows(2, edge=0), T=T,
+                              case=DELTA_REFUSALS[int(rng.integers(0, len(DELTA_REFUSALS)))])
         if name == "ask_on":
             off = np.flatnonzero(~h.mask)
             if rng.random() < 0.6 or len(off) < 2:
@@ -562,8 +823,11 @@ class Gen:
             return ("locations", dict(lat=lat, lon=lon))
         if name == "addr_rank":
             return ("addr_rank", dict(rank=rng.permutation(W).astype(np.uint32)))
-        if name == "set_asks":
-            return ("set_asks", dict(table=1 - h.ask_table, setup=s, cap=h.cap.copy(), floors=h.floors_or_zero().copy()))
+        if name == "set_asks":   # caps and floors of the new table's length, the current ones where they reach
+            cap, fl = s["cap"].copy(), s["floors"].copy()
+            n = min(T, len(cap))
+            cap[:n], fl[:n] = h.cap[:n], h.floors_or_zero()[:n]
+            return ("set_asks", dict(table=1 - h.ask_table, setup=s, cap=cap, floors=fl))
         if name == "model_table":
             return ("model_table", dict(table=1 - h.bits_table, setup=s))
         if name == "auction_params":
@@ -581,10 +845,12 @@ class Gen:
 ALL_PAIRS = [(c, k) for c in CALLS for k in PASSES]
 
 
-def generate(shape, seed, n_calls=N_CALLS, cutoff=DEFAULT_CUTOFF, slot=0, n_slots=1):
-    """A seeded history: a list of events, ("call", (name, payload)) or ("pass", kind).  The mirror it returns has
-    lived through the history with the trackers only (no auction state values).  History `slot` of `n_slots` also
-    makes every n_slots-th (table call -> pass kind) pair from the slot on, so that the histories together make all."""
+def generate(shape, seed, n_calls=N_CALLS, cutoff=DEFAULT_CUTOFF, slot=0, n_slots=1, observe=None):
+    """A seeded history: a list of events, ("call", (name, payload)), ("pass", kind) or ("probe", (t0, nt)) (a
+    pm_build_cost_tile of asks [t0, t0 + nt), which changes nothing).  The mirror it returns has lived through the
+    history, auction states included.  History `slot` of `n_slots` also makes every n_slots-th (table call -> pass
+    kind) pair from the slot on, so that the histories together make all.  observe(h, event, before): called after
+    each call with the mirror and before each pass, probe or refused call with it."""
     rng = np.random.default_rng(seed)
     must = ALL_PAIRS[slot::n_slots]
     h = History(shape, cutoff)
@@ -593,15 +859,33 @@ def generate(shape, seed, n_calls=N_CALLS, cutoff=DEFAULT_CUTOFF, slot=0, n_slot
     seen_call, seen_pass = set(), set()
     last_pass, calls_since = "start", []
     domain_at = n_calls // 2
+    done = set()                             # the scripted steps made so far
 
     def emit_call(ev):
         events.append(("call", ev))
+        if observe is not None:
+            observe(h, events[-1], True)
         h.apply(ev)
         calls_since.append(ev[0])
+        if observe is not None:
+            observe(h, events[-1], False)
+        if ev[0] == "ask_delta_refused" and not follow:   # what it left: the next incremental and warm passes show it
+            follow.extend(["lean_incr", "warm"])
+        if ev[0] in ASK_DELTAS and len(h.asks) and rng.random() < 0.25:
+            probe()
+
+    def probe():
+        T = len(h.asks)
+        t0 = int(rng.integers(0, T))
+        events.append(("probe", (t0, int(rng.integers(1, min(T - t0, 40) + 1)))))
+        if observe is not None:
+            observe(h, events[-1], True)
 
     def emit_pass(kind):
         nonlocal last_pass, calls_since
         events.append(("pass", kind))
+        if observe is not None:
+            observe(h, events[-1], True)
         why, _ = h.refusal(kind)
         if kind in REFERENCE:
             h.reference_done(why is None)
@@ -616,6 +900,107 @@ def generate(shape, seed, n_calls=N_CALLS, cutoff=DEFAULT_CUTOFF, slot=0, n_slot
             seen_pass.add((last_pass, kind))
             last_pass = kind
             calls_since = []
+        if why == "pattern_missing":        # the next update replaces the rows again
+            emit_call(g.update_asks(np.zeros(0, dtype=np.uint32), h.s["pool"][:0]))
+        elif kind in AUCTION and why is None and rng.random() < 0.25:
+            probe()                         # with the max_group_size 0 rows in the auction's form
+
+    def all_on():
+        if not h.mask.all():
+            emit_call(("ask_on", dict(idx=np.flatnonzero(~h.mask).astype(np.uint32))))
+
+    def scripted(n_passes):
+        """The ask-delta steps every history makes once (each from its pass count on)."""
+        s, T = h.s, len(h.asks)
+        if n_passes >= 4 and "held" not in done:
+            # replace the asks that are many workers' stored first ask: one by a row that still accepts them (other
+            # group sizes), one by a row that accepts none; then the same for asks holding auction workers
+            done.add("held")
+            emit_pass("lean")
+            _, first = g.held_asks()
+            keep = h.asks[first[:1]].copy()
+            keep["min_group_size"], keep["max_group_size"] = 1, 2
+            emit_call(g.update_asks(first[:2], np.concatenate([keep, s["edge"][4:5]])[:len(first[:2])]))
+            emit_pass("lean_incr")
+            all_on()
+            emit_pass("auction")
+            held, _ = g.held_asks()
+            if len(held):
+                t = held[int(rng.integers(0, len(held)))]
+                keep = h.asks[[t]].copy()
+                emit_call(g.update_asks(np.array([t, held[0]], dtype=np.uint32), np.concatenate([keep, s["edge"][4:5]])))
+            emit_pass("repair" if slot % 2 else "warm")
+            return True
+        if n_passes >= 9 and "disabled" not in done:
+            # replace a disabled row, then enable it; replace the max_group_size 0 asks with ordinary rows and append
+            # a new one
+            done.add("disabled")
+            emit_pass("lean")
+            t = np.array([int(rng.integers(0, T))], dtype=np.uint32)
+            emit_call(("ask_off", dict(idx=t)))
+            emit_call(g.update_asks(t, s["pool"][[int(rng.integers(0, len(s["pool"])))]]))
+            emit_pass("lean_incr")
+            emit_call(("ask_on", dict(idx=t)))
+            z = np.flatnonzero(h.asks["max_group_size"] == 0).astype(np.uint32)
+            if len(z):
+                emit_call(g.update_asks(z, g.ask_rows(len(z), edge=0)))
+            emit_call(g.delta("append_asks", s["edge"][:1].copy(), n=len(h.asks) + 1, cap=None))
+            emit_pass("lean_incr")
+            emit_pass("proximity_incr")     # refused: the appended max_group_size 0 ask
+            return True
+        if n_passes >= 16 and "missing" not in done:
+            done.add("missing")
+            t = np.array([int(rng.integers(0, T))], dtype=np.uint32)
+            emit_call(g.delta("update_asks", s["edge"][5 + slot % 2:6 + slot % 2].copy(), idx=t))
+            emit_pass(["lean_incr", "auction", "certificate", "warm"][slot % 4])
+            return True
+        def cut_held(j):                 # past the last j asks that hold a worker (at most 20 asks)
+            held = np.flatnonzero(h.assigned != NONE) if h.auc_state else np.zeros(0, dtype=np.int64)
+            k = len(h.asks) - int(held[-j]) if len(held) >= j else 3
+            emit_call(("shrink_asks", dict(n=len(h.asks) - min(max(k, 1), 20))))
+
+        if n_passes >= 28 and h.cutoff < 1000 and "removed_held" not in done:
+            # the removed asks that held a worker decide the cutoff: shrink past held asks, then write (unchanged) kept
+            # rows until the changes without them reach the cutoff and with them pass it; a warm pass, then a repair
+            # pass, must both run cold
+            done.add("removed_held")
+            for kind in ("warm", "repair"):
+                all_on()
+                emit_pass("auction")
+                cut_held(3)
+                if h.auc_state and h.removed_held:
+                    base = h.n_changes() - h.removed_held
+                    free = np.setdiff1d(np.arange(h.n_kept), sorted(h.rows))
+                    u = rng.choice(free, max(0, h.cutoff - base), replace=False).astype(np.uint32)
+                    if len(u):
+                        u.sort()
+                        emit_call(("update", dict(idx=u, a=h.wa[u].copy(), b=h.wb[u].copy(), lat=None, lon=None)))
+                emit_pass(kind)
+            return True
+        if n_passes >= 36 and "shrink_held" not in done:
+            # shrink past asks that hold auction workers, then warm and repair passes; shrink and grow back to the
+            # same size before a certificate, which is refused
+            done.add("shrink_held")
+            all_on()
+            emit_pass("auction")
+            cut_held(4)
+            emit_pass("warm")
+            cut_held(2)
+            emit_pass("repair")
+            emit_call(("shrink_asks", dict(n=len(h.asks) - 2)))
+            emit_call(g.delta("append_asks", g.ask_rows(2, missing=False), n=len(h.asks) + 2, cap=None))
+            emit_pass("certificate")        # refused: the ask table was resized since the last auction pass
+            return True
+        if n_passes >= 24 and h.cutoff < 1000 and "e_rows" not in done:
+            # appended asks alone past the cutoff: e_rows = ceil(|E| W / T) > PM_TUNE_INCR
+            done.add("e_rows")
+            emit_pass("lean")
+            k = -(-(h.cutoff + 1) * len(h.asks) // h.n_workers) + 1
+            emit_call(g.delta("append_asks", g.ask_rows(k, missing=False), n=len(h.asks) + k, cap=None))
+            emit_pass("lean_incr")
+            emit_call(("shrink_asks", dict(n=len(h.asks) - k)))
+            return True
+        return False
 
     def mine(a, b):
         """An unseen (pass -> pass) pair this slot is to make."""
@@ -623,8 +1008,10 @@ def generate(shape, seed, n_calls=N_CALLS, cutoff=DEFAULT_CUTOFF, slot=0, n_slot
 
     follow = []
     emit_pass("lean_incr")
-    while len(events) < n_calls:
-        if len([e for e in events if e[0] == "pass"]) == domain_at // 2 and h.params != DOMAIN_EDGE:
+    while len([e for e in events if e[0] != "probe"]) < n_calls:
+        if len([e for e in events if e[0] == "pass"]) >= domain_at // 2 and "domain" not in done \
+                and h.params != DOMAIN_EDGE:
+            done.add("domain")
             # a refusal outside the integer domain, reached through a written row, between passes on a stored state
             high = np.flatnonzero(h.wb["ext_ask_price"] >= 0xFFFFFFFE).astype(np.uint32)
             if len(high):                           # only the row written below leaves the domain
@@ -648,10 +1035,14 @@ def generate(shape, seed, n_calls=N_CALLS, cutoff=DEFAULT_CUTOFF, slot=0, n_slot
             emit_call(("auction_params", dict(params=PARAMS[int(rng.integers(0, len(PARAMS)))])))
             continue
         n_passes = len([e for e in events if e[0] == "pass"])
-        if n_passes == 12 and h.mask.all():
+        if scripted(n_passes):
+            continue
+        if n_passes >= 12 and "b12" not in done and h.mask.all():
             # warm or repair after reference passes of both modes, with asks left disabled across them
+            done.add("b12")
             emit_pass("auction")
-            emit_call(("ask_off", dict(idx=np.union1d(rng.choice(len(h.asks), 5, replace=False), [h.z]).astype(np.uint32))))
+            off = np.union1d(rng.choice(len(h.asks), 5, replace=False), h.max0_on())
+            emit_call(("ask_off", dict(idx=off.astype(np.uint32))))
             emit_pass("lean")
             emit_pass("certificate")                # refused: disabled asks
             emit_call(g.call("update"))
@@ -668,7 +1059,8 @@ def generate(shape, seed, n_calls=N_CALLS, cutoff=DEFAULT_CUTOFF, slot=0, n_slot
         p = np.array([0.15 if c in RARE else 1.0 for c in names])
         for _ in range(int(rng.integers(0, 3))):
             emit_call(g.call(names[int(rng.choice(len(names), p=p / p.sum()))]))
-        if n_passes == 20:
+        if n_passes >= 20 and "b20" not in done:
+            done.add("b20")
             # past the cutoff between two reference passes (a full pass under a small PM_TUNE_INCR), and a side column
             emit_pass("lean")
             u = np.unique(rng.choice(h.n_workers, min(h.cutoff + 20, 120), replace=False)).astype(np.uint32)
@@ -677,7 +1069,8 @@ def generate(shape, seed, n_calls=N_CALLS, cutoff=DEFAULT_CUTOFF, slot=0, n_slot
             emit_call(g.call("addr_rank"))
             emit_pass("lean_incr")
             continue
-        if n_passes == 26:
+        if n_passes >= 26 and "b26" not in done:
+            done.add("b26")
             # past the cutoff between two auction passes (a cold PM_AUCTION_WARM pass under a small PM_TUNE_INCR)
             if not h.mask.all():
                 emit_call(("ask_on", dict(idx=np.flatnonzero(~h.mask).astype(np.uint32))))
@@ -687,7 +1080,8 @@ def generate(shape, seed, n_calls=N_CALLS, cutoff=DEFAULT_CUTOFF, slot=0, n_slot
             emit_call(("update", dict(idx=u, a=a, b=b, lat=None, lon=None)))
             emit_pass("warm")
             continue
-        if n_passes == 34:
+        if n_passes >= 34 and "b34" not in done:
+            done.add("b34")
             # an incremental pass with written rows after an auction pass and a certificate since its evaluation
             emit_pass("lean")
             emit_call(g.call("update"))
@@ -725,8 +1119,8 @@ def generate(shape, seed, n_calls=N_CALLS, cutoff=DEFAULT_CUTOFF, slot=0, n_slot
             if not h.mask.all() and (forced or rng.random() < 0.75):
                 emit_call(("ask_on", dict(idx=np.flatnonzero(~h.mask).astype(np.uint32))))
         elif kind.startswith("proximity"):
-            if h.mask[h.z] and rng.random() < 0.75:
-                emit_call(("ask_off", dict(idx=np.array([h.z], dtype=np.uint32))))
+            if len(h.max0_on()) and rng.random() < 0.75:
+                emit_call(("ask_off", dict(idx=h.max0_on().astype(np.uint32))))
         emit_pass(kind)
     for c, kind in must:                    # the slot's pairs the loop had no room for
         emit_call(g.call(c))

@@ -105,6 +105,7 @@ class Incremental:
                 t = int(f[w])
                 start[w] = t if dmap[t] else t + 1
                 f[w] = NONE
+        self.n_tiles = len(start)            # rows walked in full: the written rows and the orphans
         for w, s in start.items():
             hit = np.flatnonzero(G[s:, w])
             f[w] = s + hit[0] if len(hit) else NONE
@@ -123,9 +124,18 @@ def rand_rows(rng, k, W, p=0.08):
 
 
 def check(inc, what=""):
+    """The pass equals a recomputation; its E, D and walked rows are those engine_history's mirror plans."""
+    import engine_history as eh
+
+    E, D = inc.lists()
+    en, dis = eh.split_toggles(inc.on, inc.eval_on, inc.replaced)
+    assert (set(E), {t for t, _ in D}) == (en, dis), what
+    assert all(from_ask == (t in inc.replaced) for t, from_ask in D), what
+    n_tiles = eh.walked_rows(inc.stored, inc.rows, dis)
     want = first_ask(inc.F, inc.on)
     got = inc.run()
     assert np.array_equal(got, want), what
+    assert inc.n_tiles == n_tiles, (what, inc.n_tiles, n_tiles)
 
 
 def test_trap_orphan_the_replaced_row_still_accepts():

@@ -14,88 +14,117 @@ import auction_warm_checker as wc
 import engine_history as eh
 from helpers import assert_distance_certificate
 from oracle import pm_oracle as orc
-from protocol_b200 import synth
+from protocol_b200 import abi, synth
 
 
 @functools.lru_cache(maxsize=None)
 def evidence():
-    """Replay every history the GPU file runs on the mirror alone and record what each pass saw."""
+    """Generate every history the GPU file runs and record, through the generator's mirror, what each pass saw."""
     ev = dict(call_pass=set(), pass_pass=set(), refusals={}, after_refusal={}, incr_after_auction_cert=0,
-              warm_after_both=set(), flips=set(), incr_over=0, warm_over=0, n_passes=0)
+              warm_after_both=set(), flips=set(), incr_over=0, warm_over=0, n_passes=0, incr_saw=set(),
+              e_rows_over=0, removed_held=set(), removed_held_decides=set(), max0_by=set(), probes_after_auction=0,
+              generated={})
     for shape in eh.SHAPES:
         for setting in eh.SETTINGS:
             cutoff = eh.cutoff_of(setting)
-            events, _ = eh.generate(shape, eh.seed_of(shape, setting), cutoff=cutoff, slot=eh.slot_of(shape, setting),
-                                    n_slots=eh.N_SLOTS)
-            h = eh.History(shape, cutoff)
-            last, calls = "start", []
-            # refusals waiting for the next incremental pass on the kept evaluation, and for the next warm pass on
-            # the auction state they left (name, whether a stored state existed)
-            pend_incr, pend_warm = [], []
-            since_eval = dict(auction=0, certificate=0)
-            since_state = dict(ff=0, prox=0, disabled_across=False)
-            for e in events:
+            st = dict(last="start", calls=[], pend_incr=[], pend_warm=[], since_eval=dict(auction=0, certificate=0),
+                      since_state=dict(ff=0, prox=0, disabled_across=False), max0=None, after_auction=False)
+
+            def observe(h, e, before, st=st, cutoff=cutoff):
                 if e[0] == "call":
-                    h.apply(e[1])
-                    calls.append(e[1][0])
-                    if e[1][0] in ("set_asks", "model_table", "set_workers"):
-                        since_eval = dict(auction=0, certificate=0)
-                        pend_incr, pend_warm = [], []
-                    if e[1][0] == "auction_params":
-                        pend_warm = []
+                    name = e[1][0]
+                    st["after_auction"] = False   # a delta puts the rows back in the reference form
+                    if before:
+                        st["max0"] = len(h.max0_on()) > 0
+                        if name == "ask_delta_refused":
+                            ev["refusals"]["ask_delta_refused"] = ev["refusals"].get("ask_delta_refused", 0) + 1
+                            st["pend_incr"].append("ask_delta_refused")
+                            st["pend_warm"].append(("ask_delta_refused", h.auc_state))
+                        return
+                    st["calls"].append(name)
+                    if name in eh.ASK_DELTAS and (len(h.max0_on()) > 0) != st["max0"]:
+                        ev["max0_by"].add(name)
+                    if name in ("set_asks", "model_table", "set_workers"):
+                        st["since_eval"] = dict(auction=0, certificate=0)
+                        st["pend_incr"], st["pend_warm"] = [], []
+                    if name == "auction_params":
+                        st["pend_warm"] = []
                     if not h.auc_state:
-                        since_state = dict(ff=0, prox=0, disabled_across=False)
-                    continue
+                        st["since_state"] = dict(ff=0, prox=0, disabled_across=False)
+                    return
+                if e[0] == "probe":
+                    ev["probes_after_auction"] += st["after_auction"] and len(h.asks[h.asks["max_group_size"] == 0]) > 0
+                    return
                 kind = e[1]
+                st["after_auction"] = False
                 ev["n_passes"] += 1
                 why, _ = h.refusal(kind)
                 if why is not None:
                     ev["refusals"][why] = ev["refusals"].get(why, 0) + 1
                 if kind in eh.INCREMENTAL and why is None:
                     full, n_tiles, en, dis, sure = h.incremental_plan()
-                    if not full and h.dirty and since_eval["auction"] and since_eval["certificate"]:
+                    if not full and h.dirty and st["since_eval"]["auction"] and st["since_eval"]["certificate"]:
                         ev["incr_after_auction_cert"] += 1
                     if not full:
                         ev["flips"] |= h.flipped
+                        orphans = eh.walked_rows(h.eval_ff, set(), {t for t in dis if t in h.replaced})
+                        if orphans and any(h.mask[t] for t in dis if t in h.replaced):
+                            ev["incr_saw"].add("replaced_enabled_with_orphans")
+                        if any(not h.mask[t] for t in h.replaced):
+                            ev["incr_saw"].add("replaced_disabled")
+                        if en & h.appended:
+                            ev["incr_saw"].add("append")
+                        if h.dropped:
+                            ev["incr_saw"].add("shrink_dropped_first_asks")
                     if full and h.eval and h.over and cutoff < eh.DEFAULT_CUTOFF:
                         ev["incr_over"] += 1
-                    for r in pend_incr:
+                    if full and h.eval and not h.over and len(h.dirty) <= cutoff < eh.DEFAULT_CUTOFF:
+                        ev["e_rows_over"] += 1
+                    for r in st["pend_incr"]:
                         ev["after_refusal"].setdefault(r, set()).add("incremental")
                 if kind in ("warm", "repair") and why is None:
                     warm, _ = h.warm_plan()
-                    if warm and since_state["ff"] and since_state["prox"] and since_state["disabled_across"]:
+                    if warm and h.removed_held:
+                        ev["removed_held"].add(kind)
+                    if h.auc_state and not h.auc_over and h.n_changes() - h.removed_held <= cutoff < h.n_changes():
+                        ev["removed_held_decides"].add((kind, warm))
+                    ss = st["since_state"]
+                    if warm and ss["ff"] and ss["prox"] and ss["disabled_across"]:
                         ev["warm_after_both"].add(kind)
                     if h.auc_state and not warm and h.auc_over and cutoff < eh.DEFAULT_CUTOFF:
                         ev["warm_over"] += 1
-                    for r, had_state in pend_warm:   # warm on the kept state, or cold where there was none
+                    for r, had_state in st["pend_warm"]:   # warm on the kept state, or cold where there was none
                         if warm == had_state:
                             ev["after_refusal"].setdefault(r, set()).add("warm")
-                    pend_warm = []
+                    st["pend_warm"] = []
                 if kind in eh.REFERENCE and why is None:
-                    pend_incr = []               # this pass stores an evaluation: the refusals are behind it
+                    st["pend_incr"] = []               # this pass stores an evaluation: the refusals are behind it
                 if kind in ("auction", "reverse") and why is None:
-                    pend_warm = []               # a new stored state
+                    st["pend_warm"] = []               # a new stored state
                 if why is not None:
-                    pend_incr.append(why)
-                    pend_warm.append((why, h.auc_state))
+                    st["pend_incr"].append(why)
+                    st["pend_warm"].append((why, h.auc_state))
                 if kind in eh.REFERENCE:
                     if why is None:
-                        since_state["prox" if kind.startswith("proximity") else "ff"] += 1
-                        since_state["disabled_across"] |= bool(h.auc_state and not h.mask.all())
-                    h.reference_done(why is None)
-                    since_eval = dict(auction=0, certificate=0)
+                        st["since_state"]["prox" if kind.startswith("proximity") else "ff"] += 1
+                        st["since_state"]["disabled_across"] |= bool(h.auc_state and not h.mask.all())
+                    st["since_eval"] = dict(auction=0, certificate=0)
                 elif kind in eh.AUCTION:
-                    since_eval["auction"] += 1
+                    st["since_eval"]["auction"] += 1
                     if why is None:
-                        h.auction_done(None, None)
-                        since_state = dict(ff=0, prox=0, disabled_across=False)
+                        st["since_state"] = dict(ff=0, prox=0, disabled_across=False)
+                        st["after_auction"] = True
                 elif kind == "certificate":
-                    since_eval["certificate"] += 1
+                    st["since_eval"]["certificate"] += 1
                 if kind != "auction_incr":
-                    ev["call_pass"] |= {(c, kind) for c in calls}
-                    ev["pass_pass"].add((last, kind))
-                    last = kind
-                    calls = []
+                    ev["call_pass"] |= {(c, kind) for c in st["calls"]}
+                    ev["pass_pass"].add((st["last"], kind))
+                    st["last"] = kind
+                    st["calls"] = []
+
+            ev["generated"][shape, setting] = eh.generate(shape, eh.seed_of(shape, setting), cutoff=cutoff,
+                                                          slot=eh.slot_of(shape, setting), n_slots=eh.N_SLOTS,
+                                                          observe=observe)
     return ev
 
 
@@ -129,6 +158,83 @@ def test_predicate_and_tile_flips_inside_an_incremental_window():
 def test_cutoff_crossings_on_both_trackers():
     ev = evidence()
     assert ev["incr_over"] > 0 and ev["warm_over"] > 0, (ev["incr_over"], ev["warm_over"])
+
+
+def test_incremental_passes_see_every_ask_delta():
+    """Passes that stay incremental after a replaced enabled ask with orphans, a replaced disabled ask, an append, and
+    an ask shrink that set stored first asks to NONE."""
+    want = {"replaced_enabled_with_orphans", "replaced_disabled", "append", "shrink_dropped_first_asks"}
+    assert evidence()["incr_saw"] >= want, evidence()["incr_saw"]
+
+
+def test_appended_asks_alone_pass_the_cutoff():
+    """Under PM_TUNE_INCR=40 an incremental pass goes full because ceil(|E| W / T) passes the cutoff, not the rows."""
+    assert evidence()["e_rows_over"] > 0
+
+
+def test_warm_and_repair_passes_after_removed_held_asks():
+    assert evidence()["removed_held"] >= {"warm", "repair"}, evidence()["removed_held"]
+
+
+def test_removed_held_asks_decide_the_warm_cutoff():
+    """Under PM_TUNE_INCR=40 a warm and a repair pass whose changes stay within the cutoff without the removed asks that
+    held a worker and pass it with them: both run cold."""
+    assert evidence()["removed_held_decides"] >= {("warm", False), ("repair", False)}, evidence()["removed_held_decides"]
+
+
+MIRROR = ("asks", "mask", "eval_mask", "cap", "floors", "wa", "wb", "lat", "lon", "rank", "reputation", "eval_ff")
+TRACKED = ("params", "eval", "dirty", "over", "replaced", "appended", "dropped", "flipped", "auc_state", "auc_w",
+           "auc_over", "resized", "rows", "toggled", "n_kept", "cap0", "floors0")
+
+
+@pytest.mark.parametrize("setting", list(eh.SETTINGS))
+@pytest.mark.parametrize("shape", eh.SHAPES)
+def test_events_alone_rebuild_the_mirror(shape, setting):
+    """The GPU runner rebuilds the mirror from the events alone: replaying them on a fresh History (auction passes
+    without their state values) ends with the generator's tables and trackers."""
+    events, g = evidence()["generated"][shape, setting]
+    h = eh.History(shape, eh.cutoff_of(setting))
+    for e in events:
+        if e[0] == "call":
+            h.apply(e[1])
+        elif e[0] == "pass":
+            why, _ = h.refusal(e[1])
+            if e[1] in eh.REFERENCE:
+                h.reference_done(why is None)
+            elif e[1] in eh.AUCTION and why is None:
+                h.auction_done(None, None)
+    for f in MIRROR:
+        a, b = getattr(h, f), getattr(g, f)
+        assert (a is None and b is None) or np.array_equal(a, b), f
+    for f in TRACKED:
+        a, b = getattr(h, f), getattr(g, f)
+        assert (np.array_equal(a, b) if isinstance(a, np.ndarray) else a == b), f
+
+
+def test_fast_predicate_flips_through_an_ask_row():
+    assert "ask_fast" in evidence()["flips"], evidence()["flips"]
+
+
+def test_max_group_size_zero_fact_changes_through_every_ask_delta():
+    assert evidence()["max0_by"] >= set(eh.ASK_DELTAS), evidence()["max0_by"]
+
+
+def test_cost_tile_probes_after_auction_passes_with_max0_rows():
+    assert evidence()["probes_after_auction"] > 0
+
+
+def test_a_missing_pattern_is_any_id_past_the_model_table():
+    """pattern_id >= n_patterns is missing, 0xFFFFFFFF (whose 32-bit pattern row wraps to 0) included; an option row
+    without PM_O_MODEL or an ask without requirements reads no pattern."""
+    s = eh.setup("mixed")
+    npat = s["npat"]
+    asks = np.repeat(s["edge"][5:6], 5).copy()
+    opts = np.zeros(4, dtype=s["opts"].dtype)
+    opts["present"] = [abi.PM_O_MODEL, abi.PM_O_MODEL, abi.PM_O_MODEL, 0]
+    opts["pattern_id"] = [npat - 1, npat, 0xFFFFFFFF, npat]
+    asks["opt_off"] = [0, 1, 2, 3, 1]
+    asks["flags"][4] = 0
+    assert eh.missing_pattern(asks, opts, npat).tolist() == [False, True, True, False, False]
 
 
 def test_locations_pass_the_distance_certificate():

@@ -1,11 +1,15 @@
 """One engine through long random histories of every table call, every pass kind and the auction certificate
 (tests/engine_history.py), compared after every call with plain references computed from the host mirror: the CPU
 oracle for reference passes, the exact auction checkers for auction passes, the certificate restatement for the
-certificate, and the mirror's change sets for whether a pass stays incremental or warm.  Refused calls must return the
-status the header gives and leave behind what it says: the next pass of each kind shows it.  After every reference
-pass a fresh engine with the same settings, loaded from the mirror, must return the same arrays.
+certificate, and the mirror's change sets for whether a pass stays incremental or warm (and how many rows an
+incremental pass walks).  Refused calls must return the status the header gives and leave behind what it says: the
+next pass of each kind shows it.  After every reference pass, and after every cold auction pass once the ask table has
+changed in place, a fresh engine with the same settings, loaded from the mirror, must return the same arrays.  Cost
+tile probes between passes compare pm_build_cost_tile with the oracle's cost matrix and change nothing.  The same
+histories' reference side also runs on pm_multi.
 
 PM_TEST_BIG=1 runs histories three times as long."""
+import functools
 import os
 
 import numpy as np
@@ -15,19 +19,22 @@ import auction_certificate as ac
 import engine_history as eh
 from protocol_b200 import abi
 from protocol_b200._lib import PrimeMatchError
-from protocol_b200.engine import Engine
+from oracle import pm_oracle as orc
+from protocol_b200.engine import Engine, MultiEngine
 
 pytestmark = pytest.mark.gpu
 
 FIELDS = ("worker_group", "worker_ask", "group_ask", "group_off", "group_members", "ask_best", "ask_count")
 
 
-def new_engine(setting):
+def new_engine(setting, make=None):
     """An engine created with the setting's PM_TUNE_* knobs (they are read at pm_create)."""
     env = {k: str(v) for k, v in eh.SETTINGS[setting].items()}
     old = {k: os.environ.get(k) for k in env}
     os.environ.update(env)
     try:
+        if make is not None:
+            return make(eh.TILE_BYTES.get(setting, 0))
         return Engine(cost_tile_bytes=eh.TILE_BYTES.get(setting, 0))
     finally:
         for k, v in old.items():
@@ -54,6 +61,7 @@ class Runner:
         self.eng = new_engine(setting)
         eh.load(self.eng, self.h)
         self.counts = {}
+        self.deltas = False         # the ask table has changed in place
 
     def close(self):
         self.eng.close()
@@ -122,6 +130,17 @@ class Runner:
         assert res.stats["n_rounds"] == n, (kind, "n_rounds", res.stats["n_rounds"], n)
         assert released == rel, (kind, "n_released", released, rel)
         assert rs == wrs, (kind, "reverse stats", rs, wrs)
+        if not warm and self.deltas:   # a cold pass after deltas equals a fresh engine's (prime_match.h)
+            fresh = new_engine(self.setting)
+            eh.load(fresh, h)
+            fresh.match(eh.MODES[kind])
+            q = fresh.fetch()
+            qprice, _, _ = fresh.auction_state()
+            qrs = fresh.auction_reverse_stats()
+            fresh.close()
+            assert np.array_equal(res.worker_ask, q.worker_ask), f"{kind}: assignment differs from a fresh engine's"
+            assert np.array_equal(price, qprice) and res.stats["n_rounds"] == q.stats["n_rounds"] and rs == qrs, \
+                f"{kind}: prices or rounds differ from a fresh engine's"
         h.auction_done(p, a)
 
     def certificate(self):
@@ -137,10 +156,26 @@ class Runner:
             assert out[k] == want[k], ("certificate", k, out[k], want[k])
         assert np.array_equal(out["ask_bound"], want["ask_bound"])
 
+    def probe(self, t0, nt):
+        """pm_build_cost_tile over asks [t0, t0 + nt) against the oracle's cost matrix (disabled rows PM_COST_INF)."""
+        h = self.h
+        if h.pattern_missing():
+            assert refused(lambda: self.eng.cost_tile(t0, nt), {abi.PM_E_STATE}) is not None, "probe: ran"
+            return
+        got = self.eng.cost_tile(t0, nt)
+        want = orc.soa_eval_matrix(h.wa, h.wb, h.asks, h.opts, h.bits, h.words, t0, t0 + nt, 0, h.n_workers, threads=8,
+                                   want_cost=True, want_rows=False, want_cols=False)["cost"]
+        want[~h.mask[t0:t0 + nt]] = eh.INF
+        assert np.array_equal(got, want), f"probe [{t0}, {t0 + nt}): cost tile differs from the oracle"
+
     def step(self, ev):
         if ev[0] == "call":
             eh.drive(self.eng, ev[1])
             self.h.apply(ev[1])
+            self.deltas |= ev[1][0] in eh.ASK_DELTAS
+            return
+        if ev[0] == "probe":
+            self.probe(*ev[1])
             return
         kind = ev[1]
         self.counts[kind] = self.counts.get(kind, 0) + 1
@@ -160,20 +195,94 @@ def replay(shape, setting, events):
             try:
                 r.step(ev)
             except AssertionError as ex:
-                what = ev[1] if ev[0] == "pass" else ev[1][0]
+                what = ev[1][0] if ev[0] == "call" else ev[1]
                 raise AssertionError(f"{shape}/{setting}: event {i} ({ev[0]} {what}): {ex}") from ex
     finally:
         r.close()
     return r.counts
 
 
+@functools.lru_cache(maxsize=None)
+def history(shape, setting):
+    """The events of the seeded history of (shape, setting), generated once per session."""
+    return eh.generate(shape, eh.seed_of(shape, setting), cutoff=eh.cutoff_of(setting), slot=eh.slot_of(shape, setting),
+                       n_slots=eh.N_SLOTS)[0]
+
+
 @pytest.mark.parametrize("setting", list(eh.SETTINGS))
 @pytest.mark.parametrize("shape", eh.SHAPES)
 def test_history(shape, setting):
-    events, _ = eh.generate(shape, eh.seed_of(shape, setting), cutoff=eh.cutoff_of(setting),
-                            slot=eh.slot_of(shape, setting), n_slots=eh.N_SLOTS)
+    events = history(shape, setting)
     counts = replay(shape, setting, events)
     assert all(counts.get(k, 0) for k in eh.PASSES), counts
+
+
+class ReferenceOnly:
+    """A MultiEngine behind the drive() calls: the auction's columns (caps, floors, reputation, parameters) are no
+    pm_multi calls, and none of them touches what a reference pass reads."""
+
+    def __init__(self, multi, h):
+        self.m, self.h = multi, h
+
+    @property
+    def n_workers(self):
+        return self.h.n_workers
+
+    def __getattr__(self, name):
+        if name in ("set_price_caps", "set_min_reputation", "set_worker_reputation", "set_auction_params"):
+            return lambda *a, **k: None
+        return getattr(self.m, name)
+
+
+MULTI_SKIP = ("reputation", "caps", "floors", "auction_params")   # the auction's columns: no pm_multi calls
+
+
+def test_history_on_multi():
+    """The reference side of every history on one pm_multi over every visible device: worker and ask table calls,
+    refused ask deltas (PM_E_INVALID, pm_multi_table_version unchanged), toggles, locations, ranks, table swaps and
+    every reference and incremental pass, each pass against the oracle.
+    With one device the incremental passes must walk exactly the rows the mirror plans; with more, each rank's share
+    moves when the worker table is resized, which the mirror does not model, so only the results are compared."""
+    import torch
+
+    devices = list(range(max(1, torch.cuda.device_count())))
+    n_ref = 0
+    for shape in eh.SHAPES:
+        for setting in eh.SETTINGS:
+            events = history(shape, setting)
+            h = eh.History(shape, eh.cutoff_of(setting))
+            m = new_engine(setting, lambda tb: MultiEngine(devices, cost_tile_bytes=tb))
+            eng = ReferenceOnly(m, h)
+            try:
+                eh.load(eng, h)
+                for i, ev in enumerate(events):
+                    what = f"{shape}/{setting} on {len(devices)} device(s): event {i}"
+                    if ev[0] == "call":
+                        if ev[1][0] not in MULTI_SKIP:
+                            eh.drive(eng, ev[1])
+                        h.apply(ev[1])
+                        continue
+                    if ev[0] != "pass" or ev[1] not in eh.REFERENCE:
+                        continue
+                    kind = ev[1]
+                    why, statuses = h.refusal(kind)
+                    plan = h.incremental_plan() if kind in eh.INCREMENTAL else None
+                    if refused(lambda: m.match(eh.MODES[kind]), statuses) is not None:
+                        h.reference_done(False)
+                        continue
+                    assert why is None, f"{what}: {kind} ran, expected refusal {why}"
+                    r = m.fetch()
+                    want = eh.expect_reference(h, kind)
+                    for f in FIELDS:
+                        assert np.array_equal(getattr(r, f), want[f]), f"{what}: {kind}: {f} differs from the oracle"
+                    if plan is not None and len(devices) == 1 and plan[4]:
+                        st = m.stats(0)
+                        assert st["n_tiles"] == plan[1], (what, kind, "n_tiles", st["n_tiles"], plan[1])
+                    h.reference_done(True)
+                    n_ref += 1
+            finally:
+                m.close()
+    assert n_ref > 100
 
 
 def shortened(shape, setting, events):
@@ -234,4 +343,34 @@ def test_auction_fills_an_ask_of_max_group_size_zero():
     assert c["n_bad_holds"] == 0
     got, (price, warm, released) = auction(eh.WARM)
     assert warm and released == 0 and np.array_equal(got, want) and np.array_equal(price, wprice)
+    eng.close()
+
+
+def test_a_pattern_id_of_all_ones_is_a_missing_pattern():
+    """A history finding, shortened to one delta: an option row with pattern_id 0xFFFFFFFF made pm_ask_convert's 32-bit
+    pattern row pattern_id + 1 wrap to 0, which reads as "no model pattern", so the table was accepted and the row
+    matched any model.  Like any pattern past the model table it now makes every pass, the certificate and the cost
+    tile return PM_E_STATE until the row is replaced, while the stored evaluation and auction state follow the header:
+    the reference pass that failed discards the evaluation, the refused auction pass keeps the state."""
+    h = eh.History("mixed")
+    eng = new_engine("default")
+    eh.load(eng, h)
+    s = h.s
+    eng.match(eh.MODES["auction"])
+    price, _, _ = eng.auction_state()
+    eng.match(eh.MODES["lean_incr"])
+    for row in (s["edge"][6:7], s["edge"][5:6]):      # pattern 0xFFFFFFFF, then the first pattern past the table
+        eng.update_asks([7], row, s["opts"])
+        for call in (lambda: eng.match(eh.MODES["lean_incr"]), lambda: eng.match(eh.MODES["warm"]),
+                     lambda: eng.auction_certificate(), lambda: eng.cost_tile(0, 8)):
+            assert refused(call, {abi.PM_E_STATE}) == abi.PM_E_STATE
+        assert np.array_equal(eng.auction_state()[0], price)
+    eng.update_asks([7], h.asks[7:8], s["opts"])
+    eng.match(eh.MODES["lean_incr"])
+    r = eng.fetch()
+    want = eh.expect_reference(h, "lean_incr")
+    assert all(np.array_equal(getattr(r, f), want[f]) for f in FIELDS)
+    assert r.stats["n_tiles"] == h.n_workers           # the failed pass discarded the stored evaluation
+    eng.match(eh.MODES["warm"])
+    assert eng.auction_state()[1] == 1                 # the refused auction passes kept the stored state
     eng.close()
