@@ -473,6 +473,48 @@ typedef struct pm_auction_cert {
 } pm_auction_cert;
 int pm_auction_certificate(pm_engine*, pm_auction_cert* out, int64_t* ask_bound);
 
+/* Auction state restore.  The stored state lives only in the engine that made it: pm_set_asks, pm_set_worker_count,
+ * pm_set_model_table, pm_set_shard, pm_attach_comm, a failed auction pass, a restart and a move to another engine all
+ * lose it, and the next pass is cold.  pm_auction_state (the prices) and pm_auction_assignment export it;
+ * pm_auction_restore takes it back, into this engine or another one with the same tables.
+ * pm_auction_assignment: the stored state's assignment, assigned[t] = the worker ask t holds, or PM_NONE, over the
+ * current n_asks (after the remaps of pm_update_asks / pm_resize_asks; worker indices are the stored pass's rows).
+ * PM_E_STATE where pm_auction_state returns it; a NULL assigned with n_asks > 0: PM_E_INVALID.
+ * pm_auction_restore audits the caller's state against the tables as they stand now, then makes it the stored state.
+ * With S = cost_scale, feasible(t,w) as for the reverse rounds (candidate, compatible, ask_price <= cap, reputation >=
+ * floor), and key(w), row(t) and slack(t) = key(w_t) - row(t) as for the certificate, under the current tables, caps,
+ * floors and S, every hold assigned[t] = w_t is checked in this order and dropped (the ask holds nothing) when
+ *   1. bad:     feasible(t, w_t) is false;
+ *   2. shared:  w_t is named by more than one ask (every such hold, feasible or not, counts as naming it);
+ *   3. slack:   slack(t) > 1.
+ * Every other hold is kept.  No price changes: a dropped hold's worker is unowned at its given price.  Dropping holds
+ * changes no kept ask's slack, so one pass is enough; the kept holds are feasible, unshared and eps-complementary slack
+ * at eps = 1, the state a warm start needs (DESIGN 4).
+ * On success the audited state replaces the stored state, if there is one: the stored caps and floors become the
+ * current ones, no row or ask counts as changed since it, pm_auction_state reports the restored prices with warm = 0
+ * and n_released = 0, pm_auction_reverse_stats reports zeros, and the next PM_AUCTION_WARM pass, with or without
+ * PM_AUCTION_REPAIR, starts warm from it.  The certificate of the restored state shows no bad, shared or over-slack
+ * hold, and the next warm or repair pass is within T of the optimum of the current instance (the optimum with
+ * cost_scale = T + 1), as a cold pass is.  pm_fetch_result, pm_get_stats, pm_table_version and the reference modes'
+ * stored evaluation (PM_INCREMENTAL) are untouched.  report (NULL-able) gets the counts; evals = T x W.
+ * Refusals, none of which changes anything (neither the stored state nor anything reported on it):
+ *   PM_E_INVALID      a NULL pointer with a count > 0; n_workers or n_asks other than the current tables'; an assigned
+ *                     entry neither PM_NONE nor < n_workers; a price < 0 or > (K + 1) * S + max(E, 1), K the largest
+ *                     current cap and E = eps_start (the bound the warm pass's and the repair's packed-key decisions
+ *                     assume); tables and parameters outside the auction's integer domain;
+ *   PM_E_STATE        no worker or ask table, no price caps, or an ask referencing a missing model pattern;
+ *   PM_E_UNSUPPORTED  disabled asks, a shard range or a communicator (the auction's own refusals).           */
+int pm_auction_assignment(pm_engine*, uint32_t* assigned);
+typedef struct pm_auction_restore_report {
+  uint32_t n_held;            /* holds kept                                                          */
+  uint32_t n_dropped_bad;     /* holds infeasible under the current tables                           */
+  uint32_t n_dropped_shared;  /* feasible holds of a worker named by more than one ask (all of them)   */
+  uint32_t n_dropped_slack;   /* feasible, unshared holds with slack > 1                             */
+  uint64_t evals;             /* (ask, worker) pairs evaluated: T x W                                */
+} pm_auction_restore_report;
+int pm_auction_restore(pm_engine*, const int64_t* price, uint32_t n_workers, const uint32_t* assigned, uint32_t n_asks,
+                       pm_auction_restore_report* report);
+
 typedef struct pm_stats {
   uint64_t evals;            /* predicate evaluations executed on the device        */
   uint64_t cost_bytes_written;

@@ -196,4 +196,50 @@ __global__ void pm_auction_cert_workers(CertParams c, const uint4* __restrict__ 
   }
 }
 
+// ------------------------------------------------------------------ restore (pm_auction_restore)
+// The caller's state is audited by the certificate's own sweep and per-ask pass (CertParams pointed at the staged
+// prices and assignment): row terms, held-pair feasibility and ownership counts.  Then one decision per ask and one
+// pass over the workers, both into staging buffers; the engine copies them over the stored state once nothing can
+// refuse any more.  Prices are never changed: a dropped hold's worker is unowned at its given price.
+enum RestoreAcc : int { kRstHeld, kRstBad, kRstShared, kRstSlack, kRstAccWords };
+constexpr uint32_t kRstHolder = 0x80000000u;   // own[w] after the audit: kRstHolder | t for the kept hold of ask t
+
+// Per ask, after pm_auction_cert_asks: a hold is dropped when it is infeasible, else when its worker is named by more
+// than one ask, else when its slack key(w_t) - row(t) exceeds 1; a kept hold marks its worker's count (1: nobody else
+// writes it; counts stay below 2^30, so the mark is told apart).
+__global__ void pm_auction_restore_asks(CertParams c, const uint4* __restrict__ wb, uint32_t* __restrict__ kept,
+                                        unsigned long long* __restrict__ acc) {
+  const uint32_t n = c.n_asks;
+  for (uint32_t base = blockIdx.x * blockDim.x; base < n; base += gridDim.x * blockDim.x) {   // warp-uniform trip count
+    const uint32_t t = base + threadIdx.x;
+    bool keep = false, bad = false, shared = false, over = false;
+    if (t < n) {
+      const uint32_t a = __ldg(c.assigned + t);
+      if (a < c.n_workers) {
+        bad = c.held_ok[t] == 0u;
+        shared = !bad && c.own[a] > 1u;
+        if (!bad && !shared) {
+          const unsigned long long key = (unsigned long long)__ldg(&wb[a].w) * c.scale + (unsigned long long)__ldg(c.price + a);
+          over = (long long)key - c.ask_bound[t] > 1;
+          keep = !over;
+        }
+        if (keep) c.own[a] = kRstHolder | t;
+      }
+      kept[t] = keep ? a : kNone;
+    }
+    cert_count(acc, kRstHeld, keep);
+    cert_count(acc, kRstBad, bad);
+    cert_count(acc, kRstShared, shared);
+    cert_count(acc, kRstSlack, over);
+  }
+}
+
+// Per worker, after pm_auction_restore_asks: the owner array of the kept holds
+__global__ void pm_auction_restore_workers(const uint32_t* __restrict__ own, uint32_t n_workers, uint32_t* __restrict__ owner) {
+  for (uint32_t w = blockIdx.x * blockDim.x + threadIdx.x; w < n_workers; w += gridDim.x * blockDim.x) {
+    const uint32_t o = own[w];
+    owner[w] = (o & kRstHolder) ? (o & ~kRstHolder) : kNone;
+  }
+}
+
 }  // namespace pm

@@ -492,6 +492,11 @@ struct pm_engine {
   DevBuf<long long> cert_bound;
   PinBuf<uint64_t> h_cert_acc;
   PinBuf<long long> h_cert_bound;
+  // pm_auction_restore's staging: the caller's prices and assignment, the kept assignment, the rebuilt owners, the counts
+  DevBuf<long long> rst_price;
+  DevBuf<uint32_t> rst_assigned, rst_kept, rst_owner;
+  DevBuf<uint64_t> rst_acc;
+  PinBuf<uint64_t> h_rst_acc;
   // pm_resize_asks since the stored state: the removed asks that held a kept row (those rows are unowned now, at their
   // stored prices; they count against the cutoff), and whether the ask table was resized at all (the certificate then
   // waits for the next pass)
@@ -972,6 +977,8 @@ void pm_destroy(pm_engine* e) {
   e->auc_rev_cstart.release(); e->auc_rev_offer_p.release(); e->auc_rev_best.release(); e->auc_rev_pi_s.release();
   e->cert_min.release(); e->cert_acc.release(); e->cert_ok.release(); e->cert_own.release(); e->cert_bound.release();
   e->h_cert_acc.release(); e->h_cert_bound.release();
+  e->rst_price.release(); e->rst_assigned.release(); e->rst_kept.release(); e->rst_owner.release(); e->rst_acc.release();
+  e->h_rst_acc.release();
   e->worker_group.release(); e->worker_ask.release(); e->group_ask.release();
   e->group_off.release(); e->members.release(); e->h_scalars.release();
   e->xchg_send.release(); e->xchg_recv.release();
@@ -2676,30 +2683,19 @@ int pm_auction_reverse_stats(pm_engine* e, uint32_t* n_phases, uint32_t* n_rever
   return PM_OK;
 } catch (...) { return pm_guard_rc(); }
 
-// The certificate of the stored auction state (pm_auction_cert.cuh): one sweep over every pair, then one pass over the
-// asks and one over the workers, on private buffers; one synchronisation.  Reads the stored state and the tables only:
-// the result buffers, pm_stats, the table version and the warm-start bookkeeping stay as they are.
-int pm_auction_certificate(pm_engine* e, pm_auction_cert* out, int64_t* ask_bound) try {
-  if (!e || !out) return e ? e->fail(PM_E_INVALID, "pm_auction_certificate: null output") : PM_E_INVALID;
-  std::lock_guard<std::mutex> lk(e->mu);
-  if (!e->auc_state) return e->fail(PM_E_STATE, "pm_auction_certificate: no auction pass since the engine's tables were last replaced");
+// pm_get_stats keeps reporting the last pass: the launch checks of a certificate or a restore count into e->stats,
+// which is put back on return
+struct KeepStats {
+  pm_engine* e;
+  pm_stats saved;
+  ~KeepStats() { e->stats = saved; }
+};
+
+// The certificate's kernels (pm_auction_cert.cuh) over the prices and assignment given (device, [W] and [T]), into the
+// certificate's private scratch: one sweep over every pair, then one pass over the asks and one over the workers.
+// Enqueued only; *c gets the parameters the launches took.
+static int cert_launch(pm_engine* e, const long long* price, const uint32_t* assigned, pm::CertParams* out) {
   const uint32_t W = e->n_workers, T = e->n_asks;
-  if (W != e->auc_state_w) return e->fail(PM_E_STATE, "pm_auction_certificate: the worker table was resized since the last auction pass");
-  if (e->auc_asks_resized) return e->fail(PM_E_STATE, "pm_auction_certificate: the ask table was resized since the last auction pass");
-  if (e->max_pattern_row > e->n_patterns || (e->max_pattern_row && !e->have_bits))
-    return e->fail(PM_E_STATE, "pm_auction_certificate: an ask references a model pattern missing from the model table");
-  if (e->n_off) return e->fail(PM_E_UNSUPPORTED, "pm_auction_certificate: disabled asks");
-  {
-    const int rc = use_ask_form(e, true);
-    if (rc != PM_OK) return rc;
-  }
-  // pm_get_stats keeps reporting the last pass: the launch checks below count into e->stats, which is put back on return
-  struct KeepStats {
-    pm_engine* e;
-    pm_stats saved;
-    ~KeepStats() { e->stats = saved; }
-  } keep_stats{e, e->stats};
-  PM_CUDA(cudaSetDevice(e->device));
   if (!e->have_bits) {   // as an auction pass: no model table is one all-ones word
     PM_CUDA(e->bits.ensure(1));
     PM_CUDA(cudaMemsetAsync(e->bits.p, 0xFF, 4, e->stream));
@@ -2708,16 +2704,15 @@ int pm_auction_certificate(pm_engine* e, pm_auction_cert* out, int64_t* ask_boun
   PM_CUDA(e->cert_min.ensure(std::max<uint32_t>(T, 1))); PM_CUDA(e->cert_ok.ensure(std::max<uint32_t>(T, 1)));
   PM_CUDA(e->cert_bound.ensure(std::max<uint32_t>(T, 1))); PM_CUDA(e->cert_own.ensure(std::max<uint32_t>(W, 1)));
   PM_CUDA(e->cert_acc.ensure(pm::kCertAccWords)); PM_CUDA(e->h_cert_acc.ensure(pm::kCertAccWords));
-  if (ask_bound) PM_CUDA(e->h_cert_bound.ensure(std::max<uint32_t>(T, 1)));
   PM_CUDA(cudaMemsetAsync(e->cert_min.p, 0xFF, (size_t)std::max<uint32_t>(T, 1) * 8, e->stream));
   PM_CUDA(cudaMemsetAsync(e->cert_own.p, 0, (size_t)std::max<uint32_t>(W, 1) * 4, e->stream));
   PM_CUDA(cudaMemsetAsync(e->cert_acc.p, 0, pm::kCertAccWords * 8, e->stream));
-  pm::CertParams c;
-  c.price = e->auc_price.p;
+  pm::CertParams& c = *out;
+  c.price = price;
   c.rep = e->have_min_rep && e->have_rep ? e->reputation.p : nullptr;
   c.cap = e->price_cap.p;
   c.floor = e->have_min_rep ? e->ask_min_rep.p : nullptr;
-  c.assigned = e->auc_assigned.p;
+  c.assigned = assigned;
   c.row_min = reinterpret_cast<unsigned long long*>(e->cert_min.p);
   c.held_ok = e->cert_ok.p;
   c.own = e->cert_own.p;
@@ -2755,6 +2750,34 @@ int pm_auction_certificate(pm_engine* e, pm_auction_cert* out, int64_t* ask_boun
     pm::pm_auction_cert_workers<<<std::min(blocks_for(W, 256), 4u * e->sms), 256, 0, e->stream>>>(c, e->wb.p);
     PM_LAUNCH_CHECK("pm_auction_cert_workers");
   }
+  return PM_OK;
+}
+
+// The certificate of the stored auction state (pm_auction_cert.cuh) on private buffers; one synchronisation.  Reads the
+// stored state and the tables only: the result buffers, pm_stats, the table version and the warm-start bookkeeping stay
+// as they are.
+int pm_auction_certificate(pm_engine* e, pm_auction_cert* out, int64_t* ask_bound) try {
+  if (!e || !out) return e ? e->fail(PM_E_INVALID, "pm_auction_certificate: null output") : PM_E_INVALID;
+  std::lock_guard<std::mutex> lk(e->mu);
+  if (!e->auc_state) return e->fail(PM_E_STATE, "pm_auction_certificate: no auction pass since the engine's tables were last replaced");
+  const uint32_t W = e->n_workers, T = e->n_asks;
+  if (W != e->auc_state_w) return e->fail(PM_E_STATE, "pm_auction_certificate: the worker table was resized since the last auction pass");
+  if (e->auc_asks_resized) return e->fail(PM_E_STATE, "pm_auction_certificate: the ask table was resized since the last auction pass");
+  if (e->max_pattern_row > e->n_patterns || (e->max_pattern_row && !e->have_bits))
+    return e->fail(PM_E_STATE, "pm_auction_certificate: an ask references a model pattern missing from the model table");
+  if (e->n_off) return e->fail(PM_E_UNSUPPORTED, "pm_auction_certificate: disabled asks");
+  {
+    const int rc = use_ask_form(e, true);
+    if (rc != PM_OK) return rc;
+  }
+  KeepStats keep_stats{e, e->stats};
+  PM_CUDA(cudaSetDevice(e->device));
+  if (ask_bound) PM_CUDA(e->h_cert_bound.ensure(std::max<uint32_t>(T, 1)));
+  pm::CertParams c;
+  {
+    const int rc = cert_launch(e, e->auc_price.p, e->auc_assigned.p, &c);
+    if (rc != PM_OK) return rc;
+  }
   PM_CUDA(cudaMemcpyAsync(e->h_cert_acc.p, e->cert_acc.p, pm::kCertAccWords * 8, cudaMemcpyDeviceToHost, e->stream));
   if (ask_bound && T) PM_CUDA(cudaMemcpyAsync(e->h_cert_bound.p, e->cert_bound.p, (size_t)T * 8, cudaMemcpyDeviceToHost, e->stream));
   PM_CUDA(cudaStreamSynchronize(e->stream));
@@ -2782,6 +2805,112 @@ int pm_auction_certificate(pm_engine* e, pm_auction_cert* out, int64_t* ask_boun
   r.evals = (uint64_t)T * W;
   *out = r;
   if (ask_bound && T) std::memcpy(ask_bound, e->h_cert_bound.p, (size_t)T * 8);
+  return PM_OK;
+} catch (...) { return pm_guard_rc(); }
+
+// The stored state's assignment over the current asks (remapped by pm_update_asks / pm_resize_asks like the state itself)
+int pm_auction_assignment(pm_engine* e, uint32_t* assigned) try {
+  if (!e) return PM_E_INVALID;
+  std::lock_guard<std::mutex> lk(e->mu);
+  if (!e->auc_state) return e->fail(PM_E_STATE, "pm_auction_assignment: no auction pass since the engine's tables were last replaced");
+  if (e->n_asks && !assigned) return e->fail(PM_E_INVALID, "pm_auction_assignment: null output");
+  PM_CUDA(cudaSetDevice(e->device));
+  if (e->n_asks) {
+    PM_CUDA(cudaMemcpyAsync(assigned, e->auc_assigned.p, (size_t)e->n_asks * 4, cudaMemcpyDeviceToHost, e->stream));
+    PM_CUDA(cudaStreamSynchronize(e->stream));
+  }
+  return PM_OK;
+} catch (...) { return pm_guard_rc(); }
+
+// A caller's auction state, audited on the device and made the stored state (prime_match.h "Auction state restore").
+// Every host check first, then the caller's arrays go to staging buffers and the certificate's kernels run over them;
+// the audit (pm_auction_restore_asks, pm_auction_restore_workers) writes staging buffers too.  One synchronisation,
+// the domain check on the sweep's largest ask price, and only then the stored state is overwritten, by device copies.
+int pm_auction_restore(pm_engine* e, const int64_t* price, uint32_t n_workers, const uint32_t* assigned, uint32_t n_asks,
+                       pm_auction_restore_report* report) try {
+  if (!e) return PM_E_INVALID;
+  std::lock_guard<std::mutex> lk(e->mu);
+  if ((n_workers && !price) || (n_asks && !assigned)) return e->fail(PM_E_INVALID, "pm_auction_restore: null");
+  if (!e->have_workers || !e->have_asks) return e->fail(PM_E_STATE, "pm_auction_restore: worker and ask tables must be set first");
+  if (!e->have_caps) return e->fail(PM_E_STATE, "pm_auction_restore: no price caps (pm_set_ask_price_caps)");
+  if (e->max_pattern_row > e->n_patterns || (e->max_pattern_row && !e->have_bits))
+    return e->fail(PM_E_STATE, "pm_auction_restore: an ask references a model pattern missing from the model table");
+  if (e->cfg.shard_count || e->comm) return e->fail(PM_E_UNSUPPORTED, "pm_auction_restore: auction mode is single-GPU");
+  if (e->n_off) return e->fail(PM_E_UNSUPPORTED, "pm_auction_restore: disabled asks");
+  const uint32_t W = e->n_workers, T = e->n_asks;
+  if (n_workers != W || n_asks != T) return e->fail(PM_E_INVALID, "pm_auction_restore: one price per worker and one entry per ask");
+  for (uint32_t t = 0; t < T; ++t)
+    if (assigned[t] != PM_NONE && assigned[t] >= W) return e->fail(PM_E_INVALID, "pm_auction_restore: assigned worker out of range");
+  // every price the warm pass and the repair can start from: (K + 1) * S + max(E, 1), in 128 bits
+  uint32_t K = 0;
+  for (uint32_t t = 0; t < T; ++t) K = std::max(K, e->cap_host[t]);
+  const unsigned __int128 p_max = ((unsigned __int128)K + 1u) * e->auc_scale + std::max<uint64_t>(e->auc_eps_start, 1);
+  for (uint32_t w = 0; w < W; ++w)
+    if (price[w] < 0 || (unsigned __int128)price[w] > p_max)
+      return e->fail(PM_E_INVALID, "pm_auction_restore: price outside [0, (max cap + 1) * cost_scale + eps_start]");
+  {
+    const int rc = use_ask_form(e, true);
+    if (rc != PM_OK) return rc;
+  }
+  KeepStats keep_stats{e, e->stats};
+  PM_CUDA(cudaSetDevice(e->device));
+  // the stored buffers at their pass sizes, their contents kept (a refusal below leaves the stored state as it was)
+  PM_CUDA(e->auc_price.grow_keep((size_t)W + 2, e->auc_price.n, e->stream)); PM_CUDA(e->auc_owner.grow_keep(W, e->auc_owner.n, e->stream));
+  PM_CUDA(e->auc_assigned.grow_keep(T, e->auc_assigned.n, e->stream));
+  PM_CUDA(e->rst_price.ensure(std::max<uint32_t>(W, 1))); PM_CUDA(e->rst_owner.ensure(std::max<uint32_t>(W, 1)));
+  PM_CUDA(e->rst_assigned.ensure(std::max<uint32_t>(T, 1))); PM_CUDA(e->rst_kept.ensure(std::max<uint32_t>(T, 1)));
+  PM_CUDA(e->rst_acc.ensure(pm::kRstAccWords)); PM_CUDA(e->h_rst_acc.ensure(pm::kRstAccWords));
+  if (W) PM_CUDA(cudaMemcpyAsync(e->rst_price.p, price, (size_t)W * 8, cudaMemcpyHostToDevice, e->stream));
+  if (T) PM_CUDA(cudaMemcpyAsync(e->rst_assigned.p, assigned, (size_t)T * 4, cudaMemcpyHostToDevice, e->stream));
+  PM_CUDA(cudaMemsetAsync(e->rst_acc.p, 0, pm::kRstAccWords * 8, e->stream));
+  pm::CertParams c;
+  {
+    const int rc = cert_launch(e, e->rst_price.p, e->rst_assigned.p, &c);
+    if (rc != PM_OK) return rc;
+  }
+  if (T) {
+    pm::pm_auction_restore_asks<<<std::min(blocks_for(T, 256), 4u * e->sms), 256, 0, e->stream>>>(
+        c, e->wb.p, e->rst_kept.p, reinterpret_cast<unsigned long long*>(e->rst_acc.p));
+    PM_LAUNCH_CHECK("pm_auction_restore_asks");
+  }
+  if (W) {
+    pm::pm_auction_restore_workers<<<std::min(blocks_for(W, 256), 8u * e->sms), 256, 0, e->stream>>>(e->cert_own.p, W, e->rst_owner.p);
+    PM_LAUNCH_CHECK("pm_auction_restore_workers");
+  }
+  PM_CUDA(cudaMemcpyAsync(e->h_cert_acc.p, e->cert_acc.p, pm::kCertAccWords * 8, cudaMemcpyDeviceToHost, e->stream));
+  PM_CUDA(cudaMemcpyAsync(e->h_rst_acc.p, e->rst_acc.p, pm::kRstAccWords * 8, cudaMemcpyDeviceToHost, e->stream));
+  PM_CUDA(cudaStreamSynchronize(e->stream));
+  if (!auction_in_domain((uint32_t)e->h_cert_acc.p[pm::kCertMaxAskPrice], K, e->auc_scale, e->auc_eps_start))
+    return e->fail(PM_E_INVALID, "pm_auction_restore: (max ask_price + max cap + 2) * cost_scale + eps_start must stay below 2^61");
+  // commit: from here a failure leaves a half-copied state, which is dropped
+  e->auc_discard();
+  if (W) {
+    PM_CUDA(cudaMemcpyAsync(e->auc_price.p, e->rst_price.p, (size_t)W * 8, cudaMemcpyDeviceToDevice, e->stream));
+    PM_CUDA(cudaMemcpyAsync(e->auc_owner.p, e->rst_owner.p, (size_t)W * 4, cudaMemcpyDeviceToDevice, e->stream));
+  }
+  PM_CUDA(cudaMemsetAsync(e->auc_price.p + W, 0, 2 * 8, e->stream));
+  if (T) PM_CUDA(cudaMemcpyAsync(e->auc_assigned.p, e->rst_kept.p, (size_t)T * 4, cudaMemcpyDeviceToDevice, e->stream));
+  PM_CUDA(cudaStreamSynchronize(e->stream));
+  // the bookkeeping of a pass that just ran on the current tables: nothing changed since, nothing to report
+  e->auc_state = true;
+  e->auc_state_w = e->auc_kept = W;
+  e->auc_row_mark.assign(W, 0);
+  e->auc_ask_mark.assign(T, 0);
+  e->auc_cap_stored = e->cap_host;
+  if (e->have_min_rep) e->auc_floor_stored = e->floor_host;
+  else e->auc_floor_stored.assign(T, 0u);
+  e->auc_last_warm = false;
+  e->auc_last_released = 0;
+  e->auc_last_phases = e->auc_last_rev_rounds = 0;
+  e->auc_last_rev_bids = 0;
+  if (report) {
+    const uint64_t* h = e->h_rst_acc.p;
+    report->n_held = (uint32_t)h[pm::kRstHeld];
+    report->n_dropped_bad = (uint32_t)h[pm::kRstBad];
+    report->n_dropped_shared = (uint32_t)h[pm::kRstShared];
+    report->n_dropped_slack = (uint32_t)h[pm::kRstSlack];
+    report->evals = (uint64_t)T * W;
+  }
   return PM_OK;
 } catch (...) { return pm_guard_rc(); }
 

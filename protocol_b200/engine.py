@@ -271,6 +271,23 @@ class Engine:
             out["ask_bound"] = rows
         return out
 
+    def auction_assignment(self) -> np.ndarray:
+        """The stored auction state's assignment (pm_auction_assignment): uint32[n_asks], the worker each ask holds or
+        PM_NONE.  With auction_state()'s prices this is what auction_restore() takes."""
+        out = np.zeros(self.n_asks, dtype=np.uint32)
+        self._check(self._lib.pm_auction_assignment(self._h, _ptr(out)))
+        return out
+
+    def auction_restore(self, price, assigned) -> dict:
+        """Audit (price i64[n_workers], assigned u32[n_asks]) against the current tables and make it the stored auction
+        state (pm_auction_restore): bad, shared and over-slack holds are dropped, prices kept.  Returns the report."""
+        price = np.ascontiguousarray(price, dtype=np.int64)
+        assigned = np.ascontiguousarray(assigned, dtype=np.uint32)
+        rep = abi.PmAuctionRestoreReport()
+        self._check(self._lib.pm_auction_restore(self._h, _ptr(price), len(price), _ptr(assigned), len(assigned), C.byref(rep)))
+        self._auction_workers = len(price)
+        return {n: int(getattr(rep, n)) for n, _ in rep._fields_}
+
     # ---- the pass ---------------------------------------------------------
     def match(self, mode: int = abi.PM_MODE_FIRST_FIT):
         """pm_match.  Auction passes (PM_MODE_AUCTION) take PM_AUCTION_WARM: start from the last auction pass's state,
