@@ -267,7 +267,8 @@ int      pm_create_sibling(const pm_engine*, pm_engine** out);
  * per-ask price cap against pm_worker_b.ext_ask_price, and the auction's parameters
  * (value = -(ask_price * cost_scale) - price; eps runs eps_start, /eps_div, ..., 1).
  * PM_MODE_AUCTION has no group sizes: an ask with max_group_size == 0, which no reference mode fills, takes a worker
- * like any other there (and in pm_auction_certificate).
+ * like any other there (and in pm_auction_certificate).  An ask takes one worker, or up to its demand with
+ * pm_set_ask_demand ("Auction demands" below); min_group_size is never enforced.
  * Integer domain of PM_MODE_AUCTION: with P = the largest ext_ask_price over every row of the worker table (feasible or
  * not), K = the largest price cap, S = cost_scale and E = eps_start (0 counts as 1 for both),
  *     (P + K + 2) * S + E < 2^61          (evaluated without overflow).
@@ -285,6 +286,37 @@ int pm_set_auction_params(pm_engine*, uint64_t cost_scale, uint64_t eps_start, u
  * pm_set_worker_count drops it.  min_reputation is per ask, after pm_set_asks, like the price caps.      */
 int pm_set_worker_reputation(pm_engine*, const uint32_t* reputation, uint32_t first, uint32_t n);
 int pm_set_ask_min_reputation(pm_engine*, const uint32_t* min_reputation, uint32_t n_asks);
+/* Auction demands (north-star extension column; PM_MODE_AUCTION only, the reference modes never read it).
+ * demand[t] >= 1 is the number of workers ask t may take; each of them is priced and capped separately: value(t, w),
+ * feasible(t, w) and the outside option -(cap[t] + 1) * S do not change.  Fills may be partial: an ask with demand 4
+ * may end holding 0 to 4 workers.  min_group_size is NOT enforced: an all-or-nothing gang is not an assignment
+ * problem (its LP relaxation loses integrality, and the eps-CS argument with it; DESIGN 4).
+ * THE DEFINING RULE: an engine with demands d behaves as the engine whose ask table repeats row t d[t] times at
+ * consecutive priorities, with its cap and floor repeated.  Each copy is a SLOT; there are D = sum d[t] of them, in ask
+ * order (slot s of ask t is sum_{u<t} d[u] + k, k < d[t]).  Every auction pass kind (cold, eps-scaled with
+ * PM_AUCTION_REVERSE, PM_AUCTION_WARM, PM_AUCTION_WARM | PM_AUCTION_REPAIR) gives that twin's assignment, prices,
+ * rounds, warm / n_released and reverse stats, bit for bit; the results are folded per ask; the guarantee is the twin's:
+ * a total cost within D * eps of the optimum, exact with cost_scale = D + 1.
+ * pm_set_ask_demand takes exactly n_asks entries, as pm_set_ask_price_caps does.  Without the call, or with every demand
+ * 1, behaviour is today's byte for byte (the same kernels, no extra launch).  After pm_set_asks every demand is 1;
+ * pm_update_asks keeps a replaced row's demand (as it keeps its cap); pm_resize_asks appends rows with demand 1 and a
+ * shrink drops the removed rows' demands.
+ * Refusals change nothing (not the demands, not the stored auction state, not pm_table_version): PM_E_INVALID for a
+ * NULL pointer with n_asks > 0, n_asks other than the table's, a demand of 0, or D >= 2^30 (the ask-count limit; a
+ * pm_resize_asks growth that would take D there is refused the same way); PM_E_STATE without an ask table.
+ * A demand change under a stored auction state: each ask's first min(old, new) slots keep their holds; a removed slot's
+ * worker becomes unowned at its stored price and counts against the warm cutoff, like a removed ask's holder; the added
+ * slots hold nothing and are in A0.  The warm start and the repair then run unchanged on the remapped state (DESIGN 4).
+ * Result form with demands (pm_fetch_result): one group per ask holding at least one worker, in ask order, its members
+ * in increasing worker index; worker_ask[w] is the ask and worker_group[w] the group; ask_count[t] the workers held;
+ * ask_best[t] the smallest ask_price << 32 | w over them (PM_COST_INF for none); n_groups the asks holding a worker,
+ * n_members the workers held.  With every demand 1 this is exactly the one-worker-per-ask form.
+ * pm_stats keeps its meanings, counted over slots.  pm_auction_certificate is over slots: n_held, n_slack_over and
+ * max_slack count or range over slots, bound = sum_t d[t] * row(t) - sum_w price[w], ask_bound stays per ask (every
+ * slot of an ask has the same row term), evals stays T x W.  pm_auction_assignment and pm_auction_restore return
+ * PM_E_UNSUPPORTED while any demand exceeds 1 (their format is one worker per ask).  The auction stays single-GPU: there
+ * is no pm_multi_ form. */
+int pm_set_ask_demand(pm_engine*, const uint32_t* demand, uint32_t n_asks);
 
 enum pm_mode {
   PM_MODE_FIRST_FIT = 0,   /* try_form_new_groups, ProximityOptimizationPolicy{enabled:false} */
@@ -292,7 +324,8 @@ enum pm_mode {
   PM_MODE_PROXIMITY_MERGE = 3, /* try_merge_solo_groups' batch selection (mod.rs:752-848) over a table that  */
                            /* holds only the nodes of solo groups, in get_all_groups() order               */
   PM_MODE_AUCTION   = 2    /* north-star extension: price-capped forward auction, one worker  */
-                           /* per ask (pm_auction.cuh); no reference counterpart, self-oracle */
+                           /* per ask or per slot of its demand (pm_set_ask_demand;           */
+                           /* pm_auction.cuh); no reference counterpart, self-oracle          */
 };
 enum pm_path {
   PM_PATH_MATERIALIZED = 0,      /* build a cost tile in HBM (the 32-bit cost word when every price is

@@ -62,6 +62,7 @@ def load() -> C.CDLL:
         "pm_set_ask_price_caps": (i32, [vp, vp, u32]),
         "pm_set_worker_reputation": (i32, [vp, vp, u32, u32]),
         "pm_set_ask_min_reputation": (i32, [vp, vp, u32]),
+        "pm_set_ask_demand": (i32, [vp, vp, u32]),
         "pm_set_auction_params": (i32, [vp, C.c_uint64, C.c_uint64, u32]),
         "pm_auction_state": (i32, [vp, vp, P(u32), P(u32)]),
         "pm_auction_reverse_stats": (i32, [vp, P(u32), P(u32), P(C.c_uint64)]),

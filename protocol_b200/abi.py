@@ -135,6 +135,7 @@ EXPORTS = [
     "pm_set_asks", "pm_set_ask_enabled", "pm_update_asks", "pm_resize_asks", "pm_set_model_table", "pm_set_worker_count", "pm_upsert_workers",
     "pm_set_worker_locations", "pm_set_worker_addr_rank", "pm_set_flags",
     "pm_set_ask_price_caps", "pm_set_auction_params", "pm_set_worker_reputation", "pm_set_ask_min_reputation",
+    "pm_set_ask_demand",
     "pm_auction_state", "pm_auction_reverse_stats", "pm_auction_certificate", "pm_auction_assignment", "pm_auction_restore",
     "pm_match", "pm_fetch_result", "pm_get_stats", "pm_build_cost_tile",
     "pm_match_local", "pm_match_finish", "pm_device_buffer", "pm_stream_sync", "pm_set_shard",

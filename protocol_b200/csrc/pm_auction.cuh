@@ -1,4 +1,5 @@
-// pm_auction.cuh — NORTH-STAR EXTENSION: price-capped forward auction (one worker per ask).
+// pm_auction.cuh — NORTH-STAR EXTENSION: price-capped forward auction (one worker per ask, or per slot of an ask's
+// demand: the kernels run on the slot table as on an ask table, "ask demands" at the end).
 //
 // The reference orchestrator has no prices, caps, reputation or auction (SURVEY.md 0):
 // nothing here restates reference code, and parity for this mode is against the
@@ -1264,6 +1265,98 @@ __global__ void pm_auction_emit(const uint32_t* __restrict__ assigned, const uin
   members[g] = w;
   ask_best[t] = ((long long)wb[w].w << 32) | (long long)w;
   ask_count[t] = 1;
+}
+
+// ---- ask demands (pm_set_ask_demand) -------------------------------------------------------------------
+// Ask t with demand d[t] is d[t] bidders, its SLOTS off[t] .. off[t + 1] - 1 (off: the exclusive scan of the demands):
+// the ask's row repeated d[t] times at consecutive priorities.  The auction runs on the slots as on any ask table, over
+// per-slot copies of the row, the cap and the floor; only the result is folded back per ask.
+__device__ __forceinline__ uint32_t auc_ask_of_slot(const uint32_t* __restrict__ off, uint32_t n_asks, uint32_t s) {
+  uint32_t lo = 0, hi = n_asks;   // off[lo] <= s < off[hi]; every demand is >= 1, so off is strictly increasing
+  while (hi - lo > 1u) {
+    const uint32_t mid = (lo + hi) >> 1;
+    if (off[mid] <= s) lo = mid;
+    else hi = mid;
+  }
+  return lo;
+}
+// the slot table: each slot's ask, and its copies of the ask's converted row, cap and floor (floor: null without one)
+__global__ void pm_auction_slot_table(const uint32_t* __restrict__ off, uint32_t n_asks, uint32_t n_slots, const DevAsk* __restrict__ asks,
+                                      const uint32_t* __restrict__ cap, const uint32_t* __restrict__ floor, uint32_t* __restrict__ slot_ask,
+                                      DevAsk* __restrict__ slot_row, uint32_t* __restrict__ slot_cap, uint32_t* __restrict__ slot_floor) {
+  for (uint32_t s = blockIdx.x * blockDim.x + threadIdx.x; s < n_slots; s += gridDim.x * blockDim.x) {
+    const uint32_t t = auc_ask_of_slot(off, n_asks, s);
+    slot_ask[s] = t;
+    slot_row[s] = asks[t];
+    slot_cap[s] = cap[t];
+    if (floor) slot_floor[s] = floor[t];
+  }
+}
+// A demand change under a stored state: old slot k of ask t keeps its hold as new slot k while k < the new demand;
+// past it the slot is gone and its worker becomes unowned at its stored price, counted in `count` when it is a kept row
+// (as pm_auction_drop_asks does for a removed ask).  new_assigned is all PM_NONE before: added slots hold nothing.
+__global__ void pm_auction_demand_remap(const uint32_t* __restrict__ old_off, const uint32_t* __restrict__ new_off, uint32_t n_asks,
+                                        uint32_t n_old, const uint32_t* __restrict__ old_assigned, uint32_t* __restrict__ new_assigned,
+                                        uint32_t* __restrict__ owner, uint32_t n_rows, uint32_t* __restrict__ count) {
+  uint32_t freed = 0;
+  for (uint32_t s = blockIdx.x * blockDim.x + threadIdx.x; s < n_old; s += gridDim.x * blockDim.x) {
+    const uint32_t t = auc_ask_of_slot(old_off, n_asks, s), k = s - old_off[t];
+    const uint32_t w = old_assigned[s];
+    if (k < new_off[t + 1] - new_off[t]) {
+      const uint32_t ns = new_off[t] + k;
+      new_assigned[ns] = w;
+      if (w < n_rows) owner[w] = ns;
+    } else if (w < n_rows) {
+      owner[w] = kNone;
+      ++freed;
+    }
+  }
+  if (freed) atomicAdd(count, freed);
+}
+// Grouped result (demands set): held[s] for the slots' exclusive scan `spos` (members in slot order) ...
+__global__ void pm_auction_slot_flags(const uint32_t* __restrict__ assigned, uint32_t n_slots, uint32_t* __restrict__ flag) {
+  const uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s < n_slots) flag[s] = assigned[s] != kNone ? 1u : 0u;
+  if (s == n_slots) flag[s] = 0u;
+}
+// ... per ask over its slot segment: the held count, ask_best, and whether it forms a group (for the groups' scan) ...
+__global__ void pm_auction_group_counts(const uint32_t* __restrict__ off, const uint32_t* __restrict__ spos,
+                                        const uint32_t* __restrict__ assigned, const uint4* __restrict__ wb, uint32_t n_asks,
+                                        uint32_t* __restrict__ flag, long long* __restrict__ ask_best, uint32_t* __restrict__ ask_count) {
+  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t == n_asks) flag[t] = 0u;
+  if (t >= n_asks) return;
+  const uint32_t s0 = off[t], s1 = off[t + 1], n = spos[s1] - spos[s0];
+  long long best = kInf;
+  for (uint32_t s = s0; s < s1 && n; ++s) {
+    const uint32_t w = assigned[s];
+    if (w != kNone) best = min(best, ((long long)wb[w].w << 32) | (long long)w);
+  }
+  flag[t] = n ? 1u : 0u;
+  ask_best[t] = best;
+  ask_count[t] = n;
+}
+// ... and one group per ask holding a worker, in ask order; its members in slot order (the engine sorts each group's
+// members by worker index afterwards)
+__global__ void pm_auction_group_emit(const uint32_t* __restrict__ off, const uint32_t* __restrict__ spos,
+                                      const uint32_t* __restrict__ gidx, const uint32_t* __restrict__ assigned, uint32_t n_asks,
+                                      uint32_t* __restrict__ worker_group, uint32_t* __restrict__ worker_ask,
+                                      uint32_t* __restrict__ group_ask, uint32_t* __restrict__ group_off, uint32_t* __restrict__ members) {
+  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= n_asks) return;
+  const uint32_t s0 = off[t], s1 = off[t + 1];
+  uint32_t j = spos[s0];
+  if (spos[s1] == j) return;
+  const uint32_t g = gidx[t];
+  group_ask[g] = t;
+  group_off[g] = j;
+  for (uint32_t s = s0; s < s1; ++s) {
+    const uint32_t w = assigned[s];
+    if (w == kNone) continue;
+    members[j++] = w;
+    worker_group[w] = g;
+    worker_ask[w] = t;
+  }
 }
 
 }  // namespace pm

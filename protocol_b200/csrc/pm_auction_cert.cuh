@@ -171,6 +171,52 @@ __global__ void pm_auction_cert_asks(CertParams c, const uint4* __restrict__ wb)
   }
 }
 
+// ------------------------------------------------------------------ per slot (ask demands)
+// With demands (pm_set_ask_demand) the sweep stays per ask, T x W (every slot of an ask has the ask's row term), run
+// with no holds, and this pass takes pm_auction_cert_asks' place over the slots: slot s of ask slot_ask[s] adds the
+// ask's row term, so the row sum is sum_t d[t] * row(t), and its own hold's cost, slack and ownership count.  A held
+// pair's feasibility is checked here with the predicate of eval_row_global (ask_meets), cap and floor as in the sweep.
+// c.assigned is the slots' assignment; the ask's first slot writes ask_bound.
+__global__ void pm_auction_cert_slots(CertParams c, EvalParams p, const uint32_t* __restrict__ slot_ask, uint32_t n_slots) {
+  for (uint32_t base = blockIdx.x * blockDim.x; base < n_slots; base += gridDim.x * blockDim.x) {   // warp-uniform trip count
+    const uint32_t s = base + threadIdx.x;
+    const bool in = s < n_slots;
+    unsigned long long cost = 0, bound = 0;
+    long long slack = LLONG_MIN;
+    bool held = false, bad = false;
+    if (in) {
+      const uint32_t t = __ldg(slot_ask + s);
+      const uint32_t cap = __ldg(c.cap + t);
+      const unsigned long long outside = ((unsigned long long)cap + 1ull) * c.scale;
+      bound = min(outside, c.row_min[t]);
+      if (s == 0 || __ldg(slot_ask + s - 1) != t) c.ask_bound[t] = (long long)bound;
+      const uint32_t a = __ldg(c.assigned + s);
+      held = a < c.n_workers;
+      if (held) {
+        const WorkerReg wr = make_worker(__ldg(p.wa + a), __ldg(p.wb + a));
+        const uint32_t rep = c.rep ? __ldg(c.rep + a) : 0u, fl = c.floor ? __ldg(c.floor + t) : 0u;
+        bad = !(wr.price <= cap && rep >= fl && ask_meets(p.asks[t], p.opts, wr, p.bits, p.words));
+        cost = (unsigned long long)wr.price * c.scale;
+        slack = (long long)(cost + (unsigned long long)__ldg(c.price + a)) - (long long)bound;
+        atomicAdd(c.own + a, 1u);
+      } else {
+        cost = outside;
+        slack = (long long)(outside - bound);
+      }
+    }
+    cert_add128(c.acc, kCertCostLo, cost);
+    cert_add128(c.acc, kCertRowLo, bound);
+    cert_count(c.acc, kCertHeld, held);
+    cert_count(c.acc, kCertBadHolds, bad);
+    cert_count(c.acc, kCertSlackOver, in && slack > 1);
+    long long ms = slack;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) ms = max(ms, __shfl_xor_sync(0xffffffffu, ms, o));
+    if ((threadIdx.x & 31u) == 0u && ms != LLONG_MIN)
+      atomicMax(c.acc + kCertMaxSlack, (unsigned long long)ms ^ 0x8000000000000000ull);
+  }
+}
+
 // ------------------------------------------------------------------ per worker
 // Every price into sum_w p[w]; the shared holds; the unowned workers with a positive price; the largest ask price of
 // the table (the integer domain's P).  After pm_auction_cert_asks (the ownership counts).

@@ -10,6 +10,7 @@
 // device (H100) pm_create fails with PM_E_NO_DEVICE.
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
+#include <cub/device/device_segmented_radix_sort.cuh>
 
 #include <cuda.h>   // driver types and prototypes only: the entry points are resolved at run time (TileBuf)
 #include <dlfcn.h>
@@ -488,7 +489,7 @@ struct pm_engine {
   DevBuf<long long> auc_rev_offer_p, auc_rev_best, auc_rev_pi_s;
   // pm_auction_certificate's own scratch: row minima, held-pair feasibility, ownership counts, row terms, accumulators
   DevBuf<uint64_t> cert_min, cert_acc;
-  DevBuf<uint32_t> cert_ok, cert_own;
+  DevBuf<uint32_t> cert_ok, cert_own, cert_none;   // cert_none: [T] no holds, the per-ask sweep's view with demands
   DevBuf<long long> cert_bound;
   PinBuf<uint64_t> h_cert_acc;
   PinBuf<long long> h_cert_bound;
@@ -502,8 +503,20 @@ struct pm_engine {
   // waits for the next pass)
   uint32_t auc_removed_held = 0;
   bool auc_asks_resized = false;
+  // Ask demands (pm_set_ask_demand; the auction only): empty while every ask takes one worker, and the auction then runs
+  // on the ask table itself.  Else the demands and their exclusive scan over T + 1 (host, and device in dem_off): ask t
+  // is the auction's bidders (slots) dem_off[t] .. dem_off[t + 1] - 1, and the stored assignment is per slot.  The pass
+  // builds the slot table (each slot's ask, and copies of its converted row, cap and floor) and runs on it.
+  // auc_dem_kept[t]: the leading slots of ask t that can carry a stored hold since the last pass (empty: all of them);
+  // a demand change lowers it, and the slots past it are in A0.
+  std::vector<uint32_t> demand, dem_off_h, auc_dem_kept;
+  DevBuf<uint32_t> dem_off, dem_off_old, slot_ask, slot_cap, slot_floor, auc_assigned_tmp, dem_members, dem_spos, dem_aflag;
+  DevBuf<pm::DevAsk> slot_row;
+  uint32_t n_slots() const { return demand.empty() ? n_asks : dem_off_h[n_asks]; }
+  uint32_t slot0(uint32_t t) const { return demand.empty() ? t : dem_off_h[t]; }
   void auc_discard() {
     auc_state = false;
+    auc_dem_kept.clear();
     auc_rows.clear();
     auc_toggled.clear();
     auc_row_mark.clear();
@@ -961,6 +974,8 @@ void pm_destroy(pm_engine* e) {
   e->pg_clat.release(); e->pg_clon.release(); e->pg_ccos.release();
   e->nacc.release(); e->bits_wm.release();
   e->reputation.release(); e->ask_min_rep.release(); e->auc_rep_s.release(); e->auc_split_first.release(); e->auc_skip_key.release();
+  e->dem_off.release(); e->dem_off_old.release(); e->slot_ask.release(); e->slot_cap.release(); e->slot_floor.release();
+  e->auc_assigned_tmp.release(); e->cert_none.release(); e->dem_members.release(); e->dem_spos.release(); e->dem_aflag.release(); e->slot_row.release();
   e->price_cap.release(); e->auc_owner.release(); e->auc_assigned.release(); e->auc_withdrawn.release();
   e->auc_active.release(); e->auc_bid_w.release(); e->auc_winner.release(); e->auc_flag.release(); e->auc_gidx.release();
   e->auc_price.release(); e->auc_bid_p.release(); e->auc_bid_max.release();
@@ -1038,6 +1053,8 @@ int pm_set_asks(pm_engine* e, const pm_ask* asks, uint32_t n_asks, const pm_gpu_
   recount_kinds(e);
   e->have_caps = false;
   e->have_min_rep = false;
+  e->demand.clear();
+  e->dem_off_h.clear();
   e->auc_classes_valid = false;
   e->rows_auction = false;
   e->have_asks = true;
@@ -1128,6 +1145,19 @@ template <class Body> static int ask_delta(pm_engine* e, Body&& body) {
 }
 }
 
+// The demands' offsets to the device; demands that are all 1 are dropped (the auction runs on the asks themselves).
+static int upload_demand(pm_engine* e) {
+  if (std::all_of(e->demand.begin(), e->demand.end(), [](uint32_t d) { return d == 1u; })) {
+    e->demand.clear();
+    e->dem_off_h.clear();
+    return PM_OK;
+  }
+  PM_CUDA(e->dem_off.ensure(e->dem_off_h.size()));
+  PM_CUDA(cudaMemcpyAsync(e->dem_off.p, e->dem_off_h.data(), e->dem_off_h.size() * 4, cudaMemcpyHostToDevice, e->stream));
+  PM_CUDA(cudaStreamSynchronize(e->stream));   // dem_off_h may be reallocated by the next call
+  return PM_OK;
+}
+
 int pm_update_asks(pm_engine* e, const uint32_t* idx, const pm_ask* asks, uint32_t n, const pm_gpu_opt* opts,
                    uint32_t n_opts) try {
   if (!e) return PM_E_INVALID;
@@ -1170,6 +1200,10 @@ int pm_resize_asks(pm_engine* e, uint32_t n_asks, const pm_ask* added, const pm_
     if (rc != PM_OK) return e->fail((pm_status)rc, err);
   }
   if (n_asks == old) return PM_OK;
+  // with demands the appended asks take one slot each; the slots stay below the ask-count limit
+  const uint32_t old_slots = e->n_slots();
+  const uint32_t new_slots = e->demand.empty() ? n_asks : (n_asks < old ? e->dem_off_h[n_asks] : old_slots + n_add);
+  if ((uint64_t)old_slots + n_add >= (1u << 30)) return e->fail(PM_E_INVALID, "pm_resize_asks: the ask demands' total reaches 2^30");
   ++e->table_version;
   return ask_delta(e, [&]() -> int {
     PM_CUDA(cudaSetDevice(e->device));
@@ -1191,7 +1225,7 @@ int pm_resize_asks(pm_engine* e, uint32_t n_asks, const pm_ask* added, const pm_
         cudaError_t ce = cudaMemsetAsync(e->counters.p + 17, 0, 4, e->stream);
         if (ce == cudaSuccess) {
           pm::pm_auction_drop_asks<<<std::min(blocks_for(e->auc_kept, 256), 8u * e->sms), 256, 0, e->stream>>>(e->auc_owner.p, e->auc_kept,
-                                                                                                               n_asks, e->counters.p + 17);
+                                                                                                               new_slots, e->counters.p + 17);
           ce = cudaGetLastError();
         }
         if (ce == cudaSuccess) ce = cudaMemcpyAsync(e->h_scalars.p + 17, e->counters.p + 17, 4, cudaMemcpyDeviceToHost, e->stream);
@@ -1200,8 +1234,12 @@ int pm_resize_asks(pm_engine* e, uint32_t n_asks, const pm_ask* added, const pm_
         e->auc_removed_held += e->h_scalars.p[17];
       }
       drop_from(&e->auc_toggled);
-      cut(&e->auc_ask_mark); cut(&e->auc_cap_stored); cut(&e->auc_floor_stored);
+      cut(&e->auc_ask_mark); cut(&e->auc_cap_stored); cut(&e->auc_floor_stored); cut(&e->auc_dem_kept);
       cut(&e->ask_on); cut(&e->eval_on); cut(&e->toggle_mark); cut(&e->repl_mark); cut(&e->cap_host); cut(&e->floor_host);
+      if (!e->demand.empty()) {
+        e->demand.resize(n_asks);
+        e->dem_off_h.resize((size_t)n_asks + 1);
+      }
     } else {
       // appended rows: enabled, cap 0, floor 0, in E (eval_on 0) and in A0 (no stored cap or floor), holding nothing
       e->ask_on.resize(n_asks, 1);
@@ -1223,14 +1261,24 @@ int pm_resize_asks(pm_engine* e, uint32_t n_asks, const pm_ask* added, const pm_
         e->floor_host.resize(n_asks, 0u);
         ce = zero_tail(e->ask_min_rep, 0);
       }
-      if (ce == cudaSuccess && e->auc_state) {
-        ce = zero_tail(e->auc_assigned, 0xFF);
+      if (!e->demand.empty()) {
+        e->demand.resize(n_asks, 1u);
+        for (uint32_t t = old; t < n_asks; ++t) e->dem_off_h.push_back(e->dem_off_h[t] + 1u);
+      }
+      if (ce == cudaSuccess && e->auc_state) {   // the appended slots hold nothing
+        ce = e->auc_assigned.grow_keep(new_slots, old_slots, e->stream);
+        if (ce == cudaSuccess) ce = cudaMemsetAsync(e->auc_assigned.p + old_slots, 0xFF, (size_t)(new_slots - old_slots) * 4, e->stream);
         e->auc_ask_mark.resize(n_asks, 0);
         e->auc_cap_stored.resize(n_asks, 0u);
         e->auc_floor_stored.resize(n_asks, 0u);
+        if (!e->auc_dem_kept.empty()) e->auc_dem_kept.resize(n_asks, 0u);
         for (uint32_t t = old; t < n_asks; ++t) e->auc_mark_ask(t);
       }
       if (ce != cudaSuccess) return e->fail(PM_E_CUDA, std::string("pm_resize_asks: ") + cudaGetErrorString(ce));
+    }
+    if (!e->demand.empty()) {
+      const int rc = upload_demand(e);
+      if (rc != PM_OK) return rc;
     }
     if (e->auc_state) e->auc_asks_resized = true;
     return commit_asks(e, n_asks, uidx.data(), urows.data(), (uint32_t)uidx.size(), opts);
@@ -2165,15 +2213,15 @@ static int match_finish_locked(pm_engine* e, uint32_t mode) {
 }
 
 // ------------------------------------------------------------------ extension: auction
-// Ask classes for the auction: asks with identical requirement rows (pm_auction.cuh).
-static int auction_build_classes(pm_engine* e) {
-  const uint32_t T = e->n_asks;
+// Ask classes for the auction: asks with identical requirement rows (pm_auction.cuh), over the T rows and floors given
+// (the ask table, or with demands the slot table).
+static int auction_build_classes(pm_engine* e, const pm::DevAsk* rows, const uint32_t* floor, uint32_t T) {
   e->auc_n_classes = 0;
   PM_CUDA(e->auc_class_of.ensure(T)); PM_CUDA(e->auc_class_rep.ensure(T)); PM_CUDA(e->auc_hash.ensure(T));
   PM_CUDA(e->auc_hash_out.ensure(T)); PM_CUDA(e->auc_idx.ensure(T)); PM_CUDA(e->auc_sorted.ensure(T));
   PM_CUDA(e->auc_flag.ensure((size_t)T + 1)); PM_CUDA(e->auc_incl.ensure(T));
   if (T == 0) { e->auc_classes_valid = true; return PM_OK; }
-  pm::pm_auction_ask_hash<<<blocks_for(T, 256), 256, 0, e->stream>>>(e->asks.p, e->opts.p, e->have_min_rep ? e->ask_min_rep.p : nullptr, T, e->auc_hash.p, e->auc_idx.p);
+  pm::pm_auction_ask_hash<<<blocks_for(T, 256), 256, 0, e->stream>>>(rows, e->opts.p, floor, T, e->auc_hash.p, e->auc_idx.p);
   PM_LAUNCH_CHECK("pm_auction_ask_hash");
   size_t tmp_sort = 0, tmp_scan = 0;
   cub::DeviceRadixSort::SortPairs(nullptr, tmp_sort, e->auc_hash.p, e->auc_hash_out.p, e->auc_idx.p, e->auc_sorted.p, (int)T, 0, 64, e->stream);
@@ -2181,7 +2229,7 @@ static int auction_build_classes(pm_engine* e) {
   size_t tmp = std::max(tmp_sort, tmp_scan);
   PM_CUDA(e->cub_tmp.ensure(tmp));
   PM_CUDA(cub::DeviceRadixSort::SortPairs(e->cub_tmp.p, tmp, e->auc_hash.p, e->auc_hash_out.p, e->auc_idx.p, e->auc_sorted.p, (int)T, 0, 64, e->stream));
-  pm::pm_auction_class_flags<<<blocks_for(T, 256), 256, 0, e->stream>>>(e->asks.p, e->opts.p, e->have_min_rep ? e->ask_min_rep.p : nullptr, e->auc_sorted.p, T, e->auc_flag.p);
+  pm::pm_auction_class_flags<<<blocks_for(T, 256), 256, 0, e->stream>>>(rows, e->opts.p, floor, e->auc_sorted.p, T, e->auc_flag.p);
   PM_LAUNCH_CHECK("pm_auction_class_flags");
   PM_CUDA(cub::DeviceScan::InclusiveSum(e->cub_tmp.p, tmp, e->auc_flag.p, e->auc_incl.p, (int)T, e->stream));
   pm::pm_auction_class_assign<<<blocks_for(T, 256), 256, 0, e->stream>>>(e->auc_sorted.p, e->auc_flag.p, e->auc_incl.p, T,
@@ -2202,6 +2250,53 @@ static bool auction_in_domain(uint32_t P, uint32_t K, uint64_t S, uint64_t E) {
 }
 
 static int auction_pass(pm_engine* e, bool want_warm, bool want_repair, bool reverse, bool* refused);
+
+// The grouped result of a pass with demands (prime_match.h "Auction demands"): the slots' held flags and their scan give
+// each ask's held count and its members' place; one group per ask holding a worker, in ask order; then each group's
+// members sorted by worker index (one segmented sort).  *G groups, *M members.
+static int auction_emit_groups(pm_engine* e, uint32_t* G, uint32_t* M) {
+  const uint32_t W = e->n_workers, T = e->n_asks, D = e->n_slots();
+  PM_CUDA(e->auc_flag.ensure((size_t)D + 1)); PM_CUDA(e->dem_spos.ensure((size_t)D + 1));
+  PM_CUDA(e->dem_aflag.ensure((size_t)T + 1)); PM_CUDA(e->auc_gidx.ensure((size_t)T + 1));
+  PM_CUDA(e->dem_members.ensure(std::max<uint32_t>(W, 1)));
+  pm::pm_auction_slot_flags<<<blocks_for((size_t)D + 1, 256), 256, 0, e->stream>>>(e->auc_assigned.p, D, e->auc_flag.p);
+  PM_LAUNCH_CHECK("pm_auction_slot_flags");
+  size_t tmp = 0, tmp2 = 0;
+  cub::DeviceScan::ExclusiveSum(nullptr, tmp, e->auc_flag.p, e->dem_spos.p, (int)(D + 1), e->stream);
+  cub::DeviceScan::ExclusiveSum(nullptr, tmp2, e->dem_aflag.p, e->auc_gidx.p, (int)(T + 1), e->stream);
+  PM_CUDA(e->cub_tmp.ensure(std::max(tmp, tmp2)));
+  tmp = e->cub_tmp.n;
+  PM_CUDA(cub::DeviceScan::ExclusiveSum(e->cub_tmp.p, tmp, e->auc_flag.p, e->dem_spos.p, (int)(D + 1), e->stream));
+  pm::pm_auction_group_counts<<<blocks_for((size_t)T + 1, 256), 256, 0, e->stream>>>(e->dem_off.p, e->dem_spos.p, e->auc_assigned.p, e->wb.p,
+                                                                                     T, e->dem_aflag.p, e->ask_best.p, e->ask_count.p);
+  PM_LAUNCH_CHECK("pm_auction_group_counts");
+  tmp = e->cub_tmp.n;
+  PM_CUDA(cub::DeviceScan::ExclusiveSum(e->cub_tmp.p, tmp, e->dem_aflag.p, e->auc_gidx.p, (int)(T + 1), e->stream));
+  PM_CUDA(cudaMemsetAsync(e->worker_group.p, 0xFF, (size_t)std::max<uint32_t>(W, 1) * 4, e->stream));
+  PM_CUDA(cudaMemsetAsync(e->worker_ask.p, 0xFF, (size_t)std::max<uint32_t>(W, 1) * 4, e->stream));
+  if (T) {
+    pm::pm_auction_group_emit<<<blocks_for(T, 256), 256, 0, e->stream>>>(e->dem_off.p, e->dem_spos.p, e->auc_gidx.p, e->auc_assigned.p, T,
+                                                                          e->worker_group.p, e->worker_ask.p, e->group_ask.p,
+                                                                          e->group_off.p, e->dem_members.p);
+    PM_LAUNCH_CHECK("pm_auction_group_emit");
+  }
+  PM_CUDA(cudaMemcpyAsync(e->h_scalars.p + 17, e->auc_gidx.p + T, 4, cudaMemcpyDeviceToHost, e->stream));
+  PM_CUDA(cudaMemcpyAsync(e->h_scalars.p + 18, e->dem_spos.p + D, 4, cudaMemcpyDeviceToHost, e->stream));
+  PM_CUDA(cudaStreamSynchronize(e->stream));
+  *G = e->h_scalars.p[17];
+  *M = e->h_scalars.p[18];
+  PM_CUDA(cudaMemcpyAsync(e->group_off.p + *G, e->h_scalars.p + 18, 4, cudaMemcpyHostToDevice, e->stream));
+  if (*G) {
+    tmp = 0;
+    cub::DeviceSegmentedRadixSort::SortKeys(nullptr, tmp, e->dem_members.p, e->members.p, (int)*M, (int)*G, e->group_off.p,
+                                            e->group_off.p + 1, 0, 32, e->stream);
+    PM_CUDA(e->cub_tmp.ensure(tmp));
+    PM_CUDA(cub::DeviceSegmentedRadixSort::SortKeys(e->cub_tmp.p, tmp, e->dem_members.p, e->members.p, (int)*M, (int)*G, e->group_off.p,
+                                                    e->group_off.p + 1, 0, 32, e->stream));
+  }
+  PM_CUDA(cudaStreamSynchronize(e->stream));   // (h_scalars is the copy's source)
+  return PM_OK;
+}
 static int match_auction_locked(pm_engine* e, uint32_t mode) {
   if (!e->have_workers || !e->have_asks) return e->fail(PM_E_STATE, "pm_match: worker and ask tables must be set first");
   if (!e->have_caps) return e->fail(PM_E_STATE, "pm_match: auction mode needs pm_set_ask_price_caps");
@@ -2225,6 +2320,9 @@ static int match_auction_locked(pm_engine* e, uint32_t mode) {
 static int auction_pass(pm_engine* e, bool want_warm, bool want_repair, bool reverse, bool* refused) {
   PM_CUDA(cudaSetDevice(e->device));
   const uint32_t W = e->n_workers, T = e->n_asks;
+  // the bidders: with demands the slots (pm_auction.cuh, "ask demands"), each ask t its own single bidder without
+  const bool dem = !e->demand.empty();
+  const uint32_t D = e->n_slots();
   if (!e->have_bits) {
     PM_CUDA(e->bits.ensure(1));
     PM_CUDA(cudaMemsetAsync(e->bits.p, 0xFF, 4, e->stream));
@@ -2235,14 +2333,26 @@ static int auction_pass(pm_engine* e, bool want_warm, bool want_repair, bool rev
   e->ev_used = 0;
   if (e->cfg.flags & PM_CFG_TIMING) PM_CUDA(cudaEventRecord(e->ev0, e->stream));
   Timer tm(e, &e->stats.ms_fused, e->stream);
+  const bool use_rep = e->have_min_rep;   // `reputation` clause: only when a floor was given
+  if (dem) {   // the slot table, from the current caps and floors: the auction's ask table
+    PM_CUDA(e->slot_ask.ensure(D)); PM_CUDA(e->slot_row.ensure(D)); PM_CUDA(e->slot_cap.ensure(D));
+    if (use_rep) PM_CUDA(e->slot_floor.ensure(D));
+    pm::pm_auction_slot_table<<<std::min(blocks_for(D, 256), 8u * e->sms), 256, 0, e->stream>>>(
+        e->dem_off.p, T, D, e->asks.p, e->price_cap.p, use_rep ? e->ask_min_rep.p : nullptr, e->slot_ask.p, e->slot_row.p,
+        e->slot_cap.p, use_rep ? e->slot_floor.p : nullptr);
+    PM_LAUNCH_CHECK("pm_auction_slot_table");
+  }
+  const uint32_t* cap_b = dem ? e->slot_cap.p : e->price_cap.p;   // per bidder
+  const uint32_t* floor_b = use_rep ? (dem ? e->slot_floor.p : e->ask_min_rep.p) : nullptr;
   if (!e->auc_classes_valid) {
-    const int rc = auction_build_classes(e);
+    const int rc = auction_build_classes(e, dem ? e->slot_row.p : e->asks.p, floor_b, D);
     if (rc != PM_OK) return rc;
   }
   const uint32_t C = e->auc_n_classes;
   const unsigned kScanGrid = 2u * e->sms;   // two scanning CTAs per SM (shared memory)
   // Warm start from the stored state when there is one and the changed rows R0 plus the changed asks A0 stay within the
-  // cutoff.  A0: caps or floors that differ from the stored ones (a diff of the host copies), and asks toggled since.
+  // cutoff.  A0: caps or floors that differ from the stored ones (a diff of the host copies), and asks toggled since,
+  // as bidders: every slot of such an ask, and the slots a demand change added to any other.
   std::vector<uint32_t> changed;   // the listed rows of R0, then A0
   bool warm = false;
   uint32_t n_kept = 0;
@@ -2250,7 +2360,10 @@ static int auction_pass(pm_engine* e, bool want_warm, bool want_repair, bool rev
     changed = e->auc_rows;
     for (uint32_t t = 0; t < T; ++t) {
       const uint32_t fl = e->have_min_rep ? e->floor_host[t] : 0u;
-      if (e->cap_host[t] != e->auc_cap_stored[t] || fl != e->auc_floor_stored[t] || e->auc_ask_mark[t]) changed.push_back(t);
+      const bool a0 = e->cap_host[t] != e->auc_cap_stored[t] || fl != e->auc_floor_stored[t] || e->auc_ask_mark[t];
+      const uint32_t s0 = e->slot0(t), s1 = e->slot0(t + 1);
+      const uint32_t kept = a0 ? 0u : e->auc_dem_kept.empty() ? s1 - s0 : std::min(e->auc_dem_kept[t], s1 - s0);
+      for (uint32_t s = s0 + kept; s < s1; ++s) changed.push_back(s);
     }
     n_kept = std::min(e->auc_kept, W);
     warm = (uint64_t)changed.size() + (W - n_kept) + e->auc_removed_held <= e->tune_incr;
@@ -2259,9 +2372,9 @@ static int auction_pass(pm_engine* e, bool want_warm, bool want_repair, bool rev
   const bool repair = want_repair && warm;   // PM_AUCTION_REPAIR: the same warm start, repaired by raising instead of releasing
   // the stored state survives the buffers' growth (a resize since the last pass); a cold pass overwrites it below
   PM_CUDA(e->auc_price.grow_keep((size_t)W + 2, e->auc_price.n, e->stream)); PM_CUDA(e->auc_owner.grow_keep(W, e->auc_owner.n, e->stream));
-  PM_CUDA(e->auc_assigned.grow_keep(T, e->auc_assigned.n, e->stream));
-  PM_CUDA(e->auc_bid_max.ensure(W)); PM_CUDA(e->auc_winner.ensure(W)); PM_CUDA(e->auc_withdrawn.ensure(T));
-  PM_CUDA(e->auc_active.ensure((size_t)2 * std::max<uint32_t>(T, 1))); PM_CUDA(e->auc_bid_w.ensure(T)); PM_CUDA(e->auc_bid_p.ensure(T));
+  PM_CUDA(e->auc_assigned.grow_keep(D, e->auc_assigned.n, e->stream));
+  PM_CUDA(e->auc_bid_max.ensure(W)); PM_CUDA(e->auc_winner.ensure(W)); PM_CUDA(e->auc_withdrawn.ensure(D));
+  PM_CUDA(e->auc_active.ensure((size_t)2 * std::max<uint32_t>(D, 1))); PM_CUDA(e->auc_bid_w.ensure(D)); PM_CUDA(e->auc_bid_p.ensure(D));
   PM_CUDA(e->auc_flag.ensure((size_t)T + 1)); PM_CUDA(e->auc_gidx.ensure((size_t)T + 1));
   PM_CUDA(e->auc_theta.ensure(C)); PM_CUDA(e->auc_theta_w.ensure(C)); PM_CUDA(e->auc_cand.ensure((size_t)C * pm::kAucCache));
   PM_CUDA(e->auc_pool.ensure((size_t)C * pm::kAucPool)); PM_CUDA(e->auc_pool_bound_v.ensure(C)); PM_CUDA(e->auc_pool_bound_w.ensure(C));
@@ -2271,9 +2384,9 @@ static int auction_pass(pm_engine* e, bool want_warm, bool want_repair, bool rev
   PM_CUDA(e->auc_split_first.ensure(kScanGrid)); PM_CUDA(e->auc_skip_key.ensure(std::max<uint32_t>(C, 1)));
   PM_CUDA(cudaMemsetAsync(e->auc_split_first.p, 0xFF, kScanGrid * 4, e->stream));
   PM_CUDA(cudaMemsetAsync(e->auc_skip_key.p, 0, (size_t)std::max<uint32_t>(C, 1) * 8, e->stream));
-  PM_CUDA(e->auc_class_req.ensure(C)); PM_CUDA(e->auc_class_list.ensure(C)); PM_CUDA(e->auc_retry.ensure(T)); PM_CUDA(e->auc_fallback.ensure(T));
+  PM_CUDA(e->auc_class_req.ensure(C)); PM_CUDA(e->auc_class_list.ensure(C)); PM_CUDA(e->auc_retry.ensure(D)); PM_CUDA(e->auc_fallback.ensure(D));
   PM_CUDA(e->auc_perm.ensure((size_t)W + 4)); PM_CUDA(e->auc_pos_of.ensure(W));
-  PM_CUDA(e->auc_idx.ensure(std::max(W, T))); PM_CUDA(e->auc_wa_s.ensure(W)); PM_CUDA(e->auc_wb_s.ensure(W)); PM_CUDA(e->auc_price_s.ensure((size_t)W + 2));
+  PM_CUDA(e->auc_idx.ensure(std::max(W, D))); PM_CUDA(e->auc_wa_s.ensure(W)); PM_CUDA(e->auc_wb_s.ensure(W)); PM_CUDA(e->auc_price_s.ensure((size_t)W + 2));
   PM_CUDA(e->auc_ctl.ensure(1)); PM_CUDA(e->h_ctl.ensure(1));
   PM_CUDA(e->worker_group.ensure(W)); PM_CUDA(e->worker_ask.ensure(W)); PM_CUDA(e->members.ensure(std::max(W, T)));
   PM_CUDA(e->group_ask.ensure((size_t)T + 1)); PM_CUDA(e->group_off.ensure((size_t)T + 2));
@@ -2282,12 +2395,12 @@ static int auction_pass(pm_engine* e, bool want_warm, bool want_repair, bool rev
   // The table limits, read back before anything of the stored state is touched: a pass outside the integer domain is
   // refused and leaves the stored state as it was.  The same read-back tells whether (value, worker) sorts as one packed
   // 64-bit key (decided on the device, read by the kernels).
-  pm::pm_auction_limits<<<std::max(1u, std::min(blocks_for(std::max(W, T), 256), 4u * e->sms)), 256, 0, e->stream>>>(e->wb.p, W, e->price_cap.p, T, e->auc_ctl.p);
+  pm::pm_auction_limits<<<std::max(1u, std::min(blocks_for(std::max(W, D), 256), 4u * e->sms)), 256, 0, e->stream>>>(e->wb.p, W, cap_b, D, e->auc_ctl.p);
   PM_LAUNCH_CHECK("pm_auction_limits");
   // (a warm pass: every price an ask kept was bid under its unchanged cap at eps = 1, every other price is 0, so the
   // bound on reachable costs is the cold one at eps = 1.  A warm repair keeps the stored prices of unowned workers too,
   // which an eps-scaled pass may have left at up to (K + 1) * S + eps_start: it is decided with eps_start.)
-  pm::pm_auction_decide_packed<<<1, 1, 0, e->stream>>>(e->auc_ctl.p, W, T, e->auc_scale, warm && !repair ? 1 : e->auc_eps_start,
+  pm::pm_auction_decide_packed<<<1, 1, 0, e->stream>>>(e->auc_ctl.p, W, D, e->auc_scale, warm && !repair ? 1 : e->auc_eps_start,
                                                        (uint32_t)e->tune_auction);
   PM_LAUNCH_CHECK("pm_auction_decide_packed");
   PM_CUDA(cudaMemcpyAsync(e->h_ctl.p, e->auc_ctl.p, sizeof(pm::AuctionCtl), cudaMemcpyDeviceToHost, e->stream));
@@ -2307,8 +2420,7 @@ static int auction_pass(pm_engine* e, bool want_warm, bool want_repair, bool rev
   PM_CUDA(cudaMemsetAsync(e->auc_price_s.p, 0, ((size_t)W + 2) * 8, e->stream));
   PM_CUDA(cudaMemsetAsync(e->auc_class_req.p, 0, (size_t)std::max<uint32_t>(C, 1) * 4, e->stream));
   PM_CUDA(e->auc_ckey.ensure(W)); PM_CUDA(e->auc_ckey_s.ensure(W));
-  // `reputation` clause: only when a floor was given; a missing worker column is a column of zeros
-  const bool use_rep = e->have_min_rep;
+  // a missing worker column is a column of zeros
   if (use_rep) {
     if (!e->have_rep) {
       PM_CUDA(e->reputation.ensure(std::max<size_t>(e->wa.n, 1)));
@@ -2320,11 +2432,12 @@ static int auction_pass(pm_engine* e, bool want_warm, bool want_repair, bool rev
   }
   pm::AuctionParams ap;
   ap.ev = eval_params(e);
+  if (dem) ap.ev.asks = e->slot_row.p;
   ap.wa_s = e->auc_wa_s.p; ap.wb_s = e->auc_wb_s.p; ap.perm = e->auc_perm.p; ap.pos_of = e->auc_pos_of.p; ap.price_s = e->auc_price_s.p;
   ap.csort_s = reinterpret_cast<const unsigned long long*>(e->auc_ckey_s.p);
-  ap.rep_s = use_rep ? e->auc_rep_s.p : nullptr; ap.min_rep = use_rep ? e->ask_min_rep.p : nullptr;
-  ap.price_cap = e->price_cap.p; ap.price = e->auc_price.p; ap.owner = e->auc_owner.p; ap.assigned = e->auc_assigned.p;
-  ap.withdrawn = e->auc_withdrawn.p; ap.active = e->auc_active.p; ap.n_asks = T; ap.bid_w = e->auc_bid_w.p; ap.bid_p = e->auc_bid_p.p;
+  ap.rep_s = use_rep ? e->auc_rep_s.p : nullptr; ap.min_rep = floor_b;
+  ap.price_cap = cap_b; ap.price = e->auc_price.p; ap.owner = e->auc_owner.p; ap.assigned = e->auc_assigned.p;
+  ap.withdrawn = e->auc_withdrawn.p; ap.active = e->auc_active.p; ap.n_asks = D; ap.bid_w = e->auc_bid_w.p; ap.bid_p = e->auc_bid_p.p;
   ap.bid_max = e->auc_bid_max.p; ap.winner = e->auc_winner.p; ap.scale = (long long)e->auc_scale;
   ap.class_of = e->auc_class_of.p; ap.class_rep = e->auc_class_rep.p; ap.class_req = e->auc_class_req.p;
   ap.cand = e->auc_cand.p; ap.theta = e->auc_theta.p; ap.theta_w = e->auc_theta_w.p;
@@ -2346,18 +2459,18 @@ static int auction_pass(pm_engine* e, bool want_warm, bool want_repair, bool rev
   pm::AuctionRev rv{};
   if (rev_on) {
     PM_CUDA(e->auc_rev_bidders.ensure(W)); PM_CUDA(e->auc_rev_offer_t.ensure(W)); PM_CUDA(e->auc_rev_offer_p.ensure(W));
-    PM_CUDA(e->auc_rev_best.ensure(T)); PM_CUDA(e->auc_rev_win.ensure(T)); PM_CUDA(e->auc_rev_pi_s.ensure(T));
-    PM_CUDA(e->auc_rev_cap_s.ensure(T)); PM_CUDA(e->auc_rev_cstart.ensure((size_t)C + 1));
+    PM_CUDA(e->auc_rev_best.ensure(D)); PM_CUDA(e->auc_rev_win.ensure(D)); PM_CUDA(e->auc_rev_pi_s.ensure(D));
+    PM_CUDA(e->auc_rev_cap_s.ensure(D)); PM_CUDA(e->auc_rev_cstart.ensure((size_t)C + 1));
     rv.bidders = e->auc_rev_bidders.p; rv.offer_t = e->auc_rev_offer_t.p; rv.offer_p = e->auc_rev_offer_p.p;
     rv.best = e->auc_rev_best.p; rv.win = e->auc_rev_win.p; rv.pi_s = e->auc_rev_pi_s.p; rv.cap_s = e->auc_rev_cap_s.p;
     rv.sorted = e->auc_sorted.p; rv.cls_s = e->auc_incl.p; rv.cstart = e->auc_rev_cstart.p;
     rv.rep = use_rep ? e->reputation.p : nullptr; rv.n_classes = C;
-    pm::pm_auction_rev_classes<<<blocks_for(T, 256), 256, 0, e->stream>>>(e->auc_sorted.p, e->auc_incl.p, e->price_cap.p, T, C,
+    pm::pm_auction_rev_classes<<<blocks_for(D, 256), 256, 0, e->stream>>>(e->auc_sorted.p, e->auc_incl.p, cap_b, D, C,
                                                                           e->auc_rev_cstart.p, e->auc_rev_cap_s.p);
     PM_LAUNCH_CHECK("pm_auction_rev_classes");
   }
   const bool rev_packed = cost_packed && !(e->tune_auction & 128);   // then no round launches pm_auction_rev_claim
-  const unsigned g_rev = std::max(1u, std::min(blocks_for(std::max(W, T), 256), 8u * e->sms));
+  const unsigned g_rev = std::max(1u, std::min(blocks_for(std::max(W, D), 256), 8u * e->sms));
   const unsigned g_rev_bid = 4u * e->sms;   // 64 registers per thread (no spills): four resident CTAs per SM
   // Release (warm start, steps 2 and 3 of DESIGN 4): the initial release and price reset, then the closure — per
   // iteration C x |R_new| predicate evaluations and one compare per still-assigned ask, one poll of the control block.
@@ -2376,7 +2489,7 @@ static int auction_pass(pm_engine* e, bool want_warm, bool want_repair, bool rev
     PM_CUDA(e->auc_chg.ensure(std::max<size_t>(changed.size(), 1)));
     if (!changed.empty()) PM_CUDA(cudaMemcpyAsync(e->auc_chg.p, changed.data(), changed.size() * 4, cudaMemcpyHostToDevice, e->stream));
     ap.eps = 1;
-    const unsigned g_seed = std::max(1u, std::min(blocks_for((size_t)T + changed.size(), 256), 8u * e->sms));
+    const unsigned g_seed = std::max(1u, std::min(blocks_for((size_t)D + changed.size(), 256), 8u * e->sms));
     pm::pm_auction_warm_seed<<<g_seed, 256, 0, e->stream>>>(ap, e->auc_chg.p, n_rows, e->auc_chg.p + n_rows, n_chg, n_kept);
     PM_LAUNCH_CHECK("pm_auction_warm_seed");
     if (rev_on) {
@@ -2397,7 +2510,7 @@ static int auction_pass(pm_engine* e, bool want_warm, bool want_repair, bool rev
     PM_CUDA(e->auc_cmin.ensure(std::max<uint32_t>(C, 1))); PM_CUDA(e->auc_chg.ensure(std::max<size_t>(changed.size(), 1)));
     if (!changed.empty()) PM_CUDA(cudaMemcpyAsync(e->auc_chg.p, changed.data(), changed.size() * 4, cudaMemcpyHostToDevice, e->stream));
     ap.eps = 1;
-    const unsigned g_seed = std::max(1u, std::min(blocks_for((size_t)T + changed.size(), 256), 8u * e->sms));
+    const unsigned g_seed = std::max(1u, std::min(blocks_for((size_t)D + changed.size(), 256), 8u * e->sms));
     pm::pm_auction_warm_seed<<<g_seed, 256, 0, e->stream>>>(ap, e->auc_chg.p, n_rows, e->auc_chg.p + n_rows, n_chg, n_kept);
     PM_LAUNCH_CHECK("pm_auction_warm_seed");
     if (W) {
@@ -2407,7 +2520,7 @@ static int auction_pass(pm_engine* e, bool want_warm, bool want_repair, bool rev
       pm::pm_auction_warm_rows<<<g_w, 256, 0, e->stream>>>(ap, e->auc_chg.p, n_rows, n_kept, e->auc_raised.p, e->auc_mark.p);
       PM_LAUNCH_CHECK("pm_auction_warm_rows");
     }
-    const unsigned g_t = std::max(1u, std::min(blocks_for(T, 256), 8u * e->sms));
+    const unsigned g_t = std::max(1u, std::min(blocks_for(D, 256), 8u * e->sms));
     const uint32_t kYChunk = 65535u * 256u;   // raised workers per launch of pm_auction_release_classes (grid.y limit)
     uint32_t lo = 0;
     for (;;) {
@@ -2454,10 +2567,10 @@ static int auction_pass(pm_engine* e, bool want_warm, bool want_repair, bool rev
   PM_CUDA(cudaFuncSetAttribute(pm::pm_auction_scan, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   // fixed grids: every kernel strides over a list whose length it reads from the control block
   const unsigned g_scan = kScanGrid;
-  const unsigned g_apply = std::max(1u, std::min(blocks_for(T, 256), e->sms));   // every CTA pays a fence + the ticket: one per SM at most
+  const unsigned g_apply = std::max(1u, std::min(blocks_for(D, 256), e->sms));   // every CTA pays a fence + the ticket: one per SM at most
   const unsigned g_refill = std::max(1u, std::min(C, 8u * e->sms));   // 12 KB of shared memory per CTA: eight per SM
-  const unsigned g_warp = std::max(1u, std::min(blocks_for(T, pm::kAucWarps), 8u * e->sms));
-  const unsigned g_thr = std::max(1u, std::min(blocks_for(T, 256), 4u * e->sms));
+  const unsigned g_warp = std::max(1u, std::min(blocks_for(D, pm::kAucWarps), 8u * e->sms));
+  const unsigned g_thr = std::max(1u, std::min(blocks_for(D, 256), 4u * e->sms));
   const uint32_t kBatch = 32;  // rounds launched between polls of the control block
   const uint32_t kResort = (e->tune_auction >> 8) ? (uint32_t)(e->tune_auction >> 8) : 4u;   // batches between re-sorts of the worker copy
   uint64_t eps = warm ? 1 : (e->auc_eps_start ? e->auc_eps_start : 1);   // a warm pass is one phase at eps = 1
@@ -2504,9 +2617,9 @@ static int auction_pass(pm_engine* e, bool want_warm, bool want_repair, bool rev
   for (;;) {  // eps phases: assignment cleared, prices (and so the class caches' bounds) kept
     if (!warm) {   // a warm pass starts from the released state: every unassigned ask is active (withdrawn ones too)
       PM_CUDA(cudaMemsetAsync(e->auc_owner.p, 0xFF, (size_t)std::max<uint32_t>(W, 1) * 4, e->stream));
-      PM_CUDA(cudaMemsetAsync(e->auc_assigned.p, 0xFF, (size_t)std::max<uint32_t>(T, 1) * 4, e->stream));
+      PM_CUDA(cudaMemsetAsync(e->auc_assigned.p, 0xFF, (size_t)std::max<uint32_t>(D, 1) * 4, e->stream));
     }
-    PM_CUDA(cudaMemsetAsync(e->auc_withdrawn.p, 0, (size_t)std::max<uint32_t>(T, 1) * 4, e->stream));
+    PM_CUDA(cudaMemsetAsync(e->auc_withdrawn.p, 0, (size_t)std::max<uint32_t>(D, 1) * 4, e->stream));
     if (C && first_phase) {  // no cache yet (on every pass, warm or cold): "invalid" sends every class to a scan
       pm::pm_fill_i64<<<std::min(blocks_for(C, 256), 8u * e->sms), 256, 0, e->stream>>>(e->auc_theta.p, pm::kThetaInvalid, C);
       pm::pm_fill_i64<<<std::min(blocks_for(C, 256), 8u * e->sms), 256, 0, e->stream>>>(e->auc_pool_bound_v.p, pm::kThetaInvalid, C);
@@ -2514,8 +2627,8 @@ static int auction_pass(pm_engine* e, bool want_warm, bool want_repair, bool rev
     }
     first_phase = false;
     ap.eps = (long long)eps;
-    if (T) {
-      pm::pm_auction_compact<<<blocks_for(T, 256), 256, 0, e->stream>>>(ap, T);
+    if (D) {
+      pm::pm_auction_compact<<<blocks_for(D, 256), 256, 0, e->stream>>>(ap, D);
       PM_LAUNCH_CHECK("pm_auction_compact");
     }
     pm::pm_auction_advance<<<1, 1, 0, e->stream>>>(e->auc_ctl.p, 1);
@@ -2608,30 +2721,36 @@ static int auction_pass(pm_engine* e, bool want_warm, bool want_repair, bool rev
   e->stats.n_build_launches = (uint32_t)std::min<unsigned long long>(e->h_ctl.p->n_refills, 0xFFFFFFFFull);
   tm.stop();
   Timer tr(e, &e->stats.ms_resolve, e->stream);
-  // result: one solo group per assigned ask, ask order
-  pm::pm_auction_flags<<<blocks_for((size_t)T + 1, 256), 256, 0, e->stream>>>(e->auc_assigned.p, T, e->auc_flag.p);
-  PM_LAUNCH_CHECK("pm_auction_flags");
-  {
-    size_t tmp = 0;
-    cub::DeviceScan::ExclusiveSum(nullptr, tmp, e->auc_flag.p, e->auc_gidx.p, (int)(T + 1), e->stream);
-    PM_CUDA(e->cub_tmp.ensure(tmp));
-    PM_CUDA(cub::DeviceScan::ExclusiveSum(e->cub_tmp.p, tmp, e->auc_flag.p, e->auc_gidx.p, (int)(T + 1), e->stream));
+  uint32_t G = 0, M = 0;
+  if (dem) {
+    const int rc = auction_emit_groups(e, &G, &M);
+    if (rc != PM_OK) return rc;
+  } else {
+    // result: one solo group per assigned ask, ask order
+    pm::pm_auction_flags<<<blocks_for((size_t)T + 1, 256), 256, 0, e->stream>>>(e->auc_assigned.p, T, e->auc_flag.p);
+    PM_LAUNCH_CHECK("pm_auction_flags");
+    {
+      size_t tmp = 0;
+      cub::DeviceScan::ExclusiveSum(nullptr, tmp, e->auc_flag.p, e->auc_gidx.p, (int)(T + 1), e->stream);
+      PM_CUDA(e->cub_tmp.ensure(tmp));
+      PM_CUDA(cub::DeviceScan::ExclusiveSum(e->cub_tmp.p, tmp, e->auc_flag.p, e->auc_gidx.p, (int)(T + 1), e->stream));
+    }
+    PM_CUDA(cudaMemsetAsync(e->worker_group.p, 0xFF, (size_t)std::max<uint32_t>(W, 1) * 4, e->stream));
+    PM_CUDA(cudaMemsetAsync(e->worker_ask.p, 0xFF, (size_t)std::max<uint32_t>(W, 1) * 4, e->stream));
+    if (T) {
+      pm::pm_auction_emit<<<blocks_for(T, 256), 256, 0, e->stream>>>(e->auc_assigned.p, e->auc_gidx.p, e->wb.p, T, e->worker_group.p,
+                                                                      e->worker_ask.p, e->group_ask.p, e->group_off.p, e->members.p,
+                                                                      e->ask_best.p, e->ask_count.p);
+      PM_LAUNCH_CHECK("pm_auction_emit");
+    }
+    PM_CUDA(cudaMemcpyAsync(e->h_scalars.p + 17, e->auc_gidx.p + T, 4, cudaMemcpyDeviceToHost, e->stream));
+    PM_CUDA(cudaStreamSynchronize(e->stream));
+    G = M = e->h_scalars.p[17];
+    PM_CUDA(cudaMemcpyAsync(e->group_off.p + G, e->h_scalars.p + 17, 4, cudaMemcpyHostToDevice, e->stream));
   }
-  PM_CUDA(cudaMemsetAsync(e->worker_group.p, 0xFF, (size_t)std::max<uint32_t>(W, 1) * 4, e->stream));
-  PM_CUDA(cudaMemsetAsync(e->worker_ask.p, 0xFF, (size_t)std::max<uint32_t>(W, 1) * 4, e->stream));
-  if (T) {
-    pm::pm_auction_emit<<<blocks_for(T, 256), 256, 0, e->stream>>>(e->auc_assigned.p, e->auc_gidx.p, e->wb.p, T, e->worker_group.p,
-                                                                    e->worker_ask.p, e->group_ask.p, e->group_off.p, e->members.p,
-                                                                    e->ask_best.p, e->ask_count.p);
-    PM_LAUNCH_CHECK("pm_auction_emit");
-  }
-  PM_CUDA(cudaMemcpyAsync(e->h_scalars.p + 17, e->auc_gidx.p + T, 4, cudaMemcpyDeviceToHost, e->stream));
-  PM_CUDA(cudaStreamSynchronize(e->stream));
-  const uint32_t G = e->h_scalars.p[17];
-  PM_CUDA(cudaMemcpyAsync(e->group_off.p + G, e->h_scalars.p + 17, 4, cudaMemcpyHostToDevice, e->stream));
   tr.stop();
   e->n_groups = G;
-  e->n_assigned = G;
+  e->n_assigned = M;
   if (e->cfg.flags & PM_CFG_TIMING) {
     PM_CUDA(cudaEventRecord(e->ev1, e->stream));
     PM_CUDA(cudaEventSynchronize(e->ev1));
@@ -2721,6 +2840,16 @@ static int cert_launch(pm_engine* e, const long long* price, const uint32_t* ass
   c.scale = e->auc_scale;
   c.n_workers = W;
   c.n_asks = T;
+  // With demands the assignment is per slot: the sweep runs per ask with no holds, and pm_auction_cert_slots checks
+  // them instead of pm_auction_cert_asks.
+  const bool dem = !e->demand.empty();
+  const uint32_t D = e->n_slots();
+  pm::CertParams cs = c;
+  if (dem) {
+    PM_CUDA(e->cert_none.ensure(std::max<uint32_t>(T, 1)));
+    PM_CUDA(cudaMemsetAsync(e->cert_none.p, 0xFF, (size_t)std::max<uint32_t>(T, 1) * 4, e->stream));
+    cs.assigned = e->cert_none.p;
+  }
   if (T && W) {   // the fused pass's predicate variant (pm_match, PM_PATH_FUSED)
     pm::EvalParams p = eval_params(e);
     int bits_mode = ((uint64_t)p.n_bits_rows * p.words <= (uint64_t)pm::kBitsCap) ? (p.words == 1 ? 2 : 1) : 0;
@@ -2735,14 +2864,21 @@ static int cert_launch(pm_engine* e, const long long* price, const uint32_t* ass
     for (uint32_t t0 = 0; t0 < T; t0 += rows_per_launch) {
       const uint32_t nt = std::min(rows_per_launch, T - t0);
       const dim3 grid(blocks_for(W, pm::kEvalCols), blocks_for(nt, pm::kEvalRows));
-#define PM_CERT_CASE(B, F) pm::pm_auction_cert_sweep<B, F><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, c, t0, nt)
+#define PM_CERT_CASE(B, F) pm::pm_auction_cert_sweep<B, F><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, cs, t0, nt)
       if (fast) { if (bits_mode == 2) PM_CERT_CASE(2, true); else if (bits_mode == 1) PM_CERT_CASE(1, true); else PM_CERT_CASE(0, true); }
       else { if (bits_mode == 2) PM_CERT_CASE(2, false); else if (bits_mode == 1) PM_CERT_CASE(1, false); else PM_CERT_CASE(0, false); }
 #undef PM_CERT_CASE
       PM_LAUNCH_CHECK("pm_auction_cert_sweep");
     }
   }
-  if (T) {
+  if (dem && T) {
+    PM_CUDA(e->slot_ask.ensure(D)); PM_CUDA(e->slot_row.ensure(D)); PM_CUDA(e->slot_cap.ensure(D));
+    pm::pm_auction_slot_table<<<std::min(blocks_for(D, 256), 8u * e->sms), 256, 0, e->stream>>>(
+        e->dem_off.p, T, D, e->asks.p, e->price_cap.p, nullptr, e->slot_ask.p, e->slot_row.p, e->slot_cap.p, nullptr);
+    PM_LAUNCH_CHECK("pm_auction_slot_table");
+    pm::pm_auction_cert_slots<<<std::min(blocks_for(D, 256), 4u * e->sms), 256, 0, e->stream>>>(c, eval_params(e), e->slot_ask.p, D);
+    PM_LAUNCH_CHECK("pm_auction_cert_slots");
+  } else if (T) {
     pm::pm_auction_cert_asks<<<std::min(blocks_for(T, 256), 4u * e->sms), 256, 0, e->stream>>>(c, e->wb.p);
     PM_LAUNCH_CHECK("pm_auction_cert_asks");
   }
@@ -2814,6 +2950,7 @@ int pm_auction_assignment(pm_engine* e, uint32_t* assigned) try {
   std::lock_guard<std::mutex> lk(e->mu);
   if (!e->auc_state) return e->fail(PM_E_STATE, "pm_auction_assignment: no auction pass since the engine's tables were last replaced");
   if (e->n_asks && !assigned) return e->fail(PM_E_INVALID, "pm_auction_assignment: null output");
+  if (!e->demand.empty()) return e->fail(PM_E_UNSUPPORTED, "pm_auction_assignment: an ask demand above 1 (the format is one worker per ask)");
   PM_CUDA(cudaSetDevice(e->device));
   if (e->n_asks) {
     PM_CUDA(cudaMemcpyAsync(assigned, e->auc_assigned.p, (size_t)e->n_asks * 4, cudaMemcpyDeviceToHost, e->stream));
@@ -2837,6 +2974,7 @@ int pm_auction_restore(pm_engine* e, const int64_t* price, uint32_t n_workers, c
     return e->fail(PM_E_STATE, "pm_auction_restore: an ask references a model pattern missing from the model table");
   if (e->cfg.shard_count || e->comm) return e->fail(PM_E_UNSUPPORTED, "pm_auction_restore: auction mode is single-GPU");
   if (e->n_off) return e->fail(PM_E_UNSUPPORTED, "pm_auction_restore: disabled asks");
+  if (!e->demand.empty()) return e->fail(PM_E_UNSUPPORTED, "pm_auction_restore: an ask demand above 1 (the format is one worker per ask)");
   const uint32_t W = e->n_workers, T = e->n_asks;
   if (n_workers != W || n_asks != T) return e->fail(PM_E_INVALID, "pm_auction_restore: one price per worker and one entry per ask");
   for (uint32_t t = 0; t < T; ++t)
@@ -2962,6 +3100,65 @@ int pm_set_ask_min_reputation(pm_engine* e, const uint32_t* min_reputation, uint
   e->auc_classes_valid = false;   // the floor is part of an ask's class
   e->matched = e->local_done = false;
   return PM_OK;
+} catch (...) { return pm_guard_rc(); }
+
+// Ask demands (north-star extension; PM_MODE_AUCTION only, prime_match.h "Auction demands").  Every check comes first
+// (a refusal changes nothing); a stored auction state is then remapped slot by slot on the device.
+int pm_set_ask_demand(pm_engine* e, const uint32_t* demand, uint32_t n_asks) try {
+  if (!e) return PM_E_INVALID;
+  std::lock_guard<std::mutex> lk(e->mu);
+  if (!e->have_asks) return e->fail(PM_E_STATE, "pm_set_ask_demand: no ask table");
+  if (n_asks != e->n_asks) return e->fail(PM_E_INVALID, "pm_set_ask_demand: one demand per ask");
+  if (n_asks && !demand) return e->fail(PM_E_INVALID, "pm_set_ask_demand: null");
+  const uint32_t T = n_asks;
+  std::vector<uint32_t> off((size_t)T + 1, 0u);
+  bool same = true;
+  for (uint32_t t = 0; t < T; ++t) {
+    if (demand[t] == 0) return e->fail(PM_E_INVALID, "pm_set_ask_demand: a demand of 0");
+    const uint64_t s = (uint64_t)off[t] + demand[t];
+    if (s >= (1u << 30)) return e->fail(PM_E_INVALID, "pm_set_ask_demand: the demands' total reaches 2^30");
+    off[t + 1] = (uint32_t)s;
+    same = same && demand[t] == (e->demand.empty() ? 1u : e->demand[t]);
+  }
+  if (same) return PM_OK;
+  ++e->table_version;
+  PM_CUDA(cudaSetDevice(e->device));
+  if (e->auc_state) {
+    const int rc = [&]() -> int {
+      const uint32_t D_old = e->n_slots(), D_new = off[T];
+      std::vector<uint32_t> old_off((size_t)T + 1);
+      for (uint32_t t = 0; t <= T; ++t) old_off[t] = e->slot0(t);
+      PM_CUDA(e->dem_off_old.ensure((size_t)T + 1)); PM_CUDA(e->dem_off.ensure((size_t)T + 1));
+      PM_CUDA(e->auc_assigned_tmp.ensure(std::max<uint32_t>(D_new, 1)));
+      PM_CUDA(cudaMemcpyAsync(e->dem_off_old.p, old_off.data(), old_off.size() * 4, cudaMemcpyHostToDevice, e->stream));
+      PM_CUDA(cudaMemcpyAsync(e->dem_off.p, off.data(), off.size() * 4, cudaMemcpyHostToDevice, e->stream));
+      PM_CUDA(cudaMemsetAsync(e->auc_assigned_tmp.p, 0xFF, (size_t)std::max<uint32_t>(D_new, 1) * 4, e->stream));
+      PM_CUDA(cudaMemsetAsync(e->counters.p + 17, 0, 4, e->stream));
+      if (D_old) {
+        pm::pm_auction_demand_remap<<<std::min(blocks_for(D_old, 256), 8u * e->sms), 256, 0, e->stream>>>(
+            e->dem_off_old.p, e->dem_off.p, T, D_old, e->auc_assigned.p, e->auc_assigned_tmp.p, e->auc_owner.p, e->auc_kept,
+            e->counters.p + 17);
+        PM_LAUNCH_CHECK("pm_auction_demand_remap");
+      }
+      PM_CUDA(cudaMemcpyAsync(e->h_scalars.p + 17, e->counters.p + 17, 4, cudaMemcpyDeviceToHost, e->stream));
+      PM_CUDA(cudaStreamSynchronize(e->stream));   // (old_off and off are locals)
+      std::swap(e->auc_assigned, e->auc_assigned_tmp);
+      e->auc_removed_held += e->h_scalars.p[17];
+      if (e->auc_dem_kept.empty())
+        for (uint32_t t = 0; t < T; ++t) e->auc_dem_kept.push_back(old_off[t + 1] - old_off[t]);
+      for (uint32_t t = 0; t < T; ++t) e->auc_dem_kept[t] = std::min(e->auc_dem_kept[t], demand[t]);
+      return PM_OK;
+    }();
+    if (rc != PM_OK) {
+      e->auc_discard();
+      return rc;
+    }
+  }
+  e->demand.assign(demand, demand + T);
+  e->dem_off_h = std::move(off);
+  e->auc_classes_valid = false;   // the auction's classes are built over the slots
+  e->matched = e->local_done = false;
+  return upload_demand(e);
 } catch (...) { return pm_guard_rc(); }
 
 int pm_set_auction_params(pm_engine* e, uint64_t cost_scale, uint64_t eps_start, uint32_t eps_div) try {

@@ -236,6 +236,12 @@ class Engine:
         floors = np.ascontiguousarray(floors, dtype=np.uint32)
         self._check(self._lib.pm_set_ask_min_reputation(self._h, _ptr(floors), len(floors)))
 
+    def set_ask_demand(self, demand: np.ndarray):
+        """Workers each ask may take in PM_MODE_AUCTION (pm_set_ask_demand; u32 >= 1 per ask, default 1): ask t behaves as
+        its row repeated demand[t] times, and the result holds one group per ask with its workers."""
+        demand = np.ascontiguousarray(demand, dtype=np.uint32)
+        self._check(self._lib.pm_set_ask_demand(self._h, _ptr(demand), len(demand)))
+
     def set_auction_params(self, cost_scale: int = 1, eps_start: int = 1, eps_div: int = 4):
         self._check(self._lib.pm_set_auction_params(self._h, cost_scale, eps_start, eps_div))
 
