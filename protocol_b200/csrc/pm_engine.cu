@@ -2902,11 +2902,11 @@ int pm_auction_certificate(pm_engine* e, pm_auction_cert* out, int64_t* ask_boun
   if (e->max_pattern_row > e->n_patterns || (e->max_pattern_row && !e->have_bits))
     return e->fail(PM_E_STATE, "pm_auction_certificate: an ask references a model pattern missing from the model table");
   if (e->n_off) return e->fail(PM_E_UNSUPPORTED, "pm_auction_certificate: disabled asks");
+  KeepStats keep_stats{e, e->stats};   // before the rows go to the auction's form: that launch is no pass's either
   {
     const int rc = use_ask_form(e, true);
     if (rc != PM_OK) return rc;
   }
-  KeepStats keep_stats{e, e->stats};
   PM_CUDA(cudaSetDevice(e->device));
   if (ask_bound) PM_CUDA(e->h_cert_bound.ensure(std::max<uint32_t>(T, 1)));
   pm::CertParams c;
@@ -2986,11 +2986,11 @@ int pm_auction_restore(pm_engine* e, const int64_t* price, uint32_t n_workers, c
   for (uint32_t w = 0; w < W; ++w)
     if (price[w] < 0 || (unsigned __int128)price[w] > p_max)
       return e->fail(PM_E_INVALID, "pm_auction_restore: price outside [0, (max cap + 1) * cost_scale + eps_start]");
+  KeepStats keep_stats{e, e->stats};   // before the rows go to the auction's form: that launch is no pass's either
   {
     const int rc = use_ask_form(e, true);
     if (rc != PM_OK) return rc;
   }
-  KeepStats keep_stats{e, e->stats};
   PM_CUDA(cudaSetDevice(e->device));
   // the stored buffers at their pass sizes, their contents kept (a refusal below leaves the stored state as it was)
   PM_CUDA(e->auc_price.grow_keep((size_t)W + 2, e->auc_price.n, e->stream)); PM_CUDA(e->auc_owner.grow_keep(W, e->auc_owner.n, e->stream));

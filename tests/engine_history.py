@@ -20,6 +20,22 @@ restated from the header and DESIGN §4-§6b:
       resized (the certificate waits for the next pass); pm_set_asks, pm_set_model_table, pm_set_worker_count and
       pm_set_auction_params discard it; a refused auction pass keeps it; reference-mode passes and certificates leave
       it alone.
+  ask demands (pm_set_ask_demand, "Auction demands"): ask t with demand d[t] is d[t] slots, the rows of the twin table
+      that repeats row t d[t] times; the stored assignment, A0 and the warm and repair checkers are over slots.
+      pm_set_asks resets every demand to 1, pm_update_asks keeps a replaced row's demand (all its slots join A0), an
+      append adds asks of demand 1 (empty slots in A0), a shrink drops the removed asks' demands and counts the held
+      workers of their slots below n_kept in removed_held.  A demand change under a stored state keeps each ask's first
+      min(old, new) slots; over several changes before one pass the slots kept are the minimum over the chain
+      (`dem_kept`); a removed slot's worker is unowned at its stored price and counts in removed_held when it lies below
+      n_kept; the other slots are in A0.  The warm decision counts |R0| + (W - n_kept) + |A0 in slots| + removed_held.
+      A demand change touches neither the reference tracker nor the fast / narrow facts; a refused one changes nothing.
+  restore (pm_auction_assignment / pm_auction_restore, "Auction state restore"): the export is the stored assignment
+      over the current asks and the stored pass's prices; a restore is refused while a demand exceeds 1 or an ask is
+      disabled (PM_E_UNSUPPORTED), for a missing pattern (PM_E_STATE), for lengths other than W and T, a worker >= W, a
+      price outside [0, (K + 1) S + max(E, 1)] or tables outside the integer domain (PM_E_INVALID), and changes nothing
+      then; else the stored state is auction_restore_checker.audit of the given one, with no change since it (R0, A0,
+      removed_held and the resize flag cleared, auc_w = W), warm 0, released 0 and reverse stats 0.  The reference
+      tracker, pm_fetch_result and pm_table_version stay.
 
 Ask rows referencing a model pattern the model table lacks make every pass, auction pass, certificate and cost tile
 return PM_E_STATE while they are in the table, enabled or not.
@@ -35,6 +51,8 @@ import os
 
 import numpy as np
 
+import auction_demand as ad
+import auction_restore_checker as rs
 import auction_warm_checker as wc
 from oracle import pm_oracle as orc
 from protocol_b200 import abi, synth
@@ -58,14 +76,24 @@ AUCTION = ("auction", "reverse", "warm", "repair")
 PASSES = REFERENCE + AUCTION + ("certificate",)
 CALLS = ("update", "set_flags", "upsert", "grow", "shrink", "reputation", "caps", "floors", "ask_off", "ask_on",
          "locations", "addr_rank", "set_asks", "model_table", "auction_params", "set_workers", "update_asks",
-         "append_asks", "shrink_asks", "ask_delta_refused")
-RARE = ("set_asks", "model_table", "auction_params", "set_workers", "ask_delta_refused")
+         "append_asks", "shrink_asks", "ask_delta_refused", "demand", "demand_refused", "restore", "restore_refused",
+         "move")
+RARE = ("set_asks", "model_table", "auction_params", "set_workers", "ask_delta_refused", "demand_refused",
+        "restore_refused", "move")
 ASK_DELTAS = ("update_asks", "append_asks", "shrink_asks")
+# auction-only calls: no pm_multi_ form, and nothing a reference pass reads
+AUCTION_CALLS = ("demand", "demand_refused", "restore", "restore_refused", "move")
 REFUSALS = ("auction_disabled", "auction_domain", "auction_incremental", "proximity_max0", "certificate_no_state",
             "certificate_resized", "certificate_disabled", "certificate_asks_resized", "pattern_missing",
-            "ask_delta_refused")
+            "ask_delta_refused", "demand_refused", "restore_refused")
 # the PM_E_INVALID cases of pm_update_asks / pm_resize_asks (each changes nothing, pm_table_version included)
 DELTA_REFUSALS = ("index", "sizes", "range", "grow_without_rows", "grow_bad_range", "too_many")
+# the PM_E_INVALID cases of pm_set_ask_demand (each changes nothing, pm_table_version included)
+DEMAND_REFUSALS = ("length", "zero", "total", "null")
+# refused exports and restores: (case, statuses of the restore); "demand", "no_state" also try the export
+RESTORE_REFUSALS = ("length_w", "length_t", "worker", "price_neg", "price_high", "demand", "disabled", "missing",
+                    "domain", "export_demand", "export_no_state")
+RESTORE_VARIANTS = ("own", "stale", "adversarial", "resized")
 EDGE_ASKS = ("max0", "min0", "no_opts", "big_cpu", "none", "missing")
 GROUPS = [(1, 1), (2, 3), (3, 5), (4, 4), (2, 8)]
 PARAMS = [(1, 1, 4), (1, 64, 4), (3, 1, 4)]
@@ -260,9 +288,13 @@ class History(AskMarket):
         self.dropped = 0                    # stored first asks an ask shrink set to NONE since it
         self.eval_facts = None              # (workers_small, prices_narrow, asks_small) at the stored evaluation
         self.flipped = set()                # which of the facts changed since the stored evaluation
-        # auction tracker (A0 is AskMarket's `toggled`)
+        # auction tracker (A0 is AskMarket's `toggled`, over asks; changed_slots() spreads it over slots)
         self.auc_state, self.auc_w, self.auc_over = False, 0, False
         self.resized = False                # an ask resize since the stored state
+        self.d = np.ones(len(self.asks), dtype=np.uint32)
+        self.d_pass = self.d.copy()
+        self.last_report = None             # the report of the last successful restore
+        self.outcomes = {}                  # generate(): event index -> an auction pass's prediction or restore report
 
     # ---- facts
     def facts(self):
@@ -306,6 +338,130 @@ class History(AskMarket):
         self.auc_state, self.auc_over, self.resized = False, False, False
         self.store(None, None)
 
+    # ---- slots (the twin table: row t repeated d[t] times)
+    def store(self, price, assigned):
+        super().store(price, assigned)
+        self.dem_kept = None                # the leading slots of each ask a demand change kept (None: all)
+        if hasattr(self, "d"):
+            self.d_pass = self.d.copy()     # the demands at the stored state (cut and extended with the asks)
+
+    def slot_F(self, F=None):
+        return np.repeat(self.F() if F is None else F, self.d, axis=0)
+
+    def slot_cap(self):
+        return np.repeat(self.cap, self.d)
+
+    def slot_floors(self):
+        return np.repeat(self.floors_or_zero(), self.d)
+
+    def held_asks(self):
+        """The asks holding at least one worker in the stored state."""
+        if not self.auc_state or self.assigned is None:
+            return np.zeros(0, dtype=np.int64)
+        if len(self.d) == 0:
+            return np.zeros(0, dtype=np.int64)
+        return np.flatnonzero(np.add.reduceat((self.assigned != NONE).astype(np.int64), ad.offsets(self.d)[:-1]))
+
+    def kept_slots(self):
+        """Per ask the leading slots that keep their stored hold at the next warm pass: 0 for an ask of A0."""
+        kept = self.d.astype(np.int64) if self.dem_kept is None else np.minimum(self.dem_kept, self.d).astype(np.int64)
+        kept[self.changed_asks()] = 0
+        return kept
+
+    def changed_slots(self):
+        """A0 over slots: every slot of an ask of A0, and the slots past each ask's kept ones."""
+        off = ad.offsets(self.d)
+        k = np.arange(off[-1]) - np.repeat(off[:-1], self.d)
+        return np.flatnonzero(k >= np.repeat(self.kept_slots(), self.d)).tolist()
+
+    def n_changes(self):
+        return len(self.rows) + (self.n_workers - self.n_kept) + len(self.changed_slots()) + self.removed_held
+
+    def _freed(self, gone):
+        """The workers of removed slots that count against the cutoff: those below n_kept."""
+        gone = np.asarray(gone)
+        return int(((gone != NONE) & (gone < self.n_kept)).sum())
+
+    def _slot_freed(self, gone):
+        """The workers of the slots a demand change removed that count against the cutoff."""
+        return self._freed(gone)
+
+    def _kept_after(self, new):
+        """The slots kept over the chain of demand changes since the stored state."""
+        return np.minimum(self.d if self.dem_kept is None else self.dem_kept, new)
+
+    def _free_price(self, workers):
+        """A removed slot's worker is unowned at its stored price: nothing to do."""
+
+    def set_demand(self, new):
+        new = np.asarray(new, dtype=np.uint32)
+        if np.array_equal(new, self.d):     # the same demands: nothing changes
+            return
+        if self.auc_state:
+            o_old, o_new = ad.offsets(self.d), ad.offsets(new)
+            a, _, _ = ad.remap(self.assigned, self.d, new)
+            gone = np.concatenate([self.assigned[o_old[t] + min(int(self.d[t]), int(new[t])):o_old[t + 1]]
+                                   for t in range(len(new))] or [np.zeros(0, np.uint32)])
+            gone = gone[gone != NONE]
+            self.removed_held += self._slot_freed(gone)
+            self._free_price(gone)
+            self.dem_kept = self._kept_after(new)
+            self.assigned = a
+            assert len(a) == int(o_new[-1])
+        self.d = new.copy()
+
+    # ---- restore
+    def export_refusal(self):
+        st = set()
+        if not self.auc_state:
+            st.add(abi.PM_E_STATE)
+        if (self.d > 1).any():
+            st.add(abi.PM_E_UNSUPPORTED)
+        return st
+
+    def export(self):
+        """(prices of the stored pass's rows, the stored assignment over the current asks)."""
+        return self.price.copy(), self.assigned.copy()
+
+    def restore_refusal(self, price, assigned):
+        """The statuses a restore of (price, assigned) may return, or an empty set when it must succeed."""
+        st = set()
+        W, T = self.n_workers, len(self.asks)
+        price, assigned = np.asarray(price, dtype=np.int64), np.asarray(assigned, dtype=np.uint32)
+        if self.pattern_missing():
+            st.add(abi.PM_E_STATE)
+        if not self.mask.all() or (self.d > 1).any():
+            st.add(abi.PM_E_UNSUPPORTED)
+        S, E, _ = self.params
+        top = rs.price_bound(self.cap, S, E)
+        if len(price) != W or len(assigned) != T or ((assigned != NONE) & (assigned >= W)).any() \
+                or (price < 0).any() or (price > top).any() or not in_domain(self.wb, self.cap, self.params):
+            st.add(abi.PM_E_INVALID)
+        return st
+
+    def _restore_clear(self, price, kept):
+        self.store(price, kept)
+
+    def restore(self, price, assigned):
+        """A successful restore: the audited state is the stored one, nothing changed since it.  Returns the report."""
+        price = np.array(price, dtype=np.int64)
+        out = rs.audit(self.F(), self.wb["ext_ask_price"], self.cap, self.params[0], price, assigned)
+        self._restore_clear(price, out["assigned"])
+        self.auc_state, self.auc_w, self.auc_over, self.resized = True, self.n_workers, False, False
+        self.last_report = {k: out[k] for k in ("n_held", "n_dropped_bad", "n_dropped_shared", "n_dropped_slack", "evals")}
+        return {k: out[k] for k in ("n_held", "n_dropped_bad", "n_dropped_shared", "n_dropped_slack", "evals")}
+
+    def fit(self, price, assigned):
+        """A state trimmed to the current tables: prices cut or zero-padded to W, holds >= W dropped, the assignment
+        cut or padded with PM_NONE to T."""
+        W, T = self.n_workers, len(self.asks)
+        p = np.zeros(W, dtype=np.int64)
+        p[:min(W, len(price))] = np.asarray(price, dtype=np.int64)[:W]
+        a = np.full(T, NONE, dtype=np.uint32)
+        a[:min(T, len(assigned))] = np.asarray(assigned, dtype=np.uint32)[:T]
+        a[(a != NONE) & (a >= W)] = NONE
+        return p, a
+
     def e_rows(self, en):
         """|E| x W / T rounded up: what the E-pass counts against the cutoff (the current T)."""
         T = len(self.asks)
@@ -342,14 +498,28 @@ class History(AskMarket):
         k, T = len(rows), len(self.asks)
         if self.eval:
             self.appended |= set(range(T, T + k))
-        self.append(rows)
+        self.append(rows)                   # the new asks have demand 1: one empty slot each, in A0
+        self.d = np.concatenate([self.d, np.ones(k, dtype=np.uint32)])
+        self.d_pass = np.concatenate([self.d_pass, np.ones(k, dtype=np.uint32)])
+        if self.dem_kept is not None:
+            self.dem_kept = np.concatenate([self.dem_kept, np.ones(k, dtype=self.dem_kept.dtype)])
         self.mask = np.concatenate([self.mask, np.ones(k, dtype=bool)])
         self.eval_mask = np.concatenate([self.eval_mask, np.zeros(k, dtype=bool)])
         self.resized |= self.auc_state
         self._note_facts()
 
     def shrink_asks(self, n):
+        n_slots = int(ad.offsets(self.d)[n])
+        a = self.assigned
+        if a is not None:                   # the removed asks' slots: their held workers below n_kept count
+            self.removed_held += self._freed(a[n_slots:])
+            self.assigned = None
         self.shrink(n)
+        if a is not None:
+            self.assigned = a[:n_slots].copy()
+        self.d, self.d_pass = self.d[:n].copy(), self.d_pass[:n].copy()
+        if self.dem_kept is not None:
+            self.dem_kept = self.dem_kept[:n].copy()
         self.mask, self.eval_mask = self.mask[:n].copy(), self.eval_mask[:n].copy()
         self.replaced = {t for t in self.replaced if t < n}
         self.appended = {t for t in self.appended if t < n}
@@ -483,12 +653,25 @@ class History(AskMarket):
         elif name == "shrink_asks":
             if x["n"] != len(self.asks):    # pm_resize_asks to the current size changes nothing
                 self.shrink_asks(x["n"])
-        elif name == "ask_delta_refused":   # PM_E_INVALID: nothing changes
+        elif name in ("ask_delta_refused", "demand_refused", "restore_refused"):   # refused: nothing changes
             pass
+        elif name == "demand":
+            self.set_demand(x["d"])
+        elif name == "restore":
+            self.last_report = None
+            for price, assigned in x["attempts"]:   # the first one the engine takes
+                if not self.restore_refusal(price, assigned):
+                    self.restore(price, assigned)
+                    break
+        elif name == "move":                # a fresh engine with no stored evaluation takes the state
+            price, assigned = x["fit"]
+            self.restore(price, assigned)
+            self.discard_eval()
         elif name == "set_asks":
             self.ask_table = x["table"]
             self.asks = self.s["asks"][x["table"]].copy()
             self.mask = np.ones(len(self.asks), dtype=bool)
+            self.d = np.ones(len(self.asks), dtype=np.uint32)
             self.cap, self.floors = x["cap"].copy(), x["floors"].copy()
             self.eval_mask = self.mask.copy()
             self.discard_eval()
@@ -552,6 +735,12 @@ def drive(eng, ev):
         eng.resize_asks(x["n"])
     elif name == "ask_delta_refused":
         refuse_delta(eng, x)
+    elif name == "demand":
+        eng.set_ask_demand(x["d"])
+    elif name == "demand_refused":
+        refuse_demand(eng, x)
+    elif name in ("restore", "restore_refused", "move"):
+        raise ValueError(f"{name}: the runner sends it (it checks the export and the report)")
     elif name == "set_asks":
         s = x["setup"]
         eng.set_asks(s["asks"][x["table"]], s["opts"])
@@ -605,20 +794,52 @@ def refuse_delta(eng, x):
     assert getattr(eng, "n_asks", T) == T, (x["case"], "n_asks changed")
 
 
-def load(eng, h: History):
-    """Load an engine with the mirror's current tables (a fresh engine's start, or the start of a history)."""
+def refuse_demand(eng, x):
+    """One PM_E_INVALID case of pm_set_ask_demand: the call is refused and pm_table_version stays."""
+    import ctypes
+
+    from protocol_b200._lib import PrimeMatchError
+
+    T = x["T"]
+    d = np.ones(T, dtype=np.uint32)
+    v = eng.table_version()
+    if x["case"] == "null":     # a NULL pointer with n_asks > 0
+        rc = eng._lib.pm_set_ask_demand(eng._h, ctypes.c_void_p(None), T)
+        assert rc == abi.PM_E_INVALID, ("null", rc)
+    else:
+        if x["case"] == "length":
+            d = np.ones(T + (1 if T % 2 else -1), dtype=np.uint32)
+        elif x["case"] == "zero":
+            d[T // 2] = 0
+        elif x["case"] == "total":   # D >= 2^30
+            d[-1] = (1 << 30) - (T - 1)
+        try:
+            eng.set_ask_demand(d)
+        except PrimeMatchError as ex:
+            assert ex.status == abi.PM_E_INVALID, (x["case"], ex.status)
+        else:
+            raise AssertionError(f"demand {x['case']}: accepted")
+    assert eng.table_version() == v, (x["case"], "pm_table_version changed")
+
+
+def load(eng, h: History, twin=False):
+    """Load an engine with the mirror's current tables (a fresh engine's start, or the start of a history), demands
+    included; twin: the twin tables instead (every ask row, cap and floor repeated d[t] times, every demand 1)."""
     s = h.s
-    eng.set_asks(h.asks, h.opts)
+    eng.set_asks(np.repeat(h.asks, h.d) if twin else h.asks, h.opts)
+    if (h.d != 1).any() and not twin:
+        eng.set_ask_demand(h.d)
     eng.set_model_table(s["bits"][h.bits_table], s["npat"], s["nmod"], s["words"])
     eng.set_workers(h.wa, h.wb)
     eng.set_locations(h.lat, h.lon)
     eng.set_addr_rank(h.rank)
-    eng.set_price_caps(h.cap)
+    eng.set_price_caps(h.slot_cap() if twin else h.cap)
     eng.set_worker_reputation(h.reputation)
-    eng.set_min_reputation(h.floors_or_zero())
+    eng.set_min_reputation(h.slot_floors() if twin else h.floors_or_zero())
     S, E, d = h.params
     eng.set_auction_params(cost_scale=S, eps_start=E, eps_div=d)
     if not h.mask.all():
+        assert not twin
         eng.set_ask_enabled(np.flatnonzero(~h.mask), False)
 
 
@@ -630,6 +851,7 @@ class Gen:
         self.h, self.rng = h, rng
         s = h.s
         self.pool_a, self.pool_b = s["wa"], s["wb"]
+        self.saved = None                   # a state exported earlier (the stale restore's)
 
     def rows(self, n):
         """n rows: copies of the first table's rows with flags flipped, other counts, models and prices, and sometimes
@@ -716,7 +938,7 @@ class Gen:
     def held_asks(self):
         """Asks holding a worker in the stored auction state, and asks that are many workers' stored first ask."""
         h = self.h
-        held = np.flatnonzero(h.assigned != NONE) if h.auc_state and h.assigned is not None else np.zeros(0, np.int64)
+        held = h.held_asks()
         first = np.zeros(0, dtype=np.int64)
         if h.eval and h.eval_ff is not None:
             ff = h.eval_ff[h.eval_ff != NONE].astype(np.int64)
@@ -833,6 +1055,35 @@ class Gen:
         if name == "auction_params":
             choices = [p for p in PARAMS if p != h.params]
             return ("auction_params", dict(params=choices[int(rng.integers(0, len(choices)))]))
+        if name == "demand":
+            d = h.d.copy()
+            r = rng.random()
+            if r < 0.12:
+                d[:] = 1
+            elif r < 0.2:
+                d[int(rng.integers(0, T))] = int(rng.integers(20, 120))      # one large demand
+            else:                                                            # held asks and unheld ones, 1..4
+                held = h.held_asks()
+                free = np.setdiff1d(np.arange(T), held)
+                idx = [rng.choice(p, min(len(p), int(rng.integers(1, 5))), replace=False) for p in (held, free) if len(p)]
+                idx = np.concatenate(idx).astype(np.int64)
+                d[idx] = rng.integers(1, 5, len(idx))
+            return ("demand", dict(d=d.astype(np.uint32)))
+        if name == "demand_refused":
+            return ("demand_refused", dict(T=T, case=DEMAND_REFUSALS[int(rng.integers(0, len(DEMAND_REFUSALS)))]))
+        if name == "restore":
+            own = h.auc_state and not h.export_refusal()
+            variants = ["adversarial"] + (["own", "own"] if own else []) + (["stale"] if self.saved is not None else [])
+            return self.restore(variants[int(rng.integers(0, len(variants)))])
+        if name == "restore_refused":
+            cases = ["length_w", "length_t", "worker", "price_neg", "price_high"]
+            cases += ["demand"] if (h.d > 1).any() else []
+            cases += ["disabled"] if not h.mask.all() else []
+            cases += ["export_no_state"] if not h.auc_state else ["export_demand"] if (h.d > 1).any() else []
+            return self.restore_refused(cases[int(rng.integers(0, len(cases)))])
+        if name == "move":
+            raw = h.export()
+            return ("move", dict(export=raw, fit=h.fit(*raw)))
         if name == "set_workers":
             n = int(rng.integers(W - 40, W + 40))
             a, b = self.rows(n)
@@ -840,6 +1091,48 @@ class Gen:
             return ("set_workers", dict(a=a, b=b, lat=la, lon=lo, rank=rng.permutation(n).astype(np.uint32),
                                         rep=rng.integers(0, 4, n).astype(np.uint32)))
         raise ValueError(name)
+
+
+    def restore(self, variant):
+        """A restore into the same engine: the own state as exported (after a worker resize: refused, then trimmed),
+        a state exported earlier, or adversarial_state on the current tables."""
+        h, rng = self.h, self.rng
+        if variant in ("own", "resized") and (not h.auc_state or h.export_refusal()) \
+                or variant == "stale" and self.saved is None:
+            variant = "adversarial"             # nothing to export
+        x = dict(variant=variant, export=None)
+        if variant in ("own", "resized"):
+            x["variant"] = "own" if h.n_workers == h.auc_w else "resized"
+            x["export"] = raw = h.export()
+            self.saved = raw
+            x["attempts"] = [raw] if h.n_workers == h.auc_w else [raw, h.fit(*raw)]
+        elif variant == "stale":
+            p, a = h.fit(*self.saved)
+            x["attempts"] = [(p, a), (np.minimum(p, rs.price_bound(h.cap, h.params[0], h.params[1])), a)]
+        else:
+            x["attempts"] = [rs.adversarial_state(h.F(), h.wb["ext_ask_price"], h.cap, h.params[0], rng, h.params[1])]
+        return ("restore", x)
+
+    def restore_refused(self, case):
+        """One refused export or restore: a corrupted state, or a valid one while the tables refuse it."""
+        h = self.h
+        W, T = h.n_workers, len(h.asks)
+        if h.auc_state:
+            p, a = h.fit(*h.export()) if not (h.d > 1).any() else (np.zeros(W, np.int64), np.full(T, NONE, np.uint32))
+        else:
+            p, a = np.zeros(W, dtype=np.int64), np.full(T, NONE, dtype=np.uint32)
+        p, a = p.copy(), a.copy()
+        if case == "length_w":
+            p = np.zeros(W + 1 if self.rng.random() < 0.5 else W - 1, dtype=np.int64)
+        elif case == "length_t":
+            a = np.full(T + 1, NONE, dtype=np.uint32)
+        elif case == "worker":
+            a[int(self.rng.integers(0, T))] = W
+        elif case == "price_neg":
+            p[int(self.rng.integers(0, W))] = -1
+        elif case == "price_high":
+            p[int(self.rng.integers(0, W))] = rs.price_bound(h.cap, h.params[0], h.params[1]) + 1
+        return ("restore_refused", dict(case=case, price=p, assigned=a, export=case.startswith("export")))
 
 
 ALL_PAIRS = [(c, k) for c in CALLS for k in PASSES]
@@ -865,14 +1158,33 @@ def generate(shape, seed, n_calls=N_CALLS, cutoff=DEFAULT_CUTOFF, slot=0, n_slot
         events.append(("call", ev))
         if observe is not None:
             observe(h, events[-1], True)
+        if ev[0] == "restore_refused":
+            assert h.restore_refusal(ev[1]["price"], ev[1]["assigned"]) or ev[1]["export"], ev[1]["case"]
+            assert not ev[1]["export"] or h.export_refusal(), ev[1]["case"]
         h.apply(ev)
+        if ev[0] in ("restore", "move"):
+            h.outcomes[len(events) - 1] = h.last_report
         calls_since.append(ev[0])
         if observe is not None:
             observe(h, events[-1], False)
-        if ev[0] == "ask_delta_refused" and not follow:   # what it left: the next incremental and warm passes show it
-            follow.extend(["lean_incr", "warm"])
+        if ev[0] in ("ask_delta_refused", "demand_refused", "restore_refused") and not follow:
+            follow.extend(["lean_incr", "warm"])     # what it left: the next incremental and warm passes show it
         if ev[0] in ASK_DELTAS and len(h.asks) and rng.random() < 0.25:
             probe()
+
+    def emit_named(c):
+        """g.call(c), after the calls a restore or a move needs to be taken (all asks on, every demand 1, a stored
+        state within the price bound); a move that still cannot be taken is a restore."""
+        if c in ("restore", "move") and rng.random() < 0.85:
+            all_on()
+            if (h.d > 1).any():
+                emit_call(("demand", dict(d=np.ones(len(h.asks), dtype=np.uint32))))
+        if c == "move":
+            if not h.auc_state and not h.refusal("auction")[0]:
+                emit_pass("auction")
+            if not h.auc_state or h.export_refusal() or h.restore_refusal(*h.fit(*h.export())):
+                c = "restore"
+        emit_call(g.call(c))
 
     def probe():
         T = len(h.asks)
@@ -890,8 +1202,10 @@ def generate(shape, seed, n_calls=N_CALLS, cutoff=DEFAULT_CUTOFF, slot=0, n_slot
         if kind in REFERENCE:
             h.reference_done(why is None)
         elif kind in AUCTION and why is None:   # the checkers' state: later writes can aim at the held rows
-            a, p, _, _, _ = expect_auction(h, kind, h.warm_plan()[0] if kind in ("warm", "repair") else False)
-            h.auction_done(p, a)
+            warm = h.warm_plan()[0] if kind in ("warm", "repair") else False
+            out = expect_auction(h, kind, warm)
+            h.outcomes[len(events) - 1] = (warm,) + out
+            h.auction_done(out[1], out[0])
         if why is not None and not follow:   # what the refusal kept: the next incremental and warm passes show it
             follow.extend(["lean_incr", "warm"])
         if kind != "auction_incr":          # the refused flag combination is no pass of any kind
@@ -952,13 +1266,9 @@ def generate(shape, seed, n_calls=N_CALLS, cutoff=DEFAULT_CUTOFF, slot=0, n_slot
             done.add("missing")
             t = np.array([int(rng.integers(0, T))], dtype=np.uint32)
             emit_call(g.delta("update_asks", s["edge"][5 + slot % 2:6 + slot % 2].copy(), idx=t))
+            emit_call(g.restore_refused("missing"))
             emit_pass(["lean_incr", "auction", "certificate", "warm"][slot % 4])
             return True
-        def cut_held(j):                 # past the last j asks that hold a worker (at most 20 asks)
-            held = np.flatnonzero(h.assigned != NONE) if h.auc_state else np.zeros(0, dtype=np.int64)
-            k = len(h.asks) - int(held[-j]) if len(held) >= j else 3
-            emit_call(("shrink_asks", dict(n=len(h.asks) - min(max(k, 1), 20))))
-
         if n_passes >= 28 and h.cutoff < 1000 and "removed_held" not in done:
             # the removed asks that held a worker decide the cutoff: shrink past held asks, then write (unchanged) kept
             # rows until the changes without them reach the cutoff and with them pass it; a warm pass, then a repair
@@ -991,6 +1301,10 @@ def generate(shape, seed, n_calls=N_CALLS, cutoff=DEFAULT_CUTOFF, slot=0, n_slot
             emit_call(g.delta("append_asks", g.ask_rows(2, missing=False), n=len(h.asks) + 2, cap=None))
             emit_pass("certificate")        # refused: the ask table was resized since the last auction pass
             return True
+        n0 = len(events)
+        if scripted_demand(n_passes):       # on top of the history's length
+            extra[0] += len([e for e in events[n0:] if e[0] != "probe"])
+            return True
         if n_passes >= 24 and h.cutoff < 1000 and "e_rows" not in done:
             # appended asks alone past the cutoff: e_rows = ceil(|E| W / T) > PM_TUNE_INCR
             done.add("e_rows")
@@ -999,6 +1313,185 @@ def generate(shape, seed, n_calls=N_CALLS, cutoff=DEFAULT_CUTOFF, slot=0, n_slot
             emit_call(g.delta("append_asks", g.ask_rows(k, missing=False), n=len(h.asks) + k, cap=None))
             emit_pass("lean_incr")
             emit_call(("shrink_asks", dict(n=len(h.asks) - k)))
+            emit_pass("lean_incr")          # the workers whose stored first ask was appended have none now
+            return True
+        return False
+
+    def cut_held(j):                     # past the last j asks that hold a worker (at most 20 asks)
+        held = h.held_asks()
+        k = len(h.asks) - int(held[-j]) if len(held) >= j else 3
+        emit_call(("shrink_asks", dict(n=len(h.asks) - min(max(k, 1), 20))))
+
+    def demand_held(k, value):
+        """Demand `value` on up to k asks that hold a worker (others when fewer hold one)."""
+        d = h.d.copy()
+        held = h.held_asks()
+        pool = held if len(held) else np.arange(len(h.asks))
+        idx = rng.choice(pool, min(k, len(pool)), replace=False)
+        d[idx] = value
+        emit_call(("demand", dict(d=d)))
+        return idx
+
+    def write_unchanged(n):
+        """n unchanged kept rows no change lists yet (R0 grows by n, nothing else changes)."""
+        free = np.setdiff1d(np.arange(h.n_kept), sorted(h.rows))
+        u = np.sort(rng.choice(free, max(0, n), replace=False)).astype(np.uint32)
+        if len(u):
+            emit_call(("update", dict(idx=u, a=h.wa[u].copy(), b=h.wb[u].copy(), lat=None, lon=None)))
+
+    def ones():
+        if (h.d > 1).any():
+            emit_call(("demand", dict(d=np.ones(len(h.asks), dtype=np.uint32))))
+
+    def slot_state(k=8, value=3):
+        """A stored state with demand `value` on asks that held a worker: a cold pass, the demands, a warm pass."""
+        all_on()
+        emit_pass("auction")
+        demand_held(k, value)
+        emit_pass("auction")
+
+    def scripted_demand(n_passes):
+        """The demand and restore steps every history makes once (each from its pass count on)."""
+        if n_passes >= 6 and "restore_refusals" not in done:
+            # refused exports and restores: without a state, with a demand above 1, with disabled asks
+            done.add("restore_refusals")
+            choices = [p for p in PARAMS if p != h.params]
+            emit_call(("auction_params", dict(params=choices[int(rng.integers(0, len(choices)))])))
+            emit_call(g.restore_refused("export_no_state"))
+            all_on()
+            emit_pass("auction")
+            for case in ("length_w", "length_t", "worker", "price_neg", "price_high"):
+                emit_call(g.restore_refused(case))
+            demand_held(4, 2)
+            emit_call(g.restore_refused("export_demand"))
+            emit_call(g.restore_refused("demand"))
+            ones()
+            emit_call(("ask_off", dict(idx=np.array([int(rng.integers(0, len(h.asks)))], dtype=np.uint32))))
+            emit_call(g.restore_refused("disabled"))
+            return True
+        if n_passes >= 14 and "mixed_window" not in done:
+            # one window of mixed changes before a warm pass, then again before a repair pass
+            done.add("mixed_window")
+            slot_state()
+            for kind in ("warm", "repair"):
+                emit_call(g.call("demand"))
+                big = np.flatnonzero(h.d > 1)
+                held = np.intersect1d(h.held_asks(), big)
+                t = held if len(held) else big if len(big) else h.held_asks()
+                emit_call(g.update_asks(np.array([t[int(rng.integers(0, len(t)))]], dtype=np.uint32)))
+                emit_call(g.delta("append_asks", g.ask_rows(2, missing=False), n=len(h.asks) + 2, cap=None))
+                cut_held(2)
+                i = np.array([int(rng.integers(0, len(h.asks)))], dtype=np.uint32)
+                emit_call(("ask_off", dict(idx=i)))
+                emit_call(("ask_on", dict(idx=i)))
+                emit_call(g.call("update"))
+                all_on()
+                emit_pass(kind)
+            return True
+        if n_passes >= 18 and "chain" not in done:
+            # 3 -> 1 -> 3 on held asks before one warm pass (past the cutoff by the chain's added slots under a small
+            # PM_TUNE_INCR); then a worker shrink before a demand cut whose freed workers lie past n_kept
+            done.add("chain")
+            slot_state(6, 3)
+            d3 = h.d.copy()
+            idx = np.flatnonzero(h.d == 3)
+            emit_call(("demand", dict(d=np.where(h.d == 3, 1, h.d).astype(np.uint32))))
+            emit_call(("demand", dict(d=d3)))
+            if h.cutoff < 1000 and h.auc_state:
+                write_unchanged(h.cutoff + 1 - h.n_changes())
+            emit_pass("warm")
+            all_on()
+            demand_held(6, 3)
+            emit_pass("warm")
+            if h.auc_state:   # the held slot workers past their ask's first slot, highest first
+                off = ad.offsets(h.d)
+                cand = [(int(h.assigned[s_]), t) for t in np.flatnonzero(h.d > 1)
+                        for s_ in range(off[t] + 1, off[t + 1]) if h.assigned[s_] != NONE]
+                cand = [c for c in cand if c[0] >= h.n_workers - 200]
+                if cand:
+                    w, t = max(cand)
+                    emit_call(("shrink", dict(n=w, rank=rng.permutation(w).astype(np.uint32))))
+                    d = h.d.copy()
+                    d[t] = 1
+                    emit_call(("demand", dict(d=d)))
+                    if h.cutoff < 1000:
+                        write_unchanged(h.cutoff - h.n_changes())
+            emit_pass("warm")
+            return True
+        if n_passes >= 22 and shape == "mixed" and "d_over_w" not in done:
+            # more slots than workers: a cold pass and a warm pass with D > W.  Most of the slots go to the ask with the
+            # fewest feasible workers (they withdraw at once), so the passes stay short: D > W does not make a price war
+            done.add("d_over_w")
+            all_on()
+            T = len(h.asks)
+            d = np.where(np.isin(np.arange(T), h.held_asks()[:20]), 2, 1).astype(np.uint32)
+            t = int(np.argmin(h.F().sum(axis=1)))
+            d[t] = h.n_workers + 10 - (int(d.sum()) - int(d[t]))
+            emit_call(("demand", dict(d=d)))
+            emit_pass("auction")
+            emit_call(g.call("update"))
+            emit_pass("warm")
+            ones()
+            return True
+        if n_passes >= 30 and "after_set_asks" not in done:
+            # demands above 1, then a table swap: the next pass is one with demand 1, and the export works after it
+            done.add("after_set_asks")
+            all_on()
+            demand_held(6, 3)
+            emit_call(g.call("set_asks"))
+            emit_pass("auction")
+            emit_call(g.restore("own"))
+            return True
+        if n_passes >= 34 and "back_to_one" not in done:
+            # demands above 1, then all 1 under a stored state: certificate, export and restore; then demands again
+            done.add("back_to_one")
+            slot_state(6, 2)
+            ones()
+            emit_pass("certificate")
+            emit_call(g.restore("own"))
+            demand_held(6, 3)
+            emit_pass("warm")
+            return True
+        if n_passes >= 40 and "restore_tracker" not in done:
+            # a restore between two incremental passes, a worker resize before an own export, a restore followed by a
+            # certificate, and an own restore right after its pass
+            done.add("restore_tracker")
+            all_on()
+            ones()
+            emit_pass("auction")
+            emit_call(g.restore("own"))
+            emit_pass("lean")
+            emit_call(g.call("update"))
+            emit_call(g.restore("adversarial"))
+            if h.eval:   # cut past the last stored first ask (its workers have none now) and append as many asks back
+                T = len(h.asks)
+                last = int(h.eval_ff[h.eval_ff != NONE].max(initial=0))
+                if 0 < last < T:
+                    emit_call(("shrink_asks", dict(n=last)))
+                    emit_call(g.delta("append_asks", g.ask_rows(T - last, missing=False), n=T, cap=None))
+            emit_pass("lean_incr")
+            emit_call(g.call("shrink" if h.n_workers >= 2000 else "grow"))
+            emit_call(g.restore("own"))     # refused as exported, then trimmed
+            emit_call(g.call("caps"))
+            emit_call(g.restore("stale"))
+            emit_pass("certificate")
+            emit_named("move")
+            emit_pass("lean_incr")
+            emit_pass("warm")
+            return True
+        if n_passes >= 26 and h.cutoff < 1000 and "freed_decides" not in done:
+            # freed slot workers decide the cutoff: cut the demands of held asks, then write unchanged kept rows until the
+            # changes without them reach the cutoff (the pass runs cold), or stop where the changes with them reach it
+            # (the pass runs warm); for a warm pass and a repair pass
+            done.add("freed_decides")
+            for kind in ("warm", "repair"):
+                for over in (True, False):
+                    slot_state(8, 3)
+                    emit_call(("demand", dict(d=np.minimum(h.d, 1 + (h.d > 1)).astype(np.uint32))))
+                    if h.auc_state and h.removed_held:
+                        base = h.n_changes() - h.removed_held
+                        write_unchanged(h.cutoff - base - (0 if over else h.removed_held))
+                    emit_pass(kind)
             return True
         return False
 
@@ -1007,8 +1500,15 @@ def generate(shape, seed, n_calls=N_CALLS, cutoff=DEFAULT_CUTOFF, slot=0, n_slot
         return a in PASSES and (a, b) not in seen_pass and (PASSES.index(a) * len(PASSES) + PASSES.index(b)) % n_slots == slot
 
     follow = []
+    extra = [0]                              # the events of the demand and restore steps
     emit_pass("lean_incr")
-    while len([e for e in events if e[0] != "probe"]) < n_calls:
+    while len([e for e in events if e[0] != "probe"]) - extra[0] < n_calls:
+        for _ in range(2):                  # what a refusal left, before a scripted step makes a new state
+            if follow:
+                kind = follow.pop(0)
+                if kind in AUCTION:
+                    all_on()
+                emit_pass(kind)
         if len([e for e in events if e[0] == "pass"]) >= domain_at // 2 and "domain" not in done \
                 and h.params != DOMAIN_EDGE:
             done.add("domain")
@@ -1027,6 +1527,7 @@ def generate(shape, seed, n_calls=N_CALLS, cutoff=DEFAULT_CUTOFF, slot=0, n_slot
             old = (a.copy(), b.copy())
             b["ext_ask_price"] = 0xFFFFFFFF
             emit_call(("update", dict(idx=row, a=a, b=b, lat=None, lon=None)))
+            emit_call(g.restore_refused("domain"))
             emit_pass("warm")                       # refused: the stored state stays
             emit_pass("lean_incr")
             emit_pass("certificate")                # refused too
@@ -1037,9 +1538,10 @@ def generate(shape, seed, n_calls=N_CALLS, cutoff=DEFAULT_CUTOFF, slot=0, n_slot
         n_passes = len([e for e in events if e[0] == "pass"])
         if scripted(n_passes):
             continue
-        if n_passes >= 12 and "b12" not in done and h.mask.all():
+        if n_passes >= 12 and "b12" not in done:
             # warm or repair after reference passes of both modes, with asks left disabled across them
             done.add("b12")
+            all_on()
             emit_pass("auction")
             off = np.union1d(rng.choice(len(h.asks), 5, replace=False), h.max0_on())
             emit_call(("ask_off", dict(idx=off.astype(np.uint32))))
@@ -1058,7 +1560,7 @@ def generate(shape, seed, n_calls=N_CALLS, cutoff=DEFAULT_CUTOFF, slot=0, n_slot
         names = [c for c in CALLS if not (c == "shrink" and h.n_workers < 2000)]
         p = np.array([0.15 if c in RARE else 1.0 for c in names])
         for _ in range(int(rng.integers(0, 3))):
-            emit_call(g.call(names[int(rng.choice(len(names), p=p / p.sum()))]))
+            emit_named(names[int(rng.choice(len(names), p=p / p.sum()))])
         if n_passes >= 20 and "b20" not in done:
             done.add("b20")
             # past the cutoff between two reference passes (a full pass under a small PM_TUNE_INCR), and a side column
@@ -1099,14 +1601,14 @@ def generate(shape, seed, n_calls=N_CALLS, cutoff=DEFAULT_CUTOFF, slot=0, n_slot
             j = next((i for i, (_, k) in enumerate(must) if mine(last_pass, k)),
                      next((i for i, (_, k) in enumerate(must) if (last_pass, k) not in seen_pass), 0))
             c, kind = must.pop(j)
-            emit_call(g.call(c))
+            emit_named(c)
         elif targets and rng.random() < 0.85:
             tw = np.array([0.5 if c in RARE else 1.0 for c, _ in targets])
             c, kind = targets[int(rng.choice(len(targets), p=tw / tw.sum()))]
             if c == "ask_on" and h.mask.all():
                 emit_call(g.call("ask_off"))
             if c != "shrink" or h.n_workers >= 2000:
-                emit_call(g.call(c))
+                emit_named(c)
         else:
             if not h.mask.all() and rng.random() < 0.5:
                 emit_call(g.call("ask_on"))
@@ -1122,8 +1624,10 @@ def generate(shape, seed, n_calls=N_CALLS, cutoff=DEFAULT_CUTOFF, slot=0, n_slot
             if len(h.max0_on()) and rng.random() < 0.75:
                 emit_call(("ask_off", dict(idx=h.max0_on().astype(np.uint32))))
         emit_pass(kind)
+    while scripted_demand(1 << 30):         # the demand and restore steps the loop had no room for
+        pass
     for c, kind in must:                    # the slot's pairs the loop had no room for
-        emit_call(g.call(c))
+        emit_named(c)
         emit_pass(kind)
     for i in range(slot, len(PASSES) ** 2, n_slots):
         a, b = PASSES[i // len(PASSES)], PASSES[i % len(PASSES)]
@@ -1189,28 +1693,35 @@ def expect_reference(h: History, kind):
 
 
 def expect_auction(h: History, kind, warm):
-    """(assignment, prices, forward rounds, released, (phases, reverse rounds, reverse bids)) of an auction pass: the
-    oracle's cold pass, the reverse checker, the warm checker or the repair checker."""
+    """(slot assignment, prices, forward rounds, released, (phases, reverse rounds, reverse bids)) of an auction pass,
+    all on the twin tables (row t repeated d[t] times; the ask table itself with every demand 1): the oracle's cold
+    pass, the reverse checker, the warm checker or the repair checker, from the slot-level stored state."""
     import auction_repair_checker as rp
     import auction_reverse_checker as rc
 
-    S, E, d = h.params
+    S, E, dv = h.params
     ap = h.wb["ext_ask_price"]
-    if warm and kind == "warm":
-        a, p, n, rel = h.warm(S)
-        return a, p, n, len(rel), (0, 0, 0)
-    if warm and kind == "repair":
-        out = rp.market_repair(h, S)
+    if warm:
+        F, cap = h.slot_F(), h.slot_cap()
+        if kind == "warm":
+            a, p, n, rel = wc.warm(F, ap, cap, S, h.price, h.assigned, h.n_kept, h.changed_rows(), h.changed_slots())
+            return a, p, n, len(rel), (0, 0, 0)
+        out = rp.repair(F, ap, cap, S, h.price, h.assigned, h.n_kept, h.changed_rows(), h.changed_slots())
         return out["assigned"], out["price"], out["fwd"], len(out["released"]), (1, out["rev"], out["bids"])
     if kind == "reverse":
-        a, p, fwd, rev, bids, phases = rc.scaled(h.F(), ap, h.cap, S, E, d, reverse_rounds=True)
+        a, p, fwd, rev, bids, phases = rc.scaled(h.slot_F(), ap, h.slot_cap(), S, E, dv, reverse_rounds=True)
         return a, p, fwd, 0, (phases, rev, bids)
-    a, p, n = orc.soa_auction(h.wa, h.wb, h.asks, h.opts, h.bits, h.words, h.cap, S, E, d, reputation=h.reputation,
-                              min_reputation=h.floors_or_zero())
+    a, p, n = orc.soa_auction(h.wa, h.wb, np.repeat(h.asks, h.d), h.opts, h.bits, h.words, h.slot_cap(), S, E, dv,
+                              reputation=h.reputation, min_reputation=h.slot_floors())
     return a, p, n, 0, (0, 0, 0)
 
 
-def expect_certificate(h: History):
-    import auction_certificate as ac
+def expect_result(h: History, a_slots):
+    """Every array pm_fetch_result returns after an auction pass whose slot assignment is a_slots: its fold, one group
+    per holding ask in ask order, members sorted (with every demand 1, one solo group per held ask)."""
+    return ad.result_arrays(a_slots, h.d, h.wb["ext_ask_price"], h.n_workers)
 
-    return ac.market_certificate(h, h.params[0], h.price, h.assigned)
+
+def expect_certificate(h: History):
+    """The certificate of the stored slot state on the current tables (per ask row terms weighted by the demands)."""
+    return ad.demand_certificate(h.F(), h.wb["ext_ask_price"], h.cap, h.d, h.params[0], h.price, h.assigned)

@@ -11,15 +11,12 @@ import numpy as np
 import pytest
 
 import auction_certificate as ac
+from auction_demand import demand_certificate, fold_like_device, offsets, remap
 import auction_repair_checker as rp
 import auction_reverse_checker as rc
 import auction_warm_checker as wc
 
 NONE = wc.NONE
-
-
-def offsets(d):
-    return np.concatenate([[0], np.cumsum(d)]).astype(np.int64)
 
 
 def random_instance(T, W, seed, density=0.3):
@@ -29,18 +26,6 @@ def random_instance(T, W, seed, density=0.3):
     cap = rng.integers(5, 50, T).astype(np.uint32)
     d = rng.integers(1, 5, T).astype(np.uint32)
     return F, ap, cap, d, rng
-
-
-def remap(a_slots, d_old, d_new):
-    """pm_set_ask_demand under a stored state: old slot k of ask t stays slot k while k < the new demand."""
-    o_old, o_new = offsets(d_old), offsets(d_new)
-    out = np.full(int(o_new[-1]), NONE, dtype=np.uint32)
-    added = []
-    for t in range(len(d_old)):
-        k = min(int(d_old[t]), int(d_new[t]))
-        out[o_new[t]:o_new[t] + k] = a_slots[o_old[t]:o_old[t] + k]
-        added.extend(range(int(o_new[t]) + k, int(o_new[t + 1])))
-    return out, added
 
 
 def new_demands(d, rng):
@@ -58,7 +43,7 @@ def test_remapped_state_warm_and_repair(seed, S_exact):
     S = int(d.sum()) + 1 if S_exact else 1
     a, p, _ = wc.cold(Fx, ap, capx, S)
     d2 = new_demands(d, rng)
-    a2, added = remap(a, d, d2)
+    a2, added, _ = remap(a, d, d2)
     Fx2, capx2 = np.repeat(F, d2, axis=0), np.repeat(cap, d2)
     D2 = int(d2.sum())
     # kept holds: feasible, unshared, and eps-CS against every worker at the stored prices
@@ -74,42 +59,6 @@ def test_remapped_state_warm_and_repair(seed, S_exact):
         assert opt <= cost <= opt + D2
         if S_exact:
             assert cost == opt
-
-
-def demand_certificate(F, ask_price, cap, d, S, price, a_slots):
-    """The certificate as the device computes it with demands: the row terms per ask (T x W), weighted by d; holds,
-    costs, slacks and ownership per slot."""
-    T, W = F.shape
-    S = int(S)
-    ap = [int(x) for x in np.asarray(ask_price)[:W]]
-    pr = [int(x) for x in np.asarray(price)[:W]]
-    key = [ap[w] * S + pr[w] for w in range(W)]
-    row = []
-    for t in range(T):
-        ks = [key[w] for w in np.flatnonzero(F[t])]
-        row.append(min([(int(cap[t]) + 1) * S] + ks))
-    off = offsets(d)
-    own = [0] * W
-    cost = n_held = n_bad = 0
-    slack = []
-    for t in range(T):
-        for s in range(off[t], off[t + 1]):
-            w = int(a_slots[s])
-            if w != NONE and w < W:
-                n_held += 1
-                own[w] += 1
-                n_bad += int(not F[t, w])
-                cost += ap[w] * S
-                slack.append(key[w] - row[t])
-            else:
-                cost += (int(cap[t]) + 1) * S
-                slack.append((int(cap[t]) + 1) * S - row[t])
-    bound = sum(int(d[t]) * row[t] for t in range(T)) - sum(pr)
-    free = [w for w in range(W) if own[w] == 0 and pr[w] > 0]
-    return dict(cost=cost, bound=bound, gap=cost - bound, n_held=n_held, n_bad_holds=n_bad,
-                n_shared=sum(1 for o in own if o > 1), n_priced_unowned=len(free),
-                priced_unowned_sum=sum(pr[w] for w in free), n_slack_over=sum(1 for s in slack if s > 1),
-                max_slack=max(slack) if T else 0, evals=T * W, ask_bound=np.array(row, dtype=np.int64))
 
 
 def assert_same_certificate(F, ap, cap, d, S, price, a_slots):
@@ -147,34 +96,6 @@ def test_weighted_certificate_equals_twin_adversarial():
             assert_same_certificate(F, ap, cap, d, 3, price, a)
     F0 = np.zeros_like(F)                                   # no feasible pair: every row term is the outside option
     assert_same_certificate(F0, ap, cap, d, 2, zero, np.full(D, NONE, dtype=np.uint32))
-
-
-def fold_like_device(a_slots, d, ask_price):
-    """Held flags per slot and their exclusive scan, counts per ask, groups by the scan of the ask flags, members
-    gathered in slot order and sorted per group."""
-    off = offsets(d)
-    held = (a_slots != NONE).astype(np.int64)
-    spos = np.concatenate([[0], np.cumsum(held)])
-    count = spos[off[1:]] - spos[off[:-1]]
-    gidx = np.concatenate([[0], np.cumsum(count > 0)])
-    G, M = int(gidx[-1]), int(spos[-1])
-    group_ask = np.zeros(G, dtype=np.int64)
-    group_off = np.zeros(G + 1, dtype=np.int64)
-    members = np.zeros(M, dtype=np.int64)
-    best = np.full(len(d), np.iinfo(np.int64).max, dtype=np.int64)
-    for t in range(len(d)):
-        if count[t] == 0:
-            continue
-        g = gidx[t]
-        group_ask[g], group_off[g] = t, spos[off[t]]
-        ws = a_slots[off[t]:off[t + 1]]
-        ws = ws[ws != NONE].astype(np.int64)
-        members[spos[off[t]]:spos[off[t]] + len(ws)] = ws
-        best[t] = min((int(ask_price[w]) << 32) | int(w) for w in ws)
-    group_off[G] = M
-    for g in range(G):
-        members[group_off[g]:group_off[g + 1]] = np.sort(members[group_off[g]:group_off[g + 1]])
-    return group_ask, group_off, members, count, best
 
 
 @pytest.mark.parametrize("seed", range(5))

@@ -2,14 +2,18 @@
 file runs: every (table call -> pass kind) and (pass kind -> pass kind) pair, every refusal kind followed by an
 incremental and a warm pass, incremental passes after auction passes and certificates, warm and repair passes after
 reference passes of both modes with toggles left on across them, the fast/generic and narrow/wide flips inside an
-incremental pass's window, and cutoff crossings on both trackers.  And the mirror checked against itself: the oracle's
-groups on the enabled asks equal test_gpu_ask_enabled's compaction, and the warm checker with no changes reproduces
-the stored state."""
+incremental pass's window, and cutoff crossings on both trackers; the demand and restore steps with the property each
+claims.  And the mirror checked against itself: the oracle's groups on the enabled asks equal test_gpu_ask_enabled's
+compaction, the warm checker with no changes reproduces the stored state, the slot-level mirror with every demand 1 is
+the ask-level one, and each of six wrong demand or restore rules changes some prediction of the same histories."""
 import functools
 
 import numpy as np
 import pytest
 
+import auction_certificate as ac
+import auction_demand as ad
+import auction_repair_checker as rp
 import auction_warm_checker as wc
 import engine_history as eh
 from helpers import assert_distance_certificate
@@ -23,7 +27,9 @@ def evidence():
     ev = dict(call_pass=set(), pass_pass=set(), refusals={}, after_refusal={}, incr_after_auction_cert=0,
               warm_after_both=set(), flips=set(), incr_over=0, warm_over=0, n_passes=0, incr_saw=set(),
               e_rows_over=0, removed_held=set(), removed_held_decides=set(), max0_by=set(), probes_after_auction=0,
-              generated={})
+              generated={}, cases=set(), freed_decides=set(), chain=set(), past_kept=0, d_over_w=set(),
+              variants=set(), own_clean=0, move_full=0, restore_incr=0, restore_cert=0, set_asks_export=0,
+              cert_back_to_one=0, window=set(), slot_warm=set())
     for shape in eh.SHAPES:
         for setting in eh.SETTINGS:
             cutoff = eh.cutoff_of(setting)
@@ -34,13 +40,38 @@ def evidence():
                 if e[0] == "call":
                     name = e[1][0]
                     st["after_auction"] = False   # a delta puts the rows back in the reference form
+                    x = e[1][1]
                     if before:
                         st["max0"] = len(h.max0_on()) > 0
-                        if name == "ask_delta_refused":
-                            ev["refusals"]["ask_delta_refused"] = ev["refusals"].get("ask_delta_refused", 0) + 1
-                            st["pend_incr"].append("ask_delta_refused")
-                            st["pend_warm"].append(("ask_delta_refused", h.auc_state))
+                        if name in ("ask_delta_refused", "demand_refused", "restore_refused"):
+                            ev["refusals"][name] = ev["refusals"].get(name, 0) + 1
+                            st["pend_incr"].append(name)
+                            st["pend_warm"].append((name, h.auc_state))
+                            if name != "ask_delta_refused":
+                                ev["cases"].add((name, x["case"]))
+                        if name == "demand" and h.auc_state:   # removed slots' workers past n_kept
+                            o = ad.offsets(h.d)
+                            gone = [int(w) for t in range(len(h.d)) for w in
+                                    h.assigned[o[t] + min(int(h.d[t]), int(x["d"][t])):o[t + 1]] if w != eh.NONE]
+                            ev["past_kept"] += any(w >= h.n_kept for w in gone)
+                        if name == "set_asks" and (h.d > 1).any():
+                            st["set_asks_d"] = True
+                        if name in ("restore", "move"):
+                            st["restore_eval"] = h.eval
                         return
+                    if name in ("restore", "move") and h.last_report is not None:
+                        variant = x.get("variant", "move")
+                        ev["variants"].add(variant)
+                        if variant == "own" and st["calls"] == [] and st["last"] in eh.AUCTION:
+                            ev["own_clean"] += 1
+                            assert h.last_report["n_dropped_bad"] + h.last_report["n_dropped_shared"] \
+                                + h.last_report["n_dropped_slack"] == 0, h.last_report
+                        if variant == "own" and st.get("set_asks_d"):
+                            ev["set_asks_export"] += 1
+                            st["set_asks_d"] = False
+                        st["restored"] = True
+                        st["restored_eval"] = st.get("restore_eval", False) and name == "restore"
+                        st["moved"] = name == "move"
                     st["calls"].append(name)
                     if name in eh.ASK_DELTAS and (len(h.max0_on()) > 0) != st["max0"]:
                         ev["max0_by"].add(name)
@@ -59,6 +90,31 @@ def evidence():
                 st["after_auction"] = False
                 ev["n_passes"] += 1
                 why, _ = h.refusal(kind)
+                restored, st["restored"] = st.get("restored", False), False
+                if kind == "certificate" and why is None:
+                    ev["restore_cert"] += restored
+                    ev["cert_back_to_one"] += bool(h.dem_kept is not None and (h.d == 1).all())
+                if kind in eh.INCREMENTAL and why is None:
+                    full = h.incremental_plan()[0]
+                    ev["move_full"] += bool(st.get("moved") and full and not h.eval)
+                    ev["restore_incr"] += bool(restored and st.get("restored_eval") and h.eval and not full)
+                    st["moved"] = False
+                if kind in eh.AUCTION and why is None:
+                    D = int(h.d.sum())
+                    warm = h.warm_plan()[0] if kind in ("warm", "repair") else False
+                    if D > h.n_workers:
+                        ev["d_over_w"].add("warm" if warm else "cold")
+                    if warm and (h.d > 1).any():
+                        ev["slot_warm"].add(kind)
+                    if kind in ("warm", "repair") and h.auc_state and h.dem_kept is not None:
+                        if h.removed_held and not h.auc_over and abs(h.n_changes() - h.cutoff) <= h.removed_held \
+                                and h.n_changes() - h.removed_held <= h.cutoff:
+                            ev["freed_decides"].add((kind, warm))
+                        if (h.dem_kept != np.minimum(h.d_pass, h.d)).any():
+                            ev["chain"].add(kind)
+                        if warm and {"demand", "update_asks", "append_asks", "shrink_asks", "ask_off", "ask_on",
+                                     "update"} <= set(st["calls"]):
+                            ev["window"].add(kind)
                 if why is not None:
                     ev["refusals"][why] = ev["refusals"].get(why, 0) + 1
                 if kind in eh.INCREMENTAL and why is None:
@@ -182,27 +238,37 @@ def test_removed_held_asks_decide_the_warm_cutoff():
     assert evidence()["removed_held_decides"] >= {("warm", False), ("repair", False)}, evidence()["removed_held_decides"]
 
 
-MIRROR = ("asks", "mask", "eval_mask", "cap", "floors", "wa", "wb", "lat", "lon", "rank", "reputation", "eval_ff")
+MIRROR = ("asks", "mask", "eval_mask", "cap", "floors", "wa", "wb", "lat", "lon", "rank", "reputation", "eval_ff", "d",
+          "d_pass", "dem_kept", "price", "assigned")
 TRACKED = ("params", "eval", "dirty", "over", "replaced", "appended", "dropped", "flipped", "auc_state", "auc_w",
-           "auc_over", "resized", "rows", "toggled", "n_kept", "cap0", "floors0")
+           "auc_over", "resized", "rows", "toggled", "n_kept", "cap0", "floors0", "removed_held")
+
+
+def rebuild(events, outcomes, h, until=None, on_pass=None):
+    """Replay `events` on the mirror h, each auction pass taking the state the generator predicted for it (outcomes);
+    on_pass(h, i, kind, why) runs before each pass and may return an outcome to use instead."""
+    for i, e in enumerate(events[:until]):
+        if e[0] == "call":
+            h.apply(e[1])
+        elif e[0] == "pass":
+            why, _ = h.refusal(e[1])
+            got = on_pass(h, i, e[1], why) if on_pass is not None else None
+            if e[1] in eh.REFERENCE:
+                h.reference_done(why is None)
+            elif e[1] in eh.AUCTION and why is None:
+                out = got or outcomes[i]
+                h.auction_done(out[2], out[1])
+    return h
 
 
 @pytest.mark.parametrize("setting", list(eh.SETTINGS))
 @pytest.mark.parametrize("shape", eh.SHAPES)
 def test_events_alone_rebuild_the_mirror(shape, setting):
-    """The GPU runner rebuilds the mirror from the events alone: replaying them on a fresh History (auction passes
-    without their state values) ends with the generator's tables and trackers."""
+    """The GPU runner rebuilds the mirror from the events alone: replaying them on a fresh History, each auction pass
+    storing the state its checker predicted, ends with the generator's tables and trackers, demands, kept slots and
+    slot-level state included."""
     events, g = evidence()["generated"][shape, setting]
-    h = eh.History(shape, eh.cutoff_of(setting))
-    for e in events:
-        if e[0] == "call":
-            h.apply(e[1])
-        elif e[0] == "pass":
-            why, _ = h.refusal(e[1])
-            if e[1] in eh.REFERENCE:
-                h.reference_done(why is None)
-            elif e[1] in eh.AUCTION and why is None:
-                h.auction_done(None, None)
+    h = rebuild(events, g.outcomes, eh.History(shape, eh.cutoff_of(setting)))
     for f in MIRROR:
         a, b = getattr(h, f), getattr(g, f)
         assert (a is None and b is None) or np.array_equal(a, b), f
@@ -293,3 +359,169 @@ def test_the_max_group_size_zero_ask_is_filled_by_the_auction_only(shape):
     a, _, _, _, _ = eh.expect_auction(h, "auction", False)
     assert a[z] != eh.NONE
     assert not (eh.expect_reference(h, "lean")["worker_ask"] == z).any()
+
+
+# ------------------------------------------------------------------ demands and restores
+def test_every_demand_and_restore_refusal_occurs():
+    cases = evidence()["cases"]
+    want = {("demand_refused", c) for c in eh.DEMAND_REFUSALS} | {("restore_refused", c) for c in eh.RESTORE_REFUSALS}
+    assert cases >= want, sorted(want - cases)
+
+
+def test_warm_and_repair_passes_on_slot_states_after_mixed_windows():
+    """Warm passes with demands above 1, and passes that stay warm after a window with a demand change, a replaced
+    held ask, an append, a shrink, a toggle off and on and written rows."""
+    ev = evidence()
+    assert ev["slot_warm"] >= {"warm", "repair"} and ev["window"] >= {"warm", "repair"}, (ev["slot_warm"], ev["window"])
+
+
+def test_freed_slot_workers_decide_the_cutoff():
+    """Under PM_TUNE_INCR=40, warm and repair passes whose changes pass the cutoff only with the workers of removed
+    slots (cold), and ones they leave within it (warm)."""
+    want = {(k, w) for k in ("warm", "repair") for w in (False, True)}
+    assert evidence()["freed_decides"] >= want, evidence()["freed_decides"]
+
+
+def test_demand_chains_and_freed_workers_past_n_kept():
+    """A chain of demand changes whose kept slots differ from min(demand at the pass, demand now), and a demand cut
+    whose removed slots held a worker a worker shrink had cut off."""
+    ev = evidence()
+    assert "warm" in ev["chain"] and ev["past_kept"] > 0, (ev["chain"], ev["past_kept"])
+
+
+def test_more_slots_than_workers():
+    assert evidence()["d_over_w"] >= {"cold", "warm"}, evidence()["d_over_w"]
+
+
+def test_restores_of_every_kind():
+    """Own states (one right after its pass, which the audit keeps whole), stale, adversarial and resized ones, a
+    move, an export after a table swap with demands, and a certificate after demands back to 1."""
+    ev = evidence()
+    assert ev["variants"] >= {"own", "stale", "adversarial", "resized", "move"}, ev["variants"]
+    assert ev["own_clean"] > 0 and ev["set_asks_export"] > 0 and ev["cert_back_to_one"] > 0
+
+
+def test_restores_then_incremental_passes_and_certificates():
+    """A restore between two incremental passes (the second stays incremental), a certificate right after a restore,
+    and a move followed by a full incremental pass (the fresh engine has no stored evaluation)."""
+    ev = evidence()
+    assert ev["restore_incr"] > 0 and ev["restore_cert"] > 0 and ev["move_full"] > 0, \
+        (ev["restore_incr"], ev["restore_cert"], ev["move_full"])
+
+
+def test_demands_of_one_are_the_ask_level_mirror():
+    """With every demand 1 the slot-level mirror is the ask-level one: A0 over slots is A0, the change count, the warm
+    and repair predictions, the certificate and the result fold are today's, over a history without demand calls."""
+    events, g = evidence()["generated"]["wide", "incr40"]
+    events = [e for e in events if not (e[0] == "call" and e[1][0] == "demand")]
+    checked = []
+
+    def on_pass(h, i, kind, why):
+        assert (h.d == 1).all()
+        if kind not in eh.AUCTION or why is not None:
+            return None
+        S = h.params[0]
+        warm = h.warm_plan()[0] if kind in ("warm", "repair") else False
+        out = eh.expect_auction(h, kind, warm)
+        if warm:
+            assert h.changed_slots() == h.changed_asks()
+            assert h.n_changes() == len(h.rows) + (h.n_workers - h.n_kept) + len(h.changed_asks()) + h.removed_held
+            if kind == "warm":
+                a, p, n, rel = h.warm(S)
+                assert np.array_equal(a, out[0]) and np.array_equal(p, out[1]) and (n, len(rel)) == out[2:4]
+            else:
+                r = rp.market_repair(h, S)
+                assert np.array_equal(r["assigned"], out[0]) and np.array_equal(r["price"], out[1])
+            checked.append(kind)
+        a = out[0]
+        res = eh.expect_result(h, a)
+        held = np.flatnonzero(a != eh.NONE)
+        assert np.array_equal(res["group_ask"], held) and np.array_equal(res["group_members"], a[held])
+        assert np.array_equal(res["group_off"], np.arange(len(held) + 1))
+        assert np.array_equal(res["worker_ask"][a[held]], held) and np.array_equal(res["ask_count"], a != eh.NONE)
+        if h.auc_state and not h.resized and h.auc_w == h.n_workers and h.mask.all():
+            c1, c2 = eh.expect_certificate(h), ac.market_certificate(h, S, h.price, h.assigned)
+            assert all(c1[k] == c2[k] for k in ac.FIELDS) and np.array_equal(c1["ask_bound"], c2["ask_bound"])
+        return (warm,) + out
+
+    rebuild(events, g.outcomes, eh.History("wide", eh.cutoff_of("incr40")), on_pass=on_pass)
+    assert {"warm", "repair"} <= set(checked), checked
+
+
+# ---- mutations: each wrong rule must change some prediction of the seeded histories
+class CountPastKept(eh.History):
+    def _slot_freed(self, gone):           # a removed slot's worker past n_kept counted too
+        return int(len(gone))
+
+
+class NoFreed(eh.History):
+    def _slot_freed(self, gone):           # removed slots' workers not counted at all
+        return 0
+
+
+class AllSlotsA0(eh.History):
+    def _kept_after(self, new):            # every slot of an ask whose demand changed in A0
+        return np.where(new != self.d, 0, super()._kept_after(new))
+
+
+class PassMin(eh.History):
+    def _kept_after(self, new):            # min(demand at the pass, new demand) instead of the chain's minimum
+        return np.minimum(self.d_pass, new)
+
+
+class PriceReset(eh.History):
+    def _free_price(self, workers):        # a removed slot's worker back at price 0
+        self.price = self.price.copy()
+        self.price[workers[workers < len(self.price)].astype(np.int64)] = 0
+
+
+class KeepChanges(eh.History):
+    def _restore_clear(self, price, kept):  # R0 and A0 kept across a restore
+        rows, toggled, cap0, floors0 = self.rows, self.toggled, self.cap0, self.floors0
+        super()._restore_clear(price, kept)
+        self.rows, self.toggled, self.cap0, self.floors0 = rows, toggled, cap0, floors0
+
+
+def differs(cls, shape, setting):
+    """Replay a seeded history on the true mirror and on a mutated one side by side: does any warm decision, auction
+    prediction (assignment, prices, rounds, n_released) or restore report differ?"""
+    events, g = evidence()["generated"][shape, setting]
+    t, m = eh.History(shape, eh.cutoff_of(setting)), cls(shape, eh.cutoff_of(setting))
+    inputs = ("price", "assigned", "n_kept")
+    for i, e in enumerate(events):
+        if e[0] == "call":
+            t.apply(e[1])
+            m.apply(e[1])
+            if e[1][0] in ("restore", "move") and t.last_report != m.last_report:
+                return True
+            continue
+        if e[0] != "pass":
+            continue
+        why, _ = t.refusal(e[1])
+        if e[1] in eh.REFERENCE:
+            t.reference_done(why is None)
+            m.reference_done(why is None)
+            continue
+        if e[1] not in eh.AUCTION or why is not None:
+            continue
+        out = g.outcomes[i]
+        warm = out[0]
+        if e[1] in ("warm", "repair") and m.warm_plan()[0] != warm:
+            return True
+        same = not warm or (all(np.array_equal(getattr(t, f), getattr(m, f)) for f in inputs)
+                            and t.changed_rows() == m.changed_rows() and t.changed_slots() == m.changed_slots())
+        mine = out if same else (warm,) + eh.expect_auction(m, e[1], warm)
+        if not same and not (np.array_equal(mine[1], out[1]) and np.array_equal(mine[2], out[2])
+                             and mine[3:] == out[3:]):
+            return True
+        t.auction_done(out[2], out[1])
+        m.auction_done(mine[2], mine[1])
+    return False
+
+
+@pytest.mark.parametrize("cls", [CountPastKept, NoFreed, AllSlotsA0, PassMin, PriceReset, KeepChanges],
+                         ids=lambda c: c.__name__)
+def test_a_wrong_rule_changes_a_prediction(cls):
+    order = [("mixed", "incr40"), ("wide", "incr40")] + [(sh, st) for sh in eh.SHAPES for st in eh.SETTINGS
+                                                         if st != "incr40"]
+    assert any(differs(cls, sh, st) for sh, st in order), f"{cls.__name__}: no history tells it from the rule"

@@ -10,6 +10,7 @@ import auction_certificate as ac
 import auction_repair_checker as rp
 import auction_reverse_checker as rc
 import auction_warm_checker as wc
+from auction_demand import offsets, remap
 from protocol_b200 import abi
 from protocol_b200._lib import PrimeMatchError
 from test_gpu_auction_reverse import scipy_instance
@@ -24,10 +25,6 @@ WARM = AUC | abi.PM_AUCTION_WARM
 REPAIR = WARM | abi.PM_AUCTION_REPAIR
 TUNES = [0, 1, 2, 8 | 32, 64 | 32, 128 | 32, 0x100 | 16]   # a spread of test_gpu_auction_warm's settings
 CERT = [f for f in ac.FIELDS if f != "evals"]             # evals: T x W with demands, D x W for the twin
-
-
-def offsets(d):
-    return np.concatenate([[0], np.cumsum(d)]).astype(np.int64)
 
 
 def fold_slots(a_slots, d):
@@ -245,19 +242,6 @@ def test_twin_duplicated_asks_ties():
 
 
 # ------------------------------------------------------------------ demand changes
-def remap(a_slots, d_old, d_new, W):
-    """The stored state's remap (prime_match.h "Auction demands"): (new slot assignment, added slots, freed workers)."""
-    o_old, o_new = offsets(d_old), offsets(d_new)
-    out = np.full(int(o_new[-1]), NONE, dtype=np.uint32)
-    added, freed = [], 0
-    for t in range(len(d_old)):
-        k = min(int(d_old[t]), int(d_new[t]))
-        out[o_new[t]:o_new[t] + k] = a_slots[o_old[t]:o_old[t] + k]
-        freed += int(np.sum(a_slots[o_old[t] + k:o_old[t + 1]] < W))
-        added.extend(range(int(o_new[t]) + k, int(o_new[t + 1])))
-    return out, np.array(added, dtype=np.int64), freed
-
-
 @pytest.mark.parametrize("mode", [WARM, REPAIR])
 @pytest.mark.parametrize("seed", [47, 48])
 def test_demand_changes_match_checkers(mode, seed):
@@ -281,7 +265,7 @@ def test_demand_changes_match_checkers(mode, seed):
         for t_ in pick:                                   # grow or shrink held asks, and one unheld
             d_new[t_] = max(1, int(d_new[t_]) + int(rng.choice([-2, -1, 1, 2])))
         d_new[int(rng.integers(0, 50))] = int(rng.integers(1, 6))
-        a_new, added, freed = remap(a_slots, d, d_new, W)
+        a_new, added, freed = remap(a_slots, d, d_new, n_kept=W)
         eng.set_ask_demand(d_new)
         Fx, capx = np.repeat(F, d_new, axis=0), np.repeat(cap, d_new)
         if mode == WARM:

@@ -2,13 +2,18 @@
 (tests/engine_history.py), compared after every call with plain references computed from the host mirror: the CPU
 oracle for reference passes, the exact auction checkers for auction passes, the certificate restatement for the
 certificate, and the mirror's change sets for whether a pass stays incremental or warm (and how many rows an
-incremental pass walks).  Refused calls must return the status the header gives and leave behind what it says: the
-next pass of each kind shows it.  After every reference pass, and after every cold auction pass once the ask table has
-changed in place, a fresh engine with the same settings, loaded from the mirror, must return the same arrays.  Cost
-tile probes between passes compare pm_build_cost_tile with the oracle's cost matrix and change nothing.  The same
-histories' reference side also runs on pm_multi.
+incremental pass walks).  Every auction pass's pm_fetch_result arrays are the fold of the predicted slot assignment.
+Refused calls must return the status the header gives and leave behind what it says: the next pass of each kind shows
+it.  After every reference pass, and after every cold auction pass once the ask table or the demands have changed in
+place, a fresh engine with the same settings, loaded from the mirror, must return the same arrays; after every cold
+auction pass with a demand above 1, a fresh engine loaded with the twin tables (each ask row, cap and floor repeated
+d[t] times) must return the same prices, rounds, reverse stats and slot assignment.  Exports and restores are checked
+against the mirror's state and restore_checker's audit, and a move continues the history on a fresh engine.  Cost tile
+probes between passes compare pm_build_cost_tile with the oracle's cost matrix and change nothing.  The same
+histories' reference side also runs on pm_multi (the auction-only calls skipped).
 
 PM_TEST_BIG=1 runs histories three times as long."""
+import ctypes
 import functools
 import os
 
@@ -115,17 +120,15 @@ class Runner:
             return
         assert why is None, f"{kind}: ran, expected refusal {why}"
         res = eng.fetch()
-        got = np.full(len(h.asks), eh.NONE, dtype=np.uint32)
-        for ask, members in res.groups():
-            assert len(members) == 1
-            got[ask] = members[0]
         price, warm, released = eng.auction_state()
         rs = eng.auction_reverse_stats()
         if not sure:
             want_warm = warm
         a, p, n, rel, wrs = eh.expect_auction(h, kind, want_warm)
         assert warm == want_warm, (kind, "warm", warm)
-        assert np.array_equal(got, a), f"{kind}: assignment differs from the checker"
+        want = eh.expect_result(h, a)
+        for f in FIELDS:
+            assert np.array_equal(getattr(res, f), want[f]), f"{kind}: {f} differs from the checker's fold"
         assert np.array_equal(price, p), f"{kind}: prices differ from the checker"
         assert res.stats["n_rounds"] == n, (kind, "n_rounds", res.stats["n_rounds"], n)
         assert released == rel, (kind, "n_released", released, rel)
@@ -138,23 +141,119 @@ class Runner:
             qprice, _, _ = fresh.auction_state()
             qrs = fresh.auction_reverse_stats()
             fresh.close()
-            assert np.array_equal(res.worker_ask, q.worker_ask), f"{kind}: assignment differs from a fresh engine's"
+            for f in FIELDS:
+                assert np.array_equal(getattr(res, f), getattr(q, f)), f"{kind}: {f} differs from a fresh engine's"
             assert np.array_equal(price, qprice) and res.stats["n_rounds"] == q.stats["n_rounds"] and rs == qrs, \
                 f"{kind}: prices or rounds differ from a fresh engine's"
+        if not warm and (h.d > 1).any():   # the defining rule: the twin table gives the same pass bit for bit
+            twin = new_engine(self.setting)
+            eh.load(twin, h, twin=True)
+            twin.match(eh.MODES[kind])
+            q = twin.fetch()
+            qprice, _, _ = twin.auction_state()
+            qrs = twin.auction_reverse_stats()
+            twin.close()
+            slots = np.full(int(h.d.sum()), eh.NONE, dtype=np.uint32)
+            for s, members in q.groups():
+                assert len(members) == 1
+                slots[s] = members[0]
+            assert np.array_equal(slots, a), f"{kind}: the twin's slot assignment differs"
+            assert np.array_equal(price, qprice) and res.stats["n_rounds"] == q.stats["n_rounds"] and rs == qrs, \
+                f"{kind}: prices, rounds or reverse stats differ from the twin's"
         h.auction_done(p, a)
 
     def certificate(self):
         h, eng = self.h, self.eng
         why, statuses = h.refusal("certificate")
         out = {}
+        before = self.untouched()
         if refused(lambda: out.update(eng.auction_certificate(ask_bound=True)), statuses) is not None:
             self.stored_state_kept()
             return
         assert why is None, f"certificate: ran, expected refusal {why}"
+        self.same(before, self.untouched())
         want = eh.expect_certificate(h)
         for k in ac.FIELDS:
             assert out[k] == want[k], ("certificate", k, out[k], want[k])
         assert np.array_equal(out["ask_bound"], want["ask_bound"])
+
+    # ---- exports and restores
+    def export_matches(self, want):
+        """The engine's export (pm_auction_assignment, pm_auction_state's prices) equals the mirror's."""
+        price, _, _ = self.eng.auction_state()
+        assigned = self.eng.auction_assignment()
+        assert np.array_equal(price, want[0]) and np.array_equal(assigned, want[1]), "the export differs from the mirror"
+
+    def untouched(self):
+        """What a restore and a certificate must leave as they are: pm_fetch_result, pm_get_stats, pm_table_version."""
+        try:
+            r = self.eng.fetch()
+            res = tuple(getattr(r, f).copy() for f in FIELDS)
+        except PrimeMatchError:
+            res = None
+        st = abi.PmStats()
+        assert self.eng._lib.pm_get_stats(self.eng._h, ctypes.byref(st)) == abi.PM_OK
+        return res, bytes(st), self.eng.table_version()   # pm_get_stats bit for bit (its timings are floats)
+
+    def same(self, a, b):
+        """untouched() before and after a restore or a certificate."""
+        assert (a[0] is None) == (b[0] is None) and (a[0] is None or all(np.array_equal(x, y) for x, y in zip(a[0], b[0]))), \
+            "pm_fetch_result changed"
+        if a[1] != b[1]:
+            was, now = abi.PmStats.from_buffer_copy(a[1]).as_dict(), abi.PmStats.from_buffer_copy(b[1]).as_dict()
+            raise AssertionError(f"pm_get_stats changed: {[(k, was[k], now[k]) for k in was if was[k] != now[k]]}")
+        assert a[2] == b[2], ("pm_table_version changed", a[2], b[2])
+
+    def restored(self, eng, report):
+        """A restore's report and what the engine reports after it, against the mirror's audit (just applied)."""
+        h = self.h
+        assert all(report[k] == v for k, v in h.last_report.items()), ("restore report", report, h.last_report)
+        price, warm, released = eng.auction_state()
+        assert np.array_equal(price, h.price) and not warm and released == 0, "restore: pm_auction_state"
+        assert eng.auction_reverse_stats() == (0, 0, 0), "restore: reverse stats"
+        assert np.array_equal(eng.auction_assignment(), h.assigned), "restore: the stored assignment"
+
+    def restore(self, x):
+        h, eng = self.h, self.eng
+        if x["export"] is not None:
+            self.export_matches(x["export"])
+        before = self.untouched()
+        for price, assigned in x["attempts"]:
+            st = h.restore_refusal(price, assigned)
+            out = {}
+            if refused(lambda: out.update(eng.auction_restore(price, assigned)), st) is not None:
+                self.stored_state_kept()
+                continue
+            assert not st, f"restore ({x['variant']}): taken, expected a refusal in {st}"
+            h.restore(price, assigned)
+            self.restored(eng, out)
+            break
+        self.same(before, self.untouched())
+
+    def restore_refused(self, x):
+        h, eng = self.h, self.eng
+        v = eng.table_version()
+        if x["export"]:
+            assert refused(lambda: eng.auction_assignment(), h.export_refusal()) is not None, (x["case"], "export taken")
+        else:
+            st = h.restore_refusal(x["price"], x["assigned"])
+            assert refused(lambda: eng.auction_restore(x["price"], x["assigned"]), st) is not None, (x["case"], "taken")
+        self.stored_state_kept()
+        assert eng.table_version() == v, (x["case"], "pm_table_version changed")
+
+    def move(self, x):
+        """Export, load a fresh engine from the mirror, restore into it, close the old engine and go on with the new."""
+        h = self.h
+        self.export_matches(x["export"])
+        fresh = new_engine(self.setting)
+        eh.load(fresh, h)
+        assert not h.restore_refusal(*x["fit"])
+        report = fresh.auction_restore(*x["fit"])
+        h.restore(*x["fit"])
+        h.discard_eval()                    # the fresh engine has no stored evaluation
+        self.restored(fresh, report)
+        self.eng.close()
+        self.eng = fresh
 
     def probe(self, t0, nt):
         """pm_build_cost_tile over asks [t0, t0 + nt) against the oracle's cost matrix (disabled rows PM_COST_INF)."""
@@ -170,9 +269,13 @@ class Runner:
 
     def step(self, ev):
         if ev[0] == "call":
+            name = ev[1][0]
+            if name in ("restore", "restore_refused", "move"):
+                getattr(self, name)(ev[1][1])
+                return
             eh.drive(self.eng, ev[1])
             self.h.apply(ev[1])
-            self.deltas |= ev[1][0] in eh.ASK_DELTAS
+            self.deltas |= name in eh.ASK_DELTAS or name == "demand"
             return
         if ev[0] == "probe":
             self.probe(*ev[1])
@@ -234,13 +337,16 @@ class ReferenceOnly:
         return getattr(self.m, name)
 
 
-MULTI_SKIP = ("reputation", "caps", "floors", "auction_params")   # the auction's columns: no pm_multi calls
+# the auction's columns and calls: no pm_multi calls
+MULTI_SKIP = ("reputation", "caps", "floors", "auction_params") + eh.AUCTION_CALLS
 
 
 def test_history_on_multi():
     """The reference side of every history on one pm_multi over every visible device: worker and ask table calls,
     refused ask deltas (PM_E_INVALID, pm_multi_table_version unchanged), toggles, locations, ranks, table swaps and
-    every reference and incremental pass, each pass against the oracle.
+    every reference and incremental pass, each pass against the oracle.  The demand, restore and move calls are skipped
+    (auction-only, no pm_multi_ form) while the mirror still applies them, which shows that the reference passes ignore
+    demands and restores; a move's fresh engine is not modelled (pm_multi keeps its stored evaluation).
     With one device the incremental passes must walk exactly the rows the mirror plans; with more, each rank's share
     moves when the worker table is resized, which the mirror does not model, so only the results are compared."""
     import torch
@@ -260,7 +366,8 @@ def test_history_on_multi():
                     if ev[0] == "call":
                         if ev[1][0] not in MULTI_SKIP:
                             eh.drive(eng, ev[1])
-                        h.apply(ev[1])
+                        if ev[1][0] != "move":
+                            h.apply(ev[1])
                         continue
                     if ev[0] != "pass" or ev[1] not in eh.REFERENCE:
                         continue
@@ -374,3 +481,21 @@ def test_a_pattern_id_of_all_ones_is_a_missing_pattern():
     eng.match(eh.MODES["warm"])
     assert eng.auction_state()[1] == 1                 # the refused auction passes kept the stored state
     eng.close()
+
+
+def test_restore_and_certificate_leave_the_launch_count():
+    """A history finding, shortened to a reference pass and a restore: with an enabled max_group_size 0 ask, a restore
+    or a certificate after a reference pass first puts that row back in the auction's form, a launch that counted in
+    pm_get_stats' n_launches although the header says neither call changes what pm_get_stats reports."""
+    import auction_restore_checker as rs
+
+    r = Runner("mixed", "default")
+    h = r.h
+    assert len(h.max0_on())
+    state = rs.adversarial_state(h.F(), h.wb["ext_ask_price"], h.cap, h.params[0], np.random.default_rng(3), h.params[1])
+    try:
+        for ev in [("pass", "lean"), ("call", ("restore", dict(variant="adversarial", export=None, attempts=[state]))),
+                   ("pass", "lean"), ("pass", "certificate")]:
+            r.step(ev)       # the restore and the certificate compare pm_get_stats before and after, bit for bit
+    finally:
+        r.close()
