@@ -32,7 +32,6 @@
 #include "pm_guard.hpp"
 #include "pm_kernels.cuh"
 #include "pm_proximity.cuh"
-#include "pm_proximity_band.cuh"
 #include "pm_proximity_grid.cuh"
 #include "pm_auction.cuh"
 #include "pm_auction_cert.cuh"
@@ -288,7 +287,8 @@ struct pm_engine {
     all_solo = n_on_not_solo == 0;
     any_max_zero = n_on_max_zero != 0;
   }
-  int tune_argmin = 0, tune_generic = 0, tune_build = 0, tune_auction = 0, tune_prox = 0, tune_auc_good = 0, tune_auc_extra = 0;   // PM_TUNE_*: kernel-shape experiments
+  int tune_generic = 0, tune_auction = 0, tune_prox = 0, tune_auc_good = 0, tune_auc_extra = 0;   // PM_TUNE_*: diagnostics
+  bool tune_wide = false;  // PM_TUNE_BUILD=8: the int64 cost tile on the FastRow path too (the 32-bit tile's reference)
   int tune_compress = 1;  // PM_TUNE_COMPRESS=0: the cost tile in plain cudaMalloc memory (A/B runs)
   bool tune_pipe = true;  // PM_TUNE_PIPE=0: the separate build + argmin launches instead of pm_build_argmin
   DevBuf<uint4> wa, wb;
@@ -439,8 +439,7 @@ struct pm_engine {
   DevBuf<uint32_t> base_len, xhead, xnext, xcount, popped, counters;  // counters: [0]=any_bad [1]=n_bumped
   DevBuf<unsigned char> cub_tmp;
   DevBuf<uint32_t> prox_list, prox_xs, members_raw;
-  DevBuf<double> prox_dist, prox_lat_key;
-  DevBuf<uint32_t> prox_lat_ord, prox_rank_of;
+  DevBuf<double> prox_dist;
   DevBuf<double> pg_part_d, pg_clat, pg_clon, pg_ccos;
   DevBuf<uint32_t> pg_part_i, pg_cta_cnt, pg_ctl;
   int coop_blocks = -1;   // co-resident CTAs of pm_proximity_grid on this device (0: cooperative launch unavailable)
@@ -922,15 +921,13 @@ int pm_create(const pm_cfg* cfg, pm_engine** out) try {
   if (e->cfg.cost_tile_bytes == 0) e->cfg.cost_tile_bytes = 8ull << 30;
   e->device = cfg->device;
   e->sms = (unsigned)std::max(1, prop.multiProcessorCount);
-  if (const char* t = std::getenv("PM_TUNE_ARGMIN")) e->tune_argmin = std::atoi(t);
   if (const char* t = std::getenv("PM_TUNE_GENERIC")) e->tune_generic = std::atoi(t);
-  if (const char* t = std::getenv("PM_TUNE_BUILD")) e->tune_build = std::atoi(t);   // 8: int64 tile on the FastRow path
+  if (const char* t = std::getenv("PM_TUNE_BUILD")) e->tune_wide = std::atoi(t) == 8;
   if (const char* t = std::getenv("PM_TUNE_AUCTION")) e->tune_auction = std::atoi(t);
   if (const char* t = std::getenv("PM_TUNE_AUCTION_POOL")) std::sscanf(t, "%d,%d", &e->tune_auc_good, &e->tune_auc_extra);   // pool fill of a class walk
-  if (const char* t = std::getenv("PM_TUNE_PROX")) e->tune_prox = std::atoi(t);   // 0: all-SM cooperative sweep; 2: single-CTA sweep; 1: latitude-banded single-CTA sweep (experimental)
+  if (const char* t = std::getenv("PM_TUNE_PROX")) e->tune_prox = std::atoi(t);   // 0: all-SM cooperative sweep; 2: single-CTA sweep
   if (const char* t = std::getenv("PM_TUNE_COMPRESS")) e->tune_compress = std::atoi(t);
   if (const char* t = std::getenv("PM_TUNE_INCR")) e->tune_incr = (uint32_t)std::strtoul(t, nullptr, 10);   // 0: always full
-  // any other value (8 / 16 / 32 / 64 set the rows per band of an earlier read-back) keeps the one launch
   if (const char* t = std::getenv("PM_TUNE_PIPE")) e->tune_pipe = std::atoi(t) != 0;
   bool ok = cudaSetDevice(e->device) == cudaSuccess;
   if (ok && cfg->stream) {
@@ -969,7 +966,6 @@ void pm_destroy(pm_engine* e) {
   e->base_len.release(); e->xhead.release(); e->xnext.release(); e->xcount.release();
   e->popped.release(); e->counters.release(); e->cub_tmp.release();
   e->prox_list.release(); e->prox_xs.release(); e->members_raw.release(); e->prox_dist.release();
-  e->prox_lat_key.release(); e->prox_lat_ord.release(); e->prox_rank_of.release();
   e->pg_part_d.release(); e->pg_part_i.release(); e->pg_cta_cnt.release(); e->pg_ctl.release();
   e->pg_clat.release(); e->pg_clon.release(); e->pg_ccos.release();
   e->nacc.release(); e->bits_wm.release();
@@ -1634,40 +1630,44 @@ static int worker_major(pm_engine* e, pm::EvalParams* p, int* bits_mode, const u
   return PM_OK;
 }
 
-// The 32-bit cost tile (pm_build_argmin, or pm_build_cost_fast<.., true> + pm_argmin<.., true> under PM_TUNE_PIPE=0 and
-// PM_TUNE_BUILD=5 / 6): on the default FastRow path, for tables
-// whose every price is below 0x7FFFFFFF (decide_fast).  The staged kernels (PM_TUNE_BUILD = 1, 3, 4), the generic
-// predicate and other prices keep the int64 tile; PM_TUNE_BUILD=8 keeps it on the FastRow path too, for A/B runs.
+// The predicate variant of every evaluation pass: `p` from eval_params, `bits_mode` from the acceptance table's size
+// (2: one word per row, 1: the table in shared memory, 0: in global memory), the fast predicate when decide_fast
+// allows it, and then the worker-major one-word table where the global-memory one would run (worker_major; p->nacc
+// is set exactly then).  `rows` as in decide_fast.
+static int pick_predicate(pm_engine* e, pm::EvalParams* p, int* bits_mode, bool* fast, const uint32_t* rows = nullptr,
+                          uint32_t n_rows = 0) {
+  *p = eval_params(e);
+  *bits_mode = ((uint64_t)p->n_bits_rows * p->words <= (uint64_t)pm::kBitsCap) ? (p->words == 1 ? 2 : 1) : 0;
+  const int rc = decide_fast(e, fast, rows, n_rows);
+  if (rc != PM_OK) return rc;
+  if (*fast && *bits_mode == 0 && p->n_bits_rows <= 31u) return worker_major(e, p, bits_mode, rows, n_rows);
+  return PM_OK;
+}
+
+// The 32-bit cost tile (pm_build_argmin, or pm_build_cost_fast<.., true> + pm_argmin<.., true> under PM_TUNE_PIPE=0):
+// on the FastRow path, for tables whose every price is below 0x7FFFFFFF (decide_fast).  The generic predicate and
+// other prices keep the int64 tile; PM_TUNE_BUILD=8 keeps it on the FastRow path too, for A/B runs.
 static bool narrow_tile(const pm_engine* e, bool fast) {
-  const int tb = e->tune_build;
-  return fast && e->prices_narrow && tb != 1 && tb != 3 && tb != 4 && tb != 8;
+  return fast && e->prices_narrow && !e->tune_wide;
 }
 
 static void launch_build(pm_engine* e, const pm::EvalParams& p, int bits_mode, bool fast, bool narrow, dim3 grid,
                          uint32_t t0, uint32_t nt, uint32_t w0, uint32_t nw, long long* tile, size_t ld) {
-#define PM_BUILD_CASE(B, F) pm::pm_build_cost<B, F><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, t0, nt, w0, nw, tile, ld)
-#define PM_FAST_CASE(B, R)                                                                                              \
+#define PM_BUILD_CASE(B) pm::pm_build_cost<B><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, t0, nt, w0, nw, tile, ld)
+#define PM_FAST_CASE(B)                                                                                                 \
   {                                                                                                                     \
-    grid.y = blocks_for(nt, R);                                                                                         \
-    if (narrow) pm::pm_build_cost_fast<B, R, true><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, t0, nt, w0, nw, tile, ld);   \
-    else pm::pm_build_cost_fast<B, R, false><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, t0, nt, w0, nw, tile, ld);         \
+    grid.y = blocks_for(nt, pm::kFastRows);                                                                             \
+    if (narrow) pm::pm_build_cost_fast<B, true><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, t0, nt, w0, nw, tile, ld);      \
+    else pm::pm_build_cost_fast<B, false><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, t0, nt, w0, nw, tile, ld);            \
   }
-  if (fast && bits_mode == 2 && e->tune_build == 3) {
-    pm::pm_build_cost<2, true, 3><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, t0, nt, w0, nw, tile, ld);
-  } else if (fast && bits_mode == 2 && e->tune_build == 4) {
-    pm::pm_build_cost<2, true, 4><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, t0, nt, w0, nw, tile, ld);
-  } else if (fast && e->tune_build != 1) {   // the FastRow kernel; PM_TUNE_BUILD=1 keeps the staged-CSR form for A/B runs
+  if (fast) {   // the FastRow kernel
     // one-word acceptance rows are bound into the FastRows (pm_bind_rows) however many rows there are
     if (p.words == 1) bits_mode = 2;
-    if (bits_mode == 2 && e->tune_build == 5) PM_FAST_CASE(2, 128)          // rows-per-CTA experiments (tools/tune.py)
-    else if (bits_mode == 2 && e->tune_build == 6) PM_FAST_CASE(2, 256)
-    else if (bits_mode == 2) PM_FAST_CASE(2, pm::kFastRows)
-    else if (bits_mode == 1) PM_FAST_CASE(1, pm::kFastRows)
-    else PM_FAST_CASE(0, pm::kFastRows)
-  } else if (fast) {
-    if (bits_mode == 2) PM_BUILD_CASE(2, true); else if (bits_mode == 1) PM_BUILD_CASE(1, true); else PM_BUILD_CASE(0, true);
+    if (bits_mode == 2) PM_FAST_CASE(2)
+    else if (bits_mode == 1) PM_FAST_CASE(1)
+    else PM_FAST_CASE(0)
   } else {
-    if (bits_mode == 2) PM_BUILD_CASE(2, false); else if (bits_mode == 1) PM_BUILD_CASE(1, false); else PM_BUILD_CASE(0, false);
+    if (bits_mode == 2) PM_BUILD_CASE(2); else if (bits_mode == 1) PM_BUILD_CASE(1); else PM_BUILD_CASE(0);
   }
 #undef PM_FAST_CASE
 #undef PM_BUILD_CASE
@@ -1700,31 +1700,16 @@ static void launch_build_argmin(pm_engine* e, const pm::EvalParams& p, int bits_
 
 static void launch_argmin(pm_engine* e, cudaStream_t st, bool narrow, const long long* tile, size_t ld, uint32_t nt,
                           uint32_t t0, uint32_t w0, uint32_t nw) {
-  if (narrow) {   // 16 x 16 B in flight per lane, as the wide <8, 2>; PM_TUNE_ARGMIN shapes the int64 tile's kernel only
+  // 16 x 16 B in flight per lane in both widths: a warp's slice is 8 x 128 columns of the 32-bit tile, 8 x 64 of the int64
+  if (narrow) {
     dim3 grid(blocks_for(ld, 8 * 128 * pm::kArgWarps), blocks_for(nt, pm::kArgRows));
     pm::pm_argmin<8, 2, true><<<grid, pm::kArgThreads, 0, st>>>(tile, ld, nt, t0, w0, nw, e->first_ask.p,
                                                                e->ask_best.p, e->ask_count.p);
-    return;
+  } else {
+    dim3 grid(blocks_for(ld, 8 * 64 * pm::kArgWarps), blocks_for(nt, pm::kArgRows));
+    pm::pm_argmin<8, 2, false><<<grid, pm::kArgThreads, 0, st>>>(tile, ld, nt, t0, w0, nw, e->first_ask.p,
+                                                                e->ask_best.p, e->ask_count.p);
   }
-#define PM_ARGMIN_CASE(S, RPW)                                                                      \
-  {                                                                                                  \
-    dim3 grid(blocks_for(ld, (S) * 64 * pm::kArgWarps), blocks_for(nt, pm::kArgRows));                               \
-    pm::pm_argmin<S, RPW><<<grid, pm::kArgThreads, 0, st>>>(tile, ld, nt, t0, w0, nw,                \
-                                                                   e->first_ask.p, e->ask_best.p,   \
-                                                                   e->ask_count.p);                 \
-  }
-  switch (e->tune_argmin) {
-    case 1: PM_ARGMIN_CASE(4, 1) break;
-    case 2: PM_ARGMIN_CASE(4, 2) break;
-    case 3: PM_ARGMIN_CASE(8, 2) break;
-    case 4: PM_ARGMIN_CASE(4, 4) break;
-    case 5: PM_ARGMIN_CASE(8, 1) break;
-    case 6: PM_ARGMIN_CASE(8, 4) break;
-    case 7: PM_ARGMIN_CASE(16, 1) break;
-    case 8: PM_ARGMIN_CASE(16, 2) break;
-    default: PM_ARGMIN_CASE(8, 2) break;
-  }
-#undef PM_ARGMIN_CASE
 }
 
 // The incremental evaluation.  Three walks (pm_first_ask_rows) rewrite the stored per-worker first feasible ask; each
@@ -1775,16 +1760,11 @@ static int eval_incremental(pm_engine* e, const std::vector<uint32_t>& en, const
     uint32_t* rows = e->dirty_dev.p + (one_list ? 0 : kp);
     PM_CUDA(e->incr_evals.ensure(1));
     PM_CUDA(cudaMemsetAsync(e->incr_evals.p, 0, 8, e->stream));
-    pm::EvalParams p = eval_params(e);
-    int bits_mode = ((uint64_t)p.n_bits_rows * p.words <= (uint64_t)pm::kBitsCap) ? (p.words == 1 ? 2 : 1) : 0;
+    pm::EvalParams p;
+    int bits_mode = 0;
     bool fast = false;
     {
-      const int rc = decide_fast(e, &fast, pre, kp);
-      if (rc != PM_OK) return rc;
-    }
-    const bool wm = fast && bits_mode == 0 && p.n_bits_rows <= 31u && e->tune_build != 7;   // as the full pass
-    if (wm) {
-      const int rc = worker_major(e, &p, &bits_mode, pre, kp);
+      const int rc = pick_predicate(e, &p, &bits_mode, &fast, pre, kp);
       if (rc != PM_OK) return rc;
     }
     auto walk = [&](const pm::AskWalk& a, dim3 grid) -> int {
@@ -1902,16 +1882,11 @@ static int match_local_locked(pm_engine* e, uint32_t mode) {
     const int rc = eval_incremental(e, en, dis);
     if (rc != PM_OK) return rc;
   } else if (T && nw) {
-    pm::EvalParams p = eval_params(e);
-    int bits_mode = ((uint64_t)p.n_bits_rows * p.words <= (uint64_t)pm::kBitsCap) ? (p.words == 1 ? 2 : 1) : 0;
+    pm::EvalParams p;
+    int bits_mode = 0;
     bool fast = false;
     {
-      int rc = decide_fast(e, &fast);
-      if (rc != PM_OK) return rc;
-    }
-    const bool wm = fast && bits_mode == 0 && p.n_bits_rows <= 31u && e->tune_build != 7;   // PM_TUNE_BUILD=7: keep the global-memory table
-    if (wm) {
-      const int rc = worker_major(e, &p, &bits_mode);
+      const int rc = pick_predicate(e, &p, &bits_mode, &fast);
       if (rc != PM_OK) return rc;
     }
     if (mode & PM_PATH_FUSED) {
@@ -1931,7 +1906,7 @@ static int match_local_locked(pm_engine* e, uint32_t mode) {
       // the columns past the shard hold "infeasible" and cost 0.05 % of a 1M-worker row
       const size_t ld = (((size_t)nw + pm::kEvalCols - 1) / pm::kEvalCols) * pm::kEvalCols;
       {
-        const int rc = bind_rows(e, wm);
+        const int rc = bind_rows(e, p.nacc != nullptr);
         if (rc != PM_OK) return rc;
       }
       // rows are sized by 8 B per element for both widths: the 32-bit tile covers the same asks in half the bytes, so
@@ -1948,9 +1923,9 @@ static int match_local_locked(pm_engine* e, uint32_t mode) {
         cudaGetLastError();
         return e->fail(PM_E_NOMEM, "pm_match: cannot allocate the cost tile; lower pm_cfg.cost_tile_bytes");
       }
-      // One launch per tile (pm_build_argmin) wherever the 32-bit tile runs, unless PM_TUNE_PIPE=0 or a rows-per-CTA
-      // experiment (PM_TUNE_BUILD=5 / 6) asks for the separate build and argmin
-      const bool pipe = narrow && e->tune_pipe && e->tune_build != 5 && e->tune_build != 6;
+      // One launch per tile (pm_build_argmin) wherever the 32-bit tile runs, unless PM_TUNE_PIPE=0 asks for the
+      // separate build and argmin
+      const bool pipe = narrow && e->tune_pipe;
       if (pipe) {   // each column's rank within its stripe, from this pass's prices (ordered after any table update)
         PM_CUDA(e->stripe_rank.ensure(ld));
         PM_CUDA(e->rank_best.ensure(ld));
@@ -2113,13 +2088,6 @@ static int match_finish_locked(pm_engine* e, uint32_t mode) {
       PM_CUDA(cudaLaunchCooperativeKernel((const void*)pm::pm_proximity_grid, dim3(grid), dim3(pm::kPgThreads), args, 0, e->stream));
       PM_CUDA(cudaMemcpyAsync(e->h_scalars.p + 24, e->pg_ctl.p + 4, 12, cudaMemcpyDeviceToHost, e->stream));
       prox_grid_ran = true;
-    }
-    else if (e->tune_prox & 1) {   // experimental: same groups from a latitude-ordered view (pm_proximity_band.cuh)
-      PM_CUDA(e->prox_lat_key.ensure(P)); PM_CUDA(e->prox_lat_ord.ensure(P)); PM_CUDA(e->prox_rank_of.ensure(W));
-      pm::BandParams bp;
-      bp.p = pp;
-      bp.lat_key = e->prox_lat_key.p; bp.lat_ord = e->prox_lat_ord.p; bp.rank_of = e->prox_rank_of.p;
-      pm::pm_proximity_sweep_banded<<<1, pm::kProxThreads, 0, e->stream>>>(bp);
     }
     else pm::pm_proximity_sweep<<<1, pm::kProxThreads, 0, e->stream>>>(pp);
     PM_LAUNCH_CHECK("pm_proximity_sweep");
@@ -2851,15 +2819,11 @@ static int cert_launch(pm_engine* e, const long long* price, const uint32_t* ass
     cs.assigned = e->cert_none.p;
   }
   if (T && W) {   // the fused pass's predicate variant (pm_match, PM_PATH_FUSED)
-    pm::EvalParams p = eval_params(e);
-    int bits_mode = ((uint64_t)p.n_bits_rows * p.words <= (uint64_t)pm::kBitsCap) ? (p.words == 1 ? 2 : 1) : 0;
+    pm::EvalParams p;
+    int bits_mode = 0;
     bool fast = false;
-    int rc = decide_fast(e, &fast);
+    const int rc = pick_predicate(e, &p, &bits_mode, &fast);
     if (rc != PM_OK) return rc;
-    if (fast && bits_mode == 0 && p.n_bits_rows <= 31u && e->tune_build != 7) {
-      rc = worker_major(e, &p, &bits_mode);
-      if (rc != PM_OK) return rc;
-    }
     const uint32_t rows_per_launch = 65535u * pm::kEvalRows;
     for (uint32_t t0 = 0; t0 < T; t0 += rows_per_launch) {
       const uint32_t nt = std::min(rows_per_launch, T - t0);
@@ -3389,19 +3353,14 @@ int pm_build_cost_tile(pm_engine* e, uint32_t t0, uint32_t nt, int64_t* host_out
     cudaGetLastError();
     return e->fail(PM_E_NOMEM, "pm_build_cost_tile: cannot allocate the tile");
   }
-  pm::EvalParams p = eval_params(e);
   dim3 grid(blocks_for(ld, pm::kEvalCols), blocks_for(nt, pm::kEvalRows));
+  pm::EvalParams p;
+  int bits_mode = 0;
   bool fast = false;
-  int bits_mode = ((uint64_t)p.n_bits_rows * p.words <= (uint64_t)pm::kBitsCap) ? (p.words == 1 ? 2 : 1) : 0;
   {
-    int rc = decide_fast(e, &fast);
+    int rc = pick_predicate(e, &p, &bits_mode, &fast);
     if (rc != PM_OK) return rc;
-    const bool wm = fast && bits_mode == 0 && p.n_bits_rows <= 31u && e->tune_build != 7;   // as pm_match
-    if (wm) {
-      rc = worker_major(e, &p, &bits_mode);
-      if (rc != PM_OK) return rc;
-    }
-    rc = bind_rows(e, wm);
+    rc = bind_rows(e, p.nacc != nullptr);
     if (rc != PM_OK) return rc;
   }
   launch_build(e, p, bits_mode, fast, false, grid, t0, nt, w0, nw, e->cost.p, ld);   // exports the int64 tile

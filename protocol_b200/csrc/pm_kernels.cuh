@@ -252,10 +252,9 @@ __device__ __forceinline__ void for_each_staged_row(EvalStage& s, const EvalPara
 // the staged asks, emitting two 128-bit streaming stores per row: a warp writes 1 KB
 // contiguous (two fully coalesced 512-byte stores), the CTA 8 KB contiguous per row.
 // ld is a multiple of the CTA's 1024 columns (columns past the shard hold the "infeasible" pattern of a null
-// worker), so the stores need no bounds test.  Fast form: the packed cost is formed from the predicate's sign bit
-// with one shift and two multiply-adds per worker — no compare, no select (see DevOptF).
-template <int BITS, bool FAST, int MINB = 2>
-__global__ void __launch_bounds__(kEvalThreads, MINB)
+// worker), so the stores need no bounds test.
+template <int BITS>
+__global__ void __launch_bounds__(kEvalThreads, 2)
 pm_build_cost(EvalParams p, uint32_t t0, uint32_t nt, uint32_t w0, uint32_t nw,
               long long* __restrict__ cost, size_t ld) {
   __shared__ EvalStage s;
@@ -266,7 +265,7 @@ pm_build_cost(EvalParams p, uint32_t t0, uint32_t nt, uint32_t w0, uint32_t nw,
   const uint32_t lane = threadIdx.x & 31u;
   const uint32_t cbase = blockIdx.x * kEvalCols + (threadIdx.x >> 5) * 128u + lane * 2u;
   WorkerReg w[kEvalWPT];
-  uint32_t gw[kEvalWPT], dx[kEvalWPT], dy[kEvalWPT];
+  uint32_t gw[kEvalWPT];
 #pragma unroll
   for (int k = 0; k < kEvalWPT; ++k) {
     const uint32_t col = cbase + (k >> 1) * 64u + (k & 1);
@@ -275,32 +274,19 @@ pm_build_cost(EvalParams p, uint32_t t0, uint32_t nt, uint32_t w0, uint32_t nw,
       w[k] = make_worker(__ldg(p.wa + w0 + col), __ldg(p.wb + w0 + col));
       if (p.nacc) w[k].mmask = __ldg(p.nacc + w0 + col);
     } else w[k] = null_worker();
-    dx[k] = 0xFFFFFFFFu - gw[k];          // infeasible: 0x7FFFFFFF_FFFFFFFF = feasible word + (0/1) * difference
-    dy[k] = 0x7FFFFFFFu - w[k].price;
   }
   uint4* out = reinterpret_cast<uint4*>(cost + (size_t)r0 * ld + cbase);
   const size_t row_stride = ld / 2;   // in 16-byte units; rows are visited in increasing order
-  for_each_staged_row(s, p, FAST, t0, r0, r1, [&](uint32_t, const DevAsk& a, uint32_t obegin, bool staged) {
+  for_each_staged_row(s, p, false, t0, r0, r1, [&](uint32_t, const DevAsk& a, uint32_t obegin, bool staged) {
     uint4 v0, v1;
     // feasible: (price << 32) | worker ; infeasible: 0x7FFFFFFF_FFFFFFFF
-    if (FAST && staged) {
-      uint32_t fail[kEvalWPT];
-      eval_row_fast<kEvalWPT, BITS>(s, a, obegin, w, p.bits, p.words, fail);
-      const uint32_t sh = p.sign_shift;
-      const uint32_t b0 = fail[0] >> sh, b1 = fail[1] >> sh, b2 = fail[2] >> sh, b3 = fail[3] >> sh;
-      v0.x = b0 * dx[0] + gw[0]; v0.y = b0 * dy[0] + w[0].price;
-      v0.z = b1 * dx[1] + gw[1]; v0.w = b1 * dy[1] + w[1].price;
-      v1.x = b2 * dx[2] + gw[2]; v1.y = b2 * dy[2] + w[2].price;
-      v1.z = b3 * dx[3] + gw[3]; v1.w = b3 * dy[3] + w[3].price;
-    } else {
-      uint32_t f[kEvalWPT];
-      if (staged) eval_row<kEvalWPT, BITS>(s, a, obegin, w, p.bits, p.words, f);
-      else eval_row_global<kEvalWPT>(p, a, w, f);
-      v0.x = gw[0] | ~f[0]; v0.y = (w[0].price & f[0]) | (0x7FFFFFFFu & ~f[0]);
-      v0.z = gw[1] | ~f[1]; v0.w = (w[1].price & f[1]) | (0x7FFFFFFFu & ~f[1]);
-      v1.x = gw[2] | ~f[2]; v1.y = (w[2].price & f[2]) | (0x7FFFFFFFu & ~f[2]);
-      v1.z = gw[3] | ~f[3]; v1.w = (w[3].price & f[3]) | (0x7FFFFFFFu & ~f[3]);
-    }
+    uint32_t f[kEvalWPT];
+    if (staged) eval_row<kEvalWPT, BITS>(s, a, obegin, w, p.bits, p.words, f);
+    else eval_row_global<kEvalWPT>(p, a, w, f);
+    v0.x = gw[0] | ~f[0]; v0.y = (w[0].price & f[0]) | (0x7FFFFFFFu & ~f[0]);
+    v0.z = gw[1] | ~f[1]; v0.w = (w[1].price & f[1]) | (0x7FFFFFFFu & ~f[1]);
+    v1.x = gw[2] | ~f[2]; v1.y = (w[2].price & f[2]) | (0x7FFFFFFFu & ~f[2]);
+    v1.z = gw[3] | ~f[3]; v1.w = (w[3].price & f[3]) | (0x7FFFFFFFu & ~f[3]);
     __stcs(out, v0);
     __stcs(out + 32, v1);     // + 64 columns
     out += row_stride;
@@ -349,14 +335,12 @@ __device__ __forceinline__ void eval_fast_more(const DevOptF* __restrict__ gopts
   }
 }
 
-template <int ROWS>
+constexpr int kFastRows = 512;   // asks per CTA: the prologue (worker rows from L2, the TMA of the FastRows) is paid once per CTA
 struct __align__(128) FastStage {
-  FastRow row[ROWS + 2];   // + 2: the look-ahead loads of the last pair of rows may read past it (never used)
+  FastRow row[kFastRows + 2];   // + 2: the look-ahead loads of the last pair of rows may read past it (never used)
   uint32_t bits[kBitsCap];
   uint64_t bar;
 };
-constexpr int kFastRows = 512;   // asks per CTA: the prologue (worker rows from L2, the TMA of the FastRows) is paid once per CTA
-                                 // (PM_TUNE_BUILD=5 / 6 select 128 / 256 rows for comparison)
 
 // NARROW: the tile holds only the 32-bit cost word — the worker's price when feasible, kNarrowInfeasible when not — and
 // `tile` is uint32_t[rows][ld].  The worker index the wide element carries in its low word is the column (+ w0), which
@@ -375,19 +359,19 @@ struct FoldOut {
   uint32_t* ask_count;
 };
 
-template <int BITS, int ROWS, bool NARROW, bool PIPE>
+template <int BITS, bool NARROW, bool PIPE>
 __device__ __forceinline__ void build_fast(const EvalParams& p, uint32_t t0, uint32_t nt, uint32_t w0, uint32_t nw,
                                            void* __restrict__ tile, size_t ld, const FoldOut& fo) {
   static_assert(!PIPE || NARROW, "the row fold ranks the 32-bit tile's columns");
-  __shared__ FastStage<ROWS> s;
+  __shared__ FastStage s;
   // PIPE: per warp and row of the CTA, the warp's least key (the least stripe rank of its feasible columns, or
   // kNoRank and more when it has none) and its infeasible columns — plain stores, no atomics; 12 KB at 512 rows
   constexpr int kWarps = kEvalThreads / 32;
   constexpr uint32_t kNoRank = 0x8000u;   // added to an infeasible column's rank (< 1024): the key still fits 16 bits
-  __shared__ uint16_t s_key[PIPE ? kWarps : 1][PIPE ? ROWS : 1];
-  __shared__ uint8_t s_nb[PIPE ? kWarps : 1][PIPE ? ROWS : 1];
-  const uint32_t r0 = blockIdx.y * ROWS;
-  const uint32_t nrows = min(nt - r0, (uint32_t)ROWS);
+  __shared__ uint16_t s_key[PIPE ? kWarps : 1][PIPE ? kFastRows : 1];
+  __shared__ uint8_t s_nb[PIPE ? kWarps : 1][PIPE ? kFastRows : 1];
+  const uint32_t r0 = blockIdx.y * kFastRows;
+  const uint32_t nrows = min(nt - r0, (uint32_t)kFastRows);
   if (threadIdx.x == 0) {
     mbar_init(&s.bar, 1);
     mbar_expect_tx(&s.bar, nrows * (uint32_t)sizeof(FastRow));
@@ -516,14 +500,14 @@ __device__ __forceinline__ void build_fast(const EvalParams& p, uint32_t t0, uin
   }
 }
 
-template <int BITS, int ROWS = kFastRows, bool NARROW = false>
+template <int BITS, bool NARROW>
 __global__ void __launch_bounds__(kEvalThreads, 2)
 pm_build_cost_fast(EvalParams p, uint32_t t0, uint32_t nt, uint32_t w0, uint32_t nw, void* __restrict__ tile, size_t ld) {
-  build_fast<BITS, ROWS, NARROW, false>(p, t0, nt, w0, nw, tile, ld, FoldOut{});
+  build_fast<BITS, NARROW, false>(p, t0, nt, w0, nw, tile, ld, FoldOut{});
 }
 
 // ------------------------------------------------------------------ build + argmin, one kernel
-// pm_build_cost_fast<BITS, kFastRows, true> and pm_argmin<.., true>'s outputs in one pass: the tile is written with
+// pm_build_cost_fast<BITS, true> and pm_argmin<.., true>'s outputs in one pass: the tile is written with
 // streaming stores, as the build writes it, and never read back.  Within a 1024-column stripe the packed minimum
 // (word << 32) | (w0 + column) over the feasible columns orders them by (price, column) whatever the ask, so a
 // column's rank in that order (pm_stripe_rank, once per pass) stands for its packed cost.  Per row and lane the
@@ -536,7 +520,7 @@ template <int BITS>
 __global__ void __launch_bounds__(kEvalThreads, 2)
 pm_build_argmin(EvalParams p, uint32_t t0, uint32_t nt, uint32_t w0, uint32_t nw, uint32_t* __restrict__ tile, size_t ld,
                 FoldOut fo) {
-  build_fast<BITS, kFastRows, true, true>(p, t0, nt, w0, nw, tile, ld, fo);
+  build_fast<BITS, true, true>(p, t0, nt, w0, nw, tile, ld, fo);
 }
 
 // One CTA per 1024-column stripe of a tile with leading dimension ld: sorts the stripe's (price, column) pairs —

@@ -292,36 +292,6 @@ def test_proximity_groups_at_100k_workers():
     eng.close()
 
 
-@pytest.mark.skipif(__import__("os").environ.get("PM_TEST_EXPERIMENTAL") != "1",
-                    reason="experimental latitude-banded sweep (PM_TUNE_PROX=1): run with PM_TEST_EXPERIMENTAL=1")
-@pytest.mark.parametrize("n_asks,n_workers,where", [(120, 4000, "cities"), (120, 4000, "scattered"), (50, 3000, "one_point"),
-                                                     (2000, 100_000, "scattered")])
-def test_experimental_banded_proximity_sweep(n_asks, n_workers, where, monkeypatch):
-    """pm_proximity_sweep_banded (off by default) must form the groups of the literal sweep / the checker: city
-    clusters (every distance tied: list position decides), scattered coordinates (no near-ties asserted for the
-    exact comparison of different libm's), everybody on one point, and the 100k x 2000 size of test_proximity_groups_at_100k_workers."""
-    monkeypatch.setenv("PM_TUNE_PROX", "1")
-    sizes = [(1, 1), (2, 2), (2, 4), (3, 3), (4, 8), (1, 3), (0, 2), (2, 5)]
-    w, a, t = synth_tables(n_asks, n_workers, "mixed", group_sizes=sizes, with_addresses=True, seed_shift=7)
-    rng = np.random.default_rng(7)
-    lat, lon = w.lat.copy(), w.lon.copy()
-    if where == "scattered":
-        lat = lat + rng.normal(0, 3.0, len(lat)).clip(-20, 20)
-        lon = lon + rng.normal(0, 5.0, len(lon))
-    elif where == "one_point":
-        lat[:] = 45.5
-        lon[:] = -73.5
-    t["lat"], t["lon"] = lat, lon
-    eng = Engine()
-    load_engine(eng, t, addr_rank=w.addr_rank, locations=True)
-    eng.match(abi.PM_MODE_PROXIMITY)
-    res = eng.fetch()
-    og = orc.soa_form_groups(t["wa"], t["wb"], t["asks"], t["opts"], t["bits"], t["words"], addr_rank=w.addr_rank,
-                             lat=lat, lon=lon, proximity="banded")
-    assert groups_equal(res, og), f"groups differ: engine {res.n_groups} vs checker {len(og)}"
-    eng.close()
-
-
 def test_proximity_montreal_dallas_on_device():
     """The coordinates of node_groups/tests.rs:2861-3064: interleaved arrivals still pair by city."""
     tb = TableBuilder()

@@ -1,8 +1,8 @@
 """Every selectable cost-kernel variant of the first-fit pass, with priced workers, against the CPU oracle.
 
 ask_best is each ask's signed int64 least (price << 32) | worker over the workers that meet it (PM_COST_INF when none
-does) on every path: the int64 and the 32-bit tile with each build kernel (PM_TUNE_BUILD) and argmin shape
-(PM_TUNE_ARGMIN), the generic predicate, the double-buffered tiles, plain tile memory, and the fused pass.  Prices
+does) on every path: the 32-bit tile, the int64 tile on the FastRow path (PM_TUNE_BUILD=8), the generic predicate,
+plain tile memory, and the fused pass.  Prices
 are where a row minimum goes wrong quietly: ties must go to the lowest worker, and prices of 2^31 and above make the
 packed cost negative.  Each case runs one engine and compares with the oracle (soa_eval_matrix, soa_form_groups):
   * the per-worker first feasible ask and the per-ask (best, count), read from the engine's device buffers;
@@ -35,10 +35,8 @@ TILE = 1 << 20
 # name -> (PM_TUNE_* environment read at pm_create, mode)
 VARIANTS = {
     "default": ({}, MAT),                                             # FastRow build, 32-bit tile when prices allow
-    **{f"build{b}": ({"PM_TUNE_BUILD": str(b)}, MAT) for b in (8, 1, 3, 4, 5, 6, 7)},
-    **{f"build8_argmin{k}": ({"PM_TUNE_BUILD": "8", "PM_TUNE_ARGMIN": str(k)}, MAT) for k in range(1, 9)},
+    "build8": ({"PM_TUNE_BUILD": "8"}, MAT),                          # the int64 tile on the FastRow path
     "generic": ({"PM_TUNE_GENERIC": "1"}, MAT),
-    "overlap": ({"PM_TUNE_OVERLAP": "1"}, MAT),
     "plain_memory": ({"PM_TUNE_COMPRESS": "0"}, MAT),
     "fused": ({}, FUSED),
     "fused_generic": ({"PM_TUNE_GENERIC": "1"}, FUSED),
@@ -119,8 +117,8 @@ def case(form, price):
 
 def narrow_expected(env, t):
     """The engine's width selection: the FastRow build with every price below 0x7FFFFFFF takes the 32-bit tile."""
-    b = int(env.get("PM_TUNE_BUILD", "0"))
-    return env.get("PM_TUNE_GENERIC") != "1" and b not in (1, 3, 4, 8) and int(t["wb"]["ext_ask_price"].max()) < 0x7FFFFFFF
+    return (env.get("PM_TUNE_GENERIC") != "1" and env.get("PM_TUNE_BUILD") != "8"
+            and int(t["wb"]["ext_ask_price"].max()) < 0x7FFFFFFF)
 
 
 def run_variant(t, ev, og, variant):
@@ -151,28 +149,26 @@ def run_variant(t, ev, og, variant):
 
 
 @pytest.mark.parametrize("price", PRICES)
-@pytest.mark.parametrize("variant", [v for v in VARIANTS if v != "build7"])
+@pytest.mark.parametrize("variant", list(VARIANTS))
 def test_variant_ragged_multi_tile(variant, price):
     """613 asks x 6007 workers in 29 tiles, one-word acceptance rows (BITS 2)."""
     run_variant(*case("ragged", price), variant)
 
 
-COMMON = ["default", "build8", "build1", "generic", "fused", "fused_generic", "fused_lean"]
-FORM_VARIANTS = [(f, v) for f in ("bits2", "bits1", "bits0", "worker_major") for v in COMMON] + \
-                [("bits2", v) for v in ("build3", "build4", "build5", "build6", "build8_argmin1", "build8_argmin8")] + \
-                [("worker_major", "build7"), ("bits0", "build8_argmin7")]
+COMMON = ["default", "build8", "generic", "fused", "fused_generic", "fused_lean"]
+FORM_VARIANTS = [(f, v) for f in ("bits2", "bits1", "bits0", "worker_major") for v in COMMON]
 
 
 @pytest.mark.parametrize("price", ["zipf", "sign"])
 @pytest.mark.parametrize("form,variant", FORM_VARIANTS)
 def test_variant_acceptance_forms(form, variant, price):
     """Wide catalogues: acceptance rows of one word (BITS 2), per worker in shared memory (1), in global memory (0),
-    and the worker-major table (PM_TUNE_BUILD=7 keeps the global-memory one instead)."""
+    and the worker-major table."""
     run_variant(*case(form, price), variant)
 
 
 @pytest.mark.parametrize("price", ["zipf", "sign"])
-@pytest.mark.parametrize("variant", ["default", "build8", "build1", "generic", "fused", "fused_generic"])
+@pytest.mark.parametrize("variant", ["default", "build8", "generic", "fused", "fused_generic"])
 @pytest.mark.parametrize("n_models", [16, 200])
 def test_variant_more_options_than_the_stage_holds(n_models, variant, price):
     """Asks with 384, 385, 400, 500 and 1200 OR-options: the staged kernels evaluate those beyond 384 with
@@ -181,7 +177,7 @@ def test_variant_more_options_than_the_stage_holds(n_models, variant, price):
 
 
 @pytest.mark.parametrize("price", ["zipf", "sign"])
-@pytest.mark.parametrize("variant", ["default", "build1", "generic"])
+@pytest.mark.parametrize("variant", ["default", "generic"])
 @pytest.mark.parametrize("form", ["ragged", "worker_major"])
 def test_exported_cost_rows(form, variant, price):
     """pm_build_cost_tile: the int64 rows, bit-equal to the oracle's packed costs, negative ones included."""

@@ -4,8 +4,8 @@
 and member order equal the CPU checker's on every shape the sweep has a special path for — ties everywhere (city
 clusters, one point), scattered coordinates, nobody located, groups larger than one selection pass (16), empty
 groups (min 0), long hand-downs between configurations (ordered compaction), solo configurations after grouped ones.
-The edges of the coordinate space (EDGES: poles, antimeridian, antipodes, latitudes beyond ±90) run on these and on
-the experimental latitude-banded sweep (PM_TUNE_PROX=1), whose pruning must switch off where the latitude bound fails.
+The edges of the coordinate space (EDGES: poles, antimeridian, antipodes, latitudes beyond ±90) run on both, and the
+grid sweep's latitude pruning must switch off where the latitude bound fails.
 Past the first stride (thousands of configurations, hand-downs across the shared-memory limit, seed-parallel batches on
 many CTAs, selections in several chunks of 16): tests/test_gpu_proximity_sweeps.py.
 """
@@ -23,7 +23,6 @@ from protocol_b200.engine import Engine, Interner
 pytestmark = pytest.mark.gpu
 
 KERNELS = [("0", "grid"), ("2", "single_cta")]
-BANDED = ("1", "banded")      # the experimental latitude-banded single-CTA sweep
 EDGES = ["polar", "antimeridian", "antipodal", "beyond_90"]
 R_KM = 6371.0
 KM_PER_DEG = R_KM * np.pi / 180.0
@@ -224,7 +223,7 @@ def run(kernel, w, a, checker="banded"):
     return res, og
 
 
-@pytest.mark.parametrize("kernel", [k for k, _ in KERNELS + [BANDED]], ids=[n for _, n in KERNELS + [BANDED]])
+@pytest.mark.parametrize("kernel", [k for k, _ in KERNELS], ids=[n for _, n in KERNELS])
 @pytest.mark.parametrize("where", ["cities", "scattered", "one_point", "nowhere"] + EDGES)
 def test_mixed_group_sizes(kernel, where):
     sizes = [(1, 1), (2, 2), (2, 4), (3, 3), (4, 8), (1, 3), (0, 2), (2, 5), (0, 1)]
@@ -234,13 +233,13 @@ def test_mixed_group_sizes(kernel, where):
     assert res.n_groups > 50
 
 
-@pytest.mark.parametrize("kernel", [k for k, _ in KERNELS + [BANDED]], ids=[n for _, n in KERNELS + [BANDED]])
+@pytest.mark.parametrize("kernel", [k for k, _ in KERNELS], ids=[n for _, n in KERNELS])
 @pytest.mark.parametrize("where", EDGES)
 def test_pairs_at_coordinate_edges(kernel, where):
-    """Everybody competes for pairs, so the seed-parallel batches with their latitude pruning (grid) and the banded
-    windows (more than 1 024 located candidates) both run.  The first located candidates hold one special point each:
-    under "beyond_90" every other seed's nearest neighbour is 1 km away but written beyond ±90, more than 4 000 km
-    away by R·|Δlatitude| — a sweep that kept pruning by latitude would pass it over."""
+    """Everybody competes for pairs, so the seed-parallel batches with their latitude pruning (grid) run.  The first
+    located candidates hold one special point each: under "beyond_90" every other seed's nearest neighbour is 1 km
+    away but written beyond ±90, more than 4 000 km away by R·|Δlatitude| — a sweep that kept pruning by latitude
+    would pass it over."""
     w = swarm(4000, where, seed_shift=5)
     a = custom_asks([(None, 2, 2), (None, 1, 1)])
     res, og = run(kernel, w, a)
@@ -257,7 +256,7 @@ def haversine_pair(w, p):
     return orc.haversine_km(w.lat[p[0]], w.lon[p[0]], w.lat[p[1]], w.lon[p[1]])
 
 
-@pytest.mark.parametrize("kernel", [k for k, _ in KERNELS + [BANDED]], ids=[n for _, n in KERNELS + [BANDED]])
+@pytest.mark.parametrize("kernel", [k for k, _ in KERNELS], ids=[n for _, n in KERNELS])
 def test_antipode_ranks_before_no_location(kernel):
     """A seed's exact antipode is the farthest place there is, R·π, but still nearer than a candidate without a
     location (f64::MAX).  Each configuration holds one seed, its exact antipode, a point metres from that antipode and

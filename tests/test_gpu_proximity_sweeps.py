@@ -1,7 +1,7 @@
-"""Proximity group formation past one CTA: pm_proximity_grid (the cooperative all-SM sweep), pm_proximity_sweep (the
-single-CTA fallback, PM_TUNE_PROX=2) and the experimental latitude-banded sweep (PM_TUNE_PROX=1) on thousands of
-configurations, runs of configurations nobody reaches, hand-downs of 127 / 128 / 129 / 2000, a 2200-link cascade,
-seed-parallel batches on 1, 2 and 118 CTAs, and groups selected in several chunks of 16 across CTA chunks.
+"""Proximity group formation past one CTA: pm_proximity_grid (the cooperative all-SM sweep) and pm_proximity_sweep (the
+single-CTA fallback, PM_TUNE_PROX=2) on thousands of configurations, runs of configurations nobody reaches, hand-downs
+of 127 / 128 / 129 / 2000, a 2200-link cascade, seed-parallel batches on 1, 2 and 118 CTAs, and groups selected in
+several chunks of 16 across CTA chunks.
 
 Inputs and the guards proving that each reaches its path live in tests/test_proximity_sweep_inputs.py, which runs
 them on the CPU.  Here the engine's groups, worker_group and worker_ask are compared with the checker's
@@ -24,7 +24,7 @@ from test_proximity_sweep_inputs import CASES, NONE, Case, Evidence, enabled_tab
 
 pytestmark = pytest.mark.gpu
 
-KERNELS = {"grid": "0", "single_cta": "2", "banded": "1"}
+KERNELS = {"grid": "0", "single_cta": "2"}
 INCR = abi.PM_PATH_FUSED | abi.PM_NO_ASK_STATS | abi.PM_INCREMENTAL
 
 

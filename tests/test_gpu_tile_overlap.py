@@ -1,11 +1,11 @@
-"""The double-buffered 32-bit cost tile on hardware: the argmin of tile k on the engine's side stream, beside the build
-of tile k + 1 (PM_TUNE_OVERLAP=1), against the same pass run one tile after the other (the default) and against the
+"""The materialised pass over several 32-bit cost tiles on hardware (pm_build_argmin, one launch per tile), against the
 CPU oracle.
 
-Every pm_result array, the per-worker first feasible ask and the per-ask (best, count) must be equal.  The cases aim
-at the ordering: both buffers in use and reused (1, 2 and an odd number of tiles), the shard offset, a second pass
-enqueued behind a table update with no host synchronisation in between, and the end-to-end pattern on a caller's
-stream."""
+The per-worker first feasible ask, the per-ask (best, count) and the groups must equal the oracle's, the 32-bit tile
+must have run, and the build and argmin timers must have recorded.  The cases aim at the ordering of the tiles: the
+tile buffer reused by 1, 2, an odd number and five tiles, the shard offset, a second pass enqueued behind a table
+update with no host synchronisation in between, the end-to-end pattern on a caller's stream, and the tile in plain
+rather than compressible memory."""
 import os
 
 import numpy as np
@@ -22,18 +22,10 @@ from test_gpu_narrow_tile import MAT, RESULT_FIELDS, oracle_eval, tables
 pytestmark = pytest.mark.gpu
 
 
-def make_engine(overlap, **kw):
-    os.environ["PM_TUNE_OVERLAP"] = "1" if overlap else "0"   # read at pm_create
-    try:
-        return Engine(**kw)
-    finally:
-        os.environ.pop("PM_TUNE_OVERLAP", None)
-
-
-def one_pass(t, overlap, cost_tile_bytes=0, shard=None):
+def one_pass(t, cost_tile_bytes=0, shard=None):
     """(first_ask, ask_best, ask_count, stats, result or None) of one materialised pass."""
     W, T = len(t["wa"]), len(t["asks"])
-    e = make_engine(overlap, cost_tile_bytes=cost_tile_bytes, timing=True)
+    e = Engine(cost_tile_bytes=cost_tile_bytes, timing=True)
     load_engine(e, t)
     if shard is not None:
         e.set_shard(*shard)
@@ -54,20 +46,14 @@ def assert_results_equal(a, b):
         assert np.array_equal(getattr(a, f), getattr(b, f)), f"{f} differs"
 
 
-def assert_same(t, cost_tile_bytes, shard=None):
+def narrow_pass(t, cost_tile_bytes, shard=None):
+    """one_pass, checked to have run the 32-bit tile (and, unsharded, to have timed its launches)"""
     T = len(t["asks"])
     nw = shard[1] if shard is not None else len(t["wa"])
-    o = one_pass(t, True, cost_tile_bytes, shard)
-    s = one_pass(t, False, cost_tile_bytes, shard)
-    for st in (o[3], s[3]):
-        assert st["cost_bytes_written"] == st["cost_bytes_read"] == 4 * T * nw, "the 32-bit tile did not run"
-        assert shard is not None or (st["ms_build"] > 0 and st["ms_argmin"] > 0)   # events on both streams
-    assert o[3]["n_tiles"] == s[3]["n_tiles"] and o[3]["n_build_launches"] == s[3]["n_build_launches"]
-    assert np.array_equal(o[0], s[0]), "first_ask differs"
-    assert np.array_equal(o[1], s[1]), "ask_best differs"
-    assert np.array_equal(o[2], s[2]), "ask_count differs"
-    if shard is None:
-        assert_results_equal(o[4], s[4])
+    o = one_pass(t, cost_tile_bytes, shard)
+    st = o[3]
+    assert st["cost_bytes_written"] == st["cost_bytes_read"] == 4 * T * nw, "the 32-bit tile did not run"
+    assert shard is not None or (st["ms_build"] > 0 and st["ms_argmin"] > 0)
     return o
 
 
@@ -81,7 +67,7 @@ def tile_bytes(W, rows):
                                               (1100, 1025, 256, 5), (5000, 20000, 1024, 5)])
 def test_overlap_equals_sequential(T, W, rows, n_tiles):
     t = tables(T, W, seed_shift=3 * T + W)
-    got = assert_same(t, tile_bytes(W, rows))
+    got = narrow_pass(t, tile_bytes(W, rows))
     assert got[3]["n_tiles"] == n_tiles
     ev = oracle_eval(t)
     assert np.array_equal(got[1], ev["row_best"]) and np.array_equal(got[2], ev["row_count"])
@@ -96,7 +82,7 @@ def test_overlap_equals_sequential_sharded(n_shards):
     W = len(t["wa"])
     for r in range(1, n_shards):
         lo, hi = shard_range(W, n_shards, r)
-        got = assert_same(t, tile_bytes(hi - lo, 256), shard=(lo, hi - lo))
+        got = narrow_pass(t, tile_bytes(hi - lo, 256), shard=(lo, hi - lo))
         assert got[3]["n_tiles"] == 3
         ev = oracle_eval(t, lo, hi)
         assert np.array_equal(got[2], ev["row_count"])
@@ -119,58 +105,50 @@ def changed_rows(t, seed):
 @pytest.mark.parametrize("n_tiles,T", [(2, 500), (3, 700)])
 def test_back_to_back_passes_across_a_table_update(n_tiles, T):
     """Pass 1, pm_update_workers and pass 2 are enqueued with no host synchronisation between them: pass 2's first
-    build reuses a buffer pass 1's argmins read, and its table update lands behind them."""
+    build reuses the tile pass 1's last launch wrote, and its table update lands behind pass 1."""
     W = 4099
     t = tables(T, W, seed_shift=5 + T)
     idx, a, b = changed_rows(t, T)
     t2 = dict(t, wa=t["wa"].copy(), wb=t["wb"].copy())
     t2["wa"][idx], t2["wb"][idx] = a, b
-    out = []
-    for overlap in (True, False):
-        e = make_engine(overlap, cost_tile_bytes=tile_bytes(W, 256))
-        load_engine(e, t)
-        e.match_local(MAT)
-        # the raw entry point: Engine.update_workers would synchronise the stream
-        rc = e._lib.pm_update_workers(e._h, _ptr(idx), _ptr(a), _ptr(b), None, None, len(idx))
-        assert rc == abi.PM_OK
-        e.match(MAT)
-        assert e.stats()["n_tiles"] == n_tiles
-        out.append(e.fetch())
-        e.close()
-    assert_results_equal(out[0], out[1])
+    e = Engine(cost_tile_bytes=tile_bytes(W, 256))
+    load_engine(e, t)
+    e.match_local(MAT)
+    # the raw entry point: Engine.update_workers would synchronise the stream
+    rc = e._lib.pm_update_workers(e._h, _ptr(idx), _ptr(a), _ptr(b), None, None, len(idx))
+    assert rc == abi.PM_OK
+    e.match(MAT)
+    assert e.stats()["n_tiles"] == n_tiles
+    res = e.fetch()
+    e.close()
     ev = oracle_eval(t2)
-    assert np.array_equal(out[0].ask_best, ev["row_best"]) and np.array_equal(out[0].ask_count, ev["row_count"])
-    assert groups_equal(out[0], orc.soa_form_groups(t2["wa"], t2["wb"], t2["asks"], t2["opts"], t2["bits"], t2["words"]))
+    assert np.array_equal(res.ask_best, ev["row_best"]) and np.array_equal(res.ask_count, ev["row_count"])
+    assert groups_equal(res, orc.soa_form_groups(t2["wa"], t2["wb"], t2["asks"], t2["opts"], t2["bits"], t2["words"]))
 
 
 def test_e2e_pattern_on_a_caller_stream():
     """set_asks + upsert_workers(sync=False) + match + fetch on a caller-provided stream, twice with different tables
-    on one engine: the side stream forks after the uploads and joins before the caller's stream reads the results."""
+    on one engine: every upload, launch and read-back is ordered on the caller's stream."""
     W = 4099
     t = tables(700, W, seed_shift=201)
     idx, a, b = changed_rows(t, 201)
     t2 = dict(t, asks=t["asks"][:500], wa=t["wa"].copy(), wb=t["wb"].copy())   # same model table, fewer asks
     t2["wa"][idx], t2["wb"][idx] = a, b
     passes = [t, t2]
-    got = {}
-    for overlap in (True, False):
-        stream = torch.cuda.Stream()
-        with torch.cuda.stream(stream):
-            e = make_engine(overlap, cost_tile_bytes=tile_bytes(W, 256), stream=stream.cuda_stream)
-            load_engine(e, passes[0])
-            res = []
-            for t in passes:
-                e.set_asks(t["asks"], t["opts"])
-                e.upsert_workers(t["wa"], t["wb"], sync=False)
-                e.match(MAT)
-                r = e.fetch(copy=False)
-                res.append({f: np.array(getattr(r, f), copy=True) for f in RESULT_FIELDS})
-            e.close()
-        stream.synchronize()
-        got[overlap] = res
-    for t, o, s in zip(passes, got[True], got[False]):
-        for f in RESULT_FIELDS:
-            assert np.array_equal(o[f], s[f]), f"{f} differs"
+    got = []
+    stream = torch.cuda.Stream()
+    with torch.cuda.stream(stream):
+        e = Engine(cost_tile_bytes=tile_bytes(W, 256), stream=stream.cuda_stream)
+        load_engine(e, passes[0])
+        for t in passes:
+            e.set_asks(t["asks"], t["opts"])
+            e.upsert_workers(t["wa"], t["wb"], sync=False)
+            e.match(MAT)
+            r = e.fetch(copy=False)
+            got.append({f: np.array(getattr(r, f), copy=True) for f in RESULT_FIELDS})
+        e.close()
+    stream.synchronize()
+    for t, o in zip(passes, got):
         ev = oracle_eval(t)
         assert np.array_equal(o["ask_best"], ev["row_best"]) and np.array_equal(o["ask_count"], ev["row_count"])
         og = orc.soa_form_groups(t["wa"], t["wb"], t["asks"], t["opts"], t["bits"], t["words"])
@@ -179,15 +157,14 @@ def test_e2e_pattern_on_a_caller_stream():
 
 def test_plain_tile_memory_equals_compressible():
     """The cost tile in compressible memory (the default where the device offers it) and in plain cudaMalloc memory
-    (PM_TUNE_COMPRESS=0) give the same outputs, with and without the overlap."""
+    (PM_TUNE_COMPRESS=0) give the same outputs."""
     t = tables(700, 4099, seed_shift=303)
     os.environ["PM_TUNE_COMPRESS"] = "0"
     try:
-        plain = one_pass(t, True, tile_bytes(4099, 256))
+        plain = one_pass(t, tile_bytes(4099, 256))
     finally:
         os.environ.pop("PM_TUNE_COMPRESS", None)
-    for overlap in (True, False):
-        got = one_pass(t, overlap, tile_bytes(4099, 256))
-        for a, b in zip(got[:3], plain[:3]):
-            assert np.array_equal(a, b)
-        assert_results_equal(got[4], plain[4])
+    got = one_pass(t, tile_bytes(4099, 256))
+    for a, b in zip(got[:3], plain[:3]):
+        assert np.array_equal(a, b)
+    assert_results_equal(got[4], plain[4])

@@ -142,9 +142,9 @@ def test_inputs_reach_both_clamps():
 
 
 def test_latitude_pruning_bound_holds():
-    """The lemma the latitude-pruned sweeps rest on (pm_proximity_grid.cuh pg_lat_bound, pm_proximity_band.cuh, the
-    checker's banded mode): for real latitudes, haversine ≥ R·|Δφ|·(1 − 1e-9) − 1e-9.  On the seed's own meridian
-    the two sides are equal in exact arithmetic, so half the samples are same-meridian pairs."""
+    """The lemma the latitude-pruned sweeps rest on (pm_proximity_grid.cuh pg_lat_bound, the checker's banded mode):
+    for real latitudes, haversine ≥ R·|Δφ|·(1 − 1e-9) − 1e-9.  On the seed's own meridian the two sides are equal in
+    exact arithmetic, so half the samples are same-meridian pairs."""
     rng = np.random.default_rng(21)
     n = 60_000
     lat1 = rng.uniform(-90, 90, n)

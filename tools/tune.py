@@ -70,13 +70,7 @@ if __name__ == "__main__":
     print({"hbm_peak_GBs": PEAK, "source": PEAK_SOURCE}, flush=True)
     if os.environ.get("TUNE_CEIL"):
         hbm_ceilings()
-    variants = [{}]
-    for v in os.environ.get("TUNE_ARGMIN", "1,2,3,4,5").split(","):
-        if v:
-            variants.append({"PM_TUNE_ARGMIN": v})
-    for v in os.environ.get("TUNE_BUILD", "8").split(","):   # 8: the int64 tile on the FastRow path
-        if v:
-            variants.append({"PM_TUNE_BUILD": v})
+    variants = [{}, {"PM_TUNE_BUILD": "8"}]   # 8: the int64 tile on the FastRow path
     # 0: the separate build and argmin launches, against the one-launch build + argmin of the default run above
     for v in os.environ.get("TUNE_PIPE", "0").split(","):
         if v:
