@@ -314,7 +314,9 @@ int pm_set_ask_min_reputation(pm_engine*, const uint32_t* min_reputation, uint32
  * pm_stats keeps its meanings, counted over slots.  pm_auction_certificate is over slots: n_held, n_slack_over and
  * max_slack count or range over slots, bound = sum_t d[t] * row(t) - sum_w price[w], ask_bound stays per ask (every
  * slot of an ask has the same row term), evals stays T x W.  pm_auction_assignment and pm_auction_restore return
- * PM_E_UNSUPPORTED while any demand exceeds 1 (their format is one worker per ask).  The auction stays single-GPU: there
+ * PM_E_UNSUPPORTED while any demand exceeds 1 (their format is one worker per ask); pm_auction_slot_assignment and
+ * pm_auction_restore_slots export and restore the state per slot ("Auction state restore per slot" below).  The
+ * auction stays single-GPU: there
  * is no pm_multi_ form. */
 int pm_set_ask_demand(pm_engine*, const uint32_t* demand, uint32_t n_asks);
 
@@ -547,6 +549,31 @@ typedef struct pm_auction_restore_report {
 } pm_auction_restore_report;
 int pm_auction_restore(pm_engine*, const int64_t* price, uint32_t n_workers, const uint32_t* assigned, uint32_t n_asks,
                        pm_auction_restore_report* report);
+
+/* Auction state restore per slot: the export and restore of an engine with demands ("Auction demands").  A slot is one
+ * copy of an ask row: slot s of ask t is sum_{u<t} d[u] + k, k < d[t]; there are D = sum d[t] of them (D = n_asks
+ * without demands or with every demand 1).
+ * pm_auction_slot_assignment: the stored state's assignment per slot, assigned[s] = a worker or PM_NONE, over the
+ * current slot table (after the remaps of pm_update_asks, pm_resize_asks and pm_set_ask_demand).  *n_slots is in/out:
+ * with assigned NULL the call writes D and returns PM_OK; otherwise *n_slots must equal D.  Refusals: PM_E_INVALID for
+ * a NULL n_slots, or *n_slots other than D (D is written back); PM_E_STATE where pm_auction_state returns it (before
+ * the size query: nothing is written).  Without demands the output is pm_auction_assignment's, byte for byte.
+ * pm_auction_restore_slots: THE RULE: on an engine with demands d it does what pm_auction_restore does on the twin
+ * engine (row t repeated d[t] times, its cap and floor repeated), with assigned as the twin's per-ask assignment.  So
+ * the same holds are kept, checked in the same order: bad (the pair is infeasible), shared (the worker is named by
+ * more than one slot, two slots of one ask included, every naming counts), slack (key(w) - row(t) > 1, t the slot's
+ * ask); the same counts are reported, except evals = T x W (the sweep stays per ask; the twin reports D x W, as the
+ * certificate does); no price changes.  After a success the audited state is the stored state, every slot may carry a
+ * hold, no row or ask counts as changed, pm_auction_state reports the restored prices with warm = 0 and 0 released,
+ * pm_auction_reverse_stats reports zeros; pm_fetch_result, pm_get_stats, pm_table_version and the stored evaluation of
+ * PM_INCREMENTAL are untouched; the next PM_AUCTION_WARM pass, with or without PM_AUCTION_REPAIR, equals the twin's
+ * next pass after its own restore, bit for bit.  Refusals are pm_auction_restore's, with n_slots in place of n_asks
+ * (PM_E_INVALID for n_slots other than D, which includes an array exported before a demand change), and none changes
+ * anything: not the stored state, the demands, the version or any report.  Without demands the call is
+ * pm_auction_restore in every respect. */
+int pm_auction_slot_assignment(pm_engine*, uint32_t* assigned, uint32_t* n_slots);
+int pm_auction_restore_slots(pm_engine*, const int64_t* price, uint32_t n_workers, const uint32_t* assigned, uint32_t n_slots,
+                             pm_auction_restore_report* report);
 
 typedef struct pm_stats {
   uint64_t evals;            /* predicate evaluations executed on the device        */

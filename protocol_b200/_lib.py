@@ -69,6 +69,8 @@ def load() -> C.CDLL:
         "pm_auction_certificate": (i32, [vp, P(abi.PmAuctionCert), vp]),
         "pm_auction_assignment": (i32, [vp, vp]),
         "pm_auction_restore": (i32, [vp, vp, u32, vp, u32, P(abi.PmAuctionRestoreReport)]),
+        "pm_auction_slot_assignment": (i32, [vp, vp, P(u32)]),
+        "pm_auction_restore_slots": (i32, [vp, vp, u32, vp, u32, P(abi.PmAuctionRestoreReport)]),
         "pm_match": (i32, [vp, u32]),
         "pm_fetch_result": (i32, [vp, P(abi.PmResult)]),
         "pm_get_stats": (i32, [vp, P(abi.PmStats)]),

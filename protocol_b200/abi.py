@@ -137,6 +137,7 @@ EXPORTS = [
     "pm_set_ask_price_caps", "pm_set_auction_params", "pm_set_worker_reputation", "pm_set_ask_min_reputation",
     "pm_set_ask_demand",
     "pm_auction_state", "pm_auction_reverse_stats", "pm_auction_certificate", "pm_auction_assignment", "pm_auction_restore",
+    "pm_auction_slot_assignment", "pm_auction_restore_slots",
     "pm_match", "pm_fetch_result", "pm_get_stats", "pm_build_cost_tile",
     "pm_match_local", "pm_match_finish", "pm_device_buffer", "pm_stream_sync", "pm_set_shard",
     "pm_resize_workers", "pm_update_workers", "pm_table_version", "pm_create_sibling",

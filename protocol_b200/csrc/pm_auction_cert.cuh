@@ -39,7 +39,8 @@ struct CertParams {
   const uint32_t* __restrict__ floor;        // [T] reputation floors, or null: no clause
   const uint32_t* __restrict__ assigned;     // [T] stored assignment (PM_NONE: unheld)
   unsigned long long* __restrict__ row_min;  // [T] least feasible key, ~0 before the sweep
-  uint32_t* __restrict__ held_ok;            // [T] the held pair is feasible (written for held asks only)
+  uint32_t* __restrict__ held_ok;            // [T] the held pair is feasible (written for held asks only); per slot, [D],
+                                             // with demands (pm_auction_cert_slots)
   uint32_t* __restrict__ own;                // [W] asks holding the worker, zero before pm_auction_cert_asks
   long long* __restrict__ ask_bound;         // [T] the row terms
   unsigned long long* __restrict__ acc;      // [kCertAccWords]
@@ -175,7 +176,8 @@ __global__ void pm_auction_cert_asks(CertParams c, const uint4* __restrict__ wb)
 // With demands (pm_set_ask_demand) the sweep stays per ask, T x W (every slot of an ask has the ask's row term), run
 // with no holds, and this pass takes pm_auction_cert_asks' place over the slots: slot s of ask slot_ask[s] adds the
 // ask's row term, so the row sum is sum_t d[t] * row(t), and its own hold's cost, slack and ownership count.  A held
-// pair's feasibility is checked here with the predicate of eval_row_global (ask_meets), cap and floor as in the sweep.
+// pair's feasibility is checked here with the predicate of eval_row_global (ask_meets), cap and floor as in the sweep,
+// and stored per slot in held_ok (D entries; written for held slots only), which pm_auction_restore_asks reads.
 // c.assigned is the slots' assignment; the ask's first slot writes ask_bound.
 __global__ void pm_auction_cert_slots(CertParams c, EvalParams p, const uint32_t* __restrict__ slot_ask, uint32_t n_slots) {
   for (uint32_t base = blockIdx.x * blockDim.x; base < n_slots; base += gridDim.x * blockDim.x) {   // warp-uniform trip count
@@ -196,6 +198,7 @@ __global__ void pm_auction_cert_slots(CertParams c, EvalParams p, const uint32_t
         const WorkerReg wr = make_worker(__ldg(p.wa + a), __ldg(p.wb + a));
         const uint32_t rep = c.rep ? __ldg(c.rep + a) : 0u, fl = c.floor ? __ldg(c.floor + t) : 0u;
         bad = !(wr.price <= cap && rep >= fl && ask_meets(p.asks[t], p.opts, wr, p.bits, p.words));
+        c.held_ok[s] = bad ? 0u : 1u;
         cost = (unsigned long long)wr.price * c.scale;
         slack = (long long)(cost + (unsigned long long)__ldg(c.price + a)) - (long long)bound;
         atomicAdd(c.own + a, 1u);
@@ -242,36 +245,37 @@ __global__ void pm_auction_cert_workers(CertParams c, const uint4* __restrict__ 
   }
 }
 
-// ------------------------------------------------------------------ restore (pm_auction_restore)
-// The caller's state is audited by the certificate's own sweep and per-ask pass (CertParams pointed at the staged
-// prices and assignment): row terms, held-pair feasibility and ownership counts.  Then one decision per ask and one
-// pass over the workers, both into staging buffers; the engine copies them over the stored state once nothing can
-// refuse any more.  Prices are never changed: a dropped hold's worker is unowned at its given price.
+// ------------------------------------------------------------------ restore (pm_auction_restore, pm_auction_restore_slots)
+// The caller's state is audited by the certificate's own sweep and per-ask (or per-slot) pass (CertParams pointed at
+// the staged prices and assignment): row terms, held-pair feasibility and ownership counts.  Then one decision per
+// bidder and one pass over the workers, both into staging buffers; the engine copies them over the stored state once
+// nothing can refuse any more.  Prices are never changed: a dropped hold's worker is unowned at its given price.
 enum RestoreAcc : int { kRstHeld, kRstBad, kRstShared, kRstSlack, kRstAccWords };
-constexpr uint32_t kRstHolder = 0x80000000u;   // own[w] after the audit: kRstHolder | t for the kept hold of ask t
+constexpr uint32_t kRstHolder = 0x80000000u;   // own[w] after the audit: kRstHolder | b for the kept hold of bidder b
 
-// Per ask, after pm_auction_cert_asks: a hold is dropped when it is infeasible, else when its worker is named by more
-// than one ask, else when its slack key(w_t) - row(t) exceeds 1; a kept hold marks its worker's count (1: nobody else
-// writes it; counts stay below 2^30, so the mark is told apart).
-__global__ void pm_auction_restore_asks(CertParams c, const uint4* __restrict__ wb, uint32_t* __restrict__ kept,
-                                        unsigned long long* __restrict__ acc) {
-  const uint32_t n = c.n_asks;
+// Per bidder b < n, after pm_auction_cert_asks (the asks: slot_ask null, n = T) or pm_auction_cert_slots (the slots of
+// ask demands: slot_ask the slot -> ask map, n = D): a hold is dropped when it is infeasible, else when its worker is
+// named by more than one bidder, else when its slack key(w_b) - row(ask of b) exceeds 1; a kept hold marks its worker's
+// count (1: nobody else writes it; counts and bidder indices stay below 2^30, so the mark is told apart).
+__global__ void pm_auction_restore_asks(CertParams c, const uint4* __restrict__ wb, const uint32_t* __restrict__ slot_ask,
+                                        uint32_t n, uint32_t* __restrict__ kept, unsigned long long* __restrict__ acc) {
   for (uint32_t base = blockIdx.x * blockDim.x; base < n; base += gridDim.x * blockDim.x) {   // warp-uniform trip count
-    const uint32_t t = base + threadIdx.x;
+    const uint32_t b = base + threadIdx.x;
     bool keep = false, bad = false, shared = false, over = false;
-    if (t < n) {
-      const uint32_t a = __ldg(c.assigned + t);
+    if (b < n) {
+      const uint32_t a = __ldg(c.assigned + b);
       if (a < c.n_workers) {
-        bad = c.held_ok[t] == 0u;
+        bad = c.held_ok[b] == 0u;
         shared = !bad && c.own[a] > 1u;
         if (!bad && !shared) {
+          const uint32_t t = slot_ask ? __ldg(slot_ask + b) : b;
           const unsigned long long key = (unsigned long long)__ldg(&wb[a].w) * c.scale + (unsigned long long)__ldg(c.price + a);
           over = (long long)key - c.ask_bound[t] > 1;
           keep = !over;
         }
-        if (keep) c.own[a] = kRstHolder | t;
+        if (keep) c.own[a] = kRstHolder | b;
       }
-      kept[t] = keep ? a : kNone;
+      kept[b] = keep ? a : kNone;
     }
     cert_count(acc, kRstHeld, keep);
     cert_count(acc, kRstBad, bad);
@@ -280,7 +284,8 @@ __global__ void pm_auction_restore_asks(CertParams c, const uint4* __restrict__ 
   }
 }
 
-// Per worker, after pm_auction_restore_asks: the owner array of the kept holds
+// Per worker, after pm_auction_restore_asks: the owner array of the kept holds (ask indices, or slot indices with
+// demands: what the auction's kernels read)
 __global__ void pm_auction_restore_workers(const uint32_t* __restrict__ own, uint32_t n_workers, uint32_t* __restrict__ owner) {
   for (uint32_t w = blockIdx.x * blockDim.x + threadIdx.x; w < n_workers; w += gridDim.x * blockDim.x) {
     const uint32_t o = own[w];

@@ -492,7 +492,8 @@ struct pm_engine {
   DevBuf<long long> cert_bound;
   PinBuf<uint64_t> h_cert_acc;
   PinBuf<long long> h_cert_bound;
-  // pm_auction_restore's staging: the caller's prices and assignment, the kept assignment, the rebuilt owners, the counts
+  // pm_auction_restore's staging: the caller's prices and assignment, the kept assignment (per slot with demands: D
+  // entries), the rebuilt owners, the counts
   DevBuf<long long> rst_price;
   DevBuf<uint32_t> rst_assigned, rst_kept, rst_owner;
   DevBuf<uint64_t> rst_acc;
@@ -2778,7 +2779,7 @@ struct KeepStats {
   ~KeepStats() { e->stats = saved; }
 };
 
-// The certificate's kernels (pm_auction_cert.cuh) over the prices and assignment given (device, [W] and [T]), into the
+// The certificate's kernels (pm_auction_cert.cuh) over the prices and assignment given (device, [W] and [D]), into the
 // certificate's private scratch: one sweep over every pair, then one pass over the asks and one over the workers.
 // Enqueued only; *c gets the parameters the launches took.
 static int cert_launch(pm_engine* e, const long long* price, const uint32_t* assigned, pm::CertParams* out) {
@@ -2788,7 +2789,9 @@ static int cert_launch(pm_engine* e, const long long* price, const uint32_t* ass
     PM_CUDA(cudaMemsetAsync(e->bits.p, 0xFF, 4, e->stream));
     e->words = 1;
   }
-  PM_CUDA(e->cert_min.ensure(std::max<uint32_t>(T, 1))); PM_CUDA(e->cert_ok.ensure(std::max<uint32_t>(T, 1)));
+  const bool dem = !e->demand.empty();
+  const uint32_t D = e->n_slots();
+  PM_CUDA(e->cert_min.ensure(std::max<uint32_t>(T, 1))); PM_CUDA(e->cert_ok.ensure(std::max<uint32_t>(std::max(T, D), 1)));
   PM_CUDA(e->cert_bound.ensure(std::max<uint32_t>(T, 1))); PM_CUDA(e->cert_own.ensure(std::max<uint32_t>(W, 1)));
   PM_CUDA(e->cert_acc.ensure(pm::kCertAccWords)); PM_CUDA(e->h_cert_acc.ensure(pm::kCertAccWords));
   PM_CUDA(cudaMemsetAsync(e->cert_min.p, 0xFF, (size_t)std::max<uint32_t>(T, 1) * 8, e->stream));
@@ -2809,9 +2812,7 @@ static int cert_launch(pm_engine* e, const long long* price, const uint32_t* ass
   c.n_workers = W;
   c.n_asks = T;
   // With demands the assignment is per slot: the sweep runs per ask with no holds, and pm_auction_cert_slots checks
-  // them instead of pm_auction_cert_asks.
-  const bool dem = !e->demand.empty();
-  const uint32_t D = e->n_slots();
+  // them instead of pm_auction_cert_asks (held_ok then per slot).  The slot table it builds stays in slot_ask.
   pm::CertParams cs = c;
   if (dem) {
     PM_CUDA(e->cert_none.ensure(std::max<uint32_t>(T, 1)));
@@ -2923,33 +2924,62 @@ int pm_auction_assignment(pm_engine* e, uint32_t* assigned) try {
   return PM_OK;
 } catch (...) { return pm_guard_rc(); }
 
-// A caller's auction state, audited on the device and made the stored state (prime_match.h "Auction state restore").
-// Every host check first, then the caller's arrays go to staging buffers and the certificate's kernels run over them;
-// the audit (pm_auction_restore_asks, pm_auction_restore_workers) writes staging buffers too.  One synchronisation,
-// the domain check on the sweep's largest ask price, and only then the stored state is overwritten, by device copies.
-int pm_auction_restore(pm_engine* e, const int64_t* price, uint32_t n_workers, const uint32_t* assigned, uint32_t n_asks,
-                       pm_auction_restore_report* report) try {
+// The stored state's assignment per slot over the current slot table (prime_match.h "Auction state restore per
+// slot"): the stored array itself, which every remap of the asks and demands keeps per slot.  *n_slots in/out; a size
+// query with assigned NULL.
+int pm_auction_slot_assignment(pm_engine* e, uint32_t* assigned, uint32_t* n_slots) try {
   if (!e) return PM_E_INVALID;
   std::lock_guard<std::mutex> lk(e->mu);
-  if ((n_workers && !price) || (n_asks && !assigned)) return e->fail(PM_E_INVALID, "pm_auction_restore: null");
-  if (!e->have_workers || !e->have_asks) return e->fail(PM_E_STATE, "pm_auction_restore: worker and ask tables must be set first");
-  if (!e->have_caps) return e->fail(PM_E_STATE, "pm_auction_restore: no price caps (pm_set_ask_price_caps)");
+  if (!n_slots) return e->fail(PM_E_INVALID, "pm_auction_slot_assignment: null n_slots");
+  if (!e->auc_state) return e->fail(PM_E_STATE, "pm_auction_slot_assignment: no auction pass since the engine's tables were last replaced");
+  const uint32_t D = e->n_slots();
+  if (!assigned) {
+    *n_slots = D;
+    return PM_OK;
+  }
+  if (*n_slots != D) {
+    *n_slots = D;
+    return e->fail(PM_E_INVALID, "pm_auction_slot_assignment: n_slots is not the number of slots (written back)");
+  }
+  PM_CUDA(cudaSetDevice(e->device));
+  if (D) {
+    PM_CUDA(cudaMemcpyAsync(assigned, e->auc_assigned.p, (size_t)D * 4, cudaMemcpyDeviceToHost, e->stream));
+    PM_CUDA(cudaStreamSynchronize(e->stream));
+  }
+  return PM_OK;
+} catch (...) { return pm_guard_rc(); }
+
+// A caller's auction state, audited on the device and made the stored state (prime_match.h "Auction state restore"),
+// for pm_auction_restore (per_slot false: one entry per ask, refused under demands) and pm_auction_restore_slots (one
+// entry per slot; without demands the slots are the asks).  Called with the engine's lock held.  Every host check
+// first, then the caller's arrays go to staging buffers and the certificate's kernels run over them (with demands
+// cert_launch builds the slot table and checks the holds per slot); the audit (pm_auction_restore_asks over the asks or
+// the slots, pm_auction_restore_workers) writes staging buffers too.  One synchronisation, the domain check on the
+// sweep's largest ask price, and only then the stored state is overwritten, by device copies.
+static int auction_restore(pm_engine* e, const char* fn, bool per_slot, const int64_t* price, uint32_t n_workers,
+                           const uint32_t* assigned, uint32_t n, pm_auction_restore_report* report) {
+  auto refuse = [&](pm_status st, const char* why) { return e->fail(st, std::string(fn) + ": " + why); };
+  if ((n_workers && !price) || (n && !assigned)) return refuse(PM_E_INVALID, "null");
+  if (!e->have_workers || !e->have_asks) return refuse(PM_E_STATE, "worker and ask tables must be set first");
+  if (!e->have_caps) return refuse(PM_E_STATE, "no price caps (pm_set_ask_price_caps)");
   if (e->max_pattern_row > e->n_patterns || (e->max_pattern_row && !e->have_bits))
-    return e->fail(PM_E_STATE, "pm_auction_restore: an ask references a model pattern missing from the model table");
-  if (e->cfg.shard_count || e->comm) return e->fail(PM_E_UNSUPPORTED, "pm_auction_restore: auction mode is single-GPU");
-  if (e->n_off) return e->fail(PM_E_UNSUPPORTED, "pm_auction_restore: disabled asks");
-  if (!e->demand.empty()) return e->fail(PM_E_UNSUPPORTED, "pm_auction_restore: an ask demand above 1 (the format is one worker per ask)");
-  const uint32_t W = e->n_workers, T = e->n_asks;
-  if (n_workers != W || n_asks != T) return e->fail(PM_E_INVALID, "pm_auction_restore: one price per worker and one entry per ask");
-  for (uint32_t t = 0; t < T; ++t)
-    if (assigned[t] != PM_NONE && assigned[t] >= W) return e->fail(PM_E_INVALID, "pm_auction_restore: assigned worker out of range");
+    return refuse(PM_E_STATE, "an ask references a model pattern missing from the model table");
+  if (e->cfg.shard_count || e->comm) return refuse(PM_E_UNSUPPORTED, "auction mode is single-GPU");
+  if (e->n_off) return refuse(PM_E_UNSUPPORTED, "disabled asks");
+  if (!per_slot && !e->demand.empty()) return refuse(PM_E_UNSUPPORTED, "an ask demand above 1 (the format is one worker per ask)");
+  const bool dem = !e->demand.empty();
+  const uint32_t W = e->n_workers, T = e->n_asks, D = e->n_slots();
+  if (n_workers != W || n != D)
+    return refuse(PM_E_INVALID, per_slot ? "one price per worker and one entry per slot" : "one price per worker and one entry per ask");
+  for (uint32_t s = 0; s < D; ++s)
+    if (assigned[s] != PM_NONE && assigned[s] >= W) return refuse(PM_E_INVALID, "assigned worker out of range");
   // every price the warm pass and the repair can start from: (K + 1) * S + max(E, 1), in 128 bits
   uint32_t K = 0;
   for (uint32_t t = 0; t < T; ++t) K = std::max(K, e->cap_host[t]);
   const unsigned __int128 p_max = ((unsigned __int128)K + 1u) * e->auc_scale + std::max<uint64_t>(e->auc_eps_start, 1);
   for (uint32_t w = 0; w < W; ++w)
     if (price[w] < 0 || (unsigned __int128)price[w] > p_max)
-      return e->fail(PM_E_INVALID, "pm_auction_restore: price outside [0, (max cap + 1) * cost_scale + eps_start]");
+      return refuse(PM_E_INVALID, "price outside [0, (max cap + 1) * cost_scale + eps_start]");
   KeepStats keep_stats{e, e->stats};   // before the rows go to the auction's form: that launch is no pass's either
   {
     const int rc = use_ask_form(e, true);
@@ -2958,21 +2988,21 @@ int pm_auction_restore(pm_engine* e, const int64_t* price, uint32_t n_workers, c
   PM_CUDA(cudaSetDevice(e->device));
   // the stored buffers at their pass sizes, their contents kept (a refusal below leaves the stored state as it was)
   PM_CUDA(e->auc_price.grow_keep((size_t)W + 2, e->auc_price.n, e->stream)); PM_CUDA(e->auc_owner.grow_keep(W, e->auc_owner.n, e->stream));
-  PM_CUDA(e->auc_assigned.grow_keep(T, e->auc_assigned.n, e->stream));
+  PM_CUDA(e->auc_assigned.grow_keep(D, e->auc_assigned.n, e->stream));
   PM_CUDA(e->rst_price.ensure(std::max<uint32_t>(W, 1))); PM_CUDA(e->rst_owner.ensure(std::max<uint32_t>(W, 1)));
-  PM_CUDA(e->rst_assigned.ensure(std::max<uint32_t>(T, 1))); PM_CUDA(e->rst_kept.ensure(std::max<uint32_t>(T, 1)));
+  PM_CUDA(e->rst_assigned.ensure(std::max<uint32_t>(D, 1))); PM_CUDA(e->rst_kept.ensure(std::max<uint32_t>(D, 1)));
   PM_CUDA(e->rst_acc.ensure(pm::kRstAccWords)); PM_CUDA(e->h_rst_acc.ensure(pm::kRstAccWords));
   if (W) PM_CUDA(cudaMemcpyAsync(e->rst_price.p, price, (size_t)W * 8, cudaMemcpyHostToDevice, e->stream));
-  if (T) PM_CUDA(cudaMemcpyAsync(e->rst_assigned.p, assigned, (size_t)T * 4, cudaMemcpyHostToDevice, e->stream));
+  if (D) PM_CUDA(cudaMemcpyAsync(e->rst_assigned.p, assigned, (size_t)D * 4, cudaMemcpyHostToDevice, e->stream));
   PM_CUDA(cudaMemsetAsync(e->rst_acc.p, 0, pm::kRstAccWords * 8, e->stream));
   pm::CertParams c;
   {
     const int rc = cert_launch(e, e->rst_price.p, e->rst_assigned.p, &c);
     if (rc != PM_OK) return rc;
   }
-  if (T) {
-    pm::pm_auction_restore_asks<<<std::min(blocks_for(T, 256), 4u * e->sms), 256, 0, e->stream>>>(
-        c, e->wb.p, e->rst_kept.p, reinterpret_cast<unsigned long long*>(e->rst_acc.p));
+  if (D) {
+    pm::pm_auction_restore_asks<<<std::min(blocks_for(D, 256), 4u * e->sms), 256, 0, e->stream>>>(
+        c, e->wb.p, dem ? e->slot_ask.p : nullptr, D, e->rst_kept.p, reinterpret_cast<unsigned long long*>(e->rst_acc.p));
     PM_LAUNCH_CHECK("pm_auction_restore_asks");
   }
   if (W) {
@@ -2983,15 +3013,16 @@ int pm_auction_restore(pm_engine* e, const int64_t* price, uint32_t n_workers, c
   PM_CUDA(cudaMemcpyAsync(e->h_rst_acc.p, e->rst_acc.p, pm::kRstAccWords * 8, cudaMemcpyDeviceToHost, e->stream));
   PM_CUDA(cudaStreamSynchronize(e->stream));
   if (!auction_in_domain((uint32_t)e->h_cert_acc.p[pm::kCertMaxAskPrice], K, e->auc_scale, e->auc_eps_start))
-    return e->fail(PM_E_INVALID, "pm_auction_restore: (max ask_price + max cap + 2) * cost_scale + eps_start must stay below 2^61");
-  // commit: from here a failure leaves a half-copied state, which is dropped
+    return refuse(PM_E_INVALID, "(max ask_price + max cap + 2) * cost_scale + eps_start must stay below 2^61");
+  // commit: from here a failure leaves a half-copied state, which is dropped.  auc_discard also clears the demand
+  // bookkeeping (auc_dem_kept): every slot of the restored state may carry a hold.
   e->auc_discard();
   if (W) {
     PM_CUDA(cudaMemcpyAsync(e->auc_price.p, e->rst_price.p, (size_t)W * 8, cudaMemcpyDeviceToDevice, e->stream));
     PM_CUDA(cudaMemcpyAsync(e->auc_owner.p, e->rst_owner.p, (size_t)W * 4, cudaMemcpyDeviceToDevice, e->stream));
   }
   PM_CUDA(cudaMemsetAsync(e->auc_price.p + W, 0, 2 * 8, e->stream));
-  if (T) PM_CUDA(cudaMemcpyAsync(e->auc_assigned.p, e->rst_kept.p, (size_t)T * 4, cudaMemcpyDeviceToDevice, e->stream));
+  if (D) PM_CUDA(cudaMemcpyAsync(e->auc_assigned.p, e->rst_kept.p, (size_t)D * 4, cudaMemcpyDeviceToDevice, e->stream));
   PM_CUDA(cudaStreamSynchronize(e->stream));
   // the bookkeeping of a pass that just ran on the current tables: nothing changed since, nothing to report
   e->auc_state = true;
@@ -3011,9 +3042,25 @@ int pm_auction_restore(pm_engine* e, const int64_t* price, uint32_t n_workers, c
     report->n_dropped_bad = (uint32_t)h[pm::kRstBad];
     report->n_dropped_shared = (uint32_t)h[pm::kRstShared];
     report->n_dropped_slack = (uint32_t)h[pm::kRstSlack];
-    report->evals = (uint64_t)T * W;
+    report->evals = (uint64_t)T * W;   // the sweep is per ask with demands too
   }
   return PM_OK;
+}
+
+int pm_auction_restore(pm_engine* e, const int64_t* price, uint32_t n_workers, const uint32_t* assigned, uint32_t n_asks,
+                       pm_auction_restore_report* report) try {
+  if (!e) return PM_E_INVALID;
+  std::lock_guard<std::mutex> lk(e->mu);
+  return auction_restore(e, "pm_auction_restore", false, price, n_workers, assigned, n_asks, report);
+} catch (...) { return pm_guard_rc(); }
+
+// With demands d: what pm_auction_restore does on the twin engine (row t repeated d[t] times), `assigned` the twin's
+// per-ask assignment; without demands exactly pm_auction_restore.
+int pm_auction_restore_slots(pm_engine* e, const int64_t* price, uint32_t n_workers, const uint32_t* assigned, uint32_t n_slots,
+                             pm_auction_restore_report* report) try {
+  if (!e) return PM_E_INVALID;
+  std::lock_guard<std::mutex> lk(e->mu);
+  return auction_restore(e, "pm_auction_restore_slots", true, price, n_workers, assigned, n_slots, report);
 } catch (...) { return pm_guard_rc(); }
 
 int pm_set_ask_price_caps(pm_engine* e, const uint32_t* price_cap, uint32_t n_asks) try {

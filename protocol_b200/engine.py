@@ -294,6 +294,29 @@ class Engine:
         self._auction_workers = len(price)
         return {n: int(getattr(rep, n)) for n, _ in rep._fields_}
 
+    def auction_slot_assignment(self) -> np.ndarray:
+        """The stored auction state's assignment per slot (pm_auction_slot_assignment): uint32[D], D = sum of the ask
+        demands (n_asks without demands), slot s of ask t at sum(demand[:t]) + k; a worker or PM_NONE.  With
+        auction_state()'s prices this is what auction_restore_slots() takes."""
+        n = C.c_uint32(0)
+        self._check(self._lib.pm_auction_slot_assignment(self._h, None, C.byref(n)))
+        out = np.zeros(n.value, dtype=np.uint32)
+        if n.value:
+            self._check(self._lib.pm_auction_slot_assignment(self._h, _ptr(out), C.byref(n)))
+        return out
+
+    def auction_restore_slots(self, price, assigned) -> dict:
+        """auction_restore() per slot (pm_auction_restore_slots): with demands, what auction_restore does on the engine
+        whose ask table repeats row t demand[t] times, with `assigned` (uint32[D]) as that table's assignment; report
+        evals = n_asks x n_workers.  Returns the report."""
+        price = np.ascontiguousarray(price, dtype=np.int64)
+        assigned = np.ascontiguousarray(assigned, dtype=np.uint32)
+        rep = abi.PmAuctionRestoreReport()
+        self._check(self._lib.pm_auction_restore_slots(self._h, _ptr(price), len(price), _ptr(assigned), len(assigned),
+                                                       C.byref(rep)))
+        self._auction_workers = len(price)
+        return {n: int(getattr(rep, n)) for n, _ in rep._fields_}
+
     # ---- the pass ---------------------------------------------------------
     def match(self, mode: int = abi.PM_MODE_FIRST_FIT):
         """pm_match.  Auction passes (PM_MODE_AUCTION) take PM_AUCTION_WARM: start from the last auction pass's state,

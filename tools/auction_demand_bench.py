@@ -2,6 +2,8 @@
 tools/auction_warm_bench.py builds) with demands drawn from {1, 2, 4, 8} (D ~ 94 000 slots) x 1M workers.
 
 * a cold pass with demands, and the same pass on the twin engine whose ask table repeats each row demand times;
+* the cold state exported per slot (pm_auction_slot_assignment) and restored into a fresh engine with the same tables
+  and demands (pm_auction_restore_slots): the restore and that engine's first warm pass, against the cold pass;
 * from the demand engine's stored state, 1 / 100 / 1 000 demand changes (random asks, each demand moved by -2..+2),
   each followed by a warm pass, then another change of the same size followed by a repair pass (a chain: each step
   starts from the state the previous one left);
@@ -72,6 +74,20 @@ def main():
     twin = load(np.repeat(asks, d), a.opts, wa, wb, bits, npat, nmod, words, np.repeat(cap, d))
     _, out["twin_cold_ms"] = timed(lambda: twin.match(AUC))
     out["twin_same_prices"] = bool(np.array_equal(eng.auction_state()[0], twin.auction_state()[0]))
+
+    # a restart: the cold state exported per slot and restored into a fresh engine with the same tables and demands
+    price, slots = eng.auction_state()[0], eng.auction_slot_assignment()
+    moved = load(asks, a.opts, wa, wb, bits, npat, nmod, words, cap)
+    moved.set_ask_demand(d)
+    rep, ms = timed(lambda: moved.auction_restore_slots(price, slots))
+    out["restore_ms"] = round(ms, 1)
+    out["restore_held"] = rep["n_held"]
+    out["restore_dropped"] = rep["n_dropped_bad"] + rep["n_dropped_shared"] + rep["n_dropped_slack"]
+    _, ms = timed(lambda: moved.match(WARM))
+    out["restore_first_warm_ms"] = round(ms, 1)
+    out["restore_first_warm_started_warm"] = moved.auction_state(prices=False)[1]
+    out["restore_first_warm_rounds"] = moved.stats()["n_rounds"]
+    moved.close()
 
     d_twin = d   # the twin's table stays at the first demands
     for n in (1, 100, 1000):
