@@ -209,8 +209,9 @@ int pm_set_asks(pm_engine*, const pm_ask* asks, uint32_t n_asks,
  * passes".                                                                                                          */
 int pm_set_ask_enabled(pm_engine*, const uint32_t* idx, const uint8_t* enabled, uint32_t n);
 /* Ask-table deltas: a resident ask table changed in place (a new task with a price cap is an appended row, a finished
- * one a removed row).  After any sequence of pm_set_asks, pm_update_asks, pm_resize_asks and pm_set_ask_enabled calls
- * the engine is the engine pm_set_asks would give for the current rows with the same enabled mask: every array
+ * one a removed row).  After any sequence of pm_set_asks, pm_update_asks, pm_resize_asks, pm_remove_asks, pm_insert_asks
+ * and pm_set_ask_enabled calls the engine is the engine pm_set_asks would give for the current rows with the same
+ * enabled mask, caps, floors and demands: every array
  * pm_fetch_result returns, pm_build_cost_tile and a cold auction pass are bit-identical to a fresh engine's, with or
  * without PM_INCREMENTAL, on every path and in every mode.  Ask index stays priority.
  *   pm_update_asks   replace rows idx[i] (each < n_asks) by asks[i]; asks[i].opt_off / n_opts index `opts`, as in
@@ -218,14 +219,23 @@ int pm_set_ask_enabled(pm_engine*, const uint32_t* idx, const uint8_t* enabled, 
  *                    repeated indices the last entry decides.
  *   pm_resize_asks   shrink: drop asks [n_asks, old); grow: append `n_asks - old` rows from `added` (options in `opts`)
  *                    at the lowest priorities, enabled, with cap 0 and floor 0 until pm_set_ask_price_caps /
- *                    pm_set_ask_min_reputation set them (both still take exactly n_asks entries).  Inserting in the
- *                    middle is pm_set_asks.
- * Refusals, none of which changes anything (no table, no stored evaluation, no auction state, no pm_table_version):
- * PM_E_INVALID for a null pointer with a count > 0, an index >= n_asks, max_group_size < min_group_size, an option
- * range outside `opts`, growth without `added`, n_asks >= 2^30 or more than 2^31 converted option rows; PM_E_STATE
- * without an ask table.  Every row is checked on the host before anything on the device is touched.  A row that
+ *                    pm_set_ask_min_reputation set them (both still take exactly n_asks entries).
+ *   pm_remove_asks   remove rows idx[0..n) (any order; a repeated index removes its row once); the rows after them move
+ *                    up, order kept.  Removing the tail is pm_resize_asks shrinking, bit for bit.
+ *   pm_insert_asks   insert rows asks[0..n) (options in `opts`, as pm_set_asks) before the current rows before[i];
+ *                    before[] non-decreasing, before[i] <= n_asks (n_asks = append); rows with equal before[] keep their
+ *                    order.  Inserting every row at n_asks is pm_resize_asks growing, bit for bit.
+ * A removed row takes its enabled flag, price cap, reputation floor and demand with it.  An inserted (or appended) row is
+ * enabled, with cap 0, floor 0 and demand 1 until pm_set_ask_price_caps / pm_set_ask_min_reputation /
+ * pm_set_ask_demand set them (each still takes exactly n_asks entries).  A kept row keeps its flag, cap, floor and
+ * demand under its new index.
+ * Refusals, none of which changes anything (no table, no stored evaluation, no auction state, no demands, no
+ * pm_table_version): PM_E_INVALID for a null pointer with a count > 0, an index >= n_asks, a before[] that decreases or
+ * exceeds n_asks, max_group_size < min_group_size, an option range outside `opts`, growth without `added`, n_asks >= 2^30,
+ * more than 2^31 converted option rows, or added rows that take the demands' total D to 2^30; PM_E_STATE without an
+ * ask table.  Every row is checked on the host before anything on the device is touched.  A row that
  * references a pattern beyond the model table is accepted; the next pass returns PM_E_STATE, as after pm_set_asks.
- * Unlike pm_set_asks, both keep the stored evaluation of PM_INCREMENTAL and the stored auction state: see "Incremental
+ * Unlike pm_set_asks, all four keep the stored evaluation of PM_INCREMENTAL and the stored auction state: see "Incremental
  * passes", "Auction warm start", "Auction warm repair" and "Auction certificate".  Each call converts the whole table
  * again on the device (O(T + the option rows)).  Only the option ranges the new rows reference are copied from `opts`
  * (a caller may pass its whole option table); the option rows replaced or removed rows leave behind are compacted
@@ -233,6 +243,9 @@ int pm_set_ask_enabled(pm_engine*, const uint32_t* idx, const uint8_t* enabled, 
 int pm_update_asks(pm_engine*, const uint32_t* idx, const pm_ask* asks, uint32_t n,
                    const pm_gpu_opt* opts, uint32_t n_opts);
 int pm_resize_asks(pm_engine*, uint32_t n_asks, const pm_ask* added, const pm_gpu_opt* opts, uint32_t n_opts);
+int pm_remove_asks(pm_engine*, const uint32_t* idx, uint32_t n);
+int pm_insert_asks(pm_engine*, const uint32_t* before, const pm_ask* asks, uint32_t n, const pm_gpu_opt* opts,
+                   uint32_t n_opts);
 int pm_set_model_table(pm_engine*, const uint32_t* bits, uint32_t n_patterns,
                        uint32_t n_models, uint32_t words_per_pattern);
 /* replaces NodeStore::get_nodes per pass (store/domains/node_store.rs:163-209);
@@ -299,11 +312,12 @@ int pm_set_ask_min_reputation(pm_engine*, const uint32_t* min_reputation, uint32
  * a total cost within D * eps of the optimum, exact with cost_scale = D + 1.
  * pm_set_ask_demand takes exactly n_asks entries, as pm_set_ask_price_caps does.  Without the call, or with every demand
  * 1, behaviour is today's byte for byte (the same kernels, no extra launch).  After pm_set_asks every demand is 1;
- * pm_update_asks keeps a replaced row's demand (as it keeps its cap); pm_resize_asks appends rows with demand 1 and a
- * shrink drops the removed rows' demands.
+ * pm_update_asks keeps a replaced row's demand (as it keeps its cap); pm_resize_asks and pm_insert_asks add rows with
+ * demand 1; a shrink and pm_remove_asks drop the removed rows' demands; a kept row's demand moves with it.
  * Refusals change nothing (not the demands, not the stored auction state, not pm_table_version): PM_E_INVALID for a
  * NULL pointer with n_asks > 0, n_asks other than the table's, a demand of 0, or D >= 2^30 (the ask-count limit; a
- * pm_resize_asks growth that would take D there is refused the same way); PM_E_STATE without an ask table.
+ * pm_resize_asks growth or pm_insert_asks that would take D there is refused the same way); PM_E_STATE without an ask
+ * table.
  * A demand change under a stored auction state: each ask's first min(old, new) slots keep their holds; a removed slot's
  * worker becomes unowned at its stored price and counts against the warm cutoff, like a removed ask's holder; the added
  * slots hold nothing and are in A0.  The warm start and the repair then run unchanged on the remapped state (DESIGN 4).
@@ -381,11 +395,14 @@ enum pm_path {
  * (only those whose stored first ask lies beyond the first of them; an ask switched off and on again counts as
  * neither).  With many asks enabled the pass evaluates everything instead: the pairs of that walk, |E| x nw, count as
  * |E| x nw / T written rows against the PM_TUNE_INCR cutoff, next to the range's written rows.
- * pm_update_asks and pm_resize_asks keep it too.  A replaced row counts as disabled and enabled again: it is in E when
- * it is enabled now and in D when it was enabled at the stored evaluation, and its orphans are walked from the ask
+ * pm_update_asks, pm_resize_asks, pm_remove_asks and pm_insert_asks keep it too.  A replaced row counts as disabled
+ * and enabled again: it is in E when it is enabled now and in D when it was enabled at the stored evaluation, and its orphans are walked from the ask
  * itself, not the one after it (the new row may still accept them); workers whose stored first ask lies beyond it
- * meet it in the E-pass.  Appended rows are in E.  A shrink sets every stored first ask >= the new n_asks to PM_NONE
- * (that worker had no feasible ask before it).  Replaced and appended asks count against the cutoff as E does.  Each
+ * meet it in the E-pass.  Appended and inserted rows are in E.  pm_remove_asks and pm_insert_asks (and a shrink, their
+ * tail case) move every stored first ask f with its row, on the device: f - (removed rows below f) + (rows inserted
+ * before a position <= f).  A worker whose stored first ask was removed lands on the next kept row and is walked again
+ * from that row itself (an orphan); with no kept row after it, its stored first ask is PM_NONE (it had no feasible ask
+ * before the removed one).  Replaced, appended and inserted asks count against the cutoff as E does.  Each
  * engine decides
  * against the cutoff by its own range's counts, so in one sharded pass some ranks may evaluate their range in full
  * while others run incrementally; every rank still makes the one exchange.  pm_stats under the flag (nw = the range's
@@ -412,9 +429,10 @@ enum pm_path {
  * stored state; reference-mode passes leave it alone.  An auction pass refused before it runs keeps it: disabled asks
  * (PM_E_UNSUPPORTED), tables outside the integer domain (PM_E_INVALID), and an ask, enabled or not, referencing a
  * model pattern missing from the model table (PM_E_STATE; any pattern_id >= n_patterns, 0xFFFFFFFF included); so does
- * a certificate refused for any reason.  pm_update_asks and pm_resize_asks keep it: A0 also holds every
- * replaced ask and every appended ask (which has no stored cap or floor), and step 1 also releases the holder of every
- * removed ask (a shrink of pm_resize_asks): that worker becomes unowned at its stored price as the shrink runs, joins
+ * a certificate refused for any reason.  pm_update_asks, pm_resize_asks, pm_remove_asks and pm_insert_asks keep it:
+ * kept asks keep their holds (slot by slot, under their new indices), A0 also holds every replaced ask and every
+ * appended or inserted ask (which has no stored cap or floor, and holds nothing), and step 1 also releases the holder of
+ * every removed ask (a shrink of pm_resize_asks, or pm_remove_asks): that worker becomes unowned at its stored price as the shrink runs, joins
  * R at price 0 here when its price was positive, and is not counted in n_released (its ask no longer exists).  The
  * cutoff test counts |R0| + |A0| + the rows past a worker shrink + the removed asks that held a worker.  pm_stats of a
  * warm pass: evals = the release's pair evaluations
@@ -460,7 +478,7 @@ int pm_auction_reverse_stats(pm_engine*, uint32_t* n_phases, uint32_t* n_reverse
  *   4. one reverse stage at eps = 1 (the rounds of PM_AUCTION_REVERSE), until no unowned worker has a positive price.
  * eps-complementary slackness holds after every step, so the result is within T of the optimum of the current instance
  * (the optimum with cost_scale = T + 1), as a cold pass's is (DESIGN 4); it need not equal the cold or the warm pass's
- * result.  Nothing is released beyond step 1.  After pm_update_asks / pm_resize_asks, A0 and the release are those
+ * result.  Nothing is released beyond step 1.  After pm_update_asks / pm_resize_asks / pm_remove_asks / pm_insert_asks, A0 and the release are those
  * of the warm start: a removed ask's worker is unowned at its stored price.  pm_auction_state: warm = 1, n_released =
  * the asks of step 1.
  * pm_auction_reverse_stats: 1 phase, the reverse rounds and bids of step 4.  pm_stats: n_rounds = the forward rounds;
@@ -486,8 +504,8 @@ int pm_auction_reverse_stats(pm_engine*, uint32_t* n_phases, uint32_t* n_reverse
  * priced-unowned sum are exact 128-bit integers (hi: the signed high 64 bits, lo: the low 64 bits).  evals = T x W.
  * ask_bound (NULL-able): row(t) per ask.  Refusals, none of which changes anything: NULL engine or out: PM_E_INVALID;
  * no stored state (where pm_auction_state returns PM_E_STATE), a worker count other than the stored pass's, an ask table
- * resized by pm_resize_asks since the last auction pass (pm_update_asks is audited: n_bad_holds shows the holds the new
- * rows reject), or an ask
+ * resized by pm_resize_asks, pm_remove_asks or pm_insert_asks since the last auction pass (pm_update_asks is audited:
+ * n_bad_holds shows the holds the new rows reject), or an ask
  * referencing a model pattern missing from the model table: PM_E_STATE; disabled asks: PM_E_UNSUPPORTED; tables and
  * parameters outside the auction's integer domain: PM_E_INVALID.  The call changes nothing pm_fetch_result,
  * pm_get_stats, pm_table_version, pm_auction_state or pm_auction_reverse_stats report, nor what the next warm or repair
@@ -513,7 +531,8 @@ int pm_auction_certificate(pm_engine*, pm_auction_cert* out, int64_t* ask_bound)
  * lose it, and the next pass is cold.  pm_auction_state (the prices) and pm_auction_assignment export it;
  * pm_auction_restore takes it back, into this engine or another one with the same tables.
  * pm_auction_assignment: the stored state's assignment, assigned[t] = the worker ask t holds, or PM_NONE, over the
- * current n_asks (after the remaps of pm_update_asks / pm_resize_asks; worker indices are the stored pass's rows).
+ * current n_asks (after the remaps of pm_update_asks / pm_resize_asks / pm_remove_asks / pm_insert_asks; worker
+ * indices are the stored pass's rows).
  * PM_E_STATE where pm_auction_state returns it; a NULL assigned with n_asks > 0: PM_E_INVALID.
  * pm_auction_restore audits the caller's state against the tables as they stand now, then makes it the stored state.
  * With S = cost_scale, feasible(t,w) as for the reverse rounds (candidate, compatible, ask_price <= cap, reputation >=
@@ -554,7 +573,8 @@ int pm_auction_restore(pm_engine*, const int64_t* price, uint32_t n_workers, con
  * copy of an ask row: slot s of ask t is sum_{u<t} d[u] + k, k < d[t]; there are D = sum d[t] of them (D = n_asks
  * without demands or with every demand 1).
  * pm_auction_slot_assignment: the stored state's assignment per slot, assigned[s] = a worker or PM_NONE, over the
- * current slot table (after the remaps of pm_update_asks, pm_resize_asks and pm_set_ask_demand).  *n_slots is in/out:
+ * current slot table (after the remaps of pm_update_asks, pm_resize_asks, pm_remove_asks, pm_insert_asks and
+ * pm_set_ask_demand).  *n_slots is in/out:
  * with assigned NULL the call writes D and returns PM_OK; otherwise *n_slots must equal D.  Refusals: PM_E_INVALID for
  * a NULL n_slots, or *n_slots other than D (D is written back); PM_E_STATE where pm_auction_state returns it (before
  * the size query: nothing is written).  Without demands the output is pm_auction_assignment's, byte for byte.
@@ -666,10 +686,13 @@ pm_engine*  pm_multi_engine(pm_multi*, uint32_t i);   /* per-device access (stat
 const char* pm_multi_last_error(const pm_multi*);
 int pm_multi_set_asks(pm_multi*, const pm_ask* asks, uint32_t n_asks, const pm_gpu_opt* opts, uint32_t n_opts);
 int pm_multi_set_ask_enabled(pm_multi*, const uint32_t* idx, const uint8_t* enabled, uint32_t n);
-/* pm_update_asks / pm_resize_asks on every device; a refused call changes no device */
+/* pm_update_asks / pm_resize_asks / pm_remove_asks / pm_insert_asks on every device; a refused call changes no device */
 int pm_multi_update_asks(pm_multi*, const uint32_t* idx, const pm_ask* asks, uint32_t n,
                          const pm_gpu_opt* opts, uint32_t n_opts);
 int pm_multi_resize_asks(pm_multi*, uint32_t n_asks, const pm_ask* added, const pm_gpu_opt* opts, uint32_t n_opts);
+int pm_multi_remove_asks(pm_multi*, const uint32_t* idx, uint32_t n);
+int pm_multi_insert_asks(pm_multi*, const uint32_t* before, const pm_ask* asks, uint32_t n, const pm_gpu_opt* opts,
+                         uint32_t n_opts);
 int pm_multi_set_model_table(pm_multi*, const uint32_t* bits, uint32_t n_patterns, uint32_t n_models,
                              uint32_t words_per_pattern);
 int pm_multi_set_worker_count(pm_multi*, uint32_t n_workers);

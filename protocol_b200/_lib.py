@@ -53,6 +53,8 @@ def load() -> C.CDLL:
         "pm_set_ask_enabled": (i32, [vp, vp, vp, u32]),
         "pm_update_asks": (i32, [vp, vp, vp, u32, vp, u32]),
         "pm_resize_asks": (i32, [vp, u32, vp, vp, u32]),
+        "pm_remove_asks": (i32, [vp, vp, u32]),
+        "pm_insert_asks": (i32, [vp, vp, vp, u32, vp, u32]),
         "pm_set_model_table": (i32, [vp, vp, u32, u32, u32]),
         "pm_set_worker_count": (i32, [vp, u32]),
         "pm_upsert_workers": (i32, [vp, vp, vp, u32, u32]),
@@ -97,6 +99,8 @@ def load() -> C.CDLL:
         "pm_multi_set_ask_enabled": (i32, [vp, vp, vp, u32]),
         "pm_multi_update_asks": (i32, [vp, vp, vp, u32, vp, u32]),
         "pm_multi_resize_asks": (i32, [vp, u32, vp, vp, u32]),
+        "pm_multi_remove_asks": (i32, [vp, vp, u32]),
+        "pm_multi_insert_asks": (i32, [vp, vp, vp, u32, vp, u32]),
         "pm_multi_set_model_table": (i32, [vp, vp, u32, u32, u32]),
         "pm_multi_set_worker_count": (i32, [vp, u32]),
         "pm_multi_upsert_workers": (i32, [vp, vp, vp, u32, u32]),

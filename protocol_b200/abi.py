@@ -132,7 +132,7 @@ EXPORTS = [
     "pm_interner_create", "pm_interner_destroy", "pm_intern_model", "pm_intern_pattern", "pm_interner_table",
     "pm_parse_requirements", "pm_sort_configs", "pm_address_canonical",
     "pm_create", "pm_destroy", "pm_last_error", "pm_alloc_pinned", "pm_free_pinned",
-    "pm_set_asks", "pm_set_ask_enabled", "pm_update_asks", "pm_resize_asks", "pm_set_model_table", "pm_set_worker_count", "pm_upsert_workers",
+    "pm_set_asks", "pm_set_ask_enabled", "pm_update_asks", "pm_resize_asks", "pm_remove_asks", "pm_insert_asks", "pm_set_model_table", "pm_set_worker_count", "pm_upsert_workers",
     "pm_set_worker_locations", "pm_set_worker_addr_rank", "pm_set_flags",
     "pm_set_ask_price_caps", "pm_set_auction_params", "pm_set_worker_reputation", "pm_set_ask_min_reputation",
     "pm_set_ask_demand",
@@ -143,7 +143,7 @@ EXPORTS = [
     "pm_resize_workers", "pm_update_workers", "pm_table_version", "pm_create_sibling",
     "pm_comm_unique_id", "pm_comm_create", "pm_comm_destroy", "pm_attach_comm",
     "pm_multi_create", "pm_multi_destroy", "pm_multi_size", "pm_multi_engine", "pm_multi_last_error",
-    "pm_multi_set_asks", "pm_multi_set_ask_enabled", "pm_multi_update_asks", "pm_multi_resize_asks", "pm_multi_set_model_table", "pm_multi_set_worker_count", "pm_multi_upsert_workers",
+    "pm_multi_set_asks", "pm_multi_set_ask_enabled", "pm_multi_update_asks", "pm_multi_resize_asks", "pm_multi_remove_asks", "pm_multi_insert_asks", "pm_multi_set_model_table", "pm_multi_set_worker_count", "pm_multi_upsert_workers",
     "pm_multi_set_worker_locations", "pm_multi_set_worker_addr_rank", "pm_multi_set_flags",
     "pm_multi_resize_workers", "pm_multi_update_workers", "pm_multi_sync", "pm_multi_table_version",
     "pm_multi_match", "pm_multi_fetch_result",

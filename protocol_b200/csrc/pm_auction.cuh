@@ -940,19 +940,6 @@ __global__ void pm_auction_warm_seed(AuctionParams p, const uint32_t* __restrict
     }
   }
 }
-// pm_resize_asks shrank the ask table under a stored state: every kept row held by a removed ask (index >= n_asks)
-// becomes unowned at its stored price, as a released worker does; `count` gets how many there were
-__global__ void pm_auction_drop_asks(uint32_t* __restrict__ owner, uint32_t n_rows, uint32_t n_asks, uint32_t* __restrict__ count) {
-  uint32_t k = 0;
-  for (uint32_t w = blockIdx.x * blockDim.x + threadIdx.x; w < n_rows; w += gridDim.x * blockDim.x) {
-    const uint32_t t = owner[w];
-    if (t != kNone && t >= n_asks) {
-      owner[w] = kNone;
-      ++k;
-    }
-  }
-  if (k) atomicAdd(count, k);
-}
 // every unowned worker with a positive price (the released ones, and what an eps-scaled pass left inflated) goes to 0
 // and joins R; mark[w] says whether it did
 __global__ void pm_auction_warm_reset(AuctionParams p, uint32_t* __restrict__ raised, uint32_t* __restrict__ mark) {
@@ -1292,18 +1279,21 @@ __global__ void pm_auction_slot_table(const uint32_t* __restrict__ off, uint32_t
     if (floor) slot_floor[s] = floor[t];
   }
 }
-// A demand change under a stored state: old slot k of ask t keeps its hold as new slot k while k < the new demand;
-// past it the slot is gone and its worker becomes unowned at its stored price, counted in `count` when it is a kept row
-// (as pm_auction_drop_asks does for a removed ask).  new_assigned is all PM_NONE before: added slots hold nothing.
-__global__ void pm_auction_demand_remap(const uint32_t* __restrict__ old_off, const uint32_t* __restrict__ new_off, uint32_t n_asks,
-                                        uint32_t n_old, const uint32_t* __restrict__ old_assigned, uint32_t* __restrict__ new_assigned,
-                                        uint32_t* __restrict__ owner, uint32_t n_rows, uint32_t* __restrict__ count) {
+// A demand change or an ask-table splice under a stored state: old slot k of ask t keeps its hold as slot k of ask
+// map[t] (map null: t) while that ask is kept and k < its new demand; otherwise the slot is gone and its worker becomes
+// unowned at its stored price, counted in `count` when it is a kept row.  Offsets null: one slot per ask (no demands).
+// n_asks: the old table's.  new_assigned is all PM_NONE before: added and inserted slots hold nothing.
+__global__ void pm_auction_slot_remap(const uint32_t* __restrict__ old_off, const uint32_t* __restrict__ new_off,
+                                      const uint32_t* __restrict__ map, uint32_t n_asks, uint32_t n_old,
+                                      const uint32_t* __restrict__ old_assigned, uint32_t* __restrict__ new_assigned,
+                                      uint32_t* __restrict__ owner, uint32_t n_rows, uint32_t* __restrict__ count) {
   uint32_t freed = 0;
   for (uint32_t s = blockIdx.x * blockDim.x + threadIdx.x; s < n_old; s += gridDim.x * blockDim.x) {
-    const uint32_t t = auc_ask_of_slot(old_off, n_asks, s), k = s - old_off[t];
+    const uint32_t t = old_off ? auc_ask_of_slot(old_off, n_asks, s) : s, k = old_off ? s - old_off[t] : 0u;
+    const uint32_t nt = map ? map[t] : t;
     const uint32_t w = old_assigned[s];
-    if (k < new_off[t + 1] - new_off[t]) {
-      const uint32_t ns = new_off[t] + k;
+    if (nt != kNone && k < (new_off ? new_off[nt + 1] - new_off[nt] : 1u)) {
+      const uint32_t ns = (new_off ? new_off[nt] : nt) + k;
       new_assigned[ns] = w;
       if (w < n_rows) owner[w] = ns;
     } else if (w < n_rows) {

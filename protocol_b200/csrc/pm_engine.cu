@@ -354,31 +354,35 @@ struct pm_engine {
   bool incr_evals_pending = false;      // stats.evals of the incremental pass arrives with the pass's one sync
   // The mask the stored evaluation was taken under (eval_on) and the asks toggled, replaced or appended since (toggled,
   // each once; an ask switched off and on again is listed but has eval_on == ask_on; replaced: repl_mark).  Appended
-  // asks have eval_on == 0.  walk_start: the orphan walk's start bounds.
-  std::vector<uint8_t> eval_on, toggle_mark, repl_mark;
+  // asks have eval_on == 0.  orph_mark: the next kept row of a removed ask that had workers (pm_remove_asks moved their
+  // stored first ask onto it).  walk_start: the orphan walk's start bounds.
+  std::vector<uint8_t> eval_on, toggle_mark, repl_mark, orph_mark;
   std::vector<uint32_t> toggled;
-  DevBuf<uint32_t> walk_start, toggle_dev;
+  DevBuf<uint32_t> walk_start, toggle_dev, splice_dev;   // splice_dev: pm_remove_asks / pm_insert_asks staging
 
   // E (enabled since the stored evaluation) and D (disabled since), increasing; a D entry is ask << 1 | replaced.  A
   // replaced row counts as disabled and enabled again: in E when it is enabled now, in D when it was at the stored
-  // evaluation, its orphans walked from the ask itself
+  // evaluation, its orphans walked from the ask itself.  An orph_mark row is in D with the bit too, whatever its own
+  // state: the workers of the removed ask share its index now, and are walked from it (the E-pass skips a worker's
+  // stored ask, so listing it in E alone would not test them against it).
   void split_toggles(std::vector<uint32_t>* en, std::vector<uint32_t>* dis) const {
     en->clear();
     dis->clear();
     for (uint32_t t : toggled) {
       if (repl_mark[t]) {
         if (ask_on[t]) en->push_back(t);
-        if (eval_on[t]) dis->push_back(t << 1 | 1u);
-      } else if (ask_on[t] != eval_on[t]) {
-        if (ask_on[t]) en->push_back(t);
-        else dis->push_back(t << 1);
+        if (eval_on[t] || orph_mark[t]) dis->push_back(t << 1 | 1u);
+      } else {
+        if (ask_on[t] && !eval_on[t]) en->push_back(t);
+        if (orph_mark[t]) dis->push_back(t << 1 | 1u);
+        else if (!ask_on[t] && eval_on[t]) dis->push_back(t << 1);
       }
     }
     std::sort(en->begin(), en->end());
     std::sort(dis->begin(), dis->end());
   }
   void clear_toggled() {
-    for (uint32_t t : toggled) { toggle_mark[t] = 0; repl_mark[t] = 0; eval_on[t] = ask_on[t]; }
+    for (uint32_t t : toggled) { toggle_mark[t] = 0; repl_mark[t] = 0; orph_mark[t] = 0; eval_on[t] = ask_on[t]; }
     toggled.clear();
   }
   void mark_toggled(uint32_t t) {
@@ -498,9 +502,9 @@ struct pm_engine {
   DevBuf<uint32_t> rst_assigned, rst_kept, rst_owner;
   DevBuf<uint64_t> rst_acc;
   PinBuf<uint64_t> h_rst_acc;
-  // pm_resize_asks since the stored state: the removed asks that held a kept row (those rows are unowned now, at their
-  // stored prices; they count against the cutoff), and whether the ask table was resized at all (the certificate then
-  // waits for the next pass)
+  // pm_resize_asks / pm_remove_asks / pm_insert_asks since the stored state: the removed asks that held a kept row
+  // (those rows are unowned now, at their stored prices; they count against the cutoff), and whether rows were removed
+  // or added at all (the certificate then waits for the next pass)
   uint32_t auc_removed_held = 0;
   bool auc_asks_resized = false;
   // Ask demands (pm_set_ask_demand; the auction only): empty while every ask takes one worker, and the auction then runs
@@ -786,12 +790,56 @@ static int check_ask_rows(const pm_engine* e, const char* fn, const uint32_t* id
   return PM_OK;
 }
 
-// pm_update_asks / pm_resize_asks after their checks (the masks already sized to n_asks): rows[i] goes to ask idx[i]
-// (distinct, < n_asks; a grow's rows are the indices past the kept ones), the option range it references in `opts`
-// appended to raw_opts and its opt_off rebased onto that copy; raw_opts is compacted when its dead rows outnumber the
-// live ones; then the whole table is converted again and the disabled asks are turned off (pm_ask_toggle).
+// Rows removed from and inserted into the ask table (pm_remove_asks, pm_insert_asks; pm_resize_asks is the tail case).
+// removed: old indices, increasing and distinct; before: per inserted row the old row it goes before, non-decreasing.
+// map: old index -> new index (kNone: removed); at: the new index of each inserted row; succ: per removed row the new
+// index of the next kept row (n_new: none).
+struct AskSplice {
+  uint32_t n_old = 0, n_new = 0;
+  std::vector<uint32_t> removed, before, map, at, succ;
+  AskSplice(uint32_t n, std::vector<uint32_t> rm, std::vector<uint32_t> bf)
+      : n_old(n), removed(std::move(rm)), before(std::move(bf)), map(n), at(before.size()), succ(removed.size()) {
+    uint32_t r = 0, i = 0, j = 0;
+    for (uint32_t t = 0; t <= n_old; ++t) {
+      while (i < before.size() && before[i] == t) at[i++] = j++;
+      if (t == n_old) break;
+      if (r < removed.size() && removed[r] == t) {
+        map[t] = pm::kNone;
+        succ[r++] = j;   // a call removes or inserts, never both: the next index handed out is the next kept row's
+      } else {
+        map[t] = j++;
+      }
+    }
+    n_new = j;
+  }
+  // every kept row keeps its index: a shrink or a grow (pm_resize_asks)
+  bool tail() const {
+    return (removed.empty() || removed[0] == n_old - removed.size()) && (before.empty() || before[0] == n_old);
+  }
+  // a per-ask vector moved with its rows, `fill` in the inserted rows; one of another length (empty: not in use) stays
+  template <class V> void apply(std::vector<V>* v, V fill) const {
+    if (v->size() != n_old) return;
+    std::vector<V> out(n_new, fill);
+    for (uint32_t t = 0; t < n_old; ++t)
+      if (map[t] != pm::kNone) out[map[t]] = (*v)[t];
+    v->swap(out);
+  }
+  // a list of asks renamed, the removed ones dropped
+  void apply_list(std::vector<uint32_t>* list) const {
+    size_t k = 0;
+    for (uint32_t t : *list)
+      if (map[t] != pm::kNone) (*list)[k++] = map[t];
+    list->resize(k);
+  }
+};
+
+// pm_update_asks / pm_resize_asks / pm_remove_asks / pm_insert_asks after their checks (the masks already moved to the
+// new table): with a splice, asks_h is moved first and the raw rows go up again unless every kept row keeps its index;
+// rows[i] goes to ask idx[i] (distinct, < n_asks), the option range it references in `opts` appended to raw_opts and its
+// opt_off rebased onto that copy; raw_opts is compacted when its dead rows outnumber the live ones; then the whole table
+// is converted again and the disabled asks are turned off (pm_ask_toggle).
 static int commit_asks(pm_engine* e, uint32_t n_asks, const uint32_t* idx, const pm_ask* rows, uint32_t n,
-                       const pm_gpu_opt* opts) {
+                       const pm_gpu_opt* opts, const AskSplice* sp = nullptr) {
   const uint32_t base = e->raw_n_opts;
   // only the option ranges the new rows reference go up, each row's range after the last, opt_off rebased onto it:
   // a caller may pass its whole option table for one changed ask without leaving that table behind as dead rows
@@ -802,6 +850,7 @@ static int commit_asks(pm_engine* e, uint32_t n_asks, const uint32_t* idx, const
     add.insert(add.end(), opts + a.opt_off, opts + a.opt_off + a.n_opts);
     a.opt_off = off;
   }
+  if (sp) sp->apply(&e->asks_h, pm_ask{});
   e->asks_h.resize(n_asks);
   for (uint32_t i = 0; i < n; ++i) e->asks_h[idx[i]] = moved[i];
   uint64_t opt_rows = 0, live = 0;
@@ -837,8 +886,15 @@ static int commit_asks(pm_engine* e, uint32_t n_asks, const uint32_t* idx, const
       PM_CUDA(e->raw_opts.grow_keep(raw, base, e->stream));
       PM_CUDA(cudaMemcpyAsync(e->raw_opts.p + base, add.data(), add.size() * sizeof(pm_gpu_opt), cudaMemcpyHostToDevice, e->stream));
     }
-    PM_CUDA(e->raw_asks.grow_keep(std::max<uint32_t>(n_asks, 1), std::min<size_t>(e->raw_asks.n, n_asks), e->stream));
-    if (n) {
+    const bool moved_rows = sp && !sp->tail();
+    if (moved_rows) {   // the whole table goes up again (O(T), like the conversion that follows)
+      PM_CUDA(e->raw_asks.ensure(std::max<uint32_t>(n_asks, 1)));
+      if (n_asks)
+        PM_CUDA(cudaMemcpyAsync(e->raw_asks.p, e->asks_h.data(), (size_t)n_asks * sizeof(pm_ask), cudaMemcpyHostToDevice, e->stream));
+    } else {
+      PM_CUDA(e->raw_asks.grow_keep(std::max<uint32_t>(n_asks, 1), std::min<size_t>(e->raw_asks.n, n_asks), e->stream));
+    }
+    if (n && !moved_rows) {
       PM_CUDA(e->scratch_idx.ensure(n)); PM_CUDA(e->upd_asks.ensure(n));
       PM_CUDA(cudaMemcpyAsync(e->scratch_idx.p, idx, (size_t)n * 4, cudaMemcpyHostToDevice, e->stream));
       PM_CUDA(cudaMemcpyAsync(e->upd_asks.p, moved.data(), (size_t)n * sizeof(pm_ask), cudaMemcpyHostToDevice, e->stream));
@@ -961,7 +1017,7 @@ void pm_destroy(pm_engine* e) {
   e->cost.release(); e->first_ask.release(); e->ask_count.release(); e->ask_best.release();
   e->stripe_rank.release(); e->rank_best.release();
   e->eval_first.release(); e->h_dirty.release(); e->dirty_dev.release(); e->incr_evals.release();
-  e->walk_start.release(); e->toggle_dev.release();
+  e->walk_start.release(); e->toggle_dev.release(); e->splice_dev.release();
   e->keys.release(); e->keys_sorted.release(); e->iota.release(); e->order.release();
   e->hist.release(); e->seg_start.release(); e->ngroups.release(); e->group_base.release();
   e->base_len.release(); e->xhead.release(); e->xnext.release(); e->xcount.release();
@@ -1047,6 +1103,7 @@ int pm_set_asks(pm_engine* e, const pm_ask* asks, uint32_t n_asks, const pm_gpu_
   e->eval_on.assign(n_asks, 1);
   e->toggle_mark.assign(n_asks, 0);
   e->repl_mark.assign(n_asks, 0);
+  e->orph_mark.assign(n_asks, 0);
   recount_kinds(e);
   e->have_caps = false;
   e->have_min_rep = false;
@@ -1115,7 +1172,7 @@ int pm_set_ask_enabled(pm_engine* e, const uint32_t* idx, const uint8_t* enabled
   return PM_OK;
 } catch (...) { return pm_guard_rc(); }
 
-// Ask-table deltas.  Both calls check everything on the host first (a refusal changes nothing), then edit the raw rows
+// Ask-table deltas.  Every call checks everything on the host first (a refusal changes nothing), then edit the raw rows
 // and convert the whole table again (commit_asks).  The stored evaluation and the stored auction state are kept: the
 // changed asks are listed for the next incremental pass (E / D) and the next warm pass (A0).  A failure after the
 // checks (a CUDA error) leaves tables that are not trusted: the ask table is dropped, as a failed pm_set_asks does.
@@ -1181,6 +1238,132 @@ int pm_update_asks(pm_engine* e, const uint32_t* idx, const pm_ask* asks, uint32
   });
 } catch (...) { return pm_guard_rc(); }
 
+// The part of pm_resize_asks / pm_remove_asks / pm_insert_asks after their checks.  The stored evaluation's first asks
+// and the stored auction state are remapped on the device and every per-ask host copy moves with its rows; then the
+// rows are committed.  Removed rows take their enabled flag, cap, floor and demand with them; inserted rows are enabled,
+// with cap 0, floor 0 and demand 1, in E (eval_on 0) and in A0, holding nothing; kept rows keep every mark.
+static int splice_asks(pm_engine* e, const AskSplice& sp, const pm_ask* rows, const pm_gpu_opt* opts) {
+  PM_CUDA(cudaSetDevice(e->device));
+  const uint32_t n_old = sp.n_old, n_new = sp.n_new, nr = (uint32_t)sp.removed.size(), ni = (uint32_t)sp.before.size();
+  const bool moves = nr || (ni && sp.before[0] < n_old);   // some kept row changes its index, or a row goes
+  PM_CUDA(e->splice_dev.ensure(std::max<size_t>((size_t)nr + ni + n_old, 1)));
+  uint32_t* rm_dev = e->splice_dev.p;
+  uint32_t* bf_dev = rm_dev + nr;
+  uint32_t* map_dev = bf_dev + ni;
+  if (nr) PM_CUDA(cudaMemcpyAsync(rm_dev, sp.removed.data(), (size_t)nr * 4, cudaMemcpyHostToDevice, e->stream));
+  if (ni) PM_CUDA(cudaMemcpyAsync(bf_dev, sp.before.data(), (size_t)ni * 4, cudaMemcpyHostToDevice, e->stream));
+  // the stored evaluation: the workers of a removed ask land on its next kept row, which lists them as orphans
+  std::vector<uint32_t> orphans_at;
+  if (e->eval_valid) {
+    for (uint32_t r = 0; r < nr; ++r) {
+      const uint32_t t = sp.removed[r];
+      if ((e->eval_on[t] || e->orph_mark[t]) && sp.succ[r] < n_new) orphans_at.push_back(sp.succ[r]);
+    }
+    uint32_t w0 = 0, nw = 0;
+    e->shard(&w0, &nw);
+    nw = w0 < e->n_workers ? std::min(nw, e->n_workers - w0) : 0u;
+    if (moves && nw) {
+      pm::pm_splice_first_asks<<<std::min(blocks_for(nw, 256), 8u * e->sms), 256, 0, e->stream>>>(e->eval_first.p, w0, nw, rm_dev, nr,
+                                                                                                  bf_dev, ni, n_new);
+      PM_LAUNCH_CHECK("pm_splice_first_asks");
+    }
+  }
+  sp.apply(&e->ask_on, (uint8_t)1);
+  sp.apply(&e->eval_on, (uint8_t)0);
+  sp.apply(&e->toggle_mark, (uint8_t)0);
+  sp.apply(&e->repl_mark, (uint8_t)0);
+  sp.apply(&e->orph_mark, (uint8_t)0);
+  sp.apply_list(&e->toggled);
+  for (uint32_t s : sp.at) e->mark_toggled(s);
+  for (uint32_t s : orphans_at) {
+    e->orph_mark[s] = 1;
+    e->mark_toggled(s);
+  }
+  // demands move with their rows (all 1 again: dropped, as pm_set_ask_demand drops them)
+  const uint32_t old_slots = e->n_slots();
+  const bool had_demand = !e->demand.empty();
+  if (had_demand) {
+    if (e->auc_state) {
+      PM_CUDA(e->dem_off_old.ensure((size_t)n_old + 1));
+      PM_CUDA(cudaMemcpyAsync(e->dem_off_old.p, e->dem_off_h.data(), ((size_t)n_old + 1) * 4, cudaMemcpyHostToDevice, e->stream));
+      PM_CUDA(cudaStreamSynchronize(e->stream));   // dem_off_h is rebuilt below
+    }
+    sp.apply(&e->demand, 1u);
+    e->dem_off_h.assign((size_t)n_new + 1, 0u);
+    for (uint32_t t = 0; t < n_new; ++t) e->dem_off_h[t + 1] = e->dem_off_h[t] + e->demand[t];
+    const int rc = upload_demand(e);
+    if (rc != PM_OK) return rc;
+  }
+  // the stored auction state: each kept slot's hold moves to its row's new slots; a removed slot's kept row becomes
+  // unowned at its stored price and counts against the cutoff; inserted slots hold nothing
+  if (e->auc_state) {
+    const uint32_t D_new = e->demand.empty() ? n_new : e->dem_off_h[n_new];
+    PM_CUDA(e->auc_assigned_tmp.ensure(std::max<uint32_t>(D_new, 1)));
+    PM_CUDA(cudaMemsetAsync(e->auc_assigned_tmp.p, 0xFF, (size_t)std::max<uint32_t>(D_new, 1) * 4, e->stream));
+    PM_CUDA(cudaMemsetAsync(e->counters.p + 17, 0, 4, e->stream));
+    if (old_slots) {
+      if (n_old) PM_CUDA(cudaMemcpyAsync(map_dev, sp.map.data(), (size_t)n_old * 4, cudaMemcpyHostToDevice, e->stream));
+      pm::pm_auction_slot_remap<<<std::min(blocks_for(old_slots, 256), 8u * e->sms), 256, 0, e->stream>>>(
+          had_demand ? e->dem_off_old.p : nullptr, e->demand.empty() ? nullptr : e->dem_off.p, map_dev, n_old, old_slots,
+          e->auc_assigned.p, e->auc_assigned_tmp.p, e->auc_owner.p, e->auc_kept, e->counters.p + 17);
+      PM_LAUNCH_CHECK("pm_auction_slot_remap");
+    }
+    PM_CUDA(cudaMemcpyAsync(e->h_scalars.p + 17, e->counters.p + 17, 4, cudaMemcpyDeviceToHost, e->stream));
+    PM_CUDA(cudaStreamSynchronize(e->stream));   // (the map is a host vector the caller owns)
+    std::swap(e->auc_assigned, e->auc_assigned_tmp);
+    e->auc_removed_held += e->h_scalars.p[17];
+    sp.apply(&e->auc_ask_mark, (uint8_t)0);
+    sp.apply(&e->auc_cap_stored, 0u);
+    sp.apply(&e->auc_floor_stored, 0u);
+    sp.apply(&e->auc_dem_kept, 0u);
+    sp.apply_list(&e->auc_toggled);
+    for (uint32_t s : sp.at) e->auc_mark_ask(s);
+    e->auc_asks_resized = true;
+  }
+  if (e->have_caps) {
+    sp.apply(&e->cap_host, 0u);
+    PM_CUDA(e->price_cap.ensure(std::max<uint32_t>(n_new, 1)));
+    if (n_new) PM_CUDA(cudaMemcpyAsync(e->price_cap.p, e->cap_host.data(), (size_t)n_new * 4, cudaMemcpyHostToDevice, e->stream));
+  }
+  if (e->have_min_rep) {
+    sp.apply(&e->floor_host, 0u);
+    PM_CUDA(e->ask_min_rep.ensure(std::max<uint32_t>(n_new, 1)));
+    if (n_new) PM_CUDA(cudaMemcpyAsync(e->ask_min_rep.p, e->floor_host.data(), (size_t)n_new * 4, cudaMemcpyHostToDevice, e->stream));
+  }
+  return commit_asks(e, n_new, sp.at.data(), rows, ni, opts, &sp);   // (synchronises before the host copies change again)
+}
+
+// The checks of pm_remove_asks, on the host before anything changes: the distinct indices, increasing
+static int check_remove(const pm_engine* e, const uint32_t* idx, uint32_t n, std::vector<uint32_t>* removed, std::string* err) {
+  if (n && !idx) { *err = "pm_remove_asks: null"; return PM_E_INVALID; }
+  removed->assign(idx, idx + n);
+  for (uint32_t t : *removed)
+    if (t >= e->n_asks) { *err = "pm_remove_asks: ask index out of range"; return PM_E_INVALID; }
+  std::sort(removed->begin(), removed->end());
+  removed->erase(std::unique(removed->begin(), removed->end()), removed->end());
+  return PM_OK;
+}
+
+// The checks of pm_insert_asks and of pm_resize_asks' growth (before: every row at n_asks): the positions, the rows and
+// their option ranges (check_ask_rows), the ask count and the slot total
+static int check_insert(const pm_engine* e, const char* fn, const uint32_t* before, const pm_ask* asks, uint32_t n,
+                        const pm_gpu_opt* opts, uint32_t n_opts, std::string* err) {
+  if ((n && (!before || !asks)) || (n_opts && !opts)) { *err = std::string(fn) + ": null"; return PM_E_INVALID; }
+  for (uint32_t i = 0; i < n; ++i)
+    if (before[i] > e->n_asks || (i && before[i] < before[i - 1])) {
+      *err = std::string(fn) + ": before[] decreases or exceeds n_asks";
+      return PM_E_INVALID;
+    }
+  if ((uint64_t)e->n_asks + n >= (1u << 30)) { *err = std::string(fn) + ": too many asks"; return PM_E_INVALID; }
+  std::vector<uint32_t> uidx;
+  std::vector<pm_ask> urows;
+  const int rc = check_ask_rows(e, fn, nullptr, asks, n, n_opts, &uidx, &urows, err);
+  if (rc != PM_OK) return rc;
+  // inserted asks take one slot each; the slots stay below the ask-count limit
+  if ((uint64_t)e->n_slots() + n >= (1u << 30)) { *err = std::string(fn) + ": the ask demands' total reaches 2^30"; return PM_E_INVALID; }
+  return PM_OK;
+}
+
 int pm_resize_asks(pm_engine* e, uint32_t n_asks, const pm_ask* added, const pm_gpu_opt* opts, uint32_t n_opts) try {
   if (!e) return PM_E_INVALID;
   std::lock_guard<std::mutex> lk(e->mu);
@@ -1188,97 +1371,55 @@ int pm_resize_asks(pm_engine* e, uint32_t n_asks, const pm_ask* added, const pm_
   if (n_asks >= (1u << 30)) return e->fail(PM_E_INVALID, "pm_resize_asks: too many asks");
   const uint32_t old = e->n_asks;
   const uint32_t n_add = n_asks > old ? n_asks - old : 0u;
-  if ((n_add && !added) || (n_opts && !opts)) return e->fail(PM_E_INVALID, "pm_resize_asks: null");
-  std::vector<uint32_t> uidx;
-  std::vector<pm_ask> urows;
+  // the tail case of pm_remove_asks / pm_insert_asks: drop [n_asks, old), or insert every added row at the end
+  std::vector<uint32_t> removed, before(n_add, old);
   {
     std::string err;
-    const int rc = check_ask_rows(e, "pm_resize_asks", nullptr, added, n_add, n_opts, &uidx, &urows, &err);
+    const int rc = check_insert(e, "pm_resize_asks", before.data(), added, n_add, opts, n_opts, &err);
     if (rc != PM_OK) return e->fail((pm_status)rc, err);
   }
   if (n_asks == old) return PM_OK;
-  // with demands the appended asks take one slot each; the slots stay below the ask-count limit
-  const uint32_t old_slots = e->n_slots();
-  const uint32_t new_slots = e->demand.empty() ? n_asks : (n_asks < old ? e->dem_off_h[n_asks] : old_slots + n_add);
-  if ((uint64_t)old_slots + n_add >= (1u << 30)) return e->fail(PM_E_INVALID, "pm_resize_asks: the ask demands' total reaches 2^30");
+  for (uint32_t t = n_asks; t < old; ++t) removed.push_back(t);
   ++e->table_version;
   return ask_delta(e, [&]() -> int {
-    PM_CUDA(cudaSetDevice(e->device));
-    auto drop_from = [&](std::vector<uint32_t>* list) {
-      list->erase(std::remove_if(list->begin(), list->end(), [&](uint32_t t) { return t >= n_asks; }), list->end());
-    };
-    auto cut = [&](auto* v) { if (v->size() > n_asks) v->resize(n_asks); };
-    if (n_asks < old) {
-      // a worker whose stored first ask was removed had no feasible ask before it: it has none now
-      if (e->eval_valid && e->n_workers) {
-        pm::pm_drop_first_asks<<<std::min(blocks_for(e->n_workers, 256), 8u * e->sms), 256, 0, e->stream>>>(e->eval_first.p, e->n_workers,
-                                                                                                            n_asks);
-        const cudaError_t ce = cudaGetLastError();
-        if (ce != cudaSuccess) return e->fail(PM_E_CUDA, std::string("launch pm_drop_first_asks: ") + cudaGetErrorString(ce));
-      }
-      drop_from(&e->toggled);
-      // the kept rows held by a removed ask become unowned at their stored prices; they count against the cutoff
-      if (e->auc_state && e->auc_kept) {
-        cudaError_t ce = cudaMemsetAsync(e->counters.p + 17, 0, 4, e->stream);
-        if (ce == cudaSuccess) {
-          pm::pm_auction_drop_asks<<<std::min(blocks_for(e->auc_kept, 256), 8u * e->sms), 256, 0, e->stream>>>(e->auc_owner.p, e->auc_kept,
-                                                                                                               new_slots, e->counters.p + 17);
-          ce = cudaGetLastError();
-        }
-        if (ce == cudaSuccess) ce = cudaMemcpyAsync(e->h_scalars.p + 17, e->counters.p + 17, 4, cudaMemcpyDeviceToHost, e->stream);
-        if (ce == cudaSuccess) ce = cudaStreamSynchronize(e->stream);
-        if (ce != cudaSuccess) return e->fail(PM_E_CUDA, std::string("pm_resize_asks: ") + cudaGetErrorString(ce));
-        e->auc_removed_held += e->h_scalars.p[17];
-      }
-      drop_from(&e->auc_toggled);
-      cut(&e->auc_ask_mark); cut(&e->auc_cap_stored); cut(&e->auc_floor_stored); cut(&e->auc_dem_kept);
-      cut(&e->ask_on); cut(&e->eval_on); cut(&e->toggle_mark); cut(&e->repl_mark); cut(&e->cap_host); cut(&e->floor_host);
-      if (!e->demand.empty()) {
-        e->demand.resize(n_asks);
-        e->dem_off_h.resize((size_t)n_asks + 1);
-      }
-    } else {
-      // appended rows: enabled, cap 0, floor 0, in E (eval_on 0) and in A0 (no stored cap or floor), holding nothing
-      e->ask_on.resize(n_asks, 1);
-      e->eval_on.resize(n_asks, 0);
-      e->toggle_mark.resize(n_asks, 0);
-      e->repl_mark.resize(n_asks, 0);
-      for (uint32_t t = old; t < n_asks; ++t) e->mark_toggled(t);
-      auto zero_tail = [&](auto& buf, int byte) -> cudaError_t {
-        cudaError_t ce = buf.grow_keep(n_asks, old, e->stream);
-        if (ce == cudaSuccess) ce = cudaMemsetAsync(buf.p + old, byte, (size_t)(n_asks - old) * sizeof(*buf.p), e->stream);
-        return ce;
-      };
-      cudaError_t ce = cudaSuccess;
-      if (e->have_caps) {
-        e->cap_host.resize(n_asks, 0u);
-        ce = zero_tail(e->price_cap, 0);
-      }
-      if (ce == cudaSuccess && e->have_min_rep) {
-        e->floor_host.resize(n_asks, 0u);
-        ce = zero_tail(e->ask_min_rep, 0);
-      }
-      if (!e->demand.empty()) {
-        e->demand.resize(n_asks, 1u);
-        for (uint32_t t = old; t < n_asks; ++t) e->dem_off_h.push_back(e->dem_off_h[t] + 1u);
-      }
-      if (ce == cudaSuccess && e->auc_state) {   // the appended slots hold nothing
-        ce = e->auc_assigned.grow_keep(new_slots, old_slots, e->stream);
-        if (ce == cudaSuccess) ce = cudaMemsetAsync(e->auc_assigned.p + old_slots, 0xFF, (size_t)(new_slots - old_slots) * 4, e->stream);
-        e->auc_ask_mark.resize(n_asks, 0);
-        e->auc_cap_stored.resize(n_asks, 0u);
-        e->auc_floor_stored.resize(n_asks, 0u);
-        if (!e->auc_dem_kept.empty()) e->auc_dem_kept.resize(n_asks, 0u);
-        for (uint32_t t = old; t < n_asks; ++t) e->auc_mark_ask(t);
-      }
-      if (ce != cudaSuccess) return e->fail(PM_E_CUDA, std::string("pm_resize_asks: ") + cudaGetErrorString(ce));
-    }
-    if (!e->demand.empty()) {
-      const int rc = upload_demand(e);
-      if (rc != PM_OK) return rc;
-    }
-    if (e->auc_state) e->auc_asks_resized = true;
-    return commit_asks(e, n_asks, uidx.data(), urows.data(), (uint32_t)uidx.size(), opts);
+    const AskSplice sp(old, std::move(removed), std::move(before));
+    return splice_asks(e, sp, added, opts);
+  });
+} catch (...) { return pm_guard_rc(); }
+
+int pm_remove_asks(pm_engine* e, const uint32_t* idx, uint32_t n) try {
+  if (!e) return PM_E_INVALID;
+  std::lock_guard<std::mutex> lk(e->mu);
+  if (!e->have_asks) return e->fail(PM_E_STATE, "pm_remove_asks: no ask table");
+  std::vector<uint32_t> removed;
+  {
+    std::string err;
+    const int rc = check_remove(e, idx, n, &removed, &err);
+    if (rc != PM_OK) return e->fail((pm_status)rc, err);
+  }
+  if (removed.empty()) return PM_OK;
+  ++e->table_version;
+  return ask_delta(e, [&]() -> int {
+    const AskSplice sp(e->n_asks, std::move(removed), {});
+    return splice_asks(e, sp, nullptr, nullptr);
+  });
+} catch (...) { return pm_guard_rc(); }
+
+int pm_insert_asks(pm_engine* e, const uint32_t* before, const pm_ask* asks, uint32_t n, const pm_gpu_opt* opts,
+                   uint32_t n_opts) try {
+  if (!e) return PM_E_INVALID;
+  std::lock_guard<std::mutex> lk(e->mu);
+  if (!e->have_asks) return e->fail(PM_E_STATE, "pm_insert_asks: no ask table");
+  {
+    std::string err;
+    const int rc = check_insert(e, "pm_insert_asks", before, asks, n, opts, n_opts, &err);
+    if (rc != PM_OK) return e->fail((pm_status)rc, err);
+  }
+  if (n == 0) return PM_OK;
+  ++e->table_version;
+  return ask_delta(e, [&]() -> int {
+    const AskSplice sp(e->n_asks, {}, std::vector<uint32_t>(before, before + n));
+    return splice_asks(e, sp, asks, opts);
   });
 } catch (...) { return pm_guard_rc(); }
 
@@ -3146,10 +3287,10 @@ int pm_set_ask_demand(pm_engine* e, const uint32_t* demand, uint32_t n_asks) try
       PM_CUDA(cudaMemsetAsync(e->auc_assigned_tmp.p, 0xFF, (size_t)std::max<uint32_t>(D_new, 1) * 4, e->stream));
       PM_CUDA(cudaMemsetAsync(e->counters.p + 17, 0, 4, e->stream));
       if (D_old) {
-        pm::pm_auction_demand_remap<<<std::min(blocks_for(D_old, 256), 8u * e->sms), 256, 0, e->stream>>>(
-            e->dem_off_old.p, e->dem_off.p, T, D_old, e->auc_assigned.p, e->auc_assigned_tmp.p, e->auc_owner.p, e->auc_kept,
-            e->counters.p + 17);
-        PM_LAUNCH_CHECK("pm_auction_demand_remap");
+        pm::pm_auction_slot_remap<<<std::min(blocks_for(D_old, 256), 8u * e->sms), 256, 0, e->stream>>>(
+            e->dem_off_old.p, e->dem_off.p, nullptr, T, D_old, e->auc_assigned.p, e->auc_assigned_tmp.p, e->auc_owner.p,
+            e->auc_kept, e->counters.p + 17);
+        PM_LAUNCH_CHECK("pm_auction_slot_remap");
       }
       PM_CUDA(cudaMemcpyAsync(e->h_scalars.p + 17, e->counters.p + 17, 4, cudaMemcpyDeviceToHost, e->stream));
       PM_CUDA(cudaStreamSynchronize(e->stream));   // (old_off and off are locals)
@@ -3552,6 +3693,30 @@ int pm_multi_resize_asks(pm_multi* m, uint32_t n_asks, const pm_ask* added, cons
     }
   }
   PM_MULTI_EACH(pm_resize_asks(e, n_asks, added, opts, n_opts));
+} catch (...) { return pm_guard_rc(); }
+int pm_multi_remove_asks(pm_multi* m, const uint32_t* idx, uint32_t n) try {
+  if (m && !m->engines.empty()) {
+    pm_engine* e0 = m->engines[0];
+    std::lock_guard<std::mutex> lk(e0->mu);
+    std::vector<uint32_t> removed;
+    if (e0->have_asks) {
+      const int rc = check_remove(e0, idx, n, &removed, &m->err);
+      if (rc != PM_OK) return rc;
+    }
+  }
+  PM_MULTI_EACH(pm_remove_asks(e, idx, n));
+} catch (...) { return pm_guard_rc(); }
+int pm_multi_insert_asks(pm_multi* m, const uint32_t* before, const pm_ask* asks, uint32_t n, const pm_gpu_opt* opts,
+                         uint32_t n_opts) try {
+  if (m && !m->engines.empty()) {
+    pm_engine* e0 = m->engines[0];
+    std::lock_guard<std::mutex> lk(e0->mu);
+    if (e0->have_asks) {
+      const int rc = check_insert(e0, "pm_insert_asks", before, asks, n, opts, n_opts, &m->err);
+      if (rc != PM_OK) return rc;
+    }
+  }
+  PM_MULTI_EACH(pm_insert_asks(e, before, asks, n, opts, n_opts));
 } catch (...) { return pm_guard_rc(); }
 int pm_multi_set_model_table(pm_multi* m, const uint32_t* bits, uint32_t n_patterns, uint32_t n_models, uint32_t words) try {
   PM_MULTI_EACH(pm_set_model_table(e, bits, n_patterns, n_models, words));

@@ -1072,12 +1072,28 @@ __global__ void pm_scatter_asks(pm_ask* __restrict__ asks, const uint32_t* __res
   if (i < n) asks[idx[i]] = rows[i];
 }
 
-// pm_resize_asks shrank the table under a stored evaluation: a worker whose stored first ask was removed had no feasible
-// ask before it, so it has none now (until the asks enabled since meet it in the E-pass)
-__global__ void pm_drop_first_asks(uint32_t* __restrict__ eval_first, uint32_t n, uint32_t n_asks) {
-  for (uint32_t w = blockIdx.x * blockDim.x + threadIdx.x; w < n; w += gridDim.x * blockDim.x) {
-    const uint32_t f = eval_first[w];
-    if (f != kNone && f >= n_asks) eval_first[w] = kNone;
+// pm_remove_asks / pm_insert_asks / pm_resize_asks under a stored evaluation: each stored first ask f of the range
+// [w0, w0 + nw) moves to f - (removed asks below f) + (rows inserted before a position <= f); `removed` and `before`
+// are increasing old indices.  A removed f lands on the new index of its next kept row, whose orphans the engine lists
+// for the next incremental pass; past the new end (n_asks) there is none, and the worker has no feasible ask.
+__global__ void pm_splice_first_asks(uint32_t* __restrict__ eval_first, uint32_t w0, uint32_t nw, const uint32_t* __restrict__ removed,
+                                     uint32_t nr, const uint32_t* __restrict__ before, uint32_t ni, uint32_t n_asks) {
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < nw; i += gridDim.x * blockDim.x) {
+    const uint32_t f = eval_first[w0 + i];
+    if (f == kNone) continue;
+    uint32_t lo = 0, hi = nr;   // removed asks < f
+    while (lo < hi) {
+      const uint32_t mid = (lo + hi) >> 1;
+      if (__ldg(removed + mid) < f) lo = mid + 1; else hi = mid;
+    }
+    const uint32_t r = lo;
+    lo = 0, hi = ni;            // inserted rows with before <= f
+    while (lo < hi) {
+      const uint32_t mid = (lo + hi) >> 1;
+      if (__ldg(before + mid) <= f) lo = mid + 1; else hi = mid;
+    }
+    const uint32_t g = f - r + lo;
+    eval_first[w0 + i] = g < n_asks ? g : kNone;
   }
 }
 

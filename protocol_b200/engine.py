@@ -168,6 +168,21 @@ class Engine:
         self._check(self._lib.pm_resize_asks(self._h, n, _ptr(added) if len(added) else None, _ptr(opts), len(opts)))
         self.n_asks = n
 
+    def remove_asks(self, idx):
+        """Remove the ask rows idx (any order; a repeated index removes its row once); the rows after them move up,
+        order kept (pm_remove_asks).  The stored evaluation and auction state are kept, remapped to the new indices."""
+        idx = _remove_args(idx)
+        self._check(self._lib.pm_remove_asks(self._h, _ptr(idx) if len(idx) else None, len(idx)))
+        self.n_asks -= len(np.unique(idx))
+
+    def insert_asks(self, before, asks: np.ndarray, opts: np.ndarray | None = None):
+        """Insert rows `asks` (options in `opts`) before the current rows before[i] (non-decreasing, n_asks = append;
+        rows with equal before[] keep their order), enabled, with cap 0, floor 0 and demand 1 (pm_insert_asks)."""
+        before, asks, opts = _insert_args(before, asks, opts)
+        self._check(self._lib.pm_insert_asks(self._h, _ptr(before) if len(before) else None, _ptr(asks) if len(asks) else None,
+                                             len(before), _ptr(opts), len(opts)))
+        self.n_asks += len(before)
+
     def set_model_table(self, bits: np.ndarray, n_patterns: int, n_models: int, words: int):
         bits = np.ascontiguousarray(bits, dtype=np.uint32)
         self._check(self._lib.pm_set_model_table(self._h, _ptr(bits), n_patterns, n_models, words))
@@ -385,6 +400,18 @@ def _ask_delta_args(idx, asks, opts):
     return idx, asks, opts
 
 
+def _insert_args(before, asks, opts):
+    """(before, asks, opts) as pm_insert_asks takes them: one row per position (the call reads len(before) rows)."""
+    before, asks, opts = _ask_delta_args(before, asks, opts)
+    if len(asks) != len(before):
+        raise ValueError(f"insert_asks: {len(before)} positions for {len(asks)} rows")
+    return before, asks, opts
+
+
+def _remove_args(idx):
+    return np.ascontiguousarray(np.atleast_1d(np.asarray(idx, dtype=np.int64)).astype(np.uint32))
+
+
 def _result_views(r: "abi.PmResult", copy: bool) -> MatchResult:
     def view(ptr, n, dt):
         if n == 0:
@@ -481,6 +508,17 @@ class MultiEngine:
         added = np.ascontiguousarray(np.zeros(0, dtype=abi.ASK) if added is None else added, dtype=abi.ASK)
         opts = np.ascontiguousarray(np.zeros(0, dtype=abi.GPU_OPT) if opts is None else opts, dtype=abi.GPU_OPT)
         self._check(self._lib.pm_multi_resize_asks(self._h, n, _ptr(added) if len(added) else None, _ptr(opts), len(opts)))
+
+    def remove_asks(self, idx):
+        """pm_multi_remove_asks: Engine.remove_asks on every device."""
+        idx = _remove_args(idx)
+        self._check(self._lib.pm_multi_remove_asks(self._h, _ptr(idx) if len(idx) else None, len(idx)))
+
+    def insert_asks(self, before, asks, opts=None):
+        """pm_multi_insert_asks: Engine.insert_asks on every device."""
+        before, asks, opts = _insert_args(before, asks, opts)
+        self._check(self._lib.pm_multi_insert_asks(self._h, _ptr(before) if len(before) else None,
+                                                   _ptr(asks) if len(asks) else None, len(before), _ptr(opts), len(opts)))
 
     def set_model_table(self, bits, n_patterns, n_models, words):
         bits = np.ascontiguousarray(bits, dtype=np.uint32)

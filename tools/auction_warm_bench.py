@@ -17,7 +17,13 @@ remove the last 100 asks (most of them hold a worker).  Each runs as a warm pass
 same tables, alternately, each warm or repair pass after a cold pass of the tables before the change; and as
 pm_set_asks + a cold pass, the one way to take such a change without the deltas.
 
-    python tools/auction_warm_bench.py [--repair | --asks] [--out results/auction_warm.json]
+--splice: asks removed and inserted anywhere in the table (pm_remove_asks / pm_insert_asks): remove 1, 100 and 1 000
+held asks at scattered positions, insert 1, 100 and 1 000 rows at random priorities (with caps).  Each runs as a warm
+pass and a warm repair, each after a cold pass of the tables before the change, with the calls timed.  For comparison
+each is also taken the way without the splices: pm_set_asks of the current rows, the caps, pm_auction_restore_slots of
+the remapped export (the restore audit), then the same pass from the restored state.
+
+    python tools/auction_warm_bench.py [--repair | --asks | --splice] [--out results/auction_warm.json]
 """
 from __future__ import annotations
 
@@ -123,12 +129,63 @@ def ask_series(eng, a, cap, record):
         record(f"set_asks_cold_{case}", n, r)
 
 
+def splice_series(eng, a, cap, record):
+    """--splice: held asks removed at scattered positions and rows inserted at random priorities, each change set as a
+    warm pass and a warm repair, then the same change taken by pm_set_asks + caps + pm_auction_restore_slots."""
+    rng = np.random.default_rng(4)
+    asks, cap = a.asks.copy(), cap.copy()
+    warm = abi.PM_MODE_AUCTION | abi.PM_AUCTION_WARM
+    for case, n in (("remove", 1), ("remove", 100), ("remove", 1000), ("insert", 1), ("insert", 100), ("insert", 1000)):
+        for name, mode in (("warm", warm), ("repair", warm | abi.PM_AUCTION_REPAIR)):
+            eng.set_asks(asks, a.opts)                 # the tables before the change, and a cold pass of them
+            eng.set_price_caps(cap)
+            eng.match(abi.PM_MODE_AUCTION)
+            T = len(asks)
+            if case == "remove":
+                held = np.flatnonzero(assigned_of(eng, T) != NONE)
+                idx = np.sort(rng.choice(held, n, replace=False)).astype(np.uint32)
+                t0 = time.perf_counter()
+                eng.remove_asks(idx)
+                eng.sync()
+                new_asks, new_cap = np.delete(asks, idx.astype(np.int64)), np.delete(cap, idx.astype(np.int64))
+            else:
+                before = np.sort(rng.integers(0, T + 1, n)).astype(np.uint32)
+                src = a.asks[rng.integers(0, len(a.asks), n)]
+                rows = src.copy()
+                rows["opt_off"] = np.concatenate([[0], np.cumsum(src["n_opts"])[:-1]]).astype(np.uint32)
+                own = np.concatenate([a.opts[o:o + k] for o, k in zip(src["opt_off"], src["n_opts"])] or [a.opts[:0]])
+                b = before.astype(np.int64)
+                new_asks = np.insert(asks, b, src)
+                new_cap = np.insert(cap, b, rng.integers(20, 3000, n).astype(np.uint32))
+                t0 = time.perf_counter()
+                eng.insert_asks(before, rows, own)
+                eng.set_price_caps(new_cap)
+                eng.sync()
+            call_ms = round((time.perf_counter() - t0) * 1e3, 2)
+            price, _, _ = eng.auction_state()
+            slots = eng.auction_slot_assignment()
+            r = timed(eng, mode)
+            got = assigned_of(eng, len(new_asks))
+            record(f"{name}_{case}", n, dict(r, call_ms=call_ms))
+            t0 = time.perf_counter()                   # the way without the splices
+            eng.set_asks(new_asks, a.opts)
+            eng.set_price_caps(new_cap)
+            eng.auction_restore_slots(price, slots)
+            eng.sync()
+            restore_ms = round((time.perf_counter() - t0) * 1e3, 2)
+            q = timed(eng, mode)
+            same = bool(np.array_equal(assigned_of(eng, len(new_asks)), got) and q["rounds"] == r["rounds"])
+            record(f"set_asks_restore_{name}_{case}", n, dict(q, call_ms=restore_ms, same_as_splice=same))
+        asks, cap = new_asks, new_cap
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", default=None)
     ap.add_argument("--counts", default="0,10,1000,100000")
     ap.add_argument("--repair", action="store_true", help="also run PM_AUCTION_REPAIR on every change set")
     ap.add_argument("--asks", action="store_true", help="ask-table change sets (pm_update_asks / pm_resize_asks)")
+    ap.add_argument("--splice", action="store_true", help="asks removed and inserted anywhere (pm_remove_asks / pm_insert_asks)")
     args = ap.parse_args()
     gpu = card()
     print(f"card: {gpu}", file=sys.stderr)
@@ -146,9 +203,9 @@ def main():
         rows.append(r)
         print(json.dumps(r), flush=True)
 
-    if args.asks:
+    if args.asks or args.splice:
         record("cold", 0, timed(eng, abi.PM_MODE_AUCTION))
-        ask_series(eng, a, cap, record)
+        (splice_series if args.splice else ask_series)(eng, a, cap, record)
         eng.close()
         if args.out:
             os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)

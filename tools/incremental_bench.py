@@ -28,7 +28,16 @@ sum, as the collective does) and pm_match_finish.  Per rank: `ms_local_host` (wa
 stream sync), `ms_fused` (device time of its evaluation kernels), `ms_total` (device, pm_match_local to the end of
 pm_match_finish, so it includes the wait for the host merge).  --multi: pm_multi over every visible GPU,
 pm_multi_match; per rank `ms_total`, `ms_exchange` and `exchange_bytes` as well.  Every step is checked against an
-unsharded engine's full pass (pm_fetch_result of rank 0)."""
+unsharded engine's full pass (pm_fetch_result of rank 0).
+
+    python tools/incremental_bench.py --splice [...]
+
+Asks removed and inserted anywhere in the table (pm_remove_asks / pm_insert_asks) between passes.  Per round and for
+every s in S, after a full fused lean pass that refreshes the stored evaluation: s asks that hold a group are removed
+at scattered positions, one PM_INCREMENTAL lean pass runs; then s rows (copies of the table's rows, with only their own
+option rows) are inserted at random priorities and one more runs.  Each call is timed on the host clock around the call
+and a synchronise.  For comparison a sibling engine takes the way without the splices, pm_set_asks of the current rows
+and a full lean pass (timed together, `route`), and its result is checked equal to the incremental one."""
 from __future__ import annotations
 
 import argparse
@@ -312,6 +321,8 @@ def main():
     ap.add_argument("--multi", action="store_true", help="pm_multi over every visible GPU")
     ap.add_argument("--ask-updates", dest="ask_updates", action="store_true",
                     help="asks replaced between passes (pm_update_asks) instead of rows written; also times the call")
+    ap.add_argument("--splice", action="store_true",
+                    help="asks removed and inserted anywhere between passes (pm_remove_asks / pm_insert_asks)")
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
 
@@ -322,6 +333,13 @@ def main():
         env = card()
         rows, checked, workload = ask_update_series(args, w, a, bits, npat, nmod, words)
         report(rows, checked, workload, env, "u", args.out, "incremental_ask_update_bench.json")
+        return
+    if args.splice:
+        a = synth.make_asks(args.asks, "mixed")
+        bits, npat, nmod, words = synth.intern_tables(w, a)
+        env = card()
+        rows, checked, workload = splice_series(args, w, a, bits, npat, nmod, words)
+        report(rows, checked, workload, env, "case", args.out, "incremental_splice_bench.json")
         return
     if args.shards or args.multi:
         a = synth.make_asks(args.asks, "mixed")
@@ -456,8 +474,75 @@ def ask_update_series(args, w, a, bits, npat, nmod, words):
     return rows, checked, f"{T} asks x {W} workers (synth mixed), first fit, fused lean; u asks replaced per pass"
 
 
+S = (1, 100, 1_000)
+
+
+def splice_series(args, w, a, bits, npat, nmod, words):
+    """S held asks removed at scattered positions, then S rows inserted at random priorities (pm_remove_asks /
+    pm_insert_asks), each followed by one incremental pass; the calls timed; the sibling's pm_set_asks + full pass
+    (`route`) timed and its result checked equal."""
+    os.environ["PM_TUNE_INCR"] = str(1 << 31)   # read at pm_create: never fall back
+    inc = Engine(timing=True)
+    del os.environ["PM_TUNE_INCR"]
+    ref = Engine(timing=True)
+    for e in (inc, ref):
+        e.set_asks(a.asks, a.opts)
+        e.set_model_table(bits, npat, nmod, words)
+        e.set_workers(w.a, w.b)
+        e.match(LEAN)
+    W = len(w)
+    asks = a.asks.copy()   # the current rows, opt_off into a.opts
+    rng = np.random.default_rng(2027)
+    rows = {"full": []}
+    calls, checked = [], set()
+    for rnd in range(args.rounds):
+        for n in S:
+            rows["full"].append(timed(inc, LEAN))
+            for case in ("remove", "insert"):
+                T = len(asks)
+                if case == "remove":
+                    held = np.unique(inc.fetch().group_ask)
+                    idx = np.sort(rng.choice(held, min(n, len(held)), replace=False)).astype(np.uint32)
+                    t = time.perf_counter()
+                    inc.remove_asks(idx)
+                    inc.sync()
+                    asks = np.delete(asks, idx.astype(np.int64))
+                else:
+                    before = np.sort(rng.integers(0, T + 1, n)).astype(np.uint32)
+                    src = a.asks[rng.integers(0, len(a.asks), n)]
+                    new, own = own_options(src, a.opts)
+                    t = time.perf_counter()
+                    inc.insert_asks(before, new, own)
+                    inc.sync()
+                    asks = np.insert(asks, before.astype(np.int64), src)
+                calls.append({"case": case, "s": n, "n_asks": T, "ms_call": (time.perf_counter() - t) * 1e3})
+                key = f"{case}_{n}"
+                rows.setdefault(key, []).append(timed(inc, INCR))
+                t = time.perf_counter()
+                ref.set_asks(asks, a.opts)
+                r = timed(ref, LEAN)
+                r["ms_host"] = (time.perf_counter() - t) * 1e3
+                rows.setdefault(f"route_{key}", []).append(r)
+                q, got = ref.fetch(), inc.fetch()
+                if not all(np.array_equal(getattr(got, f), getattr(q, f)) for f in FIELDS):
+                    raise SystemExit(f"{key}: the incremental result differs from pm_set_asks + the full pass")
+                checked.add(key)
+    for e in (inc, ref):
+        e.close()
+    for c in calls:
+        print(json.dumps(c))
+    summary = []
+    for case in ("remove", "insert"):
+        for n in S:
+            ms = [c["ms_call"] for c in calls if c["case"] == case and c["s"] == n]
+            summary.append({"case": case, "s": n, "ms_call_median": float(np.median(ms)), "runs": len(ms)})
+    rows["splice_calls"] = summary
+    return rows, checked, (f"{len(a.asks)} asks x {W} workers (synth mixed), first fit, fused lean; s held asks removed, "
+                           f"then s rows inserted, per pass")
+
+
 def report(rows, checked, workload, env, key_name, out_dir, file_name):
-    extra = rows.pop("update_asks_calls", None)
+    extra = {k: rows.pop(k) for k in ("update_asks_calls", "splice_calls") if k in rows}
     summary = []
     for key, rs in rows.items():
         summary.append({key_name: key, "ms_device_median": float(np.median([r["ms_device"] for r in rs])),
@@ -465,12 +550,11 @@ def report(rows, checked, workload, env, key_name, out_dir, file_name):
                         "evals": int(rs[-1]["evals"]), "n_tiles": int(rs[-1]["n_tiles"]), "runs": len(rs),
                         **{k: rs[-1][k] for k in ("n_off", "n_on") if k in rs[-1]}})
     out = {"workload": workload, "card": env, "checked_equal_to_full_pass": sorted(checked), "rows": summary}
-    if extra is not None:
-        out["update_asks_calls"] = extra
+    out.update(extra)
     print(f"{env.get('name')}  power limit {env.get('power_limit_w')} W  SM {env.get('sm_mhz')}/{env.get('sm_max_mhz')} MHz")
-    print(f"{key_name:>8} {'device ms':>10} {'host ms':>9} {'evals':>16} {'n_tiles':>9}")
+    print(f"{key_name:>16} {'device ms':>10} {'host ms':>9} {'evals':>16} {'n_tiles':>9}")
     for s in summary:
-        print(f"{s[key_name]:>8} {s['ms_device_median']:>10.3f} {s['ms_host_median']:>9.3f} {s['evals']:>16} {s['n_tiles']:>9}")
+        print(f"{s[key_name]:>16} {s['ms_device_median']:>10.3f} {s['ms_host_median']:>9.3f} {s['evals']:>16} {s['n_tiles']:>9}")
     print(json.dumps(out))
     if out_dir:
         os.makedirs(out_dir, exist_ok=True)
