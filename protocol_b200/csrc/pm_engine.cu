@@ -330,6 +330,15 @@ struct pm_engine {
   DevBuf<long long> ask_best;
   DevBuf<uint32_t> stripe_rank;        // pm_stripe_rank, once per pass of pm_build_argmin: [ld] column -> rank in its stripe
   DevBuf<long long> rank_best;         // ... [ld] stripe * 1024 + rank -> (price << 32) | worker
+  // The feature dictionary of the converted ask table (convert_asks; pm_kernels.cuh FeatDict): feat_ok when it fits
+  // the 64-bit word, and then pm_build_argmin_feat runs in place of pm_build_argmin.  Its per-pass rows: feat_w
+  // [ld] per column, feat_a [n_asks] per ask, feat_o [option rows] per further OR-option.
+  pm::FeatDict feat{};
+  bool feat_ok = false;
+  DevBuf<uint32_t> feat_buf;
+  PinBuf<uint32_t> h_feat;
+  DevBuf<uint4> feat_w, feat_a;
+  DevBuf<uint2> feat_o;
 
   // The stored evaluation of PM_INCREMENTAL: the per-worker first feasible ask of the last evaluation of this engine's
   // range (shard()), PM_NONE outside it, in its own buffer (first_ask is the resolution's working copy: the sweeps, the
@@ -699,9 +708,38 @@ static int use_ask_form(pm_engine* e, bool auction) {
   return PM_OK;
 }
 
+// The feature dictionary from the values pm_feature_collect left in h_feat: per kind the distinct values in increasing
+// order, bit positions in kind order.  The candidate and never bits are always features (pm_kernels.cuh FeatDict).
+static void build_feat_dict(pm_engine* e) {
+  const uint32_t* h = e->h_feat.p;
+  std::vector<uint32_t> vals[pm::kFeatKinds];
+  const uint32_t pres = h[0] | pm::kKeyCandBit | pm::kKeyNeverBit;
+  for (uint32_t j = 0; j < pm::kKeyPresence; ++j)
+    if ((pres >> j) & 1u) vals[pm::kFeatKey].push_back(j);
+  size_t n = vals[pm::kFeatKey].size();
+  for (uint32_t k = 1; k < pm::kFeatKinds; ++k) {
+    for (uint32_t i = 0; i < pm::kFeatSlots; ++i) {
+      const uint32_t v = h[2 + (k - 1) * pm::kFeatSlots + i];
+      if (v != pm::kNone) vals[k].push_back(v);
+    }
+    std::sort(vals[k].begin(), vals[k].end());
+    n += vals[k].size();
+  }
+  e->feat_ok = h[1] == 0 && n <= pm::kFeatMax;
+  e->feat = pm::FeatDict{};
+  if (!e->feat_ok) return;
+  uint32_t i = 0;
+  for (uint32_t k = 0; k < pm::kFeatKinds; ++k) {
+    e->feat.off[k] = i;
+    for (uint32_t v : vals[k]) e->feat.val[i++] = v;
+  }
+  e->feat.off[pm::kFeatKinds] = i;
+}
+
 // The whole ask table converted from the resident raw rows, O(T + sum K) on the device: pm_ask_counts -> scan ->
 // pm_ask_convert.  pm_set_asks and every delta of pm_update_asks / pm_resize_asks take this one path.  Every row comes
-// out enabled, in the reference modes' form; *st gets the status bits.  Sets n_opts, max_pattern_row and asks_small.
+// out enabled, in the reference modes' form; *st gets the status bits.  Sets n_opts, max_pattern_row, asks_small and the
+// feature dictionary (build_feat_dict).
 static int convert_asks(pm_engine* e, uint32_t n_asks, uint32_t n_raw_opts, uint64_t opt_rows, uint32_t* st) {
   PM_CUDA(e->ask_counts.ensure((size_t)n_asks + 1)); PM_CUDA(e->ask_newoff.ensure((size_t)n_asks + 1));
   PM_CUDA(e->asks.ensure(n_asks)); PM_CUDA(e->amin.ensure(n_asks)); PM_CUDA(e->amax.ensure(n_asks));
@@ -725,6 +763,17 @@ static int convert_asks(pm_engine* e, uint32_t n_asks, uint32_t n_raw_opts, uint
                                                                         ask_tables(e), e->counters.p + 12, e->counters.p + 13);
     PM_LAUNCH_CHECK("pm_ask_convert");
   }
+  // the feature dictionary's values, collected from the converted rows and returned with this synchronisation
+  const size_t feat_words = 2 + (pm::kFeatKinds - 1) * pm::kFeatSlots;
+  PM_CUDA(e->feat_buf.ensure(feat_words));
+  PM_CUDA(e->h_feat.ensure(feat_words));
+  PM_CUDA(cudaMemsetAsync(e->feat_buf.p, 0, 8, e->stream));
+  PM_CUDA(cudaMemsetAsync(e->feat_buf.p + 2, 0xFF, (feat_words - 2) * 4, e->stream));
+  if (n_asks) {
+    pm::pm_feature_collect<<<blocks_for(n_asks, 256), 256, 0, e->stream>>>(e->frows.p, e->opts_fast.p, n_asks, e->feat_buf.p);
+    PM_LAUNCH_CHECK("pm_feature_collect");
+  }
+  PM_CUDA(cudaMemcpyAsync(e->h_feat.p, e->feat_buf.p, feat_words * 4, cudaMemcpyDeviceToHost, e->stream));
   PM_CUDA(cudaMemcpyAsync(e->h_scalars.p + 20, e->counters.p + 12, 8, cudaMemcpyDeviceToHost, e->stream));
   PM_CUDA(cudaMemcpyAsync(e->h_scalars.p + 22, e->ask_newoff.p + n_asks, 4, cudaMemcpyDeviceToHost, e->stream));
   PM_CUDA(cudaStreamSynchronize(e->stream));
@@ -732,6 +781,7 @@ static int convert_asks(pm_engine* e, uint32_t n_asks, uint32_t n_raw_opts, uint
   e->n_opts = e->h_scalars.p[22];
   e->max_pattern_row = e->h_scalars.p[21];
   e->asks_small = (*st & pm::kAskNotSmall) == 0;
+  build_feat_dict(e);
   return PM_OK;
 }
 
@@ -1016,6 +1066,7 @@ void pm_destroy(pm_engine* e) {
   e->upd_a.release(); e->upd_b.release(); e->upd_lat.release(); e->upd_lon.release();
   e->cost.release(); e->first_ask.release(); e->ask_count.release(); e->ask_best.release();
   e->stripe_rank.release(); e->rank_best.release();
+  e->feat_buf.release(); e->h_feat.release(); e->feat_w.release(); e->feat_a.release(); e->feat_o.release();
   e->eval_first.release(); e->h_dirty.release(); e->dirty_dev.release(); e->incr_evals.release();
   e->walk_start.release(); e->toggle_dev.release(); e->splice_dev.release();
   e->keys.release(); e->keys_sorted.release(); e->iota.release(); e->order.release();
@@ -1834,6 +1885,16 @@ static void launch_build_argmin(pm_engine* e, const pm::EvalParams& p, int bits_
   const dim3 grid(blocks_for(ld, pm::kEvalCols), blocks_for(nt, pm::kFastRows));
   const pm::FoldOut fo{e->stripe_rank.p, e->rank_best.p, e->first_ask.p, e->ask_best.p, e->ask_count.p};
   uint32_t* t32 = reinterpret_cast<uint32_t*>(tile);
+  if (e->feat_ok) {   // the feature rows of this pass (match_local)
+    // Unused dynamic shared memory that holds the kernel at two CTAs per SM (228 KB each on H100).  At 64 registers
+    // and 20 KB of its own it would run four, and the step is then 13 % slower than at two (cfg3 on an H100 SXM at
+    // 700 W: 129.3 ms against 114.5 ms; three CTAs: 130.8 ms) — more row streams written at once lose DRAM efficiency.
+    constexpr int kFeatPad = 70000;
+    cudaFuncSetAttribute(pm::pm_build_argmin_feat, cudaFuncAttributeMaxDynamicSharedMemorySize, kFeatPad);
+    pm::pm_build_argmin_feat<<<grid, pm::kEvalThreads, kFeatPad, e->stream>>>(e->feat_a.p, e->feat_o.p, e->feat_w.p, t0, nt, w0, nw,
+                                                                      t32, ld, fo);
+    return;
+  }
   if (p.words == 1) bits_mode = 2;   // one-word acceptance rows are bound into the FastRows, as in launch_build
   if (bits_mode == 2) pm::pm_build_argmin<2><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, t0, nt, w0, nw, t32, ld, fo);
   else if (bits_mode == 1) pm::pm_build_argmin<1><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, t0, nt, w0, nw, t32, ld, fo);
@@ -2074,6 +2135,17 @@ static int match_local_locked(pm_engine* e, uint32_t mode) {
         pm::pm_stripe_rank<<<(unsigned)(ld / pm::kEvalCols), pm::kEvalThreads, 0, e->stream>>>(e->wb.p, w0, nw, e->stripe_rank.p,
                                                                                                e->rank_best.p);
         PM_LAUNCH_CHECK("pm_stripe_rank");
+        if (e->feat_ok) {   // the feature predicate: this pass's F per column and R per ask and option row
+          PM_CUDA(e->feat_w.ensure(ld));
+          PM_CUDA(e->feat_a.ensure(T));
+          PM_CUDA(e->feat_o.ensure(std::max<uint32_t>(e->n_opts, 1)));
+          pm::pm_feature_asks<<<blocks_for(T, 256), 256, 0, e->stream>>>(e->frows.p, e->opts_fast.p, T, e->feat, e->feat_a.p,
+                                                                         e->feat_o.p);
+          PM_LAUNCH_CHECK("pm_feature_asks");
+          pm::pm_feature_workers<<<blocks_for(ld, 256), 256, 0, e->stream>>>(e->wa.p, e->wb.p, e->bits.p, e->words, w0, nw,
+                                                                             e->stripe_rank.p, ld, e->feat, e->feat_w.p);
+          PM_LAUNCH_CHECK("pm_feature_workers");
+        }
       }
       long long* tile = e->cost.p;
       for (uint32_t t0 = 0; t0 < T; t0 += (uint32_t)rows) {

@@ -584,6 +584,235 @@ __global__ void pm_bind_rows(FastRow* __restrict__ rows, const DevOptF* __restri
   rows[t].wp = words == 1u ? bits[prow] : prow;
 }
 
+// ------------------------------------------------------------------ build + argmin, feature form
+// Every clause of the fast predicate compares one worker operand with one threshold of the ask table, and a table has
+// few distinct thresholds.  A FEATURE is one such (clause, threshold) pair; a worker's answer to each of them is
+// computed once per pass, into the 64-bit word F[w], and each OR-option o of an ask gets the mask R_o of the features
+// it requires, with the ask's own scalar clauses OR-ed in.  Then "worker w fails option o" is u_o = R_o & ~F[w] != 0
+// (folded to 32 bits as lo | hi) and "w fails the ask" is min_o u_o != 0 — a minimum, not an AND: two failing options
+// may miss different features: no threshold in the row loop (DESIGN §3).
+// The features of a kind (on the fast domain each equals the sign test eval_fast_first makes):
+//   kFeatKey      presence bit j of `key` (values j < 13)      kFeatCount   count_eff == c
+//   kFeatModel    pattern row r accepts the worker's model     kFeatMemLo / kFeatMemHi   mem_eff >= lo / <= hi
+//   kFeatTotLo / kFeatTotHi   !tot_keep || tot >= lo / <= hi   kFeatCores / kFeatRam / kFeatStorage   >= threshold
+// Thresholds that every worker meets (lo 0, hi 0x7FFFFFFF) are no feature.  The candidate and never bits are always
+// features: every row requires the first, and toggling an ask sets the second without converting the table again.
+enum FeatKind : uint32_t {
+  kFeatKey = 0, kFeatCount, kFeatModel, kFeatMemLo, kFeatMemHi, kFeatTotLo, kFeatTotHi, kFeatCores, kFeatRam, kFeatStorage,
+  kFeatKinds
+};
+constexpr uint32_t kFeatMax = 64;     // features of the 64-bit word
+constexpr uint32_t kFeatSlots = 64;   // distinct values collected per kind (more cannot fit the word anyway)
+constexpr uint32_t kKeyPresence = 13; // key bits 0..12 are presence bits, the gpu count follows
+
+// The dictionary, a kernel parameter: the features of kind k are val[off[k] .. off[k + 1]), increasing, and a
+// feature's bit in F / R is its index.
+struct FeatDict {
+  uint32_t off[kFeatKinds + 1];
+  uint32_t val[kFeatMax];
+};
+
+// Collection, after pm_ask_convert: buf[0] = the key bits some row requires, buf[1] = overflow (more than kFeatSlots
+// values of a kind, or a value equal to the empty slot), buf[2 + (k - 1) * kFeatSlots ..] = the distinct values of
+// kind k >= 1 in a table with linear probing, kNone = empty.
+__device__ __forceinline__ void feat_insert(uint32_t* __restrict__ buf, uint32_t k, uint32_t v) {
+  uint32_t* slots = buf + 2 + (k - 1) * kFeatSlots;
+  if (v == kNone) { atomicOr(buf + 1, 1u); return; }
+  uint32_t h = (v * 0x9E3779B1u) >> 26;   // 6 bits
+  for (uint32_t i = 0; i < kFeatSlots; ++i, h = (h + 1) & (kFeatSlots - 1)) {
+    uint32_t cur = *reinterpret_cast<volatile uint32_t*>(slots + h);
+    if (cur == kNone) cur = atomicCAS(slots + h, kNone, v);
+    if (cur == kNone || cur == v) return;
+  }
+  atomicOr(buf + 1, 1u);
+}
+
+// Calls fn(kind, value) for every feature option `f` requires (the scalar clauses are the ask's: kFeatCores ..).
+template <class Fn>
+__device__ __forceinline__ void opt_features(const DevOptF& f, Fn&& fn) {
+  const uint32_t pres = f.m & ((1u << kKeyPresence) - 1u);
+  for (uint32_t j = 0; j < kKeyPresence; ++j)
+    if ((pres >> j) & 1u) fn(kFeatKey, j);
+  if (f.m >> kKeyPresence) fn(kFeatCount, (f.v >> kKeyCountShift) & 0xFFFFu);
+  if (f.pattern_row) fn(kFeatModel, f.pattern_row);
+  if (f.mem_lo) fn(kFeatMemLo, f.mem_lo);
+  if (f.mem_hi < 0x7FFFFFFFu) fn(kFeatMemHi, f.mem_hi);
+  if (f.tot_lo) fn(kFeatTotLo, f.tot_lo);
+  if (f.tot_hi < 0x7FFFFFFFu) fn(kFeatTotHi, f.tot_hi);
+}
+template <class Fn>
+__device__ __forceinline__ void ask_features(const FastRow& q, Fn&& fn) {
+  if (q.cpu_cores) fn(kFeatCores, q.cpu_cores);
+  if (q.ram_mb) fn(kFeatRam, q.ram_mb);
+  if (q.storage_gb) fn(kFeatStorage, q.storage_gb);
+}
+
+__global__ void pm_feature_collect(const FastRow* __restrict__ frows, const DevOptF* __restrict__ opts_fast, uint32_t n_asks,
+                                   uint32_t* __restrict__ buf) {
+  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= n_asks) return;
+  const FastRow q = frows[t];
+  uint32_t pres = 0;
+  auto add = [&](uint32_t k, uint32_t v) {
+    if (k == kFeatKey) pres |= 1u << v;
+    else feat_insert(buf, k, v);
+  };
+  ask_features(q, add);
+  for (uint32_t o = 0; o < q.n_opts; ++o) opt_features(opts_fast[q.opt_off + o], add);
+  if (pres & ~*reinterpret_cast<volatile uint32_t*>(buf)) atomicOr(buf, pres);
+}
+
+__device__ __forceinline__ unsigned long long feat_bit(const FeatDict& d, uint32_t k, uint32_t v) {
+  for (uint32_t i = d.off[k]; i < d.off[k + 1]; ++i)
+    if (d.val[i] == v) return 1ull << i;
+  return 0ull;   // unreachable: the dictionary holds every value of the converted table (and the never bit)
+}
+
+// Per pass, in stream order: per ask {R_0 lo, R_0 hi, n_opts, opt_off} and per option row R_o (scalar bits included).
+// Reading the converted rows of this pass, a toggle or a rebind needs nothing else.
+__global__ void pm_feature_asks(const FastRow* __restrict__ frows, const DevOptF* __restrict__ opts_fast, uint32_t n_asks,
+                                FeatDict d, uint4* __restrict__ arow, uint2* __restrict__ ropt) {
+  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= n_asks) return;
+  const FastRow q = frows[t];
+  unsigned long long s = 0;
+  ask_features(q, [&](uint32_t k, uint32_t v) { s |= feat_bit(d, k, v); });
+  for (uint32_t o = 0; o < q.n_opts; ++o) {
+    unsigned long long r = s;
+    opt_features(opts_fast[q.opt_off + o], [&](uint32_t k, uint32_t v) { r |= feat_bit(d, k, v); });
+    if (o == 0) arow[t] = make_uint4((uint32_t)r, (uint32_t)(r >> 32), q.n_opts, q.opt_off);
+    else ropt[q.opt_off + o] = make_uint2((uint32_t)r, (uint32_t)(r >> 32));
+  }
+}
+
+// Per pass, in stream order: per column c of [0, ld) {F lo, F hi, price, stripe rank} of worker w0 + c (a null worker
+// past nw: it lacks the candidate bit every row requires).  `bits` is the acceptance table in its own form, `words` per
+// row, whichever form the other kernels read.
+__global__ void pm_feature_workers(const uint4* __restrict__ wa, const uint4* __restrict__ wb, const uint32_t* __restrict__ bits,
+                                   uint32_t words, uint32_t w0, uint32_t nw, const uint32_t* __restrict__ rank, size_t ld,
+                                   FeatDict d, uint4* __restrict__ feat) {
+  const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= ld) return;
+  const WorkerReg w = c < nw ? make_worker(__ldg(wa + w0 + c), __ldg(wb + w0 + c)) : null_worker();
+  unsigned long long F = 0;
+  for (uint32_t k = 0; k < kFeatKinds; ++k)
+    for (uint32_t i = d.off[k]; i < d.off[k + 1]; ++i) {
+      const uint32_t v = d.val[i];
+      bool b;
+      switch (k) {
+        case kFeatKey: b = (w.key >> v) & 1u; break;
+        case kFeatCount: b = w.count_eff == v; break;
+        case kFeatModel: b = (__ldg(bits + (size_t)v * words + w.mword) & w.mmask) != 0u; break;
+        case kFeatMemLo: b = w.mem_eff >= v; break;
+        case kFeatMemHi: b = w.mem_eff <= v; break;
+        case kFeatTotLo: b = !w.tot_keep || w.tot >= v; break;
+        case kFeatTotHi: b = !w.tot_keep || w.tot <= v; break;
+        case kFeatCores: b = w.cores >= v; break;
+        case kFeatRam: b = w.ram >= v; break;
+        default: b = w.storage >= v; break;
+      }
+      F |= (unsigned long long)b << i;
+    }
+  feat[c] = make_uint4((uint32_t)F, (uint32_t)(F >> 32), w.price, rank[c]);
+}
+
+// pm_build_argmin with the feature predicate: the same tile, stores, row fold, first-ask minimum and end-of-CTA merge
+// (build_fast<.., true, true>), the outputs bit for bit.  Per worker and row: two LOP3 for u = R & ~F over the two
+// words and one min for the fail bit b = min(u, 1).  A worker is one 16-byte load in the prologue; a row is one
+// 16-byte shared-memory load; further OR-options (R_o) are read from global memory, warp-uniform.
+__global__ void __launch_bounds__(kEvalThreads, 2)
+pm_build_argmin_feat(const uint4* __restrict__ arow, const uint2* __restrict__ ropt, const uint4* __restrict__ feat,
+                     uint32_t t0, uint32_t nt, uint32_t w0, uint32_t nw, uint32_t* __restrict__ tile, size_t ld, FoldOut fo) {
+  constexpr int kWarps = kEvalThreads / 32;
+  constexpr uint32_t kNoRank = 0x8000u;
+  __shared__ __align__(128) uint4 s_row[kFastRows + 2];   // + 2: the look-ahead loads past the last pair of rows
+  __shared__ uint64_t s_bar;
+  __shared__ uint16_t s_key[kWarps][kFastRows];
+  __shared__ uint8_t s_nb[kWarps][kFastRows];
+  const uint32_t r0 = blockIdx.y * kFastRows;
+  const uint32_t nrows = min(nt - r0, (uint32_t)kFastRows);
+  if (threadIdx.x == 0) {
+    mbar_init(&s_bar, 1);
+    mbar_expect_tx(&s_bar, nrows * 16u);
+    bulk_g2s(s_row, arow + t0 + r0, nrows * 16u, &s_bar);
+  }
+  const uint32_t lane = threadIdx.x & 31u;
+  const uint32_t cbase = blockIdx.x * kEvalCols + (threadIdx.x >> 5) * 128u + lane * 4u;
+  uint32_t fl[kEvalWPT], fh[kEvalWPT], price[kEvalWPT], dy[kEvalWPT], rk[kEvalWPT], cm[kEvalWPT];
+#pragma unroll
+  for (int k = 0; k < kEvalWPT; ++k) {
+    const uint4 v = __ldg(feat + cbase + k);
+    fl[k] = v.x; fh[k] = v.y; price[k] = v.z; rk[k] = v.w;
+    dy[k] = 0x7FFFFFFFu - v.z;
+    asm("" : "+r"(dy[k]));   // kept in a register: ptxas would otherwise recompute it from the price every row
+    cm[k] = kNone;
+  }
+  uint4* out = reinterpret_cast<uint4*>(tile + (size_t)r0 * ld + cbase);
+  size_t row_stride = ld / 4;
+  asm("" : "+l"(row_stride));
+  const uint32_t t_cta = t0 + r0;
+  uint32_t key_slot = (uint32_t)__cvta_generic_to_shared(&s_key[threadIdx.x >> 5][0]);
+  uint32_t nb_slot = (uint32_t)__cvta_generic_to_shared(&s_nb[threadIdx.x >> 5][0]);
+  asm("" : "+r"(key_slot), "+r"(nb_slot));
+  // 1 behind an opaque move: with the literal, ptxas proves b = min(u, 1) is 0 or 1 and turns the multiply-adds below
+  // into compares and selects on the busier ALU pipe (EvalParams::sign_shift does the same for the FastRow kernel)
+  uint32_t one = 1u;
+  asm("" : "+r"(one));
+  auto emit = [&](const uint4& q, uint4* dst, uint32_t r) {
+    uint32_t u[kEvalWPT];
+#pragma unroll
+    for (int k = 0; k < kEvalWPT; ++k) u[k] = (q.x & ~fl[k]) | (q.y & ~fh[k]);
+    for (uint32_t o = 1; o < q.z; ++o) {   // OR-options (node.rs:420-438): the ask fails only if every option does
+      const uint2 R = __ldg(ropt + q.w + o);
+#pragma unroll
+      for (int k = 0; k < kEvalWPT; ++k) u[k] = min(u[k], (R.x & ~fl[k]) | (R.y & ~fh[k]));   // non-zero: every option fails
+    }
+    uint32_t o[kEvalWPT];
+    uint32_t key = kNone, nb = 0;
+#pragma unroll
+    for (int k = 0; k < kEvalWPT; ++k) {
+      const uint32_t b = min(u[k], one);                      // 1 when infeasible
+      o[k] = b * dy[k] + price[k];                            // feasible: price ; infeasible: kNarrowInfeasible
+      cm[k] = min(cm[k], b * 0x80000000u + (t_cta + r));      // the ask, + 2^31 when infeasible
+      key = min(key, b * kNoRank + rk[k]);                    // the rank, + kNoRank when infeasible
+      nb += b;
+    }
+    __stcs(dst, make_uint4(o[0], o[1], o[2], o[3]));
+    key = __reduce_min_sync(0xffffffffu, key);
+    nb = __reduce_add_sync(0xffffffffu, nb);
+    asm volatile("st.shared.u16 [%0], %1;" ::"r"(key_slot + 2u * r), "r"(key) : "memory");
+    asm volatile("st.shared.u8 [%0], %1;" ::"r"(nb_slot + r), "r"(nb) : "memory");
+  };
+  __syncthreads();            // mbarrier initialised
+  mbar_wait(&s_bar, 0);
+  const uint4* q = s_row;
+  uint4 a = q[0];
+  for (uint32_t r = 0; r < nrows; r += 2, q += 2) {
+    const uint4 b = q[1];
+    emit(a, out, r);
+    a = q[2];
+    if (r + 1 < nrows) emit(b, out + row_stride, r + 1);
+    out += 2 * row_stride;
+  }
+  __syncthreads();            // every warp has written its slot of every row
+  const long long* best = fo.best_of_rank + blockIdx.x * kEvalCols;
+  for (uint32_t i = threadIdx.x; i < nrows; i += kEvalThreads) {
+    uint32_t key = kNone, nb = 0;
+#pragma unroll
+    for (int j = 0; j < kWarps; ++j) {
+      key = min(key, (uint32_t)s_key[j][i]);
+      nb += s_nb[j][i];
+    }
+    if (nb < (uint32_t)kEvalCols) {
+      atomicMin(fo.ask_best + t_cta + i, __ldg(best + key));
+      atomicAdd(fo.ask_count + t_cta + i, kEvalCols - nb);
+    }
+  }
+#pragma unroll
+  for (int k = 0; k < kEvalWPT; ++k)
+    if (cm[k] < 0x80000000u && cbase + k < nw) atomicMin(fo.first_ask + w0 + cbase + k, cm[k]);
+}
+
 // ------------------------------------------------------------------ argmin
 constexpr int kArgThreads = 256;
 constexpr int kArgWarps = kArgThreads / 32;
