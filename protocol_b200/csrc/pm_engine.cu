@@ -332,13 +332,16 @@ struct pm_engine {
   DevBuf<long long> rank_best;         // ... [ld] stripe * 1024 + rank -> (price << 32) | worker
   // The feature dictionary of the converted ask table (convert_asks; pm_kernels.cuh FeatDict): feat_ok when it fits
   // the 64-bit word, and then pm_build_argmin_feat runs in place of pm_build_argmin.  Its per-pass rows: feat_w
-  // [ld] per column, feat_a [n_asks] per ask, feat_o [option rows] per further OR-option.
+  // [ld] per column, feat_a [n_asks] per ask, feat_o [option rows] per further OR-option.  Its column order
+  // (pm_feature_keys): the sort's keys and values feat_key / feat_val, sorted into feat_key_s / feat_perm, all [ld].
   pm::FeatDict feat{};
   bool feat_ok = false;
   DevBuf<uint32_t> feat_buf;
   PinBuf<uint32_t> h_feat;
   DevBuf<uint4> feat_w, feat_a;
   DevBuf<uint2> feat_o;
+  DevBuf<unsigned long long> feat_key, feat_key_s;
+  DevBuf<uint32_t> feat_val, feat_perm;
 
   // The stored evaluation of PM_INCREMENTAL: the per-worker first feasible ask of the last evaluation of this engine's
   // range (shard()), PM_NONE outside it, in its own buffer (first_ask is the resolution's working copy: the sweeps, the
@@ -1067,6 +1070,7 @@ void pm_destroy(pm_engine* e) {
   e->cost.release(); e->first_ask.release(); e->ask_count.release(); e->ask_best.release();
   e->stripe_rank.release(); e->rank_best.release();
   e->feat_buf.release(); e->h_feat.release(); e->feat_w.release(); e->feat_a.release(); e->feat_o.release();
+  e->feat_key.release(); e->feat_key_s.release(); e->feat_val.release(); e->feat_perm.release();
   e->eval_first.release(); e->h_dirty.release(); e->dirty_dev.release(); e->incr_evals.release();
   e->walk_start.release(); e->toggle_dev.release(); e->splice_dev.release();
   e->keys.release(); e->keys_sorted.release(); e->iota.release(); e->order.release();
@@ -1883,12 +1887,13 @@ static void launch_fused(pm_engine* e, const pm::EvalParams& p, int bits_mode, b
 static void launch_build_argmin(pm_engine* e, const pm::EvalParams& p, int bits_mode, uint32_t t0, uint32_t nt, uint32_t w0,
                                 uint32_t nw, long long* tile, size_t ld) {
   const dim3 grid(blocks_for(ld, pm::kEvalCols), blocks_for(nt, pm::kFastRows));
-  const pm::FoldOut fo{e->stripe_rank.p, e->rank_best.p, e->first_ask.p, e->ask_best.p, e->ask_count.p};
+  const pm::FoldOut fo{e->stripe_rank.p, e->rank_best.p, e->first_ask.p, e->ask_best.p, e->ask_count.p, e->feat_perm.p};
   uint32_t* t32 = reinterpret_cast<uint32_t*>(tile);
   if (e->feat_ok) {   // the feature rows of this pass (match_local)
     // Unused dynamic shared memory that holds the kernel at two CTAs per SM (228 KB each on H100).  At 64 registers
-    // and 20 KB of its own it would run four, and the step is then 13 % slower than at two (cfg3 on an H100 SXM at
-    // 700 W: 129.3 ms against 114.5 ms; three CTAs: 130.8 ms) — more row streams written at once lose DRAM efficiency.
+    // and 20 KB of its own it would run four, and the step is then 10 % slower than at two, also with the columns
+    // sorted so that most of the tile compresses (cfg3 on an H100 SXM at 700 W: 118.1 ms against 107.5 ms; three
+    // CTAs: 117.9 ms) — more row streams written at once lose DRAM efficiency.
     constexpr int kFeatPad = 70000;
     cudaFuncSetAttribute(pm::pm_build_argmin_feat, cudaFuncAttributeMaxDynamicSharedMemorySize, kFeatPad);
     pm::pm_build_argmin_feat<<<grid, pm::kEvalThreads, kFeatPad, e->stream>>>(e->feat_a.p, e->feat_o.p, e->feat_w.p, t0, nt, w0, nw,
@@ -2132,19 +2137,39 @@ static int match_local_locked(pm_engine* e, uint32_t mode) {
       if (pipe) {   // each column's rank within its stripe, from this pass's prices (ordered after any table update)
         PM_CUDA(e->stripe_rank.ensure(ld));
         PM_CUDA(e->rank_best.ensure(ld));
-        pm::pm_stripe_rank<<<(unsigned)(ld / pm::kEvalCols), pm::kEvalThreads, 0, e->stream>>>(e->wb.p, w0, nw, e->stripe_rank.p,
-                                                                                               e->rank_best.p);
-        PM_LAUNCH_CHECK("pm_stripe_rank");
-        if (e->feat_ok) {   // the feature predicate: this pass's F per column and R per ask and option row
+        const uint32_t* perm = nullptr;   // worker order
+        if (e->feat_ok) {   // the feature predicate: this pass's R per ask and option row, F per worker, column order
           PM_CUDA(e->feat_w.ensure(ld));
           PM_CUDA(e->feat_a.ensure(T));
           PM_CUDA(e->feat_o.ensure(std::max<uint32_t>(e->n_opts, 1)));
+          PM_CUDA(e->feat_key.ensure(ld));
+          PM_CUDA(e->feat_key_s.ensure(ld));
+          PM_CUDA(e->feat_val.ensure(ld));
+          PM_CUDA(e->feat_perm.ensure(ld));
           pm::pm_feature_asks<<<blocks_for(T, 256), 256, 0, e->stream>>>(e->frows.p, e->opts_fast.p, T, e->feat, e->feat_a.p,
                                                                          e->feat_o.p);
           PM_LAUNCH_CHECK("pm_feature_asks");
-          pm::pm_feature_workers<<<blocks_for(ld, 256), 256, 0, e->stream>>>(e->wa.p, e->wb.p, e->bits.p, e->words, w0, nw,
-                                                                             e->stripe_rank.p, ld, e->feat, e->feat_w.p);
-          PM_LAUNCH_CHECK("pm_feature_workers");
+          pm::pm_feature_keys<<<blocks_for(ld, 256), 256, 0, e->stream>>>(e->wa.p, e->wb.p, e->bits.p, e->words, w0, nw, ld,
+                                                                          e->feat, e->feat_key.p, e->feat_val.p,
+                                                                          e->feat_key_s.p, e->feat_perm.p);
+          PM_LAUNCH_CHECK("pm_feature_keys");
+          // stable (LSD) over the key's top n bits, where __brevll put the dictionary's n features
+          const int begin_bit = 64 - std::max<int>((int)e->feat.off[pm::kFeatKinds], 1);
+          size_t tmp = 0;
+          PM_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp, e->feat_key.p, e->feat_key_s.p, e->feat_val.p, e->feat_perm.p,
+                                                  (int)nw, begin_bit, 64, e->stream));
+          PM_CUDA(e->cub_tmp.ensure(tmp));
+          PM_CUDA(cub::DeviceRadixSort::SortPairs(e->cub_tmp.p, tmp, e->feat_key.p, e->feat_key_s.p, e->feat_val.p,
+                                                  e->feat_perm.p, (int)nw, begin_bit, 64, e->stream));
+          perm = e->feat_perm.p;
+        }
+        pm::pm_stripe_rank<<<(unsigned)(ld / pm::kEvalCols), pm::kEvalThreads, 0, e->stream>>>(e->wb.p, perm, w0, nw,
+                                                                                               e->stripe_rank.p, e->rank_best.p);
+        PM_LAUNCH_CHECK("pm_stripe_rank");
+        if (e->feat_ok) {
+          pm::pm_feature_gather<<<blocks_for(ld, 256), 256, 0, e->stream>>>(e->wb.p, e->feat_key_s.p, e->feat_perm.p,
+                                                                            e->stripe_rank.p, w0, nw, ld, e->feat_w.p);
+          PM_LAUNCH_CHECK("pm_feature_gather");
         }
       }
       long long* tile = e->cost.p;

@@ -353,10 +353,11 @@ struct __align__(128) FastStage {
 // stores — see there.  `fo` is unused otherwise.
 struct FoldOut {
   const uint32_t* rank;            // [ld] each column's rank within its 1024-column stripe (pm_stripe_rank)
-  const long long* best_of_rank;   // [ld] stripe s, rank ρ at s * 1024 + ρ: that column's (price << 32) | (w0 + column)
+  const long long* best_of_rank;   // [ld] stripe s, rank ρ at s * 1024 + ρ: that column's (price << 32) | (w0 + worker)
   uint32_t* first_ask;
   long long* ask_best;
   uint32_t* ask_count;
+  const uint32_t* perm;            // pm_build_argmin_feat: [ld] column -> worker offset (pm_feature_keys); else unused
 };
 
 template <int BITS, bool NARROW, bool PIPE>
@@ -523,29 +524,36 @@ pm_build_argmin(EvalParams p, uint32_t t0, uint32_t nt, uint32_t w0, uint32_t nw
   build_fast<BITS, true, true>(p, t0, nt, w0, nw, tile, ld, fo);
 }
 
-// One CTA per 1024-column stripe of a tile with leading dimension ld: sorts the stripe's (price, column) pairs —
-// the order of the packed cost (price << 32) | (w0 + column) — and writes rank[c], each column's place in that order
-// (padding columns at or past nw last), and best_of_rank[stripe * 1024 + ρ], the packed cost of the column at place
-// ρ (kInf for padding, which is never feasible).  Prices are below 2^31 wherever the 32-bit tile runs, so a key is
-// (price << 10) | column in 41 bits.
+// One CTA per 1024-column stripe of a tile with leading dimension ld, whose column c holds worker w0 + perm[c]
+// (w0 + c when perm is null): sorts the stripe's columns by (price, worker) — the order of the packed cost
+// (price << 32) | (w0 + worker) — and writes rank[c], each column's place in that order (padding columns at or past
+// nw last), and best_of_rank[stripe * 1024 + ρ], the packed cost of the column at place ρ (kInf for padding, which is
+// never feasible).  Prices are below 2^31 wherever the 32-bit tile runs, so a key is (price << 32) | worker in 63
+// bits, and padding's all-ones key sorts past every one; the column is the sorted value.
 __global__ void __launch_bounds__(kEvalThreads)
-pm_stripe_rank(const uint4* __restrict__ wb, uint32_t w0, uint32_t nw, uint32_t* __restrict__ rank,
-               long long* __restrict__ best_of_rank) {
-  using Sort = cub::BlockRadixSort<unsigned long long, kEvalThreads, kEvalWPT>;
+pm_stripe_rank(const uint4* __restrict__ wb, const uint32_t* __restrict__ perm, uint32_t w0, uint32_t nw,
+               uint32_t* __restrict__ rank, long long* __restrict__ best_of_rank) {
+  using Sort = cub::BlockRadixSort<unsigned long long, kEvalThreads, kEvalWPT, uint32_t>;
   __shared__ typename Sort::TempStorage tmp;
   const uint32_t c0 = blockIdx.x * kEvalCols;
   unsigned long long key[kEvalWPT];
+  uint32_t col[kEvalWPT];
 #pragma unroll
   for (int k = 0; k < kEvalWPT; ++k) {
     const uint32_t c = threadIdx.x * kEvalWPT + k;
-    key[k] = c0 + c < nw ? ((unsigned long long)__ldg(&wb[w0 + c0 + c].w) << 10) | c : (1ull << 41) | c;
+    col[k] = c;
+    key[k] = ~0ull;
+    if (c0 + c < nw) {
+      const uint32_t w = perm ? __ldg(perm + c0 + c) : c0 + c;
+      key[k] = ((unsigned long long)__ldg(&wb[w0 + w].w) << 32) | w;
+    }
   }
-  Sort(tmp).Sort(key, 0, 42);   // blocked: thread i holds places 4i .. 4i + 3
+  Sort(tmp).Sort(key, col, 0, 64);   // blocked: thread i holds places 4i .. 4i + 3
 #pragma unroll
   for (int k = 0; k < kEvalWPT; ++k) {
-    const uint32_t rho = threadIdx.x * kEvalWPT + k, c = (uint32_t)key[k] & (kEvalCols - 1);
-    rank[c0 + c] = rho;
-    best_of_rank[c0 + rho] = key[k] >> 41 ? kInf : (long long)(((key[k] >> 10) << 32) | (w0 + c0 + c));
+    const uint32_t rho = threadIdx.x * kEvalWPT + k;
+    rank[c0 + col[k]] = rho;
+    best_of_rank[c0 + rho] = key[k] == ~0ull ? kInf : (long long)(((key[k] >> 32) << 32) | (w0 + (uint32_t)key[k]));
   }
 }
 
@@ -685,12 +693,22 @@ __global__ void pm_feature_asks(const FastRow* __restrict__ frows, const DevOptF
   }
 }
 
-// Per pass, in stream order: per column c of [0, ld) {F lo, F hi, price, stripe rank} of worker w0 + c (a null worker
-// past nw: it lacks the candidate bit every row requires).  `bits` is the acceptance table in its own form, `words` per
-// row, whichever form the other kernels read.
-__global__ void pm_feature_workers(const uint4* __restrict__ wa, const uint4* __restrict__ wb, const uint32_t* __restrict__ bits,
-                                   uint32_t words, uint32_t w0, uint32_t nw, const uint32_t* __restrict__ rank, size_t ld,
-                                   FeatDict d, uint4* __restrict__ feat) {
+// The column order of pm_build_argmin_feat's tile.  Its infeasible words (kNarrowInfeasible) are what compressible
+// memory stores compactly, but only in aligned blocks whose words are all equal, and in worker order a row's
+// feasible columns are scattered.  So each pass sorts the workers of [w0, w0 + nw) by __brevll(F), stably: workers
+// with the same F are adjacent, and F's first features (the dictionary's candidate and presence bits, then gpu count
+// and model) vary slowest, so a typical ask's feasible workers become a few dozen runs of columns and nearly every
+// other block of its row is uniform.  Column c < nw then holds worker w0 + perm[c]; the padding columns [nw, ld) stay
+// at the end, null workers, perm[c] = c.
+//
+// Step 1, per pass in stream order: per index c of [0, ld) the key __brevll(F) of worker w0 + c (a null worker past
+// nw: it lacks the candidate bit every row requires) and the value c, for cub::DeviceRadixSort over [0, nw).  The
+// padding entries are written to the sort's output too, which the sort fills only below nw.  `bits` is the acceptance
+// table in its own form, `words` per row, whichever form the other kernels read.
+__global__ void pm_feature_keys(const uint4* __restrict__ wa, const uint4* __restrict__ wb, const uint32_t* __restrict__ bits,
+                                uint32_t words, uint32_t w0, uint32_t nw, size_t ld, FeatDict d,
+                                unsigned long long* __restrict__ key, uint32_t* __restrict__ val,
+                                unsigned long long* __restrict__ key_sorted, uint32_t* __restrict__ perm) {
   const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= ld) return;
   const WorkerReg w = c < nw ? make_worker(__ldg(wa + w0 + c), __ldg(wb + w0 + c)) : null_worker();
@@ -713,13 +731,32 @@ __global__ void pm_feature_workers(const uint4* __restrict__ wa, const uint4* __
       }
       F |= (unsigned long long)b << i;
     }
-  feat[c] = make_uint4((uint32_t)F, (uint32_t)(F >> 32), w.price, rank[c]);
+  key[c] = __brevll(F);
+  val[c] = c;
+  if (c >= nw) {
+    key_sorted[c] = __brevll(F);
+    perm[c] = c;
+  }
 }
 
-// pm_build_argmin with the feature predicate: the same tile, stores, row fold, first-ask minimum and end-of-CTA merge
-// (build_fast<.., true, true>), the outputs bit for bit.  Per worker and row: two LOP3 for u = R & ~F over the two
-// words and one min for the fail bit b = min(u, 1).  A worker is one 16-byte load in the prologue; a row is one
-// 16-byte shared-memory load; further OR-options (R_o) are read from global memory, warp-uniform.
+// Step 3, after the sort and pm_stripe_rank over the sorted columns: per column c of [0, ld) {F lo, F hi, price,
+// stripe rank} of its worker w0 + perm[c], the 16 B pm_build_argmin_feat's prologue reads.
+__global__ void pm_feature_gather(const uint4* __restrict__ wb, const unsigned long long* __restrict__ key_sorted,
+                                  const uint32_t* __restrict__ perm, const uint32_t* __restrict__ rank, uint32_t w0,
+                                  uint32_t nw, size_t ld, uint4* __restrict__ feat) {
+  const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= ld) return;
+  const unsigned long long F = __brevll(key_sorted[c]);
+  const uint32_t price = c < nw ? __ldg(&wb[w0 + perm[c]].w) : 0u;   // the null worker's price
+  feat[c] = make_uint4((uint32_t)F, (uint32_t)(F >> 32), price, rank[c]);
+}
+
+// pm_build_argmin with the feature predicate: the same stores, row fold, first-ask minimum and end-of-CTA merge
+// (build_fast<.., true, true>), the outputs bit for bit, on a tile whose column c holds worker w0 + perm[c] (the
+// column order above; the ranks and best_of_rank carry the workers, and first_ask is flushed to them).  Per worker
+// and row: two LOP3 for u = R & ~F over the two words and one min for the fail bit b = min(u, 1).  A worker is one
+// 16-byte load in the prologue; a row is one 16-byte shared-memory load; further OR-options (R_o) are read from global
+// memory, warp-uniform.
 __global__ void __launch_bounds__(kEvalThreads, 2)
 pm_build_argmin_feat(const uint4* __restrict__ arow, const uint2* __restrict__ ropt, const uint4* __restrict__ feat,
                      uint32_t t0, uint32_t nt, uint32_t w0, uint32_t nw, uint32_t* __restrict__ tile, size_t ld, FoldOut fo) {
@@ -808,9 +845,12 @@ pm_build_argmin_feat(const uint4* __restrict__ arow, const uint2* __restrict__ r
       atomicAdd(fo.ask_count + t_cta + i, kEvalCols - nb);
     }
   }
+  // the columns' workers, loaded only now: held through the row loop they would cost 4 registers there
+  const uint4 pw = __ldg(reinterpret_cast<const uint4*>(fo.perm + cbase));
+  const uint32_t wk[kEvalWPT] = {pw.x, pw.y, pw.z, pw.w};
 #pragma unroll
   for (int k = 0; k < kEvalWPT; ++k)
-    if (cm[k] < 0x80000000u && cbase + k < nw) atomicMin(fo.first_ask + w0 + cbase + k, cm[k]);
+    if (cm[k] < 0x80000000u && cbase + k < nw) atomicMin(fo.first_ask + w0 + wk[k], cm[k]);
 }
 
 // ------------------------------------------------------------------ argmin
