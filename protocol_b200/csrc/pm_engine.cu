@@ -290,7 +290,6 @@ struct pm_engine {
   int tune_generic = 0, tune_auction = 0, tune_prox = 0, tune_auc_good = 0, tune_auc_extra = 0;   // PM_TUNE_*: diagnostics
   bool tune_wide = false;  // PM_TUNE_BUILD=8: the int64 cost tile on the FastRow path too (the 32-bit tile's reference)
   int tune_compress = 1;  // PM_TUNE_COMPRESS=0: the cost tile in plain cudaMalloc memory (A/B runs)
-  bool tune_pipe = true;  // PM_TUNE_PIPE=0: the separate build + argmin launches instead of pm_build_argmin
   DevBuf<uint4> wa, wb;
   DevBuf<double> lat, lon;
   DevBuf<uint32_t> addr_rank;
@@ -1038,7 +1037,6 @@ int pm_create(const pm_cfg* cfg, pm_engine** out) try {
   if (const char* t = std::getenv("PM_TUNE_PROX")) e->tune_prox = std::atoi(t);   // 0: all-SM cooperative sweep; 2: single-CTA sweep
   if (const char* t = std::getenv("PM_TUNE_COMPRESS")) e->tune_compress = std::atoi(t);
   if (const char* t = std::getenv("PM_TUNE_INCR")) e->tune_incr = (uint32_t)std::strtoul(t, nullptr, 10);   // 0: always full
-  if (const char* t = std::getenv("PM_TUNE_PIPE")) e->tune_pipe = std::atoi(t) != 0;
   bool ok = cudaSetDevice(e->device) == cudaSuccess;
   if (ok && cfg->stream) {
     e->stream = (cudaStream_t)cfg->stream;  // caller's stream (e.g. torch's current stream)
@@ -1841,21 +1839,22 @@ static int pick_predicate(pm_engine* e, pm::EvalParams* p, int* bits_mode, bool*
   return PM_OK;
 }
 
-// The 32-bit cost tile (pm_build_argmin, or pm_build_cost_fast<.., true> + pm_argmin<.., true> under PM_TUNE_PIPE=0):
-// on the FastRow path, for tables whose every price is below 0x7FFFFFFF (decide_fast).  The generic predicate and
-// other prices keep the int64 tile; PM_TUNE_BUILD=8 keeps it on the FastRow path too, for A/B runs.
+// The 32-bit cost tile, built and reduced in one launch per tile (pm_build_argmin, pm_build_argmin_feat): on the
+// FastRow path, for tables whose every price is below 0x7FFFFFFF (decide_fast).  The generic predicate and other
+// prices keep the int64 tile, built and reduced by separate launches; PM_TUNE_BUILD=8 keeps it on the FastRow path
+// too, the 32-bit tile's reference.
 static bool narrow_tile(const pm_engine* e, bool fast) {
   return fast && e->prices_narrow && !e->tune_wide;
 }
 
-static void launch_build(pm_engine* e, const pm::EvalParams& p, int bits_mode, bool fast, bool narrow, dim3 grid,
+// The int64 tile's build
+static void launch_build(pm_engine* e, const pm::EvalParams& p, int bits_mode, bool fast, dim3 grid,
                          uint32_t t0, uint32_t nt, uint32_t w0, uint32_t nw, long long* tile, size_t ld) {
 #define PM_BUILD_CASE(B) pm::pm_build_cost<B><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, t0, nt, w0, nw, tile, ld)
 #define PM_FAST_CASE(B)                                                                                                 \
   {                                                                                                                     \
     grid.y = blocks_for(nt, pm::kFastRows);                                                                             \
-    if (narrow) pm::pm_build_cost_fast<B, true><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, t0, nt, w0, nw, tile, ld);      \
-    else pm::pm_build_cost_fast<B, false><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, t0, nt, w0, nw, tile, ld);            \
+    pm::pm_build_cost_fast<B><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, t0, nt, w0, nw, tile, ld);                   \
   }
   if (fast) {   // the FastRow kernel
     // one-word acceptance rows are bound into the FastRows (pm_bind_rows) however many rows there are
@@ -1906,18 +1905,13 @@ static void launch_build_argmin(pm_engine* e, const pm::EvalParams& p, int bits_
   else pm::pm_build_argmin<0><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, t0, nt, w0, nw, t32, ld, fo);
 }
 
-static void launch_argmin(pm_engine* e, cudaStream_t st, bool narrow, const long long* tile, size_t ld, uint32_t nt,
-                          uint32_t t0, uint32_t w0, uint32_t nw) {
-  // 16 x 16 B in flight per lane in both widths: a warp's slice is 8 x 128 columns of the 32-bit tile, 8 x 64 of the int64
-  if (narrow) {
-    dim3 grid(blocks_for(ld, 8 * 128 * pm::kArgWarps), blocks_for(nt, pm::kArgRows));
-    pm::pm_argmin<8, 2, true><<<grid, pm::kArgThreads, 0, st>>>(tile, ld, nt, t0, w0, nw, e->first_ask.p,
-                                                               e->ask_best.p, e->ask_count.p);
-  } else {
-    dim3 grid(blocks_for(ld, 8 * 64 * pm::kArgWarps), blocks_for(nt, pm::kArgRows));
-    pm::pm_argmin<8, 2, false><<<grid, pm::kArgThreads, 0, st>>>(tile, ld, nt, t0, w0, nw, e->first_ask.p,
-                                                                e->ask_best.p, e->ask_count.p);
-  }
+// The int64 tile's argmin
+static void launch_argmin(pm_engine* e, cudaStream_t st, const long long* tile, size_t ld, uint32_t nt, uint32_t t0,
+                          uint32_t w0, uint32_t nw) {
+  // 16 x 16 B in flight per lane: a warp's slice is 8 x 64 columns
+  dim3 grid(blocks_for(ld, 8 * 64 * pm::kArgWarps), blocks_for(nt, pm::kArgRows));
+  pm::pm_argmin<8, 2><<<grid, pm::kArgThreads, 0, st>>>(tile, ld, nt, t0, w0, nw, e->first_ask.p, e->ask_best.p,
+                                                        e->ask_count.p);
 }
 
 // The incremental evaluation.  Three walks (pm_first_ask_rows) rewrite the stored per-worker first feasible ask; each
@@ -2131,10 +2125,9 @@ static int match_local_locked(pm_engine* e, uint32_t mode) {
         cudaGetLastError();
         return e->fail(PM_E_NOMEM, "pm_match: cannot allocate the cost tile; lower pm_cfg.cost_tile_bytes");
       }
-      // One launch per tile (pm_build_argmin) wherever the 32-bit tile runs, unless PM_TUNE_PIPE=0 asks for the
-      // separate build and argmin
-      const bool pipe = narrow && e->tune_pipe;
-      if (pipe) {   // each column's rank within its stripe, from this pass's prices (ordered after any table update)
+      // One launch per tile (pm_build_argmin) wherever the 32-bit tile runs; the int64 tile takes a build and an
+      // argmin launch
+      if (narrow) {   // each column's rank within its stripe, from this pass's prices (ordered after any table update)
         PM_CUDA(e->stripe_rank.ensure(ld));
         PM_CUDA(e->rank_best.ensure(ld));
         const uint32_t* perm = nullptr;   // worker order
@@ -2175,7 +2168,7 @@ static int match_local_locked(pm_engine* e, uint32_t mode) {
       long long* tile = e->cost.p;
       for (uint32_t t0 = 0; t0 < T; t0 += (uint32_t)rows) {
         const uint32_t nt = (uint32_t)std::min<uint64_t>(rows, T - t0);
-        if (pipe) {
+        if (narrow) {
           // one launch that is both: its time counts in ms_build and in ms_argmin
           Timer tb(e, &e->stats.ms_build, e->stream);
           Timer ta(e, &e->stats.ms_argmin, e->stream);
@@ -2189,14 +2182,14 @@ static int match_local_locked(pm_engine* e, uint32_t mode) {
           {
             Timer tm(e, &e->stats.ms_build, e->stream);
             dim3 grid(blocks_for(ld, pm::kEvalCols), blocks_for(nt, pm::kEvalRows));
-            launch_build(e, p, bits_mode, fast, narrow, grid, t0, nt, w0, nw, tile, ld);
+            launch_build(e, p, bits_mode, fast, grid, t0, nt, w0, nw, tile, ld);
             PM_LAUNCH_CHECK("pm_build_cost");
             tm.stop();
             ++e->stats.n_build_launches;
           }
           {
             Timer tm(e, &e->stats.ms_argmin, e->stream);
-            launch_argmin(e, e->stream, narrow, tile, ld, nt, t0, w0, nw);
+            launch_argmin(e, e->stream, tile, ld, nt, t0, w0, nw);
             PM_LAUNCH_CHECK("pm_argmin");
             tm.stop();
             ++e->stats.n_argmin_launches;
@@ -3648,7 +3641,7 @@ int pm_build_cost_tile(pm_engine* e, uint32_t t0, uint32_t nt, int64_t* host_out
     rc = bind_rows(e, p.nacc != nullptr);
     if (rc != PM_OK) return rc;
   }
-  launch_build(e, p, bits_mode, fast, false, grid, t0, nt, w0, nw, e->cost.p, ld);   // exports the int64 tile
+  launch_build(e, p, bits_mode, fast, grid, t0, nt, w0, nw, e->cost.p, ld);   // exports the int64 tile
   PM_LAUNCH_CHECK("pm_build_cost");
   PM_CUDA(cudaMemcpy2DAsync(host_out, (size_t)nw * 8, e->cost.p, ld * 8, (size_t)nw * 8, nt,
                             cudaMemcpyDeviceToHost, e->stream));

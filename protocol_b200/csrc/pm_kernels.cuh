@@ -3,8 +3,10 @@
 //   pm_build_cost   cost-matrix build: int64 cost[t][w] for a tile of asks x a
 //                   stripe of workers, HBM-write-bound (8 B per evaluation; the
 //                   FastRow form's narrow tile: the 32-bit cost word, 4 B)
-//   pm_argmin       one read of the tile (8 or 4 B per evaluation): per-ask packed
+//   pm_argmin       one read of the int64 tile (8 B per evaluation): per-ask packed
 //                   (min_cost, argmin) + feasible count, per-worker first ask
+//   pm_build_argmin the narrow tile's build with the same outputs folded in, never
+//                   read back
 //   pm_fused_eval   the same outputs without materialising the matrix
 //   pm_hist / pm_check_tails / pm_sweep / pm_emit_* : resolution sweep that turns
 //                   "first feasible ask per worker" into the reference's groups
@@ -342,15 +344,14 @@ struct __align__(128) FastStage {
   uint64_t bar;
 };
 
-// NARROW: the tile holds only the 32-bit cost word — the worker's price when feasible, kNarrowInfeasible when not — and
-// `tile` is uint32_t[rows][ld].  The worker index the wide element carries in its low word is the column (+ w0), which
-// pm_argmin<.., true> knows anyway: 4 B per evaluation instead of 8.  A lane then owns the 4 consecutive columns
-// 4l .. 4l+3 of its warp's 128, so each row is one 16-byte store per thread, 512 B per warp and 4 KB per CTA,
-// contiguous.  Only for tables whose every price is below kNarrowInfeasible (pm_check_worker_ranges): at that price a
-// feasible worker could not be told from the sentinel, and at >= 2^31 the wide tile's signed order differs.
-//
-// PIPE (pm_build_argmin, narrow only): the CTA also folds each row's minimum and feasible count from the registers it
-// stores — see there.  `fo` is unused otherwise.
+// FOLD (pm_build_argmin): the 32-bit tile, folded in the kernel that writes it.  The tile holds only the 32-bit cost
+// word — the worker's price when feasible, kNarrowInfeasible when not — and `tile` is uint32_t[rows][ld].  The worker
+// index the int64 element carries in its low word is the column (+ w0): 4 B per evaluation instead of 8.  A lane then
+// owns the 4 consecutive columns 4l .. 4l+3 of its warp's 128, so each row is one 16-byte store per thread, 512 B per
+// warp and 4 KB per CTA, contiguous.  Only for tables whose every price is below kNarrowInfeasible
+// (pm_check_worker_ranges): at that price a feasible worker could not be told from the sentinel, and at >= 2^31 the
+// int64 tile's signed order differs.  The CTA also folds each row's minimum and feasible count from the registers it
+// stores — see pm_build_argmin.  Without FOLD (pm_build_cost_fast) the tile is the int64 one and `fo` is unused.
 struct FoldOut {
   const uint32_t* rank;            // [ld] each column's rank within its 1024-column stripe (pm_stripe_rank)
   const long long* best_of_rank;   // [ld] stripe s, rank ρ at s * 1024 + ρ: that column's (price << 32) | (w0 + worker)
@@ -360,17 +361,86 @@ struct FoldOut {
   const uint32_t* perm;            // pm_build_argmin_feat: [ld] column -> worker offset (pm_feature_keys); else unused
 };
 
-template <int BITS, bool NARROW, bool PIPE>
+// Two rows per iteration share the loop test and the output-pointer bump.  Each row (q[r], emitted to `out` + r rows)
+// is loaded one row ahead, into registers the previous row has finished with, so no row is copied from one buffer to
+// another; q holds two entries past the last row for the look-ahead loads of the last pair (never used).
+template <class Row, class Emit>
+__device__ __forceinline__ void for_each_row_pair(const Row* q, uint32_t nrows, uint4* out, size_t row_stride,
+                                                  Emit&& emit) {
+  Row a = q[0];
+  for (uint32_t r = 0; r < nrows; r += 2, q += 2) {
+    const Row b = q[1];                       // in flight while row r is evaluated
+    emit(a, out, r);
+    a = q[2];                                 // in flight while row r + 1 is evaluated
+    if (r + 1 < nrows) emit(b, out + row_stride, r + 1);
+    out += 2 * row_stride;
+  }
+}
+
+// The row fold of the two build + argmin kernels (pm_build_argmin, pm_build_argmin_feat).  Per warp and row of the
+// CTA, the warp's least key (the least stripe rank of its feasible columns, or kNoRank and more when it has none) and
+// its infeasible columns are kept in s_key / s_nb[warp][row] — plain stores, no atomics; 12 KB at 512 rows.
+constexpr int kFoldWarps = kEvalThreads / 32;
+constexpr uint32_t kNoRank = 0x8000u;   // added to an infeasible column's rank (< 1024): the key still fits 16 bits
+
+// Row r's lane keys and infeasible counts over the warp's 128 columns: one reduction each, stored in the warp's slot
+// of the row (key_slot / nb_slot: the warp's row 0, shared-window addresses).
+__device__ __forceinline__ void fold_row(uint32_t key, uint32_t nb, uint32_t key_slot, uint32_t nb_slot, uint32_t r) {
+  key = __reduce_min_sync(0xffffffffu, key);
+  nb = __reduce_add_sync(0xffffffffu, nb);
+  // every lane stores the same value to the same address: one store each, without a branch around lane 0
+  asm volatile("st.shared.u16 [%0], %1;" ::"r"(key_slot + 2u * r), "r"(key) : "memory");
+  asm volatile("st.shared.u8 [%0], %1;" ::"r"(nb_slot + r), "r"(nb) : "memory");
+}
+
+// End of the CTA's rows (its first ask t_cta): each row with a feasible column merges best_of_rank[its least rank]
+// into ask_best and its feasible count into ask_count.
+__device__ __forceinline__ void fold_merge_rows(const uint16_t (&s_key)[kFoldWarps][kFastRows],
+                                                const uint8_t (&s_nb)[kFoldWarps][kFastRows], uint32_t nrows,
+                                                uint32_t t_cta, const FoldOut& fo) {
+  __syncthreads();                            // every warp has written its slot of every row
+  const long long* best = fo.best_of_rank + blockIdx.x * kEvalCols;
+  for (uint32_t i = threadIdx.x; i < nrows; i += kEvalThreads) {
+    uint32_t key = kNone, nb = 0;
+#pragma unroll
+    for (int j = 0; j < kFoldWarps; ++j) {
+      key = min(key, (uint32_t)s_key[j][i]);
+      nb += s_nb[j][i];
+    }
+    if (nb < (uint32_t)kEvalCols) {           // a feasible column: key is its least rank
+      atomicMin(fo.ask_best + t_cta + i, __ldg(best + key));
+      atomicAdd(fo.ask_count + t_cta + i, kEvalCols - nb);
+    }
+  }
+}
+
+// Per column cbase + k of the thread, its first feasible ask cm[k] (>= 2^31 while there is none) into first_ask of the
+// column's worker: w0 + the column, or with PERM w0 + perm[column] (pm_build_argmin_feat's column order; perm is loaded
+// only now: held through the row loop it would cost 4 registers there).
+template <bool PERM>
+__device__ __forceinline__ void fold_flush_first_ask(const uint32_t (&cm)[kEvalWPT], uint32_t cbase, uint32_t w0,
+                                                     uint32_t nw, const FoldOut& fo) {
+  uint32_t* first = fo.first_ask + w0;
+  uint32_t wk[kEvalWPT];   // column cbase + k's worker, as an offset from `first`
+  if constexpr (PERM) {
+    const uint4 pw = __ldg(reinterpret_cast<const uint4*>(fo.perm + cbase));
+    wk[0] = pw.x; wk[1] = pw.y; wk[2] = pw.z; wk[3] = pw.w;
+  } else {   // the thread's 4 consecutive columns: constant offsets from first + cbase
+    first += cbase;
+#pragma unroll
+    for (int k = 0; k < kEvalWPT; ++k) wk[k] = k;
+  }
+#pragma unroll
+  for (int k = 0; k < kEvalWPT; ++k)
+    if (cm[k] < 0x80000000u && cbase + k < nw) atomicMin(first + wk[k], cm[k]);
+}
+
+template <int BITS, bool FOLD>
 __device__ __forceinline__ void build_fast(const EvalParams& p, uint32_t t0, uint32_t nt, uint32_t w0, uint32_t nw,
                                            void* __restrict__ tile, size_t ld, const FoldOut& fo) {
-  static_assert(!PIPE || NARROW, "the row fold ranks the 32-bit tile's columns");
   __shared__ FastStage s;
-  // PIPE: per warp and row of the CTA, the warp's least key (the least stripe rank of its feasible columns, or
-  // kNoRank and more when it has none) and its infeasible columns — plain stores, no atomics; 12 KB at 512 rows
-  constexpr int kWarps = kEvalThreads / 32;
-  constexpr uint32_t kNoRank = 0x8000u;   // added to an infeasible column's rank (< 1024): the key still fits 16 bits
-  __shared__ uint16_t s_key[PIPE ? kWarps : 1][PIPE ? kFastRows : 1];
-  __shared__ uint8_t s_nb[PIPE ? kWarps : 1][PIPE ? kFastRows : 1];
+  __shared__ uint16_t s_key[FOLD ? kFoldWarps : 1][FOLD ? kFastRows : 1];
+  __shared__ uint8_t s_nb[FOLD ? kFoldWarps : 1][FOLD ? kFastRows : 1];
   const uint32_t r0 = blockIdx.y * kFastRows;
   const uint32_t nrows = min(nt - r0, (uint32_t)kFastRows);
   if (threadIdx.x == 0) {
@@ -383,35 +453,35 @@ __device__ __forceinline__ void build_fast(const EvalParams& p, uint32_t t0, uin
     for (uint32_t i = threadIdx.x; i < total_words; i += blockDim.x) s.bits[i] = __ldg(p.bits + i);
   }
   const uint32_t lane = threadIdx.x & 31u;
-  const uint32_t cbase = blockIdx.x * kEvalCols + (threadIdx.x >> 5) * 128u + lane * (NARROW ? 4u : 2u);
+  const uint32_t cbase = blockIdx.x * kEvalCols + (threadIdx.x >> 5) * 128u + lane * (FOLD ? 4u : 2u);
   WorkerReg w[kEvalWPT];
   uint32_t gw[kEvalWPT], dx[kEvalWPT], dy[kEvalWPT];
 #pragma unroll
   for (int k = 0; k < kEvalWPT; ++k) {
-    const uint32_t col = NARROW ? cbase + k : cbase + (k >> 1) * 64u + (k & 1);
+    const uint32_t col = FOLD ? cbase + k : cbase + (k >> 1) * 64u + (k & 1);
     gw[k] = w0 + col;
     if (col < nw) {
       w[k] = make_worker(__ldg(p.wa + w0 + col), __ldg(p.wb + w0 + col));
       if (p.nacc) w[k].mmask = __ldg(p.nacc + w0 + col);
     } else w[k] = null_worker();
     dx[k] = 0xFFFFFFFFu - gw[k];          // infeasible: 0x7FFFFFFF_FFFFFFFF = feasible word + (0/1) * difference
-    dy[k] = 0x7FFFFFFFu - w[k].price;     // (the narrow form keeps only this high word)
+    dy[k] = 0x7FFFFFFFu - w[k].price;     // (the 32-bit tile keeps only this high word)
     asm("" : "+r"(dy[k]));                // kept in a register: ptxas would otherwise recompute it from the price every row
   }
-  uint4* out = NARROW ? reinterpret_cast<uint4*>(static_cast<uint32_t*>(tile) + (size_t)r0 * ld + cbase)
-                      : reinterpret_cast<uint4*>(static_cast<long long*>(tile) + (size_t)r0 * ld + cbase);
-  size_t row_stride = NARROW ? ld / 4 : ld / 2;   // in 16-byte units
+  uint4* out = FOLD ? reinterpret_cast<uint4*>(static_cast<uint32_t*>(tile) + (size_t)r0 * ld + cbase)
+                    : reinterpret_cast<uint4*>(static_cast<long long*>(tile) + (size_t)r0 * ld + cbase);
+  size_t row_stride = FOLD ? ld / 4 : ld / 2;   // in 16-byte units
   asm("" : "+l"(row_stride));           // held in registers: ptxas would otherwise re-derive it from `ld` every row
   const uint32_t sh = p.sign_shift;
-  // PIPE: per column, the first feasible ask so far — the least of ask | fail's sign bit (asks are below 2^31): >= 2^31
+  // FOLD: per column, the first feasible ask so far — the least of ask | fail's sign bit (asks are below 2^31): >= 2^31
   // while there is none
   uint32_t cm[kEvalWPT];
 #pragma unroll
   for (int k = 0; k < kEvalWPT; ++k) cm[k] = kNone;
-  const uint32_t t_cta = t0 + r0;       // PIPE: the ask of the CTA's first row
-  uint32_t rk[kEvalWPT];                // PIPE: per column, its rank within the stripe
-  uint32_t key_slot = 0, nb_slot = 0;   // PIPE: the warp's row 0 in s_key / s_nb (shared-window addresses)
-  if constexpr (PIPE) {
+  const uint32_t t_cta = t0 + r0;       // FOLD: the ask of the CTA's first row
+  uint32_t rk[kEvalWPT];                // FOLD: per column, its rank within the stripe
+  uint32_t key_slot = 0, nb_slot = 0;   // FOLD: the warp's row 0 in s_key / s_nb (shared-window addresses)
+  if constexpr (FOLD) {
     const uint4 v = __ldg(reinterpret_cast<const uint4*>(fo.rank + cbase));
     rk[0] = v.x; rk[1] = v.y; rk[2] = v.z; rk[3] = v.w;
     key_slot = (uint32_t)__cvta_generic_to_shared(&s_key[threadIdx.x >> 5][0]);
@@ -437,91 +507,56 @@ __device__ __forceinline__ void build_fast(const EvalParams& p, uint32_t t0, uin
       for (int k = 0; k < kEvalWPT; ++k) f[k] &= um[k] | sc[k];
     }
     uint32_t o[2 * kEvalWPT];
-    uint32_t key = kNone, nb = 0;       // PIPE: the lane's least key and its infeasible columns
+    uint32_t key = kNone, nb = 0;       // FOLD: the lane's least key and its infeasible columns
 #pragma unroll
     for (int k = 0; k < kEvalWPT; ++k) {
       const uint32_t b = f[k] >> sh;                                    // 1 when infeasible (sh == 31)
-      if (NARROW) {
+      if (FOLD) {
         o[k] = b * dy[k] + w[k].price;                                  // feasible: price ; infeasible: kNarrowInfeasible
+        cm[k] = min(cm[k], (t_cta + r) | (f[k] & 0x80000000u));        // the ask, + 2^31 when infeasible
+        key = min(key, b * kNoRank + rk[k]);                            // the rank, + kNoRank when infeasible
+        nb += b;
       } else {
         o[2 * k] = b * dx[k] + gw[k];                                   // feasible: (price << 32) | worker
         o[2 * k + 1] = b * dy[k] + w[k].price;                          // infeasible: 0x7FFFFFFF_FFFFFFFF
       }
-      if (PIPE) {
-        cm[k] = min(cm[k], (t_cta + r) | (f[k] & 0x80000000u));        // the ask, + 2^31 when infeasible
-        key = min(key, b * kNoRank + rk[k]);                            // the rank, + kNoRank when infeasible
-        nb += b;
-      }
     }
-    if (NARROW) {
-      __stcs(dst, make_uint4(o[0], o[1], o[2], o[3]));
-    } else {
-      __stcs(dst, make_uint4(o[0], o[1], o[2], o[3]));
-      __stcs(dst + 32, make_uint4(o[4], o[5], o[6], o[7]));     // + 64 columns
-    }
-    if (PIPE) {   // the warp's 128 columns: one reduction each, kept in the warp's slot of the row
-      key = __reduce_min_sync(0xffffffffu, key);
-      nb = __reduce_add_sync(0xffffffffu, nb);
-      // every lane stores the same value to the same address: one store each, without a branch around lane 0
-      asm volatile("st.shared.u16 [%0], %1;" ::"r"(key_slot + 2u * r), "r"(key) : "memory");
-      asm volatile("st.shared.u8 [%0], %1;" ::"r"(nb_slot + r), "r"(nb) : "memory");
-    }
+    __stcs(dst, make_uint4(o[0], o[1], o[2], o[3]));
+    if (FOLD) fold_row(key, nb, key_slot, nb_slot, r);
+    else __stcs(dst + 32, make_uint4(o[4], o[5], o[6], o[7]));     // + 64 columns
   };
   __syncthreads();            // mbarrier initialised, acceptance words staged
   mbar_wait(&s.bar, 0);
-  // Two rows per iteration share the loop test and the output-pointer bump.  Each row's FastRow is loaded one row
-  // ahead, into registers the previous row has finished with, so no row is copied from one buffer to another.
-  const FastRow* q = s.row;
-  FastRow a = q[0];
-  for (uint32_t r = 0; r < nrows; r += 2, q += 2) {
-    const FastRow b = q[1];                   // in flight while row r is evaluated
-    emit(a, out, r);
-    a = q[2];                                 // in flight while row r + 1 is evaluated
-    if (r + 1 < nrows) emit(b, out + row_stride, r + 1);
-    out += 2 * row_stride;
-  }
-  if constexpr (PIPE) {
-    __syncthreads();                          // every warp has written its slot of every row
-    const long long* best = fo.best_of_rank + blockIdx.x * kEvalCols;
-    for (uint32_t i = threadIdx.x; i < nrows; i += kEvalThreads) {
-      uint32_t key = kNone, nb = 0;
-#pragma unroll
-      for (int j = 0; j < kWarps; ++j) {
-        key = min(key, (uint32_t)s_key[j][i]);
-        nb += s_nb[j][i];
-      }
-      if (nb < (uint32_t)kEvalCols) {         // a feasible column: key is its least rank
-        atomicMin(fo.ask_best + t_cta + i, __ldg(best + key));
-        atomicAdd(fo.ask_count + t_cta + i, kEvalCols - nb);
-      }
-    }
-#pragma unroll
-    for (int k = 0; k < kEvalWPT; ++k)
-      if (cm[k] < 0x80000000u && cbase + k < nw) atomicMin(fo.first_ask + w0 + cbase + k, cm[k]);
+  for_each_row_pair(s.row, nrows, out, row_stride, emit);
+  if constexpr (FOLD) {
+    fold_merge_rows(s_key, s_nb, nrows, t_cta, fo);
+    fold_flush_first_ask<false>(cm, cbase, w0, nw, fo);
   }
 }
 
-template <int BITS, bool NARROW>
+template <int BITS>
 __global__ void __launch_bounds__(kEvalThreads, 2)
-pm_build_cost_fast(EvalParams p, uint32_t t0, uint32_t nt, uint32_t w0, uint32_t nw, void* __restrict__ tile, size_t ld) {
-  build_fast<BITS, NARROW, false>(p, t0, nt, w0, nw, tile, ld, FoldOut{});
+pm_build_cost_fast(EvalParams p, uint32_t t0, uint32_t nt, uint32_t w0, uint32_t nw, long long* __restrict__ tile,
+                   size_t ld) {
+  build_fast<BITS, false>(p, t0, nt, w0, nw, tile, ld, FoldOut{});
 }
 
 // ------------------------------------------------------------------ build + argmin, one kernel
-// pm_build_cost_fast<BITS, true> and pm_argmin<.., true>'s outputs in one pass: the tile is written with
-// streaming stores, as the build writes it, and never read back.  Within a 1024-column stripe the packed minimum
+// The 32-bit tile's build and the int64 pm_argmin's outputs in one pass: the tile is written with streaming stores,
+// as the build writes it, and never read back.  Within a 1024-column stripe the packed minimum
 // (word << 32) | (w0 + column) over the feasible columns orders them by (price, column) whatever the ask, so a
 // column's rank in that order (pm_stripe_rank, once per pass) stands for its packed cost.  Per row and lane the
 // fold is one multiply-add per column on the fail bit the store already formed — key = b * kNoRank + rank — the
 // least of the 4 keys and the sum of the bits; per warp one min and one add reduction, stored in the warp's slot of
 // the row (no atomics, no barrier in the row loop).  At the end of the CTA each row with a feasible column merges
 // best_of_rank[its least rank] into ask_best (atomicMin) and its count into ask_count; per column the first feasible
-// ask, kept from the same sign bit, is flushed once.  The outputs are pm_argmin's bit for bit.
+// ask, kept from the same sign bit, is flushed once.  The outputs are those of pm_build_cost_fast and pm_argmin on
+// the int64 tile, bit for bit.
 template <int BITS>
 __global__ void __launch_bounds__(kEvalThreads, 2)
 pm_build_argmin(EvalParams p, uint32_t t0, uint32_t nt, uint32_t w0, uint32_t nw, uint32_t* __restrict__ tile, size_t ld,
                 FoldOut fo) {
-  build_fast<BITS, true, true>(p, t0, nt, w0, nw, tile, ld, fo);
+  build_fast<BITS, true>(p, t0, nt, w0, nw, tile, ld, fo);
 }
 
 // One CTA per 1024-column stripe of a tile with leading dimension ld, whose column c holds worker w0 + perm[c]
@@ -752,7 +787,7 @@ __global__ void pm_feature_gather(const uint4* __restrict__ wb, const unsigned l
 }
 
 // pm_build_argmin with the feature predicate: the same stores, row fold, first-ask minimum and end-of-CTA merge
-// (build_fast<.., true, true>), the outputs bit for bit, on a tile whose column c holds worker w0 + perm[c] (the
+// (build_fast<.., true>), the outputs bit for bit, on a tile whose column c holds worker w0 + perm[c] (the
 // column order above; the ranks and best_of_rank carry the workers, and first_ask is flushed to them).  Per worker
 // and row: two LOP3 for u = R & ~F over the two words and one min for the fail bit b = min(u, 1).  A worker is one
 // 16-byte load in the prologue; a row is one 16-byte shared-memory load; further OR-options (R_o) are read from global
@@ -760,12 +795,10 @@ __global__ void pm_feature_gather(const uint4* __restrict__ wb, const unsigned l
 __global__ void __launch_bounds__(kEvalThreads, 2)
 pm_build_argmin_feat(const uint4* __restrict__ arow, const uint2* __restrict__ ropt, const uint4* __restrict__ feat,
                      uint32_t t0, uint32_t nt, uint32_t w0, uint32_t nw, uint32_t* __restrict__ tile, size_t ld, FoldOut fo) {
-  constexpr int kWarps = kEvalThreads / 32;
-  constexpr uint32_t kNoRank = 0x8000u;
   __shared__ __align__(128) uint4 s_row[kFastRows + 2];   // + 2: the look-ahead loads past the last pair of rows
   __shared__ uint64_t s_bar;
-  __shared__ uint16_t s_key[kWarps][kFastRows];
-  __shared__ uint8_t s_nb[kWarps][kFastRows];
+  __shared__ uint16_t s_key[kFoldWarps][kFastRows];
+  __shared__ uint8_t s_nb[kFoldWarps][kFastRows];
   const uint32_t r0 = blockIdx.y * kFastRows;
   const uint32_t nrows = min(nt - r0, (uint32_t)kFastRows);
   if (threadIdx.x == 0) {
@@ -815,42 +848,13 @@ pm_build_argmin_feat(const uint4* __restrict__ arow, const uint2* __restrict__ r
       nb += b;
     }
     __stcs(dst, make_uint4(o[0], o[1], o[2], o[3]));
-    key = __reduce_min_sync(0xffffffffu, key);
-    nb = __reduce_add_sync(0xffffffffu, nb);
-    asm volatile("st.shared.u16 [%0], %1;" ::"r"(key_slot + 2u * r), "r"(key) : "memory");
-    asm volatile("st.shared.u8 [%0], %1;" ::"r"(nb_slot + r), "r"(nb) : "memory");
+    fold_row(key, nb, key_slot, nb_slot, r);
   };
   __syncthreads();            // mbarrier initialised
   mbar_wait(&s_bar, 0);
-  const uint4* q = s_row;
-  uint4 a = q[0];
-  for (uint32_t r = 0; r < nrows; r += 2, q += 2) {
-    const uint4 b = q[1];
-    emit(a, out, r);
-    a = q[2];
-    if (r + 1 < nrows) emit(b, out + row_stride, r + 1);
-    out += 2 * row_stride;
-  }
-  __syncthreads();            // every warp has written its slot of every row
-  const long long* best = fo.best_of_rank + blockIdx.x * kEvalCols;
-  for (uint32_t i = threadIdx.x; i < nrows; i += kEvalThreads) {
-    uint32_t key = kNone, nb = 0;
-#pragma unroll
-    for (int j = 0; j < kWarps; ++j) {
-      key = min(key, (uint32_t)s_key[j][i]);
-      nb += s_nb[j][i];
-    }
-    if (nb < (uint32_t)kEvalCols) {
-      atomicMin(fo.ask_best + t_cta + i, __ldg(best + key));
-      atomicAdd(fo.ask_count + t_cta + i, kEvalCols - nb);
-    }
-  }
-  // the columns' workers, loaded only now: held through the row loop they would cost 4 registers there
-  const uint4 pw = __ldg(reinterpret_cast<const uint4*>(fo.perm + cbase));
-  const uint32_t wk[kEvalWPT] = {pw.x, pw.y, pw.z, pw.w};
-#pragma unroll
-  for (int k = 0; k < kEvalWPT; ++k)
-    if (cm[k] < 0x80000000u && cbase + k < nw) atomicMin(fo.first_ask + w0 + wk[k], cm[k]);
+  for_each_row_pair(s_row, nrows, out, row_stride, emit);
+  fold_merge_rows(s_key, s_nb, nrows, t_cta, fo);
+  fold_flush_first_ask<true>(cm, cbase, w0, nw, fo);
 }
 
 // ------------------------------------------------------------------ argmin
@@ -865,18 +869,12 @@ constexpr int kArgRows = 64;                     // rows per CTA
 // flight at S=8, RPW=2), folds them lane-locally, then one shuffle reduction per
 // row.  Per-column "first feasible ask" never leaves the lane's registers; per-row
 // (min, count) partials are merged in shared memory and flushed once per CTA.
-//
-// NARROW: the tile is pm_build_cost_fast<.., true>'s uint32_t words (price, or kNarrowInfeasible).  A 128-bit load then
-// holds 4 columns, so a warp's slice is S*128 columns and a lane keeps the same S*RPW loads in flight.  A lane folds its
-// words into (least word, its first column) — its columns are visited in increasing order, so a strict "<" keeps the
-// first — and forms the packed (word << 32) | (w0 + column) once per row for the shuffle: the int64 the wide tile
-// holds, so ask_best, ask_count and first_ask are bit-identical to the wide form's.
-template <int S, int RPW, bool NARROW = false>
+template <int S, int RPW>
 __global__ void __launch_bounds__(kArgThreads)
-pm_argmin(const void* __restrict__ tile, size_t ld, uint32_t nt, uint32_t t0, uint32_t w0,
+pm_argmin(const long long* __restrict__ tile, size_t ld, uint32_t nt, uint32_t t0, uint32_t w0,
           uint32_t nw, uint32_t* __restrict__ first_ask, long long* __restrict__ ask_best,
           uint32_t* __restrict__ ask_count) {
-  constexpr int kWarpCols = S * (NARROW ? 128 : 64);
+  constexpr int kWarpCols = S * 64;
   __shared__ long long s_best[kArgRows];   // signed, as the packed cost: a price >= 2^31 makes it negative
   __shared__ uint32_t s_cnt[kArgRows];
   const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
@@ -889,8 +887,7 @@ pm_argmin(const void* __restrict__ tile, size_t ld, uint32_t nt, uint32_t t0, ui
   }
   __syncthreads();
 
-  constexpr int CPL = NARROW ? 4 : 2;                  // columns per 128-bit load
-  using Vec = std::conditional_t<NARROW, uint4, longlong2>;
+  constexpr int CPL = 2;                               // columns per 128-bit load
   uint32_t cm[S][CPL];
 #pragma unroll
   for (int s = 0; s < S; ++s)
@@ -899,16 +896,15 @@ pm_argmin(const void* __restrict__ tile, size_t ld, uint32_t nt, uint32_t t0, ui
 
   if (c0 < ld) {
     for (uint32_t rr = 0; rr < rows; rr += RPW) {
-      Vec v[RPW][S];
+      longlong2 v[RPW][S];
 #pragma unroll
       for (int q = 0; q < RPW; ++q) {
         const uint32_t r = r0 + rr + q;
-        const Vec* rowp = static_cast<const Vec*>(tile) + (size_t)r * (ld / CPL);
+        const longlong2* rowp = reinterpret_cast<const longlong2*>(tile) + (size_t)r * (ld / CPL);
 #pragma unroll
         for (int s = 0; s < S; ++s) {
           const uint32_t col = c0 + s * 32 * CPL + lane * CPL;
           if (rr + q < rows && col < ld) v[q][s] = __ldcs(rowp + col / CPL);
-          else if constexpr (NARROW) v[q][s] = make_uint4(kNarrowInfeasible, kNarrowInfeasible, kNarrowInfeasible, kNarrowInfeasible);
           else v[q][s] = make_longlong2(kInf, kInf);
         }
       }
@@ -917,29 +913,13 @@ pm_argmin(const void* __restrict__ tile, size_t ld, uint32_t nt, uint32_t t0, ui
         const uint32_t t = t0 + r0 + rr + q;
         long long best = kInf;
         uint32_t cnt = 0;
-        if constexpr (NARROW) {
-          uint32_t bw = kNarrowInfeasible, bc = 0;   // least word of the lane and its column offset
 #pragma unroll
-          for (int s = 0; s < S; ++s) {
-            const uint32_t x[4] = {v[q][s].x, v[q][s].y, v[q][s].z, v[q][s].w};
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const bool f = x[j] != kNarrowInfeasible;
-              cnt += (uint32_t)f;
-              cm[s][j] = f ? min(cm[s][j], t) : cm[s][j];
-              if (x[j] < bw) { bw = x[j]; bc = s * 128 + j; }
-            }
-          }
-          if (bw != kNarrowInfeasible) best = (long long)(((unsigned long long)bw << 32) | (w0 + c0 + lane * 4 + bc));
-        } else {
-#pragma unroll
-          for (int s = 0; s < S; ++s) {
-            best = min(best, min(v[q][s].x, v[q][s].y));
-            const bool fx = v[q][s].x != kInf, fy = v[q][s].y != kInf;
-            cnt += (uint32_t)fx + (uint32_t)fy;
-            cm[s][0] = fx ? min(cm[s][0], t) : cm[s][0];
-            cm[s][1] = fy ? min(cm[s][1], t) : cm[s][1];
-          }
+        for (int s = 0; s < S; ++s) {
+          best = min(best, min(v[q][s].x, v[q][s].y));
+          const bool fx = v[q][s].x != kInf, fy = v[q][s].y != kInf;
+          cnt += (uint32_t)fx + (uint32_t)fy;
+          cm[s][0] = fx ? min(cm[s][0], t) : cm[s][0];
+          cm[s][1] = fy ? min(cm[s][1], t) : cm[s][1];
         }
 #pragma unroll
         for (int off = 16; off > 0; off >>= 1) {

@@ -102,9 +102,9 @@ DOMAIN_EDGE = (2, (1 << 61) - (1 << 32) - (1 << 21), 1024)
 EDGE_PRICES = [0x7FFFFFFF, 0x80000000, 0xFFFFFFFE, 0xFFFFFFFF]
 NARROW_LIMIT = 0x7FFFFFFF        # the 32-bit cost tile holds prices below it
 SIGN = 1 << 31
-SETTINGS = {"default": {}, "generic": {"PM_TUNE_GENERIC": 1}, "unpiped": {"PM_TUNE_PIPE": 0},
+SETTINGS = {"default": {}, "generic": {"PM_TUNE_GENERIC": 1}, "int64": {"PM_TUNE_BUILD": 8},
             "incr40": {"PM_TUNE_INCR": 40}, "auction128": {"PM_TUNE_AUCTION": 128}}
-TILE_BYTES = {"unpiped": 1 << 20}     # several cost tiles
+TILE_BYTES = {"int64": 1 << 20}       # several cost tiles
 DEFAULT_CUTOFF = 1 << 18              # PM_TUNE_INCR's default
 SHAPES = ("mixed", "wide")
 BIG = os.environ.get("PM_TEST_BIG") == "1"

@@ -75,10 +75,10 @@ def test_workload_on_one_gpu(wl, path):
     eng.close()
 
 
-@pytest.mark.parametrize("env", [{"PM_TUNE_PIPE": "0"}, {"PM_TUNE_BUILD": "8"}, {"PM_TUNE_GENERIC": "1"},
-                                 {"PM_TUNE_COMPRESS": "0"}], ids=["pipe0", "build8_int64_tile", "generic", "compress0"])
+@pytest.mark.parametrize("env", [{"PM_TUNE_BUILD": "8"}, {"PM_TUNE_GENERIC": "1"}, {"PM_TUNE_COMPRESS": "0"}],
+                         ids=["build8_int64_tile", "generic", "compress0"])
 def test_cfg3_kernel_settings(env, monkeypatch):
-    """The other build / argmin forms at the headline shape: separate build and argmin, the int64 tile, the generic
+    """The other build / argmin forms at the headline shape: the int64 tile (separate build and argmin), the generic
     predicate, the uncompressed tile (the knobs are read when the engine is created)."""
     for k, v in env.items():
         monkeypatch.setenv(k, v)

@@ -1,6 +1,7 @@
 """pm_build_argmin_feat's sorted column order on hardware: column c of the tile holds worker w0 + perm[c], the workers
 of the range sorted by __brevll(F), and pm_stripe_rank ranks each stripe by (price, worker).  ask_best, ask_count and
-first_ask must be those of PM_TUNE_PIPE=0 (which builds in worker order) and of the CPU oracle, bit for bit.
+first_ask must be those of the int64 tile (PM_TUNE_BUILD=8, which builds in worker order) and of the CPU oracle, bit
+for bit.
 
 The cases aim at what a column/worker mix-up would get wrong: equal least prices on workers whose columns come in the
 opposite order (the least worker wins, not the least column), ties across stripes, ragged stripes and tiles, shards

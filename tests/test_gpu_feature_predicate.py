@@ -1,5 +1,5 @@
 """pm_build_argmin_feat, the materialised pass's build + argmin on the feature predicate, on hardware: against the
-separate build and argmin launches (PM_TUNE_PIPE=0, the fast predicate unchanged) and the CPU oracle, every result
+int64 tile (PM_TUNE_BUILD=8: separate build and argmin launches on the fast predicate) and the CPU oracle, every result
 array whole.  Tables at exactly 64 features run it and at 65 run the FastRow pm_build_argmin; ask deltas move a
 resident engine across that budget both ways; the kernel that ran is read from the kernel names torch.profiler
 records."""
@@ -14,9 +14,9 @@ from oracle import pm_oracle as orc
 from protocol_b200 import abi
 from protocol_b200.engine import Engine
 from protocol_b200.sharded import shard_range, wrap_device_buffers
-from test_gpu_narrow_tile import MAT, RESULT_FIELDS
+from test_gpu_narrow_tile import MAT, RESULT_FIELDS, assert_same, make_engine
 from test_gpu_tile_overlap import tile_bytes
-from test_gpu_tile_pipeline import assert_oracle, assert_same, pipe_env, table_dict
+from test_gpu_tile_pipeline import assert_oracle, table_dict
 from test_gpu_variants import wide_tables
 
 pytestmark = pytest.mark.gpu
@@ -134,7 +134,7 @@ def test_asks_with_hundreds_of_options():
 
 
 def history_step(engines, t, enabled=None):
-    """One pass on each engine (default, PIPE=0): every array equal, and to the oracle when every ask is enabled;
+    """One pass on each engine (default, int64 tile): every array equal, and to the oracle when every ask is enabled;
     returns the build kernels the default engine ran."""
     W, T = len(t["wa"]), len(t["asks"])
     ran = profiled_match(engines[0])
@@ -159,10 +159,7 @@ def test_deltas_across_the_budget_and_model_table_changes():
     big = ft.with_features(base, 65)
     fit = ft.with_features(base, 64)
     added = big["asks"][len(base["asks"]):]
-    engines = []
-    for pipe in (None, 0):
-        with pipe_env(pipe):
-            engines.append(Engine(cost_tile_bytes=1 << 20))
+    engines = [make_engine(wide, cost_tile_bytes=1 << 20) for wide in (False, True)]
     try:
         for e in engines:
             load_engine(e, fit)

@@ -22,6 +22,7 @@ RESULT_FIELDS = ("worker_group", "worker_ask", "group_ask", "group_off", "group_
 
 
 def make_engine(wide, **kw):
+    """wide: the int64 tile on the FastRow path (PM_TUNE_BUILD=8), the 32-bit tile's reference"""
     if wide:
         os.environ["PM_TUNE_BUILD"] = "8"   # read at pm_create
     try:
@@ -40,30 +41,37 @@ def tables(n_asks, n_workers, seed_shift, price="loguniform"):
 def one_pass(t, wide, cost_tile_bytes=0, shard=None):
     """(first_ask, ask_best, ask_count, stats, result or None) of one materialised pass."""
     W, T = len(t["wa"]), len(t["asks"])
-    e = make_engine(wide, cost_tile_bytes=cost_tile_bytes)
-    load_engine(e, t)
-    if shard is not None:
-        e.set_shard(*shard)
-    e.match_local(MAT)
-    e.sync()
-    fa, best, cnt = (x.cpu().numpy().copy() for x in wrap_device_buffers(e, W, T))
-    st = e.stats()
-    res = None
-    if shard is None:
-        e.match_finish(MAT)
-        res = e.fetch()
-    e.close()
+    e = make_engine(wide, cost_tile_bytes=cost_tile_bytes, timing=True)
+    try:
+        load_engine(e, t)
+        if shard is not None:
+            e.set_shard(*shard)
+        e.match_local(MAT)
+        e.sync()
+        fa, best, cnt = (x.cpu().numpy().copy() for x in wrap_device_buffers(e, W, T))
+        res = None
+        if shard is None:
+            e.match_finish(MAT)   # also resolves the kernel timers
+            res = e.fetch()
+        st = e.stats()
+    finally:
+        e.close()
     return fa.view(np.uint32), best, cnt.view(np.uint32), st, res
 
 
 def assert_same(t, cost_tile_bytes=0, shard=None):
+    """The 32-bit tile's pass against the int64 tile's; returns the 32-bit tile's."""
     T = len(t["asks"])
     nw = shard[1] if shard is not None else len(t["wa"])
     n = one_pass(t, False, cost_tile_bytes, shard)
     w = one_pass(t, True, cost_tile_bytes, shard)
     assert n[3]["cost_bytes_written"] == n[3]["cost_bytes_read"] == 4 * T * nw, "the narrow tile did not run"
     assert w[3]["cost_bytes_written"] == w[3]["cost_bytes_read"] == 8 * T * nw, "the int64 tile did not run"
-    assert n[3]["n_tiles"] == w[3]["n_tiles"] and n[3]["n_build_launches"] == w[3]["n_build_launches"]
+    for st in (n[3], w[3]):
+        assert shard is not None or (st["ms_build"] > 0 and st["ms_argmin"] > 0)
+    for k in ("n_tiles", "n_build_launches", "n_argmin_launches"):
+        assert n[3][k] == w[3][k], k
+    assert n[3]["n_argmin_launches"] == n[3]["n_build_launches"] == n[3]["n_tiles"]
     assert np.array_equal(n[0], w[0]), "first_ask differs"
     assert np.array_equal(n[1], w[1]), "ask_best differs"
     assert np.array_equal(n[2], w[2]), "ask_count differs"

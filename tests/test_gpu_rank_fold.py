@@ -1,5 +1,5 @@
 """pm_build_argmin's register fold on hardware: the per-stripe price rank (pm_stripe_rank) and the per-row fold of
-(least rank, feasible count), against the separate build and argmin launches (PM_TUNE_PIPE=0) and the CPU oracle.
+(least rank, feasible count), against the int64 tile (PM_TUNE_BUILD=8) and the CPU oracle.
 
 The rank table is computed from the prices at every pass.  The cases aim at what a stale or misread table would get
 wrong: prices changed by pm_update_workers between two passes with no host synchronisation in between, the worker
@@ -10,22 +10,21 @@ import pytest
 
 from helpers import load_engine
 from protocol_b200 import abi
-from protocol_b200.engine import Engine, _ptr
+from protocol_b200.engine import _ptr
 from protocol_b200.sharded import wrap_device_buffers
-from test_gpu_narrow_tile import MAT, oracle_eval, tables
+from test_gpu_narrow_tile import MAT, assert_same, make_engine, oracle_eval, tables
 from test_gpu_tile_overlap import tile_bytes
-from test_gpu_tile_pipeline import assert_oracle, assert_same, pipe_env
+from test_gpu_tile_pipeline import assert_oracle
 
 pytestmark = pytest.mark.gpu
 
 
-def passes_across_an_update(t, idx, a, b, pipe, resize=None):
+def passes_across_an_update(t, idx, a, b, wide, resize=None):
     """Pass 1, pm_update_workers (and pm_resize_workers first when `resize`) and pass 2, enqueued with no host
     synchronisation between them; returns pass 2's (first_ask, ask_best, ask_count, stats)."""
     W = resize if resize is not None else len(t["wa"])
     T = len(t["asks"])
-    with pipe_env(pipe):
-        e = Engine(cost_tile_bytes=tile_bytes(W, 256))
+    e = make_engine(wide, cost_tile_bytes=tile_bytes(W, 256))
     try:
         load_engine(e, t)
         e.match_local(MAT)
@@ -43,11 +42,12 @@ def passes_across_an_update(t, idx, a, b, pipe, resize=None):
 
 
 def check_update(t, t2, idx, a, b, resize=None):
-    ref = passes_across_an_update(t, idx, a, b, 0, resize)
-    got = passes_across_an_update(t, idx, a, b, None, resize)
+    ref = passes_across_an_update(t, idx, a, b, True, resize)
+    got = passes_across_an_update(t, idx, a, b, False, resize)
     for x, y in zip(got[:3], ref[:3]):
         assert np.array_equal(x, y)
     assert got[3]["cost_bytes_written"] == got[3]["cost_bytes_read"] == 4 * len(t2["asks"]) * len(t2["wa"])
+    assert ref[3]["cost_bytes_written"] == ref[3]["cost_bytes_read"] == 8 * len(t2["asks"]) * len(t2["wa"])
     ev = assert_oracle(t2, got)
     assert (ev["row_count"] > 0).any()
 

@@ -1,84 +1,25 @@
 """The one-launch build + argmin of the 32-bit cost tile (pm_build_argmin, the default wherever that tile runs) on
-hardware, against the separate build and argmin launches (PM_TUNE_PIPE=0) and the CPU oracle.
+hardware, against the int64 tile's separate build and argmin launches (PM_TUNE_BUILD=8) and the CPU oracle.
 
-pm_build_argmin reads each band of rows back right after writing it.  The cases aim at the band edges (ask counts
-one either side of the band and of the CTA's 512 rows), the padding columns past the last worker, short last tiles
-that leave stale rows of the previous tile in the buffer, the shard offset, every acceptance-table form, asks with
-more OR-options than the stage holds, row minima that tie across CTAs, the largest price the tile holds, and two
-passes around a table update with no host synchronisation between them.  Every pm_result array, the per-worker first
-feasible ask and the per-ask (best, count) must be equal; both tiles count 4 B per evaluation read and written."""
-import contextlib
-import os
-
+pm_build_argmin folds each row in registers as it writes it, two rows per loop iteration, 512 rows per CTA.  The cases
+aim at the row edges (ask counts around the row pairs and the CTA's 512 rows), the padding columns past the last
+worker, short last tiles that leave stale rows of the previous tile in the buffer, the shard offset, every
+acceptance-table form, asks with more OR-options than the stage holds, row minima that tie across CTAs, the largest
+price the tile holds, and two passes around a table update with no host synchronisation between them.  Every pm_result
+array, the per-worker first feasible ask and the per-ask (best, count) must be equal (test_gpu_narrow_tile.assert_same)."""
 import numpy as np
 import pytest
 
 from helpers import groups_equal, load_engine
 from oracle import pm_oracle as orc
 from protocol_b200 import abi
-from protocol_b200.engine import Engine, _ptr
-from protocol_b200.sharded import shard_range, wrap_device_buffers
-from test_gpu_narrow_tile import MAT, RESULT_FIELDS, oracle_eval, tables
+from protocol_b200.engine import _ptr
+from protocol_b200.sharded import shard_range
+from test_gpu_narrow_tile import MAT, RESULT_FIELDS, assert_same, make_engine, oracle_eval, tables
 from test_gpu_tile_overlap import changed_rows, tile_bytes
 from test_gpu_variants import many_option_tables, wide_tables
 
 pytestmark = pytest.mark.gpu
-
-BANDS = [8, 16, 32, 64]
-
-
-@contextlib.contextmanager
-def pipe_env(pipe):
-    """pipe: rows per band, 0 for the two launches, None for the engine's default"""
-    if pipe is not None:
-        os.environ["PM_TUNE_PIPE"] = str(pipe)   # read at pm_create
-    try:
-        yield
-    finally:
-        os.environ.pop("PM_TUNE_PIPE", None)
-
-
-def one_pass(t, pipe, cost_tile_bytes=0, shard=None):
-    """(first_ask, ask_best, ask_count, stats, result or None) of one materialised pass."""
-    W, T = len(t["wa"]), len(t["asks"])
-    with pipe_env(pipe):
-        e = Engine(cost_tile_bytes=cost_tile_bytes, timing=True)
-    try:
-        load_engine(e, t)
-        if shard is not None:
-            e.set_shard(*shard)
-        e.match_local(MAT)
-        e.sync()
-        fa, best, cnt = (x.cpu().numpy().copy() for x in wrap_device_buffers(e, W, T))
-        res = None
-        if shard is None:
-            e.match_finish(MAT)   # also resolves the kernel timers
-            res = e.fetch()
-        st = e.stats()
-    finally:
-        e.close()
-    return fa.view(np.uint32), best, cnt.view(np.uint32), st, res
-
-
-def assert_same(t, cost_tile_bytes=0, shard=None, pipes=(None,)):
-    """Each of `pipes` against PM_TUNE_PIPE=0; returns the last one's pass."""
-    T = len(t["asks"])
-    nw = shard[1] if shard is not None else len(t["wa"])
-    ref = one_pass(t, 0, cost_tile_bytes, shard)
-    for pipe in pipes:
-        got = one_pass(t, pipe, cost_tile_bytes, shard)
-        for st in (got[3], ref[3]):
-            assert st["cost_bytes_written"] == st["cost_bytes_read"] == 4 * T * nw, "the 32-bit tile did not run"
-            assert shard is not None or (st["ms_build"] > 0 and st["ms_argmin"] > 0)
-        assert got[3]["n_tiles"] == ref[3]["n_tiles"] and got[3]["n_build_launches"] == ref[3]["n_build_launches"]
-        assert got[3]["n_argmin_launches"] == got[3]["n_build_launches"] == got[3]["n_tiles"]
-        assert np.array_equal(got[0], ref[0]), f"first_ask differs (band {pipe})"
-        assert np.array_equal(got[1], ref[1]), f"ask_best differs (band {pipe})"
-        assert np.array_equal(got[2], ref[2]), f"ask_count differs (band {pipe})"
-        if shard is None:
-            for f in RESULT_FIELDS:
-                assert np.array_equal(getattr(got[4], f), getattr(ref[4], f)), f"{f} differs (band {pipe})"
-    return got
 
 
 def assert_oracle(t, got, w0=0, w1=None):
@@ -95,15 +36,14 @@ def table_dict(w, a, pbits, npat, nmod, words):
     return dict(asks=a.asks, opts=a.opts, wa=w.a, wb=w.b, bits=pbits, n_patterns=npat, n_models=nmod, words=words)
 
 
-@pytest.mark.parametrize("band", BANDS)
-def test_ask_counts_around_the_band_and_the_cta(band):
-    """T in {1, R - 1, R, R + 1, 511, 512, 513, 1025}: the last band and the last CTA's rows are short.  Tiles of
-    1024 rows or more are cut to whole 512-row bands, so 1025 asks take a second tile of one row."""
+def test_ask_counts_around_the_band_and_the_cta():
+    """T around 8, 16, 32 and 64 rows, and 511, 512, 513, 1025: odd and even row counts, and a short last CTA.  Tiles
+    of 1024 rows or more are cut to whole 512-row bands, so 1025 asks take a second tile of one row."""
     W = 4099
-    base = tables(1025, W, seed_shift=band)
-    for T in sorted({1, band - 1, band, band + 1, 511, 512, 513, 1025}):
+    base = tables(1025, W, seed_shift=8)
+    for T in sorted({1, 511, 512, 513, 1025} | {r + d for r in (8, 16, 32, 64) for d in (-1, 0, 1)}):
         t = dict(base, asks=base["asks"][:T])
-        got = assert_same(t, pipes=(band,))
+        got = assert_same(t)
         assert got[3]["n_tiles"] == (2 if T == 1025 else 1)
         assert_oracle(t, got)
         assert groups_equal(got[4], orc.soa_form_groups(t["wa"], t["wb"], t["asks"], t["opts"], t["bits"], t["words"]))
@@ -113,7 +53,7 @@ def test_ask_counts_around_the_band_and_the_cta(band):
 def test_worker_counts_around_the_cta_stripe(W):
     """Padding columns past the last worker hold the infeasible word and count nowhere."""
     t = tables(1025, W, seed_shift=7 + W)
-    got = assert_same(t, pipes=(8, 64))
+    got = assert_same(t)
     assert_oracle(t, got)
 
 
@@ -121,7 +61,7 @@ def test_worker_counts_around_the_cta_stripe(W):
 def test_short_last_tile_over_stale_rows(T, W, rows, n_tiles):
     """The last tile is short: the rows past it in the buffer still hold the previous tile's words."""
     t = tables(T, W, seed_shift=T + 3 * W)
-    got = assert_same(t, tile_bytes(W, rows), pipes=BANDS)
+    got = assert_same(t, tile_bytes(W, rows))
     assert got[3]["n_tiles"] == n_tiles
     assert_oracle(t, got)
 
@@ -133,7 +73,7 @@ def test_sharded_offsets(n_shards):
     W = len(t["wa"])
     for r in range(1, n_shards):
         lo, hi = shard_range(W, n_shards, r)
-        got = assert_same(t, tile_bytes(hi - lo, 256), shard=(lo, hi - lo), pipes=(8, 16))
+        got = assert_same(t, tile_bytes(hi - lo, 256), shard=(lo, hi - lo))
         assert got[3]["n_tiles"] == 3
         assert_oracle(t, got, lo, hi)
 
@@ -146,7 +86,7 @@ def test_acceptance_forms(n_models, n_patterns):
                                                         seed_shift=60 + n_patterns, last_rows=True)
     rng = np.random.default_rng(n_patterns)
     w.b["ext_ask_price"] = rng.integers(0, 3000, len(w.b)).astype(np.uint32)
-    got = assert_same(table_dict(w, a, pbits, npat, nmod, words), 1 << 20, pipes=(16, 64))
+    got = assert_same(table_dict(w, a, pbits, npat, nmod, words), 1 << 20)
     ev = orc.soa_eval_matrix(w.a, w.b, a.asks, a.opts, obits, words, 0, len(a.asks), 0, len(w.a), threads=8)
     assert np.array_equal(got[1], ev["row_best"]) and np.array_equal(got[2], ev["row_count"])
     assert np.array_equal(got[0], np.asarray(ev["col_first"]).astype(np.uint32))
@@ -156,7 +96,7 @@ def test_acceptance_forms(n_models, n_patterns):
 def test_asks_with_hundreds_of_options(n_models):
     """Asks with 384 to 1200 OR-options: their further options are read from global memory in the build phase."""
     w, a, obits, pbits, npat, nmod, words = many_option_tables(n_models)
-    got = assert_same(table_dict(w, a, pbits, npat, nmod, words), 1 << 20, pipes=(8, 32))
+    got = assert_same(table_dict(w, a, pbits, npat, nmod, words), 1 << 20)
     ev = orc.soa_eval_matrix(w.a, w.b, a.asks, a.opts, obits, words, 0, len(a.asks), 0, len(w.a), threads=8)
     assert np.array_equal(got[1], ev["row_best"]) and np.array_equal(got[2], ev["row_count"])
     assert np.array_equal(got[0], np.asarray(ev["col_first"]).astype(np.uint32))
@@ -166,7 +106,7 @@ def test_all_infeasible():
     t = tables(600, 5000, seed_shift=17)
     t["wa"] = t["wa"].copy()
     t["wa"]["flags"] &= ~np.uint32(abi.PM_W_HEALTHY)   # nobody is a candidate
-    got = assert_same(t, 1 << 20, pipes=(8, 64))
+    got = assert_same(t, 1 << 20)
     assert (got[2] == 0).all() and (got[0] == 0xFFFFFFFF).all()
     assert_oracle(t, got)
 
@@ -182,7 +122,7 @@ def test_all_feasible():
     asks["opt_off"] = 0
     asks["min_group_size"] = asks["max_group_size"] = 1
     t["asks"] = asks
-    got = assert_same(t, 1 << 20, pipes=(8, 64))
+    got = assert_same(t, 1 << 20)
     assert (got[2] == 5000).all() and (got[0] == 0).all()
     assert_oracle(t, got)
 
@@ -196,7 +136,7 @@ def test_price_ties_across_stripes(prices):
     t["wb"] = t["wb"].copy()
     t["wb"]["ext_ask_price"] = {"constant": np.full(W, 4242), "mod3": np.arange(W) % 3 + 5,
                                 "top": np.full(W, 0x7FFFFFFE)}[prices].astype(np.uint32)
-    got = assert_same(t, tile_bytes(W, 256), pipes=(16, 32))
+    got = assert_same(t, tile_bytes(W, 256))
     ev = assert_oracle(t, got)
     assert (ev["row_count"] > 1).any()
 
@@ -209,9 +149,8 @@ def test_back_to_back_passes_across_a_table_update():
     t2 = dict(t, wa=t["wa"].copy(), wb=t["wb"].copy())
     t2["wa"][idx], t2["wb"][idx] = a, b
     out = []
-    for pipe in (0, 8, None):
-        with pipe_env(pipe):
-            e = Engine(cost_tile_bytes=tile_bytes(W, 256))
+    for wide in (True, False):   # the int64 tile, then the default 32-bit one
+        e = make_engine(wide, cost_tile_bytes=tile_bytes(W, 256))
         try:
             load_engine(e, t)
             e.match_local(MAT)

@@ -1,12 +1,12 @@
-"""The 32-bit cost tile of the materialised first-fit pass (pm_kernels.cuh pm_build_cost_fast<.., NARROW> and
-pm_argmin<.., NARROW>), restated in numpy and held against the int64 tile it replaces.
+"""The 32-bit cost tile of the materialised first-fit pass (pm_kernels.cuh build_fast<.., FOLD>, which pm_build_argmin
+runs), restated in numpy and held against the int64 tile it replaces.
 
 The int64 element is (price << 32) | (w0 + column) when the worker meets the ask and 0x7FFFFFFF_FFFFFFFF when not.
 The narrow element keeps only the high word — price, or 0x7FFFFFFF — formed as b * (0x7FFFFFFF - price) + price with
-b = 1 for an infeasible pair; the reader adds the column back.  A lane of the argmin holds 4 consecutive columns per
-128-bit load and S such loads per row, keeps (least word, its first column) with a strict "<", and the packed int64 is
-formed once per lane and row.  This checks that folding the word tile that way gives the int64 fold's ask_best,
-ask_count and first_ask, and that only prices below 0x7FFFFFFF may take the narrow tile."""
+b = 1 for an infeasible pair; the reader adds the column back.  Read back a lane at a time — 4 consecutive columns per
+128-bit load and S such loads per row, (least word, its first column) kept with a strict "<", the packed int64 formed
+once per lane and row — the word tile gives the int64 fold's ask_best, ask_count and first_ask: the narrow element
+loses nothing.  Only prices below 0x7FFFFFFF may take the narrow tile."""
 import numpy as np
 import pytest
 
@@ -14,7 +14,7 @@ U32, I64 = np.uint32, np.int64
 SENTINEL = 0x7FFFFFFF
 K_INF = 0x7FFFFFFFFFFFFFFF
 NONE = 0xFFFFFFFF
-S, LANES, CPL = 8, 32, 4          # pm_argmin<8, 2, true>: a warp slice is S * 128 columns
+S, LANES, CPL = 8, 32, 4          # the lane read-back: a warp slice is S * 128 columns
 CTA_COLS = 1024                   # the build kernel's stripe: ld is a multiple of it
 
 

@@ -70,11 +70,6 @@ if __name__ == "__main__":
     print({"hbm_peak_GBs": PEAK, "source": PEAK_SOURCE}, flush=True)
     if os.environ.get("TUNE_CEIL"):
         hbm_ceilings()
-    variants = [{}, {"PM_TUNE_BUILD": "8"}]   # 8: the int64 tile on the FastRow path
-    # 0: the separate build and argmin launches, against the one-launch build + argmin of the default run above
-    for v in os.environ.get("TUNE_PIPE", "0").split(","):
-        if v:
-            variants.append({"PM_TUNE_PIPE": v})
-    for env in variants:
+    for env in ({}, {"PM_TUNE_BUILD": "8"}):   # 8: the int64 tile on the FastRow path
         run(env)
     run({}, mode=abi.PM_MODE_FIRST_FIT | abi.PM_PATH_FUSED)
