@@ -648,7 +648,9 @@ int pm_build_cost_tile(pm_engine*, uint32_t t0, uint32_t nt, int64_t* host_out);
 enum pm_buffer {
   PM_BUF_WORKER_FIRST_ASK = 0,  /* uint32[n_workers] global; only the shard range is written */
   PM_BUF_ASK_BEST         = 1,  /* int64 [n_asks] packed row argmin (allreduce MIN)          */
-  PM_BUF_ASK_COUNT        = 2   /* uint32[n_asks] (allreduce SUM)                            */
+  PM_BUF_ASK_COUNT        = 2,  /* uint32[n_asks] (allreduce SUM)                            */
+  PM_BUF_COST_TILE        = 3   /* the cost tile the last materialised pass left, read-only:  */
+                                /* bytes = what its tiles spanned (rows per tile x ld x 4 or 8) */
 };
 /* Re-target the engine at the range [first, first+count) of the worker table (count 0 = to the end). */
 int pm_set_shard(pm_engine*, uint32_t first, uint32_t count);

@@ -53,7 +53,7 @@ PM_AUCTION_WARM = 1 << 11  # PM_MODE_AUCTION: start from the last auction pass's
 PM_AUCTION_REVERSE = 1 << 12  # PM_MODE_AUCTION: end every eps phase with reverse rounds (prime_match.h)
 PM_AUCTION_REPAIR = 1 << 13  # with PM_AUCTION_WARM: keep the stored prices, raise the changed rows, end with reverse rounds
 
-PM_BUF_WORKER_FIRST_ASK, PM_BUF_ASK_BEST, PM_BUF_ASK_COUNT = 0, 1, 2
+PM_BUF_WORKER_FIRST_ASK, PM_BUF_ASK_BEST, PM_BUF_ASK_COUNT, PM_BUF_COST_TILE = 0, 1, 2, 3
 
 WORKER_A = np.dtype([("gpu_count", "<u4"), ("gpu_mem_mb", "<u4"), ("model_id", "<u4"), ("flags", "<u4")])
 WORKER_B = np.dtype([("cpu_cores", "<u4"), ("ram_mb", "<u4"), ("storage_gb", "<u4"), ("ext_ask_price", "<u4")])

@@ -103,11 +103,30 @@ template <class T> struct PinBuf {
 // HBM in compressed form and reads them back the same way, so the HBM traffic of a sparse tile shrinks while its layout,
 // contents and the kernels stay what they are.  Elsewhere (or when the driver refuses), plain cudaMalloc.  The driver's
 // virtual-memory calls are looked up at run time: the library keeps no link-time dependency on libcuda.
+//
+// `held` describes the buffer, whatever wrote it: one byte per 4 KB of it (a row slot's 1024-column stripe of the 32-bit
+// tile), bit j set when its 512-byte block j — one warp's 128 columns — holds kNarrowInfeasible in every word.  Indexed
+// by offset, it stays true across changes of ld or of the rows per tile (ld is a multiple of 1024 columns, so every
+// layout's blocks are the same 512-byte blocks).  pm_build_argmin_feat reads and writes it, and skips the stores of a
+// block that is all infeasible and already holds the sentinel.  Any other writer of the buffer calls overwritten();
+// the next pm_build_argmin_feat pass then zeroes the map (prepare_held) and writes every block once more.
 struct TileBuf {
   long long* p = nullptr;
   size_t n = 0;
   CUmemGenericAllocationHandle h = 0;   // non-zero: compressible mapping of `bytes` bytes at p
   size_t bytes = 0;
+  uint8_t* held = nullptr;              // [held_bytes()]
+  bool held_valid = false;              // false: the map is stale, every block must be written
+
+  size_t held_bytes() const { return (n * sizeof(long long) + 4095) / 4096; }
+  void overwritten() { held_valid = false; }
+  // the map, zeroed in stream order when it is stale: no host synchronisation
+  cudaError_t prepare_held(cudaStream_t st) {
+    if (held_valid) return cudaSuccess;
+    const cudaError_t e = cudaMemsetAsync(held, 0, held_bytes(), st);
+    held_valid = e == cudaSuccess;
+    return e;
+  }
 
   struct Api {
     decltype(&cuMemGetAllocationGranularity) granularity = nullptr;
@@ -195,16 +214,21 @@ struct TileBuf {
     }
     release();
     if (want == 0) want = 1;
-    if (compress && map_compressible(device, want * sizeof(long long))) {
-      n = want;
-      return cudaSuccess;
+    cudaError_t e = cudaSuccess;
+    if (!(compress && map_compressible(device, want * sizeof(long long)))) e = cudaMalloc(&p, want * sizeof(long long));
+    if (e != cudaSuccess) {
+      p = nullptr;
+      return e;
     }
-    cudaError_t e = cudaMalloc(&p, want * sizeof(long long));
-    if (e == cudaSuccess) n = want;
-    else p = nullptr;
+    n = want;
+    e = cudaMalloc(&held, held_bytes());
+    if (e != cudaSuccess) release();
     return e;
   }
   void release() {
+    if (held) cudaFree(held);
+    held = nullptr;
+    held_valid = false;
     if (h) {
       const Api& a = api();
       a.unmap(reinterpret_cast<CUdeviceptr>(p), bytes);
@@ -325,6 +349,7 @@ struct pm_engine {
 
   // evaluation
   TileBuf cost;
+  size_t cost_tile_used = 0;           // bytes of `cost` the last materialised pass laid its tiles over (PM_BUF_COST_TILE)
   DevBuf<uint32_t> first_ask, ask_count;
   DevBuf<long long> ask_best;
   DevBuf<uint32_t> stripe_rank;        // pm_stripe_rank, once per pass of pm_build_argmin: [ld] column -> rank in its stripe
@@ -1850,6 +1875,7 @@ static bool narrow_tile(const pm_engine* e, bool fast) {
 // The int64 tile's build
 static void launch_build(pm_engine* e, const pm::EvalParams& p, int bits_mode, bool fast, dim3 grid,
                          uint32_t t0, uint32_t nt, uint32_t w0, uint32_t nw, long long* tile, size_t ld) {
+  e->cost.overwritten();   // tile is e->cost.p
 #define PM_BUILD_CASE(B) pm::pm_build_cost<B><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, t0, nt, w0, nw, tile, ld)
 #define PM_FAST_CASE(B)                                                                                                 \
   {                                                                                                                     \
@@ -1882,23 +1908,22 @@ static void launch_fused(pm_engine* e, const pm::EvalParams& p, int bits_mode, b
 #undef PM_FUSED_CASE
 }
 
-// pm_build_argmin: the 32-bit tile's build and argmin in one launch (the stripe ranks of pm_stripe_rank in place)
+// pm_build_argmin: the 32-bit tile's build and argmin in one launch (the stripe ranks of pm_stripe_rank in place).
+// tile is e->cost.p; the feature kernel needs its sentinel map prepared (TileBuf::prepare_held).
 static void launch_build_argmin(pm_engine* e, const pm::EvalParams& p, int bits_mode, uint32_t t0, uint32_t nt, uint32_t w0,
                                 uint32_t nw, long long* tile, size_t ld) {
   const dim3 grid(blocks_for(ld, pm::kEvalCols), blocks_for(nt, pm::kFastRows));
   const pm::FoldOut fo{e->stripe_rank.p, e->rank_best.p, e->first_ask.p, e->ask_best.p, e->ask_count.p, e->feat_perm.p};
   uint32_t* t32 = reinterpret_cast<uint32_t*>(tile);
   if (e->feat_ok) {   // the feature rows of this pass (match_local)
-    // Unused dynamic shared memory that holds the kernel at two CTAs per SM (228 KB each on H100).  At 64 registers
-    // and 20 KB of its own it would run four, and the step is then 10 % slower than at two, also with the columns
-    // sorted so that most of the tile compresses (cfg3 on an H100 SXM at 700 W: 118.1 ms against 107.5 ms; three
-    // CTAs: 117.9 ms) — more row streams written at once lose DRAM efficiency.
-    constexpr int kFeatPad = 70000;
-    cudaFuncSetAttribute(pm::pm_build_argmin_feat, cudaFuncAttributeMaxDynamicSharedMemorySize, kFeatPad);
-    pm::pm_build_argmin_feat<<<grid, pm::kEvalThreads, kFeatPad, e->stream>>>(e->feat_a.p, e->feat_o.p, e->feat_w.p, t0, nt, w0, nw,
-                                                                      t32, ld, fo);
+    // Four CTAs per SM (64 registers, 24 KB of shared memory each).  With every store written, two were fastest: more
+    // row streams lost DRAM efficiency.  With most stores skipped (TileBuf::held), four are: cfg3 on an H100 SXM at
+    // 700 W, the kernel 52.9 ms per pass at four CTAs, 54.0 at three, 59.4-59.7 at two.
+    pm::pm_build_argmin_feat<<<grid, pm::kEvalThreads, 0, e->stream>>>(e->feat_a.p, e->feat_o.p, e->feat_w.p, t0, nt, w0, nw,
+                                                                      t32, ld, e->cost.held, fo);
     return;
   }
+  e->cost.overwritten();
   if (p.words == 1) bits_mode = 2;   // one-word acceptance rows are bound into the FastRows, as in launch_build
   if (bits_mode == 2) pm::pm_build_argmin<2><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, t0, nt, w0, nw, t32, ld, fo);
   else if (bits_mode == 1) pm::pm_build_argmin<1><<<grid, pm::kEvalThreads, 0, e->stream>>>(p, t0, nt, w0, nw, t32, ld, fo);
@@ -2165,6 +2190,8 @@ static int match_local_locked(pm_engine* e, uint32_t mode) {
           PM_LAUNCH_CHECK("pm_feature_gather");
         }
       }
+      if (narrow && e->feat_ok) PM_CUDA(e->cost.prepare_held(e->stream));
+      e->cost_tile_used = (size_t)rows * ld * elem_bytes;
       long long* tile = e->cost.p;
       for (uint32_t t0 = 0; t0 < T; t0 += (uint32_t)rows) {
         const uint32_t nt = (uint32_t)std::min<uint64_t>(rows, T - t0);
@@ -3662,6 +3689,7 @@ int pm_device_buffer(pm_engine* e, uint32_t which, void** dev_ptr, size_t* bytes
     case PM_BUF_WORKER_FIRST_ASK: *dev_ptr = e->first_ask.p; *bytes = (size_t)e->n_workers * 4; break;
     case PM_BUF_ASK_BEST: *dev_ptr = e->ask_best.p; *bytes = (size_t)e->n_asks * 8; break;
     case PM_BUF_ASK_COUNT: *dev_ptr = e->ask_count.p; *bytes = (size_t)e->n_asks * 4; break;
+    case PM_BUF_COST_TILE: *dev_ptr = e->cost.p; *bytes = e->cost_tile_used; break;
     default: return e->fail(PM_E_INVALID, "pm_device_buffer: unknown buffer");
   }
   if (!*dev_ptr) return e->fail(PM_E_STATE, "pm_device_buffer: buffer not allocated yet (run pm_match_local)");

@@ -384,29 +384,34 @@ constexpr int kFoldWarps = kEvalThreads / 32;
 constexpr uint32_t kNoRank = 0x8000u;   // added to an infeasible column's rank (< 1024): the key still fits 16 bits
 
 // Row r's lane keys and infeasible counts over the warp's 128 columns: one reduction each, stored in the warp's slot
-// of the row (key_slot / nb_slot: the warp's row 0, shared-window addresses).
-__device__ __forceinline__ void fold_row(uint32_t key, uint32_t nb, uint32_t key_slot, uint32_t nb_slot, uint32_t r) {
+// of the row (key_slot / nb_slot: the warp's row 0, shared-window addresses).  Returns the warp's infeasible count.
+__device__ __forceinline__ uint32_t fold_row(uint32_t key, uint32_t nb, uint32_t key_slot, uint32_t nb_slot, uint32_t r) {
   key = __reduce_min_sync(0xffffffffu, key);
   nb = __reduce_add_sync(0xffffffffu, nb);
   // every lane stores the same value to the same address: one store each, without a branch around lane 0
   asm volatile("st.shared.u16 [%0], %1;" ::"r"(key_slot + 2u * r), "r"(key) : "memory");
   asm volatile("st.shared.u8 [%0], %1;" ::"r"(nb_slot + r), "r"(nb) : "memory");
+  return nb;
 }
 
 // End of the CTA's rows (its first ask t_cta): each row with a feasible column merges best_of_rank[its least rank]
-// into ask_best and its feasible count into ask_count.
+// into ask_best and its feasible count into ask_count.  row_done(i, m) sees every row i < nrows with m's bit j set
+// when warp j's 128 columns of the row are all infeasible.
+template <class RowDone>
 __device__ __forceinline__ void fold_merge_rows(const uint16_t (&s_key)[kFoldWarps][kFastRows],
                                                 const uint8_t (&s_nb)[kFoldWarps][kFastRows], uint32_t nrows,
-                                                uint32_t t_cta, const FoldOut& fo) {
+                                                uint32_t t_cta, const FoldOut& fo, RowDone&& row_done) {
   __syncthreads();                            // every warp has written its slot of every row
   const long long* best = fo.best_of_rank + blockIdx.x * kEvalCols;
   for (uint32_t i = threadIdx.x; i < nrows; i += kEvalThreads) {
-    uint32_t key = kNone, nb = 0;
+    uint32_t key = kNone, nb = 0, m = 0;
 #pragma unroll
     for (int j = 0; j < kFoldWarps; ++j) {
       key = min(key, (uint32_t)s_key[j][i]);
       nb += s_nb[j][i];
+      m |= (uint32_t)(s_nb[j][i] == 128u) << j;
     }
+    row_done(i, m);
     if (nb < (uint32_t)kEvalCols) {           // a feasible column: key is its least rank
       atomicMin(fo.ask_best + t_cta + i, __ldg(best + key));
       atomicAdd(fo.ask_count + t_cta + i, kEvalCols - nb);
@@ -529,7 +534,7 @@ __device__ __forceinline__ void build_fast(const EvalParams& p, uint32_t t0, uin
   mbar_wait(&s.bar, 0);
   for_each_row_pair(s.row, nrows, out, row_stride, emit);
   if constexpr (FOLD) {
-    fold_merge_rows(s_key, s_nb, nrows, t_cta, fo);
+    fold_merge_rows(s_key, s_nb, nrows, t_cta, fo, [](uint32_t, uint32_t) {});
     fold_flush_first_ask<false>(cm, cbase, w0, nw, fo);
   }
 }
@@ -792,19 +797,37 @@ __global__ void pm_feature_gather(const uint4* __restrict__ wb, const unsigned l
 // and row: two LOP3 for u = R & ~F over the two words and one min for the fail bit b = min(u, 1).  A worker is one
 // 16-byte load in the prologue; a row is one 16-byte shared-memory load; further OR-options (R_o) are read from global
 // memory, warp-uniform.
-__global__ void __launch_bounds__(kEvalThreads, 2)
+//
+// `held` (TileBuf::held) has one byte per row slot and 1024-column stripe of the tile, at slot * (ld / 1024) + stripe:
+// bit j set when warp j's 512-byte block of it holds kNarrowInfeasible in every word.  Most blocks are all infeasible
+// row after row (the column order), so a warp stores its block only when some word changes: when the row has a
+// feasible column there or the block's bit is clear.  The tile stays what the stores would have made it.  The CTA reads
+// its rows' bytes in the prologue and writes them back after the merge; each byte belongs to one CTA of a launch, and
+// launches are stream-ordered.
+__global__ void __launch_bounds__(kEvalThreads, 4)
 pm_build_argmin_feat(const uint4* __restrict__ arow, const uint2* __restrict__ ropt, const uint4* __restrict__ feat,
-                     uint32_t t0, uint32_t nt, uint32_t w0, uint32_t nw, uint32_t* __restrict__ tile, size_t ld, FoldOut fo) {
+                     uint32_t t0, uint32_t nt, uint32_t w0, uint32_t nw, uint32_t* __restrict__ tile, size_t ld,
+                     uint8_t* __restrict__ held, FoldOut fo) {
   __shared__ __align__(128) uint4 s_row[kFastRows + 2];   // + 2: the look-ahead loads past the last pair of rows
   __shared__ uint64_t s_bar;
   __shared__ uint16_t s_key[kFoldWarps][kFastRows];
-  __shared__ uint8_t s_nb[kFoldWarps][kFastRows];
+  // [0]: fold_row's infeasible counts.  [1]: per warp and row, the count at which its block needs no store: 128 when
+  // the block holds the sentinel, else 0xFF (never); one byte past the count's, at nb_slot + kHeldOff + r
+  __shared__ uint8_t s_nb[2][kFoldWarps][kFastRows];
+  constexpr uint32_t kHeldOff = kFoldWarps * kFastRows;
   const uint32_t r0 = blockIdx.y * kFastRows;
   const uint32_t nrows = min(nt - r0, (uint32_t)kFastRows);
   if (threadIdx.x == 0) {
     mbar_init(&s_bar, 1);
     mbar_expect_tx(&s_bar, nrows * 16u);
     bulk_g2s(s_row, arow + t0 + r0, nrows * 16u, &s_bar);
+  }
+  const size_t held_stride = ld / kEvalCols;
+  uint8_t* held_cta = held + (size_t)r0 * held_stride + blockIdx.x;
+  for (uint32_t i = threadIdx.x; i < nrows; i += kEvalThreads) {
+    const uint32_t m = held_cta[i * held_stride];
+#pragma unroll
+    for (int j = 0; j < kFoldWarps; ++j) s_nb[1][j][i] = (m >> j) & 1u ? 128u : 0xFFu;
   }
   const uint32_t lane = threadIdx.x & 31u;
   const uint32_t cbase = blockIdx.x * kEvalCols + (threadIdx.x >> 5) * 128u + lane * 4u;
@@ -822,13 +845,15 @@ pm_build_argmin_feat(const uint4* __restrict__ arow, const uint2* __restrict__ r
   asm("" : "+l"(row_stride));
   const uint32_t t_cta = t0 + r0;
   uint32_t key_slot = (uint32_t)__cvta_generic_to_shared(&s_key[threadIdx.x >> 5][0]);
-  uint32_t nb_slot = (uint32_t)__cvta_generic_to_shared(&s_nb[threadIdx.x >> 5][0]);
+  uint32_t nb_slot = (uint32_t)__cvta_generic_to_shared(&s_nb[0][threadIdx.x >> 5][0]);
   asm("" : "+r"(key_slot), "+r"(nb_slot));
   // 1 behind an opaque move: with the literal, ptxas proves b = min(u, 1) is 0 or 1 and turns the multiply-adds below
   // into compares and selects on the busier ALU pipe (EvalParams::sign_shift does the same for the FastRow kernel)
   uint32_t one = 1u;
   asm("" : "+r"(one));
   auto emit = [&](const uint4& q, uint4* dst, uint32_t r) {
+    uint32_t skip_at;
+    asm volatile("ld.shared.u8 %0, [%1];" : "=r"(skip_at) : "r"(nb_slot + kHeldOff + r));
     uint32_t u[kEvalWPT];
 #pragma unroll
     for (int k = 0; k < kEvalWPT; ++k) u[k] = (q.x & ~fl[k]) | (q.y & ~fh[k]);
@@ -847,13 +872,12 @@ pm_build_argmin_feat(const uint4* __restrict__ arow, const uint2* __restrict__ r
       key = min(key, b * kNoRank + rk[k]);                    // the rank, + kNoRank when infeasible
       nb += b;
     }
-    __stcs(dst, make_uint4(o[0], o[1], o[2], o[3]));
-    fold_row(key, nb, key_slot, nb_slot, r);
+    if (fold_row(key, nb, key_slot, nb_slot, r) != skip_at) __stcs(dst, make_uint4(o[0], o[1], o[2], o[3]));
   };
-  __syncthreads();            // mbarrier initialised
+  __syncthreads();            // mbarrier initialised, s_nb[1] written
   mbar_wait(&s_bar, 0);
   for_each_row_pair(s_row, nrows, out, row_stride, emit);
-  fold_merge_rows(s_key, s_nb, nrows, t_cta, fo);
+  fold_merge_rows(s_key, s_nb[0], nrows, t_cta, fo, [&](uint32_t i, uint32_t m) { held_cta[i * held_stride] = (uint8_t)m; });
   fold_flush_first_ask<true>(cm, cbase, w0, nw, fo);
 }
 
