@@ -383,14 +383,20 @@ __device__ __forceinline__ void for_each_row_pair(const Row* q, uint32_t nrows, 
 constexpr int kFoldWarps = kEvalThreads / 32;
 constexpr uint32_t kNoRank = 0x8000u;   // added to an infeasible column's rank (< 1024): the key still fits 16 bits
 
+// The warp's key and infeasible count of row r, stored in its slot of the row (key_slot / nb_slot: the warp's row 0,
+// shared-window addresses).  Every lane stores the same value to the same address: one store each, without a branch
+// around lane 0.
+__device__ __forceinline__ void fold_slot(uint32_t key, uint32_t nb, uint32_t key_slot, uint32_t nb_slot, uint32_t r) {
+  asm volatile("st.shared.u16 [%0], %1;" ::"r"(key_slot + 2u * r), "r"(key) : "memory");
+  asm volatile("st.shared.u8 [%0], %1;" ::"r"(nb_slot + r), "r"(nb) : "memory");
+}
+
 // Row r's lane keys and infeasible counts over the warp's 128 columns: one reduction each, stored in the warp's slot
-// of the row (key_slot / nb_slot: the warp's row 0, shared-window addresses).  Returns the warp's infeasible count.
+// of the row.  Returns the warp's infeasible count.
 __device__ __forceinline__ uint32_t fold_row(uint32_t key, uint32_t nb, uint32_t key_slot, uint32_t nb_slot, uint32_t r) {
   key = __reduce_min_sync(0xffffffffu, key);
   nb = __reduce_add_sync(0xffffffffu, nb);
-  // every lane stores the same value to the same address: one store each, without a branch around lane 0
-  asm volatile("st.shared.u16 [%0], %1;" ::"r"(key_slot + 2u * r), "r"(key) : "memory");
-  asm volatile("st.shared.u8 [%0], %1;" ::"r"(nb_slot + r), "r"(nb) : "memory");
+  fold_slot(key, nb, key_slot, nb_slot, r);
   return nb;
 }
 
@@ -793,10 +799,11 @@ __global__ void pm_feature_gather(const uint4* __restrict__ wb, const unsigned l
 
 // pm_build_argmin with the feature predicate: the same stores, row fold, first-ask minimum and end-of-CTA merge
 // (build_fast<.., true>), the outputs bit for bit, on a tile whose column c holds worker w0 + perm[c] (the
-// column order above; the ranks and best_of_rank carry the workers, and first_ask is flushed to them).  Per worker
-// and row: two LOP3 for u = R & ~F over the two words and one min for the fail bit b = min(u, 1).  A worker is one
-// 16-byte load in the prologue; a row is one 16-byte shared-memory load; further OR-options (R_o) are read from global
-// memory, warp-uniform.
+// column order above; the ranks and best_of_rank carry the workers, and first_ask is flushed to them).  A warp first
+// decides its 128 columns of a row as a whole (dead or full, from the OR and AND of their F); only a mixed block is
+// evaluated per worker: two LOP3 for u = R & ~F over the two words and one min for the fail bit b = min(u, 1).
+// A worker is one 16-byte load in the prologue; a row is one 16-byte shared-memory load; further OR-options (R_o) are
+// read from global memory, warp-uniform.
 //
 // `held` (TileBuf::held) has one byte per row slot and 1024-column stripe of the tile, at slot * (ld / 1024) + stripe:
 // bit j set when warp j's 512-byte block of it holds kNarrowInfeasible in every word.  Most blocks are all infeasible
@@ -804,7 +811,7 @@ __global__ void pm_feature_gather(const uint4* __restrict__ wb, const unsigned l
 // feasible column there or the block's bit is clear.  The tile stays what the stores would have made it.  The CTA reads
 // its rows' bytes in the prologue and writes them back after the merge; each byte belongs to one CTA of a launch, and
 // launches are stream-ordered.
-__global__ void __launch_bounds__(kEvalThreads, 4)
+__global__ void __launch_bounds__(kEvalThreads, 3)
 pm_build_argmin_feat(const uint4* __restrict__ arow, const uint2* __restrict__ ropt, const uint4* __restrict__ feat,
                      uint32_t t0, uint32_t nt, uint32_t w0, uint32_t nw, uint32_t* __restrict__ tile, size_t ld,
                      uint8_t* __restrict__ held, FoldOut fo) {
@@ -840,6 +847,15 @@ pm_build_argmin_feat(const uint4* __restrict__ arow, const uint2* __restrict__ r
     asm("" : "+r"(dy[k]));   // kept in a register: ptxas would otherwise recompute it from the price every row
     cm[k] = kNone;
   }
+  // The warp's block of a row, classified as a whole: Fo / Fa = the OR / AND of its 128 words F, kmin its least rank.
+  // Column c fails option o when R_o & ~F_c != 0, and Fa ⊆ F_c ⊆ Fo: so if R_o & ~Fo != 0 for every option, every
+  // column fails the row (dead), and if R_o & ~Fa == 0 for some option, every column meets it (full).  Padding columns
+  // (F = 0) make Fa = 0, and every row requires the candidate bit, so a padded block is never full.
+  const uint32_t fo_lo = __reduce_or_sync(0xffffffffu, fl[0] | fl[1] | fl[2] | fl[3]);
+  const uint32_t fo_hi = __reduce_or_sync(0xffffffffu, fh[0] | fh[1] | fh[2] | fh[3]);
+  const uint32_t fa_lo = __reduce_and_sync(0xffffffffu, fl[0] & fl[1] & fl[2] & fl[3]);
+  const uint32_t fa_hi = __reduce_and_sync(0xffffffffu, fh[0] & fh[1] & fh[2] & fh[3]);
+  const uint32_t kmin = __reduce_min_sync(0xffffffffu, min(min(rk[0], rk[1]), min(rk[2], rk[3])));
   uint4* out = reinterpret_cast<uint4*>(tile + (size_t)r0 * ld + cbase);
   size_t row_stride = ld / 4;
   asm("" : "+l"(row_stride));
@@ -854,6 +870,27 @@ pm_build_argmin_feat(const uint4* __restrict__ arow, const uint2* __restrict__ r
   auto emit = [&](const uint4& q, uint4* dst, uint32_t r) {
     uint32_t skip_at;
     asm volatile("ld.shared.u8 %0, [%1];" : "=r"(skip_at) : "r"(nb_slot + kHeldOff + r));
+    // the least over the options, as for a column: dead != 0 when every option misses a feature of Fo, full == 0 when
+    // some option needs only features of Fa
+    uint32_t dead = (q.x & ~fo_lo) | (q.y & ~fo_hi), full = (q.x & ~fa_lo) | (q.y & ~fa_hi);
+    for (uint32_t o = 1; o < q.z; ++o) {
+      const uint2 R = __ldg(ropt + q.w + o);
+      dead = min(dead, (R.x & ~fo_lo) | (R.y & ~fo_hi));
+      full = min(full, (R.x & ~fa_lo) | (R.y & ~fa_hi));
+    }
+    if (__all_sync(0xffffffffu, dead != 0u)) {   // every word the sentinel, no feasible column: as fold_row would leave it
+      fold_slot(kNoRank, 128u, key_slot, nb_slot, r);
+      constexpr uint32_t S = kNarrowInfeasible;
+      if (skip_at != 128u) __stcs(dst, make_uint4(S, S, S, S));
+      return;
+    }
+    if (__all_sync(0xffffffffu, full == 0u)) {   // every word the column's price, every column feasible
+      fold_slot(kmin, 0u, key_slot, nb_slot, r);
+      __stcs(dst, make_uint4(price[0], price[1], price[2], price[3]));
+#pragma unroll
+      for (int k = 0; k < kEvalWPT; ++k) cm[k] = min(cm[k], t_cta + r);
+      return;
+    }
     uint32_t u[kEvalWPT];
 #pragma unroll
     for (int k = 0; k < kEvalWPT; ++k) u[k] = (q.x & ~fl[k]) | (q.y & ~fh[k]);
