@@ -11,7 +11,10 @@ restated from the header and DESIGN §4-§6b:
       dirty; a shrink drops the dirty rows it cuts off; asks enabled / disabled since count against the stored mask
       (off and on again counts as neither); a replaced ask is in E when enabled now and in D when enabled at the stored
       evaluation; appended asks were not enabled at it; an ask shrink cuts the mask and sets every stored first ask past
-      the new end to NONE (those workers are no orphans).  The next incremental pass walks the dirty rows and the
+      the new end to NONE (those workers are no orphans).  pm_remove_asks / pm_insert_asks move every stored first ask
+      with its row; a removed one lands on the next kept row, its heir, which is in D with the replaced bit whatever
+      its own state (NONE with no kept row after it, as a shrink); inserted asks are appended ones.  The next
+      incremental pass walks the dirty rows and the
       orphans of D, or everything when there is no stored evaluation or the dirty rows plus ceil(|E| W / T) pass the
       PM_TUNE_INCR cutoff.  pm_set_asks, pm_set_model_table, pm_set_worker_count and a reference-mode pass that fails
       discard it; a call refused on its mode bits and every auction-mode pass, refused or not, leave it as it is.
@@ -24,7 +27,8 @@ restated from the header and DESIGN §4-§6b:
       that repeats row t d[t] times; the stored assignment, A0 and the warm and repair checkers are over slots.
       pm_set_asks resets every demand to 1, pm_update_asks keeps a replaced row's demand (all its slots join A0), an
       append adds asks of demand 1 (empty slots in A0), a shrink drops the removed asks' demands and counts the held
-      workers of their slots below n_kept in removed_held.  A demand change under a stored state keeps each ask's first
+      workers of their slots below n_kept in removed_held; pm_remove_asks does the same for the removed asks and moves
+      the kept asks' slots with them, pm_insert_asks adds asks of demand 1 like an append.  A demand change under a stored state keeps each ask's first
       min(old, new) slots; over several changes before one pass the slots kept are the minimum over the chain
       (`dem_kept`); a removed slot's worker is unowned at its stored price and counts in removed_held when it lies below
       n_kept; the other slots are in A0.  The warm decision counts |R0| + (W - n_kept) + |A0 in slots| + removed_held.
@@ -76,18 +80,20 @@ AUCTION = ("auction", "reverse", "warm", "repair")
 PASSES = REFERENCE + AUCTION + ("certificate",)
 CALLS = ("update", "set_flags", "upsert", "grow", "shrink", "reputation", "caps", "floors", "ask_off", "ask_on",
          "locations", "addr_rank", "set_asks", "model_table", "auction_params", "set_workers", "update_asks",
-         "append_asks", "shrink_asks", "ask_delta_refused", "demand", "demand_refused", "restore", "restore_refused",
-         "move")
+         "append_asks", "shrink_asks", "remove_asks", "insert_asks", "ask_delta_refused", "demand", "demand_refused",
+         "restore", "restore_refused", "move")
 RARE = ("set_asks", "model_table", "auction_params", "set_workers", "ask_delta_refused", "demand_refused",
         "restore_refused", "move")
-ASK_DELTAS = ("update_asks", "append_asks", "shrink_asks")
+ASK_DELTAS = ("update_asks", "append_asks", "shrink_asks", "remove_asks", "insert_asks")
 # auction-only calls: no pm_multi_ form, and nothing a reference pass reads
 AUCTION_CALLS = ("demand", "demand_refused", "restore", "restore_refused", "move")
 REFUSALS = ("auction_disabled", "auction_domain", "auction_incremental", "proximity_max0", "certificate_no_state",
             "certificate_resized", "certificate_disabled", "certificate_asks_resized", "pattern_missing",
             "ask_delta_refused", "demand_refused", "restore_refused")
-# the PM_E_INVALID cases of pm_update_asks / pm_resize_asks (each changes nothing, pm_table_version included)
+# the PM_E_INVALID cases of pm_update_asks / pm_resize_asks / pm_remove_asks / pm_insert_asks (each changes nothing,
+# pm_table_version and n_asks included)
 DELTA_REFUSALS = ("index", "sizes", "range", "grow_without_rows", "grow_bad_range", "too_many")
+SPLICE_REFUSALS = ("remove_index", "remove_null", "insert_decreasing", "insert_past_end", "insert_sizes", "insert_range")
 # the PM_E_INVALID cases of pm_set_ask_demand (each changes nothing, pm_table_version included)
 DEMAND_REFUSALS = ("length", "zero", "total", "null")
 # refused exports and restores: (case, statuses of the restore); "demand", "no_state" also try the export
@@ -188,15 +194,21 @@ def missing_pattern(asks, opts, n_patterns):
     return np.array([bool(miss[list(r)].any()) if len(r) else False for r in option_rows(asks)], dtype=bool)
 
 
-def split_toggles(mask, eval_mask, replaced):
+def split_toggles(mask, eval_mask, replaced, heirs=()):
     """E and D of the next incremental pass: E = enabled now and (replaced or not enabled at the stored evaluation),
-    D = enabled at the stored evaluation and (replaced or disabled now); a replaced ask's orphans are walked from the
-    ask itself."""
+    D = enabled at the stored evaluation and (replaced or disabled now), and every heir (the next kept row of a removed
+    ask, which holds its workers now) whatever its own state; the orphans of a replaced ask or a heir are walked from
+    the ask itself."""
     rep = np.zeros(len(mask), dtype=bool)
     rep[sorted(replaced)] = True
     en = mask & (rep | ~eval_mask)
     dis = eval_mask & (rep | ~mask)
-    return set(np.flatnonzero(en).tolist()), set(np.flatnonzero(dis).tolist())
+    return set(np.flatnonzero(en).tolist()), set(np.flatnonzero(dis).tolist()) | set(heirs)
+
+
+def renamed(s, new):
+    """A set of ask indices through an index map (new[t] < 0: removed)."""
+    return {int(new[t]) for t in s if new[t] >= 0}
 
 
 def walked_rows(stored, dirty, dis):
@@ -261,11 +273,16 @@ def setup(shape):
     edge[4] = (abi.PM_A_HAS_REQ | abi.PM_A_REQ_RAM, 0, 0, 0, 0xFFFFFFFF, 0, 1, 1)
     edge[5] = (abi.PM_A_HAS_REQ, 1, len(opts) - 2, 0, 0, 0, 1, 1)
     edge[6] = (abi.PM_A_HAS_REQ, 1, len(opts) - 1, 0, 0, 0, 1, 1)
+    # a row inside the fast predicate's domain with a core-count threshold neither table has: one feature more (the
+    # wide tables hold exactly 64, the feature kernel's budget)
+    feature = asks[z:z + 1].copy()
+    feature["flags"] |= abi.PM_A_HAS_REQ | abi.PM_A_REQ_CPU | abi.PM_A_REQ_CPU_CORES
+    feature["cpu_cores"], feature["min_group_size"], feature["max_group_size"] = 3, 1, 2
     return dict(T=T, W=W, z=z, asks=[asks, asks2], opts=opts, bits=[np.asarray(bits, dtype=np.uint32), bits2],
                 npat=npat, nmod=nmod, words=words, wa=w.a.copy(), wb=wb, lat=lat, lon=lon,
                 rank=rng.permutation(W).astype(np.uint32), cap=rng.integers(50, 1500, T).astype(np.uint32),
                 rep=rng.integers(0, 4, W).astype(np.uint32), floors=rng.integers(0, 3, T).astype(np.uint32),
-                pool=np.concatenate([asks, asks2]), edge=edge)
+                pool=np.concatenate([asks, asks2]), edge=edge, feature=feature)
 
 
 # ------------------------------------------------------------------------------------------------ the mirror
@@ -284,8 +301,9 @@ class History(AskMarket):
         self.dirty, self.over = set(), False
         self.eval_mask, self.eval_ff = self.mask.copy(), None
         self.replaced = set()               # asks replaced since the stored evaluation
-        self.appended = set()               # asks appended since it
-        self.dropped = 0                    # stored first asks an ask shrink set to NONE since it
+        self.appended = set()               # asks appended or inserted since it
+        self.heirs = set()                  # kept rows that took a removed ask's stored first asks since it
+        self.dropped = 0                   # stored first asks an ask shrink set to NONE since it
         self.eval_facts = None              # (workers_small, prices_narrow, asks_small) at the stored evaluation
         self.flipped = set()                # which of the facts changed since the stored evaluation
         # auction tracker (A0 is AskMarket's `toggled`, over asks; changed_slots() spreads it over slots)
@@ -331,7 +349,7 @@ class History(AskMarket):
 
     def discard_eval(self):
         self.eval, self.dirty, self.over = False, set(), False
-        self.replaced, self.appended, self.dropped = set(), set(), 0
+        self.replaced, self.appended, self.heirs, self.dropped = set(), set(), set(), 0
         self.eval_facts, self.flipped = None, set()
 
     def discard_auction(self):
@@ -472,7 +490,7 @@ class History(AskMarket):
         W, T = self.n_workers, len(self.asks)
         if not self.eval or self.cutoff == 0 or T == 0 or W == 0:
             return True, W, set(), set(), True
-        en, dis = split_toggles(self.mask, self.eval_mask, self.replaced)
+        en, dis = self.split()
         full_now = len(self.dirty) + self.e_rows(en) > self.cutoff
         full = self.over or full_now
         sure = self.over == (len(self.dirty) > self.cutoff)   # a shrink since the count passed the cutoff: unspecified
@@ -523,12 +541,100 @@ class History(AskMarket):
         self.mask, self.eval_mask = self.mask[:n].copy(), self.eval_mask[:n].copy()
         self.replaced = {t for t in self.replaced if t < n}
         self.appended = {t for t in self.appended if t < n}
+        self.heirs = {t for t in self.heirs if t < n}
         if self.eval_ff is not None:   # a worker whose stored first ask was removed had no feasible ask before it
             cut = (self.eval_ff != NONE) & (self.eval_ff >= n)
             self.dropped += int(cut.sum()) if self.eval else 0
             self.eval_ff = np.where(cut, NONE, self.eval_ff).astype(np.uint32)
         self.resized |= self.auc_state
         self._note_facts()
+
+    def split(self):
+        """(E, D) of the next incremental pass."""
+        return split_toggles(self.mask, self.eval_mask, self.replaced, self.heirs)
+
+    def _new_heirs(self, rm, keep):
+        """The kept rows that take the stored first asks of removed rows: the next kept row after a row enabled at the
+        stored evaluation or itself a heir (no kept row after it: none)."""
+        succ = np.searchsorted(keep, rm)
+        return {int(s) for t, s in zip(rm, succ) if s < len(keep) and (self.eval_mask[t] or int(t) in self.heirs)}
+
+    def _removed_freed(self, gone):
+        """The workers of a removed ask's slots that count against the cutoff."""
+        return self._freed(gone)
+
+    def _per_ask(self, f):
+        """Apply f to every per-ask column (asks, caps, floors, demands, masks)."""
+        self.asks, self.cap, self.cap0, self.floors0 = f(self.asks), f(self.cap), f(self.cap0), f(self.floors0)
+        if self.floors is not None:
+            self.floors = f(self.floors)
+        self.d, self.d_pass = f(self.d), f(self.d_pass)
+        if self.dem_kept is not None:
+            self.dem_kept = f(self.dem_kept)
+        self.mask, self.eval_mask = f(self.mask), f(self.eval_mask)
+
+    def remove_asks(self, idx):
+        """pm_remove_asks: the rows after the removed ones move up.  Each stored first ask moves with its row; a removed
+        one lands on the next kept row, its heir (D with the replaced bit), or is NONE with no kept row after it.  Kept
+        asks keep their slots; a removed ask's held slots below n_kept count in removed_held."""
+        T = len(self.asks)
+        rm = np.unique(np.asarray(idx, dtype=np.int64))
+        keep = np.setdiff1d(np.arange(T), rm)
+        new = np.full(T, -1, np.int64)
+        new[keep] = np.arange(len(keep))
+        heirs = self._new_heirs(rm, keep) if self.eval else set()
+        self.replaced, self.appended = renamed(self.replaced, new), renamed(self.appended, new)
+        self.heirs = renamed(self.heirs, new) | heirs
+        if self.eval_ff is not None:
+            f = self.eval_ff.astype(np.int64)
+            g = f - np.searchsorted(rm, f, side="left")
+            cut = (f != NONE) & (g >= len(keep))
+            self.dropped += int(cut.sum()) if self.eval else 0
+            self.eval_ff = np.where((f == NONE) | cut, NONE, g).astype(np.uint32)
+        if self.assigned is not None:
+            off = ad.offsets(self.d)
+            gone = np.zeros(int(off[-1]), dtype=bool)
+            for t in rm:
+                gone[off[t]:off[t + 1]] = True
+            self.removed_held += self._removed_freed(self.assigned[gone])
+            self.assigned = self.assigned[~gone].copy()
+        self._per_ask(lambda v: v[keep].copy())
+        self.toggled = renamed(self.toggled, new)
+        self.resized |= self.auc_state
+        self._note_facts()
+
+    def insert_asks(self, before, rows):
+        """pm_insert_asks: rows[i] goes before the current row before[i].  Stored first asks move with their rows; the
+        inserted rows are in E (appended), with demand 1, cap 0, floor 0 and one empty slot in A0."""
+        T, k = len(self.asks), len(before)
+        before = np.asarray(before, dtype=np.int64)
+        new = np.arange(T) + np.searchsorted(before, np.arange(T), side="right")
+        at = before + np.arange(k)
+        self.replaced, self.heirs = renamed(self.replaced, new), renamed(self.heirs, new)
+        self.appended = renamed(self.appended, new) | ({int(a) for a in at} if self.eval else set())
+        if self.eval_ff is not None:
+            f = self.eval_ff.astype(np.int64)
+            self.eval_ff = np.where(f == NONE, NONE, f + np.searchsorted(before, f, side="right")).astype(np.uint32)
+        if self.assigned is not None:
+            self.assigned = np.insert(self.assigned, ad.offsets(self.d)[before], NONE).astype(np.uint32)
+        z = np.zeros(k, dtype=np.uint32)
+        self.asks, self.cap, self.cap0 = np.insert(self.asks, before, rows), np.insert(self.cap, before, z), \
+            np.insert(self.cap0, before, z)
+        self.floors0 = np.insert(self.floors0, before, z)
+        if self.floors is not None:
+            self.floors = np.insert(self.floors, before, z)
+        self.d, self.d_pass = np.insert(self.d, before, z + 1), np.insert(self.d_pass, before, z + 1)
+        if self.dem_kept is not None:
+            self.dem_kept = np.insert(self.dem_kept, before, np.ones(k, dtype=self.dem_kept.dtype))
+        self.mask, self.eval_mask = np.insert(self.mask, before, True), np.insert(self.eval_mask, before, False)
+        self.toggled = renamed(self.toggled, new) | self._inserted_a0(at)
+        self.resized |= self.auc_state
+        self._note_facts()
+        return at
+
+    def _inserted_a0(self, at):
+        """The inserted asks A0 gains: all of them (their one slot holds nothing)."""
+        return {int(a) for a in at}
 
     # ---- predictions of refusals (the set of statuses the header allows)
     def refusal(self, kind):
@@ -581,7 +687,7 @@ class History(AskMarket):
             self.discard_eval()
             return
         self.eval, self.dirty, self.over = True, set(), False
-        self.replaced, self.appended, self.dropped = set(), set(), 0
+        self.replaced, self.appended, self.heirs, self.dropped = set(), set(), set(), 0
         self.eval_mask = self.mask.copy()
         self.eval_ff = self.first_feasible()
         self.eval_facts, self.flipped = self.facts(), set()
@@ -653,6 +759,12 @@ class History(AskMarket):
         elif name == "shrink_asks":
             if x["n"] != len(self.asks):    # pm_resize_asks to the current size changes nothing
                 self.shrink_asks(x["n"])
+        elif name == "remove_asks":
+            self.remove_asks(x["idx"])
+        elif name == "insert_asks":
+            self.insert_asks(x["before"], x["rows"])
+            if x["cap"] is not None:
+                self.set_caps(x["cap"])
         elif name in ("ask_delta_refused", "demand_refused", "restore_refused"):   # refused: nothing changes
             pass
         elif name == "demand":
@@ -733,6 +845,12 @@ def drive(eng, ev):
             eng.set_price_caps(x["cap"])
     elif name == "shrink_asks":
         eng.resize_asks(x["n"])
+    elif name == "remove_asks":
+        eng.remove_asks(x["idx"])
+    elif name == "insert_asks":
+        eng.insert_asks(x["before"], *delta_rows(x))
+        if x["cap"] is not None:
+            eng.set_price_caps(x["cap"])
     elif name == "ask_delta_refused":
         refuse_delta(eng, x)
     elif name == "demand":
@@ -767,7 +885,9 @@ def delta_rows(x):
 
 
 def refuse_delta(eng, x):
-    """One PM_E_INVALID case of pm_update_asks / pm_resize_asks: the call is refused and pm_table_version stays."""
+    """One PM_E_INVALID case of pm_update_asks / pm_resize_asks / pm_remove_asks / pm_insert_asks: the call is refused
+    and pm_table_version stays.  That the tables themselves stay is shown by the incremental and warm passes that
+    follow every refusal (the history's `follow`), which compare the engine with the mirror."""
     from protocol_b200._lib import PrimeMatchError
 
     T, rows, opts = x["T"], x["rows"], x["opts"]
@@ -777,12 +897,26 @@ def refuse_delta(eng, x):
     bad_range = rows.copy()
     bad_range["opt_off"][0], bad_range["n_opts"][0] = len(opts), 1
     bad_range["flags"][0] |= abi.PM_A_HAS_REQ
+    def remove_null():   # a NULL idx with n > 0 (pm_multi keeps no ask count on the host)
+        import ctypes
+
+        fn = eng._lib.pm_remove_asks if hasattr(eng, "n_asks") else eng._lib.pm_multi_remove_asks
+        rc = fn(eng._h, ctypes.c_void_p(None), 2)
+        if rc != abi.PM_OK:
+            raise PrimeMatchError(rc, "pm_remove_asks: null")
+
     calls = {"index": lambda: eng.update_asks(np.array([1, T], dtype=np.uint32), rows, opts),
              "sizes": lambda: eng.update_asks(np.array([1, 2], dtype=np.uint32), bad_sizes, opts),
              "range": lambda: eng.update_asks(np.array([1, 2], dtype=np.uint32), bad_range, opts),
              "grow_without_rows": lambda: eng.resize_asks(T + 2),
              "grow_bad_range": lambda: eng.resize_asks(T + 2, bad_range, opts),
-             "too_many": lambda: eng.resize_asks(1 << 30, rows, opts)}
+             "too_many": lambda: eng.resize_asks(1 << 30, rows, opts),
+             "remove_index": lambda: eng.remove_asks(np.array([3, T, 1], dtype=np.uint32)),
+             "remove_null": remove_null,
+             "insert_decreasing": lambda: eng.insert_asks(np.array([2, 1], dtype=np.uint32), rows, opts),
+             "insert_past_end": lambda: eng.insert_asks(np.array([1, T + 1], dtype=np.uint32), rows, opts),
+             "insert_sizes": lambda: eng.insert_asks(np.array([0, T], dtype=np.uint32), bad_sizes, opts),
+             "insert_range": lambda: eng.insert_asks(np.array([1, 1], dtype=np.uint32), bad_range, opts)}
     v = eng.table_version()
     try:
         calls[x["case"]]()
@@ -791,7 +925,8 @@ def refuse_delta(eng, x):
     else:
         raise AssertionError(f"ask delta {x['case']}: accepted")
     assert eng.table_version() == v, (x["case"], "pm_table_version changed")
-    assert getattr(eng, "n_asks", T) == T, (x["case"], "n_asks changed")
+    # the wrapper's own count (it moves only after the library returns PM_OK), not a read of the engine
+    assert getattr(eng, "n_asks", T) == T, (x["case"], "the wrapper's n_asks changed")
 
 
 def refuse_demand(eng, x):
@@ -1028,9 +1163,31 @@ class Gen:
         if name == "shrink_asks":
             n = T - int(rng.integers(1, 6 if T > 210 else 2)) if rng.random() < 0.95 else T   # T: changes nothing
             return ("shrink_asks", dict(n=n))
+        if name == "remove_asks":   # unsorted, sometimes a repeated index; held asks, first asks, max_group_size 0 rows
+            held, first = self.held_asks()
+            k = int(rng.integers(1, 5 if T > 210 else 2))
+            r = rng.random()
+            z = np.flatnonzero(h.asks["max_group_size"] == 0)
+            pool = held if r < 0.3 and len(held) else first if r < 0.55 and len(first) else \
+                z if r < 0.7 and len(z) else np.arange(T)
+            idx = rng.permutation(rng.choice(pool, min(k, len(pool)), replace=False))
+            if rng.random() < 0.3:
+                idx = np.concatenate([idx, idx[:1]])
+            return ("remove_asks", dict(idx=idx.astype(np.uint32)))
+        if name == "insert_asks":   # equal positions, the front and the end (= an append); sometimes caps for them
+            k = int(rng.integers(1, 4 if T < 280 else 2))
+            r = rng.random()
+            before = np.zeros(k) if r < 0.2 else np.full(k, T) if r < 0.35 else np.sort(rng.integers(0, T + 1, k))
+            if rng.random() < 0.3:
+                before[:] = before[0]
+            before = before.astype(np.uint32)
+            cap = None
+            if rng.random() < 0.6:
+                cap = np.insert(h.cap, before.astype(np.int64), rng.integers(50, 1500, k)).astype(np.uint32)
+            return self.delta("insert_asks", self.ask_rows(k), before=before, cap=cap)
         if name == "ask_delta_refused":
-            return self.delta("ask_delta_refused", self.ask_rows(2, edge=0), T=T,
-                              case=DELTA_REFUSALS[int(rng.integers(0, len(DELTA_REFUSALS)))])
+            cases = DELTA_REFUSALS + SPLICE_REFUSALS
+            return self.delta("ask_delta_refused", self.ask_rows(2, edge=0), T=T, case=cases[int(rng.integers(0, len(cases)))])
         if name == "ask_on":
             off = np.flatnonzero(~h.mask)
             if rng.random() < 0.6 or len(off) < 2:
@@ -1302,7 +1459,7 @@ def generate(shape, seed, n_calls=N_CALLS, cutoff=DEFAULT_CUTOFF, slot=0, n_slot
             emit_pass("certificate")        # refused: the ask table was resized since the last auction pass
             return True
         n0 = len(events)
-        if scripted_demand(n_passes):       # on top of the history's length
+        if scripted_demand(n_passes) or scripted_splice(n_passes):   # on top of the history's length
             extra[0] += len([e for e in events[n0:] if e[0] != "probe"])
             return True
         if n_passes >= 24 and h.cutoff < 1000 and "e_rows" not in done:
@@ -1495,6 +1652,170 @@ def generate(shape, seed, n_calls=N_CALLS, cutoff=DEFAULT_CUTOFF, slot=0, n_slot
             return True
         return False
 
+    def remove(idx):
+        emit_call(("remove_asks", dict(idx=rng.permutation(np.asarray(idx, dtype=np.int64)).astype(np.uint32))))
+
+    def insert(before, rows, cap=None):
+        emit_call(g.delta("insert_asks", np.ascontiguousarray(rows).copy(), before=np.asarray(before, dtype=np.uint32),
+                          cap=cap))
+        return np.asarray(before, dtype=np.int64) + np.arange(len(before))
+
+    def flush():
+        """The passes a refusal is to be followed by, before a step's own passes."""
+        for _ in range(2):
+            if follow:
+                kind = follow.pop(0)
+                if kind in AUCTION:
+                    all_on()
+                emit_pass(kind)
+
+    def evaluated():
+        """A stored evaluation from a lean pass (again after one a missing pattern refused)."""
+        flush()
+        emit_pass("lean")
+        if not h.eval:
+            emit_pass("lean")
+        return h.eval
+
+    def first_asks():
+        """The stored first asks with a row after them, the ones most workers store first."""
+        ff = h.eval_ff[h.eval_ff != NONE].astype(np.int64)
+        c = np.bincount(ff, minlength=len(h.asks))
+        order = np.argsort(-c, kind="stable")
+        return [int(t) for t in order[:8] if c[t] > 0 and t + 1 < len(h.asks)]
+
+    def scripted_splice(n_passes):
+        """The remove and insert steps every history makes once (each from its pass count on)."""
+        s = h.s
+        if n_passes >= 3 and "splice_refusals" not in done:
+            done.add("splice_refusals")
+            for case in SPLICE_REFUSALS:
+                emit_call(g.delta("ask_delta_refused", g.ask_rows(2, edge=0), T=len(h.asks), case=case))
+            for case in DELTA_REFUSALS:   # each once too (random draws may miss one); rows drawn from nothing random
+                emit_call(("ask_delta_refused", dict(rows=s["pool"][:2].copy(), opts=h.opts, own=False, T=len(h.asks),
+                                                     case=case)))
+            return True
+        if n_passes >= 5 and "heir" not in done:
+            # remove the asks most workers store first; then one whose heir was disabled, replaced or inserted since
+            # the stored evaluation; each before an incremental pass
+            done.add("heir")
+            for variant in ("plain", "disabled", "replaced", "inserted"):
+                if not evaluated() or not first_asks():
+                    continue
+                first = first_asks()
+                t = first[0]
+                if variant == "plain":
+                    remove(first[:2] + first[:1])
+                else:
+                    if variant == "disabled":
+                        emit_call(("ask_off", dict(idx=np.array([t + 1], dtype=np.uint32))))
+                    elif variant == "replaced":
+                        emit_call(g.update_asks(np.array([t + 1], dtype=np.uint32), g.ask_rows(1, edge=0)))
+                    else:
+                        insert([t + 1], g.ask_rows(1, edge=0))
+                    remove([t])
+                emit_pass("lean_incr")
+            return True
+        if n_passes >= 7 and "no_heir" not in done:
+            # remove a stored first ask with every row after it (and one row before it): its workers store NONE
+            done.add("no_heir")
+            if evaluated():
+                T = len(h.asks)
+                ff = h.eval_ff[h.eval_ff != NONE]
+                if len(ff):
+                    f = int(ff.max())
+                    rm = list(range(f, T)) + ([int(rng.integers(0, f))] if f else [])
+                    remove(rm)
+                    emit_pass("lean_incr")
+                    insert(np.full(len(rm), len(h.asks)), g.ask_rows(len(rm), edge=0, missing=False))
+            return True
+        if n_passes >= 10 and "insert_first" not in done:
+            # a row just before a stored first ask that accepts the same workers (the ask's own row)
+            done.add("insert_first")
+            if evaluated() and first_asks():
+                t = first_asks()[0]
+                insert([t], h.asks[[t]])
+                emit_pass("lean_incr")
+            return True
+        if n_passes >= 16 and "crossings" not in done:
+            # inside one incremental window: rows that turn the fast predicate off, push the feature dictionary past 64
+            # and make proximity refuse, inserted and removed again; then each alone before a materialised or
+            # proximity pass, and removed before the next
+            done.add("crossings")
+            if len(h.max0_on()):
+                emit_call(("ask_off", dict(idx=h.max0_on().astype(np.uint32))))
+            evaluated()
+            at = []
+            for row in (s["edge"][3:4], s["feature"], s["edge"][0:1]):
+                a = int(insert(rng.integers(0, len(h.asks) + 1, 1), row)[0])
+                at = [x + (x >= a) for x in at] + [a]
+            remove(at)
+            emit_pass("lean_incr")
+            for row, kinds in ((s["feature"], ("materialized", "materialized")), (s["edge"][3:4], ("materialized",) * 2),
+                               (s["edge"][0:1], ("proximity", "proximity"))):
+                a = insert(np.sort(rng.integers(0, len(h.asks) + 1, 1)), row)
+                emit_pass(kinds[0])
+                remove(a)
+                emit_pass(kinds[1])
+            return True
+        if n_passes >= 20 and "splice_chain" not in done:
+            # 3 -> 2 on held asks, a removal past them and an insertion at the front (they move up one row), 2 -> 3,
+            # then one warm pass: the kept slots chain through the remap
+            done.add("splice_chain")
+            slot_state(6, 3)
+            big = np.flatnonzero(h.d > 1)
+            if len(big):
+                emit_call(("demand", dict(d=np.where(h.d > 1, 2, h.d).astype(np.uint32))))
+                free = np.setdiff1d(np.arange(len(h.asks)), big)
+                free = free[free > big.max()] if (free > big.max()).any() else free
+                r = int(free[int(rng.integers(0, len(free)))])
+                remove([r])
+                insert([0], g.ask_rows(1, missing=False))
+                d = h.d.copy()
+                d[big - (big > r) + 1] = 3
+                emit_call(("demand", dict(d=d)))
+                if h.cutoff < 1000 and h.auc_state:   # one change past the cutoff, the kept and inserted slots counted
+                    write_unchanged(h.cutoff + 1 - h.n_changes())
+            emit_pass("warm")
+            ones()
+            return True
+        if n_passes >= 24 and "splice_certificate" not in done:
+            # the certificate refuses after a splice until the next auction pass
+            done.add("splice_certificate")
+            all_on()
+            emit_pass("auction")
+            remove([int(rng.integers(0, len(h.asks)))])
+            emit_pass("certificate")
+            emit_pass("auction")
+            emit_pass("certificate")
+            return True
+        if n_passes >= 32 and h.cutoff < 1000 and "splice_held" not in done:
+            # a worker shrink below a worker a slot holds, then the removal of held asks of demand > 1: freed slots
+            # below and above n_kept; unchanged rows written until removed_held decides the cutoff
+            done.add("splice_held")
+            for kind, over in (("warm", slot % 2 == 0), ("repair", slot % 2 == 1)):
+                slot_state(8, 3)
+                if not h.auc_state:
+                    continue
+                off = ad.offsets(h.d)
+                cand = [(int(h.assigned[s_]), int(t)) for t in np.flatnonzero(h.d > 1)
+                        for s_ in range(off[t], off[t + 1]) if h.assigned[s_] != NONE]
+                high = [c for c in cand if c[0] >= h.n_workers - 200]
+                rm = sorted({t for _, t in cand})[:3]
+                if high:
+                    w, t = max(high)
+                    emit_call(("shrink", dict(n=w, rank=rng.permutation(w).astype(np.uint32))))
+                    rm = sorted(set(rm[:2]) | {t})
+                if rm:
+                    remove(rm)
+                if h.auc_state and h.removed_held:
+                    base = h.n_changes() - h.removed_held
+                    write_unchanged(h.cutoff - base - (0 if over else h.removed_held))
+                emit_pass(kind)
+            ones()
+            return True
+        return False
+
     def mine(a, b):
         """An unseen (pass -> pass) pair this slot is to make."""
         return a in PASSES and (a, b) not in seen_pass and (PASSES.index(a) * len(PASSES) + PASSES.index(b)) % n_slots == slot
@@ -1624,17 +1945,19 @@ def generate(shape, seed, n_calls=N_CALLS, cutoff=DEFAULT_CUTOFF, slot=0, n_slot
             if len(h.max0_on()) and rng.random() < 0.75:
                 emit_call(("ask_off", dict(idx=h.max0_on().astype(np.uint32))))
         emit_pass(kind)
-    while scripted_demand(1 << 30):         # the demand and restore steps the loop had no room for
+    while scripted_demand(1 << 30) or scripted_splice(1 << 30):   # the steps the loop had no room for
         pass
     for c, kind in must:                    # the slot's pairs the loop had no room for
         emit_named(c)
         emit_pass(kind)
+        flush()
     for i in range(slot, len(PASSES) ** 2, n_slots):
         a, b = PASSES[i // len(PASSES)], PASSES[i % len(PASSES)]
         if (a, b) not in seen_pass:
             if last_pass != a:
                 emit_pass(a)
             emit_pass(b)
+    flush()
     return events, h
 
 

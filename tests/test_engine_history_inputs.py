@@ -5,7 +5,10 @@ reference passes of both modes with toggles left on across them, the fast/generi
 incremental pass's window, and cutoff crossings on both trackers; the demand and restore steps with the property each
 claims.  And the mirror checked against itself: the oracle's groups on the enabled asks equal test_gpu_ask_enabled's
 compaction, the warm checker with no changes reproduces the stored state, the slot-level mirror with every demand 1 is
-the ask-level one, and each of six wrong demand or restore rules changes some prediction of the same histories."""
+the ask-level one, and each of twelve wrong demand, restore, removal or insertion rules changes some prediction of the
+same histories.  The removals and insertions: every refused case, incremental passes after every kind of heir, a removed
+first ask with no row after it and a row inserted before one, a demand chain through a splice, removed held slots on
+both sides of n_kept that decide the warm cutoff, and the certificate refused after a splice until an auction pass."""
 import functools
 
 import numpy as np
@@ -16,9 +19,39 @@ import auction_demand as ad
 import auction_repair_checker as rp
 import auction_warm_checker as wc
 import engine_history as eh
+import feature_tables as ft
 from helpers import assert_distance_certificate
 from oracle import pm_oracle as orc
 from protocol_b200 import abi, synth
+
+
+def n_features(h):
+    """The feature dictionary's size over the mirror's ask rows (pm_build_argmin_feat runs when it is at most 64)."""
+    return len(ft.dictionary(ft.converted(h.asks, h.opts)))
+
+
+def splice_seen(h, x, st):
+    """Before a removal: which heirs it makes (the heir's state since the stored evaluation), whether a stored first
+    ask loses every row after it, and on which side of n_kept the workers of the removed slots lie."""
+    T = len(h.asks)
+    rm = np.unique(x["idx"].astype(np.int64))
+    keep = np.setdiff1d(np.arange(T), rm)
+    if h.eval:
+        stored = set(h.eval_ff[h.eval_ff != eh.NONE].tolist())
+        for t, s in zip(rm, np.searchsorted(keep, rm)):
+            if int(t) not in stored:
+                continue
+            if s == len(keep):
+                st["splice_saw"].add("no_heir")
+                continue
+            heir = int(keep[s])
+            st["splice_saw"].add("disabled" if not h.mask[heir] else "replaced" if heir in h.replaced
+                                 else "appended" if heir in h.appended else "plain")
+    if h.auc_state and h.assigned is not None:
+        off = ad.offsets(h.d)
+        gone = np.concatenate([h.assigned[off[t]:off[t + 1]] for t in rm])
+        gone = gone[gone != eh.NONE]
+        st["splice_gone"] = (bool((gone < h.n_kept).any()), bool((gone >= h.n_kept).any()))
 
 
 @functools.lru_cache(maxsize=None)
@@ -29,12 +62,14 @@ def evidence():
               e_rows_over=0, removed_held=set(), removed_held_decides=set(), max0_by=set(), probes_after_auction=0,
               generated={}, cases=set(), freed_decides=set(), chain=set(), past_kept=0, d_over_w=set(),
               variants=set(), own_clean=0, move_full=0, restore_incr=0, restore_cert=0, set_asks_export=0,
-              cert_back_to_one=0, window=set(), slot_warm=set())
+              cert_back_to_one=0, window=set(), slot_warm=set(), splice_incr=set(), splice_chain=set(),
+              splice_held=set(), splice_cert=set(), crossings=set())
     for shape in eh.SHAPES:
         for setting in eh.SETTINGS:
             cutoff = eh.cutoff_of(setting)
             st = dict(last="start", calls=[], pend_incr=[], pend_warm=[], since_eval=dict(auction=0, certificate=0),
-                      since_state=dict(ff=0, prox=0, disabled_across=False), max0=None, after_auction=False)
+                      since_state=dict(ff=0, prox=0, disabled_across=False), max0=None, after_auction=False,
+                      splice_saw=set(), window=dict(feats=[], fast=[], max0=[], start=0, start_fast=False))
 
             def observe(h, e, before, st=st, cutoff=cutoff):
                 if e[0] == "call":
@@ -47,8 +82,7 @@ def evidence():
                             ev["refusals"][name] = ev["refusals"].get(name, 0) + 1
                             st["pend_incr"].append(name)
                             st["pend_warm"].append((name, h.auc_state))
-                            if name != "ask_delta_refused":
-                                ev["cases"].add((name, x["case"]))
+                            ev["cases"].add((name, x["case"]))
                         if name == "demand" and h.auc_state:   # removed slots' workers past n_kept
                             o = ad.offsets(h.d)
                             gone = [int(w) for t in range(len(h.d)) for w in
@@ -58,6 +92,10 @@ def evidence():
                             st["set_asks_d"] = True
                         if name in ("restore", "move"):
                             st["restore_eval"] = h.eval
+                        if name == "remove_asks":
+                            splice_seen(h, x, st)
+                        if name == "insert_asks" and h.eval and set(x["before"].tolist()) & set(h.eval_ff.tolist()):
+                            st["splice_saw"].add("insert_before_first")
                         return
                     if name in ("restore", "move") and h.last_report is not None:
                         variant = x.get("variant", "move")
@@ -73,6 +111,11 @@ def evidence():
                         st["restored_eval"] = st.get("restore_eval", False) and name == "restore"
                         st["moved"] = name == "move"
                     st["calls"].append(name)
+                    if name in ("remove_asks", "insert_asks"):   # the facts each splice leaves inside the window
+                        w = st["window"]
+                        w["feats"].append(n_features(h))
+                        w["fast"].append(eh.asks_small(h.asks, h.opts))
+                        w["max0"].append(len(h.max0_on()) > 0)
                     if name in eh.ASK_DELTAS and (len(h.max0_on()) > 0) != st["max0"]:
                         ev["max0_by"].add(name)
                     if name in ("set_asks", "model_table", "set_workers"):
@@ -99,6 +142,43 @@ def evidence():
                     ev["move_full"] += bool(st.get("moved") and full and not h.eval)
                     ev["restore_incr"] += bool(restored and st.get("restored_eval") and h.eval and not full)
                     st["moved"] = False
+                spliced = bool({"remove_asks", "insert_asks"} & set(st["calls"]))
+                if kind == "certificate" and why == "certificate_asks_resized" and spliced:
+                    ev["splice_cert"].add("refused")
+                    st["cert_splice"] = True
+                elif kind == "certificate" and why is None and st.get("cert_splice") and st["last"] == "auction":
+                    ev["splice_cert"].add("ran")
+                if kind in ("warm", "repair") and why is None and h.auc_state and not h.auc_over \
+                        and st.get("splice_gone") == (True, True) and h.n_changes() - h.removed_held <= cutoff:
+                    ev["splice_held"].add((kind, h.n_changes() <= cutoff))
+                if kind in ("warm", "repair") and why is None and spliced and h.dem_kept is not None \
+                        and (h.dem_kept != np.minimum(h.d_pass, h.d)).any():
+                    ev["splice_chain"].add(kind)
+                if kind in eh.AUCTION and why is None:
+                    st["splice_gone"] = None
+                if kind in eh.INCREMENTAL and why is None and not h.incremental_plan()[0]:
+                    ev["splice_incr"] |= st["splice_saw"]
+                    w = st["window"]
+                    if w["feats"]:   # splices inside this incremental pass's window
+                        if shape == "wide" and w["start"] <= ft.MAX_FEATURES < max(w["feats"]) \
+                                and n_features(h) <= ft.MAX_FEATURES:
+                            ev["crossings"].add("past_64_and_back")
+                        if w["start_fast"] and not all(w["fast"]) and eh.asks_small(h.asks, h.opts) \
+                                and "ask_fast" in h.flipped:
+                            ev["crossings"].add("fast_off_and_on")
+                        if any(w["max0"]) and not len(h.max0_on()):
+                            ev["crossings"].add("max0_on_and_off")
+                if kind.startswith("proximity") and why == "proximity_max0" and st["calls"][-1:] == ["insert_asks"]:
+                    ev["crossings"].add("proximity_refused")
+                    st["prox_splice"] = True
+                elif kind.startswith("proximity") and why is None and st.get("prox_splice") \
+                        and st["calls"][-1:] == ["remove_asks"]:
+                    ev["crossings"].add("proximity_cleared")
+                if kind in eh.REFERENCE:
+                    st["splice_saw"] = set()
+                    if why is None:   # a new stored evaluation: a new window
+                        st["window"] = dict(feats=[], fast=[], max0=[], start=n_features(h),
+                                            start_fast=eh.asks_small(h.asks, h.opts))
                 if kind in eh.AUCTION and why is None:
                     D = int(h.d.sum())
                     warm = h.warm_plan()[0] if kind in ("warm", "repair") else False
@@ -240,7 +320,7 @@ def test_removed_held_asks_decide_the_warm_cutoff():
 
 MIRROR = ("asks", "mask", "eval_mask", "cap", "floors", "wa", "wb", "lat", "lon", "rank", "reputation", "eval_ff", "d",
           "d_pass", "dem_kept", "price", "assigned")
-TRACKED = ("params", "eval", "dirty", "over", "replaced", "appended", "dropped", "flipped", "auc_state", "auc_w",
+TRACKED = ("params", "eval", "dirty", "over", "replaced", "appended", "heirs", "dropped", "flipped", "auc_state", "auc_w",
            "auc_over", "resized", "rows", "toggled", "n_kept", "cap0", "floors0", "removed_held")
 
 
@@ -482,9 +562,59 @@ class KeepChanges(eh.History):
         self.rows, self.toggled, self.cap0, self.floors0 = rows, toggled, cap0, floors0
 
 
+class HeirInE(eh.History):
+    def split(self):                       # the heir listed in E instead of D
+        en, dis = eh.split_toggles(self.mask, self.eval_mask, self.replaced)
+        return en | self.heirs, dis
+
+
+class NoHeir(eh.History):
+    def _new_heirs(self, rm, keep):        # the heir not marked at all
+        return set()
+
+
+class RemovedPastKept(eh.History):
+    def _removed_freed(self, gone):        # a removed ask's held slots past n_kept counted too
+        return int((np.asarray(gone) != eh.NONE).sum())
+
+
+class InsertedNotA0(eh.History):
+    def _inserted_a0(self, at):            # an inserted ask's empty slot not in A0
+        return set()
+
+
+class DemKeptNotRemapped(eh.History):      # the kept slots of a demand chain left at their old indices
+    def remove_asks(self, idx):
+        k = self.dem_kept
+        super().remove_asks(idx)
+        if k is not None:
+            self.dem_kept = k[:len(self.d)].copy()
+
+    def insert_asks(self, before, rows):
+        k = self.dem_kept
+        at = super().insert_asks(before, rows)
+        if k is not None:
+            self.dem_kept = np.concatenate([k, np.ones(len(at), dtype=k.dtype)])
+        return at
+
+
+class SpliceNotResized(eh.History):        # a removal or an insertion leaves the certificate's resize flag
+    def remove_asks(self, idx):
+        r = self.resized
+        super().remove_asks(idx)
+        self.resized = r
+
+    def insert_asks(self, before, rows):
+        r = self.resized
+        at = super().insert_asks(before, rows)
+        self.resized = r
+        return at
+
+
 def differs(cls, shape, setting):
-    """Replay a seeded history on the true mirror and on a mutated one side by side: does any warm decision, auction
-    prediction (assignment, prices, rounds, n_released) or restore report differ?"""
+    """Replay a seeded history on the true mirror and on a mutated one side by side: does any incremental plan (full or
+    not, rows walked), certificate refusal, warm decision, auction prediction (assignment, prices, rounds, n_released)
+    or restore report differ?"""
     events, g = evidence()["generated"][shape, setting]
     t, m = eh.History(shape, eh.cutoff_of(setting)), cls(shape, eh.cutoff_of(setting))
     inputs = ("price", "assigned", "n_kept")
@@ -498,6 +628,10 @@ def differs(cls, shape, setting):
         if e[0] != "pass":
             continue
         why, _ = t.refusal(e[1])
+        if e[1] in eh.INCREMENTAL and why is None and t.incremental_plan()[:2] != m.incremental_plan()[:2]:
+            return True
+        if e[1] == "certificate" and m.refusal(e[1])[0] != why:
+            return True
         if e[1] in eh.REFERENCE:
             t.reference_done(why is None)
             m.reference_done(why is None)
@@ -519,9 +653,93 @@ def differs(cls, shape, setting):
     return False
 
 
-@pytest.mark.parametrize("cls", [CountPastKept, NoFreed, AllSlotsA0, PassMin, PriceReset, KeepChanges],
+@pytest.mark.parametrize("cls", [CountPastKept, NoFreed, AllSlotsA0, PassMin, PriceReset, KeepChanges, HeirInE, NoHeir,
+                                 RemovedPastKept, InsertedNotA0, DemKeptNotRemapped, SpliceNotResized],
                          ids=lambda c: c.__name__)
 def test_a_wrong_rule_changes_a_prediction(cls):
     order = [("mixed", "incr40"), ("wide", "incr40")] + [(sh, st) for sh in eh.SHAPES for st in eh.SETTINGS
                                                          if st != "incr40"]
     assert any(differs(cls, sh, st) for sh, st in order), f"{cls.__name__}: no history tells it from the rule"
+
+
+# ------------------------------------------------------------------ removals and insertions
+def test_every_ask_delta_refusal_occurs():
+    cases = evidence()["cases"]
+    want = {("ask_delta_refused", c) for c in eh.DELTA_REFUSALS + eh.SPLICE_REFUSALS}
+    assert cases >= want, sorted(want - cases)
+
+
+def test_incremental_passes_walk_every_kind_of_heir():
+    """Passes that stay incremental after a removal whose heir was enabled and untouched, disabled, replaced or
+    inserted since the stored evaluation, after one that left a stored first ask without a row after it, and after a
+    row inserted just before a stored first ask."""
+    want = {"plain", "disabled", "replaced", "appended", "no_heir", "insert_before_first"}
+    assert evidence()["splice_incr"] >= want, evidence()["splice_incr"]
+
+
+def test_demand_chains_through_a_splice():
+    assert "warm" in evidence()["splice_chain"], evidence()["splice_chain"]
+
+
+def test_removed_held_slots_on_both_sides_of_n_kept_decide_the_cutoff():
+    """Under PM_TUNE_INCR=40, warm and repair passes after removed asks whose slots held workers below and above
+    n_kept, which are within the cutoff without the removed holds: cold where those pass it, warm where not, each
+    side at least once."""
+    held = evidence()["splice_held"]
+    assert {k for k, _ in held} == {"warm", "repair"} and {w for _, w in held} == {False, True}, held
+
+
+def test_the_certificate_waits_for_an_auction_pass_after_a_splice():
+    assert evidence()["splice_cert"] >= {"refused", "ran"}, evidence()["splice_cert"]
+
+
+def test_splices_cross_the_predicate_the_feature_budget_and_proximity_inside_one_window():
+    """Inside one incremental window, splices turn the fast predicate off and on again, take the wide tables' current
+    rows past 64 features and back, and enable and remove a max_group_size 0 row; a proximity pass right after such an
+    insertion is refused and one right after its removal runs."""
+    want = {"past_64_and_back", "fast_off_and_on", "max0_on_and_off", "proximity_refused", "proximity_cleared"}
+    assert evidence()["crossings"] >= want, evidence()["crossings"]
+
+
+def test_the_feature_row_takes_the_wide_tables_past_the_budget():
+    for shape, n in (("mixed", 46), ("wide", 64)):
+        s = eh.setup(shape)
+        for k in (0, 1):
+            assert len(ft.dictionary(ft.converted(s["asks"][k], s["opts"]))) == n
+            with_row = np.concatenate([s["asks"][k], s["feature"]])
+            assert len(ft.dictionary(ft.converted(with_row, s["opts"]))) == n + 1 and eh.asks_small(with_row, s["opts"])
+
+
+@pytest.mark.parametrize("shape", eh.SHAPES)
+def test_removing_the_tail_is_a_shrink_and_inserting_at_the_end_an_append(shape):
+    """On the mirror, with a stored evaluation, a stored auction state and demands above 1."""
+    import copy
+
+    events, g = evidence()["generated"][shape, "default"]
+    found = []
+
+    def on_pass(h, i, kind, why):
+        if not found and h.eval and h.auc_state and (h.d > 1).any() and h.held_asks()[-1] > len(h.asks) - 10:
+            found.append(copy.deepcopy(h))
+
+    rebuild(events, g.outcomes, eh.History(shape), on_pass=on_pass)
+    assert found
+    a, b = found[0], copy.deepcopy(found[0])
+    T = len(a.asks)
+
+    def same():
+        for f in MIRROR:
+            x, y = getattr(a, f), getattr(b, f)
+            assert (x is None and y is None) or np.array_equal(x, y), f
+        for f in TRACKED:
+            x, y = getattr(a, f), getattr(b, f)
+            assert (np.array_equal(x, y) if isinstance(x, np.ndarray) else x == y), f
+
+    a.remove_asks(np.random.default_rng(1).permutation(np.arange(T - 10, T)))
+    b.shrink_asks(T - 10)
+    assert b.removed_held
+    same()
+    rows = a.s["pool"][:4]
+    a.insert_asks(np.full(4, T - 10), rows)
+    b.append_asks(rows)
+    same()
