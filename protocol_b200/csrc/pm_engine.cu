@@ -1916,10 +1916,11 @@ static void launch_build_argmin(pm_engine* e, const pm::EvalParams& p, int bits_
   const pm::FoldOut fo{e->stripe_rank.p, e->rank_best.p, e->first_ask.p, e->ask_best.p, e->ask_count.p, e->feat_perm.p};
   uint32_t* t32 = reinterpret_cast<uint32_t*>(tile);
   if (e->feat_ok) {   // the feature rows of this pass (match_local)
-    // Four CTAs per SM (64 registers, 24 KB of shared memory each).  With every store written, two were fastest: more
-    // row streams lost DRAM efficiency.  With most stores skipped (TileBuf::held), four are: cfg3 on an H100 SXM at
-    // 700 W, the kernel 52.9 ms per pass at four CTAs, 54.0 at three, 59.4-59.7 at two.
-    pm::pm_build_argmin_feat<<<grid, pm::kEvalThreads, 0, e->stream>>>(e->feat_a.p, e->feat_o.p, e->feat_w.p, t0, nt, w0, nw,
+    // Three CTAs per SM (__launch_bounds__: 72 registers, 12.5 KB of shared memory each; four would need 64 registers).
+    // With every store written, two were fastest: more row streams lost DRAM efficiency.  The grid's rows are
+    // pm::kFeatRows per CTA, half the FastRow kernels' (see there).
+    const dim3 fgrid(grid.x, blocks_for(nt, pm::kFeatRows));
+    pm::pm_build_argmin_feat<<<fgrid, pm::kEvalThreads, 0, e->stream>>>(e->feat_a.p, e->feat_o.p, e->feat_w.p, t0, nt, w0, nw,
                                                                       t32, ld, e->cost.held, fo);
     return;
   }

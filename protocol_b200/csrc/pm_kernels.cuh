@@ -402,14 +402,19 @@ __device__ __forceinline__ uint32_t fold_row(uint32_t key, uint32_t nb, uint32_t
 
 // End of the CTA's rows (its first ask t_cta): each row with a feasible column merges best_of_rank[its least rank]
 // into ask_best and its feasible count into ask_count.  row_done(i, m) sees every row i < nrows with m's bit j set
-// when warp j's 128 columns of the row are all infeasible.
-template <class RowDone>
-__device__ __forceinline__ void fold_merge_rows(const uint16_t (&s_key)[kFoldWarps][kFastRows],
-                                                const uint8_t (&s_nb)[kFoldWarps][kFastRows], uint32_t nrows,
-                                                uint32_t t_cta, const FoldOut& fo, RowDone&& row_done) {
-  __syncthreads();                            // every warp has written its slot of every row
+// when warp j's 128 columns of the row are all infeasible.  A row for which live(i) is false has no feasible column
+// and its warps wrote no slots: it merges nothing, and row_done sees every bit set.
+template <int ROWS, class RowLive, class RowDone>
+__device__ __forceinline__ void fold_merge_rows(const uint16_t (&s_key)[kFoldWarps][ROWS],
+                                                const uint8_t (&s_nb)[kFoldWarps][ROWS], uint32_t nrows,
+                                                uint32_t t_cta, const FoldOut& fo, RowLive&& live, RowDone&& row_done) {
+  __syncthreads();                            // every warp has written its slot of every live row
   const long long* best = fo.best_of_rank + blockIdx.x * kEvalCols;
   for (uint32_t i = threadIdx.x; i < nrows; i += kEvalThreads) {
+    if (!live(i)) {
+      row_done(i, (1u << kFoldWarps) - 1u);
+      continue;
+    }
     uint32_t key = kNone, nb = 0, m = 0;
 #pragma unroll
     for (int j = 0; j < kFoldWarps; ++j) {
@@ -540,7 +545,7 @@ __device__ __forceinline__ void build_fast(const EvalParams& p, uint32_t t0, uin
   mbar_wait(&s.bar, 0);
   for_each_row_pair(s.row, nrows, out, row_stride, emit);
   if constexpr (FOLD) {
-    fold_merge_rows(s_key, s_nb, nrows, t_cta, fo, [](uint32_t, uint32_t) {});
+    fold_merge_rows(s_key, s_nb, nrows, t_cta, fo, [](uint32_t) { return true; }, [](uint32_t, uint32_t) {});
     fold_flush_first_ask<false>(cm, cbase, w0, nw, fo);
   }
 }
@@ -809,21 +814,37 @@ __global__ void pm_feature_gather(const uint4* __restrict__ wb, const unsigned l
 // bit j set when warp j's 512-byte block of it holds kNarrowInfeasible in every word.  Most blocks are all infeasible
 // row after row (the column order), so a warp stores its block only when some word changes: when the row has a
 // feasible column there or the block's bit is clear.  The tile stays what the stores would have made it.  The CTA reads
-// its rows' bytes in the prologue and writes them back after the merge; each byte belongs to one CTA of a launch, and
-// launches are stream-ordered.
+// its rows' bytes in the prologue and writes back those that change after the merge; each byte belongs to one CTA of a
+// launch, and launches are stream-ordered.
+//
+// Most rows have nothing to do in the whole stripe, and the column order makes that knowable for the CTA at once: So,
+// the OR of the 8 warps' Fo, is nearly as selective as each Fo.  Once the rows have landed, one thread per row triages
+// it: if R_o & ~So != 0 for every option, every block of the row is dead (each Fo ⊆ So).  Such a row is SKIP when its
+// map byte is 0xFF (every block already holds the sentinel: no store, no slot, no fold, no byte to write) and
+// SENTINEL otherwise (each warp whose bit is clear stores the sentinel block; the byte becomes 0xFF).  Every other row
+// is LIVE and runs the per-block code.  The LIVE and SENTINEL rows are compacted, in increasing order, into two lists
+// the warps walk; the merge takes no slot of a row that is not LIVE.
+//
+// A CTA takes 256 rows, not the FastRow kernels' 512.  Its stores go wherever its LIVE rows are, and the resident CTAs'
+// LIVE rows differ, so the fewer rows a CTA spans, the narrower the band of tile rows the SMs store into at once.  On
+// cfg3 (H100 SXM, 700 W), per step in this kernel: 45.6 ms at 512 rows against 37.1 before the triage, and 12.7 with its
+// stores removed, so the scattered store stream bound it; 29.1 ms at 256 rows, 32.0 at 128 (more CTAs, each paying
+// the prologue, the merge and the first-ask flush).
+constexpr int kFeatRows = 256;
 __global__ void __launch_bounds__(kEvalThreads, 3)
 pm_build_argmin_feat(const uint4* __restrict__ arow, const uint2* __restrict__ ropt, const uint4* __restrict__ feat,
                      uint32_t t0, uint32_t nt, uint32_t w0, uint32_t nw, uint32_t* __restrict__ tile, size_t ld,
                      uint8_t* __restrict__ held, FoldOut fo) {
-  __shared__ __align__(128) uint4 s_row[kFastRows + 2];   // + 2: the look-ahead loads past the last pair of rows
+  __shared__ __align__(128) uint4 s_row[kFeatRows];
   __shared__ uint64_t s_bar;
-  __shared__ uint16_t s_key[kFoldWarps][kFastRows];
-  // [0]: fold_row's infeasible counts.  [1]: per warp and row, the count at which its block needs no store: 128 when
-  // the block holds the sentinel, else 0xFF (never); one byte past the count's, at nb_slot + kHeldOff + r
-  __shared__ uint8_t s_nb[2][kFoldWarps][kFastRows];
-  constexpr uint32_t kHeldOff = kFoldWarps * kFastRows;
-  const uint32_t r0 = blockIdx.y * kFastRows;
-  const uint32_t nrows = min(nt - r0, (uint32_t)kFastRows);
+  __shared__ uint16_t s_key[kFoldWarps][kFeatRows];
+  __shared__ uint8_t s_nb[kFoldWarps][kFeatRows];    // fold_row's infeasible counts
+  __shared__ uint8_t s_held[kFeatRows];              // each row's map byte as the launch found it
+  __shared__ uint2 s_fo[kFoldWarps];                 // each warp's Fo
+  __shared__ uint32_t s_live_bits[kFeatRows / 32], s_sent_bits[kFeatRows / 32];   // bit i & 31 of word i / 32: row i
+  __shared__ uint16_t s_live[kFeatRows + 2], s_sent[kFeatRows];   // + 2: the look-ahead loads past the last live row
+  const uint32_t r0 = blockIdx.y * kFeatRows;
+  const uint32_t nrows = min(nt - r0, (uint32_t)kFeatRows);
   if (threadIdx.x == 0) {
     mbar_init(&s_bar, 1);
     mbar_expect_tx(&s_bar, nrows * 16u);
@@ -831,12 +852,8 @@ pm_build_argmin_feat(const uint4* __restrict__ arow, const uint2* __restrict__ r
   }
   const size_t held_stride = ld / kEvalCols;
   uint8_t* held_cta = held + (size_t)r0 * held_stride + blockIdx.x;
-  for (uint32_t i = threadIdx.x; i < nrows; i += kEvalThreads) {
-    const uint32_t m = held_cta[i * held_stride];
-#pragma unroll
-    for (int j = 0; j < kFoldWarps; ++j) s_nb[1][j][i] = (m >> j) & 1u ? 128u : 0xFFu;
-  }
-  const uint32_t lane = threadIdx.x & 31u;
+  for (uint32_t i = threadIdx.x; i < nrows; i += kEvalThreads) s_held[i] = held_cta[i * held_stride];
+  const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
   const uint32_t cbase = blockIdx.x * kEvalCols + (threadIdx.x >> 5) * 128u + lane * 4u;
   uint32_t fl[kEvalWPT], fh[kEvalWPT], price[kEvalWPT], dy[kEvalWPT], rk[kEvalWPT], cm[kEvalWPT];
 #pragma unroll
@@ -856,20 +873,23 @@ pm_build_argmin_feat(const uint4* __restrict__ arow, const uint2* __restrict__ r
   const uint32_t fa_lo = __reduce_and_sync(0xffffffffu, fl[0] & fl[1] & fl[2] & fl[3]);
   const uint32_t fa_hi = __reduce_and_sync(0xffffffffu, fh[0] & fh[1] & fh[2] & fh[3]);
   const uint32_t kmin = __reduce_min_sync(0xffffffffu, min(min(rk[0], rk[1]), min(rk[2], rk[3])));
+  if (lane == 0) s_fo[warp] = make_uint2(fo_lo, fo_hi);
   uint4* out = reinterpret_cast<uint4*>(tile + (size_t)r0 * ld + cbase);
   size_t row_stride = ld / 4;
   asm("" : "+l"(row_stride));
   const uint32_t t_cta = t0 + r0;
-  uint32_t key_slot = (uint32_t)__cvta_generic_to_shared(&s_key[threadIdx.x >> 5][0]);
-  uint32_t nb_slot = (uint32_t)__cvta_generic_to_shared(&s_nb[0][threadIdx.x >> 5][0]);
+  uint32_t key_slot = (uint32_t)__cvta_generic_to_shared(&s_key[warp][0]);
+  uint32_t nb_slot = (uint32_t)__cvta_generic_to_shared(&s_nb[warp][0]);
   asm("" : "+r"(key_slot), "+r"(nb_slot));
   // 1 behind an opaque move: with the literal, ptxas proves b = min(u, 1) is 0 or 1 and turns the multiply-adds below
   // into compares and selects on the busier ALU pipe (EvalParams::sign_shift does the same for the FastRow kernel)
   uint32_t one = 1u;
   asm("" : "+r"(one));
+  constexpr uint32_t S = kNarrowInfeasible;
+  // A LIVE row r.  The warp's block needs no store when it holds the sentinel (its bit of the map byte) and the row
+  // leaves every word the sentinel: skip_at is the infeasible count at which that is so, 128, or 0xFF (never).
   auto emit = [&](const uint4& q, uint4* dst, uint32_t r) {
-    uint32_t skip_at;
-    asm volatile("ld.shared.u8 %0, [%1];" : "=r"(skip_at) : "r"(nb_slot + kHeldOff + r));
+    const uint32_t skip_at = (s_held[r] >> warp) & 1u ? 128u : 0xFFu;
     // the least over the options, as for a column: dead != 0 when every option misses a feature of Fo, full == 0 when
     // some option needs only features of Fa
     uint32_t dead = (q.x & ~fo_lo) | (q.y & ~fo_hi), full = (q.x & ~fa_lo) | (q.y & ~fa_hi);
@@ -880,7 +900,6 @@ pm_build_argmin_feat(const uint4* __restrict__ arow, const uint2* __restrict__ r
     }
     if (__all_sync(0xffffffffu, dead != 0u)) {   // every word the sentinel, no feasible column: as fold_row would leave it
       fold_slot(kNoRank, 128u, key_slot, nb_slot, r);
-      constexpr uint32_t S = kNarrowInfeasible;
       if (skip_at != 128u) __stcs(dst, make_uint4(S, S, S, S));
       return;
     }
@@ -911,10 +930,84 @@ pm_build_argmin_feat(const uint4* __restrict__ arow, const uint2* __restrict__ r
     }
     if (fold_row(key, nb, key_slot, nb_slot, r) != skip_at) __stcs(dst, make_uint4(o[0], o[1], o[2], o[3]));
   };
-  __syncthreads();            // mbarrier initialised, s_nb[1] written
+  __syncthreads();            // mbarrier initialised, s_held and s_fo written
+  uint32_t so_lo = 0, so_hi = 0;   // the stripe's So
+#pragma unroll
+  for (int j = 0; j < kFoldWarps; ++j) {
+    const uint2 v = s_fo[j];
+    so_lo |= v.x;
+    so_hi |= v.y;
+  }
   mbar_wait(&s_bar, 0);
-  for_each_row_pair(s_row, nrows, out, row_stride, emit);
-  fold_merge_rows(s_key, s_nb[0], nrows, t_cta, fo, [&](uint32_t i, uint32_t m) { held_cta[i * held_stride] = (uint8_t)m; });
+  // The triage of rows h * 256 + threadIdx.x: the ballots of a warp's 32 rows are word h * 8 + warp of the bit sets
+  constexpr int kTriage = (kFeatRows + kEvalThreads - 1) / kEvalThreads;
+  uint32_t lb[kTriage], sb[kTriage];
+#pragma unroll
+  for (int h = 0; h < kTriage; ++h) {
+    const uint32_t i = h * kEvalThreads + threadIdx.x;
+    bool live = false, sent = false;
+    if (i < nrows) {   // nrows <= kFeatRows
+      const uint4 q = s_row[i];
+      uint32_t dead = (q.x & ~so_lo) | (q.y & ~so_hi);   // the least over the options, as emit's dead test
+      for (uint32_t o = 1; o < q.z; ++o) {
+        const uint2 R = __ldg(ropt + q.w + o);
+        dead = min(dead, (R.x & ~so_lo) | (R.y & ~so_hi));
+      }
+      live = dead == 0u;
+      sent = !live && s_held[i] != 0xFFu;
+    }
+    lb[h] = __ballot_sync(0xffffffffu, live);
+    sb[h] = __ballot_sync(0xffffffffu, sent);
+    if (lane == 0 && i < kFeatRows) {
+      s_live_bits[i >> 5] = lb[h];
+      s_sent_bits[i >> 5] = sb[h];
+    }
+  }
+  __syncthreads();
+  // Each LIVE / SENTINEL row's place in its list: the rows of the words before its own, then the lanes below it
+  uint32_t n_live = 0, n_sent = 0, pl[kTriage] = {}, ps[kTriage] = {};
+#pragma unroll
+  for (int k = 0; k < kFeatRows / 32; ++k) {
+    const uint32_t a = __popc(s_live_bits[k]), b = __popc(s_sent_bits[k]);
+#pragma unroll
+    for (int h = 0; h < kTriage; ++h)
+      if (k < h * kFoldWarps + (int)warp) {
+        pl[h] += a;
+        ps[h] += b;
+      }
+    n_live += a;
+    n_sent += b;
+  }
+  const uint32_t below = (1u << lane) - 1u;
+#pragma unroll
+  for (int h = 0; h < kTriage; ++h) {
+    const uint32_t i = h * kEvalThreads + threadIdx.x;
+    if ((lb[h] >> lane) & 1u) s_live[pl[h] + __popc(lb[h] & below)] = (uint16_t)i;
+    if ((sb[h] >> lane) & 1u) s_sent[ps[h] + __popc(sb[h] & below)] = (uint16_t)i;
+  }
+  if (threadIdx.x == 0) s_live[n_live] = s_live[n_live + 1] = 0;   // the look-ahead past the last rows: row 0, unused
+  __syncthreads();
+  // LIVE rows: each index loaded two rows ahead, each row one row ahead, in registers the row before has finished with
+  uint32_t r = s_live[0], rn = s_live[1];
+  uint4 q = s_row[r];
+  for (uint32_t j = 0; j < n_live; ++j) {
+    const uint4 qn = s_row[rn];
+    const uint32_t rnn = s_live[j + 2];
+    emit(q, out + r * row_stride, r);
+    r = rn;
+    rn = rnn;
+    q = qn;
+  }
+  // SENTINEL rows: the sentinel block wherever the map's bit is clear
+  for (uint32_t j = 0; j < n_sent; ++j) {
+    const uint32_t i = s_sent[j];
+    if (!((s_held[i] >> warp) & 1u)) __stcs(out + i * row_stride, make_uint4(S, S, S, S));
+  }
+  fold_merge_rows(
+      s_key, s_nb, nrows, t_cta, fo, [&](uint32_t i) { return (s_live_bits[i >> 5] >> (i & 31u)) & 1u; },
+      [&](uint32_t i, uint32_t m) {   // only the bytes that change: a SKIP row's is 0xFF already
+        if (m != s_held[i]) held_cta[i * held_stride] = (uint8_t)m;
+      });
   fold_flush_first_ask<true>(cm, cbase, w0, nw, fo);
 }
 
