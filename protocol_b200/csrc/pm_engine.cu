@@ -110,20 +110,27 @@ template <class T> struct PinBuf {
 // layout's blocks are the same 512-byte blocks).  pm_build_argmin_feat reads and writes it, and skips the stores of a
 // block that is all infeasible and already holds the sentinel.  Any other writer of the buffer calls overwritten();
 // the next pm_build_argmin_feat pass then zeroes the map (prepare_held) and writes every block once more.
+//
+// `priced` is its twin, indexed the same way: bit j set when block j holds this pass's column prices in every word (a
+// row feasible in all 128 columns), and pm_build_argmin_feat skips the store of such a row's block there too.  A
+// block's two bits are never both set.  The prices and the column order are the pass's own, so prepare_held zeroes
+// `priced` at every pass start; within a pass no other writer touches the buffer.
 struct TileBuf {
   long long* p = nullptr;
   size_t n = 0;
   CUmemGenericAllocationHandle h = 0;   // non-zero: compressible mapping of `bytes` bytes at p
   size_t bytes = 0;
-  uint8_t* held = nullptr;              // [held_bytes()]
+  uint8_t* held = nullptr;              // [held_bytes()], then `priced` in the same allocation
+  uint8_t* priced = nullptr;            // [held_bytes()]
   bool held_valid = false;              // false: the map is stale, every block must be written
 
   size_t held_bytes() const { return (n * sizeof(long long) + 4095) / 4096; }
   void overwritten() { held_valid = false; }
-  // the map, zeroed in stream order when it is stale: no host synchronisation
+  // once per pm_build_argmin_feat pass, in stream order (no host synchronisation): `priced` zeroed, and `held` too
+  // when it is stale (one memset over both)
   cudaError_t prepare_held(cudaStream_t st) {
-    if (held_valid) return cudaSuccess;
-    const cudaError_t e = cudaMemsetAsync(held, 0, held_bytes(), st);
+    const cudaError_t e = held_valid ? cudaMemsetAsync(priced, 0, held_bytes(), st)
+                                     : cudaMemsetAsync(held, 0, 2 * held_bytes(), st);
     held_valid = e == cudaSuccess;
     return e;
   }
@@ -221,13 +228,18 @@ struct TileBuf {
       return e;
     }
     n = want;
-    e = cudaMalloc(&held, held_bytes());
-    if (e != cudaSuccess) release();
+    e = cudaMalloc(&held, 2 * held_bytes());
+    if (e != cudaSuccess) {
+      held = nullptr;
+      release();
+      return e;
+    }
+    priced = held + held_bytes();
     return e;
   }
   void release() {
     if (held) cudaFree(held);
-    held = nullptr;
+    held = priced = nullptr;
     held_valid = false;
     if (h) {
       const Api& a = api();
@@ -366,6 +378,11 @@ struct pm_engine {
   DevBuf<uint2> feat_o;
   DevBuf<unsigned long long> feat_key, feat_key_s;
   DevBuf<uint32_t> feat_val, feat_perm;
+  // Its slot schedule (pm_sched_keys / pm_sched_gather), [n_asks] each: the sort's keys and asks sched_key / sched_val,
+  // sorted into sched_key_s / sched_val_s; the launches' rows and asks in write order, sched_row / sched_ask.
+  DevBuf<unsigned long long> sched_key, sched_key_s;
+  DevBuf<uint32_t> sched_val, sched_val_s, sched_ask;
+  DevBuf<uint4> sched_row;
 
   // The stored evaluation of PM_INCREMENTAL: the per-worker first feasible ask of the last evaluation of this engine's
   // range (shard()), PM_NONE outside it, in its own buffer (first_ask is the resolution's working copy: the sweeps, the
@@ -1093,6 +1110,8 @@ void pm_destroy(pm_engine* e) {
   e->cost.release(); e->first_ask.release(); e->ask_count.release(); e->ask_best.release();
   e->stripe_rank.release(); e->rank_best.release();
   e->feat_buf.release(); e->h_feat.release(); e->feat_w.release(); e->feat_a.release(); e->feat_o.release();
+  e->sched_key.release(); e->sched_key_s.release(); e->sched_val.release(); e->sched_val_s.release();
+  e->sched_ask.release(); e->sched_row.release();
   e->feat_key.release(); e->feat_key_s.release(); e->feat_val.release(); e->feat_perm.release();
   e->eval_first.release(); e->h_dirty.release(); e->dirty_dev.release(); e->incr_evals.release();
   e->walk_start.release(); e->toggle_dev.release(); e->splice_dev.release();
@@ -1909,19 +1928,21 @@ static void launch_fused(pm_engine* e, const pm::EvalParams& p, int bits_mode, b
 }
 
 // pm_build_argmin: the 32-bit tile's build and argmin in one launch (the stripe ranks of pm_stripe_rank in place).
-// tile is e->cost.p; the feature kernel needs its sentinel map prepared (TileBuf::prepare_held).
+// tile is e->cost.p; the feature kernel needs its maps prepared (TileBuf::prepare_held), and takes positions
+// [t0, t0 + nt) of the pass's slot schedule (sched_row / sched_ask); pm_build_argmin takes asks [t0, t0 + nt).
 static void launch_build_argmin(pm_engine* e, const pm::EvalParams& p, int bits_mode, uint32_t t0, uint32_t nt, uint32_t w0,
                                 uint32_t nw, long long* tile, size_t ld) {
   const dim3 grid(blocks_for(ld, pm::kEvalCols), blocks_for(nt, pm::kFastRows));
   const pm::FoldOut fo{e->stripe_rank.p, e->rank_best.p, e->first_ask.p, e->ask_best.p, e->ask_count.p, e->feat_perm.p};
   uint32_t* t32 = reinterpret_cast<uint32_t*>(tile);
   if (e->feat_ok) {   // the feature rows of this pass (match_local)
-    // Three CTAs per SM (__launch_bounds__: 72 registers, 12.5 KB of shared memory each; four would need 64 registers).
-    // With every store written, two were fastest: more row streams lost DRAM efficiency.  The grid's rows are
-    // pm::kFeatRows per CTA, half the FastRow kernels' (see there).
+    // Four CTAs per SM (__launch_bounds__: 64 registers, no spills, 12.75 KB of shared memory each), the fastest of 2, 3
+    // and 4 with the slot schedule (pm::kFeatRows).  The grid's rows are pm::kFeatRows per CTA, half the FastRow
+    // kernels'; t0 / nt are positions of the slot schedule.
     const dim3 fgrid(grid.x, blocks_for(nt, pm::kFeatRows));
-    pm::pm_build_argmin_feat<<<fgrid, pm::kEvalThreads, 0, e->stream>>>(e->feat_a.p, e->feat_o.p, e->feat_w.p, t0, nt, w0, nw,
-                                                                      t32, ld, e->cost.held, fo);
+    pm::pm_build_argmin_feat<<<fgrid, pm::kEvalThreads, 0, e->stream>>>(e->sched_row.p, e->sched_ask.p, e->feat_o.p,
+                                                                      e->feat_w.p, t0, nt, w0, nw, t32, ld, e->cost.held,
+                                                                      e->cost.priced, fo);
     return;
   }
   e->cost.overwritten();
@@ -2146,6 +2167,10 @@ static int match_local_locked(pm_engine* e, uint32_t mode) {
       rows = std::min<uint64_t>(rows, T);
       rows = std::min<uint64_t>(rows, 65535ull * pm::kArgRows);
       if (rows >= 1024) rows &= ~(uint64_t)511;   // whole row bands of the build kernel (no ragged last band in every tile)
+      // pm_build_argmin_feat's launches follow the slot schedule: Ks = n_tiles - 1 scheduled launches before the final
+      // writers' when there are three tiles or more, else the natural order (Ks = 0)
+      const uint32_t n_tiles = (uint32_t)((T + rows - 1) / rows);
+      const uint32_t sched_ks = narrow && e->feat_ok && n_tiles >= 3 ? n_tiles - 1 : 0u;
       const size_t tile_elems = (size_t)rows * ld * elem_bytes / 8;   // TileBuf elements; ld is a multiple of 1024
       if (e->cost.ensure(tile_elems, e->device, e->tune_compress != 0, e->stream) != cudaSuccess) {
         cudaGetLastError();
@@ -2168,6 +2193,30 @@ static int match_local_locked(pm_engine* e, uint32_t mode) {
           pm::pm_feature_asks<<<blocks_for(T, 256), 256, 0, e->stream>>>(e->frows.p, e->opts_fast.p, T, e->feat, e->feat_a.p,
                                                                          e->feat_o.p);
           PM_LAUNCH_CHECK("pm_feature_asks");
+          // the slot schedule (pm_kernels.cuh pm_sched_gather): the asks before the final writers sorted by R_0
+          PM_CUDA(e->sched_row.ensure(T));
+          PM_CUDA(e->sched_ask.ensure(T));
+          const uint32_t* sorted = nullptr;
+          if (sched_ks) {
+            const uint32_t m = T - (uint32_t)rows;
+            PM_CUDA(e->sched_key.ensure(m));
+            PM_CUDA(e->sched_key_s.ensure(m));
+            PM_CUDA(e->sched_val.ensure(m));
+            PM_CUDA(e->sched_val_s.ensure(m));
+            pm::pm_sched_keys<<<blocks_for(m, 256), 256, 0, e->stream>>>(e->feat_a.p, m, e->sched_key.p, e->sched_val.p);
+            PM_LAUNCH_CHECK("pm_sched_keys");
+            const int begin_bit = 64 - std::max<int>((int)e->feat.off[pm::kFeatKinds], 1);   // as the column sort's
+            size_t tmp = 0;
+            PM_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp, e->sched_key.p, e->sched_key_s.p, e->sched_val.p,
+                                                    e->sched_val_s.p, (int)m, begin_bit, 64, e->stream));
+            PM_CUDA(e->cub_tmp.ensure(tmp));
+            PM_CUDA(cub::DeviceRadixSort::SortPairs(e->cub_tmp.p, tmp, e->sched_key.p, e->sched_key_s.p, e->sched_val.p,
+                                                    e->sched_val_s.p, (int)m, begin_bit, 64, e->stream));
+            sorted = e->sched_val_s.p;
+          }
+          pm::pm_sched_gather<<<blocks_for(T, 256), 256, 0, e->stream>>>(e->feat_a.p, sorted, T, (uint32_t)rows, sched_ks,
+                                                                         e->sched_row.p, e->sched_ask.p);
+          PM_LAUNCH_CHECK("pm_sched_gather");
           pm::pm_feature_keys<<<blocks_for(ld, 256), 256, 0, e->stream>>>(e->wa.p, e->wb.p, e->bits.p, e->words, w0, nw, ld,
                                                                           e->feat, e->feat_key.p, e->feat_val.p,
                                                                           e->feat_key_s.p, e->feat_perm.p);
@@ -2194,8 +2243,14 @@ static int match_local_locked(pm_engine* e, uint32_t mode) {
       if (narrow && e->feat_ok) PM_CUDA(e->cost.prepare_held(e->stream));
       e->cost_tile_used = (size_t)rows * ld * elem_bytes;
       long long* tile = e->cost.p;
-      for (uint32_t t0 = 0; t0 < T; t0 += (uint32_t)rows) {
-        const uint32_t nt = (uint32_t)std::min<uint64_t>(rows, T - t0);
+      for (uint32_t k = 0; k < n_tiles; ++k) {
+        uint32_t t0 = k * (uint32_t)rows;
+        uint32_t nt = (uint32_t)std::min<uint64_t>(rows, T - t0);
+        if (sched_ks) {   // launch k of the schedule: positions [base_k, base_k + nt_k), the last one the final writers
+          const uint32_t m = T - (uint32_t)rows, a = m / sched_ks, b = m % sched_ks;
+          t0 = k < sched_ks ? k * a + std::min(k, b) : m;
+          nt = k < sched_ks ? a + (k < b ? 1u : 0u) : (uint32_t)rows;
+        }
         if (narrow) {
           // one launch that is both: its time counts in ms_build and in ms_argmin
           Timer tb(e, &e->stats.ms_build, e->stream);

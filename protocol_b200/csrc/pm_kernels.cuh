@@ -400,32 +400,34 @@ __device__ __forceinline__ uint32_t fold_row(uint32_t key, uint32_t nb, uint32_t
   return nb;
 }
 
-// End of the CTA's rows (its first ask t_cta): each row with a feasible column merges best_of_rank[its least rank]
-// into ask_best and its feasible count into ask_count.  row_done(i, m) sees every row i < nrows with m's bit j set
-// when warp j's 128 columns of the row are all infeasible.  A row for which live(i) is false has no feasible column
-// and its warps wrote no slots: it merges nothing, and row_done sees every bit set.
-template <int ROWS, class RowLive, class RowDone>
+// End of the CTA's rows: each row with a feasible column merges best_of_rank[its least rank] into ask_best and its
+// feasible count into ask_count, at its ask: at(p, i) is row i's entry of the per-ask array p.  row_done(i, m, pr) sees every row i < nrows with m's bit j set
+// when warp j's 128 columns of the row are all infeasible, and pr's when they are all feasible.  A row for which
+// live(i) is false has no feasible column and its warps wrote no slots: it merges nothing, and row_done sees every bit
+// of m set and none of pr.
+template <int ROWS, class RowLive, class RowAt, class RowDone>
 __device__ __forceinline__ void fold_merge_rows(const uint16_t (&s_key)[kFoldWarps][ROWS],
                                                 const uint8_t (&s_nb)[kFoldWarps][ROWS], uint32_t nrows,
-                                                uint32_t t_cta, const FoldOut& fo, RowLive&& live, RowDone&& row_done) {
+                                                const FoldOut& fo, RowLive&& live, RowAt&& at, RowDone&& row_done) {
   __syncthreads();                            // every warp has written its slot of every live row
   const long long* best = fo.best_of_rank + blockIdx.x * kEvalCols;
   for (uint32_t i = threadIdx.x; i < nrows; i += kEvalThreads) {
     if (!live(i)) {
-      row_done(i, (1u << kFoldWarps) - 1u);
+      row_done(i, (1u << kFoldWarps) - 1u, 0u);
       continue;
     }
-    uint32_t key = kNone, nb = 0, m = 0;
+    uint32_t key = kNone, nb = 0, m = 0, pr = 0;
 #pragma unroll
     for (int j = 0; j < kFoldWarps; ++j) {
       key = min(key, (uint32_t)s_key[j][i]);
       nb += s_nb[j][i];
       m |= (uint32_t)(s_nb[j][i] == 128u) << j;
+      pr |= (uint32_t)(s_nb[j][i] == 0u) << j;
     }
-    row_done(i, m);
+    row_done(i, m, pr);
     if (nb < (uint32_t)kEvalCols) {           // a feasible column: key is its least rank
-      atomicMin(fo.ask_best + t_cta + i, __ldg(best + key));
-      atomicAdd(fo.ask_count + t_cta + i, kEvalCols - nb);
+      atomicMin(at(fo.ask_best, i), __ldg(best + key));
+      atomicAdd(at(fo.ask_count, i), kEvalCols - nb);
     }
   }
 }
@@ -545,7 +547,8 @@ __device__ __forceinline__ void build_fast(const EvalParams& p, uint32_t t0, uin
   mbar_wait(&s.bar, 0);
   for_each_row_pair(s.row, nrows, out, row_stride, emit);
   if constexpr (FOLD) {
-    fold_merge_rows(s_key, s_nb, nrows, t_cta, fo, [](uint32_t) { return true; }, [](uint32_t, uint32_t) {});
+    fold_merge_rows(s_key, s_nb, nrows, fo, [](uint32_t) { return true; }, [&](auto* a, uint32_t i) { return a + t_cta + i; },
+                    [](uint32_t, uint32_t, uint32_t) {});
     fold_flush_first_ask<false>(cm, cbase, w0, nw, fo);
   }
 }
@@ -802,6 +805,53 @@ __global__ void pm_feature_gather(const uint4* __restrict__ wb, const unsigned l
   feat[c] = make_uint4((uint32_t)F, (uint32_t)(F >> 32), price, rank[c]);
 }
 
+// The slot schedule of pm_build_argmin_feat's launches.  A pass over T asks in tiles of `rows` row slots writes each
+// slot once per launch, and the blocks it stores are the transitions: a block that held the sentinel or the prices for
+// the slot's last ask and does not for this one.  In natural order a slot's successive asks t and t + rows are
+// unrelated, so most stores are transitions; the outputs do not depend on which asks share a launch (atomic min and
+// add per ask, a per-column minimum of asks), so the launches take the asks in an order that makes them rare.
+//
+// The contract of the buffer (PM_BUF_COST_TILE) is what the natural order leaves: slot i holds ask a of [T - rows, T)
+// with a % rows == i.  Those final writers form the last launch, in slot order.  The other M = T - rows asks are
+// sorted by (__brevll(R_0), ask) — R_0 the first option's requirement mask, its first features varying slowest, as the
+// column order's key — into S, and laid out slot-major over Ks = ceil(M / rows) launches: slot r of launch k holds
+// S[r * Ks + k], so a slot's successive asks are neighbours in S, and launch k covers the slots r < ceil((M - k) / Ks),
+// a prefix.  The launches stay ceil(T / rows).  The rows go in write order into srow (R_0 lo, R_0 hi, n_opts,
+// opt_off, as feat_a) and sask (the ask): launch k's at base_k = k * a + min(k, b) with M = a * Ks + b, the last at M.
+// With at most two tiles each slot is written at most twice a pass: the schedule is the natural order (Ks = 0).
+//
+// Key step, per pass in stream order: asks [0, M) keyed for cub::DeviceRadixSort.
+__global__ void pm_sched_keys(const uint4* __restrict__ arow, uint32_t m, unsigned long long* __restrict__ key,
+                              uint32_t* __restrict__ val) {
+  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= m) return;
+  const uint4 q = arow[t];
+  key[t] = __brevll((unsigned long long)q.y << 32 | q.x);
+  val[t] = t;
+}
+
+// Gather step: write position p of [0, T) from the sorted asks (Ks > 0) or the natural order (Ks = 0).
+__global__ void pm_sched_gather(const uint4* __restrict__ arow, const uint32_t* __restrict__ sorted, uint32_t n_asks,
+                                uint32_t rows, uint32_t ks, uint4* __restrict__ srow, uint32_t* __restrict__ sask) {
+  const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= n_asks) return;
+  uint32_t t = p;
+  if (ks) {
+    const uint32_t m = n_asks - rows;
+    if (p >= m) {   // the last launch: slot i's final writer, row i of the last tile or of the one before it
+      const uint32_t i = p - m, t_last = (n_asks - 1) / rows * rows;
+      t = i < n_asks - t_last ? t_last + i : t_last - rows + i;
+    } else {        // launch k's slot r: launches k < b take a + 1 slots, the others a
+      const uint32_t a = m / ks, b = m % ks, big = b * (a + 1);
+      const uint32_t k = p < big ? p / (a + 1) : b + (p - big) / a;
+      const uint32_t r = p < big ? p % (a + 1) : (p - big) % a;
+      t = sorted[r * ks + k];
+    }
+  }
+  srow[p] = arow[t];
+  sask[p] = t;
+}
+
 // pm_build_argmin with the feature predicate: the same stores, row fold, first-ask minimum and end-of-CTA merge
 // (build_fast<.., true>), the outputs bit for bit, on a tile whose column c holds worker w0 + perm[c] (the
 // column order above; the ranks and best_of_rank carry the workers, and first_ask is flushed to them).  A warp first
@@ -810,36 +860,46 @@ __global__ void pm_feature_gather(const uint4* __restrict__ wb, const unsigned l
 // A worker is one 16-byte load in the prologue; a row is one 16-byte shared-memory load; further OR-options (R_o) are
 // read from global memory, warp-uniform.
 //
+// The CTA's rows are positions t0 + r0 + i of the slot schedule (pm_sched_gather): their requirement rows come from
+// srow, their asks from sask, and row i goes to tile slot r0 + i.
+//
 // `held` (TileBuf::held) has one byte per row slot and 1024-column stripe of the tile, at slot * (ld / 1024) + stripe:
-// bit j set when warp j's 512-byte block of it holds kNarrowInfeasible in every word.  Most blocks are all infeasible
-// row after row (the column order), so a warp stores its block only when some word changes: when the row has a
-// feasible column there or the block's bit is clear.  The tile stays what the stores would have made it.  The CTA reads
-// its rows' bytes in the prologue and writes back those that change after the merge; each byte belongs to one CTA of a
-// launch, and launches are stream-ordered.
+// bit j set when warp j's 512-byte block of it holds kNarrowInfeasible in every word.  `priced` (TileBuf::priced),
+// indexed the same way, has bit j set when the block holds this pass's price of each of its columns in every word —
+// what a row feasible in all 128 columns stores; it is zeroed at every pass start, as column order and prices may
+// change between passes.  A block's two bits are never both set.  Most blocks are all infeasible row after row (the
+// column order), and in the scheduled order a slot's next ask usually needs what the last one did, so a warp stores its
+// block only when some word changes: unless the row is infeasible there and the held bit set, or feasible in every
+// column and the priced bit set.  The tile stays what the stores would have made it.  The CTA reads its rows' bytes in
+// the prologue and writes back those that change after the merge; each byte belongs to one CTA of a launch, and
+// launches are stream-ordered.
 //
 // Most rows have nothing to do in the whole stripe, and the column order makes that knowable for the CTA at once: So,
 // the OR of the 8 warps' Fo, is nearly as selective as each Fo.  Once the rows have landed, one thread per row triages
 // it: if R_o & ~So != 0 for every option, every block of the row is dead (each Fo ⊆ So).  Such a row is SKIP when its
 // map byte is 0xFF (every block already holds the sentinel: no store, no slot, no fold, no byte to write) and
-// SENTINEL otherwise (each warp whose bit is clear stores the sentinel block; the byte becomes 0xFF).  Every other row
+// SENTINEL otherwise (each warp whose bit is clear stores the sentinel block; the byte becomes 0xFF and the priced
+// byte 0).  Every other row
 // is LIVE and runs the per-block code.  The LIVE and SENTINEL rows are compacted, in increasing order, into two lists
 // the warps walk; the merge takes no slot of a row that is not LIVE.
 //
-// A CTA takes 256 rows, not the FastRow kernels' 512.  Its stores go wherever its LIVE rows are, and the resident CTAs'
-// LIVE rows differ, so the fewer rows a CTA spans, the narrower the band of tile rows the SMs store into at once.  On
-// cfg3 (H100 SXM, 700 W), per step in this kernel: 45.6 ms at 512 rows against 37.1 before the triage, and 12.7 with its
-// stores removed, so the scattered store stream bound it; 29.1 ms at 256 rows, 32.0 at 128 (more CTAs, each paying
-// the prologue, the merge and the first-ask flush).
+// A CTA takes 256 rows, not the FastRow kernels' 512.  Chosen while the scattered store stream bound the kernel (cfg3,
+// H100 SXM, 700 W, per step in this kernel: 45.6 ms at 512 rows, 29.1 at 256, 32.0 at 128, 12.7 with its stores
+// removed), and kept with the slot schedule, which stores few blocks: cfg3 steps of 17.3 ms at 256 rows and 3 CTAs/SM,
+// 17.6 at 512 rows and 3, 18.1 at 256 and 2, 19.9 at 512 and 2 (one session, 10 steps each); then 16.7 at 256 rows
+// and 4 CTAs/SM against 17.1-17.3 at 3 (20 steps each), so four CTAs per SM, 64 registers, no spills.
 constexpr int kFeatRows = 256;
-__global__ void __launch_bounds__(kEvalThreads, 3)
-pm_build_argmin_feat(const uint4* __restrict__ arow, const uint2* __restrict__ ropt, const uint4* __restrict__ feat,
-                     uint32_t t0, uint32_t nt, uint32_t w0, uint32_t nw, uint32_t* __restrict__ tile, size_t ld,
-                     uint8_t* __restrict__ held, FoldOut fo) {
+__global__ void __launch_bounds__(kEvalThreads, 4)
+pm_build_argmin_feat(const uint4* __restrict__ srow, const uint32_t* __restrict__ sask, const uint2* __restrict__ ropt,
+                     const uint4* __restrict__ feat, uint32_t t0, uint32_t nt, uint32_t w0, uint32_t nw,
+                     uint32_t* __restrict__ tile, size_t ld, uint8_t* __restrict__ held, uint8_t* __restrict__ priced,
+                     FoldOut fo) {
   __shared__ __align__(128) uint4 s_row[kFeatRows];
   __shared__ uint64_t s_bar;
   __shared__ uint16_t s_key[kFoldWarps][kFeatRows];
   __shared__ uint8_t s_nb[kFoldWarps][kFeatRows];    // fold_row's infeasible counts
-  __shared__ uint8_t s_held[kFeatRows];              // each row's map byte as the launch found it
+  __shared__ uint8_t s_held[kFeatRows], s_priced[kFeatRows];   // each row's map bytes as the launch found them
+  __shared__ uint32_t s_ask[kFeatRows];              // each row's ask
   __shared__ uint2 s_fo[kFoldWarps];                 // each warp's Fo
   __shared__ uint32_t s_live_bits[kFeatRows / 32], s_sent_bits[kFeatRows / 32];   // bit i & 31 of word i / 32: row i
   __shared__ uint16_t s_live[kFeatRows + 2], s_sent[kFeatRows];   // + 2: the look-ahead loads past the last live row
@@ -848,11 +908,16 @@ pm_build_argmin_feat(const uint4* __restrict__ arow, const uint2* __restrict__ r
   if (threadIdx.x == 0) {
     mbar_init(&s_bar, 1);
     mbar_expect_tx(&s_bar, nrows * 16u);
-    bulk_g2s(s_row, arow + t0 + r0, nrows * 16u, &s_bar);
+    bulk_g2s(s_row, srow + t0 + r0, nrows * 16u, &s_bar);
   }
   const size_t held_stride = ld / kEvalCols;
   uint8_t* held_cta = held + (size_t)r0 * held_stride + blockIdx.x;
-  for (uint32_t i = threadIdx.x; i < nrows; i += kEvalThreads) s_held[i] = held_cta[i * held_stride];
+  uint8_t* priced_cta = priced + (size_t)r0 * held_stride + blockIdx.x;
+  for (uint32_t i = threadIdx.x; i < nrows; i += kEvalThreads) {
+    s_held[i] = held_cta[i * held_stride];
+    s_priced[i] = priced_cta[i * held_stride];
+    s_ask[i] = __ldg(sask + t0 + r0 + i);
+  }
   const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
   const uint32_t cbase = blockIdx.x * kEvalCols + (threadIdx.x >> 5) * 128u + lane * 4u;
   uint32_t fl[kEvalWPT], fh[kEvalWPT], price[kEvalWPT], dy[kEvalWPT], rk[kEvalWPT], cm[kEvalWPT];
@@ -877,7 +942,6 @@ pm_build_argmin_feat(const uint4* __restrict__ arow, const uint2* __restrict__ r
   uint4* out = reinterpret_cast<uint4*>(tile + (size_t)r0 * ld + cbase);
   size_t row_stride = ld / 4;
   asm("" : "+l"(row_stride));
-  const uint32_t t_cta = t0 + r0;
   uint32_t key_slot = (uint32_t)__cvta_generic_to_shared(&s_key[warp][0]);
   uint32_t nb_slot = (uint32_t)__cvta_generic_to_shared(&s_nb[warp][0]);
   asm("" : "+r"(key_slot), "+r"(nb_slot));
@@ -886,10 +950,13 @@ pm_build_argmin_feat(const uint4* __restrict__ arow, const uint2* __restrict__ r
   uint32_t one = 1u;
   asm("" : "+r"(one));
   constexpr uint32_t S = kNarrowInfeasible;
-  // A LIVE row r.  The warp's block needs no store when it holds the sentinel (its bit of the map byte) and the row
-  // leaves every word the sentinel: skip_at is the infeasible count at which that is so, 128, or 0xFF (never).
+  // A LIVE row r.  The warp's block needs no store when the row leaves every word as the block holds it: the sentinel
+  // (its bit of `held`) and the row infeasible there, or the prices (its bit of `priced`) and the row feasible there.
+  // skip_at is the infeasible count at which that is so: 128, 0, or 0xFF (never); the two bits are never both set.
   auto emit = [&](const uint4& q, uint4* dst, uint32_t r) {
-    const uint32_t skip_at = (s_held[r] >> warp) & 1u ? 128u : 0xFFu;
+    const uint32_t hb = (s_held[r] >> warp) & 1u, pb = (s_priced[r] >> warp) & 1u;
+    const uint32_t skip_at = hb ? 128u : pb ? 0u : 0xFFu;
+    const uint32_t ask = s_ask[r];
     // the least over the options, as for a column: dead != 0 when every option misses a feature of Fo, full == 0 when
     // some option needs only features of Fa
     uint32_t dead = (q.x & ~fo_lo) | (q.y & ~fo_hi), full = (q.x & ~fa_lo) | (q.y & ~fa_hi);
@@ -900,14 +967,14 @@ pm_build_argmin_feat(const uint4* __restrict__ arow, const uint2* __restrict__ r
     }
     if (__all_sync(0xffffffffu, dead != 0u)) {   // every word the sentinel, no feasible column: as fold_row would leave it
       fold_slot(kNoRank, 128u, key_slot, nb_slot, r);
-      if (skip_at != 128u) __stcs(dst, make_uint4(S, S, S, S));
+      if (!hb) __stcs(dst, make_uint4(S, S, S, S));
       return;
     }
     if (__all_sync(0xffffffffu, full == 0u)) {   // every word the column's price, every column feasible
       fold_slot(kmin, 0u, key_slot, nb_slot, r);
-      __stcs(dst, make_uint4(price[0], price[1], price[2], price[3]));
+      if (!pb) __stcs(dst, make_uint4(price[0], price[1], price[2], price[3]));
 #pragma unroll
-      for (int k = 0; k < kEvalWPT; ++k) cm[k] = min(cm[k], t_cta + r);
+      for (int k = 0; k < kEvalWPT; ++k) cm[k] = min(cm[k], ask);
       return;
     }
     uint32_t u[kEvalWPT];
@@ -924,13 +991,13 @@ pm_build_argmin_feat(const uint4* __restrict__ arow, const uint2* __restrict__ r
     for (int k = 0; k < kEvalWPT; ++k) {
       const uint32_t b = min(u[k], one);                      // 1 when infeasible
       o[k] = b * dy[k] + price[k];                            // feasible: price ; infeasible: kNarrowInfeasible
-      cm[k] = min(cm[k], b * 0x80000000u + (t_cta + r));      // the ask, + 2^31 when infeasible
+      cm[k] = min(cm[k], b * 0x80000000u + ask);              // the ask, + 2^31 when infeasible
       key = min(key, b * kNoRank + rk[k]);                    // the rank, + kNoRank when infeasible
       nb += b;
     }
     if (fold_row(key, nb, key_slot, nb_slot, r) != skip_at) __stcs(dst, make_uint4(o[0], o[1], o[2], o[3]));
   };
-  __syncthreads();            // mbarrier initialised, s_held and s_fo written
+  __syncthreads();            // mbarrier initialised, s_held, s_priced, s_ask and s_fo written
   uint32_t so_lo = 0, so_hi = 0;   // the stripe's So
 #pragma unroll
   for (int j = 0; j < kFoldWarps; ++j) {
@@ -1004,9 +1071,11 @@ pm_build_argmin_feat(const uint4* __restrict__ arow, const uint2* __restrict__ r
     if (!((s_held[i] >> warp) & 1u)) __stcs(out + i * row_stride, make_uint4(S, S, S, S));
   }
   fold_merge_rows(
-      s_key, s_nb, nrows, t_cta, fo, [&](uint32_t i) { return (s_live_bits[i >> 5] >> (i & 31u)) & 1u; },
-      [&](uint32_t i, uint32_t m) {   // only the bytes that change: a SKIP row's is 0xFF already
+      s_key, s_nb, nrows, fo, [&](uint32_t i) { return (s_live_bits[i >> 5] >> (i & 31u)) & 1u; },
+      [&](auto* a, uint32_t i) { return a + s_ask[i]; },
+      [&](uint32_t i, uint32_t m, uint32_t pr) {   // only the bytes that change: a SKIP row's are 0xFF and 0 already
         if (m != s_held[i]) held_cta[i * held_stride] = (uint8_t)m;
+        if (pr != s_priced[i]) priced_cta[i * held_stride] = (uint8_t)pr;
       });
   fold_flush_first_ask<true>(cm, cbase, w0, nw, fo);
 }
