@@ -273,6 +273,43 @@ int pm_set_flags(pm_engine*, const uint32_t* idx, const uint32_t* flags, uint32_
 int      pm_resize_workers(pm_engine*, uint32_t n_workers);
 int      pm_update_workers(pm_engine*, const uint32_t* idx, const pm_worker_a* a, const pm_worker_b* b,
                            const double* lat, const double* lon, uint32_t n);
+/* Worker-table splices: a worker leaves (deregistered, banned, out of the auction's market) or joins at any position.
+ *   pm_remove_workers  remove rows idx[0..n) (any order; a repeated index removes its row once); the rows after them
+ *                      move up, order kept.  Removing the tail is pm_resize_workers shrinking.
+ *   pm_insert_workers  insert rows a[i], b[i] before the current rows before[i]; before[] non-decreasing, before[i] <=
+ *                      n_workers (n_workers = append); rows with equal before[] keep their order.  lat / lon both NULL
+ *                      (the new rows at (0, 0), as rows added by pm_resize_workers) or both given.  Inserting every row
+ *                      at n_workers is pm_resize_workers growing followed by pm_update_workers of the new rows.
+ * Every per-row column moves with its row: planes A and B, location, address rank and reputation.  An inserted row has
+ * address rank 0 and reputation 0 until pm_set_worker_addr_rank / pm_set_worker_reputation set them.
+ * THE DEFINING RULE: after any sequence of worker- and ask-table calls the engine equals a fresh engine loaded with the
+ * current rows (pm_set_worker_count + pm_upsert_workers + locations + ranks + reputation, the same asks, enabled mask,
+ * caps, floors and demands): every pm_fetch_result array, pm_build_cost_tile and a cold auction pass are bit-identical,
+ * in every mode, on every path, with and without PM_INCREMENTAL.  The tail cases equal pm_resize_workers (+
+ * pm_update_workers) in the tables, the stored evaluation, and the next pass's results, auction state and pm_stats.
+ * The exports between the call and that pass differ: after a splice they report the current rows (n_workers prices,
+ * PM_NONE for a removed holder), while after a shrink pm_auction_state still returns the stored pass's W prices and
+ * pm_auction_assignment the cut-off row's old index.
+ * Both calls keep the stored evaluation of PM_INCREMENTAL: each row's stored first ask moves with it on the device,
+ * removed rows vanish and inserted rows are written.  A communicator's share and an open-ended pm_set_shard range move
+ * with W as under pm_resize_workers (rows that enter a rank's range count as written there, rows that leave it return
+ * to PM_NONE); a fixed pm_set_shard range stays where it is and the rows that shift into it count as written.  The
+ * next incremental pass walks the inserted rows and the rows that crossed a range boundary only.
+ * Both keep the stored auction state: prices and owners move with their rows and the per-slot assignment is renamed to
+ * the new indices.  The holder of a removed row is released in step 1 of the next PM_AUCTION_WARM (or repair) pass and
+ * counts in n_released, exactly as the holder of a row a shrink cut off; the warm cutoff counts the removed rows as it
+ * counts the rows a shrink cut off.  Inserted rows are changed rows (R0): price 0, unowned.  pm_auction_state,
+ * pm_auction_assignment and pm_auction_slot_assignment report the renamed state over the current rows (a removed
+ * holder reads PM_NONE); pm_auction_certificate returns PM_E_STATE until the next auction pass.
+ * Refusals, none of which changes anything (no table, no stored evaluation, no auction state, no pm_table_version):
+ * PM_E_STATE without a worker table; PM_E_INVALID for a NULL pointer with n > 0, an index >= n_workers, a before[] that
+ * decreases or exceeds n_workers, lat without lon or the reverse, or a table that would reach PM_NONE rows.  Every
+ * check runs on the host before anything on the device is touched.  A call is one O(W) device pass.  The first
+ * splice allocates a second copy of every per-row column in use (up to 76 bytes per row: 76 MB at 1M workers), kept
+ * for the splices that follow and released by pm_set_worker_count. */
+int      pm_remove_workers(pm_engine*, const uint32_t* idx, uint32_t n);
+int      pm_insert_workers(pm_engine*, const uint32_t* before, const pm_worker_a* a, const pm_worker_b* b,
+                           const double* lat, const double* lon, uint32_t n);
 uint64_t pm_table_version(const pm_engine*);
 int      pm_create_sibling(const pm_engine*, pm_engine** out);
 
@@ -706,6 +743,11 @@ int pm_multi_set_flags(pm_multi*, const uint32_t* idx, const uint32_t* flags, ui
  * runs PM_INCREMENTAL through pm_multi_match, each device re-evaluating only its share's written rows */
 int pm_multi_resize_workers(pm_multi*, uint32_t n_workers);
 int pm_multi_update_workers(pm_multi*, const uint32_t* idx, const pm_worker_a* a, const pm_worker_b* b, const double* lat,
+                            const double* lon, uint32_t n);
+/* pm_remove_workers / pm_insert_workers on every device's replicated table, each device keeping its own share's stored
+ * evaluation (as pm_multi_resize_workers does); a refused call changes no device */
+int pm_multi_remove_workers(pm_multi*, const uint32_t* idx, uint32_t n);
+int pm_multi_insert_workers(pm_multi*, const uint32_t* before, const pm_worker_a* a, const pm_worker_b* b, const double* lat,
                             const double* lon, uint32_t n);
 int pm_multi_sync(pm_multi*);
 /* changes whenever any table call changed a table on any device, including calls made directly on

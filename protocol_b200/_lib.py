@@ -84,6 +84,8 @@ def load() -> C.CDLL:
         "pm_set_shard": (i32, [vp, u32, u32]),
         "pm_resize_workers": (i32, [vp, u32]),
         "pm_update_workers": (i32, [vp, vp, vp, vp, vp, vp, u32]),
+        "pm_remove_workers": (i32, [vp, vp, u32]),
+        "pm_insert_workers": (i32, [vp, vp, vp, vp, vp, vp, u32]),
         "pm_table_version": (C.c_uint64, [vp]),
         "pm_create_sibling": (i32, [vp, P(vp)]),
         "pm_comm_unique_id": (i32, [vp]),
@@ -109,6 +111,8 @@ def load() -> C.CDLL:
         "pm_multi_set_flags": (i32, [vp, vp, vp, u32]),
         "pm_multi_resize_workers": (i32, [vp, u32]),
         "pm_multi_update_workers": (i32, [vp, vp, vp, vp, vp, vp, u32]),
+        "pm_multi_remove_workers": (i32, [vp, vp, u32]),
+        "pm_multi_insert_workers": (i32, [vp, vp, vp, vp, vp, vp, u32]),
         "pm_multi_sync": (i32, [vp]),
         "pm_multi_table_version": (C.c_uint64, [vp]),
         "pm_multi_match": (i32, [vp, u32]),

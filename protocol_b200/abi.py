@@ -140,12 +140,12 @@ EXPORTS = [
     "pm_auction_slot_assignment", "pm_auction_restore_slots",
     "pm_match", "pm_fetch_result", "pm_get_stats", "pm_build_cost_tile",
     "pm_match_local", "pm_match_finish", "pm_device_buffer", "pm_stream_sync", "pm_set_shard",
-    "pm_resize_workers", "pm_update_workers", "pm_table_version", "pm_create_sibling",
+    "pm_resize_workers", "pm_update_workers", "pm_remove_workers", "pm_insert_workers", "pm_table_version", "pm_create_sibling",
     "pm_comm_unique_id", "pm_comm_create", "pm_comm_destroy", "pm_attach_comm",
     "pm_multi_create", "pm_multi_destroy", "pm_multi_size", "pm_multi_engine", "pm_multi_last_error",
     "pm_multi_set_asks", "pm_multi_set_ask_enabled", "pm_multi_update_asks", "pm_multi_resize_asks", "pm_multi_remove_asks", "pm_multi_insert_asks", "pm_multi_set_model_table", "pm_multi_set_worker_count", "pm_multi_upsert_workers",
     "pm_multi_set_worker_locations", "pm_multi_set_worker_addr_rank", "pm_multi_set_flags",
-    "pm_multi_resize_workers", "pm_multi_update_workers", "pm_multi_sync", "pm_multi_table_version",
+    "pm_multi_resize_workers", "pm_multi_update_workers", "pm_multi_remove_workers", "pm_multi_insert_workers", "pm_multi_sync", "pm_multi_table_version",
     "pm_multi_match", "pm_multi_fetch_result",
     "pm_plugin_create", "pm_plugin_create_multi", "pm_plugin_destroy", "pm_plugin_last_error", "pm_plugin_add_config", "pm_plugin_seal_configs",
     "pm_plugin_enable_configuration", "pm_plugin_upsert_node", "pm_plugin_set_node_status", "pm_plugin_sync_discovery", "pm_plugin_sync_discovery_json", "pm_plugin_get_node", "pm_plugin_add_task",

@@ -355,8 +355,14 @@ struct pm_engine {
   bool workers_checked = false;
   DevBuf<uint32_t> amin, amax, bits;
   DevBuf<uint32_t> scratch_idx, scratch_flags;
-  DevBuf<uint4> upd_a, upd_b;          // staging of pm_update_workers
+  DevBuf<uint4> upd_a, upd_b;          // staging of pm_update_workers (and of pm_insert_workers' rows)
   DevBuf<double> upd_lat, upd_lon;
+  // pm_remove_workers / pm_insert_workers: the second buffer of every per-row column (each splice writes the moved
+  // table into these and swaps them with the live ones), and the removed rows and positions (wsplice_dev)
+  DevBuf<uint4> wa_alt, wb_alt;
+  DevBuf<double> lat_alt, lon_alt;
+  DevBuf<uint32_t> rank_alt, rep_alt, nacc_alt, first_alt, owner_alt, wsplice_dev;
+  DevBuf<long long> price_alt;
   uint64_t table_version = 0;          // bumped by every call that changes a table (pm_table_version)
 
   // evaluation
@@ -560,6 +566,8 @@ struct pm_engine {
   // or added at all (the certificate then waits for the next pass)
   uint32_t auc_removed_held = 0;
   bool auc_asks_resized = false;
+  // pm_remove_workers / pm_insert_workers since the stored state (the certificate then waits for the next pass)
+  bool auc_workers_spliced = false;
   // Ask demands (pm_set_ask_demand; the auction only): empty while every ask takes one worker, and the auction then runs
   // on the ask table itself.  Else the demands and their exclusive scan over T + 1 (host, and device in dem_off): ask t
   // is the auction's bidders (slots) dem_off[t] .. dem_off[t + 1] - 1, and the stored assignment is per slot.  The pass
@@ -581,6 +589,7 @@ struct pm_engine {
     auc_rows_over = false;
     auc_removed_held = 0;
     auc_asks_resized = false;
+    auc_workers_spliced = false;
   }
   void auc_mark_ask(uint32_t t) {   // A0: toggled, replaced or appended since the stored state
     if (auc_state && !auc_ask_mark[t]) {
@@ -1107,6 +1116,9 @@ void pm_destroy(pm_engine* e) {
   e->raw_asks.release(); e->raw_opts.release(); e->upd_asks.release(); e->ask_counts.release(); e->ask_newoff.release(); e->amin.release(); e->amax.release(); e->bits.release();
   e->scratch_idx.release(); e->scratch_flags.release();
   e->upd_a.release(); e->upd_b.release(); e->upd_lat.release(); e->upd_lon.release();
+  e->wa_alt.release(); e->wb_alt.release(); e->lat_alt.release(); e->lon_alt.release(); e->rank_alt.release();
+  e->rep_alt.release(); e->nacc_alt.release(); e->first_alt.release(); e->owner_alt.release(); e->wsplice_dev.release();
+  e->price_alt.release();
   e->cost.release(); e->first_ask.release(); e->ask_count.release(); e->ask_best.release();
   e->stripe_rank.release(); e->rank_best.release();
   e->feat_buf.release(); e->h_feat.release(); e->feat_w.release(); e->feat_a.release(); e->feat_o.release();
@@ -1569,6 +1581,9 @@ int pm_set_worker_count(pm_engine* e, uint32_t n_workers) try {
   e->invalidate_eval();
   e->auc_discard();
   PM_CUDA(cudaSetDevice(e->device));
+  // a full reload replaces the table: the second buffers of the worker splices go until the next splice needs them
+  e->wa_alt.release(); e->wb_alt.release(); e->lat_alt.release(); e->lon_alt.release(); e->rank_alt.release();
+  e->rep_alt.release(); e->nacc_alt.release(); e->first_alt.release(); e->owner_alt.release(); e->price_alt.release();
   if (n_workers > e->wa.n || !e->wa.p) {
     // grow, preserving nothing: callers upsert after (re)sizing
     PM_CUDA(e->wa.ensure(n_workers));
@@ -1779,6 +1794,233 @@ int pm_update_workers(pm_engine* e, const uint32_t* idx, const pm_worker_a* a, c
   e->nacc_valid = false;
   e->matched = e->local_done = false;
   return PM_OK;
+} catch (...) { return pm_guard_rc(); }
+
+// Rows removed from and inserted into the worker table (pm_remove_workers, pm_insert_workers).  removed: old rows,
+// increasing and distinct; before: per inserted row the old row it goes before, non-decreasing.  There is no W-entry
+// map: a row's new index is two binary searches away (pm_kernels.cuh WorkerSplice), here for the host's marked rows.
+struct WorkerSpliceH {
+  uint32_t n_old = 0, n_new = 0;
+  std::vector<uint32_t> removed, before;
+  WorkerSpliceH(uint32_t n, std::vector<uint32_t> rm, std::vector<uint32_t> bf)
+      : n_old(n), n_new(n - (uint32_t)rm.size() + (uint32_t)bf.size()), removed(std::move(rm)), before(std::move(bf)) {}
+  uint32_t rm_below(uint32_t x) const { return (uint32_t)(std::lower_bound(removed.begin(), removed.end(), x) - removed.begin()); }
+  bool is_removed(uint32_t i) const { return std::binary_search(removed.begin(), removed.end(), i); }
+  // the new index of kept old row i
+  uint32_t map(uint32_t i) const {
+    return i - rm_below(i) + (uint32_t)(std::upper_bound(before.begin(), before.end(), i) - before.begin());
+  }
+  // the new index of inserted row k
+  uint32_t at(uint32_t k) const { return before[k] - rm_below(before[k]) + k; }
+  // the new index of the boundary in front of old row x, ahead of the rows inserted before x: the new rows below it are
+  // the kept rows below x and the rows inserted before a position < x
+  uint32_t edge(uint32_t x) const {
+    return x - rm_below(x) + (uint32_t)(std::lower_bound(before.begin(), before.end(), x) - before.begin());
+  }
+  // a list of rows renamed, the removed ones dropped (and their marks cleared)
+  void apply_list(std::vector<uint32_t>* list, std::vector<uint8_t>* mark) const {
+    size_t k = 0;
+    for (uint32_t i : *list) {
+      (*mark)[i] = 0;
+      if (!is_removed(i)) (*list)[k++] = map(i);
+    }
+    list->resize(k);
+  }
+};
+
+// The checks of pm_remove_workers, on the host before anything changes: the distinct indices, increasing
+static int check_remove_workers(const pm_engine* e, const uint32_t* idx, uint32_t n, std::vector<uint32_t>* removed, std::string* err) {
+  if (n && !idx) { *err = "pm_remove_workers: null"; return PM_E_INVALID; }
+  removed->assign(idx, idx + n);
+  for (uint32_t i : *removed)
+    if (i >= e->n_workers) { *err = "pm_remove_workers: worker index out of range"; return PM_E_INVALID; }
+  std::sort(removed->begin(), removed->end());
+  removed->erase(std::unique(removed->begin(), removed->end()), removed->end());
+  return PM_OK;
+}
+
+// The checks of pm_insert_workers: the pointers, the positions and the table size (it stays below PM_NONE rows)
+static int check_insert_workers(const pm_engine* e, const uint32_t* before, const pm_worker_a* a, const pm_worker_b* b,
+                                const double* lat, const double* lon, uint32_t n, std::string* err) {
+  if ((n && (!before || !a || !b)) || ((lat == nullptr) != (lon == nullptr))) { *err = "pm_insert_workers: null"; return PM_E_INVALID; }
+  if ((uint64_t)e->n_workers + n >= PM_NONE) { *err = "pm_insert_workers: the table would reach PM_NONE rows"; return PM_E_INVALID; }
+  for (uint32_t i = 0; i < n; ++i)
+    if (before[i] > e->n_workers || (i && before[i] < before[i - 1])) {
+      *err = "pm_insert_workers: before[] decreases or exceeds n_workers";
+      return PM_E_INVALID;
+    }
+  return PM_OK;
+}
+
+// The part of pm_remove_workers / pm_insert_workers after their checks.  One launch of pm_splice_workers moves every
+// per-row column into its second buffer (the planes, location, address rank, reputation, the worker-major acceptance
+// words while they hold, the stored first ask, the stored auction price and owner), the buffers are swapped, and one
+// launch of pm_splice_worker_holds renames the stored assignment in place.  The host marks (dirty_rows, auc_rows) move
+// with their rows.  Nothing else outlives a pass keyed by worker index: the cost tile's held-sentinel maps describe
+// the tile buffer's contents, whatever rows they came from, and the auction's class caches, pools and sorted worker
+// copy are rebuilt by every pass.
+static int splice_workers(pm_engine* e, const WorkerSpliceH& sp, const pm_worker_a* a, const pm_worker_b* b,
+                          const double* lat, const double* lon) {
+  PM_CUDA(cudaSetDevice(e->device));
+  const uint32_t n_old = sp.n_old, n_new = sp.n_new, nr = (uint32_t)sp.removed.size(), ni = (uint32_t)sp.before.size();
+  uint32_t a0 = 0, na = 0;   // the range before the splice
+  e->shard(&a0, &na);
+  const uint32_t a1 = (uint32_t)std::min<uint64_t>((uint64_t)a0 + na, n_old);
+  PM_CUDA(e->wsplice_dev.ensure(std::max<size_t>((size_t)nr + ni, 1)));
+  const uint32_t* rm_dev = e->wsplice_dev.p;
+  const uint32_t* bf_dev = e->wsplice_dev.p + nr;
+  if (nr) PM_CUDA(cudaMemcpyAsync(e->wsplice_dev.p, sp.removed.data(), (size_t)nr * 4, cudaMemcpyHostToDevice, e->stream));
+  if (ni) {
+    PM_CUDA(cudaMemcpyAsync(e->wsplice_dev.p + nr, sp.before.data(), (size_t)ni * 4, cudaMemcpyHostToDevice, e->stream));
+    PM_CUDA(e->upd_a.ensure(ni)); PM_CUDA(e->upd_b.ensure(ni));
+    PM_CUDA(cudaMemcpyAsync(e->upd_a.p, a, (size_t)ni * 16, cudaMemcpyHostToDevice, e->stream));
+    PM_CUDA(cudaMemcpyAsync(e->upd_b.p, b, (size_t)ni * 16, cudaMemcpyHostToDevice, e->stream));
+    if (lat) {
+      PM_CUDA(e->upd_lat.ensure(ni)); PM_CUDA(e->upd_lon.ensure(ni));
+      PM_CUDA(cudaMemcpyAsync(e->upd_lat.p, lat, (size_t)ni * 8, cudaMemcpyHostToDevice, e->stream));
+      PM_CUDA(cudaMemcpyAsync(e->upd_lon.p, lon, (size_t)ni * 8, cudaMemcpyHostToDevice, e->stream));
+    }
+  }
+  if (lat && ni && !e->have_loc) {   // the first coordinates: every other row at (0, 0), as pm_update_workers does
+    PM_CUDA(e->lat.ensure(e->wa.n)); PM_CUDA(e->lon.ensure(e->wa.n));
+    PM_CUDA(cudaMemsetAsync(e->lat.p, 0, e->wa.n * 8, e->stream));
+    PM_CUDA(cudaMemsetAsync(e->lon.p, 0, e->wa.n * 8, e->stream));
+    e->have_loc = true;
+  }
+  const bool move_nacc = e->eval_valid && e->nacc_base;   // nacc holds every row outside dirty_rows
+  const bool move_auc = e->auc_state;
+  const uint32_t auc_kept = std::min(e->auc_kept, n_old);
+  // the range after the splice (a communicator's share and an open-ended pm_set_shard range move with W)
+  e->n_workers = n_new;
+  uint32_t b0 = 0, nb = 0;
+  e->shard(&b0, &nb);
+  const uint32_t b1 = (uint32_t)std::min<uint64_t>((uint64_t)b0 + nb, n_new);
+  // the second buffers, with room to grow
+  const size_t want = std::max<size_t>(n_new, 1);
+  auto room = [&](auto& buf, size_t need) -> cudaError_t { return buf.p && buf.n >= need ? cudaSuccess : buf.ensure(need + need / 8); };
+  PM_CUDA(room(e->wa_alt, want)); PM_CUDA(room(e->wb_alt, want));
+  if (e->have_loc) { PM_CUDA(room(e->lat_alt, want)); PM_CUDA(room(e->lon_alt, want)); }
+  if (e->have_rank) PM_CUDA(room(e->rank_alt, want));
+  if (e->have_rep) PM_CUDA(room(e->rep_alt, want));
+  if (move_nacc) PM_CUDA(room(e->nacc_alt, want));
+  if (e->eval_valid) PM_CUDA(room(e->first_alt, want));
+  if (move_auc) { PM_CUDA(room(e->price_alt, want + 2)); PM_CUDA(room(e->owner_alt, want)); }
+  pm::WorkerSplice s{};
+  s.removed = rm_dev; s.before = bf_dev; s.nr = nr; s.ni = ni; s.n_old = n_old;
+  s.wa = e->wa.p; s.wb = e->wb.p; s.ins_a = e->upd_a.p; s.ins_b = e->upd_b.p; s.wa_out = e->wa_alt.p; s.wb_out = e->wb_alt.p;
+  if (e->have_loc) {
+    s.lat = e->lat.p; s.lon = e->lon.p; s.lat_out = e->lat_alt.p; s.lon_out = e->lon_alt.p;
+    s.ins_lat = lat ? e->upd_lat.p : nullptr; s.ins_lon = lat ? e->upd_lon.p : nullptr;
+  }
+  if (e->have_rank) { s.rank = e->addr_rank.p; s.rank_out = e->rank_alt.p; }
+  if (e->have_rep) { s.rep = e->reputation.p; s.rep_out = e->rep_alt.p; }
+  if (move_nacc) { s.nacc = e->nacc.p; s.nacc_out = e->nacc_alt.p; s.nacc_n = (uint32_t)std::min<size_t>(e->nacc.n, n_old); }
+  if (e->eval_valid) { s.first = e->eval_first.p; s.first_out = e->first_alt.p; s.a0 = a0; s.a1 = std::max(a0, a1); s.b0 = b0; s.b1 = std::max(b0, b1); }
+  if (move_auc) { s.price = e->auc_price.p; s.price_out = e->price_alt.p; s.owner = e->auc_owner.p; s.owner_out = e->owner_alt.p; s.auc_kept = auc_kept; }
+  if (n_old + ni) {
+    pm::pm_splice_workers<<<std::min(blocks_for((size_t)n_old + ni, 256), 8u * e->sms), 256, 0, e->stream>>>(s);
+    PM_LAUNCH_CHECK("pm_splice_workers");
+  }
+  std::swap(e->wa, e->wa_alt); std::swap(e->wb, e->wb_alt);
+  if (e->have_loc) { std::swap(e->lat, e->lat_alt); std::swap(e->lon, e->lon_alt); }
+  if (e->have_rank) std::swap(e->addr_rank, e->rank_alt);
+  if (e->have_rep) std::swap(e->reputation, e->rep_alt);
+  if (move_nacc) std::swap(e->nacc, e->nacc_alt);
+  if (e->eval_valid) std::swap(e->eval_first, e->first_alt);
+  if (move_auc) {
+    std::swap(e->auc_price, e->price_alt); std::swap(e->auc_owner, e->owner_alt);
+    PM_CUDA(cudaMemsetAsync(e->auc_price.p + n_new, 0, 2 * 8, e->stream));
+    const uint32_t D = e->n_slots();
+    if (D) {
+      pm::pm_splice_worker_holds<<<std::min(blocks_for(D, 256), 8u * e->sms), 256, 0, e->stream>>>(e->auc_assigned.p, D, rm_dev, nr, bf_dev,
+                                                                                                  ni, auc_kept);
+      PM_LAUNCH_CHECK("pm_splice_worker_holds");
+    }
+  }
+  // the caller's arrays and the host vectors behind the staging copies are released once the copies are done
+  PM_CUDA(cudaStreamSynchronize(e->stream));
+  if (e->eval_valid) {
+    // The written rows move with their rows.  Rows that enter the range (their old row was outside it, or they are
+    // inserted) count as written; the rest of [L, U) are kept rows of the old range.  Inserted rows are written
+    // wherever they lie, for the preludes.
+    sp.apply_list(&e->dirty_rows, &e->dirty_mark);
+    e->dirty_mark.assign(n_new, 0);
+    for (uint32_t i : e->dirty_rows) e->dirty_mark[i] = 1;
+    e->dirty_in = 0;
+    for (uint32_t i : e->dirty_rows) e->dirty_in += e->in_range(i);
+    if (e->dirty_in > e->tune_incr) e->mark_all_dirty();
+    uint32_t lo = a0, hi = a1;   // the first and one past the last kept row of the old range
+    while (lo < hi && sp.is_removed(lo)) ++lo;
+    while (hi > lo && sp.is_removed(hi - 1)) --hi;
+    const uint32_t L = lo < hi ? sp.map(lo) : n_new, U = lo < hi ? sp.map(hi - 1) + 1 : n_new;
+    if (std::min(b1, L) > b0) e->mark_range_dirty(b0, std::min(b1, L) - b0);
+    if (b1 > std::max(b0, U)) e->mark_range_dirty(std::max(b0, U), b1 - std::max(b0, U));
+    for (uint32_t k = 0; k < ni; ++k) e->mark_dirty(sp.at(k));
+  }
+  if (move_auc) {
+    // Rows below the new auc_kept are the kept rows below the old one and the rows inserted before them (listed, as
+    // changed rows); every row from it on is the old range past auc_kept, and the rows inserted there.
+    sp.apply_list(&e->auc_rows, &e->auc_row_mark);
+    e->auc_kept = sp.edge(auc_kept);
+    e->auc_state_w = n_new;
+    e->auc_row_mark.assign(n_new, 0);
+    for (uint32_t i : e->auc_rows) e->auc_row_mark[i] = 1;
+    for (uint32_t k = 0; k < ni && sp.before[k] < auc_kept; ++k) e->auc_mark_row(sp.at(k));
+    e->auc_workers_spliced = true;
+  }
+  e->workers_checked = false;
+  e->nacc_valid = false;
+  e->matched = e->local_done = false;
+  return PM_OK;
+}
+
+// A failure after the checks (a CUDA error, a host exception) leaves tables that are not trusted: the worker table is
+// dropped with the stored evaluation and auction state, and the next call that needs it is PM_E_STATE
+static int worker_splice(pm_engine* e, const WorkerSpliceH& sp, const pm_worker_a* a, const pm_worker_b* b,
+                         const double* lat, const double* lon) {
+  int rc;
+  try {
+    rc = splice_workers(e, sp, a, b, lat, lon);
+  } catch (...) {
+    rc = pm_guard_rc();
+    e->err = "worker table splice: host exception (the worker table was dropped)";
+  }
+  if (rc != PM_OK) {
+    e->have_workers = false;
+    e->invalidate_eval();
+    e->auc_discard();
+  }
+  return rc;
+}
+
+int pm_remove_workers(pm_engine* e, const uint32_t* idx, uint32_t n) try {
+  if (!e) return PM_E_INVALID;
+  std::lock_guard<std::mutex> lk(e->mu);
+  if (!e->have_workers) return e->fail(PM_E_STATE, "pm_remove_workers: no worker table");
+  std::vector<uint32_t> removed;
+  {
+    std::string err;
+    const int rc = check_remove_workers(e, idx, n, &removed, &err);
+    if (rc != PM_OK) return e->fail((pm_status)rc, err);
+  }
+  if (removed.empty()) return PM_OK;
+  ++e->table_version;
+  return worker_splice(e, WorkerSpliceH(e->n_workers, std::move(removed), {}), nullptr, nullptr, nullptr, nullptr);
+} catch (...) { return pm_guard_rc(); }
+
+int pm_insert_workers(pm_engine* e, const uint32_t* before, const pm_worker_a* a, const pm_worker_b* b, const double* lat,
+                      const double* lon, uint32_t n) try {
+  if (!e) return PM_E_INVALID;
+  std::lock_guard<std::mutex> lk(e->mu);
+  if (!e->have_workers) return e->fail(PM_E_STATE, "pm_insert_workers: no worker table");
+  {
+    std::string err;
+    const int rc = check_insert_workers(e, before, a, b, lat, lon, n, &err);
+    if (rc != PM_OK) return e->fail((pm_status)rc, err);
+  }
+  if (n == 0) return PM_OK;
+  ++e->table_version;
+  return worker_splice(e, WorkerSpliceH(e->n_workers, {}, std::vector<uint32_t>(before, before + n)), a, b, lat, lon);
 } catch (...) { return pm_guard_rc(); }
 
 uint64_t pm_table_version(const pm_engine* e) { return e ? e->table_version : 0; }
@@ -3178,6 +3420,8 @@ int pm_auction_certificate(pm_engine* e, pm_auction_cert* out, int64_t* ask_boun
   const uint32_t W = e->n_workers, T = e->n_asks;
   if (W != e->auc_state_w) return e->fail(PM_E_STATE, "pm_auction_certificate: the worker table was resized since the last auction pass");
   if (e->auc_asks_resized) return e->fail(PM_E_STATE, "pm_auction_certificate: the ask table was resized since the last auction pass");
+  if (e->auc_workers_spliced)
+    return e->fail(PM_E_STATE, "pm_auction_certificate: workers were removed or inserted since the last auction pass");
   if (e->max_pattern_row > e->n_patterns || (e->max_pattern_row && !e->have_bits))
     return e->fail(PM_E_STATE, "pm_auction_certificate: an ask references a model pattern missing from the model table");
   if (e->n_off) return e->fail(PM_E_UNSUPPORTED, "pm_auction_certificate: disabled asks");
@@ -3223,6 +3467,13 @@ int pm_auction_certificate(pm_engine* e, pm_auction_cert* out, int64_t* ask_boun
   return PM_OK;
 } catch (...) { return pm_guard_rc(); }
 
+// After a worker splice the stored assignment marks a hold on a removed row kCutHold (pm_splice_worker_holds): it
+// is released by the next warm pass, and exported as PM_NONE
+static void cut_holds_read_none(uint32_t* assigned, uint32_t n) {
+  for (uint32_t s = 0; s < n; ++s)
+    if (assigned[s] == pm::kCutHold) assigned[s] = PM_NONE;
+}
+
 // The stored state's assignment over the current asks (remapped by pm_update_asks / pm_resize_asks like the state itself)
 int pm_auction_assignment(pm_engine* e, uint32_t* assigned) try {
   if (!e) return PM_E_INVALID;
@@ -3234,6 +3485,7 @@ int pm_auction_assignment(pm_engine* e, uint32_t* assigned) try {
   if (e->n_asks) {
     PM_CUDA(cudaMemcpyAsync(assigned, e->auc_assigned.p, (size_t)e->n_asks * 4, cudaMemcpyDeviceToHost, e->stream));
     PM_CUDA(cudaStreamSynchronize(e->stream));
+    if (e->auc_workers_spliced) cut_holds_read_none(assigned, e->n_asks);
   }
   return PM_OK;
 } catch (...) { return pm_guard_rc(); }
@@ -3259,6 +3511,7 @@ int pm_auction_slot_assignment(pm_engine* e, uint32_t* assigned, uint32_t* n_slo
   if (D) {
     PM_CUDA(cudaMemcpyAsync(assigned, e->auc_assigned.p, (size_t)D * 4, cudaMemcpyDeviceToHost, e->stream));
     PM_CUDA(cudaStreamSynchronize(e->stream));
+    if (e->auc_workers_spliced) cut_holds_read_none(assigned, D);
   }
   return PM_OK;
 } catch (...) { return pm_guard_rc(); }
@@ -3916,6 +4169,31 @@ int pm_multi_resize_workers(pm_multi* m, uint32_t n_workers) try {
 int pm_multi_update_workers(pm_multi* m, const uint32_t* idx, const pm_worker_a* a, const pm_worker_b* b, const double* lat,
                             const double* lon, uint32_t n) try {
   PM_MULTI_EACH(pm_update_workers(e, idx, a, b, lat, lon, n));
+} catch (...) { return pm_guard_rc(); }
+// the replicated tables agree, so device 0's checks decide for all of them: a refused call changes no device
+int pm_multi_remove_workers(pm_multi* m, const uint32_t* idx, uint32_t n) try {
+  if (m && !m->engines.empty()) {
+    pm_engine* e0 = m->engines[0];
+    std::lock_guard<std::mutex> lk(e0->mu);
+    std::vector<uint32_t> removed;
+    if (e0->have_workers) {
+      const int rc = check_remove_workers(e0, idx, n, &removed, &m->err);
+      if (rc != PM_OK) return rc;
+    }
+  }
+  PM_MULTI_EACH(pm_remove_workers(e, idx, n));
+} catch (...) { return pm_guard_rc(); }
+int pm_multi_insert_workers(pm_multi* m, const uint32_t* before, const pm_worker_a* a, const pm_worker_b* b, const double* lat,
+                            const double* lon, uint32_t n) try {
+  if (m && !m->engines.empty()) {
+    pm_engine* e0 = m->engines[0];
+    std::lock_guard<std::mutex> lk(e0->mu);
+    if (e0->have_workers) {
+      const int rc = check_insert_workers(e0, before, a, b, lat, lon, n, &m->err);
+      if (rc != PM_OK) return rc;
+    }
+  }
+  PM_MULTI_EACH(pm_insert_workers(e, before, a, b, lat, lon, n));
 } catch (...) { return pm_guard_rc(); }
 int pm_multi_sync(pm_multi* m) try {
   PM_MULTI_EACH(pm_stream_sync(e));

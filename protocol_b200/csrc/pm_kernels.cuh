@@ -1633,6 +1633,113 @@ __global__ void pm_scatter_rows(uint4* wa, uint4* wb, double* lat, double* lon, 
   if (lat) { lat[w] = la[i]; lon[w] = lo[i]; }
 }
 
+// ---- worker-table splice (pm_remove_workers / pm_insert_workers) ------------------------------------------------
+// `removed`: old rows, increasing and distinct (nr); `before`: per inserted row the old row it goes before,
+// non-decreasing (ni).  Kept old row i goes to i - |{r < i}| + |{before <= i}|; inserted row k to
+// before[k] - |{r < before[k]}| + k.
+struct WorkerSplice {
+  const uint32_t* removed;
+  const uint32_t* before;
+  uint32_t nr, ni, n_old;
+  // every column is moved from its old buffer into the second one of its pair; a null column is not in use
+  const uint4 *wa, *wb, *ins_a, *ins_b;
+  uint4 *wa_out, *wb_out;
+  const double *lat, *lon, *ins_lat, *ins_lon;   // ins_lat null: inserted rows at (0, 0)
+  double *lat_out, *lon_out;
+  const uint32_t *rank, *rep;
+  uint32_t *rank_out, *rep_out;
+  // the worker-major acceptance words: old rows below nacc_n hold them; inserted rows are listed as written
+  const uint32_t* nacc;
+  uint32_t* nacc_out;
+  uint32_t nacc_n;
+  // the stored evaluation: kept where the old row was in [a0, a1) and the new one is in [b0, b1), else PM_NONE
+  const uint32_t* first;
+  uint32_t* first_out;
+  uint32_t a0, a1, b0, b1;
+  // the stored auction state: old rows below auc_kept keep price and owner, every other row is 0 / unowned
+  const long long* price;
+  long long* price_out;
+  const uint32_t* owner;
+  uint32_t* owner_out;
+  uint32_t auc_kept;
+};
+__device__ __forceinline__ uint32_t splice_lower(const uint32_t* __restrict__ v, uint32_t n, uint32_t x) {
+  uint32_t lo = 0, hi = n;   // entries < x
+  while (lo < hi) {
+    const uint32_t mid = (lo + hi) >> 1;
+    if (__ldg(v + mid) < x) lo = mid + 1; else hi = mid;
+  }
+  return lo;
+}
+__device__ __forceinline__ uint32_t splice_upper(const uint32_t* __restrict__ v, uint32_t n, uint32_t x) {
+  uint32_t lo = 0, hi = n;   // entries <= x
+  while (lo < hi) {
+    const uint32_t mid = (lo + hi) >> 1;
+    if (__ldg(v + mid) <= x) lo = mid + 1; else hi = mid;
+  }
+  return lo;
+}
+// One thread per old row and per inserted row: every output row is written exactly once (the destinations of the
+// kept and inserted rows are disjoint and cover [0, n_old - nr + ni)), in increasing order along the grid, so the
+// stores stay coalesced.
+__global__ void pm_splice_workers(WorkerSplice s) {
+  const uint32_t n = s.n_old + s.ni;
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    if (i < s.n_old) {
+      const uint32_t r = splice_lower(s.removed, s.nr, i);
+      if (r < s.nr && __ldg(s.removed + r) == i) continue;
+      const uint32_t j = i - r + splice_upper(s.before, s.ni, i);
+      s.wa_out[j] = s.wa[i];
+      s.wb_out[j] = s.wb[i];
+      if (s.lat_out) { s.lat_out[j] = s.lat[i]; s.lon_out[j] = s.lon[i]; }
+      if (s.rank_out) s.rank_out[j] = s.rank[i];
+      if (s.rep_out) s.rep_out[j] = s.rep[i];
+      if (s.nacc_out) s.nacc_out[j] = i < s.nacc_n ? s.nacc[i] : 0u;
+      if (s.first_out)
+        s.first_out[j] = (i - s.a0 < s.a1 - s.a0 && j - s.b0 < s.b1 - s.b0) ? s.first[i] : kNone;
+      if (s.price_out) {
+        const bool kept = i < s.auc_kept;
+        s.price_out[j] = kept ? s.price[i] : 0ll;
+        s.owner_out[j] = kept ? s.owner[i] : kNone;
+      }
+    } else {
+      const uint32_t k = i - s.n_old, b = __ldg(s.before + k);
+      const uint32_t j = b - splice_lower(s.removed, s.nr, b) + k;
+      s.wa_out[j] = s.ins_a[k];
+      s.wb_out[j] = s.ins_b[k];
+      if (s.lat_out) {
+        s.lat_out[j] = s.ins_lat ? s.ins_lat[k] : 0.0;
+        s.lon_out[j] = s.ins_lat ? s.ins_lon[k] : 0.0;
+      }
+      if (s.rank_out) s.rank_out[j] = 0u;
+      if (s.rep_out) s.rep_out[j] = 0u;
+      if (s.nacc_out) s.nacc_out[j] = 0u;
+      if (s.first_out) s.first_out[j] = kNone;
+      if (s.price_out) {
+        s.price_out[j] = 0ll;
+        s.owner_out[j] = kNone;
+      }
+    }
+  }
+}
+// The stored auction assignment under a worker splice, in place (one entry per slot): a kept row's hold moves to its
+// new index; a hold on a removed row, or on a row at or past auc_kept (cut off by an earlier shrink), becomes
+// kCutHold, which the next warm pass releases in its step 1 as it releases the holder of a row a shrink cut off.
+constexpr uint32_t kCutHold = 0xFFFFFFFEu;
+__global__ void pm_splice_worker_holds(uint32_t* __restrict__ assigned, uint32_t n_slots, const uint32_t* __restrict__ removed,
+                                       uint32_t nr, const uint32_t* __restrict__ before, uint32_t ni, uint32_t auc_kept) {
+  for (uint32_t s = blockIdx.x * blockDim.x + threadIdx.x; s < n_slots; s += gridDim.x * blockDim.x) {
+    const uint32_t w = assigned[s];
+    if (w == kNone) continue;
+    if (w >= auc_kept) {
+      assigned[s] = kCutHold;
+      continue;
+    }
+    const uint32_t r = splice_lower(removed, nr, w);
+    assigned[s] = (r < nr && __ldg(removed + r) == w) ? kCutHold : w - r + splice_upper(before, ni, w);
+  }
+}
+
 // Do all workers satisfy the fast-path operand limits (values < 2^31, gpu count < 2^16,
 // count * memory_mb < 2^31 without wrapping)?  Clears ok[0] otherwise.  Is every price below
 // kNarrowInfeasible, so that the 32-bit cost tile can hold it?  Clears ok[1] otherwise.

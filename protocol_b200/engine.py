@@ -228,6 +228,26 @@ class Engine:
                                                 _ptr(lo) if lo is not None else None, len(idx)))
         self.sync()
 
+    def remove_workers(self, idx):
+        """Remove the worker rows idx (any order; a repeated index removes its row once); the rows after them move up,
+        order kept (pm_remove_workers).  The stored evaluation and auction state are kept, remapped to the new indices."""
+        idx = _remove_args(idx)
+        self._check(self._lib.pm_remove_workers(self._h, _ptr(idx) if len(idx) else None, len(idx)))
+        self.n_workers -= len(np.unique(idx))
+        if self._auction_workers:   # the stored auction state follows the splice: one price per current row
+            self._auction_workers = self.n_workers
+
+    def insert_workers(self, before, a, b, lat=None, lon=None):
+        """Insert rows a[i], b[i] before the current rows before[i] (non-decreasing, n_workers = append; rows with equal
+        before[] keep their order), at (lat, lon) or (0, 0), address rank 0 and reputation 0 (pm_insert_workers)."""
+        before, a, b, la, lo = _worker_insert_args(before, a, b, lat, lon)
+        self._check(self._lib.pm_insert_workers(self._h, _ptr(before) if len(before) else None, _ptr(a) if len(a) else None,
+                                                _ptr(b) if len(b) else None, _ptr(la) if la is not None else None,
+                                                _ptr(lo) if lo is not None else None, len(before)))
+        self.n_workers += len(before)
+        if self._auction_workers:
+            self._auction_workers = self.n_workers
+
     def table_version(self) -> int:
         return int(self._lib.pm_table_version(self._h))
 
@@ -412,6 +432,21 @@ def _remove_args(idx):
     return np.ascontiguousarray(np.atleast_1d(np.asarray(idx, dtype=np.int64)).astype(np.uint32))
 
 
+def _worker_insert_args(before, a, b, lat, lon):
+    """(before, a, b, lat, lon) as pm_insert_workers takes them: one row per position (the call reads len(before) rows);
+    lat / lon None or one value per row."""
+    before = np.ascontiguousarray(np.atleast_1d(np.asarray(before, dtype=np.int64)).astype(np.uint32))
+    a = np.ascontiguousarray(np.atleast_1d(a), dtype=abi.WORKER_A)
+    b = np.ascontiguousarray(np.atleast_1d(b), dtype=abi.WORKER_B)
+    la = np.ascontiguousarray(np.atleast_1d(lat), dtype=np.float64) if lat is not None else None
+    lo = np.ascontiguousarray(np.atleast_1d(lon), dtype=np.float64) if lon is not None else None
+    if len(a) != len(before) or len(b) != len(before):
+        raise ValueError(f"insert_workers: {len(before)} positions for {len(a)} / {len(b)} rows")
+    if (la is not None and len(la) != len(before)) or (lo is not None and len(lo) != len(before)):
+        raise ValueError("insert_workers: lat / lon need one value per inserted row")
+    return before, a, b, la, lo
+
+
 def _result_views(r: "abi.PmResult", copy: bool) -> MatchResult:
     def view(ptr, n, dt):
         if n == 0:
@@ -568,6 +603,19 @@ class MultiEngine:
                                                       _ptr(la) if la is not None else None,
                                                       _ptr(lo) if lo is not None else None, len(idx)))
         self._check(self._lib.pm_multi_sync(self._h))
+
+    def remove_workers(self, idx):
+        """pm_multi_remove_workers: Engine.remove_workers on every device."""
+        idx = _remove_args(idx)
+        self._check(self._lib.pm_multi_remove_workers(self._h, _ptr(idx) if len(idx) else None, len(idx)))
+
+    def insert_workers(self, before, a, b, lat=None, lon=None):
+        """pm_multi_insert_workers: Engine.insert_workers on every device."""
+        before, a, b, la, lo = _worker_insert_args(before, a, b, lat, lon)
+        self._check(self._lib.pm_multi_insert_workers(self._h, _ptr(before) if len(before) else None,
+                                                      _ptr(a) if len(a) else None, _ptr(b) if len(b) else None,
+                                                      _ptr(la) if la is not None else None,
+                                                      _ptr(lo) if lo is not None else None, len(before)))
 
     def table_version(self) -> int:
         """Changes whenever a table call changed a table on any device (pm_multi_table_version)."""

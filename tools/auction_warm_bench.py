@@ -23,7 +23,15 @@ pass and a warm repair, each after a cold pass of the tables before the change, 
 each is also taken the way without the splices: pm_set_asks of the current rows, the caps, pm_auction_restore_slots of
 the remapped export (the restore audit), then the same pass from the restored state.
 
-    python tools/auction_warm_bench.py [--repair | --asks | --splice] [--out results/auction_warm.json]
+--worker-splice: worker rows removed and inserted anywhere in the table (pm_remove_workers / pm_insert_workers):
+remove 1, 100 and 1 000 held workers at scattered positions, insert 1, 100 and 1 000 rows (copies of other rows) at
+random positions.  Each runs as a warm pass and a warm repair, each after a reload and a cold pass of the tables
+before the change, with the calls timed.  For comparison each is also taken the way without the splices: the export
+before the change (pm_auction_state, pm_auction_assignment), the indices remapped on the host, pm_set_worker_count +
+the upload of the current rows, pm_auction_restore of the remapped state, then the same pass; `same_as_splice` says
+whether that pass gave the same assignment and rounds.
+
+    python tools/auction_warm_bench.py [--repair | --asks | --splice | --worker-splice] [--out results/auction_warm.json]
 """
 from __future__ import annotations
 
@@ -179,6 +187,60 @@ def splice_series(eng, a, cap, record):
         asks, cap = new_asks, new_cap
 
 
+def worker_splice_series(eng, wa, wb, record):
+    """--worker-splice: held workers removed at scattered positions and rows inserted at random positions, each change
+    set as a warm pass and a warm repair, then the same change taken by export + host remap + reload + restore."""
+    rng = np.random.default_rng(5)
+    wa, wb = wa.copy(), wb.copy()
+    warm = abi.PM_MODE_AUCTION | abi.PM_AUCTION_WARM
+    for case, n in (("remove", 1), ("remove", 100), ("remove", 1000), ("insert", 1), ("insert", 100), ("insert", 1000)):
+        for name, mode in (("warm", warm), ("repair", warm | abi.PM_AUCTION_REPAIR)):
+            eng.set_workers(wa, wb)                    # the tables before the change, and a cold pass of them
+            eng.match(abi.PM_MODE_AUCTION)
+            W, T = len(wa), eng.n_asks
+            t0 = time.perf_counter()                   # the export the way without the splices starts from
+            price0, _, _ = eng.auction_state()
+            assigned0 = eng.auction_assignment()
+            export_ms = (time.perf_counter() - t0) * 1e3
+            held = assigned0 != NONE
+            if case == "remove":
+                idx = np.sort(rng.choice(assigned0[held], n, replace=False)).astype(np.uint32)
+                t0 = time.perf_counter()
+                eng.remove_workers(idx)
+                eng.sync()
+                i = idx.astype(np.int64)
+                new_wa, new_wb = np.delete(wa, i), np.delete(wb, i)
+            else:
+                before = np.sort(rng.integers(0, W + 1, n)).astype(np.uint32)
+                src = rng.integers(0, W, n)
+                t0 = time.perf_counter()
+                eng.insert_workers(before, wa[src], wb[src])
+                eng.sync()
+                b = before.astype(np.int64)
+                new_wa, new_wb = np.insert(wa, b, wa[src]), np.insert(wb, b, wb[src])
+            call_ms = round((time.perf_counter() - t0) * 1e3, 2)
+            r = timed(eng, mode)
+            got = assigned_of(eng, T)
+            record(f"{name}_worker_{case}", n, dict(r, call_ms=call_ms))
+            t0 = time.perf_counter()                   # the way without the splices
+            a = assigned0.astype(np.int64)
+            if case == "remove":
+                gone = held & np.isin(a, i)
+                price = np.delete(price0, i)
+                a = np.where(held & ~gone, a - np.searchsorted(i, a), NONE)
+            else:
+                price = np.insert(price0, b, 0)
+                a = np.where(held, a + np.searchsorted(b, a, "right"), NONE)
+            eng.set_workers(new_wa, new_wb)
+            eng.auction_restore(price, a.astype(np.uint32))
+            eng.sync()
+            restore_ms = round(export_ms + (time.perf_counter() - t0) * 1e3, 2)
+            q = timed(eng, mode)
+            same = bool(np.array_equal(assigned_of(eng, T), got) and q["rounds"] == r["rounds"])
+            record(f"reload_restore_{name}_worker_{case}", n, dict(q, call_ms=restore_ms, same_as_splice=same))
+        wa, wb = new_wa, new_wb
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", default=None)
@@ -186,6 +248,8 @@ def main():
     ap.add_argument("--repair", action="store_true", help="also run PM_AUCTION_REPAIR on every change set")
     ap.add_argument("--asks", action="store_true", help="ask-table change sets (pm_update_asks / pm_resize_asks)")
     ap.add_argument("--splice", action="store_true", help="asks removed and inserted anywhere (pm_remove_asks / pm_insert_asks)")
+    ap.add_argument("--worker-splice", dest="worker_splice", action="store_true",
+                    help="workers removed and inserted anywhere (pm_remove_workers / pm_insert_workers)")
     args = ap.parse_args()
     gpu = card()
     print(f"card: {gpu}", file=sys.stderr)
@@ -203,9 +267,12 @@ def main():
         rows.append(r)
         print(json.dumps(r), flush=True)
 
-    if args.asks or args.splice:
+    if args.asks or args.splice or args.worker_splice:
         record("cold", 0, timed(eng, abi.PM_MODE_AUCTION))
-        (splice_series if args.splice else ask_series)(eng, a, cap, record)
+        if args.worker_splice:
+            worker_splice_series(eng, wa, wb, record)
+        else:
+            (splice_series if args.splice else ask_series)(eng, a, cap, record)
         eng.close()
         if args.out:
             os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)

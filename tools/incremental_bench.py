@@ -37,7 +37,16 @@ every s in S, after a full fused lean pass that refreshes the stored evaluation:
 at scattered positions, one PM_INCREMENTAL lean pass runs; then s rows (copies of the table's rows, with only their own
 option rows) are inserted at random priorities and one more runs.  Each call is timed on the host clock around the call
 and a synchronise.  For comparison a sibling engine takes the way without the splices, pm_set_asks of the current rows
-and a full lean pass (timed together, `route`), and its result is checked equal to the incremental one."""
+and a full lean pass (timed together, `route`), and its result is checked equal to the incremental one.
+
+    python tools/incremental_bench.py --worker-splice [...]
+
+Worker rows removed and inserted anywhere in the table (pm_remove_workers / pm_insert_workers) between passes.  Per
+round and for every s in S, after a full fused lean pass that refreshes the stored evaluation: s rows are removed at
+scattered positions and one PM_INCREMENTAL lean pass runs; then s rows (copies of other nodes' rows) are inserted at
+random positions and one more runs.  Each call is timed on the host clock around the call and a synchronise.  For
+comparison a sibling engine takes the way without the splices, pm_set_worker_count + pm_upsert_workers of the current
+rows and a full lean pass (timed together, `route`), and its result is checked equal to the incremental one."""
 from __future__ import annotations
 
 import argparse
@@ -323,6 +332,8 @@ def main():
                     help="asks replaced between passes (pm_update_asks) instead of rows written; also times the call")
     ap.add_argument("--splice", action="store_true",
                     help="asks removed and inserted anywhere between passes (pm_remove_asks / pm_insert_asks)")
+    ap.add_argument("--worker-splice", dest="worker_splice", action="store_true",
+                    help="worker rows removed and inserted anywhere between passes (pm_remove_workers / pm_insert_workers)")
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
 
@@ -340,6 +351,14 @@ def main():
         env = card()
         rows, checked, workload = splice_series(args, w, a, bits, npat, nmod, words)
         report(rows, checked, workload, env, "case", args.out, "incremental_splice_bench.json")
+        return
+    if args.worker_splice:
+        a = synth.make_asks(args.asks, "mixed")
+        bits, npat, nmod, words = synth.intern_tables(w, a)
+        env = card()
+        pool = synth.make_workers(200_000, seed=synth.SEED_WORKERS + 101)
+        rows, checked, workload = worker_splice_series(args, w, a, bits, npat, nmod, words, pool)
+        report(rows, checked, workload, env, "case", args.out, "incremental_worker_splice_bench.json")
         return
     if args.shards or args.multi:
         a = synth.make_asks(args.asks, "mixed")
@@ -539,6 +558,69 @@ def splice_series(args, w, a, bits, npat, nmod, words):
     rows["splice_calls"] = summary
     return rows, checked, (f"{len(a.asks)} asks x {W} workers (synth mixed), first fit, fused lean; s held asks removed, "
                            f"then s rows inserted, per pass")
+
+
+def worker_splice_series(args, w, a, bits, npat, nmod, words, pool):
+    """S worker rows removed at scattered positions, then S rows inserted at random positions (pm_remove_workers /
+    pm_insert_workers), each followed by one incremental pass; the calls timed; the sibling's pm_set_worker_count +
+    upload + full pass (`route`) timed and its result checked equal."""
+    os.environ["PM_TUNE_INCR"] = str(1 << 31)   # read at pm_create: never fall back
+    inc = Engine(timing=True)
+    del os.environ["PM_TUNE_INCR"]
+    ref = Engine(timing=True)
+    for e in (inc, ref):
+        e.set_asks(a.asks, a.opts)
+        e.set_model_table(bits, npat, nmod, words)
+        e.set_workers(w.a, w.b)
+        e.match(LEAN)
+    wa, wb = w.a.copy(), w.b.copy()   # the current rows
+    rng = np.random.default_rng(2028)
+    rows = {"full": []}
+    calls, checked = [], set()
+    for rnd in range(args.rounds):
+        for n in S:
+            rows["full"].append(timed(inc, LEAN))
+            for case in ("remove", "insert"):
+                W = len(wa)
+                if case == "remove":
+                    idx = np.sort(rng.choice(W, n, replace=False)).astype(np.uint32)
+                    t = time.perf_counter()
+                    inc.remove_workers(idx)
+                    inc.sync()
+                    wa, wb = np.delete(wa, idx.astype(np.int64)), np.delete(wb, idx.astype(np.int64))
+                else:
+                    before = np.sort(rng.integers(0, W + 1, n)).astype(np.uint32)
+                    src = rng.integers(0, len(pool), n)
+                    na, nb = pool.a[src].copy(), pool.b[src].copy()
+                    t = time.perf_counter()
+                    inc.insert_workers(before, na, nb)
+                    inc.sync()
+                    b = before.astype(np.int64)
+                    wa, wb = np.insert(wa, b, na), np.insert(wb, b, nb)
+                calls.append({"case": case, "s": n, "n_workers": W, "ms_call": (time.perf_counter() - t) * 1e3})
+                key = f"{case}_{n}"
+                rows.setdefault(key, []).append(timed(inc, INCR))
+                t = time.perf_counter()
+                ref.set_workers(wa, wb)
+                r = timed(ref, LEAN)
+                r["ms_host"] = (time.perf_counter() - t) * 1e3
+                rows.setdefault(f"route_{key}", []).append(r)
+                q, got = ref.fetch(), inc.fetch()
+                if not all(np.array_equal(getattr(got, f), getattr(q, f)) for f in FIELDS):
+                    raise SystemExit(f"{key}: the incremental result differs from pm_set_worker_count + upload + the full pass")
+                checked.add(key)
+    for e in (inc, ref):
+        e.close()
+    for c in calls:
+        print(json.dumps(c))
+    summary = []
+    for case in ("remove", "insert"):
+        for n in S:
+            ms = [c["ms_call"] for c in calls if c["case"] == case and c["s"] == n]
+            summary.append({"case": case, "s": n, "ms_call_median": float(np.median(ms)), "runs": len(ms)})
+    rows["splice_calls"] = summary
+    return rows, checked, (f"{len(a.asks)} asks x {len(w)} workers (synth mixed), first fit, fused lean; s worker rows "
+                           f"removed, then s rows inserted, per pass")
 
 
 def report(rows, checked, workload, env, key_name, out_dir, file_name):
